@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the GraphCast 6 h step on B200 (contract: see DESIGN.md section 6).
+"""Benchmark of the GraphCast 6 h step on H100 (contract: see DESIGN.md section 6).
 
   python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
   python bench.py --impl reference --gpus N --steps K ...  # CPU baseline arm
@@ -14,7 +14,7 @@ Haiku-default random weights.  Prints ONE JSON line on rank 0.
              GPU, no data-path collective ("weak" scaling).
   e2e      : steps/s through the public API (GraphCast.__call__) with pinned HOST
              inputs: per step H2D of inputs+forcings and D2H of the predictions.
-  roofline : the dominant kernel family (the tcgen05 fused layer / chain kernels) --
+  roofline : the dominant kernel family (the wgmma fused layer / chain kernels) --
              algorithmic FLOPs of all its launches in a step / their summed CUDA-event time,
              measured in a SEPARATE profiling pass of the same loop (events around every launch,
              direct launches); `hbm` gives every kernel's achieved GB/s and fraction of the
@@ -30,6 +30,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -308,6 +309,8 @@ def run_b200(args):
     dist.barrier()
   elapsed_ms = ev0.elapsed_time(ev1)
   clocks = sampler.stop() if rank == 0 else None
+  # What the last timed step delivered, captured before any later pass overwrites it.
+  dumped = sample_outputs(planes_out, torch) if args.dump_outputs and rank == 0 else None
 
   # Profiling pass (separate from the headline): the same loop with a CUDA-event pair around
   # every launch (direct launches instead of graph replay) -> per-kernel durations.
@@ -360,17 +363,17 @@ def run_b200(args):
     peaks = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))
   except Exception:
     pass
-  peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-  peak_hbm = peaks.get("hbm_gbs", 6500.0)
+  peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
+  peak_hbm = peaks.get("hbm_gbs", 3350.0)
   peak_src = ("measured (MEASURED_PEAKS.json: bf16_tflops_sustained, hbm_gbs)" if peaks
-              else "fallback 1.4 PFLOP/s, 6.5 TB/s (B200_PROFILING.md)")
+              else "H100 SXM data sheet: 989 TFLOP/s dense BF16, 3.35 TB/s HBM3 (700 W card)")
   products = {"bf16x3": 3, "bf16": 1, "fp32_simt": 1}[args.precision]
   # MACs the kernels really issue (the split edge layers execute fewer than the reference
   # dataflow the algorithmic figure is defined on), times the products per MAC.
   executed_tflops = (tc[1] / prof_steps) * products / (tc_ms_per_step * 1e-3) / 1e12
   traffic, traffic_src = ncu_traffic(args.workload, args.precision)
   roofline = {
-      "kernel": "gcb::mlp_chain_tc_kernel + gcb::mlp_layer_tc_kernel (fused tcgen05 layers)",
+      "kernel": "gcb::mlp_chain_tc_kernel + gcb::mlp_layer_tc_kernel (fused wgmma layers)",
       "bound": "tensor",
       "achieved": achieved_tflops, "peak": peak_tf, "unit": "TFLOP/s",
       "frac": achieved_tflops / peak_tf, "traffic": traffic,
@@ -451,7 +454,7 @@ def run_b200(args):
                    "pregather": bool(args.pregather), "fuse": bool(args.fuse), "chain_lag": args.chain_lag,
                    "image_residual": bool(args.image_residual), "deep_chains": bool(args.deep_chains),
                    "parallelism": "1 forecast per GPU (ensemble members), no collective",
-                   "l2_policy": "working set per step (>20 GB) far exceeds the 126 MB L2; no flush needed",
+                   "l2_policy": "working set per step (>20 GB) far exceeds the 50 MB L2; no flush needed",
                    "setup_s": setup_s},
         "clocks": clocks,
         "e2e": {"value": e2e_value, "unit": "steps/s", "h2d_bytes_per_step": h2d,
@@ -461,9 +464,35 @@ def run_b200(args):
         "roofline": roofline,
         "cpu_baseline": cpu,
     }
+    if dumped is not None:
+      write_outputs(args.dump_outputs, dumped)
     print(json.dumps(line), flush=True)
   if world > 1:
     dist.destroy_process_group()
+
+
+DUMP_BUDGET_BYTES = 48 << 20
+DUMP_SEED = 0
+
+
+def sample_outputs(planes_out, torch):
+  """The predictions of the timed path ([n_out, num_grid] fp32 planes, the array a caller of the
+  step receives) as host arrays: whole when they fit DUMP_BUDGET_BYTES, else the planes at a
+  fixed, seeded, sorted sample of grid nodes (the same nodes for every channel and run)."""
+  n_out, n_grid = planes_out.shape
+  keep = min(n_grid, (DUMP_BUDGET_BYTES - (1 << 20)) // (4 * n_out))
+  if keep == n_grid:
+    return {"predictions": planes_out.cpu().numpy()}
+  idx = np.sort(np.random.default_rng(DUMP_SEED).choice(n_grid, size=keep, replace=False))
+  sel = planes_out.index_select(1, torch.as_tensor(idx, device=planes_out.device))
+  return {"predictions_sampled": sel.cpu().numpy(),
+          "predictions_sampled_grid_index": idx.astype(np.float64)}
+
+
+def write_outputs(out_dir, arrays):
+  os.makedirs(out_dir, exist_ok=True)
+  for name, a in arrays.items():
+    np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def run_partitioned(args):
@@ -664,7 +693,7 @@ def run_partitioned(args):
         "gpu_launches_note": "kernels launched through the C ABI per forecast step, summed over ranks "
                              "(rank 0 counted, x world); the NCCL all_to_all kernels come on top",
         "roofline": {
-            "kernel": "gcb::mlp_chain_tc_kernel + gcb::mlp_layer_tc_kernel (fused tcgen05 layers), rank 0",
+            "kernel": "gcb::mlp_chain_tc_kernel + gcb::mlp_layer_tc_kernel (fused wgmma layers), rank 0",
             "bound": "tensor", "unit": "TFLOP/s",
             "achieved": alg_flops / world / (max(tc_ms, 1e-9) * 1e-3) / 1e12, "peak": peak_tf,
             "frac": alg_flops / world / (max(tc_ms, 1e-9) * 1e-3) / 1e12 / peak_tf,
@@ -765,6 +794,9 @@ def main():
   ap.add_argument("--skip-cpu-baseline", action="store_true")
   ap.add_argument("--cluster", type=int, default=0, help="CTAs per cluster (0 = library default)")
   ap.add_argument("--dump-launches", default="", help="write per-launch (kind, ms, GFLOP, GB) of the last timed step to this file")
+  ap.add_argument("--dump-outputs", dest="dump_outputs", default="",
+                  help="write the predictions of the last timed step to DIR/<name>.npy (float32; a fixed "
+                       "seeded sample of grid nodes when the whole array exceeds 48 MiB)")
   ap.add_argument("--no-fuse", dest="fuse", action="store_false",
                   help="one launch per linear layer (hidden activations through HBM)")
   ap.add_argument("--chain-lag", dest="chain_lag", type=int, default=0)
@@ -775,6 +807,12 @@ def main():
   ap.add_argument("--no-pregather", dest="pregather", action="store_false",
                   help="evaluate the first edge-MLP layer over the concatenated K=1536 input")
   args = ap.parse_args()
+  # The static-graph cache goes to a temporary directory: the source tree may be read-only.
+  os.environ.setdefault("GRAPHCAST_B200_CACHE", os.path.join(tempfile.gettempdir(), "graphcast_b200_graph_cache"))
+  single = not (args.impl == "reference" or args.rollout > 0 or args.mode == "partitioned" or
+                (args.mode == "auto" and dist_env()[1] > 1))
+  if args.dump_outputs and not single:
+    ap.error("--dump-outputs applies to the single-GPU step (--impl b200, one process)")
   if args.impl == "reference":
     run_reference(args)
   elif args.rollout > 0:

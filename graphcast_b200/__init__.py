@@ -1,4 +1,4 @@
-"""b200cast: the GraphCast 6 h step and rollout on NVIDIA B200 (sm_100a).
+"""b200cast: the GraphCast 6 h step and rollout on NVIDIA H100 (sm_90a).
 
 The compute path is `libgraphcast_b200.so` (hand-written CUDA behind the C ABI of
 `include/graphcast_b200.h`); the modules of this package mirror the reference's Python surface for

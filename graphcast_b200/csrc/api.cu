@@ -56,11 +56,11 @@ float bf16_to_f32(uint16_t h) {
 int sm_count_cached() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -171,6 +171,10 @@ int launch_tc_variant(const gcb_layer_desc& d, cudaStream_t stream) {
     attr_set[dev] = true;
   }
   const int csize = g_cluster_size;
+  // A consumer warpgroup holds the accumulator of one 256-column unit only: LayerNorm over a
+  // 512-wide row needs the N-split schedule, where each CTA of the pair owns one half.
+  if (kLN && d.n == 512 && csize != 2)
+    return fail(GCB_ERR_INVALID, "LayerNorm with n = 512 needs the cluster size 2 (N-split) schedule");
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.blockDim = dim3(gcb::kThreads);
@@ -334,10 +338,8 @@ int launch_chain_variant(const gcb_chain_desc& d, const ChainShape& sh, cudaStre
     GCB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set[dev] = true;
     // The scratch ring is accessed with the L2 evict_last policy.  Experiment switch: with
-    // GCB_L2_PERSIST_MB > 0 those lines also get a persisting set-aside of that size (at most 79 MB
-    // on B200).  Measured at 0.25 degree: DRAM traffic per step 183 -> 147 GB with the full
-    // set-aside, but the step gets SLOWER (75.3 -> 80.2 ms; the gathers lose the L2 they lived in),
-    // so the default is no set-aside (profiles/r02_l2_persist_experiment.log).
+    // GCB_L2_PERSIST_MB > 0 those lines also get a persisting set-aside of that size (capped at the
+    // device's cudaDevAttrMaxPersistingL2CacheSize); the default is no set-aside.
     static bool l2_set[64] = {false};
     if (!l2_set[dev]) {
       l2_set[dev] = true;

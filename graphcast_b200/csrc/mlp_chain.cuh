@@ -1,4 +1,4 @@
-// Fused layer CHAINS on tcgen05 tensor cores (sm_100a): up to GCB_MAX_CHAIN fused layers
+// Fused layer CHAINS on Hopper tensor cores (sm_90a, wgmma): up to GCB_MAX_CHAIN fused layers
 // (see mlp_tc.cuh for one layer) over the same rows in ONE persistent kernel.
 //
 //   layer l:  y_l[r] = residual_l[r] + LN|swish( concat_s A_{l,s}(r) @ W_l + b_l + gathered addends )
@@ -11,26 +11,27 @@
 // ("keep") writes it, as an operand image, into a per-cluster SCRATCH ring in global memory:
 // (lag * max_distance + 1) slots of 264 KB per kept layer and cluster, 40 MB for a whole
 // two-layer MLP launch.  The ring is rewritten in place tile after tile by the same cluster and
-// read back within microseconds, so it lives in the 126 MB L2 and never has to be written to
-// HBM; the consumer streams it with the same TMA bulk copies as any other operand image.  This
+// read back within microseconds, and its lines are written with the L2 evict_last policy so
+// that they stay in the L2 rather than go to HBM; the consumer streams it with the same TMA bulk copies as any other operand image.  This
 // keeps the [rows, 512] hidden activation of every MLP (84 GB of HBM traffic per 0.25 degree
 // step when the two linears were separate launches) on chip.
 //
 // Schedule.  Work is a sequence of UNITS (tile, layer); per cluster, step s runs the units
 // (tile_{s - l*lag}, layer l) for l = 0..L-1 (or L-1..0: gcb_chain_desc.order), i.e. a tile advances one layer per `lag` steps, so
 // that between a layer's MMAs and the dependent layer's MMAs the tensor pipe has `lag` other
-// units to execute while the epilogue converts the accumulator and hands it over.  TMEM holds
-// two 128x256 fp32 accumulators (unit u uses buffer u & 1).
+// units to execute while the epilogue converts the accumulator and hands it over.  Each of the
+// two consumer warpgroups holds the 64 x 256 fp32 accumulator of its half of the tile in
+// registers and runs the MMAs and the epilogue of every unit in turn (mlp_tc.cuh).
 //
 // Hand-over protocol of a kept layer's scratch slot (both CTAs write half of the columns and
 // both read all of them):
-//   h_full[q][slot]  count 8: the 4 epilogue warps of BOTH CTAs arrive (release.cluster) after
+//   h_full[q][slot]  count 16: the 8 consumer warps of BOTH CTAs arrive (release.cluster) after
 //                    their st.global + fence.proxy.async; the TMA warp of each CTA waits
 //                    (acquire.cluster) before the first bulk copy out of the slot.
-//   h_free[q][slot]  count 2 x consumers: every consuming unit's MMA warp commits
-//                    (tcgen05.commit, multicast to both CTAs) after its last MMA, i.e. when all
-//                    bulk copies out of the slot have landed and been consumed in that CTA; the
-//                    epilogue warps wait for it before overwriting the slot.
+//   h_free[q][slot]  count 16 x consumers: every consumer warp of a consuming unit arrives in
+//                    both CTAs once its last MMA has retired, i.e. when all bulk copies out of
+//                    the slot have landed and been consumed in that CTA; the consumers wait for
+//                    it before overwriting the slot.
 #pragma once
 #include <type_traits>
 
@@ -41,19 +42,6 @@ namespace gcb {
 constexpr int kChainSlotsMax = 5;
 constexpr int kScratchTileBytes = (kMaxN / kKStep) * GCB_A_IMAGE_BLOCK;   // 32 x 8448 = 270336
 constexpr int kChainTailBytes = 3072;
-// Epilogue warpgroups.  The epilogue is the critical path of every unit and is bound by
-// instruction latency (one warp per scheduler: ncu source view, profiles/r02_ncu_full_chain_*): two
-// warpgroups (warps 4-7 and 8-11) take alternate 32-column chunks of the unit's accumulator, warp w
-// and w + 4 sharing a TMEM lane quarter.  Warps 12-15 gather the pre-activation addends (chunk c ->
-// staging buffer c & 1 -> epilogue group c & 1); fp32-table segments are produced by the otherwise
-// idle warps 2-3 of the issue warpgroup.
-#ifndef GCB_EPI_GROUPS
-#define GCB_EPI_GROUPS 2
-#endif
-constexpr int kEpiGroups = GCB_EPI_GROUPS;
-constexpr int kGatherGroups = 3 - kEpiGroups;                  // producer warpgroups left: 1 or 2
-constexpr int kATableWarps = 2;                                // warps 2 and 3
-static_assert(kEpiGroups == 1 || kEpiGroups == 2, "one or two epilogue warpgroups");
 
 // kBig: room for 8 instead of 4 [512]-float parameter vectors (biases, LayerNorm scale / offset):
 // chains of two MLPs; costs 8 KB of shared memory (one operand stage in some variants).
@@ -65,8 +53,7 @@ struct ChainConfig {
   static constexpr int kStageBytes = kAStageBytes + kBStageBytes;
   static constexpr int kParamBytes = kParamVecs * kMaxN * 4;
   static constexpr int kGRegionBytes = kPre ? kGBytes : 0;
-  static constexpr int kFixedBytes =
-      kParamBytes + kEpiGroups * kEpiStageBytes + kGRegionBytes + kEpiGroups * kLnxBytes + kChainTailBytes;
+  static constexpr int kFixedBytes = kParamBytes + kGRegionBytes + kLnxBytes + kChainTailBytes;
   static constexpr int kFit = (kSmemLimit - kFixedBytes) / kStageBytes;
 #ifdef GCB_FORCE_STAGES          // experiment: sensitivity of a launch to the ring depth
   static constexpr int kStages = GCB_FORCE_STAGES < kFit ? GCB_FORCE_STAGES : kFit;
@@ -111,24 +98,20 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* stage_base = smem;
   float* s_param = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes);
-  float* s_epi = s_param + Cfg::kParamBytes / 4;                    // [kEpiGroups][4][32][36]
-  float* s_g = s_epi + kEpiGroups * 4 * 32 * kEpiRowFloats;         // [2][128][36] (kPre only)
-  float2* s_lnx = reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(s_g) + Cfg::kGRegionBytes);  // [kEpiGroups][2][128]
-  uint8_t* tail = reinterpret_cast<uint8_t*>(s_lnx) + kEpiGroups * kLnxBytes;
+  float* s_g = s_param + Cfg::kParamBytes / 4;                      // [2][128][36] (kPre only)
+  float2* s_lnx = reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(s_g) + Cfg::kGRegionBytes);  // [2][128]
+  uint8_t* tail = reinterpret_cast<uint8_t*>(s_lnx) + kLnxBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);          // [12]
   uint64_t* empty_bar = full_bar + 12;                             // [12]
-  uint64_t* tmem_full_bar = empty_bar + 12;                        // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;                    // [2]
-  uint64_t* g_full_bar = tmem_empty_bar + 2;                       // [2]
+  uint64_t* g_full_bar = empty_bar + 12;                           // [2]
   uint64_t* g_empty_bar = g_full_bar + 2;                          // [2]
-  uint64_t* lnx_bar = g_empty_bar + 2;                             // [kEpiGroups][2]
+  uint64_t* lnx_bar = g_empty_bar + 2;                             // [2 warpgroups][2]
   uint64_t* h_full_bar = lnx_bar + 4;                              // [GCB_MAX_CHAIN][kChainSlotsMax]
   uint64_t* h_free_bar = h_full_bar + GCB_MAX_CHAIN * kChainSlotsMax;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(h_free_bar + GCB_MAX_CHAIN * kChainSlotsMax);
-  ChainLayer* s_layer = reinterpret_cast<ChainLayer*>(tmem_base_slot + 2);           // [4]
+  ChainLayer* s_layer = reinterpret_cast<ChainLayer*>(h_free_bar + GCB_MAX_CHAIN * kChainSlotsMax);  // [4]
   ChainSeg* s_seg = reinterpret_cast<ChainSeg*>(s_layer + GCB_MAX_CHAIN);            // [4][3]
   PreAddInfo* s_pre = reinterpret_cast<PreAddInfo*>(s_seg + GCB_MAX_CHAIN * 3);      // [4][2]
-  static_assert((2 * 12 + 12 + 2 * GCB_MAX_CHAIN * kChainSlotsMax) * 8 + 8 +
+  static_assert((2 * 12 + 8 + 2 * GCB_MAX_CHAIN * kChainSlotsMax) * 8 +
                     GCB_MAX_CHAIN * (sizeof(ChainLayer) + 3 * sizeof(ChainSeg) + 2 * sizeof(PreAddInfo))
                     <= kChainTailBytes, "tail region too small");
 
@@ -230,47 +213,29 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
       }
     }
     for (int s = 0; s < Cfg::kStages; ++s) {
-      ptx::mbar_init(&full_bar[s], any_table ? 1 + kATableWarps : 1);   // TMA lane (+ the A-table warps)
-      ptx::mbar_init(&empty_bar[s], 2);                   // tcgen05.commit of both CTAs
+      ptx::mbar_init(&full_bar[s], any_table ? 1 + kProducerWarps : 1);   // TMA lane (+ the producer warps)
+      ptx::mbar_init(&empty_bar[s], 2 * kConsumerWarps);                   // every consumer warp of both CTAs
     }
     for (int b = 0; b < 2; ++b) {
-      ptx::mbar_init(&tmem_full_bar[b], 1);
-      ptx::mbar_init(&tmem_empty_bar[b], 4 * kEpiGroups);   // every epilogue warp
-      ptx::mbar_init(&g_full_bar[b], 4);        // the 4 warps of the gather group that filled it
-      ptx::mbar_init(&g_empty_bar[b], 4);       // the 4 warps of the epilogue group that read it
-      for (int eg = 0; eg < kEpiGroups; ++eg) ptx::mbar_init(&lnx_bar[eg * 2 + b], 1);
+      ptx::mbar_init(&g_full_bar[b], kProducerWarps);
+      ptx::mbar_init(&g_empty_bar[b], kConsumerWarps);
+      ptx::mbar_init(&lnx_bar[b], 1);
+      ptx::mbar_init(&lnx_bar[2 + b], 1);
     }
     for (int l = 0; l < L; ++l) {
       if (q_of_layer[l] < 0) continue;
       for (int sl = 0; sl < nslots; ++sl) {
-        ptx::mbar_init(&h_full_bar[q_of_layer[l] * kChainSlotsMax + sl], 8 * kEpiGroups);
+        ptx::mbar_init(&h_full_bar[q_of_layer[l] * kChainSlotsMax + sl], 2 * kConsumerWarps);
         ptx::mbar_init(&h_free_bar[q_of_layer[l] * kChainSlotsMax + sl],
-                       2 * (consumers[l] > 0 ? consumers[l] : 1));
+                       2 * kConsumerWarps * (consumers[l] > 0 ? consumers[l] : 1));
       }
     }
     ptx::fence_mbar_init();
   }
-  if (warp == 2) {
-    ptx::tmem_alloc(tmem_base_slot, kTmemCols);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before_sync();
   __syncthreads();
   ptx::cluster_sync_all();
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_base_slot;
 
   // ---- roles ------------------------------------------------------------------
-  // Register re-allocation per warpgroup (setmaxnreg): the epilogue is the critical path of
-  // every unit and, at the 128 registers a 512-thread CTA starts with, it spills its residual /
-  // staging values to local memory inside the chunk loops; the issue warps need a fraction of
-  // that.  One epilogue group: 56 x 4 + 216 x 4 + 112 x 8 warps = 1984; two: 72 x 4 + 176 x 8 +
-  // 88 x 4 = 2048 of the 2048 register slices of the SM.
-  constexpr int kRegsCtl = kEpiGroups == 2 ? 72 : 56;
-  constexpr int kRegsEpi = kEpiGroups == 2 ? 176 : 216;
-  constexpr int kRegsProd = kEpiGroups == 2 ? 88 : 112;
-  if (warp < 4) {
-    ptx::setmaxnreg_dec<kRegsCtl>();
   if (warp == 0) {
     // ===== TMA warp (converged; every lane polls, one elected lane issues) =====
     const uint32_t b_bytes = Cfg::kBStageBytes;
@@ -334,70 +299,207 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         ++tu;
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA warp =====
-    const uint32_t idesc = ptx::make_idesc_bf16(kTileM, kUnitN);
-    uint32_t stage = 0, phase = 0, u = 0;
+  } else if (warp >= 4) {
+    // ===== consumers: MMA + epilogue =====
+    const int eg = (warp - 4) >> 2;                // warpgroup: tile rows [64 eg, 64 eg + 64)
+    const int q = lane & 3;
+    const int lr0 = eg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile rows lr0, lr0 + 8
+    const bool lead = lane == 0 && (warp & 3) == 0;
+    const int col_base = static_cast<int>(crank) * kUnitN;   // my 256 columns of every layer
+    uint32_t stage = 0, phase = 0, g_count = 0, ln_count = 0, u = 0;
+    const uint64_t keep_policy = ptx::l2_policy_evict_last();
+    float acc[128];
+
     for (int st = 0; st < nsteps; ++st) {
       for (int li = 0; li < L; ++li) {
         const int l = desc ? L - 1 - li : li;
         const int ti = st - l * lag;
         if (ti < 0 || ti >= T) continue;
-        const uint32_t buf = u & 1;
-        ptx::mbar_wait(&tmem_empty_bar[buf], ((u >> 1) & 1) ^ 1);
-        ptx::tc_fence_after_sync();
-        if (lane == 0) trace(u, 0);
-        const uint32_t dcol = tmem_base + buf * kUnitN;
-        const int ksteps = s_layer[l].ksteps;
-        const bool tr = tracing(u);
-        long long starved = 0;
-        for (int ks = 0; ks < ksteps; ++ks) {
-          const long long w0 = tr ? clock64() : 0;
-          ptx::mbar_wait(&full_bar[stage], phase);
-          if (tr) starved += clock64() - w0;
-          ptx::tc_fence_after_sync();
-          if (ks == 0 && lane == 0) trace(u, 1);
-          const uint32_t sa = ptx::smem_addr(stage_base + stage * Cfg::kStageBytes);
-          const uint32_t sb = sa + Cfg::kAStageBytes;
-          const uint64_t a_hi = ptx::make_smem_desc(sa, kALbo, 128);
-          const uint64_t b_hi = ptx::make_smem_desc(sb, kBLbo, 128);
-          if (ptx::elect_one()) {
-            ptx::mma_bf16_ss(dcol, a_hi, b_hi, idesc, ks > 0 ? 1u : 0u);
-            if (kSplit) {
-              const uint64_t a_lo = a_hi + (kAPartBytes >> 4);
-              const uint64_t b_lo = b_hi + (kBPartBytes >> 4);
-              ptx::mma_bf16_ss(dcol, a_hi, b_lo, idesc, 1u);
-              ptx::mma_bf16_ss(dcol, a_lo, b_hi, idesc, 1u);
+        const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
+        const ChainLayer& cl = s_layer[l];
+        const int kind = cl.kind;
+        float* const out_ptr = cl.out;
+        float* const outy_ptr = cl.out_y;
+        const float* const res_ptr = kind == kKindLNRes ? cl.residual : nullptr;
+        const long long ld_out = cl.ld_out, ld_outy = cl.ld_outy, ld_res = cl.ld_res;
+        const float* const s_bias = cl.bias_off >= 0 ? s_param + cl.bias_off : nullptr;
+        const float* const s_scale = cl.scale_off >= 0 ? s_param + cl.scale_off : nullptr;
+        const float* const s_offset = cl.offset_off >= 0 ? s_param + cl.offset_off : nullptr;
+        uint8_t* const img0 = cl.out_img != nullptr
+                                  ? cl.out_img + static_cast<size_t>(tile) * (kMaxN / kKStep) * GCB_A_IMAGE_BLOCK
+                                  : nullptr;
+        const uint8_t* res_img = cl.res_img != nullptr
+                                     ? cl.res_img + static_cast<size_t>(tile) * (kMaxN / kKStep) * GCB_A_IMAGE_BLOCK
+                                     : nullptr;
+        // Residual = the kept result of an earlier layer: the slot this CTA's consumers wrote for
+        // this tile (same threads, same rows and columns: program order makes it visible, and the
+        // slot cannot be rewritten before these warps reach tile ti + nslots themselves).
+        if (cl.res_q >= 0) res_img = scratch_slot(cl.res_q, ti);
+        if (kind != kKindLNImg) res_img = nullptr;
+        if (eg == 0 && ti + 1 < T && (cl.residual != nullptr || cl.res_img != nullptr)) {
+          // Pull the residual of this layer's NEXT tile into L2 now (a whole step ahead).
+          const uint32_t ntile = tile + ncl;
+          const int pr = (warp & 3) * 32 + lane;      // 128 threads: one row each
+          if (cl.residual != nullptr) {
+            const long long nrow = static_cast<long long>(ntile) * kTileM + pr;
+            if (nrow < rows_total) ptx::bulk_prefetch_l2(cl.residual + nrow * cl.ld_res + col_base, kUnitN * 4);
+          } else if (pr < kUnitN / kKStep) {
+            ptx::bulk_prefetch_l2(cl.res_img + (static_cast<size_t>(ntile) * (kMaxN / kKStep) +
+                                                (col_base >> 4) + pr) * GCB_A_IMAGE_BLOCK,
+                                  GCB_A_IMAGE_BLOCK);
+          }
+        }
+        const int keep_q = cl.keep_q;
+        uint8_t* img1 = nullptr;
+        if (keep_q >= 0) {
+          // previous readers of this slot (tile ti - nslots) are done in both CTAs
+          ptx::mbar_wait(&h_free_bar[keep_q * kChainSlotsMax + (ti % nslots)],
+                         (static_cast<uint32_t>(ti / nslots) & 1u) ^ 1u);
+          img1 = scratch_slot(keep_q, ti);
+        }
+        if (lead && eg == 0) trace(u, 0);
+        mma_unit<kSplit, Cfg::kStages, Cfg::kStageBytes, Cfg::kAStageBytes>(
+            acc, stage_base, full_bar, empty_bar, stage, phase, cl.ksteps, eg * 64 * 16, cmask);
+        if (lane == 0) {
+          // Every scratch slot this unit read is reusable (in both CTAs) once these MMAs retired.
+          for (int s = 0; s < cl.nseg; ++s) {
+            const int sq = s_seg[l * 3 + s].src_q;
+            if (sq >= 0) {
+              const uint32_t a = ptx::smem_addr(&h_free_bar[sq * kChainSlotsMax + (ti % nslots)]);
+              ptx::mbar_arrive_remote(ptx::mapa(a, 0));
+              ptx::mbar_arrive_remote(ptx::mapa(a, 1));
             }
-            ptx::mma_commit_multicast(&empty_bar[stage], cmask);
           }
+        }
+        if (lead && eg == 0) trace(u, 3);
+        const bool is_ln = kind >= kKindLN;
+        float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
+        if (is_ln) {
+          // Each CTA computes (mean, M2) of its 256 columns of a row, hands them to the partner
+          // through distributed shared memory, and both combine them (Chan's parallel update).
+          float shift[2], s1[2], s2[2];
+          row_shifted_sums(acc, s_bias != nullptr ? s_bias + col_base : nullptr, kUnitN, shift, s1, s2);
+          const uint32_t lb = ln_count & 1, par = (ln_count >> 1) & 1;
+          uint64_t* bar = &lnx_bar[eg * 2 + lb];
+          float mh[2], m2h[2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            mh[h] = shift[h] + s1[h] * (1.0f / kUnitN);
+            m2h[h] = fmaxf(s2[h] - s1[h] * s1[h] * (1.0f / kUnitN), 0.f);
+            if (q == 0)
+              ptx::st_async_f32x2(ptx::mapa(ptx::smem_addr(&s_lnx[lb * kTileM + lr0 + 8 * h]), peer),
+                                  mh[h], m2h[h], ptx::mapa(ptx::smem_addr(bar), peer));
+          }
+          if (lead) ptx::mbar_arrive_expect_tx(bar, 64 * 8);
+          ptx::mbar_wait(bar, par);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float2 other = s_lnx[lb * kTileM + lr0 + 8 * h];
+            const float delta = other.x - mh[h];
+            mean[h] = 0.5f * (mh[h] + other.x);
+            const float var = (m2h[h] + other.y + delta * delta * (0.5f * kUnitN)) * (1.0f / (2 * kUnitN));
+            rstd[h] = rsqrtf(var + 1e-5f);
+          }
+          ++ln_count;
+          if (lead && eg == 0) trace(u, 4);
+        }
+        // Epilogue, 32 columns (j0 .. j0 + 3) at a time; unrolled so that the accumulator is
+        // only ever indexed with constants (it must stay in registers).
+        const bool want_pre = kPre && !is_ln && cl.n_pre > 0;
+        const long long grow0 = static_cast<long long>(tile) * kTileM + lr0;
+#pragma unroll
+        for (int c0 = 0; c0 < kUnitN; c0 += 32) {
+          const int j0 = c0 >> 3;
+          if (want_pre) {
+            const uint32_t gb = g_count & 1;
+            ptx::mbar_wait(&g_full_bar[gb], (g_count >> 1) & 1);
+            add_staged_chunk(acc, j0, s_g + gb * kGBufFloats, lr0);
+            __syncwarp();
+            if (lane == 0) ptx::mbar_arrive(&g_empty_bar[gb]);
+            ++g_count;
+          }
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int gc = col_base + c0 + 8 * jj + 2 * q;
+            const float2 b = s_bias != nullptr ? *reinterpret_cast<const float2*>(s_bias + gc) : make_float2(0.f, 0.f);
+            float2 sc = make_float2(1.f, 1.f), of = make_float2(0.f, 0.f);
+            if (is_ln) {
+              sc = *reinterpret_cast<const float2*>(s_scale + gc);
+              of = *reinterpret_cast<const float2*>(s_offset + gc);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float* v = &acc[4 * (j0 + jj) + 2 * h];
+              const int r = lr0 + 8 * h;
+              const long long grow = grow0 + 8 * h;
+              const bool row_ok = grow < rows_total;
+              float2 y = make_float2(v[0] + b.x, v[1] + b.y);
+              if (kind == kKindSwish) { y.x = swish_f(y.x); y.y = swish_f(y.y); }
+              if (is_ln) {
+                y.x = (y.x - mean[h]) * rstd[h] * sc.x + of.x;
+                y.y = (y.y - mean[h]) * rstd[h] * sc.y + of.y;
+              }
+              // fp32 residual (rows past the end: none)
+              float2 rs = make_float2(0.f, 0.f);
+              if (res_ptr != nullptr && row_ok) rs = *reinterpret_cast<const float2*>(res_ptr + grow * ld_res + gc);
+              if (row_ok) {
+                if (outy_ptr != nullptr) *reinterpret_cast<float2*>(outy_ptr + grow * ld_outy + gc) = y;
+                if (out_ptr != nullptr)
+                  *reinterpret_cast<float2*>(out_ptr + grow * ld_out + gc) = make_float2(y.x + rs.x, y.y + rs.y);
+              }
+              if (img0 != nullptr || img1 != nullptr) {
+                // Operand image of the result (+ residual): the four threads of a row complete
+                // one 16-byte piece, eight rows a 128-byte line.
+                float2 x = make_float2(y.x + rs.x, y.y + rs.y);
+                const size_t o = image_offset(gc, r);
+                if (res_img != nullptr) {
+                  // Residual held as an operand image (x = hi + lo, two bf16); a packed word
+                  // holds the even column in its low and the odd column in its high half.
+                  const uint32_t hw = *reinterpret_cast<const uint32_t*>(res_img + o);
+                  const uint32_t lw = *reinterpret_cast<const uint32_t*>(res_img + o + kAPartBytes);
+                  x.x += __uint_as_float(hw << 16) + __uint_as_float(lw << 16);
+                  x.y += __uint_as_float(hw & 0xffff0000u) + __uint_as_float(lw & 0xffff0000u);
+                }
+                uint32_t hi, lo;
+                ptx::split_bf16x2(x.x, x.y, hi, lo);
+                if (img0 != nullptr) {
+                  *reinterpret_cast<uint32_t*>(img0 + o) = hi;
+                  *reinterpret_cast<uint32_t*>(img0 + o + kAPartBytes) = lo;
+                }
+                if (img1 != nullptr) {       // scratch slot: keep these lines in the L2
+                  ptx::st_global_b32_hint(img1 + o, hi, keep_policy);
+                  ptx::st_global_b32_hint(img1 + o + kAPartBytes, lo, keep_policy);
+                }
+              }
+            }
+          }
+        }
+        if (lead && eg == 0) trace(u, 5);
+        if (keep_q >= 0) {
+          // Hand the slot to the TMA warps of both CTAs: my generic-proxy global stores must be
+          // visible to their async-proxy bulk copies.
+          ptx::fence_proxy_async_global();
           __syncwarp();
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        if (ptx::elect_one()) {
-          ptx::mma_commit(&tmem_full_bar[buf]);
-          // Every scratch slot this unit read is reusable (in both CTAs) once these MMAs retire.
-          const int nseg = s_layer[l].nseg;
-          for (int s = 0; s < nseg; ++s) {
-            const int q = s_seg[l * 3 + s].src_q;
-            if (q >= 0) ptx::mma_commit_multicast(&h_free_bar[q * kChainSlotsMax + (ti % nslots)], cmask);
+          if (lane == 0) {
+            uint64_t* hb = &h_full_bar[keep_q * kChainSlotsMax + (ti % nslots)];
+            ptx::mbar_arrive_release_cluster(hb);
+            ptx::mbar_arrive_remote(ptx::mapa(ptx::smem_addr(hb), peer));
           }
         }
-        __syncwarp();
-        if (lane == 0) { trace(u, 2); trace_val(u, 6, starved); }
         ++u;
       }
     }
-  } else if (any_table) {
-    // ===== A-table warps (2 and 3): segments given as fp32 tables =====
-    // Gather through the segment's index, optional fan-in sum, split to bf16 hi / lo, store in
-    // the UMMA K-major core-matrix layout.  They arrive on EVERY K-step's full barrier (for image
-    // / scratch K-steps without writing anything), so the barrier count is uniform.
-    const int t64 = threadIdx.x - 64;
+  } else if (warp >= 4 - kProducerWarps) {
+    // ===== producers (warps 2-3): fp32-table segments, then gathered addends, unit by unit =====
+    // A table segment is gathered through its index (optional fan-in sum), split to bf16 hi / lo
+    // and stored in the K-major core-matrix layout.  The producers arrive on EVERY K-step's full
+    // barrier when some layer has a table segment (for image / scratch K-steps without writing
+    // anything), so the barrier count is uniform.
+    const int t64 = threadIdx.x - 32 * (4 - kProducerWarps);
     const int sub = t64 & 3;                        // which float4 of the 16-wide K-step
     const int rg = t64 >> 2;                        // 0..15; rows rg + 16*i
     const uint32_t sts_off = (sub >> 1) * kALbo + (sub & 1) * 8;
-    uint32_t stage = 0, phase = 0;
+    uint32_t stage = 0, phase = 0, gc = 0;
     for (int st = 0; st < nsteps; ++st) {
       for (int li = 0; li < L; ++li) {
         const int l = desc ? L - 1 - li : li;
@@ -405,7 +507,7 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         if (ti < 0 || ti >= T) continue;
         const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
         const int nseg = s_layer[l].nseg;
-        for (int s = 0; s < nseg; ++s) {
+        for (int s = 0; any_table && s < nseg; ++s) {
           const ChainSeg sg = s_seg[l * 3 + s];
           const bool is_tab = sg.src_q < 0 && sg.img == nullptr;
           int src[8];
@@ -424,16 +526,16 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
               const bool kvalid = koff < sg.k_valid;
 #pragma unroll
               for (int i = 0; i < 8; ++i) {
-                float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+                float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
                 if (kvalid && src[i] >= 0) {
                   const float* p = sg.table + static_cast<long long>(src[i]) * sg.fan * sg.ld + koff;
-                  acc = __ldg(reinterpret_cast<const float4*>(p));
+                  a = __ldg(reinterpret_cast<const float4*>(p));
                   for (int j = 1; j < sg.fan; ++j) {
                     const float4 t = __ldg(reinterpret_cast<const float4*>(p + static_cast<long long>(j) * sg.ld));
-                    acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
+                    a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
                   }
                 }
-                cur[i] = acc;
+                cur[i] = a;
               }
             }
             ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -454,469 +556,17 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
             if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
           }
         }
-      }
-    }
-  }
-  } else if (warp < 4 + 4 * kEpiGroups) {
-    // ===== epilogue =====
-    ptx::setmaxnreg_inc<kRegsEpi>();
-    const int eg = (warp - 4) >> 2;               // epilogue group: chunks with (chunk & 1) == eg
-    const int ew = warp & 3;                      // TMEM lane quarter
-    const uint32_t lane_base = static_cast<uint32_t>(ew * 32) << 16;
-    float* my_epi = s_epi + (eg * 4 + ew) * 32 * kEpiRowFloats;
-    float2* my_lnx = s_lnx + eg * 2 * kTileM;     // [2][128] of this group
-    uint64_t* my_lnx_bar = lnx_bar + eg * 2;
-    const int cg = lane & 7;
-    const int rsub = lane >> 3;
-    const int col_base = static_cast<int>(crank) * kUnitN;   // my 256 columns of every layer
-    uint32_t g_count = 0, ln_count = 0, u = 0;
-    const uint64_t keep_policy = ptx::l2_policy_evict_last();
-
-    // Per-unit context, passed BY VALUE: as mutable locals captured by reference these lived in
-    // local memory and every use in the chunk loops was an LDL on the critical path.
-    struct EpiCtx {
-      float* out_ptr; float* outy_ptr; const float* res_ptr;
-      long long ld_out, ld_outy, ld_res;
-      uint8_t* img0;                  // external operand image of this TILE (block base), or null
-      uint8_t* img1;                  // scratch slot of this tile, or null
-      const uint8_t* res_img;         // residual as an operand image: block base of this TILE, or null
-      const float* s_bias; const float* s_scale; const float* s_offset;
-      int n_pre;
-      int trace_u;                    // unit index when this unit is traced, else -1
-    };
-
-    auto finish_unit = [&](auto kind_tag, const EpiCtx cx, uint32_t g_count_in, uint32_t taddr,
-                           long long row0, float mean, float rstd) -> uint32_t {
-      constexpr int kind = decltype(kind_tag)::value;
-      uint32_t g_count = g_count_in;
-      // Compile-time leanness: a swish layer only feeds later layers (operand image / scratch, no
-      // fp32 output, no residual) and a plain layer has no residual (validate_chain enforces both),
-      // so those paths - and the registers they keep alive - exist in the LayerNorm variant only.
-      constexpr bool is_ln = kind >= kKindLN;
-      float* const out_ptr = kind == kKindSwish ? nullptr : cx.out_ptr;
-      float* const outy_ptr = kind == kKindSwish ? nullptr : cx.outy_ptr;
-      const float* const res_ptr = kind == kKindLNRes ? cx.res_ptr : nullptr;
-      const uint8_t* const res_img = kind == kKindLNImg ? cx.res_img : nullptr;
-      const long long ld_out = cx.ld_out, ld_outy = cx.ld_outy, ld_res = cx.ld_res;
-      uint8_t* const img0 = cx.img0; uint8_t* const img1 = cx.img1;
-      const float* const s_bias = cx.s_bias; const float* const s_scale = cx.s_scale;
-      const float* const s_offset = cx.s_offset;
-      const int n_pre = cx.n_pre;
-      const bool rows_full = row0 + 32 <= rows_total;
-      const bool want_img = (img0 != nullptr) || (img1 != nullptr);
-      // Residual of the CURRENT chunk, requested at the end of the previous one.
-      //   rr     fp32 master, coalesced layout: rows rsub + 4i, 16 bytes at column cg*4
-      //   rh/rl  operand image (hi | lo bf16), thread = row layout: the four 16-byte pieces
-      //          (K-step ks2, chunk c) of this thread's row
-      float4 rr[8];
-      uint4 rh[4], rl[4];
-      const size_t row_off = static_cast<size_t>(ew * 32 + lane) * 16;
-      auto load_res = [&](int c0) {
-        if (kind == kKindLNRes && rows_full) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            rr[i] = *reinterpret_cast<const float4*>(res_ptr + (row0 + rsub + 4 * i) * ld_res + col_base + c0 + cg * 4);
-        }
-        if (kind == kKindLNImg) {
-          const uint8_t* b = res_img + static_cast<size_t>((col_base + c0) >> 4) * GCB_A_IMAGE_BLOCK + row_off;
-#pragma unroll
-          for (int ks2 = 0; ks2 < 2; ++ks2) {
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              rh[ks2 * 2 + c] = *reinterpret_cast<const uint4*>(b + ks2 * GCB_A_IMAGE_BLOCK + c * kALbo);
-              rl[ks2 * 2 + c] = *reinterpret_cast<const uint4*>(b + ks2 * GCB_A_IMAGE_BLOCK + c * kALbo + kAPartBytes);
-            }
-          }
-        }
-      };
-      constexpr int kChunkStep = 32 * kEpiGroups;          // my chunks: eg, eg + kEpiGroups, ...
-      load_res(32 * eg);
-      const bool trp = cx.trace_u >= 0 && ew == 0 && lane == 0 && eg == 0;
-      long long t_ld = 0, t_math = 0, t_f32 = 0, t_img = 0;
-      for (int c0 = 32 * eg; c0 < kUnitN; c0 += kChunkStep) {
-        const int gc0 = col_base + c0;
-        const int col = gc0 + cg * 4;
-        float v[32];
-        long long tp = trp ? clock64() : 0;
-        ptx::tmem_ld32(taddr + c0, v);
-        if (trp) { const long long t = clock64(); t_ld += t - tp; tp = t; }
-        if (s_bias != nullptr) {
-          float b[32];
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(&b[4 * q]) = *reinterpret_cast<const float4*>(s_bias + gc0 + 4 * q);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += b[j];
-        }
-        if (kPre && !is_ln && n_pre > 0) {
-          // staging buffer = chunk parity; with two epilogue groups that is my group index and
-          // every fill of that buffer is mine
-          const uint32_t gb = kEpiGroups == 2 ? static_cast<uint32_t>(eg) : (g_count & 1);
-          ptx::mbar_wait(&g_full_bar[gb], (kEpiGroups == 2 ? g_count : (g_count >> 1)) & 1);
-          const float* gp = s_g + gb * kGBufFloats + (ew * 32 + lane) * kEpiRowFloats;
-          float g[32];
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(&g[4 * q]) = *reinterpret_cast<const float4*>(gp + 4 * q);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += g[j];
-          __syncwarp();
-          if (lane == 0) ptx::mbar_arrive(&g_empty_bar[gb]);
-          ++g_count;
-        }
-        if (kind == kKindSwish) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = swish_f(v[j]);
-        }
-        if (is_ln) {
-          float g[32];
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(&g[4 * q]) = *reinterpret_cast<const float4*>(s_scale + gc0 + 4 * q);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = (v[j] - mean) * rstd * g[j];
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(&g[4 * q]) = *reinterpret_cast<const float4*>(s_offset + gc0 + 4 * q);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += g[j];
-        }
-        if (trp) { const long long t = clock64(); t_math += t - tp; tp = t; }
-        if (out_ptr != nullptr || outy_ptr != nullptr) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(my_epi + lane * kEpiRowFloats + q * 4) =
-                make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-          __syncwarp();
-          if (rows_full) {
-            float4 y[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-              y[i] = *reinterpret_cast<const float4*>(my_epi + (rsub + 4 * i) * kEpiRowFloats + cg * 4);
-            if (outy_ptr != nullptr) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                *reinterpret_cast<float4*>(outy_ptr + (row0 + rsub + 4 * i) * ld_outy + col) = y[i];
-            }
-            if (res_ptr != nullptr) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                y[i].x += rr[i].x; y[i].y += rr[i].y; y[i].z += rr[i].z; y[i].w += rr[i].w;
-              }
-            }
-            if (out_ptr != nullptr) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                *reinterpret_cast<float4*>(out_ptr + (row0 + rsub + 4 * i) * ld_out + col) = y[i];
-            }
-            if (want_img && res_ptr != nullptr) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                *reinterpret_cast<float4*>(my_epi + (rsub + 4 * i) * kEpiRowFloats + cg * 4) = y[i];
-            }
-          } else {
-            for (int i = 0; i < 8; ++i) {
-              const int r = rsub + 4 * i;
-              const long long grow = row0 + r;
-              if (grow < rows_total) {
-                for (int e = 0; e < 4; ++e) {
-                  const float yv = my_epi[r * kEpiRowFloats + cg * 4 + e];
-                  const float ov = yv + (res_ptr ? res_ptr[grow * ld_res + col + e] : 0.f);
-                  if (outy_ptr != nullptr) outy_ptr[grow * ld_outy + col + e] = yv;
-                  if (out_ptr != nullptr) out_ptr[grow * ld_out + col + e] = ov;
-                  if (want_img) my_epi[r * kEpiRowFloats + cg * 4 + e] = ov;
-                }
-              }
-            }
-          }
-          __syncwarp();
-          if (want_img && res_ptr != nullptr) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              *reinterpret_cast<float4*>(&v[4 * q]) =
-                  *reinterpret_cast<const float4*>(my_epi + lane * kEpiRowFloats + q * 4);
-            __syncwarp();
-          }
-        } else if (want_img && res_ptr != nullptr) {
-          // Image-only result with an fp32 residual: transpose the coalesced residual rows to the
-          // thread = row layout through the tile.
-          if (rows_full) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-              *reinterpret_cast<float4*>(my_epi + (rsub + 4 * i) * kEpiRowFloats + cg * 4) = rr[i];
-            __syncwarp();
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const float4 t = *reinterpret_cast<const float4*>(my_epi + lane * kEpiRowFloats + q * 4);
-              v[4 * q] += t.x; v[4 * q + 1] += t.y; v[4 * q + 2] += t.z; v[4 * q + 3] += t.w;
-            }
-            __syncwarp();
-          } else {
-            const long long grow = row0 + lane;
-            if (grow < rows_total) {
-              const float* rp = res_ptr + grow * ld_res + gc0;
-#pragma unroll
-              for (int q = 0; q < 8; ++q) {
-                const float4 t = *reinterpret_cast<const float4*>(rp + 4 * q);
-                v[4 * q] += t.x; v[4 * q + 1] += t.y; v[4 * q + 2] += t.z; v[4 * q + 3] += t.w;
-              }
-            }
-          }
-        }
-        if (trp) { const long long t = clock64(); t_f32 += t - tp; tp = t; }
-        if (kind == kKindLNImg) {
-          // Residual held as an operand image (x = hi + lo, two bf16): already in this thread's
-          // row layout.  A packed word holds element 2k in its low and 2k+1 in its high half.
-#pragma unroll
-          for (int pc = 0; pc < 4; ++pc) {
-            const uint32_t hw[4] = {rh[pc].x, rh[pc].y, rh[pc].z, rh[pc].w};
-            const uint32_t lw[4] = {rl[pc].x, rl[pc].y, rl[pc].z, rl[pc].w};
-#pragma unroll
-            for (int k2 = 0; k2 < 4; ++k2) {
-              v[pc * 8 + 2 * k2] += __uint_as_float(hw[k2] << 16) + __uint_as_float(lw[k2] << 16);
-              v[pc * 8 + 2 * k2 + 1] += __uint_as_float(hw[k2] & 0xffff0000u) + __uint_as_float(lw[k2] & 0xffff0000u);
-            }
-          }
-        }
-        if (want_img) {
-          // thread = row: the 16-byte pieces of 32 consecutive rows are contiguous -> 512-byte
-          // coalesced warp stores, to the external image and / or the scratch slot.
-          const size_t boff = static_cast<size_t>(gc0 >> 4) * GCB_A_IMAGE_BLOCK + row_off;
-#pragma unroll
-          for (int ks2 = 0; ks2 < 2; ++ks2) {
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              const float* x = &v[ks2 * 16 + c * 8];
-              uint2 h0, l0, h1, l1;
-              ptx::split_bf16x4(make_float4(x[0], x[1], x[2], x[3]), h0, l0);
-              ptx::split_bf16x4(make_float4(x[4], x[5], x[6], x[7]), h1, l1);
-              const size_t o = boff + ks2 * GCB_A_IMAGE_BLOCK + c * kALbo;
-              if (img0 != nullptr) {
-                *reinterpret_cast<uint4*>(img0 + o) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-                *reinterpret_cast<uint4*>(img0 + o + kAPartBytes) = make_uint4(l0.x, l0.y, l1.x, l1.y);
-              }
-              if (img1 != nullptr) {       // scratch slot: keep these lines in the L2
-                ptx::st_global_v4_hint(img1 + o, make_uint4(h0.x, h0.y, h1.x, h1.y), keep_policy);
-                ptx::st_global_v4_hint(img1 + o + kAPartBytes, make_uint4(l0.x, l0.y, l1.x, l1.y), keep_policy);
-              }
-            }
-          }
-        }
-        // Next chunk's residual: requested once this chunk's values are dead (no extra registers);
-        // the line is already in L2 (prefetched a step ahead), so the TMEM load and LayerNorm
-        // math of the next chunk cover its latency.
-        if (c0 + kChunkStep < kUnitN) load_res(c0 + kChunkStep);
-        if (trp) { const long long t = clock64(); t_img += t - tp; tp = t; }
-      }
-      if (trp) {
-        trace_val(cx.trace_u, 12, t_ld); trace_val(cx.trace_u, 13, t_math);
-        trace_val(cx.trace_u, 14, t_f32); trace_val(cx.trace_u, 15, t_img);
-      }
-      return g_count;
-    };
-
-    auto unit_shifted_sums = [&](const float* s_bias, uint32_t taddr, float& shift, float& s1, float& s2) {
-      float p1 = 0.f, p2 = 0.f, q1 = 0.f, q2 = 0.f;
-      for (int c0 = 0; c0 < kUnitN; c0 += 32) {
-        float v[32];
-        ptx::tmem_ld32(taddr + c0, v);
-        float b[32];
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          *reinterpret_cast<float4*>(&b[4 * q]) =
-              s_bias != nullptr ? *reinterpret_cast<const float4*>(s_bias + col_base + c0 + 4 * q)
-                                : make_float4(0.f, 0.f, 0.f, 0.f);
-        if (c0 == 0) shift = v[0] + b[0];
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          const float x0 = v[j] + b[j] - shift, x1 = v[j + 1] + b[j + 1] - shift;
-          p1 += x0; p2 = fmaf(x0, x0, p2);
-          q1 += x1; q2 = fmaf(x1, x1, q2);
-        }
-      }
-      s1 = p1 + q1;
-      s2 = p2 + q2;
-    };
-
-    for (int st = 0; st < nsteps; ++st) {
-      for (int li = 0; li < L; ++li) {
-        const int l = desc ? L - 1 - li : li;
-        const int ti = st - l * lag;
-        if (ti < 0 || ti >= T) continue;
-        const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
-        const long long row0 = static_cast<long long>(tile) * kTileM + ew * 32;
-        const ChainLayer& cl = s_layer[l];
-        EpiCtx cx;
-        cx.out_ptr = cl.out; cx.outy_ptr = cl.out_y; cx.res_ptr = cl.residual;
-        cx.ld_out = cl.ld_out; cx.ld_outy = cl.ld_outy; cx.ld_res = cl.ld_res;
-        cx.s_bias = cl.bias_off >= 0 ? s_param + cl.bias_off : nullptr;
-        cx.s_scale = cl.scale_off >= 0 ? s_param + cl.scale_off : nullptr;
-        cx.s_offset = cl.offset_off >= 0 ? s_param + cl.offset_off : nullptr;
-        cx.n_pre = cl.n_pre;
-        cx.trace_u = tracing(u) ? static_cast<int>(u) : -1;
-        cx.img0 = cl.out_img != nullptr
-                      ? cl.out_img + static_cast<size_t>(tile) * (kMaxN / kKStep) * GCB_A_IMAGE_BLOCK
-                      : nullptr;
-        cx.img1 = nullptr;
-        cx.res_img = cl.res_img != nullptr
-                         ? cl.res_img + static_cast<size_t>(tile) * (kMaxN / kKStep) * GCB_A_IMAGE_BLOCK
-                         : nullptr;
-        // Residual = the kept result of an earlier layer: the slot this CTA's epilogue wrote for
-        // this tile (same threads, same rows and columns: program order makes it visible, and the
-        // slot cannot be rewritten before these warps reach tile ti + nslots themselves).
-        if (cl.res_q >= 0) cx.res_img = scratch_slot(cl.res_q, ti);
-        if (eg == 0 && ti + 1 < T && (cl.residual != nullptr || cl.res_img != nullptr)) {
-          // Pull the residual of this layer's NEXT tile into L2 now (a whole step ahead).
-          const uint32_t ntile = tile + ncl;
-          if (cl.residual != nullptr) {
-            const long long nrow = static_cast<long long>(ntile) * kTileM + ew * 32 + lane;
-            if (nrow < rows_total) ptx::bulk_prefetch_l2(cl.residual + nrow * cl.ld_res + col_base, kUnitN * 4);
-          } else if (ew == 0 && lane < kUnitN / kKStep) {
-            ptx::bulk_prefetch_l2(cl.res_img + (static_cast<size_t>(ntile) * (kMaxN / kKStep) +
-                                                (col_base >> 4) + lane) * GCB_A_IMAGE_BLOCK,
-                                  GCB_A_IMAGE_BLOCK);
-          }
-        }
-        const int keep_q = cl.keep_q;
-        const int kind = cl.kind;
-        if (keep_q >= 0) {
-          // previous readers of this slot (tile ti - nslots) are done in both CTAs
-          const long long w0 = tracing(u) ? clock64() : 0;
-          ptx::mbar_wait(&h_free_bar[keep_q * kChainSlotsMax + (ti % nslots)],
-                         (static_cast<uint32_t>(ti / nslots) & 1u) ^ 1u);
-          if (ew == 0 && lane == 0 && eg == 0) trace_val(u, 9, clock64() - w0);
-          cx.img1 = scratch_slot(keep_q, ti);
-        }
-        const uint32_t buf = u & 1;
-        ptx::mbar_wait(&tmem_full_bar[buf], (u >> 1) & 1);
-        ptx::tc_fence_after_sync();
-        if (ew == 0 && lane == 0 && eg == 0) trace(u, 3);
-        const uint32_t taddr = tmem_base + lane_base + buf * kUnitN;
-        if (kind >= kKindLN) {
-          const uint32_t lb = ln_count & 1, par = (ln_count >> 1) & 1;
-          float shift, s1, s2;
-          unit_shifted_sums(cx.s_bias, taddr, shift, s1, s2);
-          const float mean_h = shift + s1 * (1.0f / kUnitN);
-          const float m2_h = fmaxf(s2 - s1 * s1 * (1.0f / kUnitN), 0.f);
-          const int myrow = ew * 32 + lane;
-          // (with two epilogue groups both compute the statistics of all 256 columns and run
-          // their own exchange with the same group of the partner CTA: no coupling between groups)
-          ptx::st_async_f32x2(ptx::mapa(ptx::smem_addr(&my_lnx[lb * kTileM + myrow]), peer), mean_h, m2_h,
-                              ptx::mapa(ptx::smem_addr(&my_lnx_bar[lb]), peer));
-          if (ew == 0 && lane == 0) ptx::mbar_arrive_expect_tx(&my_lnx_bar[lb], kTileM * 8);
-          ptx::mbar_wait(&my_lnx_bar[lb], par);
-          const float2 other = my_lnx[lb * kTileM + myrow];
-          const float delta = other.x - mean_h;
-          const float mean = 0.5f * (mean_h + other.x);
-          const float var = (m2_h + other.y + delta * delta * (0.5f * kUnitN)) * (1.0f / (2 * kUnitN));
-          const float rstd = rsqrtf(var + 1e-5f);
-          if (ew == 0 && lane == 0 && eg == 0) trace(u, 4);
-          if (kind == kKindLNRes)
-            g_count = finish_unit(std::integral_constant<int, kKindLNRes>{}, cx, g_count, taddr, row0, mean, rstd);
-          else if (kind == kKindLNImg)
-            g_count = finish_unit(std::integral_constant<int, kKindLNImg>{}, cx, g_count, taddr, row0, mean, rstd);
-          else
-            g_count = finish_unit(std::integral_constant<int, kKindLN>{}, cx, g_count, taddr, row0, mean, rstd);
-          ++ln_count;
-        } else if (kind == kKindSwish) {
-          g_count = finish_unit(std::integral_constant<int, kKindSwish>{}, cx, g_count, taddr, row0, 0.f, 1.f);
-        } else {
-          g_count = finish_unit(std::integral_constant<int, kKindPlain>{}, cx, g_count, taddr, row0, 0.f, 1.f);
-        }
-        if (ew == 0 && lane == 0 && eg == 0) trace(u, 5);
-        // accumulator free for the MMA warp
-        ptx::tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[buf]);
-        if (keep_q >= 0) {
-          // Hand the slot to the TMA warps of both CTAs: my generic-proxy global stores must be
-          // visible to their async-proxy bulk copies.
-          ptx::fence_proxy_async_global();
-          __syncwarp();
-          if (lane == 0) {
-            uint64_t* hb = &h_full_bar[keep_q * kChainSlotsMax + (ti % nslots)];
-            ptx::mbar_arrive_release_cluster(hb);
-            ptx::mbar_arrive_remote(ptx::mapa(ptx::smem_addr(hb), peer));
-          }
-        }
-        if (ew == 0 && lane == 0 && eg == 0) trace(u, 10);
-        ++u;
-      }
-    }
-  } else {
-    // ===== gather warps: pre-activation addends of the split edge MLP =====
-    ptx::setmaxnreg_dec<kRegsProd>();
-    const int first_warp = 4 + 4 * kEpiGroups;
-    const int group = (warp - first_warp) >> 2;        // 0 (.. 1 with a single epilogue group)
-    const int tid_g = threadIdx.x - 32 * first_warp - group * 128;
-    if (kPre) {
-      // Thread (rp, cgp): rows rp + 16*p (p < 8), 16-byte column group cgp of each 32-column
-      // chunk: 8 lanes read one 128-byte line segment of a gathered row.  Chunk c goes to staging
-      // buffer c & 1; with two gather groups group g fills the chunks of its parity.
-      const int cgp = tid_g & 7, rp = tid_g >> 3;
-      uint32_t gc = 0;
-      const int gcol_lo = static_cast<int>(crank) * kUnitN, gcol_hi = gcol_lo + kUnitN;
-      for (int st = 0; st < nsteps; ++st) {
-        for (int li = 0; li < L; ++li) {
-          const int l = desc ? L - 1 - li : li;
-          const int ti = st - l * lag;
-          if (ti < 0 || ti >= T) continue;
-          const int n_pre = s_layer[l].n_pre;
-          if (n_pre == 0 || s_layer[l].kind >= kKindLN) continue;
-          const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
-          const long long trow0 = static_cast<long long>(tile) * kTileM;
-          const float* p0[8];
-          const float* p1[8];
-#pragma unroll
-          for (int p = 0; p < 8; ++p) {
-            const long long grow = trow0 + rp + 16 * p;
-            p0[p] = nullptr; p1[p] = nullptr;
-            if (grow < rows_total) {
-              const PreAddInfo a = s_pre[l * 2];
-              p0[p] = a.table + (a.idx ? static_cast<long long>(__ldg(a.idx + grow)) : grow) * a.ld + cgp * 4;
-              if (n_pre > 1) {
-                const PreAddInfo b = s_pre[l * 2 + 1];
-                p1[p] = b.table + (b.idx ? static_cast<long long>(__ldg(b.idx + grow)) : grow) * b.ld + cgp * 4;
-              }
-            }
-          }
-          for (int c0 = gcol_lo; c0 < gcol_hi; c0 += 32, ++gc) {
-            const uint32_t gb = gc & 1;
-            if (kGatherGroups == 2 && gb != static_cast<uint32_t>(group)) continue;
-            float4 acc[8];
-#pragma unroll
-            for (int p = 0; p < 8; ++p)
-              acc[p] = p0[p] ? __ldg(reinterpret_cast<const float4*>(p0[p] + c0)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            if (n_pre > 1) {
-#pragma unroll
-              for (int p = 0; p < 8; ++p) {
-                if (p1[p]) {
-                  const float4 t = __ldg(reinterpret_cast<const float4*>(p1[p] + c0));
-                  acc[p].x += t.x; acc[p].y += t.y; acc[p].z += t.z; acc[p].w += t.w;
-                }
-              }
-            }
-            ptx::mbar_wait(&g_empty_bar[gb], ((gc >> 1) & 1) ^ 1);
-            float* gdst = s_g + gb * kGBufFloats + rp * kEpiRowFloats + cgp * 4;
-#pragma unroll
-            for (int p = 0; p < 8; ++p)
-              *reinterpret_cast<float4*>(gdst + 16 * p * kEpiRowFloats) = acc[p];
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&g_full_bar[gb]);
-          }
-        }
+        if (kPre && s_layer[l].n_pre > 0 && s_layer[l].kind < kKindLN)
+          gc = stage_addends(s_g, g_full_bar, g_empty_bar, s_pre + l * 2, s_layer[l].n_pre,
+                             static_cast<long long>(tile) * kTileM, rows_total,
+                             static_cast<int>(crank) * kUnitN, gc, t64);
       }
     }
   }
 
   // ---- teardown ---------------------------------------------------------------
-  ptx::tc_fence_before_sync();
   __syncthreads();
   ptx::cluster_sync_all();
-  if (warp == 2) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 }  // namespace gcb

@@ -1,7 +1,7 @@
 // FP32 CUDA-core arm of the fused layer (GCB_PREC_FP32_SIMT).  Same contract as
 // the tensor-core kernel in mlp_tc.cuh (segments, gather, fan-in sum, bias,
 // swish, LayerNorm, residual), exact fp32 FFMA arithmetic.  It exists to
-// validate the tcgen05 path on the device; it is not a performance path.
+// validate the tensor-core (wgmma) path on the device; it is not a performance path.
 #pragma once
 #include <cuda_bf16.h>
 

@@ -1,37 +1,32 @@
-// Fused linear layer on tcgen05 tensor cores (sm_100a).
+// Fused linear layer on Hopper tensor cores (sm_90a, wgmma).
 //
 //   out[r] = residual[r] + LN( act( concat_s A_s(r) @ W + bias + gathered addends ) )
 //
-// One persistent 512-thread CTA per SM.  Work is cut into UNITS of 128 rows x 256 output
-// columns; TMEM holds TWO 128x256 fp32 accumulators, so the epilogue of unit u overlaps
-// the MMAs of unit u+1.  Two schedules:
+// One persistent 384-thread CTA per SM.  Work is cut into UNITS of 128 rows x 256 output
+// columns.  Two schedules:
 //   N-split (n = 512, cluster of 2): both CTAs of the cluster work on the SAME 128-row
 //     tile, CTA r owning output columns [256r, 256r+256).  The A block of every K-step is
 //     fetched once and multicast to both CTAs, each CTA streams only its half of the
 //     weights, and LayerNorm row statistics are combined across the pair through
 //     distributed shared memory.  Consecutive units of a CTA are consecutive tiles.
-//   unsplit (n = 256, or cluster of 1): every CTA walks its own tiles (n/256 units per
-//     tile); the CTAs of a cluster share the weight stream by multicast.
+//   unsplit (n = 256, or cluster of 1 / 4): every CTA walks its own tiles (n/256 units per
+//     tile); the CTAs of a cluster share the weight stream by multicast.  LayerNorm over
+//     512 columns needs the N-split schedule (the launcher enforces it).
 // Warp roles:
 //   warp 0        TMA lane: per K-step streams (a) 1/cluster of the pre-packed bf16 weight
 //                 tile with cp.async.bulk, multicast to every CTA of the cluster, and (b)
 //                 the A block of segments that are stored as operand images.
-//   warp 1        MMA lane: tcgen05.mma (M=128, N=256, K=16), three products per K-step in
-//                 BF16X3 mode (hi*hi, hi*lo, lo*hi), fp32 accumulation in TMEM; commits free
-//                 the stage (cluster-wide) and finally publish the accumulator.
-//   warp 2        TMEM allocator (512 columns).
-//   warps 4-7     epilogue: tcgen05.ld (thread = row), bias, gathered pre-activation
-//                 addends, swish | LayerNorm (+ residual).  fp32 outputs go through a
-//                 32x32 shared-memory transpose (full 128-byte lines); operand-image
-//                 outputs are written straight from the row layout (512-byte warp stores).
-//                 LayerNorm needs the whole 512-wide row: statistics are accumulated over
-//                 both units of a tile while the second unit's MMAs run, then both halves
-//                 are normalised and their accumulators released one after the other.
-//   warps 8-15    two producer groups.  A segments given as fp32 tables (optionally
-//                 gathered through an index, optionally a fan-in sum) are converted to
-//                 bf16 hi/lo and stored in the UMMA K-major core-matrix layout; gathered
-//                 pre-activation addends (node projections of the split edge MLP) are
-//                 staged into shared memory in 32-column chunks.
+//   warps 4-11    two consumer warpgroups, rows [0, 64) and [64, 128) of the tile: wgmma
+//                 (M=64, N=256, K=16), three products per K-step in BF16X3 mode (hi*hi,
+//                 hi*lo, lo*hi), fp32 accumulation in registers (128 per thread), then the
+//                 epilogue straight from the accumulator fragment: bias, gathered
+//                 pre-activation addends, swish | LayerNorm (+ residual), fp32 and / or
+//                 operand-image outputs.
+//   warps 2-3     producers.  A segments given as fp32 tables (optionally gathered through
+//                 an index, optionally a fan-in sum) are converted to bf16 hi/lo and stored
+//                 in the K-major core-matrix layout; gathered pre-activation addends (node
+//                 projections of the split edge MLP) are staged into shared memory in
+//                 32-column chunks, unit by unit after that unit's A operand.
 //
 // Shared-memory operand layout (no swizzle, K-major): a [R x 16] bf16 operand of one
 // K-step is two "K chunks" of 8 elements; chunk c, row r lives at byte c*LBO + r*16.
@@ -46,7 +41,7 @@ namespace gcb {
 constexpr int kTileM = 128;
 constexpr int kUnitN = 256;                       // output columns per unit / accumulator
 constexpr int kKStep = 16;
-constexpr int kThreads = 512;
+constexpr int kThreads = 384;
 // A operand: the two 8-element K chunks of a K-step are 2048 + 64 bytes apart.  The
 // 64-byte skew puts chunk 1 on the other 16 banks so that the producers' 8-byte
 // stores (rows 0-3 of both chunks per half-warp) are conflict-free.
@@ -55,23 +50,21 @@ constexpr int kAPartBytes = 2 * kALbo;            // 4224: one of {hi, lo}
 constexpr int kBLbo = kUnitN * 16;                // 4096
 constexpr int kBPartBytes = 2 * kBLbo;            // 8192: one of {hi, lo} of a 256-row weight block
 constexpr int kEpiRowFloats = 36;                 // 32 + 4 pad: conflict-free 16 B accesses
-constexpr int kEpiStageBytes = 4 * 32 * kEpiRowFloats * 4;   // per-warp 32x32 transpose tiles
 // Pre-activation addend chunks (gathered node projections), double buffered:
 // [2][128 rows][36 floats], filled by the producer groups, read by the epilogue.
 constexpr int kGBufFloats = kTileM * kEpiRowFloats;
 constexpr int kGBytes = 2 * kGBufFloats * 4;
 constexpr int kMaxN = 512;
 constexpr int kMaxKSteps = 128;                   // K <= 2048
-constexpr int kTmemCols = 512;
+constexpr int kConsumerWarps = 8;                 // warps 4-11: two warpgroups of 64 tile rows each
+constexpr int kProducerWarps = 2;                 // warps 2-3
 static_assert(2 * kAPartBytes == GCB_A_IMAGE_BLOCK, "A image block must match the stage layout");
 
-// Shared-memory budget: everything the variant does not need goes to pipeline stages -
-// the operand ring is latency-bound (tools/pipe_rate.cu: 6 stages 411, 8 stages 389 cycles
-// per K-step for a 384-cycle bf16x3 K-step).  LayerNorm variants never stage gathered
-// addends (only the 2 KB statistics exchange aliases that region); the others carry no
-// LayerNorm scale / offset.
+// Shared-memory budget: everything the variant does not need goes to pipeline stages.
+// LayerNorm variants never stage gathered addends (only the 2 KB statistics exchange
+// aliases that region); the others carry no LayerNorm scale / offset.
 constexpr int kSmemLimit = 227 * 1024;            // opt-in dynamic shared memory per CTA
-constexpr int kTailBytes = 1024;                  // barriers, TMEM slot, segment tables
+constexpr int kTailBytes = 1024;                  // barriers, segment tables
 constexpr int kLnxBytes = 2 * kTileM * 8;         // [2][128] (mean, M2) pairs
 
 template <bool kSplit, bool kLN>
@@ -81,9 +74,9 @@ struct TcConfig {
   static constexpr int kStageBytes = kAStageBytes + kBStageBytes;
   static constexpr int kParamBytes = (kLN ? 3 : 1) * kMaxN * 4;   // bias (, ln scale, ln offset)
   static constexpr int kGRegionBytes = kLN ? kLnxBytes : kGBytes;
-  static constexpr int kFixedBytes = kParamBytes + kEpiStageBytes + kGRegionBytes + kTailBytes;
+  static constexpr int kFixedBytes = kParamBytes + kGRegionBytes + kTailBytes;
   static constexpr int kFit = (kSmemLimit - kFixedBytes) / kStageBytes;
-  static constexpr int kStages = kFit < 12 ? kFit : 12;           // tail holds 2*12+10 barriers
+  static constexpr int kStages = kFit < 12 ? kFit : 12;           // tail holds 2*12+8 barriers
   static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
   static_assert(kStages >= 4, "operand ring too shallow");
 };
@@ -133,6 +126,163 @@ struct PreAddInfo {
   long long ld;
 };
 
+// ---- consumer warpgroup helpers (shared with mlp_chain.cuh) ------------------------
+// Fragment coordinates: consumer thread t of warp w of warpgroup g holds tile rows
+// frag_row(h) = 64g + 16w + t/4 + 8h and columns 8j + 2(t%4) + e of the unit (ptx.cuh).
+
+// The MMAs of one unit for this warpgroup's 64 rows (A rows start a_row_off bytes into the
+// stage).  After each K-step the previous one is retired and its stage released: one arrival
+// per warp, on the local barrier (rel_mask == 0) or on the barrier of every CTA in rel_mask.
+template <bool kSplit, int kStages, int kStageBytes, int kAStageBytes>
+__device__ __forceinline__ void mma_unit(float (&acc)[128], uint8_t* stage_base, uint64_t* full_bar,
+                                         uint64_t* empty_bar, uint32_t& stage, uint32_t& phase,
+                                         int ksteps, uint32_t a_row_off, uint32_t rel_mask) {
+  const bool lead = (threadIdx.x & 31) == 0;
+  auto release = [&](uint32_t s) {
+    if (!lead) return;
+    if (rel_mask == 0) {
+      ptx::mbar_arrive(&empty_bar[s]);
+    } else {
+      const uint32_t a = ptx::smem_addr(&empty_bar[s]);
+      for (uint32_t r = 0; r < 4; ++r)
+        if ((rel_mask >> r) & 1u) ptx::mbar_arrive_remote(ptx::mapa(a, r));
+    }
+  };
+  uint32_t prev = 0;
+  for (int ks = 0; ks < ksteps; ++ks) {
+    ptx::mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = ptx::smem_addr(stage_base + stage * kStageBytes);
+    const uint64_t a_hi = ptx::make_smem_desc(sa + a_row_off, kALbo, 128);
+    const uint64_t b_hi = ptx::make_smem_desc(sa + kAStageBytes, kBLbo, 128);
+    ptx::fence_regs(acc);
+    ptx::wgmma_fence();
+    ptx::wgmma_bf16_m64n256(acc, a_hi, b_hi, ks > 0 ? 1u : 0u);
+    if (kSplit) {
+      // descriptors differ only in the 16-byte-unit start address field
+      ptx::wgmma_bf16_m64n256(acc, a_hi, b_hi + (kBPartBytes >> 4), 1u);
+      ptx::wgmma_bf16_m64n256(acc, a_hi + (kAPartBytes >> 4), b_hi, 1u);
+    }
+    ptx::wgmma_commit();
+    ptx::fence_regs(acc);
+    if (ks > 0) {
+      ptx::wgmma_wait<1>();
+      release(prev);
+    }
+    prev = stage;
+    if (++stage == kStages) { stage = 0; phase ^= 1; }
+  }
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(acc);
+  release(prev);
+}
+
+// Shifted sums of this thread's two rows over the unit columns c < ncols, bias included:
+// s1 = sum(x - shift), s2 = sum((x - shift)^2) with shift = the row's value in column 0,
+// reduced over the four threads that share a row.
+__device__ __forceinline__ void row_shifted_sums(const float (&acc)[128], const float* bias, int ncols,
+                                                 float (&shift)[2], float (&s1)[2], float (&s2)[2]) {
+  const int q = threadIdx.x & 3;
+  const float b0 = bias != nullptr ? bias[0] : 0.f;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    shift[h] = __shfl_sync(0xffffffffu, acc[2 * h] + b0, (threadIdx.x & 31) & ~3);
+    s1[h] = 0.f;
+    s2[h] = 0.f;
+  }
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const int c = 8 * j + 2 * q;
+    const float2 b = bias != nullptr ? *reinterpret_cast<const float2*>(bias + c) : make_float2(0.f, 0.f);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (c < ncols) {
+        const float x = acc[4 * j + 2 * h] + b.x - shift[h];
+        s1[h] += x; s2[h] = fmaf(x, x, s2[h]);
+      }
+      if (c + 1 < ncols) {
+        const float x = acc[4 * j + 2 * h + 1] + b.y - shift[h];
+        s1[h] += x; s2[h] = fmaf(x, x, s2[h]);
+      }
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      s1[h] += __shfl_xor_sync(0xffffffffu, s1[h], o);
+      s2[h] += __shfl_xor_sync(0xffffffffu, s2[h], o);
+    }
+  }
+}
+
+// Adds the staged pre-activation addends of one 32-column chunk (rows of this thread).
+__device__ __forceinline__ void add_staged_chunk(float (&acc)[128], int j0, const float* gbuf, int lr0) {
+  const int q = threadIdx.x & 3;
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float2 g = *reinterpret_cast<const float2*>(gbuf + (lr0 + 8 * h) * kEpiRowFloats + 8 * jj + 2 * q);
+      acc[4 * (j0 + jj) + 2 * h] += g.x;
+      acc[4 * (j0 + jj) + 2 * h + 1] += g.y;
+    }
+  }
+}
+
+// Byte offset of the 4-byte (two-column) piece of global column gc (even) of tile row r in
+// the operand image of one 128-row tile; "lo" lives kAPartBytes further.
+__device__ __forceinline__ size_t image_offset(int gc, int r) {
+  return static_cast<size_t>(gc >> 4) * GCB_A_IMAGE_BLOCK + ((gc >> 3) & 1) * kALbo + r * 16 + (gc & 7) * 2;
+}
+
+// Gathered pre-activation addends (node projections of the split edge MLP) of the 256 columns
+// [gcol_lo, gcol_lo + 256) of one tile, staged 32 columns at a time into the double buffer s_g
+// ([2][128][36]; chunk count gc selects buffer and phase) by the kProducerWarps producer warps.
+// Thread t: rows t/8 + 8p (p < 16), 16-byte column group t%8 of each chunk, so that 8 lanes read
+// one 128-byte line segment of a gathered row.  Returns the updated chunk count.
+__device__ __forceinline__ uint32_t stage_addends(float* s_g, uint64_t* g_full_bar, uint64_t* g_empty_bar,
+                                                  const PreAddInfo* s_pre, int n_pre, long long trow0,
+                                                  long long rows_total, int gcol_lo, uint32_t gc, int t64) {
+  const int cgp = t64 & 7, rp = t64 >> 3;
+  const PreAddInfo a = s_pre[0];
+  const PreAddInfo b = s_pre[n_pre > 1 ? 1 : 0];
+  int r0[16], r1[16];                            // source rows (-1: past the end)
+#pragma unroll
+  for (int p = 0; p < 16; ++p) {
+    const long long grow = trow0 + rp + 8 * p;
+    r0[p] = -1; r1[p] = -1;
+    if (grow < rows_total) {
+      r0[p] = a.idx ? __ldg(a.idx + grow) : static_cast<int>(grow);
+      if (n_pre > 1) r1[p] = b.idx ? __ldg(b.idx + grow) : static_cast<int>(grow);
+    }
+  }
+  for (int c0 = gcol_lo; c0 < gcol_lo + kUnitN; c0 += 32, ++gc) {
+    const uint32_t gb = gc & 1;
+    ptx::mbar_wait(&g_empty_bar[gb], ((gc >> 1) & 1) ^ 1);
+    float* gdst = s_g + gb * kGBufFloats + rp * kEpiRowFloats + cgp * 4;
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      float4 v[8];
+#pragma unroll
+      for (int p = 0; p < 8; ++p) {
+        const int i = 8 * half + p;
+        v[p] = r0[i] >= 0 ? __ldg(reinterpret_cast<const float4*>(a.table + static_cast<long long>(r0[i]) * a.ld + c0 + cgp * 4))
+                          : make_float4(0.f, 0.f, 0.f, 0.f);
+        if (r1[i] >= 0) {
+          const float4 t = __ldg(reinterpret_cast<const float4*>(b.table + static_cast<long long>(r1[i]) * b.ld + c0 + cgp * 4));
+          v[p].x += t.x; v[p].y += t.y; v[p].z += t.z; v[p].w += t.w;
+        }
+      }
+#pragma unroll
+      for (int p = 0; p < 8; ++p)
+        *reinterpret_cast<float4*>(gdst + 8 * (8 * half + p) * kEpiRowFloats) = v[p];
+    }
+    __syncwarp();
+    if ((t64 & 31) == 0) ptx::mbar_arrive(&g_full_bar[gb]);
+  }
+  return gc;
+}
+
 // kSplit: bf16x3 (hi/lo) vs single bf16 product.  kSwish / kLN: epilogue variant,
 // compile-time so the per-element loops are straight-line code.
 template <bool kSplit, bool kSwish, bool kLN>
@@ -144,18 +294,14 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
   float* s_bias = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes);
   float* s_scale = s_bias + kMaxN;                                  // LayerNorm variants only
   float* s_offset = s_scale + kMaxN;                                // LayerNorm variants only
-  float* s_epi = s_bias + Cfg::kParamBytes / 4;                     // [4][32][36]
-  float* s_g = s_epi + 4 * 32 * kEpiRowFloats;                      // [2][128][36] (not kLN)
+  float* s_g = s_bias + Cfg::kParamBytes / 4;                       // [2][128][36] (not kLN)
   uint8_t* tail = reinterpret_cast<uint8_t*>(s_g) + Cfg::kGRegionBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);          // [kStages]
   uint64_t* empty_bar = full_bar + Cfg::kStages;                   // [kStages]
-  uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;              // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;                    // [2]
-  uint64_t* g_full_bar = tmem_empty_bar + 2;                       // [2]
+  uint64_t* g_full_bar = empty_bar + Cfg::kStages;                 // [2]
   uint64_t* g_empty_bar = g_full_bar + 2;                          // [2]
-  uint64_t* lnx_bar = g_empty_bar + 2;                             // [2] LayerNorm pair exchange
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(lnx_bar + 2);
-  SegInfo* s_seg = reinterpret_cast<SegInfo*>(tmem_base_slot + 2);        // [3]
+  uint64_t* lnx_bar = g_empty_bar + 2;                             // [2 warpgroups][2] LayerNorm pair exchange
+  SegInfo* s_seg = reinterpret_cast<SegInfo*>(lnx_bar + 4);               // [3]
   PreAddInfo* s_pre = reinterpret_cast<PreAddInfo*>(s_seg + 3);           // [2]
   KStepInfo* ks_info = reinterpret_cast<KStepInfo*>(s_pre + 2);           // [kMaxKSteps]
   // [2][128] LayerNorm statistics received from the partner CTA (N-split).  Aliases the
@@ -199,6 +345,7 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
   // (experiment, debug flag 4) N-split pair without A multicast: each CTA streams the whole
   // block itself and recycles its stages on its own MMAs only.
   const bool decouple = nsplit && (dbg & 4);
+  const bool gather_mode = !kLN && n_pre > 0;
 
   // ---- one-time setup ---------------------------------------------------------
   for (int i = threadIdx.x; i < n; i += kThreads) {
@@ -232,37 +379,27 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
         ++ks;
       }
     for (int s = 0; s < Cfg::kStages; ++s) {
-      // 1 TMA lane (+ 4 activation-producer warps unless A comes from images only)
-      ptx::mbar_init(&full_bar[s], a_is_img ? 1 : 5);
-      ptx::mbar_init(&empty_bar[s], decouple ? 1 : csize);  // tcgen05.commit of every CTA in the cluster
+      // 1 TMA lane (+ the producer warps unless A comes from images only)
+      ptx::mbar_init(&full_bar[s], a_is_img ? 1 : 1 + kProducerWarps);
+      // every consumer warp of every CTA that shares the stage
+      ptx::mbar_init(&empty_bar[s], (decouple ? 1 : csize) * kConsumerWarps);
     }
     for (int b = 0; b < 2; ++b) {
-      ptx::mbar_init(&tmem_full_bar[b], 1);
-      ptx::mbar_init(&tmem_empty_bar[b], 4);   // 4 epilogue warps
-      ptx::mbar_init(&g_full_bar[b], 4);       // 4 warps of one producer group
-      ptx::mbar_init(&g_empty_bar[b], 4);      // 4 epilogue warps
-      ptx::mbar_init(&lnx_bar[b], 1);          // my expect_tx; the partner's 128 st.async complete it
+      ptx::mbar_init(&g_full_bar[b], kProducerWarps);     // every producer warp
+      ptx::mbar_init(&g_empty_bar[b], kConsumerWarps);    // every consumer warp
+      ptx::mbar_init(&lnx_bar[b], 1);          // my expect_tx; the partner's 64 st.async complete it
+      ptx::mbar_init(&lnx_bar[2 + b], 1);
     }
     ptx::fence_mbar_init();
   }
-  if (warp == 2) {
-    ptx::tmem_alloc(tmem_base_slot, kTmemCols);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before_sync();
   __syncthreads();
   ptx::cluster_sync_all();          // barrier inits visible cluster-wide before remote arrives
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_base_slot;
 
   // ---- roles ------------------------------------------------------------------
   if (warp == 0) {
     // ===== TMA warp =====
-    // Converged warp, every lane polls, ONE elected lane issues (see the MMA warp).  The
-    // loop body is kept minimal - running pointers, ring counters, one SegInfo read per
-    // segment: the issuing warp shares its scheduler with an epilogue warp, and a body of
-    // ~500 cycles per K-step (table lookups + 64-bit address math + waterfall loops) made
-    // this warp, not HBM or the tensor pipe, the limiter of the whole kernel.
+    // Converged warp, every lane polls, ONE elected lane issues.  The loop body is kept
+    // minimal - running pointers, ring counters, one SegInfo read per segment.
     const uint32_t b_bytes = Cfg::kBStageBytes;                 // hi (| lo) of a 256-row block
     const size_t b_block = 2 * kBPartBytes;                     // image always holds hi|lo
     const size_t b_stride = static_cast<size_t>(n_halves) * b_block;   // next K-step, same half
@@ -321,444 +458,176 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
         if (lane == 0) trace_val(tu, 7, blocked);
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA warp =====
-    // The whole warp runs the loop on warp-uniform values and ONE elected lane issues the
-    // tcgen05 instructions.  Under `if (lane == 0)` every operand is divergent and the
-    // compiler wraps each UTCHMMA / UTCBAR in a vector->uniform "waterfall" loop, which
-    // made the issuing thread, not the tensor pipe, the limiter (tools/pipe_rate.cu: 432 vs
-    // 389 cycles per K-step).  All lanes poll: a single poller with 31 lanes parked at the
-    // warp barrier is 2x slower (same benchmark, style 2).
-    {
-      const uint32_t idesc = ptx::make_idesc_bf16(kTileM, kUnitN);
-      uint32_t stage = 0, phase = 0, u = 0;
-      for (uint32_t base = tile_first; base < static_cast<uint32_t>(num_tiles); base += tile_stride) {
-        for (int uh = 0; uh < units_per_tile; ++uh, ++u) {
-          const uint32_t buf = u & 1;
-          ptx::mbar_wait(&tmem_empty_bar[buf], ((u >> 1) & 1) ^ 1);
-          ptx::tc_fence_after_sync();
-          if (lane == 0) trace(u, 0);
-          const uint32_t dcol = tmem_base + buf * kUnitN;
-          long long starved = 0;
-          const bool tr = tracing(u);
-          for (int ks = 0; ks < ksteps; ++ks) {
-            const long long w0 = tr ? clock64() : 0;
-            ptx::mbar_wait(&full_bar[stage], phase);
-            if (tr) starved += clock64() - w0;
-            ptx::tc_fence_after_sync();
-            if (ks == 0 && lane == 0) trace(u, 1);
-            const uint32_t sa = ptx::smem_addr(stage_base + stage * Cfg::kStageBytes);
-            const uint32_t sb = sa + Cfg::kAStageBytes;
-            const uint64_t a_hi = ptx::make_smem_desc(sa, kALbo, 128);
-            const uint64_t b_hi = ptx::make_smem_desc(sb, kBLbo, 128);
-            if (ptx::elect_one()) {
-              ptx::mma_bf16_ss(dcol, a_hi, b_hi, idesc, ks > 0 ? 1u : 0u);
-              if (kSplit) {
-                // descriptors differ only in the 16-byte-unit start address field
-                const uint64_t a_lo = a_hi + (kAPartBytes >> 4);
-                const uint64_t b_lo = b_hi + (kBPartBytes >> 4);
-                ptx::mma_bf16_ss(dcol, a_hi, b_lo, idesc, 1u);
-                ptx::mma_bf16_ss(dcol, a_lo, b_hi, idesc, 1u);
-              }
-              // stage reusable (cluster-wide) once these MMAs retire
-              if (csize == 1 || decouple) ptx::mma_commit(&empty_bar[stage]);
-              else ptx::mma_commit_multicast(&empty_bar[stage], cmask);
-            }
-            __syncwarp();
-            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-          }
-          if (ptx::elect_one()) ptx::mma_commit(&tmem_full_bar[buf]);          // accumulator complete
-          __syncwarp();
-          if (lane == 0) {
-            trace(u, 2);
-            trace_val(u, 6, starved);
-          }
-        }
-      }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===== epilogue =====
-    const int ew = warp - 4;                     // == warp % 4: TMEM lane quarter
-    const uint32_t lane_base = static_cast<uint32_t>(ew * 32) << 16;
+  } else if (warp >= 4) {
+    // ===== consumers: MMA + epilogue =====
+    const int eg = (warp - 4) >> 2;                // warpgroup: tile rows [64 eg, 64 eg + 64)
+    const int q = lane & 3;
+    const int lr0 = eg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile rows lr0, lr0 + 8
     const int n_valid = d.n_valid;
-    float* my_epi = s_epi + ew * 32 * kEpiRowFloats;
-    const int cg = lane & 7;                     // 16-byte column group inside the 32-col block
-    const int rsub = lane >> 3;                  // row within a group of 4
-    uint32_t g_count = 0;
-
-    // LayerNorm statistics of one unit: shifted sums over its valid columns.
-    auto stats_unit = [&](uint32_t taddr, int col_base, int ncols, float& shift, float& s1,
-                          float& s2, bool first) {
-      for (int c0 = 0; c0 < ncols; c0 += 32) {
-        float v[32];
-        ptx::tmem_ld32(taddr + c0, v);
-        float b[32];
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          *reinterpret_cast<float4*>(&b[4 * q]) =
-              *reinterpret_cast<const float4*>(s_bias + col_base + c0 + 4 * q);
-        if (first && c0 == 0) shift = v[0] + b[0];
-        if (c0 + 32 <= ncols) {
-          float p1 = 0.f, p2 = 0.f, q1 = 0.f, q2 = 0.f;   // two chains for ILP
-#pragma unroll
-          for (int j = 0; j < 32; j += 2) {
-            const float x0 = v[j] + b[j] - shift, x1 = v[j + 1] + b[j + 1] - shift;
-            p1 += x0; p2 = fmaf(x0, x0, p2);
-            q1 += x1; q2 = fmaf(x1, x1, q2);
-          }
-          s1 += p1 + q1; s2 += p2 + q2;
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            if (c0 + j < ncols) {
-              const float x = v[j] + b[j] - shift;
-              s1 += x;
-              s2 = fmaf(x, x, s2);
-            }
-          }
-        }
-      }
-    };
-
-    // Finish one unit: bias, addends, activation / normalisation, outputs.  Only one warp
-    // per SM sub-partition runs this, so nothing hides latency for it: the fast path is
-    // branch-free and batches its loads (residual rows are requested before the TMEM read,
-    // the eight shared-memory reads are issued back to back).
-    auto finish_unit = [&](uint32_t taddr, uint32_t tile, long long row0, int col_base, int ncols,
-                           float mean, float rstd) {
-      const bool rows_full = row0 + 32 <= rows_total;
-      const bool tile_ok = tile < static_cast<uint32_t>(num_tiles);
-      for (int c0 = 0; c0 < ncols; c0 += 32) {
-        const int gc0 = col_base + c0;             // global column of this 32-wide block
-        const int col = gc0 + cg * 4;
-        const bool fast = rows_full && (c0 + 32 <= ncols);
-        float4 rr[8];
-        if (fast && res_ptr != nullptr) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            rr[i] = *reinterpret_cast<const float4*>(res_ptr + (row0 + rsub + 4 * i) * ld_res + col);
-        }
-        float v[32];
-        ptx::tmem_ld32(taddr + c0, v);
-        {
-          float b[32];
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(&b[4 * q]) = *reinterpret_cast<const float4*>(s_bias + gc0 + 4 * q);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += b[j];
-        }
-        if (!kLN && n_pre > 0) {
-          // Add the gathered node projections staged by the producer groups.
-          const uint32_t gb = g_count & 1;
-          ptx::mbar_wait(&g_full_bar[gb], (g_count >> 1) & 1);
-          const float* gp = s_g + gb * kGBufFloats + (ew * 32 + lane) * kEpiRowFloats;
-          float g[32];
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(&g[4 * q]) = *reinterpret_cast<const float4*>(gp + 4 * q);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += g[j];
-          __syncwarp();
-          if (lane == 0) ptx::mbar_arrive(&g_empty_bar[gb]);
-          ++g_count;
-        }
-        if (kSwish) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = swish_f(v[j]);
-        }
-        if (kLN) {
-          float g[32];
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(&g[4 * q]) = *reinterpret_cast<const float4*>(s_scale + gc0 + 4 * q);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = (v[j] - mean) * rstd * g[j];
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(&g[4 * q]) = *reinterpret_cast<const float4*>(s_offset + gc0 + 4 * q);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += g[j];
-        }
-        if (out_ptr != nullptr || outy_ptr != nullptr) {
-          // 32x32 transpose through the padded per-warp tile: 8 lanes then cover one
-          // 128-byte row segment and a warp store writes four complete lines.
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(my_epi + lane * kEpiRowFloats + q * 4) =
-                make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-          __syncwarp();
-          if (fast) {
-            float4 y[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-              y[i] = *reinterpret_cast<const float4*>(my_epi + (rsub + 4 * i) * kEpiRowFloats + cg * 4);
-            if (outy_ptr != nullptr) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                *reinterpret_cast<float4*>(outy_ptr + (row0 + rsub + 4 * i) * ld_outy + col) = y[i];
-            }
-            if (out_ptr != nullptr) {
-              if (res_ptr != nullptr) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  y[i].x += rr[i].x; y[i].y += rr[i].y; y[i].z += rr[i].z; y[i].w += rr[i].w;
-                }
-              }
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                *reinterpret_cast<float4*>(out_ptr + (row0 + rsub + 4 * i) * ld_out + col) = y[i];
-            }
-            if (out_img != nullptr && res_ptr != nullptr) {
-              // The image must hold residual + y: hand the sums back through the tile.
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                *reinterpret_cast<float4*>(my_epi + (rsub + 4 * i) * kEpiRowFloats + cg * 4) = y[i];
-            }
-          } else {
-            // Ragged edge (last rows of the matrix / last partial column block).
-            for (int i = 0; i < 8; ++i) {
-              const int r = rsub + 4 * i;
-              const long long grow = row0 + r;
-              if (grow < rows_total) {
-                for (int e = 0; e < 4 && c0 + cg * 4 + e < ncols; ++e) {
-                  const float yv = my_epi[r * kEpiRowFloats + cg * 4 + e];
-                  const float ov = yv + (res_ptr ? res_ptr[grow * ld_res + col + e] : 0.f);
-                  if (outy_ptr != nullptr) outy_ptr[grow * ld_outy + col + e] = yv;
-                  if (out_ptr != nullptr) out_ptr[grow * ld_out + col + e] = ov;
-                  if (out_img != nullptr) my_epi[r * kEpiRowFloats + cg * 4 + e] = ov;
-                }
-              }
-            }
-          }
-          __syncwarp();
-          if (out_img != nullptr && res_ptr != nullptr) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              *reinterpret_cast<float4*>(&v[4 * q]) =
-                  *reinterpret_cast<const float4*>(my_epi + lane * kEpiRowFloats + q * 4);
-            __syncwarp();
-          }
-        }
-        if (out_img != nullptr && tile_ok) {
-          // Operand image of this tile for a later layer: thread = row, so the 16-byte
-          // pieces of 32 consecutive rows are contiguous -> 512-byte coalesced warp stores.
-          uint8_t* blk = out_img + (static_cast<size_t>(tile) * (n >> 4) + (gc0 >> 4)) * GCB_A_IMAGE_BLOCK +
-                         (ew * 32 + lane) * 16;
-#pragma unroll
-          for (int ks2 = 0; ks2 < 2; ++ks2) {
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              const float* x = &v[ks2 * 16 + c * 8];
-              uint2 h0, l0, h1, l1;
-              ptx::split_bf16x4(make_float4(x[0], x[1], x[2], x[3]), h0, l0);
-              ptx::split_bf16x4(make_float4(x[4], x[5], x[6], x[7]), h1, l1);
-              uint8_t* dst = blk + ks2 * GCB_A_IMAGE_BLOCK + c * kALbo;
-              *reinterpret_cast<uint4*>(dst) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-              *reinterpret_cast<uint4*>(dst + kAPartBytes) = make_uint4(l0.x, l0.y, l1.x, l1.y);
-            }
-          }
-        }
-      }
-    };
-
-    auto release = [&](uint32_t buf) {
-      ptx::tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[buf]);
-    };
-
-    // One pass over a full 256-column unit: shifted sums  s1 = sum(x - shift),
-    // s2 = sum((x - shift)^2)  with shift = the row's first value of this unit.
-    auto unit_shifted_sums = [&](uint32_t taddr, int col_base, float& shift, float& s1, float& s2) {
-      float p1 = 0.f, p2 = 0.f, q1 = 0.f, q2 = 0.f;     // two chains for ILP
-      for (int c0 = 0; c0 < kUnitN; c0 += 32) {
-        float v[32];
-        ptx::tmem_ld32(taddr + c0, v);
-        float b[32];
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          *reinterpret_cast<float4*>(&b[4 * q]) =
-              *reinterpret_cast<const float4*>(s_bias + col_base + c0 + 4 * q);
-        if (c0 == 0) shift = v[0] + b[0];
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          const float x0 = v[j] + b[j] - shift, x1 = v[j + 1] + b[j + 1] - shift;
-          p1 += x0; p2 = fmaf(x0, x0, p2);
-          q1 += x1; q2 = fmaf(x1, x1, q2);
-        }
-      }
-      s1 = p1 + q1;
-      s2 = p2 + q2;
-    };
-
-    uint32_t u = 0;
+    const bool lead = lane == 0 && (warp & 3) == 0;
+    const uint32_t rel_mask = (csize == 1 || decouple) ? 0u : cmask;
+    // The image holds residual + y when an fp32 output is written, y otherwise.
+    const bool img_res = res_ptr != nullptr && (out_ptr != nullptr || outy_ptr != nullptr);
+    uint32_t stage = 0, phase = 0, g_count = 0, ln_count = 0, u = 0;
+    float acc[128];
     for (uint32_t base = tile_first; base < static_cast<uint32_t>(num_tiles); base += tile_stride) {
       const uint32_t tile = base + tile_off;
-      const long long row0 = static_cast<long long>(tile) * kTileM + ew * 32;
-      if (!kLN) {
-        for (int uh = 0; uh < units_per_tile; ++uh, ++u) {
-          const int h = nsplit ? static_cast<int>(crank) : uh;
-          const uint32_t buf = u & 1;
-          ptx::mbar_wait(&tmem_full_bar[buf], (u >> 1) & 1);
-          ptx::tc_fence_after_sync();
-          if (ew == 0 && lane == 0) trace(u, 3);
-          const int col_base = h * kUnitN;
-          const int ncols = min(kUnitN, n_valid - col_base);
-          finish_unit(tmem_base + lane_base + buf * kUnitN, tile, row0, col_base, ncols, 0.f, 1.f);
-          if (ew == 0 && lane == 0) trace(u, 5);
-          release(buf);
-        }
-      } else if (nsplit) {
-        // LayerNorm over a row whose two halves live in the two CTAs of the cluster: each
-        // CTA computes (mean, M2) of its 256 columns, hands them to the partner through
-        // distributed shared memory, and both combine them (Chan's parallel update).
-        const uint32_t buf = u & 1, par = (u >> 1) & 1;
-        ptx::mbar_wait(&tmem_full_bar[buf], par);
-        ptx::tc_fence_after_sync();
-        if (ew == 0 && lane == 0) trace(u, 3);
-        const int col_base = static_cast<int>(crank) * kUnitN;
-        const uint32_t taddr = tmem_base + lane_base + buf * kUnitN;
-        float shift, s1, s2;
-        unit_shifted_sums(taddr, col_base, shift, s1, s2);
-        const float mean_h = shift + s1 * (1.0f / kUnitN);              // mean of my 256 columns
-        const float m2_h = fmaxf(s2 - s1 * s1 * (1.0f / kUnitN), 0.f);  // sum of squared deviations
-        const int myrow = ew * 32 + lane;
-        const uint32_t peer = crank ^ 1u;
-        ptx::st_async_f32x2(ptx::mapa(ptx::smem_addr(&s_lnx[buf * kTileM + myrow]), peer), mean_h, m2_h,
-                            ptx::mapa(ptx::smem_addr(&lnx_bar[buf]), peer));
-        if (ew == 0 && lane == 0) ptx::mbar_arrive_expect_tx(&lnx_bar[buf], kTileM * 8);
-        ptx::mbar_wait(&lnx_bar[buf], par);
-        const float2 other = s_lnx[buf * kTileM + myrow];
-        const float delta = other.x - mean_h;
-        const float mean = 0.5f * (mean_h + other.x);
-        const float var = (m2_h + other.y + delta * delta * (0.5f * kUnitN)) * (1.0f / (2 * kUnitN));
-        const float rstd = rsqrtf(var + 1e-5f);
-        if (ew == 0 && lane == 0) trace(u, 4);
-        finish_unit(taddr, tile, row0, col_base, kUnitN, mean, rstd);
-        if (ew == 0 && lane == 0) trace(u, 5);
-        release(buf);
-        ++u;
-      } else {
-        // Statistics over all units of the row (overlapping the MMAs of the later ones),
-        // then normalise / store unit by unit, releasing each accumulator as soon as done.
-        float shift = 0.f, s1 = 0.f, s2 = 0.f;
-        const uint32_t u0 = u;
-        for (int h = 0; h < n_halves; ++h, ++u) {
-          const uint32_t buf = u & 1;
-          ptx::mbar_wait(&tmem_full_bar[buf], (u >> 1) & 1);
-          ptx::tc_fence_after_sync();
-          if (ew == 0 && lane == 0) trace(u, 3);
-          const int col_base = h * kUnitN;
-          stats_unit(tmem_base + lane_base + buf * kUnitN, col_base, min(kUnitN, n_valid - col_base),
-                     shift, s1, s2, h == 0);
-          if (ew == 0 && lane == 0) trace(u, 4);
-        }
-        const float inv_n = 1.0f / static_cast<float>(n_valid);
-        const float m1 = s1 * inv_n;
-        const float mean = shift + m1;
-        const float rstd = rsqrtf(fmaxf(s2 * inv_n - m1 * m1, 0.f) + 1e-5f);
-        for (int h = 0; h < n_halves; ++h) {
-          const uint32_t uu = u0 + h, buf = uu & 1;
-          const int col_base = h * kUnitN;
-          finish_unit(tmem_base + lane_base + buf * kUnitN, tile, row0, col_base,
-                      min(kUnitN, n_valid - col_base), mean, rstd);
-          if (ew == 0 && lane == 0) trace(uu, 5);
-          release(buf);
-        }
-      }
-    }
-  } else if (warp >= 8) {
-    // ===== producers =====
-    const int group = (warp - 8) >> 2;            // 0 or 1
-    const int tid_g = threadIdx.x - 256 - group * 128;
-    const int sub = tid_g & 3;                    // which float4 of the 16-wide K-step
-    const int rg = tid_g >> 2;                    // 0..31; rows rg + 32*i
-    const uint32_t sts_off = (sub >> 1) * kALbo + (sub & 1) * 8;
-    const bool gather_mode = !kLN && n_pre > 0;
-    // With an image-fed A operand both groups gather (alternating chunks, one buffer
-    // each); otherwise group 0 produces A and group 1 gathers.
-    if (gather_mode && (a_is_img || group == 1)) {
-      // ----- pre-activation addend producer -----
-      // Thread (rp, cgp): rows rp + 16*p (p < 8), 16-byte column group cgp of each 32-column
-      // chunk: 8 lanes read one 128-byte line segment of a gathered row.
-      const int cgp = tid_g & 7, rp = tid_g >> 3;
-      uint32_t gc = 0;
-      // Columns this CTA finishes: its own 256-wide block when N-split, else all n.
-      const int gcol_lo = nsplit ? static_cast<int>(crank) * kUnitN : 0;
-      const int gcol_hi = nsplit ? gcol_lo + kUnitN : n;
-      for (uint32_t base = tile_first; base < static_cast<uint32_t>(num_tiles); base += tile_stride) {
-        const long long trow0 = static_cast<long long>(base + tile_off) * kTileM;
-        const float* p0[8];
-        const float* p1[8];
+      const bool tile_ok = tile < static_cast<uint32_t>(num_tiles);
+      const long long grow0 = static_cast<long long>(tile) * kTileM + lr0;
+      for (int uh = 0; uh < units_per_tile; ++uh, ++u) {
+        const int h_blk = nsplit ? static_cast<int>(crank) : uh;
+        const int col_base = h_blk * kUnitN;
+        const int ncols = min(kUnitN, n_valid - col_base);
+        if (lead && eg == 0) trace(u, 0);
+        mma_unit<kSplit, Cfg::kStages, Cfg::kStageBytes, Cfg::kAStageBytes>(
+            acc, stage_base, full_bar, empty_bar, stage, phase, ksteps, eg * 64 * 16, rel_mask);
+        if (lead && eg == 0) trace(u, 3);
+        float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
+        if (kLN) {
+          float shift[2], s1[2], s2[2];
+          row_shifted_sums(acc, s_bias + col_base, ncols, shift, s1, s2);
+          if (nsplit) {
+            // LayerNorm over a row whose two halves live in the two CTAs of the cluster: each
+            // CTA computes (mean, M2) of its 256 columns, hands them to the partner through
+            // distributed shared memory, and both combine them (Chan's parallel update).
+            const uint32_t lb = ln_count & 1, par = (ln_count >> 1) & 1;
+            uint64_t* bar = &lnx_bar[eg * 2 + lb];
+            const uint32_t peer = crank ^ 1u;
+            float mh[2], m2h[2];
 #pragma unroll
-        for (int p = 0; p < 8; ++p) {
-          const long long grow = trow0 + rp + 16 * p;
-          p0[p] = nullptr; p1[p] = nullptr;
-          if (grow < rows_total) {
-            const PreAddInfo a = s_pre[0];
-            p0[p] = a.table + (a.idx ? static_cast<long long>(__ldg(a.idx + grow)) : grow) * a.ld + cgp * 4;
-            if (n_pre > 1) {
-              const PreAddInfo b = s_pre[1];
-              p1[p] = b.table + (b.idx ? static_cast<long long>(__ldg(b.idx + grow)) : grow) * b.ld + cgp * 4;
+            for (int h = 0; h < 2; ++h) {
+              mh[h] = shift[h] + s1[h] * (1.0f / kUnitN);
+              m2h[h] = fmaxf(s2[h] - s1[h] * s1[h] * (1.0f / kUnitN), 0.f);
+              if (q == 0)
+                ptx::st_async_f32x2(ptx::mapa(ptx::smem_addr(&s_lnx[lb * kTileM + lr0 + 8 * h]), peer),
+                                    mh[h], m2h[h], ptx::mapa(ptx::smem_addr(bar), peer));
+            }
+            if (lead) ptx::mbar_arrive_expect_tx(bar, 64 * 8);
+            ptx::mbar_wait(bar, par);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float2 other = s_lnx[lb * kTileM + lr0 + 8 * h];
+              const float delta = other.x - mh[h];
+              mean[h] = 0.5f * (mh[h] + other.x);
+              const float var = (m2h[h] + other.y + delta * delta * (0.5f * kUnitN)) * (1.0f / (2 * kUnitN));
+              rstd[h] = rsqrtf(var + 1e-5f);
+            }
+            ++ln_count;
+          } else {
+            const float inv_n = 1.0f / static_cast<float>(ncols);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float m1 = s1[h] * inv_n;
+              mean[h] = shift[h] + m1;
+              rstd[h] = rsqrtf(fmaxf(s2[h] * inv_n - m1 * m1, 0.f) + 1e-5f);
             }
           }
+          if (lead && eg == 0) trace(u, 4);
         }
-        for (int c0 = gcol_lo; c0 < gcol_hi; c0 += 32, ++gc) {
-          const uint32_t gb = gc & 1;
-          if (a_is_img && gb != static_cast<uint32_t>(group)) continue;
-          float4 acc[8];
+        // Epilogue, 32 columns (j0 .. j0 + 3) at a time; unrolled so that the accumulator is
+        // only ever indexed with constants (it must stay in registers).
 #pragma unroll
-          for (int p = 0; p < 8; ++p)
-            acc[p] = p0[p] ? __ldg(reinterpret_cast<const float4*>(p0[p] + c0)) : make_float4(0.f, 0.f, 0.f, 0.f);
-          if (n_pre > 1) {
+        for (int c0 = 0; c0 < kUnitN; c0 += 32) {
+          if (c0 >= ncols) continue;
+          const int j0 = c0 >> 3;
+          if (gather_mode) {
+            // Add the gathered node projections staged by the producer warps.
+            const uint32_t gb = g_count & 1;
+            ptx::mbar_wait(&g_full_bar[gb], (g_count >> 1) & 1);
+            add_staged_chunk(acc, j0, s_g + gb * kGBufFloats, lr0);
+            __syncwarp();
+            if (lane == 0) ptx::mbar_arrive(&g_empty_bar[gb]);
+            ++g_count;
+          }
 #pragma unroll
-            for (int p = 0; p < 8; ++p) {
-              if (p1[p]) {
-                const float4 t = __ldg(reinterpret_cast<const float4*>(p1[p] + c0));
-                acc[p].x += t.x; acc[p].y += t.y; acc[p].z += t.z; acc[p].w += t.w;
+          for (int jj = 0; jj < 4; ++jj) {
+            const int c = c0 + 8 * jj + 2 * q;                 // unit column of this pair
+            const int gc = col_base + c;
+            const float2 b = *reinterpret_cast<const float2*>(s_bias + gc);
+            float2 sc = make_float2(1.f, 1.f), of = make_float2(0.f, 0.f);
+            if (kLN) {
+              sc = *reinterpret_cast<const float2*>(s_scale + gc);
+              of = *reinterpret_cast<const float2*>(s_offset + gc);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float* v = &acc[4 * (j0 + jj) + 2 * h];
+              v[0] += b.x; v[1] += b.y;
+              if (kSwish) { v[0] = swish_f(v[0]); v[1] = swish_f(v[1]); }
+              if (kLN) {
+                v[0] = (v[0] - mean[h]) * rstd[h] * sc.x + of.x;
+                v[1] = (v[1] - mean[h]) * rstd[h] * sc.y + of.y;
+              }
+              const long long grow = grow0 + 8 * h;
+              const bool row_ok = grow < rows_total;
+              float2 y = make_float2(v[0], v[1]);
+              float2 r = make_float2(0.f, 0.f);
+              if (res_ptr != nullptr && row_ok) {
+                if (c + 1 < ncols) r = *reinterpret_cast<const float2*>(res_ptr + grow * ld_res + gc);
+                else if (c < ncols) r.x = res_ptr[grow * ld_res + gc];
+              }
+              if (row_ok && c < ncols) {
+                if (c + 1 < ncols) {
+                  if (outy_ptr != nullptr) *reinterpret_cast<float2*>(outy_ptr + grow * ld_outy + gc) = y;
+                  if (out_ptr != nullptr)
+                    *reinterpret_cast<float2*>(out_ptr + grow * ld_out + gc) = make_float2(y.x + r.x, y.y + r.y);
+                } else {
+                  if (outy_ptr != nullptr) outy_ptr[grow * ld_outy + gc] = y.x;
+                  if (out_ptr != nullptr) out_ptr[grow * ld_out + gc] = y.x + r.x;
+                }
+              }
+              if (out_img != nullptr && tile_ok) {
+                // Operand image of this tile for a later layer (n = n_valid = 512): the four
+                // threads of a row complete one 16-byte piece, eight rows a 128-byte line.
+                if (img_res) { y.x += r.x; y.y += r.y; }
+                uint32_t hi, lo;
+                ptx::split_bf16x2(y.x, y.y, hi, lo);
+                uint8_t* dst = out_img + static_cast<size_t>(tile) * (n >> 4) * GCB_A_IMAGE_BLOCK +
+                               image_offset(gc, lr0 + 8 * h);
+                *reinterpret_cast<uint32_t*>(dst) = hi;
+                *reinterpret_cast<uint32_t*>(dst + kAPartBytes) = lo;
               }
             }
           }
-          ptx::mbar_wait(&g_empty_bar[gb], ((gc >> 1) & 1) ^ 1);
-          float* gdst = s_g + gb * kGBufFloats + rp * kEpiRowFloats + cgp * 4;
-#pragma unroll
-          for (int p = 0; p < 8; ++p)
-            *reinterpret_cast<float4*>(gdst + 16 * p * kEpiRowFloats) = acc[p];
-          __syncwarp();
-          if (lane == 0) ptx::mbar_arrive(&g_full_bar[gb]);
         }
+        if (lead && eg == 0) trace(u, 5);
       }
-    } else if (!a_is_img) {
-      // ----- activation (A operand) producer -----
-      uint32_t it = 0;
-      for (uint32_t base = tile_first; base < static_cast<uint32_t>(num_tiles); base += tile_stride) {
-        const uint32_t tile = base + tile_off;       // may be past the end: all-zero dummy tile
-        // Source row of each of my 4 tile rows, per segment (-1 = out of range).
-        long long src[3][4];
+    }
+  } else if (warp >= 4 - kProducerWarps) {
+    // ===== producers (warps 2-3) =====
+    const int t64 = threadIdx.x - 32 * (4 - kProducerWarps);
+    const int sub = t64 & 3;                      // which float4 of the 16-wide K-step
+    const int rg = t64 >> 2;                      // 0..15; rows rg + 16*i
+    const uint32_t sts_off = (sub >> 1) * kALbo + (sub & 1) * 8;
+    uint32_t it = 0, gc = 0;
+    for (uint32_t base = tile_first; base < static_cast<uint32_t>(num_tiles); base += tile_stride) {
+      const uint32_t tile = base + tile_off;       // may be past the end: all-zero dummy tile
+      for (int uh = 0; uh < units_per_tile; ++uh) {
+        if (!a_is_img) {
+          // ----- activation (A operand) producer -----
+          // Source row of each of my 8 tile rows, per segment (-1 = out of range).
+          int src[3][8];
 #pragma unroll
-        for (int s = 0; s < 3; ++s) {
+          for (int s = 0; s < 3; ++s) {
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            src[s][i] = -1;
-            if (s < nseg) {
-              const long long grow = static_cast<long long>(tile) * kTileM + rg + 32 * i;
-              const int32_t* ip = s_seg[s].idx;
-              if (grow < rows_total) src[s][i] = ip ? static_cast<long long>(__ldg(ip + grow)) : grow;
+            for (int i = 0; i < 8; ++i) {
+              src[s][i] = -1;
+              if (s < nseg) {
+                const long long grow = static_cast<long long>(tile) * kTileM + rg + 16 * i;
+                const int32_t* ip = s_seg[s].idx;
+                if (grow < rows_total) src[s][i] = ip ? __ldg(ip + grow) : static_cast<int>(grow);
+              }
             }
           }
-        }
-        for (int uh = 0; uh < units_per_tile; ++uh) {
-          float4 cur[4];
+          float4 cur[8];
           bool have_cur = false, cur_img = false;
           uint32_t cur_it = 0;
-          // Software pipeline over the K-steps this group owns: the loads of the next
-          // owned K-step are in flight while the current one is converted and stored.
+          // Software pipeline over the K-steps: the loads of the next K-step are in flight
+          // while the current one is converted and stored.
           for (int ks = 0; ks <= ksteps; ++ks) {
             const uint32_t this_it = it + ks;
-            // Normal mode: the two groups alternate K-steps.  Gather mode: group 0 owns all.
-            const bool mine = (ks < ksteps) && (gather_mode || (this_it & 1u) == static_cast<uint32_t>(group));
-            float4 nxt[4];
+            const bool mine = ks < ksteps;
+            float4 nxt[8];
             const bool img_step = mine && ks_info[ks].is_img;   // TMA brings the data: arrive only
             if (mine && !img_step) {
               const int s = ks_info[ks].seg;
@@ -766,31 +635,31 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
               const SegInfo sg = s_seg[s];
               const bool kvalid = koff < sg.k_valid;
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-                const long long sr = (s == 0) ? src[0][i] : (s == 1 ? src[1][i] : src[2][i]);
+              for (int i = 0; i < 8; ++i) {
+                float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+                const int sr = (s == 0) ? src[0][i] : (s == 1 ? src[1][i] : src[2][i]);
                 if (kvalid && sr >= 0) {
-                  const float* p = sg.table + sr * sg.fan * sg.ld + koff;
-                  acc = __ldg(reinterpret_cast<const float4*>(p));
+                  const float* p = sg.table + static_cast<long long>(sr) * sg.fan * sg.ld + koff;
+                  a = __ldg(reinterpret_cast<const float4*>(p));
                   for (int j = 1; j < sg.fan; ++j) {
                     const float4 t = __ldg(reinterpret_cast<const float4*>(p + static_cast<long long>(j) * sg.ld));
-                    acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
+                    a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
                   }
                 }
-                nxt[i] = acc;
+                nxt[i] = a;
               }
             }
-            if (have_cur && (mine || ks == ksteps)) {
+            if (have_cur) {
               const uint32_t stage = cur_it % Cfg::kStages;
               const uint32_t phase = (cur_it / Cfg::kStages) & 1;
               ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
               uint8_t* a_hi = stage_base + stage * Cfg::kStageBytes;
               if (!cur_img) {
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
+                for (int i = 0; i < 8; ++i) {
                   uint2 hi, lo;
                   ptx::split_bf16x4(cur[i], hi, lo);
-                  const uint32_t off = sts_off + (rg + 32 * i) * 16;
+                  const uint32_t off = sts_off + (rg + 16 * i) * 16;
                   *reinterpret_cast<uint2*>(a_hi + off) = hi;
                   if (kSplit) *reinterpret_cast<uint2*>(a_hi + kAPartBytes + off) = lo;
                 }
@@ -802,13 +671,18 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
             }
             if (mine) {
 #pragma unroll
-              for (int i = 0; i < 4; ++i) cur[i] = nxt[i];
+              for (int i = 0; i < 8; ++i) cur[i] = nxt[i];
               cur_it = this_it;
               cur_img = img_step;
               have_cur = true;
             }
           }
           it += ksteps;
+        }
+        if (gather_mode) {
+          const int gcol_lo = (nsplit ? static_cast<int>(crank) : uh) * kUnitN;
+          gc = stage_addends(s_g, g_full_bar, g_empty_bar, s_pre, n_pre,
+                             static_cast<long long>(tile) * kTileM, rows_total, gcol_lo, gc, t64);
         }
       }
     }
@@ -817,13 +691,8 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
   // ---- teardown ---------------------------------------------------------------
   // No CTA may exit while a peer can still multicast into its shared memory or arrive
   // on its barriers.
-  ptx::tc_fence_before_sync();
   __syncthreads();
   ptx::cluster_sync_all();
-  if (warp == 2) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 }  // namespace gcb

@@ -1,7 +1,6 @@
-// Thin inline-PTX wrappers for the sm_100a features the MLP kernel uses:
-// mbarrier, 1-D bulk async copy (TMA engine, SASS UBLKCP), tcgen05 MMA / TMEM.
-// Descriptor bit layouts follow the PTX ISA tcgen05 "shared memory descriptor"
-// and "instruction descriptor" tables.
+// Thin inline-PTX wrappers for the sm_90a features the MLP kernels use:
+// mbarrier, 1-D bulk async copy (TMA engine), thread-block clusters and wgmma.
+// Descriptor bit layouts follow the PTX ISA wgmma "matrix descriptor" table.
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
@@ -82,7 +81,7 @@ __device__ __forceinline__ void mbar_spin(uint64_t* bar, uint32_t parity) {
 
 // ---- proxies / fences ---------------------------------------------------------
 // Make generic-proxy shared-memory writes (st.shared) visible to the async
-// proxy (tcgen05.mma operand reads, bulk copies).
+// proxy (wgmma operand reads, bulk copies).
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -90,12 +89,6 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 // (cp.async.bulk reads through the async proxy) that are ordered after this thread.
 __device__ __forceinline__ void fence_proxy_async_global() {
   asm volatile("fence.proxy.async.global;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ---- bulk async copy global -> shared (TMA engine, no tensor map) ------------
@@ -117,10 +110,8 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
-__device__ __forceinline__ void st_global_v4_hint(void* ptr, const uint4& v, uint64_t policy) {
-  asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(ptr), "r"(v.x),
-               "r"(v.y), "r"(v.z), "r"(v.w), "l"(policy)
-               : "memory");
+__device__ __forceinline__ void st_global_b32_hint(void* ptr, uint32_t v, uint64_t policy) {
+  asm volatile("st.global.L2::cache_hint.b32 [%0], %1, %2;" ::"l"(ptr), "r"(v), "l"(policy) : "memory");
 }
 // bulk copy global -> shared, multicast, with an L2 cache policy for the source lines
 __device__ __forceinline__ void bulk_g2s_multicast_hint(void* smem_dst, const void* gmem_src,
@@ -229,108 +220,79 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
   }
 }
 
-// ---- TMEM ---------------------------------------------------------------------
-// Whole-warp, .sync.aligned.  Writes the allocated base address to smem.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_addr(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp gets row
-// (lane base + i), registers j = columns (col base + j).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// ---- tcgen05.mma ------------------------------------------------------------------
+// ---- wgmma ---------------------------------------------------------------------
 // Shared-memory matrix descriptor, K-major operand, no swizzle ("interleave"):
 // the operand is a grid of core matrices, each 8 rows x 16 bytes stored as 128
 // contiguous bytes;  SBO = byte distance between core matrices adjacent along
 // M/N (next 8 rows),  LBO = byte distance between core matrices adjacent along
 // K (next 16 bytes of K).  Fields are in units of 16 bytes.
 //   [0,14)  start address >> 4      [16,30) LBO >> 4      [32,46) SBO >> 4
-//   [46,48) version = 1 (sm_100)    [61,64) layout type = 0 (no swizzle)
+//   [49,52) base offset = 0         [62,64) layout type = 0 (no swizzle)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes,
                                                    uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
   return d;
 }
 
-// Instruction descriptor for kind::f16: bf16 x bf16 -> f32, A and B K-major.
-//   [4,6) D format: 1 = f32     [7,10) A format: 1 = bf16   [10,13) B format: 1 = bf16
-//   [15] A major: 0 = K         [16] B major: 0 = K
-//   [17,23) N >> 3              [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t m, uint32_t n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
+// The accumulator of a 64 x 256 fp32 tile, owned by one warpgroup: thread t of warp w holds
+// d[4j + 2h + e] = D[16w + t/4 + 8h][8j + 2(t%4) + e]  (j < 32, h, e < 2).
+// D (+)= A[smem] * B[smem]^T for one K-step of 16, issued by the whole warpgroup.
+__device__ __forceinline__ void wgmma_bf16_m64n256(float (&d)[128], uint64_t a_desc, uint64_t b_desc,
+                                                   uint32_t scale_d) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+        "}, %128, %129, p, 1, 1, 0, 0;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),
+          "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+          "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]),
+          "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]),
+          "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),
+          "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]),
+          "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]),
+          "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]),
+          "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]),
+          "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]),
+          "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]),
+          "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]),
+          "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]),
+          "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
-
-// D[tmem] (+)= A[smem] * B[smem]^T, issued by ONE thread.
-__device__ __forceinline__ void mma_bf16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}"
-      ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-
-// Arrive on an mbarrier when all previously issued MMAs of this thread are done
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::
-                   "r"(smem_addr(bar))
-               : "memory");
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-
-// Same, arriving on the barrier at the same CTA-relative offset in every CTA of cta_mask.
-__device__ __forceinline__ void mma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;" ::"r"(smem_addr(bar)),
-      "h"(cta_mask)
-      : "memory");
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
-
-// ---- warpgroup register re-allocation -----------------------------------------------
-// All four warps of a warpgroup (warps 4k..4k+3) must execute the same setmaxnreg.
-template <int kRegs>
-__device__ __forceinline__ void setmaxnreg_inc() {
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs));
-}
-template <int kRegs>
-__device__ __forceinline__ void setmaxnreg_dec() {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs));
+// Keeps the compiler from moving accesses of the accumulator across wgmma issue / wait.
+__device__ __forceinline__ void fence_regs(float (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // ---- misc ---------------------------------------------------------------------
@@ -359,6 +321,16 @@ __device__ __forceinline__ void split_bf16x4(const float4& x, uint2& hi, uint2& 
   hi.y = *reinterpret_cast<uint32_t*>(&h23);
   lo.x = *reinterpret_cast<uint32_t*>(&l01);
   lo.y = *reinterpret_cast<uint32_t*>(&l23);
+}
+
+// Same for two floats (two adjacent columns): one packed 32-bit word each for hi and lo,
+// the first float in the low half.
+__device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  const float2 f = __bfloat1622float2(h);
+  __nv_bfloat162 l = __floats2bfloat162_rn(a - f.x, b - f.y);
+  hi = *reinterpret_cast<uint32_t*>(&h);
+  lo = *reinterpret_cast<uint32_t*>(&l);
 }
 
 }  // namespace ptx

@@ -16,7 +16,7 @@ runs in libgraphcast_b200.so.  HBM layout (fp32 unless noted):
              is consumed as an identity-row A operand: grid_in, grid_lat, mesh_lat,
              mesh_agg, mesh_edge, the embedded bipartite edges, the summed m2g messages
   grid_out   [Ng, 256]          decoder output (n_out valid columns)
-  weights    per linear layer: bf16 hi|lo tile image (tcgen05 B operand) + fp32 copy
+  weights    per linear layer: bf16 hi|lo tile image (wgmma B operand) + fp32 copy
 """
 
 from __future__ import annotations

@@ -9,7 +9,7 @@ Same public surface as `weathernext/weathernext1_graph/graphcast.py`:
 What differs is only *how* the step is computed: the three GNN calls
 (`_run_grid2mesh_gnn` :550, `_run_mesh_gnn` :606, `_run_mesh2grid_gnn` :641) and
 the channel (un)packing (`_inputs_to_grid_node_features` :680,
-`_grid_node_outputs_to_prediction` :701) run as hand-written sm_100a kernels
+`_grid_node_outputs_to_prediction` :701) run as hand-written sm_90a kernels
 behind the C ABI in include/graphcast_b200.h.  There is no CPU path: without a
 CUDA device or the built library this module raises.
 
@@ -115,7 +115,7 @@ class FusedNormalization:
 
 
 class GraphCast(Predictor):
-  """GraphCast predictor running on one B200."""
+  """GraphCast predictor running on one H100."""
 
   def __init__(self, model_config: ModelConfig, task_config: TaskConfig, *,
                params: Optional[Mapping[str, Mapping[str, np.ndarray]]] = None,
@@ -124,9 +124,9 @@ class GraphCast(Predictor):
                image_residual: bool = True, deep_chains: bool = True):
     if model_config.latent_size != engine_lib.LATENT:
       raise ValueError(f"latent_size {model_config.latent_size} is not supported by the "
-                       f"sm_100a kernels (only {engine_lib.LATENT})")
+                       f"sm_90a kernels (only {engine_lib.LATENT})")
     if model_config.hidden_layers != 1:
-      raise ValueError("only hidden_layers=1 is supported by the sm_100a kernels")
+      raise ValueError("only hidden_layers=1 is supported by the sm_90a kernels")
     self._model_config = model_config
     self._task_config = task_config
     self._precision = precision

@@ -8,7 +8,7 @@ Semantics kept:
   prediction       = y * std + mean                   for targets not in inputs
   only single-step targets are supported (ValueError otherwise, :114-117).
 
-When the wrapped predictor is the B200 `GraphCast`, the affine maps are not
+When the wrapped predictor is this package's `GraphCast`, the affine maps are not
 applied to the Datasets at all: they are folded into per-channel vectors and
 executed inside the pack / unpack kernels (`gcb_pack_grid_features`,
 `gcb_unpack_grid_outputs`), which removes three full passes over the 0.25 degree

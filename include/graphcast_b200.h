@@ -1,9 +1,9 @@
-/* graphcast_b200 -- C ABI of the B200-native GraphCast hot path.
+/* graphcast_b200 -- C ABI of the H100-native GraphCast hot path.
  *
  * This is the drop-in boundary: a plain C interface (pointers and sizes, no
- * torch / C++ types) over hand-written sm_100a CUDA kernels.  The reference is
+ * torch / C++ types) over hand-written sm_90a CUDA kernels.  The reference is
  * pure Python/JAX and has no FFI of its own; each entry point below names the
- * reference function (file:line under /root/reference) whose work it replaces.
+ * reference function (file:line in the reference, google-deepmind/graphcast) whose work it replaces.
  * The Python mirror (graphcast_b200/graphcast.py, rollout.py) binds these with
  * ctypes; INTEGRATION.md shows the stub a reference maintainer would add.
  *
@@ -37,8 +37,8 @@ typedef enum {
 
 /* Arithmetic of the dense MLP contractions.
  *   BF16X3    : every fp32 operand is split x = hi + lo (two bf16), the product is
- *               formed as hi*hi + hi*lo + lo*hi on tcgen05 tensor cores with fp32
- *               accumulation in TMEM.  ~2^-17 relative operand error: this is the
+ *               formed as hi*hi + hi*lo + lo*hi on wgmma tensor cores with fp32
+ *               accumulation in registers.  ~2^-17 relative operand error: this is the
  *               parity mode (<= 1e-4 vs the fp32 oracle over a full step).
  *   BF16      : single bf16 product (the numerics of the reference's
  *               casting.Bfloat16Cast demo stack, utils/casting.py:31-65); fast,
@@ -212,9 +212,9 @@ int gcb_unpack_grid_outputs(const float* y, int32_t ld_y, int32_t n_out, int64_t
  * A CHAIN runs up to GCB_MAX_CHAIN fused layers over the same `rows` rows in ONE kernel: a
  * cluster pair owns a 128-row tile and takes it through layer 0, 1, ... while the intermediate
  * results stay on chip -- each layer that later layers consume writes its result (as an
- * operand image) into a small per-cluster SCRATCH ring that lives in the 126 MB L2 and is
+ * operand image) into a small per-cluster SCRATCH ring that is written with an L2 evict_last policy and is
  * streamed back by TMA as the A operand of the consumer; it is overwritten in place tile after
- * tile, so it never has to reach HBM.  This is how the two linears of every MLP of
+ * tile, so most of it is served from the L2 instead of HBM.  This is how the two linears of every MLP of
  * build_mlp_with_maybe_layer_norm (utils/legacy/deep_typed_graph_net.py:205-247) execute as one
  * launch with the [rows, 512] hidden activation never written to HBM.
  * All layers of a chain have n = n_valid = 512.  Layer results are bit-identical to running the

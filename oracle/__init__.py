@@ -3,7 +3,7 @@
 This package restates, on the CPU (numpy / torch-CPU, float32 or float64), the
 arithmetic of the reference's GraphCast single 6 h step and the host logic
 around it.  Every function cites the reference file:line it follows
-(paths relative to /root/reference).
+(paths relative to the root of the reference, google-deepmind/graphcast).
 
 Who may import it: `tests/`, `__graft_entry__.smoke()` and `bench.py`'s
 `cpu_baseline` / `--impl reference` legs -- as the checker or the reported CPU

@@ -18,7 +18,7 @@ Restates, for explicit index arrays and a Haiku-named parameter dict:
   * the three GNN calls and their glue (weathernext1_graph/graphcast.py:550-678).
 
 Third-party arithmetic restated from its published definition (packages are not
-in /root/reference; versions unpinned in its setup.py:37,43):
+in the reference; versions unpinned in its setup.py:37,43):
   hk.Linear      y = x @ w + b, w:[in,out]
   hk.nets.MLP    activation between layers, none after the last
   hk.LayerNorm   axis=-1, eps=1e-5: (x-mean)*rsqrt(var_biased+eps)*scale+offset

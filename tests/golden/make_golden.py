@@ -1,5 +1,6 @@
-"""Generates tests/golden/*.npz by IMPORTING THE REFERENCE (run in the build
-container only: PYTHONPATH=/root/reference python tests/golden/make_golden.py).
+"""Generates tests/golden/*.npz by IMPORTING THE REFERENCE (a checkout of
+google-deepmind/graphcast, `weathernext`):
+  GRAPHCAST_REFERENCE=<path of the checkout> python tests/golden/make_golden.py
 
 The reference's JAX model stack is not installable here, but
 `weathernext.utils.icosahedral_mesh` is pure numpy/scipy and imports fine; its
@@ -14,7 +15,7 @@ import sys
 
 import numpy as np
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["GRAPHCAST_REFERENCE"])
 from weathernext.utils import icosahedral_mesh as ref  # noqa: E402
 
 here = os.path.dirname(os.path.abspath(__file__))

@@ -31,11 +31,21 @@ def test_thread_candidates(bench):
   assert bench.thread_candidates(48) == [48, 32, 16]
 
 
-def test_ncu_traffic_reads_the_committed_launch_list():
+def test_ncu_traffic_reads_a_launch_list(tmp_path, monkeypatch):
   import bench
+  assert bench.ncu_traffic(bench.DEFAULT_WORKLOAD, "bf16x3") == (None, None)   # none committed
+  # A launch list in the format tools/ncu_launch_list.py writes: kernel names may contain commas.
+  (tmp_path / "profiles").mkdir()
+  (tmp_path / "profiles" / "r02_launches_ncu.csv").write_text(
+      "# one step\n"
+      "id,kernel,ms,dram_read,dram_write\n"
+      "0,gcb::mlp_chain_tc_kernel<true, true, false>(gcb_chain_desc, int, int),9.5,60e9,40e9\n"
+      "1,gcb::segment_sum_kernel<4>(const float *, int),3.2,12e9,5e9\n"
+      "2,gcb::mlp_layer_tc_kernel<true, false, true>(gcb_layer_desc),1.1,7e9,3e9\n")
+  monkeypatch.setattr(bench, "REPO", str(tmp_path))
   tc, src = bench.ncu_traffic(bench.DEFAULT_WORKLOAD, "bf16x3")
-  assert tc is not None and 100e9 < tc < 250e9           # tensor-core kernels: DRAM bytes per step
-  assert "r02_launches_ncu.csv" in src
+  assert tc == 110e9                                      # tensor-core kernels: DRAM bytes per step
+  assert "r02_launches_ncu.csv" in src and "127.0 GB" in src
   assert bench.ncu_traffic("graphcast_small_1deg_13lvl", "bf16x3") == (None, None)
 
 

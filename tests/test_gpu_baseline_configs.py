@@ -91,8 +91,8 @@ def _subgraph_decoder(g, grid_rows):
 
 
 def test_config2_quarter_degree_stagewise_matches_the_oracle():
-  if torch.cuda.get_device_properties(0).total_memory < 120e9:
-    pytest.skip("needs a 180 GB B200")
+  if torch.cuda.get_device_properties(0).total_memory < 75e9:
+    pytest.skip("needs an 80 GB GPU")
   _threads()
   task = graphcast.TASK
   g, params, c_in, n_out = _setup(0.25, 6, task)

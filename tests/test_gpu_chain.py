@@ -145,7 +145,7 @@ def _release_tensors():
 def test_two_layer_mlp_chain_is_bit_identical_to_two_layer_launches(prec, tol, lag, kind):
   lib = _native.lib()
   g = torch.Generator().manual_seed(5)
-  rows = 128 * 330 + 77            # > 4 tiles per cluster on 74 clusters, ragged last tile
+  rows = 128 * 330 + 77            # > 4 tiles per cluster on 66 clusters, ragged last tile
   n_nodes = 5000
   f = lambda *shape: torch.randn(*shape, generator=g)
   nan = lambda: torch.full((rows, 512), float("nan"), device=DEV)

@@ -13,7 +13,7 @@ fp64 oracle (the parity metric of tests/ and bench.py).
           x2a = two products, activations rounded to bf16 a_hi*(w_hi+w_lo)
           x3  = the product's parity mode (drops only a_lo*w_lo), for scale
 
-  python tests/tools/precision_budget.py --workload sample_2deg_13lvl [--out profiles/r02_precision_budget.md]
+  python tests/tools/precision_budget.py --workload sample_2deg_13lvl [--out precision_budget.md]
 """
 import argparse
 import os

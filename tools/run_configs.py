@@ -1,4 +1,4 @@
-"""Measures the BASELINE.json configs beyond the headline bench (run on a B200 box):
+"""Measures the BASELINE.json configs beyond the headline bench (run on an H100):
 rollout (config 3), operational 13-level batch-of-4 (config 5), bf16 mode, 1-degree small."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -59,7 +59,7 @@ def run(rows, k, n, ln, act, csize, out_y=False, residual=False, idx=False, pre=
   torch.cuda.synchronize()
   lib.gcb_debug_trace(None)
   t = tr.cpu().numpy().reshape(64, 16)
-  ntile = min(64, (rows + 127) // 128 // 148)
+  ntile = min(64, (rows + 127) // 128 // 132)
   print(f"rows={rows} k={k} n={n} ln={ln} act={act} cluster={csize} out_y={out_y} res={residual} idx={idx} pre={pre} img_in={img_in} img_out={img_out}: {e0.elapsed_time(e1):.3f} ms; tiles/CTA~{ntile}")
   base = t[1, 0]
   for i in range(1, min(ntile, 6)):
@@ -75,11 +75,11 @@ if len(sys.argv) > 1 and sys.argv[1] == "cluster":
     for fl in (0, 2):
       print("== cluster", cs, "flags", fl)
       lib.gcb_debug_flags(fl)
-      run(148 * 128 * 160, 512, 512, False, True, cs, img_in=True, img_out=True)
-      run(148 * 128 * 160, 512, 512, True, False, cs, img_in=True)
+      run(132 * 128 * 160, 512, 512, False, True, cs, img_in=True, img_out=True)
+      run(132 * 128 * 160, 512, 512, True, False, cs, img_in=True)
   lib.gcb_debug_flags(0)
   sys.exit(0)
-rows = 148 * 128 * (160 if big else 8)
+rows = 132 * 128 * (160 if big else 8)
 if len(sys.argv) > 1 and sys.argv[1] == "flags":
   # attribution sweep: 2 no global stores | 4 N-split pair without A multicast | 16 L2 prefetch
   for fl in (0, 2, 4, 16, 2 | 4):

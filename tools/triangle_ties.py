@@ -3,7 +3,7 @@
 containing-triangle lookup (utils/legacy/grid_mesh_connectivity.py:89-134: trimesh's
 `nearest.on_surface` in the reference, `closest_face_indices` here) has to break a tie.
 
-  python tools/triangle_ties.py > profiles/r02_triangle_ties.log
+  python tools/triangle_ties.py > triangle_ties.log
 """
 import collections
 import os
