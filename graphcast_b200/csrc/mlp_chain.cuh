@@ -28,8 +28,8 @@
 //   h_full[q][slot]  count 16: the 8 consumer warps of BOTH CTAs arrive (release.cluster) after
 //                    their st.global + fence.proxy.async; the TMA warp of each CTA waits
 //                    (acquire.cluster) before the first bulk copy out of the slot.
-//   h_free[q][slot]  count 16 x consumers: every consumer warp of a consuming unit arrives in
-//                    both CTAs once its last MMA has retired, i.e. when all bulk copies out of
+//   h_free[q][slot]  count 16 x consumers: every consumer warp of a consuming unit arrives (CTA
+//                    scope) in both CTAs once its last MMA has retired, i.e. when all bulk copies out of
 //                    the slot have landed and been consumed in that CTA; the consumers wait for
 //                    it before overwriting the slot.
 #pragma once
@@ -236,70 +236,147 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
   ptx::cluster_sync_all();
 
   // ---- roles ------------------------------------------------------------------
-  if (warp == 0) {
-    // ===== TMA warp (converged; every lane polls, one elected lane issues) =====
-    const uint32_t b_bytes = Cfg::kBStageBytes;
-    const size_t b_block = 2 * kBPartBytes;
-    const size_t b_stride = 2 * b_block;                          // n = 512: two blocks per K-step
-    const uint32_t a_bytes = Cfg::kAStageBytes;
-    const uint32_t a_half = a_bytes / 2;
-    uint32_t stage = 0, phase = 0, tu = 0;
-    const uint64_t keep_policy = ptx::l2_policy_evict_last();
-    for (int st = 0; st < nsteps; ++st) {
-      for (int li = 0; li < L; ++li) {
-        const int l = desc ? L - 1 - li : li;
-        const int ti = st - l * lag;
-        if (ti < 0 || ti >= T) continue;
-        const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
-        const int nseg = s_layer[l].nseg;
-        const uint8_t* b_ptr = s_layer[l].w + static_cast<size_t>(crank) * b_block;
-        const bool tr = tracing(tu);
-        long long blocked = 0, hwait = 0;
-        for (int s = 0; s < nseg; ++s) {
-          const ChainSeg sg = s_seg[l * 3 + s];
-          const uint8_t* a_ptr = nullptr;
-          bool a_copy = false;
-          const bool a_scratch = sg.src_q >= 0;
-          if (sg.src_q >= 0) {
-            const long long w0 = tr ? clock64() : 0;
-            // Poll at CTA scope (a cluster-scope acquire per retry is far more expensive), then
-            // take the cluster-scope acquire once on the completed phase.
-            ptx::mbar_wait(&h_full_bar[sg.src_q * kChainSlotsMax + (ti % nslots)],
-                           static_cast<uint32_t>(ti / nslots) & 1u);
-            ptx::mbar_wait_cluster(&h_full_bar[sg.src_q * kChainSlotsMax + (ti % nslots)],
-                                   static_cast<uint32_t>(ti / nslots) & 1u);
-            if (tr) hwait += clock64() - w0;
-            a_ptr = scratch_slot(sg.src_q, ti) + crank * a_half;
-            a_copy = true;
-          } else if (sg.img != nullptr) {
-            a_ptr = sg.img + static_cast<size_t>(tile) * sg.ksteps * GCB_A_IMAGE_BLOCK + crank * a_half;
-            a_copy = true;
-          }
-          const uint32_t tx = b_bytes + (a_copy ? a_bytes : 0u);
-          for (int k = 0; k < sg.ksteps; ++k) {
-            const long long w0 = tr ? clock64() : 0;
-            ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-            if (tr) blocked += clock64() - w0;
-            uint8_t* a_dst = stage_base + stage * Cfg::kStageBytes;
-            if (ptx::elect_one()) {
-              ptx::mbar_arrive_expect_tx(&full_bar[stage], tx);
-              if (a_scratch)
-                ptx::bulk_g2s_multicast_hint(a_dst + crank * a_half, a_ptr, a_half, &full_bar[stage], cmask, keep_policy);
-              else if (a_copy)
-                ptx::bulk_g2s_multicast(a_dst + crank * a_half, a_ptr, a_half, &full_bar[stage], cmask);
-              ptx::bulk_g2s(a_dst + Cfg::kAStageBytes, b_ptr, b_bytes, &full_bar[stage]);
+  if (warp < 4) {
+    ptx::setmaxnreg_dec<kChainProducerRegs>();       // whole warpgroup 0, before its warps split up
+    if (warp == 0) {
+      // ===== TMA warp (converged; every lane polls, one elected lane issues) =====
+      const uint32_t b_bytes = Cfg::kBStageBytes;
+      const size_t b_block = 2 * kBPartBytes;
+      const size_t b_stride = 2 * b_block;                          // n = 512: two blocks per K-step
+      const uint32_t a_bytes = Cfg::kAStageBytes;
+      const uint32_t a_half = a_bytes / 2;
+      uint32_t stage = 0, phase = 0, tu = 0;
+      const uint64_t keep_policy = ptx::l2_policy_evict_last();
+      for (int st = 0; st < nsteps; ++st) {
+        for (int li = 0; li < L; ++li) {
+          const int l = desc ? L - 1 - li : li;
+          const int ti = st - l * lag;
+          if (ti < 0 || ti >= T) continue;
+          const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
+          const int nseg = s_layer[l].nseg;
+          const uint8_t* b_ptr = s_layer[l].w + static_cast<size_t>(crank) * b_block;
+          const bool tr = tracing(tu);
+          long long blocked = 0, hwait = 0;
+          for (int s = 0; s < nseg; ++s) {
+            const ChainSeg sg = s_seg[l * 3 + s];
+            const uint8_t* a_ptr = nullptr;
+            bool a_copy = false;
+            const bool a_scratch = sg.src_q >= 0;
+            if (sg.src_q >= 0) {
+              const long long w0 = tr ? clock64() : 0;
+              // Poll at CTA scope (a cluster-scope acquire per retry is far more expensive), then
+              // take the cluster-scope acquire once on the completed phase.
+              ptx::mbar_wait(&h_full_bar[sg.src_q * kChainSlotsMax + (ti % nslots)],
+                             static_cast<uint32_t>(ti / nslots) & 1u);
+              ptx::mbar_wait_cluster(&h_full_bar[sg.src_q * kChainSlotsMax + (ti % nslots)],
+                                     static_cast<uint32_t>(ti / nslots) & 1u);
+              if (tr) hwait += clock64() - w0;
+              a_ptr = scratch_slot(sg.src_q, ti) + crank * a_half;
+              a_copy = true;
+            } else if (sg.img != nullptr) {
+              a_ptr = sg.img + static_cast<size_t>(tile) * sg.ksteps * GCB_A_IMAGE_BLOCK + crank * a_half;
+              a_copy = true;
             }
-            __syncwarp();
-            a_ptr += GCB_A_IMAGE_BLOCK;
-            b_ptr += b_stride;
-            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+            const uint32_t tx = b_bytes + (a_copy ? a_bytes : 0u);
+            for (int k = 0; k < sg.ksteps; ++k) {
+              const long long w0 = tr ? clock64() : 0;
+              ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+              if (tr) blocked += clock64() - w0;
+              uint8_t* a_dst = stage_base + stage * Cfg::kStageBytes;
+              if (ptx::elect_one()) {
+                ptx::mbar_arrive_expect_tx(&full_bar[stage], tx);
+                if (a_scratch)
+                  ptx::bulk_g2s_multicast_hint(a_dst + crank * a_half, a_ptr, a_half, &full_bar[stage], cmask, keep_policy);
+                else if (a_copy)
+                  ptx::bulk_g2s_multicast(a_dst + crank * a_half, a_ptr, a_half, &full_bar[stage], cmask);
+                ptx::bulk_g2s(a_dst + Cfg::kAStageBytes, b_ptr, b_bytes, &full_bar[stage]);
+              }
+              __syncwarp();
+              a_ptr += GCB_A_IMAGE_BLOCK;
+              b_ptr += b_stride;
+              if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+            }
           }
+          if (lane == 0) { trace_val(tu, 7, blocked); trace_val(tu, 8, hwait); trace_val(tu, 11, l); }
+          ++tu;
         }
-        if (lane == 0) { trace_val(tu, 7, blocked); trace_val(tu, 8, hwait); trace_val(tu, 11, l); }
-        ++tu;
+      }
+    } else if (warp >= 4 - kProducerWarps) {
+      // ===== producers (warps 2-3): fp32-table segments, then gathered addends, unit by unit =====
+      // A table segment is gathered through its index (optional fan-in sum), split to bf16 hi / lo
+      // and stored in the K-major core-matrix layout.  The producers arrive on EVERY K-step's full
+      // barrier when some layer has a table segment (for image / scratch K-steps without writing
+      // anything), so the barrier count is uniform.
+      const int t64 = threadIdx.x - 32 * (4 - kProducerWarps);
+      const int sub = t64 & 3;                        // which float4 of the 16-wide K-step
+      const int rg = t64 >> 2;                        // 0..15; rows rg + 16*i
+      const uint32_t sts_off = (sub >> 1) * kALbo + (sub & 1) * 8;
+      uint32_t stage = 0, phase = 0, gc = 0;
+      for (int st = 0; st < nsteps; ++st) {
+        for (int li = 0; li < L; ++li) {
+          const int l = desc ? L - 1 - li : li;
+          const int ti = st - l * lag;
+          if (ti < 0 || ti >= T) continue;
+          const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
+          const int nseg = s_layer[l].nseg;
+          for (int s = 0; any_table && s < nseg; ++s) {
+            const ChainSeg sg = s_seg[l * 3 + s];
+            const bool is_tab = sg.src_q < 0 && sg.img == nullptr;
+            int src[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              src[i] = -1;
+              if (is_tab) {
+                const long long grow = static_cast<long long>(tile) * kTileM + rg + 16 * i;
+                if (grow < rows_total) src[i] = sg.idx ? __ldg(sg.idx + grow) : static_cast<int>(grow);
+              }
+            }
+            for (int k = 0; k < sg.ksteps; ++k) {
+              float4 cur[8];
+              if (is_tab) {
+                const int koff = k * kKStep + sub * 4;
+                const bool kvalid = koff < sg.k_valid;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+                  if (kvalid && src[i] >= 0) {
+                    const float* p = sg.table + static_cast<long long>(src[i]) * sg.fan * sg.ld + koff;
+                    a = __ldg(reinterpret_cast<const float4*>(p));
+                    for (int j = 1; j < sg.fan; ++j) {
+                      const float4 t = __ldg(reinterpret_cast<const float4*>(p + static_cast<long long>(j) * sg.ld));
+                      a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
+                    }
+                  }
+                  cur[i] = a;
+                }
+              }
+              ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+              if (is_tab) {
+                uint8_t* a_hi = stage_base + stage * Cfg::kStageBytes;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                  uint2 hi, lo;
+                  ptx::split_bf16x4(cur[i], hi, lo);
+                  const uint32_t off = sts_off + (rg + 16 * i) * 16;
+                  *reinterpret_cast<uint2*>(a_hi + off) = hi;
+                  if (kSplit) *reinterpret_cast<uint2*>(a_hi + kAPartBytes + off) = lo;
+                }
+                ptx::fence_proxy_async_smem();
+              }
+              __syncwarp();
+              if (lane == 0) ptx::mbar_arrive(&full_bar[stage]);
+              if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+            }
+          }
+          if (kPre && s_layer[l].n_pre > 0 && s_layer[l].kind < kKindLN)
+            gc = stage_addends(s_g, g_full_bar, g_empty_bar, s_pre + l * 2, s_layer[l].n_pre,
+                               static_cast<long long>(tile) * kTileM, rows_total,
+                               static_cast<int>(crank) * kUnitN, gc, t64);
+        }
       }
     }
-  } else if (warp >= 4) {
+  } else {
+    ptx::setmaxnreg_inc<consumer_regs(kChainProducerRegs)>();
     // ===== consumers: MMA + epilogue =====
     const int eg = (warp - 4) >> 2;                // warpgroup: tile rows [64 eg, 64 eg + 64)
     const int q = lane & 3;
@@ -351,23 +428,27 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         }
         const int keep_q = cl.keep_q;
         uint8_t* img1 = nullptr;
+        if (lead && eg == 0) trace(u, 0);
         if (keep_q >= 0) {
           // previous readers of this slot (tile ti - nslots) are done in both CTAs
           ptx::mbar_wait(&h_free_bar[keep_q * kChainSlotsMax + (ti % nslots)],
                          (static_cast<uint32_t>(ti / nslots) & 1u) ^ 1u);
           img1 = scratch_slot(keep_q, ti);
         }
-        if (lead && eg == 0) trace(u, 0);
+        if (lead && eg == 0) { trace(u, 2); trace_val(u, 9, cl.ksteps); }
         mma_unit<kSplit, Cfg::kStages, Cfg::kStageBytes, Cfg::kAStageBytes>(
-            acc, stage_base, full_bar, empty_bar, stage, phase, cl.ksteps, eg * 64 * 16, cmask);
+            acc, stage_base, full_bar, empty_bar, stage, phase, cl.ksteps, eg * 64 * 16, cmask, u);
         if (lane == 0) {
           // Every scratch slot this unit read is reusable (in both CTAs) once these MMAs retired.
+          // The slot's readers are bulk copies that have completed (their bytes were counted on
+          // full barriers this warp passed); the next writers wait on h_free first.  So, as for
+          // the stage release in mma_unit, a CTA-scope arrive suffices.
           for (int s = 0; s < cl.nseg; ++s) {
             const int sq = s_seg[l * 3 + s].src_q;
             if (sq >= 0) {
               const uint32_t a = ptx::smem_addr(&h_free_bar[sq * kChainSlotsMax + (ti % nslots)]);
-              ptx::mbar_arrive_remote(ptx::mapa(a, 0));
-              ptx::mbar_arrive_remote(ptx::mapa(a, 1));
+              ptx::mbar_arrive_remote_cta(ptx::mapa(a, 0));
+              ptx::mbar_arrive_remote_cta(ptx::mapa(a, 1));
             }
           }
         }
@@ -486,80 +567,8 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
             ptx::mbar_arrive_remote(ptx::mapa(ptx::smem_addr(hb), peer));
           }
         }
+        if (lead && eg == 0) trace(u, 6);
         ++u;
-      }
-    }
-  } else if (warp >= 4 - kProducerWarps) {
-    // ===== producers (warps 2-3): fp32-table segments, then gathered addends, unit by unit =====
-    // A table segment is gathered through its index (optional fan-in sum), split to bf16 hi / lo
-    // and stored in the K-major core-matrix layout.  The producers arrive on EVERY K-step's full
-    // barrier when some layer has a table segment (for image / scratch K-steps without writing
-    // anything), so the barrier count is uniform.
-    const int t64 = threadIdx.x - 32 * (4 - kProducerWarps);
-    const int sub = t64 & 3;                        // which float4 of the 16-wide K-step
-    const int rg = t64 >> 2;                        // 0..15; rows rg + 16*i
-    const uint32_t sts_off = (sub >> 1) * kALbo + (sub & 1) * 8;
-    uint32_t stage = 0, phase = 0, gc = 0;
-    for (int st = 0; st < nsteps; ++st) {
-      for (int li = 0; li < L; ++li) {
-        const int l = desc ? L - 1 - li : li;
-        const int ti = st - l * lag;
-        if (ti < 0 || ti >= T) continue;
-        const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
-        const int nseg = s_layer[l].nseg;
-        for (int s = 0; any_table && s < nseg; ++s) {
-          const ChainSeg sg = s_seg[l * 3 + s];
-          const bool is_tab = sg.src_q < 0 && sg.img == nullptr;
-          int src[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            src[i] = -1;
-            if (is_tab) {
-              const long long grow = static_cast<long long>(tile) * kTileM + rg + 16 * i;
-              if (grow < rows_total) src[i] = sg.idx ? __ldg(sg.idx + grow) : static_cast<int>(grow);
-            }
-          }
-          for (int k = 0; k < sg.ksteps; ++k) {
-            float4 cur[8];
-            if (is_tab) {
-              const int koff = k * kKStep + sub * 4;
-              const bool kvalid = koff < sg.k_valid;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (kvalid && src[i] >= 0) {
-                  const float* p = sg.table + static_cast<long long>(src[i]) * sg.fan * sg.ld + koff;
-                  a = __ldg(reinterpret_cast<const float4*>(p));
-                  for (int j = 1; j < sg.fan; ++j) {
-                    const float4 t = __ldg(reinterpret_cast<const float4*>(p + static_cast<long long>(j) * sg.ld));
-                    a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
-                  }
-                }
-                cur[i] = a;
-              }
-            }
-            ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-            if (is_tab) {
-              uint8_t* a_hi = stage_base + stage * Cfg::kStageBytes;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                uint2 hi, lo;
-                ptx::split_bf16x4(cur[i], hi, lo);
-                const uint32_t off = sts_off + (rg + 16 * i) * 16;
-                *reinterpret_cast<uint2*>(a_hi + off) = hi;
-                if (kSplit) *reinterpret_cast<uint2*>(a_hi + kAPartBytes + off) = lo;
-              }
-              ptx::fence_proxy_async_smem();
-            }
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&full_bar[stage]);
-            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-          }
-        }
-        if (kPre && s_layer[l].n_pre > 0 && s_layer[l].kind < kKindLN)
-          gc = stage_addends(s_g, g_full_bar, g_empty_bar, s_pre + l * 2, s_layer[l].n_pre,
-                             static_cast<long long>(tile) * kTileM, rows_total,
-                             static_cast<int>(crank) * kUnitN, gc, t64);
       }
     }
   }

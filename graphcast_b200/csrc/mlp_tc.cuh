@@ -81,6 +81,22 @@ struct TcConfig {
   static_assert(kStages >= 4, "operand ring too shallow");
 };
 
+// Register split between warpgroup 0 (TMA, idle and producer warps) and the two consumer
+// warpgroups.  __launch_bounds__(kThreads, 1) gives every warp kLaunchRegs (65536 / 384, rounded
+// down to a multiple of 8); warpgroup 0 hands registers back so that the consumers, which hold a
+// 128-register accumulator through the epilogue, can run it without spilling:
+// 128 * producer registers + 256 * consumer registers <= 384 * kLaunchRegs.  The splits were
+// picked from ptxas spill counts and H100 step times: the layer kernel's producers keep 24
+// source rows and two K-steps of A in flight and need 120 (consumers 192); the chain kernel
+// runs faster at 56 / 224 than at 88 / 208 although its addend staging then spills.
+constexpr int kLaunchRegs = 168;
+constexpr int kLayerProducerRegs = 120;
+constexpr int kChainProducerRegs = 56;
+__host__ __device__ constexpr int consumer_regs(int producer_regs) { return (3 * kLaunchRegs - producer_regs) / 2 / 8 * 8; }
+static_assert(kLayerProducerRegs % 8 == 0 && kLayerProducerRegs >= 24 && consumer_regs(kLayerProducerRegs) <= 256 &&
+              kChainProducerRegs % 8 == 0 && kChainProducerRegs >= 24 && consumer_regs(kChainProducerRegs) <= 256,
+              "setmaxnreg takes a multiple of 8 in [24, 256]");
+
 __device__ __forceinline__ float swish_f(float x) {
   // x * sigmoid(x) = x / (1 + 2^(-x*log2 e)): one ex2.approx and one rcp.approx,
   // branch-free (~2 ulp), so 32 independent elements pipeline through the SFU.
@@ -88,7 +104,12 @@ __device__ __forceinline__ float swish_f(float x) {
 }
 
 // Optional timeline trace (debug): when non-null, CTA 0 records clock64() at a few
-// points of each of its first kTraceTiles units; see gcb_debug_trace in api.cu.
+// points of each of its first kTraceTiles units; see gcb_debug_trace in api.cu.  Events of a
+// unit (clock64 stamps of consumer warp 4 unless a count):
+//   0 unit start  1 first full barrier passed  2 h_free passed (chain)  3 MMAs retired
+//   4 LayerNorm statistics combined  5 epilogue stored  6 hand-over done (chain)
+//   7 cycles the TMA warp waited on empty barriers  8 cycles it waited on h_full (chain)
+//   9 K-steps  11 layer (chain)
 constexpr int kTraceTiles = 64;
 constexpr int kTraceEvents = 16;
 __device__ long long* g_trace = nullptr;
@@ -133,11 +154,18 @@ struct PreAddInfo {
 // The MMAs of one unit for this warpgroup's 64 rows (A rows start a_row_off bytes into the
 // stage).  After each K-step the previous one is retired and its stage released: one arrival
 // per warp, on the local barrier (rel_mask == 0) or on the barrier of every CTA in rel_mask.
+// `unit` only indexes the timeline trace (event 1: first full barrier passed).
 template <bool kSplit, int kStages, int kStageBytes, int kAStageBytes>
 __device__ __forceinline__ void mma_unit(float (&acc)[128], uint8_t* stage_base, uint64_t* full_bar,
                                          uint64_t* empty_bar, uint32_t& stage, uint32_t& phase,
-                                         int ksteps, uint32_t a_row_off, uint32_t rel_mask) {
+                                         int ksteps, uint32_t a_row_off, uint32_t rel_mask, uint32_t unit) {
   const bool lead = (threadIdx.x & 31) == 0;
+  // The stage's readers are this warpgroup's wgmma operand fetches (async proxy), retired by
+  // the wgmma.wait_group before the call; its next writers are TMA bulk copies and producer
+  // st.shared, both issued by a thread that has observed the empty barrier.  This warp made no
+  // generic-proxy writes the writers must see, so the arrive needs no release beyond CTA scope.
+  // A release.cluster arrive would put MEMBAR.ALL.GPU in front of every arrive, i.e. stall the
+  // warpgroup's next wgmma per K-step, right after an epilogue until all its stores are acked.
   auto release = [&](uint32_t s) {
     if (!lead) return;
     if (rel_mask == 0) {
@@ -145,12 +173,13 @@ __device__ __forceinline__ void mma_unit(float (&acc)[128], uint8_t* stage_base,
     } else {
       const uint32_t a = ptx::smem_addr(&empty_bar[s]);
       for (uint32_t r = 0; r < 4; ++r)
-        if ((rel_mask >> r) & 1u) ptx::mbar_arrive_remote(ptx::mapa(a, r));
+        if ((rel_mask >> r) & 1u) ptx::mbar_arrive_remote_cta(ptx::mapa(a, r));
     }
   };
   uint32_t prev = 0;
   for (int ks = 0; ks < ksteps; ++ks) {
     ptx::mbar_wait(&full_bar[stage], phase);
+    if (ks == 0 && threadIdx.x == 4 * 32) trace(unit, 1);      // operands of the unit arrived
     const uint32_t sa = ptx::smem_addr(stage_base + stage * kStageBytes);
     const uint64_t a_hi = ptx::make_smem_desc(sa + a_row_off, kALbo, 128);
     const uint64_t b_hi = ptx::make_smem_desc(sa + kAStageBytes, kBLbo, 128);
@@ -396,69 +425,166 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
   ptx::cluster_sync_all();          // barrier inits visible cluster-wide before remote arrives
 
   // ---- roles ------------------------------------------------------------------
-  if (warp == 0) {
-    // ===== TMA warp =====
-    // Converged warp, every lane polls, ONE elected lane issues.  The loop body is kept
-    // minimal - running pointers, ring counters, one SegInfo read per segment.
-    const uint32_t b_bytes = Cfg::kBStageBytes;                 // hi (| lo) of a 256-row block
-    const size_t b_block = 2 * kBPartBytes;                     // image always holds hi|lo
-    const size_t b_stride = static_cast<size_t>(n_halves) * b_block;   // next K-step, same half
-    const uint32_t slice = b_bytes / csize;
-    const uint32_t a_bytes = Cfg::kAStageBytes;                 // hi (| lo) block of one K-step
-    const uint32_t a_half = a_bytes / 2;
-    const bool b_own = (csize == 1) || nsplit;                  // my own weight block, no multicast
-    const uint8_t* wimg = static_cast<const uint8_t*>(d.w_packed);
-    uint32_t stage = 0, phase = 0, tu = 0;
-    for (uint32_t base = tile_first; base < static_cast<uint32_t>(num_tiles); base += tile_stride) {
-      const uint32_t tile = base + tile_off;
-      const bool tile_ok = tile < static_cast<uint32_t>(num_tiles);   // else: dummy tile
-      for (int uh = 0; uh < units_per_tile; ++uh, ++tu) {
-        const int h = nsplit ? static_cast<int>(crank) : uh;          // my 256-column block
-        const uint8_t* b_ptr = wimg + static_cast<size_t>(h) * b_block + (b_own ? 0u : crank * slice);
-        const bool tr = tracing(tu);
-        long long blocked = 0;
-        for (int s = 0; s < nseg; ++s) {
-          const SegInfo sg = s_seg[s];
-          const bool a_copy = tile_ok && sg.img != nullptr;
-          // Same tile in both CTAs of an N-split pair: each fetches half of every block and
-          // multicasts it to both.
-          const uint8_t* a_ptr = sg.img + static_cast<size_t>(tile) * sg.ksteps * GCB_A_IMAGE_BLOCK +
-                                 (nsplit && !decouple ? crank * a_half : 0u);
-          const uint32_t tx = b_bytes + (a_copy ? a_bytes : 0u);
-          // (experiment, debug flag 16) L2 prefetch of the same block of my next tile
-          const bool pf_next = (dbg & 16) && uh == units_per_tile - 1 &&
-                               tile + tile_stride < static_cast<uint32_t>(num_tiles);
-          const size_t pf_off = static_cast<size_t>(tile_stride) * sg.ksteps * GCB_A_IMAGE_BLOCK;
-          for (int k = 0; k < sg.ksteps; ++k) {
-            const long long w0 = tr ? clock64() : 0;
-            ptx::mbar_wait(&empty_bar[stage], phase ^ 1);   // free in every CTA of the cluster
-            if (tr) blocked += clock64() - w0;
-            uint8_t* a_dst = stage_base + stage * Cfg::kStageBytes;
-            if (ptx::elect_one()) {
-              ptx::mbar_arrive_expect_tx(&full_bar[stage], tx);
-              if (pf_next && a_copy) ptx::bulk_prefetch_l2(a_ptr + pf_off, nsplit ? a_half : a_bytes);
-              if (a_copy) {
-                if (nsplit && !decouple) ptx::bulk_g2s_multicast(a_dst + crank * a_half, a_ptr, a_half, &full_bar[stage], cmask);
-                else ptx::bulk_g2s(a_dst, a_ptr, a_bytes, &full_bar[stage]);
+  if (warp < 4) {
+    ptx::setmaxnreg_dec<kLayerProducerRegs>();       // whole warpgroup 0, before its warps split up
+    if (warp == 0) {
+      // ===== TMA warp =====
+      // Converged warp, every lane polls, ONE elected lane issues.  The loop body is kept
+      // minimal - running pointers, ring counters, one SegInfo read per segment.
+      const uint32_t b_bytes = Cfg::kBStageBytes;                 // hi (| lo) of a 256-row block
+      const size_t b_block = 2 * kBPartBytes;                     // image always holds hi|lo
+      const size_t b_stride = static_cast<size_t>(n_halves) * b_block;   // next K-step, same half
+      const uint32_t slice = b_bytes / csize;
+      const uint32_t a_bytes = Cfg::kAStageBytes;                 // hi (| lo) block of one K-step
+      const uint32_t a_half = a_bytes / 2;
+      const bool b_own = (csize == 1) || nsplit;                  // my own weight block, no multicast
+      const uint8_t* wimg = static_cast<const uint8_t*>(d.w_packed);
+      uint32_t stage = 0, phase = 0, tu = 0;
+      for (uint32_t base = tile_first; base < static_cast<uint32_t>(num_tiles); base += tile_stride) {
+        const uint32_t tile = base + tile_off;
+        const bool tile_ok = tile < static_cast<uint32_t>(num_tiles);   // else: dummy tile
+        for (int uh = 0; uh < units_per_tile; ++uh, ++tu) {
+          const int h = nsplit ? static_cast<int>(crank) : uh;          // my 256-column block
+          const uint8_t* b_ptr = wimg + static_cast<size_t>(h) * b_block + (b_own ? 0u : crank * slice);
+          const bool tr = tracing(tu);
+          long long blocked = 0;
+          for (int s = 0; s < nseg; ++s) {
+            const SegInfo sg = s_seg[s];
+            const bool a_copy = tile_ok && sg.img != nullptr;
+            // Same tile in both CTAs of an N-split pair: each fetches half of every block and
+            // multicasts it to both.
+            const uint8_t* a_ptr = sg.img + static_cast<size_t>(tile) * sg.ksteps * GCB_A_IMAGE_BLOCK +
+                                   (nsplit && !decouple ? crank * a_half : 0u);
+            const uint32_t tx = b_bytes + (a_copy ? a_bytes : 0u);
+            // (experiment, debug flag 16) L2 prefetch of the same block of my next tile
+            const bool pf_next = (dbg & 16) && uh == units_per_tile - 1 &&
+                                 tile + tile_stride < static_cast<uint32_t>(num_tiles);
+            const size_t pf_off = static_cast<size_t>(tile_stride) * sg.ksteps * GCB_A_IMAGE_BLOCK;
+            for (int k = 0; k < sg.ksteps; ++k) {
+              const long long w0 = tr ? clock64() : 0;
+              ptx::mbar_wait(&empty_bar[stage], phase ^ 1);   // free in every CTA of the cluster
+              if (tr) blocked += clock64() - w0;
+              uint8_t* a_dst = stage_base + stage * Cfg::kStageBytes;
+              if (ptx::elect_one()) {
+                ptx::mbar_arrive_expect_tx(&full_bar[stage], tx);
+                if (pf_next && a_copy) ptx::bulk_prefetch_l2(a_ptr + pf_off, nsplit ? a_half : a_bytes);
+                if (a_copy) {
+                  if (nsplit && !decouple) ptx::bulk_g2s_multicast(a_dst + crank * a_half, a_ptr, a_half, &full_bar[stage], cmask);
+                  else ptx::bulk_g2s(a_dst, a_ptr, a_bytes, &full_bar[stage]);
+                }
+                if (b_own) {
+                  ptx::bulk_g2s(a_dst + Cfg::kAStageBytes, b_ptr, b_bytes, &full_bar[stage]);
+                } else {
+                  // Same block in every CTA: each fetches 1/csize and multicasts it to all.
+                  ptx::bulk_g2s_multicast(a_dst + Cfg::kAStageBytes + crank * slice, b_ptr, slice,
+                                          &full_bar[stage], cmask);
+                }
               }
-              if (b_own) {
-                ptx::bulk_g2s(a_dst + Cfg::kAStageBytes, b_ptr, b_bytes, &full_bar[stage]);
-              } else {
-                // Same block in every CTA: each fetches 1/csize and multicasts it to all.
-                ptx::bulk_g2s_multicast(a_dst + Cfg::kAStageBytes + crank * slice, b_ptr, slice,
-                                        &full_bar[stage], cmask);
+              __syncwarp();
+              a_ptr += GCB_A_IMAGE_BLOCK;
+              b_ptr += b_stride;
+              if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+            }
+          }
+          if (lane == 0) trace_val(tu, 7, blocked);
+        }
+      }
+    } else if (warp >= 4 - kProducerWarps) {
+      // ===== producers (warps 2-3) =====
+      const int t64 = threadIdx.x - 32 * (4 - kProducerWarps);
+      const int sub = t64 & 3;                      // which float4 of the 16-wide K-step
+      const int rg = t64 >> 2;                      // 0..15; rows rg + 16*i
+      const uint32_t sts_off = (sub >> 1) * kALbo + (sub & 1) * 8;
+      uint32_t it = 0, gc = 0;
+      for (uint32_t base = tile_first; base < static_cast<uint32_t>(num_tiles); base += tile_stride) {
+        const uint32_t tile = base + tile_off;       // may be past the end: all-zero dummy tile
+        for (int uh = 0; uh < units_per_tile; ++uh) {
+          if (!a_is_img) {
+            // ----- activation (A operand) producer -----
+            // Source row of each of my 8 tile rows, per segment (-1 = out of range).
+            int src[3][8];
+#pragma unroll
+            for (int s = 0; s < 3; ++s) {
+#pragma unroll
+              for (int i = 0; i < 8; ++i) {
+                src[s][i] = -1;
+                if (s < nseg) {
+                  const long long grow = static_cast<long long>(tile) * kTileM + rg + 16 * i;
+                  const int32_t* ip = s_seg[s].idx;
+                  if (grow < rows_total) src[s][i] = ip ? __ldg(ip + grow) : static_cast<int>(grow);
+                }
               }
             }
-            __syncwarp();
-            a_ptr += GCB_A_IMAGE_BLOCK;
-            b_ptr += b_stride;
-            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+            float4 cur[8];
+            bool have_cur = false, cur_img = false;
+            uint32_t cur_it = 0;
+            // Software pipeline over the K-steps: the loads of the next K-step are in flight
+            // while the current one is converted and stored.
+            for (int ks = 0; ks <= ksteps; ++ks) {
+              const uint32_t this_it = it + ks;
+              const bool mine = ks < ksteps;
+              float4 nxt[8];
+              const bool img_step = mine && ks_info[ks].is_img;   // TMA brings the data: arrive only
+              if (mine && !img_step) {
+                const int s = ks_info[ks].seg;
+                const int koff = ks_info[ks].koff + sub * 4;
+                const SegInfo sg = s_seg[s];
+                const bool kvalid = koff < sg.k_valid;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+                  const int sr = (s == 0) ? src[0][i] : (s == 1 ? src[1][i] : src[2][i]);
+                  if (kvalid && sr >= 0) {
+                    const float* p = sg.table + static_cast<long long>(sr) * sg.fan * sg.ld + koff;
+                    a = __ldg(reinterpret_cast<const float4*>(p));
+                    for (int j = 1; j < sg.fan; ++j) {
+                      const float4 t = __ldg(reinterpret_cast<const float4*>(p + static_cast<long long>(j) * sg.ld));
+                      a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
+                    }
+                  }
+                  nxt[i] = a;
+                }
+              }
+              if (have_cur) {
+                const uint32_t stage = cur_it % Cfg::kStages;
+                const uint32_t phase = (cur_it / Cfg::kStages) & 1;
+                ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+                uint8_t* a_hi = stage_base + stage * Cfg::kStageBytes;
+                if (!cur_img) {
+#pragma unroll
+                  for (int i = 0; i < 8; ++i) {
+                    uint2 hi, lo;
+                    ptx::split_bf16x4(cur[i], hi, lo);
+                    const uint32_t off = sts_off + (rg + 16 * i) * 16;
+                    *reinterpret_cast<uint2*>(a_hi + off) = hi;
+                    if (kSplit) *reinterpret_cast<uint2*>(a_hi + kAPartBytes + off) = lo;
+                  }
+                }
+                ptx::fence_proxy_async_smem();
+                __syncwarp();
+                if (lane == 0) ptx::mbar_arrive(&full_bar[stage]);
+                have_cur = false;
+              }
+              if (mine) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) cur[i] = nxt[i];
+                cur_it = this_it;
+                cur_img = img_step;
+                have_cur = true;
+              }
+            }
+            it += ksteps;
+          }
+          if (gather_mode) {
+            const int gcol_lo = (nsplit ? static_cast<int>(crank) : uh) * kUnitN;
+            gc = stage_addends(s_g, g_full_bar, g_empty_bar, s_pre, n_pre,
+                               static_cast<long long>(tile) * kTileM, rows_total, gcol_lo, gc, t64);
           }
         }
-        if (lane == 0) trace_val(tu, 7, blocked);
       }
     }
-  } else if (warp >= 4) {
+  } else {
+    ptx::setmaxnreg_inc<consumer_regs(kLayerProducerRegs)>();
     // ===== consumers: MMA + epilogue =====
     const int eg = (warp - 4) >> 2;                // warpgroup: tile rows [64 eg, 64 eg + 64)
     const int q = lane & 3;
@@ -480,8 +606,8 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
         const int ncols = min(kUnitN, n_valid - col_base);
         if (lead && eg == 0) trace(u, 0);
         mma_unit<kSplit, Cfg::kStages, Cfg::kStageBytes, Cfg::kAStageBytes>(
-            acc, stage_base, full_bar, empty_bar, stage, phase, ksteps, eg * 64 * 16, rel_mask);
-        if (lead && eg == 0) trace(u, 3);
+            acc, stage_base, full_bar, empty_bar, stage, phase, ksteps, eg * 64 * 16, rel_mask, u);
+        if (lead && eg == 0) { trace(u, 3); trace_val(u, 9, ksteps); }
         float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
         if (kLN) {
           float shift[2], s1[2], s2[2];
@@ -591,99 +717,6 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
           }
         }
         if (lead && eg == 0) trace(u, 5);
-      }
-    }
-  } else if (warp >= 4 - kProducerWarps) {
-    // ===== producers (warps 2-3) =====
-    const int t64 = threadIdx.x - 32 * (4 - kProducerWarps);
-    const int sub = t64 & 3;                      // which float4 of the 16-wide K-step
-    const int rg = t64 >> 2;                      // 0..15; rows rg + 16*i
-    const uint32_t sts_off = (sub >> 1) * kALbo + (sub & 1) * 8;
-    uint32_t it = 0, gc = 0;
-    for (uint32_t base = tile_first; base < static_cast<uint32_t>(num_tiles); base += tile_stride) {
-      const uint32_t tile = base + tile_off;       // may be past the end: all-zero dummy tile
-      for (int uh = 0; uh < units_per_tile; ++uh) {
-        if (!a_is_img) {
-          // ----- activation (A operand) producer -----
-          // Source row of each of my 8 tile rows, per segment (-1 = out of range).
-          int src[3][8];
-#pragma unroll
-          for (int s = 0; s < 3; ++s) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              src[s][i] = -1;
-              if (s < nseg) {
-                const long long grow = static_cast<long long>(tile) * kTileM + rg + 16 * i;
-                const int32_t* ip = s_seg[s].idx;
-                if (grow < rows_total) src[s][i] = ip ? __ldg(ip + grow) : static_cast<int>(grow);
-              }
-            }
-          }
-          float4 cur[8];
-          bool have_cur = false, cur_img = false;
-          uint32_t cur_it = 0;
-          // Software pipeline over the K-steps: the loads of the next K-step are in flight
-          // while the current one is converted and stored.
-          for (int ks = 0; ks <= ksteps; ++ks) {
-            const uint32_t this_it = it + ks;
-            const bool mine = ks < ksteps;
-            float4 nxt[8];
-            const bool img_step = mine && ks_info[ks].is_img;   // TMA brings the data: arrive only
-            if (mine && !img_step) {
-              const int s = ks_info[ks].seg;
-              const int koff = ks_info[ks].koff + sub * 4;
-              const SegInfo sg = s_seg[s];
-              const bool kvalid = koff < sg.k_valid;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-                const int sr = (s == 0) ? src[0][i] : (s == 1 ? src[1][i] : src[2][i]);
-                if (kvalid && sr >= 0) {
-                  const float* p = sg.table + static_cast<long long>(sr) * sg.fan * sg.ld + koff;
-                  a = __ldg(reinterpret_cast<const float4*>(p));
-                  for (int j = 1; j < sg.fan; ++j) {
-                    const float4 t = __ldg(reinterpret_cast<const float4*>(p + static_cast<long long>(j) * sg.ld));
-                    a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
-                  }
-                }
-                nxt[i] = a;
-              }
-            }
-            if (have_cur) {
-              const uint32_t stage = cur_it % Cfg::kStages;
-              const uint32_t phase = (cur_it / Cfg::kStages) & 1;
-              ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-              uint8_t* a_hi = stage_base + stage * Cfg::kStageBytes;
-              if (!cur_img) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  uint2 hi, lo;
-                  ptx::split_bf16x4(cur[i], hi, lo);
-                  const uint32_t off = sts_off + (rg + 16 * i) * 16;
-                  *reinterpret_cast<uint2*>(a_hi + off) = hi;
-                  if (kSplit) *reinterpret_cast<uint2*>(a_hi + kAPartBytes + off) = lo;
-                }
-              }
-              ptx::fence_proxy_async_smem();
-              __syncwarp();
-              if (lane == 0) ptx::mbar_arrive(&full_bar[stage]);
-              have_cur = false;
-            }
-            if (mine) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) cur[i] = nxt[i];
-              cur_it = this_it;
-              cur_img = img_step;
-              have_cur = true;
-            }
-          }
-          it += ksteps;
-        }
-        if (gather_mode) {
-          const int gcol_lo = (nsplit ? static_cast<int>(crank) : uh) * kUnitN;
-          gc = stage_addends(s_g, g_full_bar, g_empty_bar, s_pre, n_pre,
-                             static_cast<long long>(tile) * kTileM, rows_total, gcol_lo, gc, t64);
-        }
       }
     }
   }

@@ -181,8 +181,9 @@ __device__ __forceinline__ void st_cluster_f32x2(uint32_t raddr, float a, float 
 }
 // Asynchronous 8-byte store into another CTA's shared memory that signals that CTA's
 // mbarrier (complete_tx, 8 bytes) when the data is visible there.  No release fence in the
-// sender: a per-thread `mbarrier.arrive.release.cluster` drains the thread's outstanding
-// global stores first (ERRBAR + MEMBAR: 11 % of the LayerNorm epilogue's time in ncu).
+// sender: the alternative, st.shared::cluster followed by `mbarrier.arrive.release.cluster`
+// (mbar_arrive_remote), compiles to MEMBAR.ALL.GPU, which first waits until every global
+// store the thread has outstanding is acknowledged.
 __device__ __forceinline__ void st_async_f32x2(uint32_t raddr, float a, float b, uint32_t rbar) {
   asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];"
                ::"r"(raddr), "f"(a), "f"(b), "r"(rbar) : "memory");
@@ -192,9 +193,18 @@ __device__ __forceinline__ void st_async_f32x2(uint32_t raddr, float a, float b,
 __device__ __forceinline__ void mbar_arrive_release_cluster(uint64_t* bar) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
 }
-// Arrive (release at cluster scope) on an mbarrier of another CTA of the cluster.
+// Arrive (release at cluster scope) on an mbarrier of another CTA of the cluster.  Compiles
+// to MEMBAR.ALL.CTA + MEMBAR.ALL.GPU before the arrive: for hand-overs of generic-proxy
+// writes only.
 __device__ __forceinline__ void mbar_arrive_remote(uint32_t raddr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
+}
+// Arrive (default semantics: release at CTA scope) on an mbarrier of another CTA of the
+// cluster: a bare SYNCS.ARRIVE, no memory fence.  Enough to free a buffer whose readers were
+// async-proxy operations that have already completed (retired wgmma, landed bulk copies) and
+// whose next writer is a bulk copy or a thread that first observes the barrier.
+__device__ __forceinline__ void mbar_arrive_remote_cta(uint32_t raddr) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
 }
 // Wait with acquire at cluster scope (pairs with mbar_arrive_remote).
 __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
@@ -293,6 +303,17 @@ __device__ __forceinline__ void wgmma_wait() {
 __device__ __forceinline__ void fence_regs(float (&d)[128]) {
 #pragma unroll
   for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// ---- register reallocation between warpgroups ---------------------------------------
+// Every warp of a warpgroup must execute the same one; kRegs is a multiple of 8 in [24, 256].
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs));
+}
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs));
 }
 
 // ---- misc ---------------------------------------------------------------------

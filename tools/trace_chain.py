@@ -5,7 +5,8 @@
 For an edge-MLP-shaped problem (image A operand + two gathered addends -> swish -> LN + residual,
 fp32 + image outputs) and a node-MLP-shaped one it prints: NaN diagnostics, bitwise equality of
 the two paths, CUDA-event times, and the in-kernel timeline of cluster 0 / CTA 0 of the chain
-launch (cycles; per executed unit: MMA issue, epilogue, barrier waits)."""
+launch (cycles; per executed unit: barrier waits, MMA phase per K-step against the 768-cycle
+tensor-pipe ideal, LayerNorm statistics, epilogue stores, scratch hand-over)."""
 import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
@@ -91,14 +92,32 @@ def case(kind):
   lib.gcb_debug_trace(tr.data_ptr())
   fused(); torch.cuda.synchronize()
   lib.gcb_debug_trace(None)
-  t = tr.cpu().numpy().reshape(64, 16)
+  print_timeline(tr.cpu().numpy().reshape(64, 16))
+
+
+IDEAL_KSTEP = 768   # tensor cycles per K-step and CTA: 6 x m64n256k16 (bf16x3, 2 warpgroups) at 128
+
+
+def print_timeline(t):
+  """Events: see the trace comment in graphcast_b200/csrc/mlp_tc.cuh.  Cycles after the previous
+  event of the same unit; per K-step = MMA phase (first full barrier -> MMAs retired) / K-steps."""
   base = t[2, 0]
-  print("   u L | mma: start  ops_ready  issue_done (starved) | epi: start(after mma)  stats  stored  handed | tma: blocked  h_full_wait | epi h_free_wait")
+  print("   u L | start  h_free  ops_ready  mma (per K-step / ideal) | ln_stats  stored  handed | next unit"
+        " | tma: blocked h_full_wait")
+  tot = np.zeros(6)
   for u in range(2, 14):
     r = t[u]
-    print(f"  {u:2d} {r[11]} | {r[0]-base:8d} +{r[1]-r[0]:6d} +{r[2]-r[1]:6d} ({r[6]:6d}) | +{r[3]-r[2]:6d} +{max(r[4]-r[3],0):6d} "
-          f"+{r[5]-max(r[4],r[3]):6d} +{r[10]-r[5]:6d} | {r[7]:6d} {r[8]:6d} | {r[9]:6d}   next unit starts +{t[u+1,0]-r[0]:6d}"
-          f" | epi phases: tmem_ld {r[12]} math {r[13]} f32out {r[14]} img {r[15]}")
+    mma = r[3] - r[1]
+    ln = r[4] - r[3] if r[4] > 0 else 0
+    stored = r[5] - max(r[4], r[3])
+    handed = r[6] - r[5]
+    nxt = t[u + 1, 0] - r[0]
+    tot += [r[2] - r[0], r[1] - r[2], mma, ln + stored + handed, nxt, r[9]]
+    print(f"  {u:2d} {r[11]} | {r[0]-base:8d} +{r[2]-r[0]:6d} +{r[1]-r[2]:6d} +{mma:7d} ({mma / max(r[9], 1):6.0f} / {IDEAL_KSTEP}) | "
+          f"+{ln:6d} +{stored:6d} +{handed:6d} | +{nxt:7d} | {r[7]:7d} {r[8]:7d}")
+  print(f"  units 2-13: h_free wait {tot[0]:.0f}, operand wait {tot[1]:.0f}, MMA {tot[2]:.0f} "
+        f"({tot[2] / tot[5]:.0f} cycles per K-step vs {IDEAL_KSTEP}), epilogue + hand-over {tot[3]:.0f}, "
+        f"unit to unit {tot[4]:.0f} cycles")
 
 
 case("edge")

@@ -5,9 +5,9 @@
   python tools/trace_layer.py flags      # attribution sweep over gcb_debug_flags (2, 4, 16)
   python tools/trace_layer.py cluster    # cluster 1 vs 2, with / without global stores
 
-Columns: cycles (clock64) of the MMA warp / epilogue of the first units, plus the cycles the MMA
-warp spent waiting on `full` barriers (mma_starved) and the TMA warp on `empty` barriers
-(tma_blocked) per unit."""
+Columns: cycles (clock64) of consumer warp 4 for the first units of CTA 0 (wait for the first
+operands, MMA phase and its cycles per K-step against the tensor-pipe ideal, LayerNorm statistics,
+epilogue stores), plus the cycles the TMA warp spent waiting on `empty` barriers (tma_blocked)."""
 import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -62,11 +62,14 @@ def run(rows, k, n, ln, act, csize, out_y=False, residual=False, idx=False, pre=
   ntile = min(64, (rows + 127) // 128 // 132)
   print(f"rows={rows} k={k} n={n} ln={ln} act={act} cluster={csize} out_y={out_y} res={residual} idx={idx} pre={pre} img_in={img_in} img_out={img_out}: {e0.elapsed_time(e1):.3f} ms; tiles/CTA~{ntile}")
   base = t[1, 0]
+  ideal = 128 * (6 if d.precision == 0 else 2)   # tensor cycles per K-step: bf16x3 | bf16, 2 warpgroups
   for i in range(1, min(ntile, 6)):
     r = t[i]
-    print(f"  tile {i}: acc_free@{r[0]-base:7d} ops_ready+{r[1]-r[0]:6d} mma_issue+{r[2]-r[1]:6d} | "
-          f"epi_start(after commit)+{r[3]-r[2]:6d} ln_stats+{r[4]-r[3]:6d} store+{r[5]-r[4]:6d} | "
-          f"next_acc_free+{t[i+1,0]-r[5]:6d}  tile_total={t[i+1,0]-r[0]} | mma_starved={r[6]} tma_blocked={r[7]}")
+    mma = r[3] - r[1]
+    ln = r[4] - r[3] if r[4] > 0 else 0
+    print(f"  unit {i}: start@{r[0]-base:8d} ops_ready+{r[1]-r[0]:6d} mma+{mma:7d} "
+          f"({mma / max(r[9], 1):5.0f}/K-step, ideal {ideal}) | ln_stats+{ln:6d} stored+{r[5]-max(r[4], r[3]):6d} | "
+          f"next unit+{t[i+1,0]-r[0]:7d} | tma_blocked={r[7]}")
 
 import sys
 big = len(sys.argv) > 1 and sys.argv[1] in ("big", "flags", "cluster")
