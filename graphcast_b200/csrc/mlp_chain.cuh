@@ -52,8 +52,7 @@ struct ChainConfig {
   static constexpr int kBStageBytes = kSplit ? 2 * kBPartBytes : kBPartBytes;
   static constexpr int kStageBytes = kAStageBytes + kBStageBytes;
   static constexpr int kParamBytes = kParamVecs * kMaxN * 4;
-  static constexpr int kGRegionBytes = kPre ? kGBytes : 0;
-  static constexpr int kFixedBytes = kParamBytes + kGRegionBytes + kLnxBytes + kChainTailBytes;
+  static constexpr int kFixedBytes = kParamBytes + kLnxBytes + kChainTailBytes;
   static constexpr int kFit = (kSmemLimit - kFixedBytes) / kStageBytes;
 #ifdef GCB_FORCE_STAGES          // experiment: sensitivity of a launch to the ring depth
   static constexpr int kStages = GCB_FORCE_STAGES < kFit ? GCB_FORCE_STAGES : kFit;
@@ -98,20 +97,17 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* stage_base = smem;
   float* s_param = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes);
-  float* s_g = s_param + Cfg::kParamBytes / 4;                      // [2][128][36] (kPre only)
-  float2* s_lnx = reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(s_g) + Cfg::kGRegionBytes);  // [2][128]
+  float2* s_lnx = reinterpret_cast<float2*>(s_param + Cfg::kParamBytes / 4);   // [2][128]
   uint8_t* tail = reinterpret_cast<uint8_t*>(s_lnx) + kLnxBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);          // [12]
   uint64_t* empty_bar = full_bar + 12;                             // [12]
-  uint64_t* g_full_bar = empty_bar + 12;                           // [2]
-  uint64_t* g_empty_bar = g_full_bar + 2;                          // [2]
-  uint64_t* lnx_bar = g_empty_bar + 2;                             // [2 warpgroups][2]
+  uint64_t* lnx_bar = empty_bar + 12;                              // [2 warpgroups][2]
   uint64_t* h_full_bar = lnx_bar + 4;                              // [GCB_MAX_CHAIN][kChainSlotsMax]
   uint64_t* h_free_bar = h_full_bar + GCB_MAX_CHAIN * kChainSlotsMax;
   ChainLayer* s_layer = reinterpret_cast<ChainLayer*>(h_free_bar + GCB_MAX_CHAIN * kChainSlotsMax);  // [4]
   ChainSeg* s_seg = reinterpret_cast<ChainSeg*>(s_layer + GCB_MAX_CHAIN);            // [4][3]
   PreAddInfo* s_pre = reinterpret_cast<PreAddInfo*>(s_seg + GCB_MAX_CHAIN * 3);      // [4][2]
-  static_assert((2 * 12 + 8 + 2 * GCB_MAX_CHAIN * kChainSlotsMax) * 8 +
+  static_assert((2 * 12 + 4 + 2 * GCB_MAX_CHAIN * kChainSlotsMax) * 8 +
                     GCB_MAX_CHAIN * (sizeof(ChainLayer) + 3 * sizeof(ChainSeg) + 2 * sizeof(PreAddInfo))
                     <= kChainTailBytes, "tail region too small");
 
@@ -217,8 +213,6 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
       ptx::mbar_init(&empty_bar[s], 2 * kConsumerWarps);                   // every consumer warp of both CTAs
     }
     for (int b = 0; b < 2; ++b) {
-      ptx::mbar_init(&g_full_bar[b], kProducerWarps);
-      ptx::mbar_init(&g_empty_bar[b], kConsumerWarps);
       ptx::mbar_init(&lnx_bar[b], 1);
       ptx::mbar_init(&lnx_bar[2 + b], 1);
     }
@@ -302,7 +296,7 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         }
       }
     } else if (warp >= 4 - kProducerWarps) {
-      // ===== producers (warps 2-3): fp32-table segments, then gathered addends, unit by unit =====
+      // ===== producers (warps 2-3): fp32-table segments, unit by unit =====
       // A table segment is gathered through its index (optional fan-in sum), split to bf16 hi / lo
       // and stored in the K-major core-matrix layout.  The producers arrive on EVERY K-step's full
       // barrier when some layer has a table segment (for image / scratch K-steps without writing
@@ -311,7 +305,7 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
       const int sub = t64 & 3;                        // which float4 of the 16-wide K-step
       const int rg = t64 >> 2;                        // 0..15; rows rg + 16*i
       const uint32_t sts_off = (sub >> 1) * kALbo + (sub & 1) * 8;
-      uint32_t stage = 0, phase = 0, gc = 0;
+      uint32_t stage = 0, phase = 0;
       for (int st = 0; st < nsteps; ++st) {
         for (int li = 0; li < L; ++li) {
           const int l = desc ? L - 1 - li : li;
@@ -368,10 +362,6 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
               if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
             }
           }
-          if (kPre && s_layer[l].n_pre > 0 && s_layer[l].kind < kKindLN)
-            gc = stage_addends(s_g, g_full_bar, g_empty_bar, s_pre + l * 2, s_layer[l].n_pre,
-                               static_cast<long long>(tile) * kTileM, rows_total,
-                               static_cast<int>(crank) * kUnitN, gc, t64);
         }
       }
     }
@@ -383,7 +373,7 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
     const int lr0 = eg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile rows lr0, lr0 + 8
     const bool lead = lane == 0 && (warp & 3) == 0;
     const int col_base = static_cast<int>(crank) * kUnitN;   // my 256 columns of every layer
-    uint32_t stage = 0, phase = 0, g_count = 0, ln_count = 0, u = 0;
+    uint32_t stage = 0, phase = 0, ln_count = 0, u = 0;
     const uint64_t keep_policy = ptx::l2_policy_evict_last();
     float acc[128];
 
@@ -426,6 +416,73 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
                                   GCB_A_IMAGE_BLOCK);
           }
         }
+        const bool is_ln = kind >= kKindLN;
+        const bool want_pre = kPre && !is_ln && cl.n_pre > 0;
+        const long long grow0 = static_cast<long long>(tile) * kTileM + lr0;
+        // Inputs of the epilogue that live in global memory - the gathered pre-activation addends
+        // (two tables, gathered through their row indices) or the residual (fp32 rows or an operand
+        // image) - are loaded into registers one 32-column chunk ahead of their use, chunk 0 before
+        // the MMAs, so that their latency hides behind the MMAs and the previous chunk.  With the
+        // loads next to the stores they were paid once per column pair: the compiler cannot move a
+        // load above a store that may alias it.  Loading ahead is safe for the in-place updates
+        // (out_img == res_img, out == residual): every word is read and then written by the same
+        // thread, and a chunk's loads touch other columns than the stores they move ahead of.
+        // buf (32 registers) holds, for i = 2 jj + h (column pair jj, row h of the chunk):
+        //   addends: buf[i] / buf[8 + i] = table a / table b of the next chunk, as float bits
+        //            (they are added to the accumulator before that chunk's loads are issued);
+        //   residual: buf[i] = fp32 pair or (hi, lo) image words of this chunk, buf[8 + i] those
+        //            of the next one.
+        const float* pre_src[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};   // [table][h], nullptr = none
+        const float* res_src[2] = {nullptr, nullptr};                            // [h]
+        if (want_pre) {
+          const PreAddInfo pa = s_pre[l * 2];
+          const PreAddInfo pb = s_pre[l * 2 + 1];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const long long grow = grow0 + 8 * h;
+            if (grow < rows_total) {
+              const int ra = pa.idx ? __ldg(pa.idx + grow) : static_cast<int>(grow);
+              pre_src[0][h] = pa.table + static_cast<long long>(ra) * pa.ld + col_base + 2 * q;
+              if (cl.n_pre > 1) {
+                const int rb = pb.idx ? __ldg(pb.idx + grow) : static_cast<int>(grow);
+                pre_src[1][h] = pb.table + static_cast<long long>(rb) * pb.ld + col_base + 2 * q;
+              }
+            }
+          }
+        } else if (res_ptr != nullptr) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            if (grow0 + 8 * h < rows_total) res_src[h] = res_ptr + (grow0 + 8 * h) * ld_res + col_base + 2 * q;
+        }
+        uint2 buf[16];
+        auto load_pre = [&](int c0) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int c = c0 + 8 * (i >> 1);
+            buf[i] = make_uint2(0u, 0u);
+            buf[8 + i] = make_uint2(0u, 0u);
+            if (pre_src[0][i & 1] != nullptr) buf[i] = __ldg(reinterpret_cast<const uint2*>(pre_src[0][i & 1] + c));
+            if (pre_src[1][i & 1] != nullptr) buf[8 + i] = __ldg(reinterpret_cast<const uint2*>(pre_src[1][i & 1] + c));
+          }
+        };
+        auto load_res = [&](int c0, int half) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int c = c0 + 8 * (i >> 1);
+            uint2 v = make_uint2(0u, 0u);
+            if (res_src[i & 1] != nullptr) {
+              v = *reinterpret_cast<const uint2*>(res_src[i & 1] + c);
+            } else if (res_img != nullptr) {
+              const size_t o = image_offset(col_base + c + 2 * q, lr0 + 8 * (i & 1));
+              v.x = *reinterpret_cast<const uint32_t*>(res_img + o);
+              v.y = *reinterpret_cast<const uint32_t*>(res_img + o + kAPartBytes);
+            }
+            buf[half + i] = v;
+          }
+        };
+        const bool has_res = res_ptr != nullptr || res_img != nullptr;
+        if (want_pre) load_pre(0);
+        else if (has_res) load_res(0, 0);
         const int keep_q = cl.keep_q;
         uint8_t* img1 = nullptr;
         if (lead && eg == 0) trace(u, 0);
@@ -453,7 +510,6 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
           }
         }
         if (lead && eg == 0) trace(u, 3);
-        const bool is_ln = kind >= kKindLN;
         float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
         if (is_ln) {
           // Each CTA computes (mean, M2) of its 256 columns of a row, hands them to the partner
@@ -484,20 +540,28 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
           ++ln_count;
           if (lead && eg == 0) trace(u, 4);
         }
-        // Epilogue, 32 columns (j0 .. j0 + 3) at a time; unrolled so that the accumulator is
-        // only ever indexed with constants (it must stay in registers).
-        const bool want_pre = kPre && !is_ln && cl.n_pre > 0;
-        const long long grow0 = static_cast<long long>(tile) * kTileM + lr0;
-#pragma unroll
+        // Epilogue, 32 columns at a time.  The loop is NOT unrolled: it runs once per unit, and
+        // unrolled over the 8 chunks its straight-line code (~150 KB) streamed through the
+        // instruction cache, which bounded the epilogue at ~100 000 cycles per unit.  To keep the
+        // accumulator indexed with constants only (it must stay in registers), every iteration
+        // works on acc[0..15] and then shifts the accumulator down by one chunk.
+#pragma unroll 1
         for (int c0 = 0; c0 < kUnitN; c0 += 32) {
-          const int j0 = c0 >> 3;
           if (want_pre) {
-            const uint32_t gb = g_count & 1;
-            ptx::mbar_wait(&g_full_bar[gb], (g_count >> 1) & 1);
-            add_staged_chunk(acc, j0, s_g + gb * kGBufFloats, lr0);
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&g_empty_bar[gb]);
-            ++g_count;
+            // a + b (b only where there is a second table), then added to the accumulator
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              float2 g = make_float2(__uint_as_float(buf[i].x), __uint_as_float(buf[i].y));
+              if (pre_src[1][i & 1] != nullptr) {
+                g.x += __uint_as_float(buf[8 + i].x);
+                g.y += __uint_as_float(buf[8 + i].y);
+              }
+              acc[4 * (i >> 1) + 2 * (i & 1)] += g.x;
+              acc[4 * (i >> 1) + 2 * (i & 1) + 1] += g.y;
+            }
+            if (c0 + 32 < kUnitN) load_pre(c0 + 32);
+          } else if (has_res && c0 + 32 < kUnitN) {
+            load_res(c0 + 32, 8);
           }
 #pragma unroll
           for (int jj = 0; jj < 4; ++jj) {
@@ -510,7 +574,8 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
             }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-              float* v = &acc[4 * (j0 + jj) + 2 * h];
+              float* v = &acc[4 * jj + 2 * h];
+              const uint2 rin = buf[2 * jj + h];                  // residual of this chunk
               const int r = lr0 + 8 * h;
               const long long grow = grow0 + 8 * h;
               const bool row_ok = grow < rows_total;
@@ -522,7 +587,7 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
               }
               // fp32 residual (rows past the end: none)
               float2 rs = make_float2(0.f, 0.f);
-              if (res_ptr != nullptr && row_ok) rs = *reinterpret_cast<const float2*>(res_ptr + grow * ld_res + gc);
+              if (res_ptr != nullptr && row_ok) rs = make_float2(__uint_as_float(rin.x), __uint_as_float(rin.y));
               if (row_ok) {
                 if (outy_ptr != nullptr) *reinterpret_cast<float2*>(outy_ptr + grow * ld_outy + gc) = y;
                 if (out_ptr != nullptr)
@@ -536,8 +601,7 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
                 if (res_img != nullptr) {
                   // Residual held as an operand image (x = hi + lo, two bf16); a packed word
                   // holds the even column in its low and the odd column in its high half.
-                  const uint32_t hw = *reinterpret_cast<const uint32_t*>(res_img + o);
-                  const uint32_t lw = *reinterpret_cast<const uint32_t*>(res_img + o + kAPartBytes);
+                  const uint32_t hw = rin.x, lw = rin.y;
                   x.x += __uint_as_float(hw << 16) + __uint_as_float(lw << 16);
                   x.y += __uint_as_float(hw & 0xffff0000u) + __uint_as_float(lw & 0xffff0000u);
                 }
@@ -553,6 +617,12 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
                 }
               }
             }
+          }
+#pragma unroll
+          for (int i = 0; i < 128 - 16; ++i) acc[i] = acc[i + 16];
+          if (!want_pre) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) buf[i] = buf[8 + i];
           }
         }
         if (lead && eg == 0) trace(u, 5);

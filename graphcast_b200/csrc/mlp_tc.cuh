@@ -88,7 +88,7 @@ struct TcConfig {
 // 128 * producer registers + 256 * consumer registers <= 384 * kLaunchRegs.  The splits were
 // picked from ptxas spill counts and H100 step times: the layer kernel's producers keep 24
 // source rows and two K-steps of A in flight and need 120 (consumers 192); the chain kernel
-// runs faster at 56 / 224 than at 88 / 208 although its addend staging then spills.
+// runs faster at 56 / 224 than at 88 / 208 (its producers only convert fp32-table segments).
 constexpr int kLaunchRegs = 168;
 constexpr int kLayerProducerRegs = 120;
 constexpr int kChainProducerRegs = 56;

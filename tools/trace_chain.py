@@ -102,22 +102,23 @@ def print_timeline(t):
   """Events: see the trace comment in graphcast_b200/csrc/mlp_tc.cuh.  Cycles after the previous
   event of the same unit; per K-step = MMA phase (first full barrier -> MMAs retired) / K-steps."""
   base = t[2, 0]
-  print("   u L | start  h_free  ops_ready  mma (per K-step / ideal) | ln_stats  stored  handed | next unit"
-        " | tma: blocked h_full_wait")
-  tot = np.zeros(6)
+  print("   u L | start  h_free  ops_ready  mma (per K-step / ideal) | ln_stats  columns  handed"
+        " | next unit | tma: blocked h_full_wait")
+  tot = np.zeros(8)
   for u in range(2, 14):
     r = t[u]
     mma = r[3] - r[1]
     ln = r[4] - r[3] if r[4] > 0 else 0
-    stored = r[5] - max(r[4], r[3])
-    handed = r[6] - r[5]
+    stored = r[5] - max(r[4], r[3])      # column loop
+    handed = r[6] - r[5]                 # last store issued -> h_full arrives done
     nxt = t[u + 1, 0] - r[0]
-    tot += [r[2] - r[0], r[1] - r[2], mma, ln + stored + handed, nxt, r[9]]
+    tot += [r[2] - r[0], r[1] - r[2], mma, ln + stored + handed, nxt, r[9], stored, handed]
     print(f"  {u:2d} {r[11]} | {r[0]-base:8d} +{r[2]-r[0]:6d} +{r[1]-r[2]:6d} +{mma:7d} ({mma / max(r[9], 1):6.0f} / {IDEAL_KSTEP}) | "
-          f"+{ln:6d} +{stored:6d} +{handed:6d} | +{nxt:7d} | {r[7]:7d} {r[8]:7d}")
+          f"+{ln:6d} +{stored:7d} +{handed:6d} | +{nxt:7d} | {r[7]:7d} {r[8]:7d}")
   print(f"  units 2-13: h_free wait {tot[0]:.0f}, operand wait {tot[1]:.0f}, MMA {tot[2]:.0f} "
         f"({tot[2] / tot[5]:.0f} cycles per K-step vs {IDEAL_KSTEP}), epilogue + hand-over {tot[3]:.0f}, "
         f"unit to unit {tot[4]:.0f} cycles")
+  print(f"  epilogue of units 2-13: column loop {tot[6]:.0f}, last store -> h_full arrive {tot[7]:.0f} cycles")
 
 
 case("edge")
