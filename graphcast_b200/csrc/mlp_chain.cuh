@@ -90,6 +90,169 @@ struct ChainLayer {
   int res_q;                             // residual = the kept result in scratch ring res_q, -1 = none
 };
 
+// ---- epilogue ----------------------------------------------------------------------------
+// A consumer thread owns rows lr0 + 8h (h = 0, 1) of the tile and, in each 32-column chunk of its
+// 256 unit columns, the column pairs 8jj + 2q (jj = 0..3): 16 results per chunk, kept in
+// acc[16 * chunk .. + 16) at acc[4jj + 2h], acc[4jj + 2h + 1].  Every pointer below addresses
+// column col_base + 2q of the first chunk of the unit; a chunk's accesses are the pointer plus a
+// compile-time offset, and the column loop advances the pointers once per iteration.
+struct ChainEpi {
+  const float* pre[2][2];     // [table][h]: gathered pre-activation addend rows
+  const float* res[2];        // [h]: fp32 residual rows
+  float* out[2];              // [h]: result + residual, fp32
+  float* outy[2];             // [h]: result without residual, fp32
+  uint8_t* img0;              // operand images at the piece of (column col_base + 2q, row lr0)
+  uint8_t* img1;              // (scratch slot of a kept layer)
+  const uint8_t* res_img;
+  uint32_t s_bias, s_scale, s_offset;   // shared-memory parameter vectors
+  bool row_ok[2];             // [h]: row < rows (rows past the end exist in the images only)
+  bool pre_b;                 // second addend table present
+  bool has_bias, st_out, st_outy, st_img0, st_img1;
+  float mean[2], rstd[2];
+};
+
+// Chunks per column-loop iteration.  The loop cannot be unrolled (8 chunks of straight-line code
+// per unit overflow the instruction cache, DESIGN.md §3.1b), and a rolled loop can only index the
+// accumulator with constants by shifting it down after every iteration: two chunks per
+// iteration shift 96 registers 4 times per unit instead of 112 registers 8 times.
+constexpr int kEpiChunks = 2;
+constexpr int kEpiIters = kUnitN / 32 / kEpiChunks;
+static_assert(kEpiChunks % 2 == 0 && kEpiIters * kEpiChunks * 32 == kUnitN,
+              "the residual double buffer alternates halves chunk by chunk");
+
+// p + bytes as integer arithmetic: also defined for p == nullptr (an absent output or input,
+// whose accesses are predicated off).
+template <typename T>
+__device__ __forceinline__ T* byte_offset(T* p, long long bytes) {
+  return reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(p) + bytes);
+}
+
+// Byte offset, in an operand image, of (chunk c, column pair jj, row h) from the thread's piece
+// in chunk 0 (image_offset with gc = col_base + 32c + 8jj + 2q, r = lr0 + 8h).
+__device__ __forceinline__ constexpr int epi_img_off(int c, int jj, int h) {
+  return (2 * c + (jj >> 1)) * GCB_A_IMAGE_BLOCK + (jj & 1) * kALbo + h * 8 * 16;
+}
+
+// Gathered addends of chunk c: buf[2jj + h] = table a, buf[8 + 2jj + h] = table b.  Table a
+// reads as 0 and table b as -0 where they are missing (rows past the end; no second table): the
+// sum a + b is then exactly a, or +0, as when the missing addends were skipped.
+__device__ __forceinline__ void epi_load_pre(const ChainEpi& e, uint2 (&buf)[16], int c, bool ok) {
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int o = 32 * c + 8 * jj;
+      buf[2 * jj + h] = ptx::ld_global_nc_v2_pred(e.pre[0][h] + o, ok && e.row_ok[h], 0u);
+      buf[8 + 2 * jj + h] = ptx::ld_global_nc_v2_pred(e.pre[1][h] + o, ok && e.row_ok[h] && e.pre_b, 0x80000000u);
+    }
+}
+// fp32 residual of chunk c into buf[half + 2jj + h] (rows past the end: 0).
+__device__ __forceinline__ void epi_load_res(const ChainEpi& e, uint2 (&buf)[16], int half, int c, bool ok) {
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      buf[half + 2 * jj + h] = ptx::ld_global_v2_pred(e.res[h] + 32 * c + 8 * jj, ok && e.row_ok[h]);
+}
+// Operand-image residual of chunk c: buf[half + 2jj + h] = (hi, lo) words.
+__device__ __forceinline__ void epi_load_res_img(const ChainEpi& e, uint2 (&buf)[16], int half, int c, bool ok) {
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint8_t* p = e.res_img + epi_img_off(c, jj, h);
+      buf[half + 2 * jj + h] = make_uint2(ptx::ld_global_b32_pred(p, ok), ptx::ld_global_b32_pred(p + kAPartBytes, ok));
+    }
+}
+
+// The column loop of one unit for one layer kind (kAdd: Plain / Swish with gathered addends).
+// buf holds chunk 0's inputs on entry (loaded before the MMAs).  Each chunk adds the addends, then
+// loads the next chunk's inputs, then computes and stores its 16 results; nothing in the loop
+// branches, so the 16 independent element chains of a chunk interleave.  The arithmetic per
+// element is that of mlp_layer_tc_kernel, in the same order, so the two kernels agree bit for
+// bit (including the + 0 of an absent residual, which turns -0 into +0).
+template <int kKind, bool kAdd>
+__device__ __forceinline__ void chain_epilogue(float (&acc)[128], uint2 (&buf)[16], ChainEpi e,
+                                               uint64_t keep_policy) {
+  constexpr bool kLN = kKind >= kKindLN;
+  constexpr bool kFp32Out = kKind != kKindSwish;     // swish layers deliver operand images only
+  constexpr bool kOut = kFp32Out && kKind != kKindLNImg;
+#pragma unroll 1
+  for (int it = 0; it < kEpiIters; ++it) {
+    const bool more = it + 1 < kEpiIters;
+#pragma unroll
+    for (int cc = 0; cc < kEpiChunks; ++cc) {
+      float* v = &acc[16 * cc];
+      const bool next = cc + 1 < kEpiChunks || more;
+      const int cur = 8 * (cc & 1);                  // residual: this chunk in buf[cur..], next in the other half
+      if constexpr (kAdd) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float gx = __uint_as_float(buf[i].x) + __uint_as_float(buf[8 + i].x);
+          const float gy = __uint_as_float(buf[i].y) + __uint_as_float(buf[8 + i].y);
+          v[4 * (i >> 1) + 2 * (i & 1)] += gx;
+          v[4 * (i >> 1) + 2 * (i & 1) + 1] += gy;
+        }
+        epi_load_pre(e, buf, cc + 1, next);
+      } else if constexpr (kKind == kKindLNRes) {
+        epi_load_res(e, buf, 8 - cur, cc + 1, next);
+      } else if constexpr (kKind == kKindLNImg) {
+        epi_load_res_img(e, buf, 8 - cur, cc + 1, next);
+      }
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int co = 4 * (32 * cc + 8 * jj);       // byte offset of the column pair in a row
+        const float2 b = ptx::ld_shared_v2_pred(e.s_bias + co, e.has_bias);
+        float2 sc = make_float2(1.f, 1.f), of = make_float2(0.f, 0.f);
+        if constexpr (kLN) {
+          sc = ptx::ld_shared_v2_pred(e.s_scale + co, true);
+          of = ptx::ld_shared_v2_pred(e.s_offset + co, true);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float* a = &v[4 * jj + 2 * h];
+          const uint2 rin = buf[cur + 2 * jj + h];
+          float2 y = make_float2(a[0] + b.x, a[1] + b.y);
+          if constexpr (kKind == kKindSwish) { y.x = swish_f(y.x); y.y = swish_f(y.y); }
+          if constexpr (kLN) {
+            y.x = (y.x - e.mean[h]) * e.rstd[h] * sc.x + of.x;
+            y.y = (y.y - e.mean[h]) * e.rstd[h] * sc.y + of.y;
+          }
+          float2 rs = make_float2(0.f, 0.f);
+          if constexpr (kKind == kKindLNRes) rs = make_float2(__uint_as_float(rin.x), __uint_as_float(rin.y));
+          float2 x = make_float2(y.x + rs.x, y.y + rs.y);
+          if constexpr (kFp32Out) ptx::st_global_v2_pred(e.outy[h] + co / 4, y, e.st_outy && e.row_ok[h]);
+          if constexpr (kOut) ptx::st_global_v2_pred(e.out[h] + co / 4, x, e.st_out && e.row_ok[h]);
+          if constexpr (kKind == kKindLNImg) {
+            // (hi, lo) bf16 words; a packed word holds the even column in its low half
+            x.x += __uint_as_float(rin.x << 16) + __uint_as_float(rin.y << 16);
+            x.y += __uint_as_float(rin.x & 0xffff0000u) + __uint_as_float(rin.y & 0xffff0000u);
+          }
+          uint32_t hi, lo;
+          ptx::split_bf16x2(x.x, x.y, hi, lo);
+          const int io = epi_img_off(cc, jj, h);
+          ptx::st_global_b32_pred(e.img0 + io, hi, e.st_img0);
+          ptx::st_global_b32_pred(e.img0 + io + kAPartBytes, lo, e.st_img0);
+          ptx::st_global_b32_hint_pred(e.img1 + io, hi, keep_policy, e.st_img1);
+          ptx::st_global_b32_hint_pred(e.img1 + io + kAPartBytes, lo, keep_policy, e.st_img1);
+        }
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 128 - 16 * kEpiChunks; ++i) acc[i] = acc[i + 16 * kEpiChunks];
+    constexpr int kCols = 32 * kEpiChunks;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      e.pre[0][h] += kCols; e.pre[1][h] += kCols; e.res[h] += kCols;
+      e.out[h] += kCols; e.outy[h] += kCols;
+    }
+    e.img0 += 2 * kEpiChunks * GCB_A_IMAGE_BLOCK;
+    e.img1 += 2 * kEpiChunks * GCB_A_IMAGE_BLOCK;
+    e.res_img += 2 * kEpiChunks * GCB_A_IMAGE_BLOCK;
+    e.s_bias += 4 * kCols; e.s_scale += 4 * kCols; e.s_offset += 4 * kCols;
+  }
+}
+
 template <bool kSplit, bool kPre, bool kBig>
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, const int nslots) {
@@ -385,24 +548,7 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
         const ChainLayer& cl = s_layer[l];
         const int kind = cl.kind;
-        float* const out_ptr = cl.out;
-        float* const outy_ptr = cl.out_y;
-        const float* const res_ptr = kind == kKindLNRes ? cl.residual : nullptr;
-        const long long ld_out = cl.ld_out, ld_outy = cl.ld_outy, ld_res = cl.ld_res;
         const float* const s_bias = cl.bias_off >= 0 ? s_param + cl.bias_off : nullptr;
-        const float* const s_scale = cl.scale_off >= 0 ? s_param + cl.scale_off : nullptr;
-        const float* const s_offset = cl.offset_off >= 0 ? s_param + cl.offset_off : nullptr;
-        uint8_t* const img0 = cl.out_img != nullptr
-                                  ? cl.out_img + static_cast<size_t>(tile) * (kMaxN / kKStep) * GCB_A_IMAGE_BLOCK
-                                  : nullptr;
-        const uint8_t* res_img = cl.res_img != nullptr
-                                     ? cl.res_img + static_cast<size_t>(tile) * (kMaxN / kKStep) * GCB_A_IMAGE_BLOCK
-                                     : nullptr;
-        // Residual = the kept result of an earlier layer: the slot this CTA's consumers wrote for
-        // this tile (same threads, same rows and columns: program order makes it visible, and the
-        // slot cannot be rewritten before these warps reach tile ti + nslots themselves).
-        if (cl.res_q >= 0) res_img = scratch_slot(cl.res_q, ti);
-        if (kind != kKindLNImg) res_img = nullptr;
         if (eg == 0 && ti + 1 < T && (cl.residual != nullptr || cl.res_img != nullptr)) {
           // Pull the residual of this layer's NEXT tile into L2 now (a whole step ahead).
           const uint32_t ntile = tile + ncl;
@@ -418,79 +564,69 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         }
         const bool is_ln = kind >= kKindLN;
         const bool want_pre = kPre && !is_ln && cl.n_pre > 0;
-        const long long grow0 = static_cast<long long>(tile) * kTileM + lr0;
-        // Inputs of the epilogue that live in global memory - the gathered pre-activation addends
-        // (two tables, gathered through their row indices) or the residual (fp32 rows or an operand
-        // image) - are loaded into registers one 32-column chunk ahead of their use, chunk 0 before
-        // the MMAs, so that their latency hides behind the MMAs and the previous chunk.  With the
-        // loads next to the stores they were paid once per column pair: the compiler cannot move a
-        // load above a store that may alias it.  Loading ahead is safe for the in-place updates
-        // (out_img == res_img, out == residual): every word is read and then written by the same
-        // thread, and a chunk's loads touch other columns than the stores they move ahead of.
-        // buf (32 registers) holds, for i = 2 jj + h (column pair jj, row h of the chunk):
-        //   addends: buf[i] / buf[8 + i] = table a / table b of the next chunk, as float bits
-        //            (they are added to the accumulator before that chunk's loads are issued);
-        //   residual: buf[i] = fp32 pair or (hi, lo) image words of this chunk, buf[8 + i] those
-        //            of the next one.
-        const float* pre_src[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};   // [table][h], nullptr = none
-        const float* res_src[2] = {nullptr, nullptr};                            // [h]
-        if (want_pre) {
-          const PreAddInfo pa = s_pre[l * 2];
-          const PreAddInfo pb = s_pre[l * 2 + 1];
+        const int keep_q = cl.keep_q;
+        // Epilogue state of this unit (ChainEpi).  Pointers of absent outputs are formed from
+        // nullptr; their stores are predicated off.
+        ChainEpi e;
+        {
+          const long long grow0 = static_cast<long long>(tile) * kTileM + lr0;
+          const int c0 = col_base + 2 * q;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const long long grow = grow0 + 8 * h;
-            if (grow < rows_total) {
-              const int ra = pa.idx ? __ldg(pa.idx + grow) : static_cast<int>(grow);
-              pre_src[0][h] = pa.table + static_cast<long long>(ra) * pa.ld + col_base + 2 * q;
-              if (cl.n_pre > 1) {
-                const int rb = pb.idx ? __ldg(pb.idx + grow) : static_cast<int>(grow);
-                pre_src[1][h] = pb.table + static_cast<long long>(rb) * pb.ld + col_base + 2 * q;
+            e.row_ok[h] = grow < rows_total;
+            e.out[h] = byte_offset(cl.out, 4 * (grow * cl.ld_out + c0));
+            e.outy[h] = byte_offset(cl.out_y, 4 * (grow * cl.ld_outy + c0));
+            e.res[h] = byte_offset(cl.residual, 4 * (grow * cl.ld_res + c0));
+            if (want_pre) {
+              const PreAddInfo pa = s_pre[l * 2];
+              const PreAddInfo pb = s_pre[l * 2 + 1];
+              int ra = 0, rb = 0;
+              if (e.row_ok[h]) {
+                ra = pa.idx ? __ldg(pa.idx + grow) : static_cast<int>(grow);
+                if (cl.n_pre > 1) rb = pb.idx ? __ldg(pb.idx + grow) : static_cast<int>(grow);
               }
+              e.pre[0][h] = byte_offset(pa.table, 4 * (static_cast<long long>(ra) * pa.ld + c0));
+              e.pre[1][h] = byte_offset(pb.table, 4 * (static_cast<long long>(rb) * pb.ld + c0));
             }
           }
-        } else if (res_ptr != nullptr) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            if (grow0 + 8 * h < rows_total) res_src[h] = res_ptr + (grow0 + 8 * h) * ld_res + col_base + 2 * q;
+          const long long piece = static_cast<long long>(image_offset(c0, lr0));
+          const long long tile_img = static_cast<long long>(tile) * (kMaxN / kKStep) * GCB_A_IMAGE_BLOCK;
+          e.img0 = byte_offset(cl.out_img, tile_img + piece);
+          // keep: this tile's slot of the scratch ring (written once h_free has been passed below)
+          e.img1 = byte_offset(keep_q >= 0 ? scratch_slot(keep_q, ti) : nullptr, piece);
+          // Residual = the kept result of an earlier layer: the slot this CTA's consumers wrote for
+          // this tile (same threads, same rows and columns: program order makes it visible, and the
+          // slot cannot be rewritten before these warps reach tile ti + nslots themselves).
+          e.res_img = cl.res_q >= 0 ? scratch_slot(cl.res_q, ti) + piece : byte_offset(cl.res_img, tile_img + piece);
+          e.pre_b = cl.n_pre > 1;
+          e.has_bias = s_bias != nullptr;
+          e.st_out = cl.out != nullptr;
+          e.st_outy = cl.out_y != nullptr;
+          e.st_img0 = cl.out_img != nullptr;
+          // Through a vote: a predicate the compiler knows to be warp-uniform lets it predicate the
+          // cache-hinted stores (it branches around them otherwise).
+          e.st_img1 = __all_sync(0xffffffffu, keep_q >= 0);
+          e.s_bias = ptx::smem_addr(s_param + (cl.bias_off >= 0 ? cl.bias_off : 0) + c0);
+          e.s_scale = ptx::smem_addr(s_param + (cl.scale_off >= 0 ? cl.scale_off : 0) + c0);
+          e.s_offset = ptx::smem_addr(s_param + (cl.offset_off >= 0 ? cl.offset_off : 0) + c0);
         }
+        // Inputs of the epilogue that live in global memory - the gathered pre-activation addends
+        // (two tables, gathered through their row indices) or the residual (fp32 rows or an operand
+        // image) - are loaded into registers one 32-column chunk ahead of their use, chunk 0 before
+        // the MMAs, so that their latency hides behind the MMAs and the previous chunk.  Loading
+        // ahead is safe for the in-place updates (out_img == res_img, out == residual): every word
+        // is read and then written by the same thread, and a chunk's loads touch other columns than
+        // the stores they move ahead of.
         uint2 buf[16];
-        auto load_pre = [&](int c0) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int c = c0 + 8 * (i >> 1);
-            buf[i] = make_uint2(0u, 0u);
-            buf[8 + i] = make_uint2(0u, 0u);
-            if (pre_src[0][i & 1] != nullptr) buf[i] = __ldg(reinterpret_cast<const uint2*>(pre_src[0][i & 1] + c));
-            if (pre_src[1][i & 1] != nullptr) buf[8 + i] = __ldg(reinterpret_cast<const uint2*>(pre_src[1][i & 1] + c));
-          }
-        };
-        auto load_res = [&](int c0, int half) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int c = c0 + 8 * (i >> 1);
-            uint2 v = make_uint2(0u, 0u);
-            if (res_src[i & 1] != nullptr) {
-              v = *reinterpret_cast<const uint2*>(res_src[i & 1] + c);
-            } else if (res_img != nullptr) {
-              const size_t o = image_offset(col_base + c + 2 * q, lr0 + 8 * (i & 1));
-              v.x = *reinterpret_cast<const uint32_t*>(res_img + o);
-              v.y = *reinterpret_cast<const uint32_t*>(res_img + o + kAPartBytes);
-            }
-            buf[half + i] = v;
-          }
-        };
-        const bool has_res = res_ptr != nullptr || res_img != nullptr;
-        if (want_pre) load_pre(0);
-        else if (has_res) load_res(0, 0);
-        const int keep_q = cl.keep_q;
-        uint8_t* img1 = nullptr;
+        if (want_pre) epi_load_pre(e, buf, 0, true);
+        else if (kind == kKindLNRes) epi_load_res(e, buf, 0, 0, true);
+        else if (kind == kKindLNImg) epi_load_res_img(e, buf, 0, 0, true);
         if (lead && eg == 0) trace(u, 0);
         if (keep_q >= 0) {
           // previous readers of this slot (tile ti - nslots) are done in both CTAs
           ptx::mbar_wait(&h_free_bar[keep_q * kChainSlotsMax + (ti % nslots)],
                          (static_cast<uint32_t>(ti / nslots) & 1u) ^ 1u);
-          img1 = scratch_slot(keep_q, ti);
         }
         if (lead && eg == 0) { trace(u, 2); trace_val(u, 9, cl.ksteps); }
         mma_unit<kSplit, Cfg::kStages, Cfg::kStageBytes, Cfg::kAStageBytes>(
@@ -510,7 +646,8 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
           }
         }
         if (lead && eg == 0) trace(u, 3);
-        float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
+        e.mean[0] = e.mean[1] = 0.f;
+        e.rstd[0] = e.rstd[1] = 1.f;
         if (is_ln) {
           // Each CTA computes (mean, M2) of its 256 columns of a row, hands them to the partner
           // through distributed shared memory, and both combine them (Chan's parallel update).
@@ -533,97 +670,27 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
           for (int h = 0; h < 2; ++h) {
             const float2 other = s_lnx[lb * kTileM + lr0 + 8 * h];
             const float delta = other.x - mh[h];
-            mean[h] = 0.5f * (mh[h] + other.x);
+            e.mean[h] = 0.5f * (mh[h] + other.x);
             const float var = (m2h[h] + other.y + delta * delta * (0.5f * kUnitN)) * (1.0f / (2 * kUnitN));
-            rstd[h] = rsqrtf(var + 1e-5f);
+            e.rstd[h] = rsqrtf(var + 1e-5f);
           }
           ++ln_count;
           if (lead && eg == 0) trace(u, 4);
         }
-        // Epilogue, 32 columns at a time.  The loop is NOT unrolled: it runs once per unit, and
-        // unrolled over the 8 chunks its straight-line code (~150 KB) streamed through the
-        // instruction cache, which bounded the epilogue at ~100 000 cycles per unit.  To keep the
-        // accumulator indexed with constants only (it must stay in registers), every iteration
-        // works on acc[0..15] and then shifts the accumulator down by one chunk.
-#pragma unroll 1
-        for (int c0 = 0; c0 < kUnitN; c0 += 32) {
-          if (want_pre) {
-            // a + b (b only where there is a second table), then added to the accumulator
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              float2 g = make_float2(__uint_as_float(buf[i].x), __uint_as_float(buf[i].y));
-              if (pre_src[1][i & 1] != nullptr) {
-                g.x += __uint_as_float(buf[8 + i].x);
-                g.y += __uint_as_float(buf[8 + i].y);
-              }
-              acc[4 * (i >> 1) + 2 * (i & 1)] += g.x;
-              acc[4 * (i >> 1) + 2 * (i & 1) + 1] += g.y;
-            }
-            if (c0 + 32 < kUnitN) load_pre(c0 + 32);
-          } else if (has_res && c0 + 32 < kUnitN) {
-            load_res(c0 + 32, 8);
-          }
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int gc = col_base + c0 + 8 * jj + 2 * q;
-            const float2 b = s_bias != nullptr ? *reinterpret_cast<const float2*>(s_bias + gc) : make_float2(0.f, 0.f);
-            float2 sc = make_float2(1.f, 1.f), of = make_float2(0.f, 0.f);
-            if (is_ln) {
-              sc = *reinterpret_cast<const float2*>(s_scale + gc);
-              of = *reinterpret_cast<const float2*>(s_offset + gc);
-            }
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              float* v = &acc[4 * jj + 2 * h];
-              const uint2 rin = buf[2 * jj + h];                  // residual of this chunk
-              const int r = lr0 + 8 * h;
-              const long long grow = grow0 + 8 * h;
-              const bool row_ok = grow < rows_total;
-              float2 y = make_float2(v[0] + b.x, v[1] + b.y);
-              if (kind == kKindSwish) { y.x = swish_f(y.x); y.y = swish_f(y.y); }
-              if (is_ln) {
-                y.x = (y.x - mean[h]) * rstd[h] * sc.x + of.x;
-                y.y = (y.y - mean[h]) * rstd[h] * sc.y + of.y;
-              }
-              // fp32 residual (rows past the end: none)
-              float2 rs = make_float2(0.f, 0.f);
-              if (res_ptr != nullptr && row_ok) rs = make_float2(__uint_as_float(rin.x), __uint_as_float(rin.y));
-              if (row_ok) {
-                if (outy_ptr != nullptr) *reinterpret_cast<float2*>(outy_ptr + grow * ld_outy + gc) = y;
-                if (out_ptr != nullptr)
-                  *reinterpret_cast<float2*>(out_ptr + grow * ld_out + gc) = make_float2(y.x + rs.x, y.y + rs.y);
-              }
-              if (img0 != nullptr || img1 != nullptr) {
-                // Operand image of the result (+ residual): the four threads of a row complete
-                // one 16-byte piece, eight rows a 128-byte line.
-                float2 x = make_float2(y.x + rs.x, y.y + rs.y);
-                const size_t o = image_offset(gc, r);
-                if (res_img != nullptr) {
-                  // Residual held as an operand image (x = hi + lo, two bf16); a packed word
-                  // holds the even column in its low and the odd column in its high half.
-                  const uint32_t hw = rin.x, lw = rin.y;
-                  x.x += __uint_as_float(hw << 16) + __uint_as_float(lw << 16);
-                  x.y += __uint_as_float(hw & 0xffff0000u) + __uint_as_float(lw & 0xffff0000u);
-                }
-                uint32_t hi, lo;
-                ptx::split_bf16x2(x.x, x.y, hi, lo);
-                if (img0 != nullptr) {
-                  *reinterpret_cast<uint32_t*>(img0 + o) = hi;
-                  *reinterpret_cast<uint32_t*>(img0 + o + kAPartBytes) = lo;
-                }
-                if (img1 != nullptr) {       // scratch slot: keep these lines in the L2
-                  ptx::st_global_b32_hint(img1 + o, hi, keep_policy);
-                  ptx::st_global_b32_hint(img1 + o + kAPartBytes, lo, keep_policy);
-                }
-              }
-            }
-          }
-#pragma unroll
-          for (int i = 0; i < 128 - 16; ++i) acc[i] = acc[i + 16];
-          if (!want_pre) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) buf[i] = buf[8 + i];
-          }
+        // One column loop per layer kind, chosen once per unit.
+        if (kPre && want_pre) {
+          if (kind == kKindSwish) chain_epilogue<kKindSwish, kPre>(acc, buf, e, keep_policy);
+          else chain_epilogue<kKindPlain, kPre>(acc, buf, e, keep_policy);
+        } else if (kind == kKindSwish) {
+          chain_epilogue<kKindSwish, false>(acc, buf, e, keep_policy);
+        } else if (kind == kKindPlain) {
+          chain_epilogue<kKindPlain, false>(acc, buf, e, keep_policy);
+        } else if (kind == kKindLN) {
+          chain_epilogue<kKindLN, false>(acc, buf, e, keep_policy);
+        } else if (kind == kKindLNRes) {
+          chain_epilogue<kKindLNRes, false>(acc, buf, e, keep_policy);
+        } else {
+          chain_epilogue<kKindLNImg, false>(acc, buf, e, keep_policy);
         }
         if (lead && eg == 0) trace(u, 5);
         if (keep_q >= 0) {

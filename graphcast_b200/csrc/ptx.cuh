@@ -113,6 +113,55 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
 __device__ __forceinline__ void st_global_b32_hint(void* ptr, uint32_t v, uint64_t policy) {
   asm volatile("st.global.L2::cache_hint.b32 [%0], %1, %2;" ::"l"(ptr), "r"(v), "l"(policy) : "memory");
 }
+
+// ---- predicated accesses (the chain kernel's epilogue) ----------------------------------
+// Predicated instructions instead of branches: a load whose predicate is false leaves `fill` in
+// its destination, a store whose predicate is false does nothing, and the code around them stays
+// one straight-line block that the compiler can schedule freely.
+__device__ __forceinline__ uint2 ld_global_nc_v2_pred(const void* ptr, bool pred, uint32_t fill) {
+  uint2 v;
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %3, 0;\n mov.b32 %0, %4;\n mov.b32 %1, %4;\n"
+      " @p ld.global.nc.v2.b32 {%0, %1}, [%2];\n}"
+      : "=r"(v.x), "=r"(v.y) : "l"(ptr), "r"(static_cast<uint32_t>(pred)), "r"(fill));
+  return v;
+}
+// Coherent (not .nc): the fp32 residual may be the output this kernel updates in place.
+__device__ __forceinline__ uint2 ld_global_v2_pred(const void* ptr, bool pred) {
+  uint2 v;
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %3, 0;\n mov.b32 %0, 0;\n mov.b32 %1, 0;\n"
+      " @p ld.global.v2.b32 {%0, %1}, [%2];\n}"
+      : "=r"(v.x), "=r"(v.y) : "l"(ptr), "r"(static_cast<uint32_t>(pred)));
+  return v;
+}
+__device__ __forceinline__ uint32_t ld_global_b32_pred(const void* ptr, bool pred) {
+  uint32_t v;
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %2, 0;\n mov.b32 %0, 0;\n @p ld.global.b32 %0, [%1];\n}"
+      : "=r"(v) : "l"(ptr), "r"(static_cast<uint32_t>(pred)));
+  return v;
+}
+__device__ __forceinline__ float2 ld_shared_v2_pred(uint32_t saddr, bool pred) {
+  float2 v;
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %3, 0;\n mov.b32 %0, 0f00000000;\n mov.b32 %1, 0f00000000;\n"
+      " @p ld.shared.v2.f32 {%0, %1}, [%2];\n}"
+      : "=f"(v.x), "=f"(v.y) : "r"(saddr), "r"(static_cast<uint32_t>(pred)));
+  return v;
+}
+__device__ __forceinline__ void st_global_v2_pred(void* ptr, float2 v, bool pred) {
+  asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %3, 0;\n @p st.global.v2.f32 [%0], {%1, %2};\n}"
+               ::"l"(ptr), "f"(v.x), "f"(v.y), "r"(static_cast<uint32_t>(pred)) : "memory");
+}
+__device__ __forceinline__ void st_global_b32_pred(void* ptr, uint32_t v, bool pred) {
+  asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %2, 0;\n @p st.global.b32 [%0], %1;\n}"
+               ::"l"(ptr), "r"(v), "r"(static_cast<uint32_t>(pred)) : "memory");
+}
+__device__ __forceinline__ void st_global_b32_hint_pred(void* ptr, uint32_t v, uint64_t policy, bool pred) {
+  asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %3, 0;\n @p st.global.L2::cache_hint.b32 [%0], %1, %2;\n}"
+               ::"l"(ptr), "r"(v), "l"(policy), "r"(static_cast<uint32_t>(pred)) : "memory");
+}
 // bulk copy global -> shared, multicast, with an L2 cache policy for the source lines
 __device__ __forceinline__ void bulk_g2s_multicast_hint(void* smem_dst, const void* gmem_src,
                                                         uint32_t bytes, uint64_t* bar,
