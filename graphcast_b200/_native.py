@@ -131,7 +131,10 @@ EXPORTS = {
                                       C.c_int32, _fp, _fp]),
     "gcb_unpack_grid_outputs": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int64, _fp, _fp, _fp,
                                           _fp, _fp, _fp]),
-    "gcb_forward": (C.c_int, [C.POINTER(Model), _fp, _fp, _fp, C.POINTER(C.c_int32)]),
+    "gcb_output_loss": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp, _fp,
+                                  _fp, _fp, _fp, _fp, _fp, C.c_int64, _fp, _fp]),
+    "gcb_output_loss_workspace_bytes": (C.c_int64, [C.c_int32]),
+    "gcb_forward":(C.c_int, [C.POINTER(Model), _fp, _fp, _fp, C.POINTER(C.c_int32)]),
     "gcb_forward_stage": (C.c_int, [C.POINTER(Model), C.c_int32, C.c_int32, _fp, _fp, _fp,
                                     C.POINTER(C.c_int32)]),
     "gcb_chain_scratch_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),

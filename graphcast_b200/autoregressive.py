@@ -1,4 +1,4 @@
-"""Inference mirror of `autoregressive.Predictor` (weathernext/utils/autoregressive.py:36-222).
+"""Inference mirror of `autoregressive.Predictor` (weathernext/utils/autoregressive.py:36-312).
 
 The reference wrapper turns a one-step predictor into a multi-step one: a call with a
 `targets_template` of T time steps unrolls the inner predictor T times (`hk.scan`), feeding
@@ -8,14 +8,26 @@ one of `rollout.chunked_prediction_generator` (pinned against the reference's ge
 tests/test_reference_rollout_golden.py), so this mirror unrolls through it and concatenates the
 per-step predictions on the device.  Kept from the reference: the validation errors
 (:88-116), constant inputs passed through unchanged, predictions carrying the template's time
-coordinate.  Not provided: `loss` / `loss_and_predictions`, input noise and gradient
-checkpointing (training-side features, outside the inference hot path)."""
+coordinate.
+
+`loss` (:224-312) is the mean over the target times of the inner predictor's per-step losses:
+with one target time it delegates to the inner `loss`; otherwise it unrolls the same way, calling
+the inner `loss_and_predictions` with the targets of each step and feeding its predictions back.
+When the inner predictor is this package's `GraphCast` (directly or under a fused
+`normalization.InputsAndResiduals`), every step's loss stays on the device as per-channel sums of
+`gcb_output_loss` and all of them are read back once, after the last step.
+
+Not provided: input noise and gradient checkpointing (training-side features)."""
 
 from __future__ import annotations
 
 from typing import Optional
 
+import numpy as np
+import torch
+
 from graphcast_b200 import graphcast
+from graphcast_b200 import normalization
 from graphcast_b200 import rollout
 from graphcast_b200 import xarray_shim as xs
 
@@ -61,3 +73,53 @@ class Predictor(graphcast.Predictor):
         step, rng=None, inputs=inputs, targets_template=targets_template,
         num_steps_per_chunk=1, forcings=forcings))
     return xs.concat_time(chunks)
+
+  def _device_step(self):
+    """(inputs, targets, forcings) -> (finish, predictions, device channel sums) when the inner
+    predictor reduces its loss on the device, else None."""
+    p = self._predictor
+    if isinstance(p, graphcast.GraphCast):
+      return lambda i, t, f: p._device_loss(i, t, f, None, True)
+    if isinstance(p, normalization.InputsAndResiduals) and p._fuses():
+      return lambda i, t, f: p._device_loss(i, t, f, True)
+    return None
+
+  def loss(self, inputs, targets, forcings, **kwargs):
+    """The mean over target times of the per-step losses of the underlying predictor."""
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    forcings = xs.from_xarray(forcings)
+    if targets.sizes["time"] == 1:
+      return self._predictor.loss(inputs, targets, forcings, **kwargs)
+    self._validate(inputs, targets, forcings)
+    device_step = self._device_step()
+    records = []
+
+    def step(rng, inputs, targets_template, forcings):
+      if device_step is not None:
+        finish, predictions, sums = device_step(inputs, targets_template, forcings)
+        records.append((finish, sums))
+      else:
+        loss_and_diagnostics, predictions = self._predictor.loss_and_predictions(
+            inputs, targets_template, forcings, **kwargs)
+        records.append(loss_and_diagnostics)
+      return predictions
+
+    for _ in rollout.chunked_prediction_generator(
+        step, rng=None, inputs=inputs, targets_template=targets, num_steps_per_chunk=1,
+        forcings=forcings):
+      pass
+    if device_step is not None:
+      sums = torch.stack([s for _, s in records]).cpu().numpy()      # the one read-back
+      records = [finish(sums[t]) for t, (finish, _) in enumerate(records)]
+    return _mean_over_time([l for l, _ in records], [d for _, d in records])
+
+
+def _mean_over_time(step_losses, step_diagnostics):
+  """Mean over the steps of `(batch,)` losses and diagnostics (NaNs propagate)."""
+  mean = lambda arrays: xs.DataArray(
+      np.mean(np.stack([np.asarray(a.values, np.float64) for a in arrays]), axis=0
+              ).astype(np.float32), step_losses[0].dims)
+  diagnostics = xs.Dataset()
+  for name in step_diagnostics[0].keys():
+    diagnostics[name] = mean([d.data_vars[name] for d in step_diagnostics])
+  return mean(step_losses), diagnostics

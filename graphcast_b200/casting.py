@@ -19,6 +19,11 @@ at 0.25 degree), so switching to this backend does not lose accuracy against wha
 in the reference.  Inputs and predictions stay float32 Datasets, which is what the reference wrapper
 returns.
 
+The same holds for `loss` / `loss_and_predictions` (reference :67-117): the reference evaluates the
+loss in bfloat16 and casts it back to the targets' dtype; here the outputs of the bf16 step are
+compared with the targets in float32 and the weighted squared errors are summed in float64
+(`gcb_output_loss`), so the loss is not rounded to bfloat16 anywhere.
+
 To keep the demo's wrapper stack working unchanged,
 
     predictor = graphcast.GraphCast(model_config, task_config, params=...)
@@ -51,3 +56,9 @@ class Bfloat16Cast(graphcast.Predictor):
 
   def __call__(self, inputs, targets_template, forcings, **kwargs):
     return self._predictor(inputs, targets_template, forcings, **kwargs)
+
+  def loss(self, inputs, targets, forcings, **kwargs):
+    return self._predictor.loss(inputs, targets, forcings, **kwargs)
+
+  def loss_and_predictions(self, inputs, targets, forcings, **kwargs):
+    return self._predictor.loss_and_predictions(inputs, targets, forcings, **kwargs)

@@ -765,6 +765,41 @@ int gcb_unpack_grid_outputs(const float* y, int32_t ld_y, int32_t n_out, int64_t
   return GCB_OK;
 }
 
+int64_t gcb_output_loss_workspace_bytes(int32_t n_out) {
+  if (n_out <= 0) return -1;
+  return static_cast<int64_t>(gcb::kLossGroups) * n_out * static_cast<int64_t>(sizeof(double));
+}
+
+int gcb_output_loss(const float* y, int32_t ld_y, int32_t n_out, int32_t n_lat, int32_t n_lon,
+                    const float* scale, const float* offset, const float* add_planes,
+                    const int32_t* add_plane_index, const float* targets, const float* lat_weight,
+                    float* planes_out, void* workspace, int64_t workspace_bytes,
+                    double* channel_sums, void* stream) {
+  GCB_CHECK_ARG(y && targets && lat_weight && workspace && channel_sums, "null pointer");
+  GCB_CHECK_ARG(n_out > 0 && ld_y >= n_out, "ld_y too small");
+  GCB_CHECK_ARG(n_lat > 0 && n_lon > 0, "empty grid");
+  GCB_CHECK_ARG((add_planes == nullptr) == (add_plane_index == nullptr), "add_planes/index mismatch");
+  GCB_CHECK_ARG(workspace_bytes >= gcb_output_loss_workspace_bytes(n_out), "workspace too small");
+  GCB_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 7u) == 0 &&
+                (reinterpret_cast<uintptr_t>(channel_sums) & 7u) == 0, "unaligned fp64 buffer");
+  const long long n_nodes = static_cast<long long>(n_lat) * n_lon;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // algorithmic bytes: y and the targets read, the add planes read and the predictions written
+  // when present, the partials written and read back
+  ProfScope prof(st, GCB_KIND_LOSS, 0.0,
+                 4.0 * n_nodes * n_out * (2.0 + (add_planes ? 1.0 : 0.0) + (planes_out ? 1.0 : 0.0)) +
+                     16.0 * gcb::kLossGroups * n_out);
+  dim3 grid(gcb::kLossGroups, static_cast<unsigned>((n_out + 31) / 32));
+  double* partial = static_cast<double*>(workspace);
+  gcb::output_loss_kernel<<<grid, 256, 0, st>>>(y, ld_y, n_out, n_lon, n_nodes, scale, offset,
+                                               add_planes, add_plane_index, targets, lat_weight,
+                                               planes_out, partial);
+  GCB_CUDA(cudaGetLastError());
+  gcb::loss_partials_kernel<<<(n_out + 127) / 128, 128, 0, st>>>(partial, n_out, channel_sums);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
 int gcb_toa_incident_solar_radiation(const float* table, int32_t n_times, int32_t bins,
                                      const float* sin_lat, const float* cos_lat,
                                      const float* cos_lon, const float* sin_lon, int32_t n_lat,

@@ -331,6 +331,96 @@ unpack_grid_outputs_kernel(const float* __restrict__ y, int ld_y, int n_out, lon
   }
 }
 
+// Fixed number of node groups of the loss reduction: every device splits the node tiles the same
+// way, so the fp64 partial sums -- and the result -- are bit-identical on any GPU.
+constexpr int kLossGroups = 512;
+
+// Latitude-weighted squared error of the raw outputs against normalised targets (the loss of
+// normalization.InputsAndResiduals / GraphCast.loss_and_predictions), per channel:
+//   t_norm = ((target - add) - offset) / scale           (fp32, true division)
+//   partial[g, c] = sum over the node tiles of group g of lat_weight[node / n_lon] * (y - t_norm)^2
+// in fp64.  Same 32x32 transpose as unpack_grid_outputs_kernel (y is node-major, the target and
+// prediction planes channel-major); `planes_out` (optional) receives exactly what that kernel
+// writes, from the same expression.  Block (g, channel tile) walks the node tiles g, g + G, ... in
+// order; each warp owns four channels and folds its 32 lanes with a fixed butterfly.  No atomics.
+__global__ void __launch_bounds__(256)
+output_loss_kernel(const float* __restrict__ y, int ld_y, int n_out, int n_lon, long long n_nodes,
+                   const float* __restrict__ scale, const float* __restrict__ offset,
+                   const float* __restrict__ add_planes, const int* __restrict__ add_plane_index,
+                   const float* __restrict__ targets, const float* __restrict__ lat_weight,
+                   float* __restrict__ planes_out, double* __restrict__ partial) {
+  __shared__ float tile[32][33];
+  const int c0 = blockIdx.y * 32;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const long long n_tiles = (n_nodes + 31) / 32;
+  // The thread's four channels c0 + ty + 8j: their constants once, outside the node loop.
+  float sc[4], of[4];
+  int ap[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int c = min(c0 + ty + 8 * j, n_out - 1);
+    sc[j] = scale ? scale[c] : 1.f;
+    of[j] = offset ? offset[c] : 0.f;
+    ap[j] = add_plane_index ? add_plane_index[c] : -1;
+  }
+  double acc[4] = {0.0, 0.0, 0.0, 0.0};
+  for (long long t = blockIdx.x; t < n_tiles; t += kLossGroups) {
+    const long long node0 = t * 32;
+    for (int r = ty; r < 32; r += 8) {
+      const long long node = node0 + r;
+      const int c = c0 + tx;
+      tile[r][tx] = (node < n_nodes && c < n_out) ? y[node * ld_y + c] : 0.f;
+    }
+    const long long node = node0 + tx;
+    // the plane reads of the tile, issued together
+    float tv[4], av[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int c = c0 + ty + 8 * j;
+      const bool ok = c < n_out && node < n_nodes;
+      tv[j] = ok ? targets[static_cast<long long>(c) * n_nodes + node] : 0.f;
+      av[j] = ok && ap[j] >= 0 ? add_planes[static_cast<long long>(ap[j]) * n_nodes + node] : 0.f;
+    }
+    const double w = node < n_nodes ? static_cast<double>(lat_weight[node / n_lon]) : 0.0;
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int c = c0 + ty + 8 * j;
+      if (c < n_out && node < n_nodes) {
+        const float raw = tile[tx][ty + 8 * j];
+        // the prediction: the expression of unpack_grid_outputs_kernel, same operations in order
+        float v = raw;
+        if (scale) v *= sc[j];
+        if (offset) v += of[j];
+        if (ap[j] >= 0) v += av[j];
+        if (planes_out) planes_out[static_cast<long long>(c) * n_nodes + node] = v;
+        const float t_norm = __fdiv_rn(__fsub_rn(__fsub_rn(tv[j], av[j]), of[j]), sc[j]);
+        const double d = static_cast<double>(__fsub_rn(raw, t_norm));
+        acc[j] += w * (d * d);
+      }
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    double s = acc[j];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    const int c = c0 + ty + 8 * j;
+    if (tx == 0 && c < n_out) partial[static_cast<long long>(blockIdx.x) * n_out + c] = s;
+  }
+}
+
+// channel_sums[c] = sum over g = 0..kLossGroups-1 (in this order) of partial[g, c].
+__global__ void __launch_bounds__(128)
+loss_partials_kernel(const double* __restrict__ partial, int n_out, double* __restrict__ channel_sums) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_out) return;
+  double s = 0.0;
+  for (int g = 0; g < kLossGroups; ++g) s += partial[static_cast<long long>(g) * n_out + c];
+  channel_sums[c] = s;
+}
+
 // img[r, 0:k] = sum_{j<fan} src[r*fan + j, 0:k] written as an operand image (bf16 hi/lo
 // in the tensor-core A layout, see gcb_layer_desc).  A block handles 32 output rows:
 // phase 1 sums the fan input rows with coalesced float4 reads into a padded shared tile,

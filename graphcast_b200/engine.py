@@ -58,6 +58,7 @@ class Engine:
                        f"{sorted(_native.PRECISIONS)}")
     self._lib = _native.lib()            # raises if the CUDA library is missing
     self._step_stream = None             # created on first use (see step)
+    self._loss_workspace = None          # fp64 partial sums of output_loss, created on first use
     if not torch.cuda.is_available():
       raise RuntimeError("graphcast_b200 requires a CUDA device (no CPU fallback)")
     self.device = torch.device(device if device is not None else
@@ -422,6 +423,43 @@ class Engine:
           self._ptr(add_planes), self._ptr(add_plane_index), planes_out.data_ptr(), self._stream()),
           "gcb_unpack_grid_outputs")
     return planes_out
+
+  def output_loss(self, targets_planes: torch.Tensor, lat_weight: torch.Tensor, *,
+                  channel_sums: torch.Tensor, scale: Optional[torch.Tensor] = None,
+                  offset: Optional[torch.Tensor] = None, add_planes: Optional[torch.Tensor] = None,
+                  add_plane_index: Optional[torch.Tensor] = None,
+                  planes_out: Optional[torch.Tensor] = None,
+                  grid_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Latitude-weighted squared error of grid_out against the normalised targets, per output
+    channel, into `channel_sums` ([n_out] fp64 device slice; see gcb_output_loss).  Optionally
+    writes the predictions to `planes_out` as unpack_outputs would.  Launches on the current stream
+    and does not synchronise, so a multi-step loss stays on the device until it is read."""
+    if self.num_grid_owned:
+      raise NotImplementedError(
+          "the loss is not available in the node-partitioned engine: each rank holds only its own "
+          "grid rows; evaluate it with a single-GPU GraphCast")
+    grid_out = self.grid_out if grid_out is None else grid_out
+    n_lat = lat_weight.shape[0]
+    if n_lat == 0 or self.num_grid % n_lat:
+      raise ValueError(f"{n_lat} latitude weights do not tile {self.num_grid} grid nodes")
+    for name, t, dt, shape in (("targets_planes", targets_planes, torch.float32, (self.n_out, self.num_grid)),
+                               ("lat_weight", lat_weight, torch.float32, (n_lat,)),
+                               ("channel_sums", channel_sums, torch.float64, (self.n_out,)),
+                               ("planes_out", planes_out, torch.float32, (self.n_out, self.num_grid))):
+      if t is not None and (tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous()
+                            or t.device != self.device):
+        raise ValueError(f"{name} must be a contiguous {dt} {list(shape)} tensor on {self.device}")
+    nbytes = self._lib.gcb_output_loss_workspace_bytes(self.n_out)
+    ws = self._loss_workspace
+    if ws is None or ws.numel() < nbytes:
+      ws = self._loss_workspace = torch.empty([nbytes], dtype=torch.uint8, device=self.device)
+    with self._on_device():
+      _native.check(self._lib.gcb_output_loss(
+          grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat, self._ptr(scale),
+          self._ptr(offset), self._ptr(add_planes), self._ptr(add_plane_index),
+          targets_planes.data_ptr(), lat_weight.data_ptr(), self._ptr(planes_out), ws.data_ptr(),
+          nbytes, channel_sums.data_ptr(), self._stream()), "gcb_output_loss")
+    return channel_sums
 
   def forward_features(self, grid_features: torch.Tensor) -> torch.Tensor:
     """Convenience for parity tests: grid_features [Ng, B, c_in] (the reference's

@@ -4,13 +4,15 @@ Same public surface as `weathernext/weathernext1_graph/graphcast.py`:
   ModelConfig (:115-142), TaskConfig (utils/task.py:21-28), CheckPoint (:145-151),
   TASK / TASK_13 / TASK_13_PRECIP_OUT (:86-112),
   GraphCast(model_config, task_config).__call__(inputs, targets_template,
-  forcings, is_training=False) -> Dataset (:184, :298-329).
+  forcings, is_training=False) -> Dataset (:184, :298-329),
+  loss / loss_and_predictions(inputs, targets, forcings) (:331-366).
 
 What differs is only *how* the step is computed: the three GNN calls
 (`_run_grid2mesh_gnn` :550, `_run_mesh_gnn` :606, `_run_mesh2grid_gnn` :641) and
 the channel (un)packing (`_inputs_to_grid_node_features` :680,
 `_grid_node_outputs_to_prediction` :701) run as hand-written sm_90a kernels
-behind the C ABI in include/graphcast_b200.h.  There is no CPU path: without a
+behind the C ABI in include/graphcast_b200.h, and so does the loss's reduction
+(`gcb_output_loss`, fused into the output unpack).  There is no CPU path: without a
 CUDA device or the built library this module raises.
 
 Parameters: the reference threads a Haiku parameter dict through
@@ -31,6 +33,7 @@ import torch
 
 from graphcast_b200 import engine as engine_lib
 from graphcast_b200 import graph as graph_lib
+from graphcast_b200 import losses
 from graphcast_b200 import model_utils
 from graphcast_b200 import variables
 from graphcast_b200 import xarray_shim as xs
@@ -90,10 +93,22 @@ class Predictor(abc.ABC):
     """Returns predictions shaped like `targets_template`."""
 
   def loss(self, inputs, targets, forcings, **optional_kwargs):
-    raise NotImplementedError("training losses are outside the inference hot path")
+    """Returns (loss, diagnostics): `(batch,)` DataArray and Dataset of per-variable losses."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement a loss")
 
   def loss_and_predictions(self, inputs, targets, forcings, **optional_kwargs):
-    raise NotImplementedError("training losses are outside the inference hot path")
+    """Returns ((loss, diagnostics), predictions)."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement a loss")
+
+
+# Per-variable weights of GraphCast's loss (reference graphcast.py:341-356); others weigh 1.
+LOSS_PER_VARIABLE_WEIGHTS = {
+    "2m_temperature": 1.0,
+    "10m_u_component_of_wind": 0.1,
+    "10m_v_component_of_wind": 0.1,
+    "mean_sea_level_pressure": 0.1,
+    "total_precipitation_6hr": 0.1,
+}
 
 
 def num_outputs(task_config: TaskConfig) -> int:
@@ -148,6 +163,11 @@ class GraphCast(Predictor):
     self._planes_bufs: List[Optional[torch.Tensor]] = [None, None]
     self._buf_free: List[Optional[torch.cuda.Event]] = [None, None]
     self._call_index = 0
+    # The loss: target planes staged like the inputs (same slots, same events), the latitude
+    # weights of the last target grid, the per-channel sums of the last call.
+    self._target_bufs: List[Optional[torch.Tensor]] = [None, None]
+    self._lat_weight_cache = None
+    self._channel_sums: Optional[torch.Tensor] = None
 
   # -- parameters ------------------------------------------------------------------
   def set_params(self, params: Mapping[str, Mapping[str, np.ndarray]]) -> None:
@@ -199,13 +219,65 @@ class GraphCast(Predictor):
                **unused_kwargs):
     return self._call(inputs, targets_template, forcings, norm=None)
 
+  # -- the loss (reference loss_and_predictions / loss :331-366) ------------------------
+  def loss_and_predictions(self, inputs, targets, forcings, **unused_kwargs):
+    """((loss, diagnostics), predictions): the step, then `losses.weighted_mse_per_level` of the
+    predictions against `targets` with GraphCast's per-variable weights.  The error is reduced on the
+    device in the kernel that unpacks the outputs (gcb_output_loss: fp32 differences, fp64 sums)."""
+    return self._loss(inputs, targets, forcings, norm=None, predictions=True)
+
+  def loss(self, inputs, targets, forcings, **unused_kwargs):
+    """(loss, diagnostics) of `loss_and_predictions`; the predictions are not materialised."""
+    return self._loss(inputs, targets, forcings, norm=None, predictions=False)[0]
+
+  def _loss(self, inputs, targets, forcings, norm: Optional[FusedNormalization], predictions: bool):
+    finish, preds, sums = self._device_loss(inputs, targets, forcings, norm, predictions)
+    return finish(sums.cpu().numpy()), preds
+
+  def _device_loss(self, inputs, targets, forcings, norm: Optional[FusedNormalization],
+                   predictions: bool):
+    """Queues one step with the fused loss of every batch element and returns
+    (finish, predictions or None, channel_sums): `channel_sums` [batch, n_out] fp64 on the device
+    receives the latitude-weighted squared-error sums of gcb_output_loss, and
+    finish(host copy of those sums) -> (loss, diagnostics).  Nothing is synchronised here, so a
+    multi-step loss reads all its sums back once."""
+    targets = xs.from_xarray(targets)
+    preds = self._call(inputs, targets, forcings, norm=norm, targets=targets,
+                       predictions=predictions)
+    slabs = model_utils.channel_layout(targets)
+    num_grid = self._engine.num_grid
+    finish = lambda sums: losses.losses_from_channel_sums(sums, slabs, num_grid,
+                                                          LOSS_PER_VARIABLE_WEIGHTS)
+    return finish, preds, self._channel_sums
+
+  def _lat_weight(self, targets: xs.Dataset, device) -> torch.Tensor:
+    """Normalised latitude weights of the targets' grid (float32, on the device), cached."""
+    name = sorted(targets.data_vars.keys())[0]
+    w = losses.normalized_latitude_weights(targets[name])
+    w = np.ascontiguousarray(w, np.float32)
+    key = (w.tobytes(), str(device))
+    if self._lat_weight_cache is None or self._lat_weight_cache[0] != key:
+      self._lat_weight_cache = (key, torch.as_tensor(w).to(device))
+    return self._lat_weight_cache[1]
+
   def _channel_plan(self, inputs: xs.Dataset, forcings: xs.Dataset):
     in_slabs = model_utils.channel_layout(inputs)
     n_in = sum(s.count for s in in_slabs)
     f_slabs = model_utils.channel_layout(forcings, start=n_in)
     return in_slabs, f_slabs, n_in + sum(s.count for s in f_slabs)
 
-  def _call(self, inputs, targets_template, forcings, norm: Optional[FusedNormalization]):
+  def _staging(self, bufs: List[Optional[torch.Tensor]], buf: int, shape) -> Tuple[torch.Tensor, bool]:
+    fresh = bufs[buf] is None or bufs[buf].shape != shape
+    if fresh:
+      bufs[buf] = torch.empty(list(shape), dtype=torch.float32, device=self._engine.device)
+    return bufs[buf], fresh
+
+  def _call(self, inputs, targets_template, forcings, norm: Optional[FusedNormalization],
+            targets: Optional[xs.Dataset] = None, predictions: bool = True):
+    """The step for every batch element.  With `targets` (shaped like the template, usually the
+    same Dataset) the outputs go through gcb_output_loss instead of the plain unpack: the loss sums
+    land in a new [batch, n_out] fp64 device tensor, self._channel_sums, and the predictions are
+    returned only when `predictions` is set (else None)."""
     inputs = xs.from_xarray(inputs)
     forcings = xs.from_xarray(forcings)
     targets_template = xs.from_xarray(targets_template)
@@ -218,44 +290,56 @@ class GraphCast(Predictor):
     n_lat, n_lon = sizes["lat"], sizes["lon"]
     if n_lat * n_lon != eng.num_grid:
       raise ValueError("inputs lat/lon grid differs from the grid the model was built on")
+    if targets is not None:
+      t_slabs = self._check_template(targets, eng.n_out)
+      lat_weight = self._lat_weight(targets, eng.device)
+      if lat_weight.shape[0] != n_lat:
+        raise ValueError(f"targets have {lat_weight.shape[0]} latitudes, the inputs {n_lat}")
+      channel_sums = torch.empty([batch, eng.n_out], dtype=torch.float64, device=eng.device)
+      self._channel_sums = channel_sums
 
     # xarray -> channel-major planes [B, C, lat*lon] on the device
-    # (reference _inputs_to_grid_node_features :680-699; dataset_to_stacked order).
+    # (reference _inputs_to_grid_node_features :680-699; dataset_to_stacked order); the targets of a
+    # loss are staged the same way, in the order of the predictions' channels.
     buf = self._call_index % 2
     self._call_index += 1
-    fresh = self._planes_bufs[buf] is None or self._planes_bufs[buf].shape != (batch, c_in, eng.num_grid)
-    if fresh:
-      self._planes_bufs[buf] = torch.empty([batch, c_in, eng.num_grid], dtype=torch.float32,
-                                           device=eng.device)
-      self._buf_free[buf] = None
-    planes_in = self._planes_bufs[buf]
+    planes_in, fresh = self._staging(self._planes_bufs, buf, (batch, c_in, eng.num_grid))
     self._planes_in = planes_in
+    jobs = [(planes_in, inputs, in_slabs), (planes_in, forcings, f_slabs)]
+    staged = [(planes_in, fresh)]
+    if targets is not None:
+      planes_tgt, fresh_tgt = self._staging(self._target_bufs, buf, (batch, eng.n_out, eng.num_grid))
+      jobs.append((planes_tgt, targets, t_slabs))
+      staged.append((planes_tgt, fresh_tgt))
+    if all(f for _, f in staged):
+      self._buf_free[buf] = None
     sources = []
-    for ds, slabs in ((inputs, in_slabs), (forcings, f_slabs)):
+    for dst_planes, ds, slabs in jobs:
       for s in slabs:
         src = model_utils.variable_to_planes(ds.data_vars[s.name], sizes)
         if not isinstance(src, torch.Tensor):
           src = torch.from_numpy(np.ascontiguousarray(src, dtype=np.float32))
-        sources.append((s, src))
+        sources.append((dst_planes, s, src))
     compute = torch.cuda.current_stream(eng.device)
-    all_host = all(src.device.type == "cpu" for _, src in sources)
+    all_host = all(src.device.type == "cpu" for _, _, src in sources)
     if all_host:
       if self._h2d_stream is None:
         self._h2d_stream = torch.cuda.Stream(device=eng.device)
       copy_stream = self._h2d_stream
-      if fresh:
-        # The caching allocator may hand back a block whose previous user still has kernels
-        # queued on the compute stream: order the first copy after them, and tell the allocator
-        # that the copy stream uses this block too.
-        copy_stream.wait_stream(compute)
-        planes_in.record_stream(copy_stream)
+      for planes, f in staged:
+        if f:
+          # The caching allocator may hand back a block whose previous user still has kernels
+          # queued on the compute stream: order the first copy after them, and tell the allocator
+          # that the copy stream uses this block too.
+          copy_stream.wait_stream(compute)
+          planes.record_stream(copy_stream)
       if self._buf_free[buf] is not None:
         copy_stream.wait_event(self._buf_free[buf])      # kernels of call k-2 are done with it
     else:
       copy_stream = compute                              # device-resident inputs: stay in order
     with torch.cuda.stream(copy_stream):
-      for s, src in sources:
-        dst = planes_in[:, s.start:s.start + s.count].view(batch, s.count, n_lat, n_lon)
+      for dst_planes, s, src in sources:
+        dst = dst_planes[:, s.start:s.start + s.count].view(batch, s.count, n_lat, n_lon)
         dst.copy_(src, non_blocking=True)
       if all_host:
         ready = torch.cuda.Event()
@@ -264,10 +348,23 @@ class GraphCast(Predictor):
       compute.wait_event(ready)
 
     # Predictions are produced into fresh planes each call (they are handed out).
-    planes_out = torch.empty([batch, eng.n_out, eng.num_grid], dtype=torch.float32,
-                             device=eng.device)
+    planes_out = None
+    if predictions:
+      planes_out = torch.empty([batch, eng.n_out, eng.num_grid], dtype=torch.float32,
+                               device=eng.device)
     for b in range(batch):
-      if norm is None:
+      if targets is not None:
+        affine = {} if norm is None else dict(
+            scale=norm.out_scale, offset=norm.out_offset, add_planes=planes_in[b],
+            add_plane_index=norm.add_plane_index)
+        if norm is None:
+          eng.pack_inputs(planes_in[b])
+        else:
+          eng.pack_inputs(planes_in[b], mean=norm.in_mean, scale=norm.in_scale)
+        eng.step()
+        eng.output_loss(planes_tgt[b], lat_weight, channel_sums=channel_sums[b],
+                        planes_out=None if planes_out is None else planes_out[b], **affine)
+      elif norm is None:
         eng.pack_inputs(planes_in[b])
         eng.step()
         eng.unpack_outputs(planes_out[b])
@@ -280,12 +377,15 @@ class GraphCast(Predictor):
     free.record(compute)
     self._buf_free[buf] = free
 
+    if planes_out is None:
+      return None
     # planes -> Dataset shaped like the template
     # (reference _grid_node_outputs_to_prediction :701-723, stacked_to_dataset).
     return self._planes_to_dataset(planes_out, targets_template, n_lat, n_lon)
 
-  def _planes_to_dataset(self, planes_out: torch.Tensor, template: xs.Dataset,
-                         n_lat: int, n_lon: int) -> xs.Dataset:
+  @staticmethod
+  def _check_template(template: xs.Dataset, n_channels: int):
+    """Channel slabs of `template`, with stacked_to_dataset's two errors (model_utils.py:713-776)."""
     preserved = ("batch", "lat", "lon")
     for name in sorted(template.data_vars.keys()):
       tv = template.data_vars[name]
@@ -295,9 +395,14 @@ class GraphCast(Predictor):
             f"dimensions, but found only {tv.dims}.")
     slabs = model_utils.channel_layout(template)
     expected = sum(s.count for s in slabs)
-    if expected != planes_out.shape[1]:
-      raise ValueError(f"Expected {expected} channels but found {planes_out.shape[1]}, when "
+    if expected != n_channels:
+      raise ValueError(f"Expected {expected} channels but found {n_channels}, when "
                        f"trying to convert the model output to a dataset of shape {template}.")
+    return slabs
+
+  def _planes_to_dataset(self, planes_out: torch.Tensor, template: xs.Dataset,
+                         n_lat: int, n_lon: int) -> xs.Dataset:
+    slabs = self._check_template(template, planes_out.shape[1])
     batch = planes_out.shape[0]
     out = xs.Dataset(coords=template.coords)
     for s in slabs:

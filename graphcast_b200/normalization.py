@@ -13,6 +13,13 @@ applied to the Datasets at all: they are folded into per-channel vectors and
 executed inside the pack / unpack kernels (`gcb_pack_grid_features`,
 `gcb_unpack_grid_outputs`), which removes three full passes over the 0.25 degree
 state per step.  Any other predictor gets the generic Dataset arithmetic.
+
+`loss` / `loss_and_predictions` (reference :134-146, :162-196) score the inner predictor in normalised
+space: targets that are also inputs become (target - last input frame) / diffs_std, the others
+(target - mean) / std, and the inner predictor's raw output is compared with them;
+`loss_and_predictions` returns un-normalised predictions.  Around `GraphCast` the same per-channel
+vectors normalise the targets inside the loss kernel (`gcb_output_loss`), so the normalised targets
+are never built as Datasets.
 """
 
 from __future__ import annotations
@@ -198,3 +205,56 @@ class InputsAndResiduals(graphcast.Predictor):
                                        **kwargs)
     return norm_predictions.map(
         lambda pred: self._unnormalize_prediction_and_add_input(inputs, pred))
+
+  # -- the loss, in normalised space (reference :134-146, :162-196) -------------------
+  def _subtract_input_and_normalize_target(self, inputs, target):
+    if target.sizes.get("time") != 1:
+      raise ValueError("normalization.InputsAndResiduals only supports wrapping predictors"
+                       "that predict a single timestep.")
+    if target.name in inputs:
+      residual = target - inputs[target.name].isel(time=-1)
+      return normalize(xs.Dataset({target.name: residual}), self._residual_scales,
+                       self._residual_locations)[target.name]
+    return normalize(xs.Dataset({target.name: target}), self._scales, self._locations)[target.name]
+
+  def _normalized(self, inputs, targets, forcings):
+    return (normalize(inputs, self._scales, self._locations),
+            targets.map(lambda t: self._subtract_input_and_normalize_target(inputs, t)),
+            normalize(forcings, self._scales, self._locations))
+
+  def _fuses(self) -> bool:
+    return isinstance(self._predictor, graphcast.GraphCast)
+
+  def _device_loss(self, inputs, targets, forcings, predictions: bool):
+    """GraphCast only: the step with the fused loss (graphcast.GraphCast._device_loss), the
+    target normalisation applied inside the kernel from the fused constants."""
+    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
+    targets = xs.from_xarray(targets)
+    device = self._predictor._device or f"cuda:{torch.cuda.current_device()}"
+    consts = self._fused_constants(inputs, targets, forcings, torch.device(device))
+    return self._predictor._device_loss(inputs, targets, forcings, consts, predictions)
+
+  def loss(self, inputs, targets, forcings, **kwargs):
+    """The loss computed on normalised inputs and targets (targets that are also inputs as
+    normalised residuals against the last input frame)."""
+    if self._fuses():
+      finish, _, sums = self._device_loss(inputs, targets, forcings, predictions=False)
+      return finish(sums.cpu().numpy())
+    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
+    norm_inputs, norm_targets, norm_forcings = self._normalized(inputs, xs.from_xarray(targets),
+                                                                forcings)
+    return self._predictor.loss(norm_inputs, norm_targets, forcings=norm_forcings, **kwargs)
+
+  def loss_and_predictions(self, inputs, targets, forcings, **kwargs):
+    """The loss computed on normalised data, with un-normalised predictions."""
+    if self._fuses():
+      finish, predictions, sums = self._device_loss(inputs, targets, forcings, predictions=True)
+      return finish(sums.cpu().numpy()), predictions
+    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
+    norm_inputs, norm_targets, norm_forcings = self._normalized(inputs, xs.from_xarray(targets),
+                                                                forcings)
+    (loss, diagnostics), norm_predictions = self._predictor.loss_and_predictions(
+        norm_inputs, norm_targets, forcings=norm_forcings, **kwargs)
+    predictions = norm_predictions.map(
+        lambda pred: self._unnormalize_prediction_and_add_input(inputs, pred))
+    return (loss, diagnostics), predictions

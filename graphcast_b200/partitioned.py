@@ -188,6 +188,11 @@ class PartitionedEngine:
     self.skip_exchange = False      # measurement aid (bench.py): time a step without exchanges
     self._events = []
 
+  def output_loss(self, *args, **kwargs):
+    """Not provided: a rank holds only its own grid rows, and the loss is a mean over all of them."""
+    raise NotImplementedError("the loss is not available in the node-partitioned engine; "
+                              "evaluate it with a single-GPU GraphCast")
+
   def exchange_halo(self, timed: bool = False) -> None:
     """Owned boundary rows of mesh_lat -> the halo rows of the peers that need them; then the
     halo part of the operand image is rebuilt."""

@@ -208,6 +208,30 @@ int gcb_unpack_grid_outputs(const float* y, int32_t ld_y, int32_t n_out, int64_t
                             const float* add_planes, const int32_t* add_plane_index,
                             float* planes_out, void* stream);
 
+/* Forecast loss of one batch element, fused into the output transpose: per output channel c,
+ *   channel_sums[c] = sum over nodes of lat_weight[node / n_lon] * (y[node, c] - t_norm)^2
+ *   t_norm          = ((targets[c, node] - add) - offset[c]) / scale[c]        (fp32, true division)
+ * with add = add_planes[add_plane_index[c], node] (0 when the index is < 0 or NULL), offset = 0 and
+ * scale = 1 when NULL: the targets normalised exactly as normalization.InputsAndResiduals normalises
+ * them ((t - last input frame) / diffs_std or (t - mean) / std), compared with the RAW outputs.  The
+ * difference is fp32, the weighted squares and their sums fp64.  Reference semantics:
+ * losses.weighted_mse_per_level (weathernext/utils/losses.py:85-132) before its division by the
+ * element count and its level / variable weights, which the caller applies per variable.
+ *   y            [n_lat * n_lon, ld_y] decoder output (as gcb_unpack_grid_outputs)
+ *   targets      [n_out, n_lat * n_lon] un-normalised target planes (device)
+ *   lat_weight   [n_lat] latitude weights, normalised to mean 1 (device, fp32)
+ *   planes_out   optional: also the predictions, bit-identical to gcb_unpack_grid_outputs
+ *   workspace    gcb_output_loss_workspace_bytes(n_out) bytes, 8-byte aligned
+ *   channel_sums [n_out] fp64 (device)
+ * Deterministic: a fixed split of the nodes into groups, fixed-order fp64 reductions, no atomics --
+ * bit-identical run to run and on any device.  Two launches on `stream`. */
+int gcb_output_loss(const float* y, int32_t ld_y, int32_t n_out, int32_t n_lat, int32_t n_lon,
+                    const float* scale, const float* offset, const float* add_planes,
+                    const int32_t* add_plane_index, const float* targets, const float* lat_weight,
+                    float* planes_out, void* workspace, int64_t workspace_bytes,
+                    double* channel_sums, void* stream);
+int64_t gcb_output_loss_workspace_bytes(int32_t n_out);
+
 /* ---- fused layer chains ---------------------------------------------------------------
  * A CHAIN runs up to GCB_MAX_CHAIN fused layers over the same `rows` rows in ONE kernel: a
  * cluster pair owns a 128-row tile and takes it through layer 0, 1, ... while the intermediate
@@ -421,7 +445,8 @@ int gcb_set_graph_replay(int32_t enabled);
  * Not thread safe. */
 typedef enum {
   GCB_KIND_LAYER_TC = 0, GCB_KIND_SEGMENT_SUM = 1, GCB_KIND_PACK = 2, GCB_KIND_UNPACK = 3,
-  GCB_KIND_LAYER_SIMT = 4, GCB_KIND_ROWS_TO_IMAGE = 5, GCB_KIND_CHAIN_TC = 6, GCB_KIND_GATHER = 7
+  GCB_KIND_LAYER_SIMT = 4, GCB_KIND_ROWS_TO_IMAGE = 5, GCB_KIND_CHAIN_TC = 6, GCB_KIND_GATHER = 7,
+  GCB_KIND_LOSS = 8         /* gcb_output_loss (both of its launches) */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
 int gcb_profile_end(int32_t capacity, int32_t* kinds, float* ms, double* flops, double* bytes,
