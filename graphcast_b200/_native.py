@@ -134,6 +134,23 @@ EXPORTS = {
     "gcb_output_loss": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp, _fp,
                                   _fp, _fp, _fp, _fp, _fp, C.c_int64, _fp, _fp]),
     "gcb_output_loss_workspace_bytes": (C.c_int64, [C.c_int32]),
+    "gcb_output_loss_grad": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp,
+                                       _fp, _fp, _fp, _fp, _fp, _fp, C.c_int32, _fp]),
+    "gcb_weight_grad_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
+    "gcb_weight_grad": (C.c_int, [_fp, C.c_int32, C.c_int32, _fp, C.c_int32, _fp, C.c_int32,
+                                  C.c_int64, C.c_int32, C.c_int32, C.c_int32, _fp, C.c_int64, _fp,
+                                  C.c_int32, _fp]),
+    "gcb_rowwise_workspace_bytes": (C.c_int64, [C.c_int32]),
+    "gcb_layernorm_backward": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, _fp, C.c_int64, C.c_int32,
+                                         _fp, C.c_int32, _fp, C.c_int64, _fp, _fp, _fp, C.c_int32,
+                                         _fp]),
+    "gcb_swish_backward": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, C.c_int64, C.c_int32, _fp,
+                                     C.c_int32, _fp, C.c_int64, _fp, C.c_int32, _fp]),
+    "gcb_segment_sum_sorted": (C.c_int, [_fp, C.c_int32, _fp, _fp, C.c_int32, _fp, C.c_int32, _fp,
+                                         C.c_int32, C.c_int32, _fp]),
+    "gcb_swish_rows": (C.c_int, [_fp, C.c_int32, C.c_int64, C.c_int32, _fp, C.c_int32, _fp]),
+    "gcb_gather_add": (C.c_int, [_fp, C.c_int32, _fp, C.c_int64, _fp, C.c_int32, _fp, C.c_int32,
+                                 C.c_int32, _fp]),
     "gcb_forward":(C.c_int, [C.POINTER(Model), _fp, _fp, _fp, C.POINTER(C.c_int32)]),
     "gcb_forward_stage": (C.c_int, [C.POINTER(Model), C.c_int32, C.c_int32, _fp, _fp, _fp,
                                     C.POINTER(C.c_int32)]),

@@ -113,6 +113,16 @@ class Predictor(graphcast.Predictor):
       records = [finish(sums[t]) for t, (finish, _) in enumerate(records)]
     return _mean_over_time([l for l, _ in records], [d for _, d in records])
 
+  def loss_and_grads(self, inputs, targets, forcings, **kwargs):
+    """(loss, diagnostics, grads) of the underlying predictor for ONE target time.  Several target
+    times would need the gradient through the fed-back predictions (backprop through time), which is
+    not implemented."""
+    targets = xs.from_xarray(targets)
+    if targets.sizes["time"] != 1:
+      raise NotImplementedError("loss_and_grads supports one target time; backprop through time "
+                                "(several target times) is not implemented")
+    return self._predictor.loss_and_grads(inputs, targets, forcings, **kwargs)
+
 
 def _mean_over_time(step_losses, step_diagnostics):
   """Mean over the steps of `(batch,)` losses and diagnostics (NaNs propagate)."""

@@ -62,3 +62,6 @@ class Bfloat16Cast(graphcast.Predictor):
 
   def loss_and_predictions(self, inputs, targets, forcings, **kwargs):
     return self._predictor.loss_and_predictions(inputs, targets, forcings, **kwargs)
+
+  def loss_and_grads(self, inputs, targets, forcings, **kwargs):
+    return self._predictor.loss_and_grads(inputs, targets, forcings, **kwargs)

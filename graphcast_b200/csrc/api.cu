@@ -14,6 +14,7 @@
 #include "mlp_simt.cuh"
 #include "mlp_tc.cuh"
 #include "mlp_chain.cuh"
+#include "backward_kernels.cuh"
 
 namespace {
 
@@ -796,6 +797,193 @@ int gcb_output_loss(const float* y, int32_t ld_y, int32_t n_out, int32_t n_lat, 
                                                planes_out, partial);
   GCB_CUDA(cudaGetLastError());
   gcb::loss_partials_kernel<<<(n_out + 127) / 128, 128, 0, st>>>(partial, n_out, channel_sums);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+// ---- parameter gradients ---------------------------------------------------------------------
+int gcb_output_loss_grad(const float* y, int32_t ld_y, int32_t n_out, int32_t n_lat, int32_t n_lon,
+                         const float* scale, const float* offset, const float* add_planes,
+                         const int32_t* add_plane_index, const float* targets,
+                         const float* lat_weight, const double* coef, float* g, int32_t ld_g,
+                         void* stream) {
+  GCB_CHECK_ARG(y && targets && lat_weight && coef && g, "null pointer");
+  GCB_CHECK_ARG(n_out > 0 && ld_y >= n_out && ld_g >= n_out, "ld_y / ld_g too small");
+  GCB_CHECK_ARG(n_lat > 0 && n_lon > 0, "empty grid");
+  GCB_CHECK_ARG((add_planes == nullptr) == (add_plane_index == nullptr), "add_planes/index mismatch");
+  const long long n_nodes = static_cast<long long>(n_lat) * n_lon;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * n_nodes * n_out * (3.0 + (add_planes ? 1.0 : 0.0)));
+  dim3 grid(static_cast<unsigned>((n_nodes + 31) / 32), static_cast<unsigned>((n_out + 31) / 32));
+  gcb::output_loss_grad_kernel<<<grid, 256, 0, st>>>(y, ld_y, n_out, n_lon, n_nodes, scale, offset,
+                                                    add_planes, add_plane_index, targets, lat_weight,
+                                                    coef, g, ld_g);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int64_t gcb_weight_grad_workspace_bytes(int32_t k, int32_t n) {
+  if (k <= 0 || n <= 0) return -1;
+  return static_cast<int64_t>(gcb::kWgSlices) * k * n * static_cast<int64_t>(sizeof(float));
+}
+
+int gcb_weight_grad(const float* x, int32_t ld_x, int32_t k_valid, const void* x_img, int32_t x_swish,
+                    const float* g, int32_t ld_g, int64_t rows, int32_t k, int32_t n,
+                    int32_t precision, void* workspace, int64_t workspace_bytes, float* dw,
+                    int32_t accumulate, void* stream) {
+  GCB_CHECK_ARG(g && dw && workspace, "null pointer");
+  GCB_CHECK_ARG(k > 0 && k % 16 == 0 && n > 0 && n % 64 == 0, "k must be a multiple of 16, n of 64");
+  GCB_CHECK_ARG(rows >= 0, "rows < 0");
+  GCB_CHECK_ARG(ld_g % 4 == 0 && ld_g >= n && aligned16(g), "G must have 16-byte rows and ld_g >= n");
+  if (x_img) {
+    GCB_CHECK_ARG(aligned16(x_img), "x_img unaligned");
+  } else {
+    GCB_CHECK_ARG(x && aligned16(x) && ld_x % 4 == 0 && k_valid > 0 && k_valid % 4 == 0 &&
+                      k_valid <= k && ld_x >= k_valid,
+                  "x must have 16-byte rows, k_valid a multiple of 4 in (0, k]");
+  }
+  GCB_CHECK_ARG(precision == GCB_PREC_BF16X3 || precision == GCB_PREC_BF16,
+                "weight gradients support the tensor-core precisions only");
+  GCB_CHECK_ARG(workspace_bytes >= gcb_weight_grad_workspace_bytes(k, n), "workspace too small");
+  GCB_CHECK_ARG(aligned16(workspace), "workspace unaligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const double macs = static_cast<double>(rows) * k * n;
+  ProfScope prof(st, GCB_KIND_WGRAD, 2.0 * macs,   // algorithmic, as for the layers
+                 4.0 * static_cast<double>(rows) * (k + n) + 8.0 * gcb::kWgSlices * k * n);
+  float* partial = static_cast<float*>(workspace);
+  dim3 grid(static_cast<unsigned>(n / gcb::kWgBN), static_cast<unsigned>((k + gcb::kWgBM - 1) / gcb::kWgBM),
+            gcb::kWgSlices);
+  const unsigned char* img = static_cast<const unsigned char*>(x_img);
+  if (precision == GCB_PREC_BF16X3)
+    gcb::weight_grad_kernel<true><<<grid, 128, 0, st>>>(x, ld_x, k_valid, img, k, x_swish, g, ld_g,
+                                                        rows, k, n, partial);
+  else
+    gcb::weight_grad_kernel<false><<<grid, 128, 0, st>>>(x, ld_x, k_valid, img, k, x_swish, g, ld_g,
+                                                         rows, k, n, partial);
+  GCB_CUDA(cudaGetLastError());
+  const long long count = static_cast<long long>(k) * n;
+  gcb::slices_reduce_kernel<<<static_cast<unsigned>((count + 255) / 256), 256, 0, st>>>(
+      partial, gcb::kWgSlices, count, count, dw, accumulate);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int64_t gcb_rowwise_workspace_bytes(int32_t n) {
+  if (n <= 0) return -1;
+  return static_cast<int64_t>(gcb::kRowSlices) * 3 * n * static_cast<int64_t>(sizeof(float));
+}
+
+namespace {
+int rowwise_launch(int mode, const float* dy, int32_t ld_dy, const float* z, int32_t ld_z,
+                   const float* scale, int64_t rows, int32_t n, float* dz, int32_t ld_dz,
+                   void* workspace, int64_t workspace_bytes, float* const* sums, int nsums,
+                   int32_t accumulate, void* stream) {
+  GCB_CHECK_ARG(dy && workspace && rows >= 0, "null pointer");
+  GCB_CHECK_ARG(n == 256 || n == 512, "n must be 256 or 512");
+  GCB_CHECK_ARG(ld_dy >= n && (!z || ld_z >= n) && (!dz || ld_dz >= n), "leading dimension < n");
+  GCB_CHECK_ARG(workspace_bytes >= gcb_rowwise_workspace_bytes(n), "workspace too small");
+  for (int q = 0; q < nsums; ++q) GCB_CHECK_ARG(sums[q] != nullptr, "null column-sum output");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * static_cast<double>(rows) * n * (1.0 + (z ? 1.0 : 0.0) + (dz ? 1.0 : 0.0)));
+  float* partial = static_cast<float*>(workspace);
+#define GCB_ROWWISE(M, C)                                                                   \
+  gcb::rowwise_backward_kernel<M, C><<<gcb::kRowSlices, 256, 0, st>>>(dy, ld_dy, z, ld_z, scale, \
+                                                                       rows, dz, ld_dz, partial)
+  if (mode == gcb::kRowLayerNorm) {
+    GCB_CHECK_ARG(n == 512, "the LayerNorm backward needs n = 512");
+    GCB_ROWWISE(gcb::kRowLayerNorm, 16);
+  } else if (mode == gcb::kRowSwish) {
+    if (n == 512) GCB_ROWWISE(gcb::kRowSwish, 16); else GCB_ROWWISE(gcb::kRowSwish, 8);
+  } else {
+    if (n == 512) GCB_ROWWISE(gcb::kRowCopy, 16); else GCB_ROWWISE(gcb::kRowCopy, 8);
+  }
+#undef GCB_ROWWISE
+  GCB_CUDA(cudaGetLastError());
+  for (int q = 0; q < nsums; ++q) {
+    gcb::slices_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(partial + q * n, gcb::kRowSlices,
+                                                               static_cast<long long>(nsums) * n, n,
+                                                               sums[q], accumulate);
+    GCB_CUDA(cudaGetLastError());
+  }
+  return GCB_OK;
+}
+}  // namespace
+
+int gcb_layernorm_backward(const float* dy, int32_t ld_dy, const float* z, int32_t ld_z,
+                           const float* scale, int64_t rows, int32_t n, float* dz, int32_t ld_dz,
+                           void* workspace, int64_t workspace_bytes, float* dbias, float* dscale,
+                           float* doffset, int32_t accumulate, void* stream) {
+  if (scale) {
+    GCB_CHECK_ARG(z && dz, "the LayerNorm backward needs z and dz");
+    float* sums[3] = {dbias, dscale, doffset};
+    return rowwise_launch(gcb::kRowLayerNorm, dy, ld_dy, z, ld_z, scale, rows, n, dz, ld_dz,
+                          workspace, workspace_bytes, sums, 3, accumulate, stream);
+  }
+  float* sums[1] = {dbias};
+  return rowwise_launch(gcb::kRowCopy, dy, ld_dy, nullptr, 0, nullptr, rows, n, dz, ld_dz, workspace,
+                        workspace_bytes, sums, 1, accumulate, stream);
+}
+
+int gcb_swish_backward(const float* da, int32_t ld_da, const float* h, int32_t ld_h, int64_t rows,
+                       int32_t n, float* dh, int32_t ld_dh, void* workspace, int64_t workspace_bytes,
+                       float* dbias, int32_t accumulate, void* stream) {
+  GCB_CHECK_ARG(h && dh, "null pointer");
+  float* sums[1] = {dbias};
+  return rowwise_launch(gcb::kRowSwish, da, ld_da, h, ld_h, nullptr, rows, n, dh, ld_dh, workspace,
+                        workspace_bytes, sums, 1, accumulate, stream);
+}
+
+int gcb_segment_sum_sorted(const float* msg, int32_t ld_msg, const int32_t* order,
+                           const int32_t* ptr, int32_t num_nodes, const int32_t* heavy,
+                           int32_t num_heavy, float* out, int32_t ld_out, int32_t width, void* stream) {
+  GCB_CHECK_ARG(msg && order && ptr && out, "null pointer");
+  GCB_CHECK_ARG(num_heavy >= 0 && (num_heavy == 0 || heavy != nullptr), "heavy list is null");
+  GCB_CHECK_ARG(width == 512, "segment_sum_sorted supports width 512");
+  GCB_CHECK_ARG(ld_msg % 4 == 0 && ld_out % 4 == 0 && aligned16(msg) && aligned16(out), "unaligned");
+  if (num_nodes == 0) return GCB_OK;
+  long long light = (static_cast<long long>(num_nodes) + 7) / 8;
+  const long long cap = static_cast<long long>(sm_count_cached()) * 16;
+  if (light > cap) light = cap;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0, 4.0 * width * static_cast<double>(num_nodes));
+  gcb::segment_sum_sorted_kernel<<<static_cast<unsigned>(light) + num_heavy, 256, 0, st>>>(
+      msg, ld_msg, order, ptr, num_nodes, heavy, num_heavy, static_cast<int>(light), out, ld_out);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int gcb_swish_rows(const float* h, int32_t ld_h, int64_t rows, int32_t n, float* a, int32_t ld_a,
+                   void* stream) {
+  GCB_CHECK_ARG(h && a, "null pointer");
+  GCB_CHECK_ARG(n > 0 && n % 4 == 0 && ld_h % 4 == 0 && ld_a % 4 == 0 && ld_h >= n && ld_a >= n &&
+                    aligned16(h) && aligned16(a),
+                "n / leading dimensions must be multiples of 4 with 16-byte rows");
+  if (rows <= 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0, 8.0 * n * static_cast<double>(rows));
+  const long long total = rows * (n / 4);
+  gcb::swish_rows_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(h, ld_h, rows, n / 4,
+                                                                                     a, ld_a);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int gcb_gather_add(const float* src, int32_t ld_src, const int32_t* idx, int64_t n,
+                   const float* addend, int32_t ld_add, float* dst, int32_t ld_dst, int32_t width,
+                   void* stream) {
+  GCB_CHECK_ARG(src && idx && dst, "null pointer");
+  GCB_CHECK_ARG(width > 0 && width % 4 == 0 && ld_src % 4 == 0 && ld_dst % 4 == 0 &&
+                    aligned16(src) && aligned16(dst) && ld_src >= width && ld_dst >= width,
+                "width / leading dimensions must be multiples of 4 with 16-byte rows");
+  if (addend) GCB_CHECK_ARG(aligned16(addend) && ld_add % 4 == 0 && ld_add >= width, "addend unaligned");
+  if (n <= 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0, 4.0 * width * static_cast<double>(n) * (addend ? 3.0 : 2.0));
+  const long long total = n * (width / 4);
+  gcb::gather_add_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
+      src, ld_src, idx, n, addend, ld_add, dst, ld_dst, width / 4);
   GCB_CUDA(cudaGetLastError());
   return GCB_OK;
 }

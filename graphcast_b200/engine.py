@@ -117,6 +117,8 @@ class Engine:
     self._upload_weights(params)
     self._alloc_workspace()
     self.launches_per_step = 0
+    self._params = params                 # host dict: transposed weights of the backward pass
+    self._backward = None                 # gradient workspace, created by the first loss_and_grads
 
   # -- helpers -------------------------------------------------------------------
   def _dev(self, array: np.ndarray, dtype) -> torch.Tensor:
@@ -153,6 +155,9 @@ class Engine:
     self.m2g_snd = self._dev(g.m2g_senders, torch.int32)
     self.m2g_rcv = self._dev(g.m2g_receivers, torch.int32)
     self.m2g_feat = self._dev(g.m2g_edge_feats, torch.float32)
+    # senders in execution order (host): the sender CSRs of the backward pass are built from them
+    self.exec_senders = {"g2m": s1, "mesh": s2, "m2g": np.asarray(g.m2g_senders, np.int32)}
+    self.exec_row_ptr = {"g2m": rp1}      # receiver CSR of grid2mesh: the backward's edge chunks
     # Mesh-node encoder input: zeros for the data channels + 3 structural
     # features (reference graphcast.py:573-583).
     mesh_in = np.zeros([g.num_mesh_nodes, self.c_in_pad], np.float32)
@@ -460,6 +465,67 @@ class Engine:
           targets_planes.data_ptr(), lat_weight.data_ptr(), self._ptr(planes_out), ws.data_ptr(),
           nbytes, channel_sums.data_ptr(), self._stream()), "gcb_output_loss")
     return channel_sums
+
+  # -- parameter gradients (graphcast_b200/backward.py) ------------------------------------------------
+  def grads_begin(self, chunk_rows: Optional[int] = None) -> None:
+    """Zeroes the gradient accumulators of `loss_and_grads_element`; the gradient workspace (transposed
+    weights, sender CSRs, accumulators) is created by the first call, so inference never holds it.
+    chunk_rows: edges per chunk of the grid2mesh / mesh2grid edge-MLP backward passes (default 2^19;
+    the peak memory of the backward pass scales with it)."""
+    if self.num_grid_owned:
+      raise NotImplementedError(
+          "parameter gradients are not available in the node-partitioned engine: each rank holds "
+          "only its own grid rows; compute them with a single-GPU GraphCast")
+    if self.precision not in ("bf16x3", "bf16"):
+      raise NotImplementedError(f"parameter gradients support the tensor-core precisions 'bf16x3' "
+                                f"and 'bf16', not {self.precision!r}")
+    if self._backward is None or (chunk_rows and chunk_rows != self._backward.chunk_rows):
+      from graphcast_b200 import backward
+      self._backward = None
+      with self._on_device():
+        self._backward = (backward.Backward(self, self._params, chunk_rows) if chunk_rows
+                          else backward.Backward(self, self._params))
+    self._backward.prec = _native.PRECISIONS[self.precision]
+    self._backward.zero_grads()
+
+  def loss_and_grads_element(self, targets_planes: torch.Tensor, lat_weight: torch.Tensor,
+                             coef: torch.Tensor, *, channel_sums: torch.Tensor,
+                             grid_in: Optional[torch.Tensor] = None, **affine) -> None:
+    """One batch element: the step stage by stage from `grid_in` (default: the packed grid_in_img)
+    with snapshots of what the backward pass reads, the loss sums of `output_loss` into channel_sums,
+    the loss derivative seed (gcb_output_loss_grad with coef = 2 kappa / batch) and the backward pass,
+    which ADDS this element's parameter gradients to the accumulators (see grads_begin / grads)."""
+    if self._backward is None:
+      raise RuntimeError("call grads_begin() first")
+    grid_in = self.grid_in_img if grid_in is None else grid_in
+    snaps = {"v": [], "agg": [], "e": [None]}
+    self.run_stage("encode", grid_in=grid_in)
+    snaps["vg1"], snaps["agg1"] = self.grid_lat_img.clone(), self.mesh_agg_img.clone()
+    snaps["v"].append(self.mesh_lat_img.clone())
+    self.run_stage("process_embed")
+    for k in range(self.msg_steps):
+      self.run_stage("process_step", k)
+      snaps["v"].append(self.mesh_lat_img.clone())
+      snaps["agg"].append(self.mesh_agg_img.clone())
+      if k < self.msg_steps - 1:
+        snaps["e"].append(self.mesh_edge_img.clone())
+    self.run_stage("decode", grid_in=grid_in)
+    snaps["vg2"], snaps["agg3"] = self.grid_lat_img.clone(), self.grid_agg_img.clone()
+    self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
+    g_out = torch.zeros([self.num_grid, 256], dtype=torch.float32, device=self.device)
+    n_lat = lat_weight.shape[0]
+    with self._on_device():
+      _native.check(self._lib.gcb_output_loss_grad(
+          self.grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat,
+          self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
+          self._ptr(affine.get("add_planes")), self._ptr(affine.get("add_plane_index")),
+          targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), g_out.data_ptr(), 256,
+          self._stream()), "gcb_output_loss_grad")
+      self._backward.element(grid_in, g_out, snaps)
+
+  def grads(self):
+    """The accumulated gradients: device fp32 tensors keyed and shaped like the params."""
+    return self._backward.grads()
 
   def forward_features(self, grid_features: torch.Tensor) -> torch.Tensor:
     """Convenience for parity tests: grid_features [Ng, B, c_in] (the reference's

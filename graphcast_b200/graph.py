@@ -129,6 +129,20 @@ def receiver_sorted(senders: np.ndarray, receivers: np.ndarray, num_receivers: i
           np.ascontiguousarray(receivers[perm], np.int32), row_ptr)
 
 
+def sender_csr(senders: np.ndarray, num_senders: int, heavy_threshold: int = 256):
+  """CSR of an edge set by SENDER, for the backward of the sender gather (gcb_segment_sum_sorted).
+  `senders` are in the edges' execution order.  Returns (order, ptr, heavy): order [E] int32 edge ids
+  grouped by sender (stable, so each sender's edges stay in execution order), ptr [num_senders+1]
+  int32 offsets into order, heavy int32 ids of the senders with more than `heavy_threshold` edges."""
+  senders = np.asarray(senders).astype(np.int64)
+  order = np.argsort(senders, kind="stable").astype(np.int32)
+  counts = np.bincount(senders, minlength=num_senders)
+  ptr = np.zeros([num_senders + 1], dtype=np.int32)
+  np.cumsum(counts, out=ptr[1:])
+  heavy = np.nonzero(counts > heavy_threshold)[0].astype(np.int32)
+  return order, ptr, heavy
+
+
 def cached_static_graph(*, grid_lat: np.ndarray, grid_lon: np.ndarray,
                         mesh_size: int, radius_query_fraction_edge_length: float,
                         mesh2grid_edge_normalization_factor: Optional[float] = None,

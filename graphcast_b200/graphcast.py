@@ -100,6 +100,11 @@ class Predictor(abc.ABC):
     """Returns ((loss, diagnostics), predictions)."""
     raise NotImplementedError(f"{type(self).__name__} does not implement a loss")
 
+  def loss_and_grads(self, inputs, targets, forcings, **optional_kwargs):
+    """Returns (loss, diagnostics, grads): `loss` / `diagnostics` as `loss` returns them, `grads`
+    the gradient of loss.mean() (the mean over the batch) with respect to the parameters."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement parameter gradients")
+
 
 # Per-variable weights of GraphCast's loss (reference graphcast.py:341-356); others weigh 1.
 LOSS_PER_VARIABLE_WEIGHTS = {
@@ -230,6 +235,35 @@ class GraphCast(Predictor):
     """(loss, diagnostics) of `loss_and_predictions`; the predictions are not materialised."""
     return self._loss(inputs, targets, forcings, norm=None, predictions=False)[0]
 
+  def loss_and_grads(self, inputs, targets, forcings, **unused_kwargs):
+    """(loss, diagnostics, grads) for one target time.
+
+    `loss` and `diagnostics` are exactly what `loss()` returns for the same call.  `grads` is the
+    gradient of the MEAN OVER THE BATCH of `loss` -- the scalar the reference demo's `loss_fn` hands
+    to `jax.value_and_grad` (`loss.mean()`) -- with respect to every parameter: a dict shaped like
+    `params` ({module path: {"w", "b"} | {"scale", "offset"}}, float32 numpy arrays), with exact
+    zeros for the parameters the step never reads (the mesh2grid mesh-node MLP).  The forward runs
+    stage by stage on the device, the backward pass through the sm_90a kernels of the C ABI (see
+    graphcast_b200/backward.py) in the model's precision ("bf16x3" or "bf16")."""
+    return self._loss_and_grads(inputs, targets, forcings, norm=None)
+
+  def _loss_and_grads(self, inputs, targets, forcings, norm: Optional[FusedNormalization]):
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    if targets.sizes.get("time", 1) != 1:
+      raise NotImplementedError("parameter gradients cover one target time (no backprop through time)")
+    sizes = dict(inputs.sizes)
+    batch = sizes.get("batch", 1)
+    num_grid = sizes["lat"] * sizes["lon"]
+    slabs = model_utils.channel_layout(targets)
+    coef = 2.0 * losses.channel_kappa(slabs, num_grid, LOSS_PER_VARIABLE_WEIGHTS) / batch
+    self._call(inputs, targets, forcings, norm=norm, targets=targets, predictions=False,
+               grad_coef=coef)
+    loss, diagnostics = losses.losses_from_channel_sums(
+        self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
+    grads = {name: {f: t.cpu().numpy() for f, t in fields.items()}
+             for name, fields in self._engine.grads().items()}
+    return loss, diagnostics, grads
+
   def _loss(self, inputs, targets, forcings, norm: Optional[FusedNormalization], predictions: bool):
     finish, preds, sums = self._device_loss(inputs, targets, forcings, norm, predictions)
     return finish(sums.cpu().numpy()), preds
@@ -273,11 +307,14 @@ class GraphCast(Predictor):
     return bufs[buf], fresh
 
   def _call(self, inputs, targets_template, forcings, norm: Optional[FusedNormalization],
-            targets: Optional[xs.Dataset] = None, predictions: bool = True):
+            targets: Optional[xs.Dataset] = None, predictions: bool = True,
+            grad_coef: Optional[np.ndarray] = None):
     """The step for every batch element.  With `targets` (shaped like the template, usually the
     same Dataset) the outputs go through gcb_output_loss instead of the plain unpack: the loss sums
     land in a new [batch, n_out] fp64 device tensor, self._channel_sums, and the predictions are
-    returned only when `predictions` is set (else None)."""
+    returned only when `predictions` is set (else None).  With `grad_coef` ([n_out] coefficients
+    2 kappa / batch of the loss derivative) every element also runs the backward pass, which
+    accumulates the parameter gradients in the engine (Engine.loss_and_grads_element)."""
     inputs = xs.from_xarray(inputs)
     forcings = xs.from_xarray(forcings)
     targets_template = xs.from_xarray(targets_template)
@@ -348,6 +385,9 @@ class GraphCast(Predictor):
       compute.wait_event(ready)
 
     # Predictions are produced into fresh planes each call (they are handed out).
+    if grad_coef is not None:
+      coef_dev = torch.as_tensor(np.asarray(grad_coef, np.float64)).to(eng.device)
+      eng.grads_begin()
     planes_out = None
     if predictions:
       planes_out = torch.empty([batch, eng.n_out, eng.num_grid], dtype=torch.float32,
@@ -361,6 +401,10 @@ class GraphCast(Predictor):
           eng.pack_inputs(planes_in[b])
         else:
           eng.pack_inputs(planes_in[b], mean=norm.in_mean, scale=norm.in_scale)
+        if grad_coef is not None:
+          eng.loss_and_grads_element(planes_tgt[b], lat_weight, coef_dev,
+                                     channel_sums=channel_sums[b], **affine)
+          continue
         eng.step()
         eng.output_loss(planes_tgt[b], lat_weight, channel_sums=channel_sums[b],
                         planes_out=None if planes_out is None else planes_out[b], **affine)

@@ -179,6 +179,22 @@ def channel_level_weights(slab, dtype=np.float32) -> np.ndarray:
   return np.broadcast_to(w.reshape(shape), slab.stack_sizes).reshape(-1)
 
 
+def channel_kappa(slabs, num_nodes: int,
+                  per_variable_weights: Optional[Mapping[str, float]] = None) -> np.ndarray:
+  """[channels] float64 coefficients kappa with  total loss = sum_c kappa_c * channel_sums[c]  (up to
+  the fp32 roundings of `losses_from_channel_sums`, which applies the same weights):
+  kappa_c = variable weight * level weight_c / (channels of the variable * num_nodes).  The linear map
+  the parameter gradients differentiate."""
+  weights = per_variable_weights or {}
+  count = sum(s.count for s in slabs)
+  kappa = np.zeros([count], np.float64)
+  for s in slabs:
+    var_w = weights.get(s.name, DEFAULT_PER_VARIABLE_WEIGHT)
+    kappa[s.start:s.start + s.count] = (var_w * channel_level_weights(s)
+                                        / (float(s.count) * num_nodes))
+  return kappa
+
+
 def losses_from_channel_sums(channel_sums: np.ndarray, slabs, num_nodes: int,
                              per_variable_weights: Optional[Mapping[str, float]] = None
                              ) -> LossAndDiagnostics:

@@ -234,6 +234,18 @@ class InputsAndResiduals(graphcast.Predictor):
     consts = self._fused_constants(inputs, targets, forcings, torch.device(device))
     return self._predictor._device_loss(inputs, targets, forcings, consts, predictions)
 
+  def loss_and_grads(self, inputs, targets, forcings, **kwargs):
+    """(loss, diagnostics, grads) of `loss` and its parameter gradients (GraphCast.loss_and_grads),
+    with the normalisation fused into the kernels as in `loss`.  GraphCast only."""
+    if not self._fuses():
+      raise NotImplementedError("parameter gradients need a GraphCast predictor directly inside "
+                                "InputsAndResiduals (the fused normalisation)")
+    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
+    targets = xs.from_xarray(targets)
+    device = self._predictor._device or f"cuda:{torch.cuda.current_device()}"
+    consts = self._fused_constants(inputs, targets, forcings, torch.device(device))
+    return self._predictor._loss_and_grads(inputs, targets, forcings, norm=consts)
+
   def loss(self, inputs, targets, forcings, **kwargs):
     """The loss computed on normalised inputs and targets (targets that are also inputs as
     normalised residuals against the last input frame)."""

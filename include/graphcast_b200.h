@@ -232,6 +232,80 @@ int gcb_output_loss(const float* y, int32_t ld_y, int32_t n_out, int32_t n_lat, 
                     double* channel_sums, void* stream);
 int64_t gcb_output_loss_workspace_bytes(int32_t n_out);
 
+/* ---- parameter gradients (backward pass of one step's loss) ------------------------------
+ * The kernels below differentiate the step of gcb_forward; the orchestration (forward recompute
+ * through gcb_layer_forward, dX products through gcb_layer_forward with transposed packed weights)
+ * is host code, see graphcast_b200/backward.py.  Every reduction runs over a FIXED split of the rows
+ * and is summed in a fixed order: two runs are bit-identical on any device; no atomics. */
+
+/* Seed of the backward pass: the derivative of  sum_c kappa_c * channel_sums[c]  (gcb_output_loss)
+ * with respect to the decoder output,
+ *   g[node, c] = coef[c] * lat_weight[node / n_lon] * (y[node, c] - t_norm[c, node]),   c < n_out
+ * with t_norm formed exactly as gcb_output_loss forms it (same scale / offset / add_planes /
+ * add_plane_index arguments) and coef = 2 kappa / batch (fp64, device).  Columns >= n_out of g are
+ * not written.  Differentiates losses.weighted_mse_per_level (weathernext/utils/losses.py:85-132)
+ * and the per-variable weighting of GraphCast.loss (weathernext1_graph/graphcast.py:341-356). */
+int gcb_output_loss_grad(const float* y, int32_t ld_y, int32_t n_out, int32_t n_lat, int32_t n_lon,
+                         const float* scale, const float* offset, const float* add_planes,
+                         const int32_t* add_plane_index, const float* targets,
+                         const float* lat_weight, const double* coef, float* g, int32_t ld_g,
+                         void* stream);
+
+/* Weight gradient of one hk.Linear (utils/legacy/deep_typed_graph_net.py:205-247):
+ *   dw[0:k, 0:n] (+)= sum_{r < rows} X[r, 0:k]^T G[r, 0:n]          (dw dense, row stride n)
+ * X is an fp32 table (x, ld_x; columns >= k_valid read as 0) or, when x_img != NULL, an operand image
+ * of a [rows, k] matrix; x_swish = 1 uses swish(X) (the hidden activation recomputed from its
+ * pre-activation).  k a multiple of 16, n a multiple of 64, G rows 16-byte aligned.  Tensor cores,
+ * `precision` BF16X3 (hi*hi + hi*lo + lo*hi) or BF16; a fixed number of row slices each write an fp32
+ * partial tile into `workspace` (gcb_weight_grad_workspace_bytes), a second launch sums the slices in
+ * order in fp64 and writes (accumulate = 0) or adds to (accumulate = 1) dw. */
+int64_t gcb_weight_grad_workspace_bytes(int32_t k, int32_t n);
+int gcb_weight_grad(const float* x, int32_t ld_x, int32_t k_valid, const void* x_img, int32_t x_swish,
+                    const float* g, int32_t ld_g, int64_t rows, int32_t k, int32_t n,
+                    int32_t precision, void* workspace, int64_t workspace_bytes, float* dw,
+                    int32_t accumulate, void* stream);
+
+/* Row-wise backward of the layer tail, n = 256 or 512 columns (the LayerNorm needs n = 512):
+ *   scale != NULL: hk.LayerNorm (eps 1e-5, deep_typed_graph_net.py:240-246) at the recomputed
+ *                  pre-LayerNorm z:  dz = rstd * (dy*scale - mean(dy*scale) - zhat*mean(dy*scale*zhat));
+ *                  dscale (+)= sum_r dy*zhat, doffset (+)= sum_r dy
+ *   scale == NULL: dz = dy (dz may be NULL: column sums only)
+ * and in both cases dbias (+)= sum_r dz, the gradient of the bias of the linear in front.
+ * workspace: gcb_rowwise_workspace_bytes(n) bytes. */
+int64_t gcb_rowwise_workspace_bytes(int32_t n);
+int gcb_layernorm_backward(const float* dy, int32_t ld_dy, const float* z, int32_t ld_z,
+                           const float* scale, int64_t rows, int32_t n, float* dz, int32_t ld_dz,
+                           void* workspace, int64_t workspace_bytes, float* dbias, float* dscale,
+                           float* doffset, int32_t accumulate, void* stream);
+/* jax.nn.swish between the two linears of an MLP:  dh = da * swish'(h),  dbias (+)= sum_r dh. */
+int gcb_swish_backward(const float* da, int32_t ld_da, const float* h, int32_t ld_h, int64_t rows,
+                       int32_t n, float* dh, int32_t ld_dh, void* workspace, int64_t workspace_bytes,
+                       float* dbias, int32_t accumulate, void* stream);
+
+/* Backward of a gather v[senders] (jax_gather, utils/typed_graph_net.py:124-125,431-445):
+ *   out[i, 0:512] = sum_{j in [ptr[i], ptr[i+1])} msg[order[j], 0:512]
+ * (order / ptr: the sender CSR of an edge set, host-built), summed in j order; the rows listed in
+ * `heavy` (ascending node ids; meant for the rows with many entries, e.g. the mesh nodes next to a
+ * pole in mesh2grid) get one thread block each, every other row one warp.  The result does not
+ * depend on the list.  Deterministic. */
+int gcb_segment_sum_sorted(const float* msg, int32_t ld_msg, const int32_t* order,
+                           const int32_t* ptr, int32_t num_nodes, const int32_t* heavy,
+                           int32_t num_heavy, float* out, int32_t ld_out, int32_t width, void* stream);
+
+/* The hidden activation of an MLP recomputed from its pre-activation h (jax.nn.swish between the two
+ * linears of build_mlp_with_maybe_layer_norm, deep_typed_graph_net.py:205-247):
+ *   a[r, 0:n] = h / (1 + exp(-h))      (n a multiple of 4, 16-byte rows) */
+int gcb_swish_rows(const float* h, int32_t ld_h, int64_t rows, int32_t n, float* a, int32_t ld_a,
+                   void* stream);
+
+/* Backward of jraph.segment_sum (typed_graph_net.py:532-538) plus an edge residual:
+ *   dst[i, 0:width] = (addend ? addend[i, 0:width] : 0) + src[idx[i], 0:width]   (i < n)
+ * dm = de' + dagg[receivers] in the processor, dm = dagg[receivers] in grid2mesh and (the fan-in-3
+ * broadcast) mesh2grid.  width a multiple of 4, rows 16-byte aligned. */
+int gcb_gather_add(const float* src, int32_t ld_src, const int32_t* idx, int64_t n,
+                   const float* addend, int32_t ld_add, float* dst, int32_t ld_dst, int32_t width,
+                   void* stream);
+
 /* ---- fused layer chains ---------------------------------------------------------------
  * A CHAIN runs up to GCB_MAX_CHAIN fused layers over the same `rows` rows in ONE kernel: a
  * cluster pair owns a 128-row tile and takes it through layer 0, 1, ... while the intermediate
@@ -446,7 +520,10 @@ int gcb_set_graph_replay(int32_t enabled);
 typedef enum {
   GCB_KIND_LAYER_TC = 0, GCB_KIND_SEGMENT_SUM = 1, GCB_KIND_PACK = 2, GCB_KIND_UNPACK = 3,
   GCB_KIND_LAYER_SIMT = 4, GCB_KIND_ROWS_TO_IMAGE = 5, GCB_KIND_CHAIN_TC = 6, GCB_KIND_GATHER = 7,
-  GCB_KIND_LOSS = 8         /* gcb_output_loss (both of its launches) */
+  GCB_KIND_LOSS = 8,        /* gcb_output_loss (both of its launches) */
+  GCB_KIND_WGRAD = 9,       /* gcb_weight_grad (both of its launches) */
+  GCB_KIND_ROWWISE_BWD = 10 /* gcb_layernorm_backward, gcb_swish_backward, gcb_output_loss_grad,
+                             * gcb_segment_sum_sorted, gcb_gather_add, gcb_swish_rows */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
 int gcb_profile_end(int32_t capacity, int32_t* kinds, float* ms, double* flops, double* bytes,
