@@ -136,6 +136,11 @@ EXPORTS = {
     "gcb_output_loss_workspace_bytes": (C.c_int64, [C.c_int32]),
     "gcb_output_loss_grad": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp,
                                        _fp, _fp, _fp, _fp, _fp, _fp, C.c_int32, _fp]),
+    "gcb_output_loss_grad_feedback": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp,
+                                                C.c_int32, _fp, _fp, _fp, _fp, C.c_int32, _fp]),
+    "gcb_input_grad": (C.c_int, [_fp, C.c_int32, C.c_int64, C.c_int32, _fp, _fp, _fp, C.c_int32,
+                                 _fp]),
     "gcb_weight_grad_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
     "gcb_weight_grad": (C.c_int, [_fp, C.c_int32, C.c_int32, _fp, C.c_int32, _fp, C.c_int32,
                                   C.c_int64, C.c_int32, C.c_int32, C.c_int32, _fp, C.c_int64, _fp,

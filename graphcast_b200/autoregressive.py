@@ -17,7 +17,15 @@ When the inner predictor is this package's `GraphCast` (directly or under a fuse
 `normalization.InputsAndResiduals`), every step's loss stays on the device as per-channel sums of
 `gcb_output_loss` and all of them are read back once, after the last step.
 
-Not provided: input noise and gradient checkpointing (training-side features)."""
+`loss_and_grads` (the reference demo's `jax.value_and_grad` of `loss` with
+`gradient_checkpointing=True`, :262-310) differentiates that mean through the fed-back predictions:
+backprop through time.  Every step is recomputed from its saved input planes in the backward pass,
+which is what the reference's per-step `hk.remat` asks for; without `gradient_checkpointing` only one
+target time is supported.  The gradient reaches a step's inputs through the residual add and the
+target normalisation of InputsAndResiduals, the frame shift and the grid embedder; see
+graphcast_b200/feedback.py and DESIGN.md section 3.5.
+
+Not provided: input noise (a training-side feature)."""
 
 from __future__ import annotations
 
@@ -26,7 +34,10 @@ from typing import Optional
 import numpy as np
 import torch
 
+from graphcast_b200 import feedback
 from graphcast_b200 import graphcast
+from graphcast_b200 import losses
+from graphcast_b200 import model_utils
 from graphcast_b200 import normalization
 from graphcast_b200 import rollout
 from graphcast_b200 import xarray_shim as xs
@@ -39,7 +50,9 @@ class Predictor(graphcast.Predictor):
                gradient_checkpointing: bool = False):
     if noise_level:
       raise NotImplementedError("input noise is a training-time feature")
-    del gradient_checkpointing            # no backward pass here
+    # The multi-step gradient recomputes every step from its saved inputs (the reference's hk.remat
+    # per step); without checkpointing it would hold every step's activations, which is not offered.
+    self._gradient_checkpointing = bool(gradient_checkpointing)
     self._predictor = predictor
 
   @staticmethod
@@ -113,15 +126,74 @@ class Predictor(graphcast.Predictor):
       records = [finish(sums[t]) for t, (finish, _) in enumerate(records)]
     return _mean_over_time([l for l, _ in records], [d for _, d in records])
 
+  def _device_parts(self):
+    """(GraphCast, norm_of) when the inner predictor's loss runs on the device, else None;
+    norm_of(inputs, targets, forcings) -> the FusedNormalization of a step or None."""
+    p = self._predictor
+    if isinstance(p, graphcast.GraphCast):
+      return p, lambda i, t, f: None
+    if isinstance(p, normalization.InputsAndResiduals) and p._fuses():
+      def norm_of(i, t, f):
+        device = p._predictor._device or f"cuda:{torch.cuda.current_device()}"
+        return p._fused_constants(i, t, f, torch.device(device))
+      return p._predictor, norm_of
+    return None
+
   def loss_and_grads(self, inputs, targets, forcings, **kwargs):
-    """(loss, diagnostics, grads) of the underlying predictor for ONE target time.  Several target
-    times would need the gradient through the fed-back predictions (backprop through time), which is
-    not implemented."""
-    targets = xs.from_xarray(targets)
-    if targets.sizes["time"] != 1:
-      raise NotImplementedError("loss_and_grads supports one target time; backprop through time "
-                                "(several target times) is not implemented")
-    return self._predictor.loss_and_grads(inputs, targets, forcings, **kwargs)
+    """(loss, diagnostics, grads): `loss` and `diagnostics` exactly as `loss` returns them, `grads`
+    the gradient of loss.mean() (the mean over the batch) with respect to the parameters.
+
+    One target time delegates to the inner predictor.  Several target times differentiate through the
+    fed-back predictions (backprop through time, the reference demo's gradient cell): this needs
+    gradient_checkpointing=True, and GraphCast directly or under a fused InputsAndResiduals.  The
+    forward is the device path of `loss`, which also keeps every step's input and target planes in
+    pinned host memory; the backward pass then recomputes each step from them, last step first, and
+    carries dL/d(inputs) from step to step (feedback.FeedbackPlan, gcb_output_loss_grad_feedback,
+    gcb_input_grad)."""
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    forcings = xs.from_xarray(forcings)
+    if targets.sizes["time"] == 1:
+      return self._predictor.loss_and_grads(inputs, targets, forcings, **kwargs)
+    if not self._gradient_checkpointing:
+      raise NotImplementedError(
+          "loss_and_grads over several target times (backprop through time) recomputes every step "
+          "from its saved inputs: construct autoregressive.Predictor with gradient_checkpointing=True")
+    parts = self._device_parts()
+    if parts is None:
+      raise NotImplementedError("backprop through time needs a GraphCast predictor, directly or inside "
+                                "InputsAndResiduals (the fused normalisation)")
+    model, norm_of = parts
+    self._validate(inputs, targets, forcings)
+    records, first = [], {}
+    stash = None
+
+    def step(rng, inputs, targets_template, forcings):
+      nonlocal stash
+      norm = norm_of(inputs, targets_template, forcings)
+      finish, predictions, sums = model._device_loss(inputs, targets_template, forcings, norm, True)
+      records.append((finish, sums))
+      if stash is None:
+        stash = graphcast.StepStash(model.engine.device)
+        first.update(inputs=inputs, targets=targets_template, forcings=forcings, norm=norm)
+      model._stash_step(stash)
+      return predictions
+
+    for _ in rollout.chunked_prediction_generator(
+        step, rng=None, inputs=inputs, targets_template=targets, num_steps_per_chunk=1,
+        forcings=forcings):
+      pass
+    sums = torch.stack([s for _, s in records]).cpu().numpy()      # the one read-back
+    records = [finish(sums[t]) for t, (finish, _) in enumerate(records)]
+    loss, diagnostics = _mean_over_time([l for l, _ in records], [d for _, d in records])
+
+    plan = feedback.FeedbackPlan(first["inputs"], first["targets"], first["forcings"])
+    num_steps, batch = len(records), stash.batch
+    slabs = model_utils.channel_layout(first["targets"])
+    kappa = losses.channel_kappa(slabs, model.engine.num_grid, graphcast.LOSS_PER_VARIABLE_WEIGHTS)
+    lat_weight = model._lat_weight(first["targets"], model.engine.device)
+    grads = model._bptt_grads(stash, plan, first["norm"], lat_weight,
+                              2.0 * kappa / (batch * num_steps))
+    return loss, diagnostics, grads
 
 
 def _mean_over_time(step_losses, step_diagnostics):

@@ -162,6 +162,22 @@ class Backward:
     elif w0.shape[0] == D:
       info.t["w0_0"] = self._pack(w0.T, D, D)
 
+  def input_transposed(self):
+    """(packed [512, n] transpose of the grid embedder's first layer, n): the dX product of the grid
+    inputs (backprop through time), n = 256 | 512 >= c_in_pad.  Packed on first use, so the one-step
+    gradient never holds it."""
+    info = self.mlps["enc_grid"]
+    if "w0_in" not in info.t:
+      cin = self.eng.c_in_pad
+      if cin > 2 * 256:
+        raise NotImplementedError(f"input gradients support at most 512 padded input channels, "
+                                  f"not {cin}")
+      n = 256 if cin <= 256 else 512
+      w0 = np.asarray(self.params[f"{info.stem}_mlp/~/linear_0"]["w"], np.float32)   # [c_in + 3, 512]
+      info.t["w0_in"] = self._pack(w0.T, D, n)
+      self.n_in_t = n
+    return info.t["w0_in"], self.n_in_t
+
   def _alloc_grads(self, info: _MlpInfo) -> None:
     z = lambda *s: torch.zeros(list(s), dtype=torch.float32, device=self.dev)
     info.g = {"w0": z(sum(info.k_segs), D), "b0": z(D), "w1": z(D, info.n1), "b1": z(info.n1)}
@@ -369,10 +385,13 @@ class Backward:
     return s_tab, r_tab
 
   # -- one batch element ---------------------------------------------------------------------------
-  def element(self, grid_in_img: torch.Tensor, g_out: torch.Tensor, snaps: dict) -> None:
+  def element(self, grid_in_img: torch.Tensor, g_out: torch.Tensor, snaps: dict,
+              dgrid_in: bool = False) -> Optional[torch.Tensor]:
     """Accumulates the parameter gradients of one batch element whose loss derivative with respect
     to the decoder output is g_out [Ng, 256] (gcb_output_loss_grad) and whose forward left `snaps`
-    (whose entries are dropped as they are consumed)."""
+    (whose entries are dropped as they are consumed).  dgrid_in: also return the derivative with
+    respect to the packed grid inputs, dh_enc_grid W0^T [Ng, n] (see input_transposed; columns >=
+    c_in + 3 are zero)."""
     eng, m = self.eng, self.m
     ng, nm = m.num_grid, m.num_mesh
     K = eng.msg_steps
@@ -474,8 +493,15 @@ class Backward:
     self.layer(nm, [tab(R)], info.t["w0_2"], self.zero_bias, residual=dvm0, out=t)
     dvm0 = t
     del S, R, vg0, vm0
-    self.mlp_backward(mp["enc_grid"], ng, [grid_in], dvg0)
+    dh = self.mlp_backward(mp["enc_grid"], ng, [grid_in], dvg0)
+    dx = None
+    if dgrid_in:
+      w0t, n = self.input_transposed()
+      dx = self.empty(ng, n)
+      self.layer(ng, [tab(dh)], w0t, self.zero_bias, out_y=dx, n=n)
+    del dh, dvg0
     self.mlp_backward(mp["enc_mesh"], nm, [mesh_in], dvm0)
+    return dx
 
   # -- result ----------------------------------------------------------------------------------------
   def grads(self) -> Dict[str, Dict[str, torch.Tensor]]:

@@ -823,6 +823,52 @@ int gcb_output_loss_grad(const float* y, int32_t ld_y, int32_t n_out, int32_t n_
   return GCB_OK;
 }
 
+int gcb_output_loss_grad_feedback(const float* y, int32_t ld_y, int32_t n_out, int32_t n_lat,
+                                  int32_t n_lon, const float* scale, const float* offset,
+                                  const float* add_planes, const int32_t* add_plane_index,
+                                  const float* targets, const float* lat_weight, const double* coef,
+                                  const float* a_next, const int32_t* dpred_row, int32_t n_rows,
+                                  const int32_t* resid_channel, const int32_t* carry_row,
+                                  float* a_out, float* g, int32_t ld_g, void* stream) {
+  GCB_CHECK_ARG(y && targets && lat_weight && coef && g, "null pointer");
+  GCB_CHECK_ARG(n_out > 0 && ld_y >= n_out && ld_g >= n_out, "ld_y / ld_g too small");
+  GCB_CHECK_ARG(n_lat > 0 && n_lon > 0, "empty grid");
+  GCB_CHECK_ARG((add_planes == nullptr) == (add_plane_index == nullptr), "add_planes/index mismatch");
+  GCB_CHECK_ARG(a_next == nullptr || dpred_row != nullptr, "a_next needs dpred_row");
+  GCB_CHECK_ARG(n_rows >= 0 && (n_rows == 0 || (a_out && resid_channel)), "rows need a_out and resid_channel");
+  const long long n_nodes = static_cast<long long>(n_lat) * n_lon;
+  const int c_tiles = (n_out + 31) / 32, r_tiles = (n_rows + 31) / 32;
+  GCB_CHECK_ARG(c_tiles + r_tiles <= 65535, "too many channels / rows");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // algorithmic bytes: the seed's reads and g, the rows written and the feedback rows read once
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * n_nodes * (n_out * (3.0 + (add_planes ? 1.0 : 0.0) + (a_next ? 1.0 : 0.0)) +
+                                  n_rows * (a_next ? 2.0 : 1.0)));
+  dim3 grid(static_cast<unsigned>((n_nodes + 31) / 32), static_cast<unsigned>(c_tiles + r_tiles));
+  gcb::output_loss_grad_feedback_kernel<<<grid, 256, 0, st>>>(
+      y, ld_y, n_out, n_lon, n_nodes, scale, offset, add_planes, add_plane_index, targets, lat_weight,
+      coef, a_next, dpred_row, n_rows, resid_channel, carry_row, a_out, g, ld_g, c_tiles);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int gcb_input_grad(const float* dx, int32_t ld_dx, int64_t n_nodes, int32_t n_rows,
+                   const int32_t* channel, const float* scale, float* a, int32_t accumulate,
+                   void* stream) {
+  GCB_CHECK_ARG(dx && channel && a, "null pointer");
+  GCB_CHECK_ARG(ld_dx > 0 && n_nodes >= 0 && n_rows >= 0, "bad shape");
+  GCB_CHECK_ARG((n_rows + 31) / 32 <= 65535, "too many rows");
+  if (n_nodes == 0 || n_rows == 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * static_cast<double>(n_nodes) * n_rows * (accumulate ? 3.0 : 2.0));
+  dim3 grid(static_cast<unsigned>((n_nodes + 31) / 32), static_cast<unsigned>((n_rows + 31) / 32));
+  gcb::input_grad_kernel<<<grid, 256, 0, st>>>(dx, ld_dx, n_nodes, n_rows, channel, scale, a,
+                                               accumulate ? 1 : 0);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
 int64_t gcb_weight_grad_workspace_bytes(int32_t k, int32_t n) {
   if (k <= 0 || n <= 0) return -1;
   return static_cast<int64_t>(gcb::kWgSlices) * k * n * static_cast<int64_t>(sizeof(float));

@@ -412,4 +412,135 @@ output_loss_grad_kernel(const float* __restrict__ y, int ld_y, int n_out, int n_
   }
 }
 
+// ---- backprop through time -----------------------------------------------------------------------
+// Differentiates the feeding of one step's predictions into the next step's inputs
+// (autoregressive.py:114-125, the loss unroll :262-310) through the residual add and the target
+// normalisation of InputsAndResiduals (normalization.py:113-146).  A = dL / d(input planes) of a step,
+// restricted to a list of rows (input channels); a_next is that of the following step.
+//
+// Blocks with blockIdx.y < c_tiles: the seed, node-major, as output_loss_grad_kernel plus the derivative
+// that reaches the prediction through the next step's inputs:
+//   g[node, c] = coef[c] * w * (y - t_norm) + scale[c] * a_next[dpred_row[c], node]   (fp64, rounded once)
+// the second term only when a_next != NULL and dpred_row[c] >= 0, so that without it g is bit-identical
+// to output_loss_grad_kernel.  The other blocks: rows r of a_out, channel-major,
+//   a_out[r, node] = (c = resid_channel[r]) >= 0 ? (float)(g_loss[node, c] / scale[c] + a_next[dpred_row[c], node]) : 0
+//                    (+ a_next[carry_row[r], node] when carry_row[r] >= 0)
+// g_loss the first term of g: the residual add and the target normalisation both read the same last
+// input frame; the carry is the frame shift.  Both tile kinds use the 32 x 32 shared-memory transpose.
+__device__ __forceinline__ float loss_t_norm(int c, long long node, long long n_nodes,
+                                             const float* __restrict__ scale, const float* __restrict__ offset,
+                                             const float* __restrict__ add_planes,
+                                             const int* __restrict__ add_plane_index,
+                                             const float* __restrict__ targets) {
+  const float sc = scale ? scale[c] : 1.f, of = offset ? offset[c] : 0.f;
+  const int ap = add_plane_index ? add_plane_index[c] : -1;
+  const float av = ap >= 0 ? add_planes[static_cast<long long>(ap) * n_nodes + node] : 0.f;
+  return __fdiv_rn(__fsub_rn(__fsub_rn(targets[static_cast<long long>(c) * n_nodes + node], av), of), sc);
+}
+
+__global__ void __launch_bounds__(256)
+output_loss_grad_feedback_kernel(const float* __restrict__ y, int ld_y, int n_out, int n_lon,
+                                 long long n_nodes, const float* __restrict__ scale,
+                                 const float* __restrict__ offset, const float* __restrict__ add_planes,
+                                 const int* __restrict__ add_plane_index, const float* __restrict__ targets,
+                                 const float* __restrict__ lat_weight, const double* __restrict__ coef,
+                                 const float* __restrict__ a_next, const int* __restrict__ dpred_row,
+                                 int n_rows, const int* __restrict__ resid_channel,
+                                 const int* __restrict__ carry_row, float* __restrict__ a_out,
+                                 float* __restrict__ g, int ld_g, int c_tiles) {
+  __shared__ float tile[32][33];
+  __shared__ float tile_dp[32][33];
+  const long long node0 = static_cast<long long>(blockIdx.x) * 32;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  if (static_cast<int>(blockIdx.y) < c_tiles) {
+    const int c0 = blockIdx.y * 32;
+    for (int r = ty; r < 32; r += 8) {
+      const int c = c0 + r;
+      const long long node = node0 + tx;
+      float t_norm = 0.f, dp = 0.f;
+      if (c < n_out && node < n_nodes) {
+        t_norm = loss_t_norm(c, node, n_nodes, scale, offset, add_planes, add_plane_index, targets);
+        const int q = a_next ? dpred_row[c] : -1;
+        if (q >= 0) dp = a_next[static_cast<long long>(q) * n_nodes + node];
+      }
+      tile[r][tx] = t_norm;
+      tile_dp[r][tx] = dp;
+    }
+    __syncthreads();
+    for (int r = ty; r < 32; r += 8) {
+      const long long node = node0 + r;
+      const int c = c0 + tx;
+      if (c < n_out && node < n_nodes) {
+        const double d = static_cast<double>(__fsub_rn(y[node * ld_y + c], tile[tx][r]));
+        double v = coef[c] * static_cast<double>(lat_weight[node / n_lon]) * d;
+        if (a_next && dpred_row[c] >= 0)
+          v += static_cast<double>(scale ? scale[c] : 1.f) * static_cast<double>(tile_dp[tx][r]);
+        g[node * ld_g + c] = static_cast<float>(v);
+      }
+    }
+    return;
+  }
+  const int r0 = (static_cast<int>(blockIdx.y) - c_tiles) * 32;
+  // y[node, resid_channel[r]] of the tile's rows, node-major reads
+  for (int q = ty; q < 32; q += 8) {
+    const long long node = node0 + q;
+    const int r = r0 + tx;
+    float v = 0.f;
+    if (r < n_rows && node < n_nodes) {
+      const int c = resid_channel[r];
+      if (c >= 0) v = y[node * ld_y + c];
+    }
+    tile[q][tx] = v;
+  }
+  __syncthreads();
+  for (int q = ty; q < 32; q += 8) {
+    const int r = r0 + q;
+    const long long node = node0 + tx;
+    if (r >= n_rows || node >= n_nodes) continue;
+    float v = 0.f;
+    const int c = resid_channel[r];
+    if (c >= 0) {
+      const float t_norm = loss_t_norm(c, node, n_nodes, scale, offset, add_planes, add_plane_index, targets);
+      const double d = static_cast<double>(__fsub_rn(tile[tx][q], t_norm));
+      const double gl = coef[c] * static_cast<double>(lat_weight[node / n_lon]) * d;
+      const int p = a_next ? dpred_row[c] : -1;
+      const double dp = p >= 0 ? static_cast<double>(a_next[static_cast<long long>(p) * n_nodes + node]) : 0.0;
+      v = static_cast<float>(gl / static_cast<double>(scale ? scale[c] : 1.f) + dp);
+    }
+    const int k = (a_next && carry_row) ? carry_row[r] : -1;
+    if (k >= 0) v = __fadd_rn(v, a_next[static_cast<long long>(k) * n_nodes + node]);
+    a_out[static_cast<long long>(r) * n_nodes + node] = v;
+  }
+}
+
+// Transpose of pack_grid_image_kernel's normalisation for a list of rows (normalization.py:113-146,
+// the input side of InputsAndResiduals): a[r, node] (+)= dx[node, channel[r]] / scale[channel[r]]
+// (true division; scale == NULL divides by 1).  dx is read node-major through a 32 x 32 shared tile,
+// a written channel-major.  One addition per element: deterministic.
+__global__ void __launch_bounds__(256)
+input_grad_kernel(const float* __restrict__ dx, int ld_dx, long long n_nodes, int n_rows,
+                  const int* __restrict__ channel, const float* __restrict__ scale,
+                  float* __restrict__ a, int accumulate) {
+  __shared__ float tile[32][33];
+  const long long node0 = static_cast<long long>(blockIdx.x) * 32;
+  const int r0 = blockIdx.y * 32;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  for (int q = ty; q < 32; q += 8) {
+    const long long node = node0 + q;
+    const int r = r0 + tx;
+    tile[q][tx] = (r < n_rows && node < n_nodes) ? __ldg(dx + node * ld_dx + channel[r]) : 0.f;
+  }
+  __syncthreads();
+  for (int q = ty; q < 32; q += 8) {
+    const int r = r0 + q;
+    const long long node = node0 + tx;
+    if (r < n_rows && node < n_nodes) {
+      float v = tile[tx][q];
+      if (scale) v = __fdiv_rn(v, scale[channel[r]]);
+      float* p = a + static_cast<long long>(r) * n_nodes + node;
+      *p = accumulate ? __fadd_rn(*p, v) : v;
+    }
+  }
+}
+
 }  // namespace gcb

@@ -490,14 +490,41 @@ class Engine:
 
   def loss_and_grads_element(self, targets_planes: torch.Tensor, lat_weight: torch.Tensor,
                              coef: torch.Tensor, *, channel_sums: torch.Tensor,
-                             grid_in: Optional[torch.Tensor] = None, **affine) -> None:
+                             grid_in: Optional[torch.Tensor] = None,
+                             feedback: Optional["Feedback"] = None, input_grad: bool = False,
+                             **affine) -> None:
     """One batch element: the step stage by stage from `grid_in` (default: the packed grid_in_img)
     with snapshots of what the backward pass reads, the loss sums of `output_loss` into channel_sums,
     the loss derivative seed (gcb_output_loss_grad with coef = 2 kappa / batch) and the backward pass,
-    which ADDS this element's parameter gradients to the accumulators (see grads_begin / grads)."""
+    which ADDS this element's parameter gradients to the accumulators (see grads_begin / grads).
+
+    feedback: one step of backprop through time.  The seed also carries feedback.a, dL/d(inputs) of
+    the following step (None for the last step), into the predictions (gcb_output_loss_grad_feedback);
+    with input_grad, feedback.a is then replaced by dL/d(inputs) of this step, the residual and
+    frame-shift terms from the seed plus the derivative through the grid embedder (gcb_input_grad),
+    else it is dropped."""
     if self._backward is None:
       raise RuntimeError("call grads_begin() first")
+    if feedback is not None:
+      self._bptt_element(targets_planes, lat_weight, coef, channel_sums, grid_in, feedback,
+                         input_grad, affine)
+      return
     grid_in = self.grid_in_img if grid_in is None else grid_in
+    snaps = self._forward_snapshots(grid_in)
+    self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
+    g_out = torch.zeros([self.num_grid, 256], dtype=torch.float32, device=self.device)
+    n_lat = lat_weight.shape[0]
+    with self._on_device():
+      _native.check(self._lib.gcb_output_loss_grad(
+          self.grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat,
+          self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
+          self._ptr(affine.get("add_planes")), self._ptr(affine.get("add_plane_index")),
+          targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), g_out.data_ptr(), 256,
+          self._stream()), "gcb_output_loss_grad")
+      self._backward.element(grid_in, g_out, snaps)
+
+  def _forward_snapshots(self, grid_in: torch.Tensor) -> dict:
+    """The step stage by stage, with copies of what the backward pass reads."""
     snaps = {"v": [], "agg": [], "e": [None]}
     self.run_stage("encode", grid_in=grid_in)
     snaps["vg1"], snaps["agg1"] = self.grid_lat_img.clone(), self.mesh_agg_img.clone()
@@ -511,21 +538,53 @@ class Engine:
         snaps["e"].append(self.mesh_edge_img.clone())
     self.run_stage("decode", grid_in=grid_in)
     snaps["vg2"], snaps["agg3"] = self.grid_lat_img.clone(), self.grid_agg_img.clone()
+    return snaps
+
+  def _bptt_element(self, targets_planes, lat_weight, coef, channel_sums, grid_in, fb: "Feedback",
+                    input_grad: bool, affine) -> None:
+    grid_in = self.grid_in_img if grid_in is None else grid_in
+    snaps = self._forward_snapshots(grid_in)
     self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
     g_out = torch.zeros([self.num_grid, 256], dtype=torch.float32, device=self.device)
+    n_rows = fb.n_rows if input_grad else 0
+    a_out = torch.empty([n_rows, self.num_grid], dtype=torch.float32, device=self.device) \
+        if n_rows else None
     n_lat = lat_weight.shape[0]
     with self._on_device():
-      _native.check(self._lib.gcb_output_loss_grad(
+      _native.check(self._lib.gcb_output_loss_grad_feedback(
           self.grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat,
           self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
           self._ptr(affine.get("add_planes")), self._ptr(affine.get("add_plane_index")),
-          targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), g_out.data_ptr(), 256,
-          self._stream()), "gcb_output_loss_grad")
-      self._backward.element(grid_in, g_out, snaps)
+          targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), self._ptr(fb.a),
+          fb.dpred_row.data_ptr(), n_rows, fb.resid_channel.data_ptr(), fb.carry_row.data_ptr(),
+          self._ptr(a_out), g_out.data_ptr(), 256, self._stream()), "gcb_output_loss_grad_feedback")
+      fb.a = a_out                         # the following step's rows are consumed: release them
+      dx = self._backward.element(grid_in, g_out, snaps, dgrid_in=bool(n_rows))
+      if n_rows:
+        _native.check(self._lib.gcb_input_grad(
+            dx.data_ptr(), dx.shape[1], self.num_grid, n_rows, fb.rows.data_ptr(),
+            self._ptr(fb.in_scale), a_out.data_ptr(), 1, self._stream()), "gcb_input_grad")
 
   def grads(self):
     """The accumulated gradients: device fp32 tensors keyed and shaped like the params."""
     return self._backward.grads()
+
+  def feedback(self, plan, add_plane_index=None, in_scale: Optional[torch.Tensor] = None) -> "Feedback":
+    """Backprop-through-time state of one batch element for a feedback.FeedbackPlan (host) of this
+    engine's channels; add_plane_index / in_scale as in FusedNormalization (None: no normalisation).
+    Packs the transposed grid-embedder weight of the input gradient."""
+    if plan.c_in != self.c_in or plan.n_out != self.n_out:
+      raise ValueError(f"feedback plan of {plan.c_in} -> {plan.n_out} channels, engine "
+                       f"{self.c_in} -> {self.n_out}")
+    if self._backward is None:
+      raise RuntimeError("call grads_begin() first")
+    with self._on_device():
+      self._backward.input_transposed()
+    if add_plane_index is not None and isinstance(add_plane_index, torch.Tensor):
+      add_plane_index = add_plane_index.cpu().numpy()
+    i32 = lambda a: torch.as_tensor(np.ascontiguousarray(a, np.int32)).to(self.device)
+    return Feedback(i32(plan.rows), i32(plan.dpred_row), i32(plan.resid_channel(add_plane_index)),
+                    i32(plan.carry_row), in_scale)
 
   def forward_features(self, grid_features: torch.Tensor) -> torch.Tensor:
     """Convenience for parity tests: grid_features [Ng, B, c_in] (the reference's
@@ -538,3 +597,17 @@ class Engine:
       self.step()
       outs.append(self.grid_out[:, :self.n_out].clone())
     return torch.stack(outs, dim=1)
+
+
+class Feedback:
+  """Backprop through time of one batch element (Engine.loss_and_grads_element(feedback=...)): the
+  device copies of a feedback.FeedbackPlan's row maps and `a`, dL/d(input planes) [n_rows, Ng] of the
+  step after the one being differentiated (None before the last step)."""
+
+  def __init__(self, rows: torch.Tensor, dpred_row: torch.Tensor, resid_channel: torch.Tensor,
+               carry_row: torch.Tensor, in_scale: Optional[torch.Tensor]):
+    self.rows, self.dpred_row = rows, dpred_row
+    self.resid_channel, self.carry_row = resid_channel, carry_row
+    self.in_scale = in_scale
+    self.n_rows = int(rows.shape[0])
+    self.a: Optional[torch.Tensor] = None

@@ -171,6 +171,7 @@ class GraphCast(Predictor):
     # The loss: target planes staged like the inputs (same slots, same events), the latitude
     # weights of the last target grid, the per-channel sums of the last call.
     self._target_bufs: List[Optional[torch.Tensor]] = [None, None]
+    self._planes_tgt: Optional[torch.Tensor] = None
     self._lat_weight_cache = None
     self._channel_sums: Optional[torch.Tensor] = None
 
@@ -264,6 +265,52 @@ class GraphCast(Predictor):
              for name, fields in self._engine.grads().items()}
     return loss, diagnostics, grads
 
+  def _stash_step(self, stash: "StepStash") -> None:
+    """Keeps the input and target planes of the last `_call` (with targets) in pinned host memory."""
+    stash.save(self._planes_in, self._planes_tgt)
+
+  def _bptt_grads(self, stash: "StepStash", plan, norm: Optional[FusedNormalization],
+                  lat_weight: torch.Tensor, coef: np.ndarray):
+    """Parameter gradients of the multi-step loss whose steps `stash` holds (backprop through time,
+    see autoregressive.Predictor.loss_and_grads).  For every batch element, last step first: the
+    step's planes are uploaded again, packed and differentiated by Engine.loss_and_grads_element with
+    the feedback of the following step; the gradients accumulate in this fixed order."""
+    eng = self._engine
+    dev = eng.device
+    eng.grads_begin()
+    fb = eng.feedback(plan, None if norm is None else norm.add_plane_index,
+                      None if norm is None else norm.in_scale)
+    # The rollout's staging buffers are not needed any more: their memory goes to the backward pass.
+    self._planes_bufs, self._target_bufs, self._buf_free = [None, None], [None, None], [None, None]
+    self._planes_in = self._planes_tgt = None
+    # Return the rollout's cached blocks to the driver, so that the backward pass allocates from an
+    # unfragmented pool: at 0.25 degree it peaks within a few GiB of an 80 GB card's capacity, and a
+    # second call would otherwise find its 1 GiB tables only in the gaps the first one left.
+    torch.cuda.empty_cache()
+    planes = torch.empty([eng.c_in, eng.num_grid], dtype=torch.float32, device=dev)
+    tgt = torch.empty([eng.n_out, eng.num_grid], dtype=torch.float32, device=dev)
+    scratch = torch.empty([eng.n_out], dtype=torch.float64, device=dev)
+    coef_dev = torch.as_tensor(np.asarray(coef, np.float64)).to(dev)
+    compute = torch.cuda.current_stream(dev)
+    for b in range(stash.batch):
+      fb.a = None
+      for t in range(len(stash.steps) - 1, -1, -1):
+        (host_in, host_tgt), done = stash.steps[t]
+        compute.wait_event(done)
+        planes.copy_(host_in[b], non_blocking=True)
+        tgt.copy_(host_tgt[b], non_blocking=True)
+        affine = {}
+        if norm is None:
+          eng.pack_inputs(planes)
+        else:
+          eng.pack_inputs(planes, mean=norm.in_mean, scale=norm.in_scale)
+          affine = dict(scale=norm.out_scale, offset=norm.out_offset, add_planes=planes,
+                        add_plane_index=norm.add_plane_index)
+        eng.loss_and_grads_element(tgt, lat_weight, coef_dev, channel_sums=scratch, feedback=fb,
+                                   input_grad=t > 0, **affine)
+    return {name: {f: t.cpu().numpy() for f, t in fields.items()}
+            for name, fields in eng.grads().items()}
+
   def _loss(self, inputs, targets, forcings, norm: Optional[FusedNormalization], predictions: bool):
     finish, preds, sums = self._device_loss(inputs, targets, forcings, norm, predictions)
     return finish(sums.cpu().numpy()), preds
@@ -346,6 +393,7 @@ class GraphCast(Predictor):
     staged = [(planes_in, fresh)]
     if targets is not None:
       planes_tgt, fresh_tgt = self._staging(self._target_bufs, buf, (batch, eng.n_out, eng.num_grid))
+      self._planes_tgt = planes_tgt
       jobs.append((planes_tgt, targets, t_slabs))
       staged.append((planes_tgt, fresh_tgt))
     if all(f for _, f in staged):
@@ -506,3 +554,32 @@ def init_params(model_config: ModelConfig, task_config: TaskConfig, c_in: int,
   add(g, "processor_nodes_0_", "mesh_nodes", D, D)
   add(g, "decoder_nodes_", "grid_nodes", D, n_out, layer_norm=False)
   return params
+
+
+class StepStash:
+  """Pinned host copies of the input and target planes of every step of a multi-step loss, for the
+  recompute of backprop through time.  Each step's planes are first copied on the device (the staging
+  buffers are reused two calls later), then to the host on a side stream, so the copy overlaps the
+  next step's kernels.  steps[t] = ((inputs [batch, c_in, Ng], targets [batch, n_out, Ng]), event)."""
+
+  def __init__(self, device):
+    self.device = torch.device(device)
+    self.stream = torch.cuda.Stream(device=self.device)
+    self.steps = []
+    self.batch = 0
+
+  def save(self, *planes: torch.Tensor) -> None:
+    compute = torch.cuda.current_stream(self.device)
+    copies = [p.clone() for p in planes]
+    ready = torch.cuda.Event()
+    ready.record(compute)
+    hosts = [torch.empty(p.shape, dtype=p.dtype, pin_memory=True) for p in planes]
+    with torch.cuda.stream(self.stream):
+      self.stream.wait_event(ready)
+      for h, c in zip(hosts, copies):
+        h.copy_(c, non_blocking=True)
+        c.record_stream(self.stream)
+      done = torch.cuda.Event()
+      done.record(self.stream)
+    self.steps.append((tuple(hosts), done))
+    self.batch = int(planes[0].shape[0])

@@ -251,6 +251,40 @@ int gcb_output_loss_grad(const float* y, int32_t ld_y, int32_t n_out, int32_t n_
                          const float* lat_weight, const double* coef, float* g, int32_t ld_g,
                          void* stream);
 
+/* ---- backprop through time (the multi-step loss of autoregressive.Predictor) ---------------------
+ * A step's input planes P [c_in, n_nodes] feed the next step through the frame shift and the fed-back
+ * predictions (weathernext/utils/autoregressive.py:114-125; the loss unroll :262-310).  A = dL/dP of a
+ * step, kept for a list of ROWS (input channels that depend on the parameters), row-major
+ * [n_rows, n_nodes] fp32; `a_next` is that of the following step (NULL for the last step).
+ *
+ * Seed with feedback: everything gcb_output_loss_grad does, plus the derivative reaching the
+ * prediction of channel c through the next step's inputs (pred = y * scale + offset + add, the
+ * un-normalisation of normalization.py:113-132):
+ *   g[node, c] = coef[c] * lat_weight * (y - t_norm) + scale[c] * a_next[dpred_row[c], node]
+ * in fp64, rounded once; the second term only when a_next != NULL and dpred_row[c] >= 0, so with
+ * a_next == NULL g is bit-identical to gcb_output_loss_grad.  In the same launch, for r < n_rows:
+ *   a_out[r, node] = c >= 0 ? (float)(g_loss[node, c] / scale[c] + a_next[dpred_row[c], node]) : 0,
+ *                    c = resid_channel[r]                  (the residual add and the target
+ *                                                           normalisation of normalization.py:134-146)
+ *                  + a_next[carry_row[r], node]           when carry_row[r] >= 0 (the frame shift)
+ * with g_loss the first term of g.  After it a_next is no longer needed.  Deterministic, no atomics. */
+int gcb_output_loss_grad_feedback(const float* y, int32_t ld_y, int32_t n_out, int32_t n_lat,
+                                  int32_t n_lon, const float* scale, const float* offset,
+                                  const float* add_planes, const int32_t* add_plane_index,
+                                  const float* targets, const float* lat_weight, const double* coef,
+                                  const float* a_next, const int32_t* dpred_row, int32_t n_rows,
+                                  const int32_t* resid_channel, const int32_t* carry_row,
+                                  float* a_out, float* g, int32_t ld_g, void* stream);
+
+/* Input gradient: the transpose of gcb_pack_grid_image's normalisation (normalization.py:113-146,
+ * (x - mean) / scale) for a list of rows,
+ *   a[r, node] = (accumulate ? a[r, node] : 0) + dx[node, channel[r]] / scale[channel[r]]
+ * (true division; scale NULL = 1).  dx [n_nodes, ld_dx] node-major (the dX of the grid embedder's
+ * first layer), a [n_rows, n_nodes] channel-major.  Deterministic. */
+int gcb_input_grad(const float* dx, int32_t ld_dx, int64_t n_nodes, int32_t n_rows,
+                   const int32_t* channel, const float* scale, float* a, int32_t accumulate,
+                   void* stream);
+
 /* Weight gradient of one hk.Linear (utils/legacy/deep_typed_graph_net.py:205-247):
  *   dw[0:k, 0:n] (+)= sum_{r < rows} X[r, 0:k]^T G[r, 0:n]          (dw dense, row stride n)
  * X is an fp32 table (x, ld_x; columns >= k_valid read as 0) or, when x_img != NULL, an operand image
@@ -523,7 +557,8 @@ typedef enum {
   GCB_KIND_LOSS = 8,        /* gcb_output_loss (both of its launches) */
   GCB_KIND_WGRAD = 9,       /* gcb_weight_grad (both of its launches) */
   GCB_KIND_ROWWISE_BWD = 10 /* gcb_layernorm_backward, gcb_swish_backward, gcb_output_loss_grad,
-                             * gcb_segment_sum_sorted, gcb_gather_add, gcb_swish_rows */
+                             * gcb_segment_sum_sorted, gcb_gather_add, gcb_swish_rows,
+                             * gcb_output_loss_grad_feedback, gcb_input_grad */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
 int gcb_profile_end(int32_t capacity, int32_t* kinds, float* ms, double* flops, double* bytes,
