@@ -26,6 +26,7 @@ buffers.  Allocation is lazy: nothing here exists until the first loss_and_grads
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -59,7 +60,9 @@ class Backward:
   def __init__(self, eng, params, chunk_rows: int = 1 << 19):
     if not eng.pregather:
       raise NotImplementedError("parameter gradients need the pre-gathered edge layers (pregather=True)")
-    self.eng = eng
+    # The engine owns this workspace: a weak reference, so that dropping the engine frees both at
+    # once instead of leaving a cycle for the garbage collector.
+    self.eng = weakref.proxy(eng)
     self.lib = eng._lib
     self.m = eng._model
     dev = eng.device
@@ -143,24 +146,42 @@ class Backward:
       g0 = g1
     return out
 
-  def _pack(self, w: np.ndarray, k_pad: int, n_pad: int) -> torch.Tensor:
+  def _pack(self, w: np.ndarray, k_pad: int, n_pad: int,
+            out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The packed image of w [k, n] zero padded to [k_pad, n_pad], on the device (into `out`)."""
     w = np.ascontiguousarray(w, np.float32)
     nbytes = self.lib.gcb_packed_weight_bytes(k_pad, n_pad)
     img = np.empty([nbytes], np.uint8)
     _native.check(self.lib.gcb_pack_weight_host(w.ctypes.data, w.shape[0], w.shape[1], k_pad, n_pad,
                                                 img.ctypes.data), "gcb_pack_weight_host")
+    if out is not None:
+      return out.copy_(torch.from_numpy(img))
     return torch.as_tensor(img).to(self.dev)
 
   def _pack_transposed(self, info: _MlpInfo) -> None:
+    """Packs the transposed weights of one MLP, into the existing buffers when there are some."""
     p = self.params
+
+    def pack(key, w, k_pad, n_pad):
+      info.t[key] = self._pack(w, k_pad, n_pad, info.t.get(key))
     w1 = np.asarray(p[f"{info.stem}_mlp/~/linear_1"]["w"], np.float32)       # [512, n1_valid]
-    info.t["w1"] = self._pack(w1.T, info.n1, D)                               # [n1, 512]
+    pack("w1", w1.T, info.n1, D)                                               # [n1, 512]
     w0 = np.asarray(p[f"{info.stem}_mlp/~/linear_0"]["w"], np.float32)
     if len(info.k_segs) >= 2 and w0.shape[0] == len(info.k_segs) * D:
       for s in range(len(info.k_segs)):
-        info.t[f"w0_{s}"] = self._pack(w0[s * D:(s + 1) * D].T, D, D)        # block s, transposed
+        pack(f"w0_{s}", w0[s * D:(s + 1) * D].T, D, D)                         # block s, transposed
     elif w0.shape[0] == D:
-      info.t["w0_0"] = self._pack(w0.T, D, D)
+      pack("w0_0", w0.T, D, D)
+    if "w0_in" in info.t:                                  # the grid embedder's input transpose
+      pack("w0_in", w0.T, D, self.n_in_t)
+
+  def load_params(self, params, stems) -> None:
+    """The engine's weights were rewritten (Engine.load_params): repacks the transposed weights of
+    the MLPs whose module path stem is in `stems`, in place."""
+    self.params = params
+    for info in self._all:
+      if info.stem in stems:
+        self._pack_transposed(info)
 
   def input_transposed(self):
     """(packed [512, n] transpose of the grid embedder's first layer, n): the dX product of the grid

@@ -112,6 +112,7 @@ class Engine:
     # updates, aggregation and the decoder cover the owned rows only.  0 = every row is owned.
     self.num_grid_owned, self.num_mesh_owned = int(num_grid_owned), int(num_mesh_owned)
     self._keep = []                       # device tensors referenced by raw pointer
+    self._weights = {}                    # weight buffer groups, rewritten by load_params
     self._model = _native.Model()
     self._upload_graph(g)
     self._upload_weights(params)
@@ -178,7 +179,7 @@ class Engine:
 
   # -- weights ---------------------------------------------------------------------
   def _pack_linear(self, w: np.ndarray, seg_real, seg_pad, n_pad: int):
-    """w [sum(seg_real), n_real] -> (packed image tensor, fp32 padded tensor).
+    """w [sum(seg_real), n_real] -> (packed image, fp32 padded weight), host arrays.
 
     Rows are re-laid so that segment s occupies seg_pad[s] rows (zero padded)."""
     w = np.asarray(w, np.float32)
@@ -196,55 +197,108 @@ class Engine:
     img = np.empty([nbytes], np.uint8)
     _native.check(self._lib.gcb_pack_weight_host(
         wp.ctypes.data, k_pad, n_pad, k_pad, n_pad, img.ctypes.data), "gcb_pack_weight_host")
-    return self._dev(img, torch.uint8), self._dev(wp, torch.float32), k_pad
+    return img, wp
+
+  def _upload_group(self, key, build, params, sources) -> dict:
+    """Uploads the host arrays build(self, params) of one group of weight buffers and remembers how
+    to rebuild them in place (load_params).  sources: the (module, field) parameters they are made of.
+    `build` takes the engine as an argument rather than closing over it: the engine keeps `build`, and
+    a cycle would keep a dropped engine's device memory alive until the garbage collector ran."""
+    bufs = {name: self._dev(a, torch.uint8 if a.dtype == np.uint8 else torch.float32)
+            for name, a in build(self, params).items()}
+    copies = [np.array(params[n][f], np.float32) for n, f in sources]
+    self._weights[key] = (build, bufs, sources, copies)
+    return bufs
 
   def _make_mlp(self, params, stem: str, seg_real, seg_pad, n1_real: int,
                 layer_norm: bool) -> _native.Mlp:
-    def get(name, field):
+    def get(params, name, field):
       try:
         return np.asarray(params[name][field], np.float32)
       except KeyError as e:
         raise KeyError(f"missing parameter {name}:{field}") from e
     if f"{stem}_mlp/~/linear_2" in params:
       raise ValueError("only hidden_layers=1 MLPs are supported")
-    w0, b0 = get(f"{stem}_mlp/~/linear_0", "w"), get(f"{stem}_mlp/~/linear_0", "b")
-    w1, b1 = get(f"{stem}_mlp/~/linear_1", "w"), get(f"{stem}_mlp/~/linear_1", "b")
-    if w0.shape[1] != LATENT or w1.shape[0] != LATENT:
-      raise ValueError(f"{stem}: only latent/hidden size {LATENT} is supported")
-    if w1.shape[1] != n1_real:
-      raise ValueError(f"{stem}: output width {w1.shape[1]} != expected {n1_real}")
+    l0, l1, ln = f"{stem}_mlp/~/linear_0", f"{stem}_mlp/~/linear_1", f"{stem}_layer_norm"
     n1_pad = 512 if n1_real > 256 else 256
     if n1_real == LATENT:
       n1_pad = 512
-    mlp = _native.Mlp()
-    img0, f0, k0 = self._pack_linear(w0, seg_real, seg_pad, LATENT)
-    img1, f1, _ = self._pack_linear(w1, [LATENT], [LATENT], n1_pad)
     pad = lambda v, n: np.concatenate([v, np.zeros([n - v.shape[0]], np.float32)])
-    mlp.w0_packed, mlp.w0_f32 = self._ptr(img0), self._ptr(f0)
-    mlp.b0 = self._ptr(self._dev(b0, torch.float32))
-    mlp.w1_packed, mlp.w1_f32 = self._ptr(img1), self._ptr(f1)
-    mlp.b1 = self._ptr(self._dev(pad(b1, n1_pad), torch.float32))
+
+    def build(eng, params):
+      w0, w1 = get(params, l0, "w"), get(params, l1, "w")
+      if w0.shape[1] != LATENT or w1.shape[0] != LATENT:
+        raise ValueError(f"{stem}: only latent/hidden size {LATENT} is supported")
+      if w1.shape[1] != n1_real:
+        raise ValueError(f"{stem}: output width {w1.shape[1]} != expected {n1_real}")
+      out = {}
+      out["w0_packed"], out["w0_f32"] = eng._pack_linear(w0, seg_real, seg_pad, LATENT)
+      out["w1_packed"], out["w1_f32"] = eng._pack_linear(w1, [LATENT], [LATENT], n1_pad)
+      out["b0"], out["b1"] = get(params, l0, "b"), pad(get(params, l1, "b"), n1_pad)
+      if layer_norm:
+        out["ln_scale"] = pad(get(params, ln, "scale"), n1_pad)
+        out["ln_offset"] = pad(get(params, ln, "offset"), n1_pad)
+      return out
+    sources = [(l0, "w"), (l0, "b"), (l1, "w"), (l1, "b")]
     if layer_norm:
-      mlp.ln_scale = self._ptr(self._dev(pad(get(f"{stem}_layer_norm", "scale"), n1_pad),
-                                         torch.float32))
-      mlp.ln_offset = self._ptr(self._dev(pad(get(f"{stem}_layer_norm", "offset"), n1_pad),
-                                          torch.float32))
-    mlp.k0, mlp.n1, mlp.n1_valid = k0, n1_pad, n1_real
+      sources += [(ln, "scale"), (ln, "offset")]
+    bufs = self._upload_group(stem, build, params, sources)
+    mlp = _native.Mlp()
+    for name, t in bufs.items():
+      setattr(mlp, name, self._ptr(t))
+    mlp.k0, mlp.n1, mlp.n1_valid = sum(seg_pad), n1_pad, n1_real
     return mlp
 
   def _make_split(self, params, stem: str) -> _native.MlpSplit:
     """Row blocks [edge | sender | receiver] of a [1536,512] first edge-MLP layer
     (concat order of the reference, typed_graph_net.py:637-638), each packed alone."""
-    w0 = np.asarray(params[f"{stem}_mlp/~/linear_0"]["w"], np.float32)
+    l0 = f"{stem}_mlp/~/linear_0"
     D = LATENT
-    if w0.shape != (3 * D, D):
-      raise ValueError(f"{stem}: expected a [{3 * D},{D}] first layer")
+
+    def build(eng, params):
+      w0 = np.asarray(params[l0]["w"], np.float32)
+      if w0.shape != (3 * D, D):
+        raise ValueError(f"{stem}: expected a [{3 * D},{D}] first layer")
+      out = {}
+      for name, block in (("we", w0[:D]), ("ws", w0[D:2 * D]), ("wr", w0[2 * D:])):
+        out[f"{name}_packed"], out[f"{name}_f32"] = eng._pack_linear(block, [D], [D], D)
+      return out
+    bufs = self._upload_group((stem, "split"), build, params, [(l0, "w")])
     sp = _native.MlpSplit()
-    for name, block in (("we", w0[:D]), ("ws", w0[D:2 * D]), ("wr", w0[2 * D:])):
-      img, f32, _ = self._pack_linear(block, [D], [D], D)
-      setattr(sp, f"{name}_packed", self._ptr(img))
-      setattr(sp, f"{name}_f32", self._ptr(f32))
+    for name, t in bufs.items():
+      setattr(sp, name, self._ptr(t))
     return sp
+
+  def load_params(self, params: Mapping[str, Mapping[str, np.ndarray]]) -> None:
+    """Rewrites every weight buffer from `params`, which must have the shapes of the current ones:
+    packed and fp32 weights, padded biases and LayerNorm vectors, the pre-gathered split blocks, and
+    the transposed weights of the gradient workspace if it exists.  The device pointers stay the
+    same, so the recorded step graph stays valid and device memory does not grow.  Groups whose
+    arrays equal what was loaded last are not repacked.  Raises ValueError on a missing parameter or
+    a shape mismatch, before anything is written."""
+    for name, fields in self._params.items():
+      for f, a in fields.items():
+        try:
+          b = params[name][f]
+        except KeyError:
+          raise ValueError(f"missing parameter {name}:{f}") from None
+        if np.shape(b) != np.shape(a):
+          raise ValueError(f"{name}:{f} has shape {np.shape(b)}, the engine holds {np.shape(a)}")
+    changed = set()
+    for key, (build, bufs, sources, copies) in self._weights.items():
+      new = [np.asarray(params[n][f], np.float32) for n, f in sources]
+      if all(np.array_equal(a, c) for a, c in zip(new, copies)):
+        continue
+      with self._on_device():
+        for name, a in build(self, params).items():
+          bufs[name].copy_(torch.from_numpy(a))
+      for c, a in zip(copies, new):
+        c[...] = a
+      changed.add(key if isinstance(key, str) else key[0])
+    self._params = params
+    if self._backward is not None:
+      with self._on_device():
+        self._backward.load_params(params, changed)
 
   def _upload_weights(self, params) -> None:
     m = self._model

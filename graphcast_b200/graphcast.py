@@ -177,8 +177,15 @@ class GraphCast(Predictor):
 
   # -- parameters ------------------------------------------------------------------
   def set_params(self, params: Mapping[str, Mapping[str, np.ndarray]]) -> None:
+    """New weights.  An engine that exists already is reloaded in place (Engine.load_params) when
+    the shapes match: no graph upload, no new workspace.  Otherwise it is dropped and the next call
+    builds one."""
+    if self._engine is not None:
+      try:
+        self._engine.load_params(params)
+      except ValueError:
+        self._engine = None
     self._params = params
-    self._engine = None
 
   def set_precision(self, precision: str) -> None:
     """Arithmetic mode of the fused layers: "bf16x3" (parity), "bf16", "fp32_simt"."""

@@ -243,25 +243,70 @@ def _compare(got, ref, params, tol):
   return worst
 
 
-@pytest.mark.parametrize("prec,tol,chunk_rows", [("bf16x3", 1e-4, None), ("bf16x3", 1e-4, 2000),
-                                                 ("bf16", 5e-2, None)])
-def test_model_grads_against_fp64_autograd(prec, tol, chunk_rows):
-  g, params, x = _cases.small_case(c_in=31, n_out=23, msg_steps=3, batch=2, randomize_affine=True)
-  n_lat = 46
-  assert g.num_grid_nodes % n_lat == 0
+_REFERENCE = {}          # fp64 autograd gradients of a small case, shared by its engine variants
+
+
+def _small_grad_case(res, mesh_size):
+  """The small case on a res-degree grid: graph, params, inputs, targets, latitude weights, coef, and
+  the fp64 autograd reference (computed once per grid)."""
+  g, params, x = _cases.small_case(c_in=31, n_out=23, msg_steps=3, batch=2, res=res,
+                                   mesh_size=mesh_size, randomize_affine=True)
+  n_lat = len(g.grid_lat)
+  assert g.num_grid_nodes == n_lat * len(g.grid_lon)
   lat_w = _lat_weight(np.linspace(-90, 90, n_lat))
   rng = np.random.default_rng(7)
   targets = rng.standard_normal((g.num_grid_nodes, 2, 23)).astype(np.float32)
   kappa = rng.uniform(0.5, 2.0, 23) / (23 * g.num_grid_nodes)
   coef = 2 * kappa / 2                                       # 2 kappa / batch
-  eng = engine.Engine(g, params, c_in=31, n_out=23, msg_steps=3, precision=prec)
+  if (res, mesh_size) not in _REFERENCE:
+    _REFERENCE[(res, mesh_size)] = _oracle_grads(g, params, x, targets, lat_w, coef)
+  return g, params, x, targets, lat_w, coef, _REFERENCE[(res, mesh_size)]
+
+
+def _chunk_plan(eng):
+  """Counts over the grid2mesh and mesh2grid edge chunks of the backward pass: chunks, chunks with
+  heavy receivers (> 256 edges), single-receiver chunks larger than chunk_rows, chunks whose sender
+  CSR has heavy senders."""
+  chunks = eng._backward.chunks["g2m"] + eng._backward.chunks["m2g"]
+  cr = eng._backward.chunk_rows
+  return {"chunks": len(chunks),
+          "heavy_receivers": sum(c[6] > 0 for c in chunks),
+          "oversized": sum(c[3] - c[2] == 1 and c[1] - c[0] > cr for c in chunks),
+          "heavy_senders": sum(c[7][3] > 0 for c in chunks)}
+
+
+_MODES = [{"fuse": False}, {"image_residual": False}, {"deep_chains": False}, {"chain_lag": 1},
+          {"chain_lag": 2}, {"reorder_mesh": True}]
+
+
+@pytest.mark.parametrize("prec,tol,chunk_rows,res,mode", [
+    pytest.param("bf16x3", 1e-4, None, 4.0, {}, id="bf16x3-0.0001-None"),
+    pytest.param("bf16x3", 1e-4, 2000, 4.0, {}, id="bf16x3-0.0001-2000"),
+    pytest.param("bf16", 5e-2, None, 4.0, {}, id="bf16-0.05-None"),
+    # 2 deg / mesh 3: in-degree up to 467 and mesh2grid out-degree up to 757, so the chunks meet
+    # heavy receivers, receivers with more edges than chunk_rows and heavy senders
+    pytest.param("bf16x3", 1e-4, None, 2.0, {}, id="2deg-bf16x3-0.0001-None"),
+    pytest.param("bf16x3", 1e-4, 300, 2.0, {}, id="2deg-bf16x3-0.0001-300"),
+] + [pytest.param("bf16x3", 1e-4, None, 4.0, m, id="-".join(f"{k}={v}" for k, v in m.items()))
+     for m in _MODES])
+def test_model_grads_against_fp64_autograd(prec, tol, chunk_rows, res, mode):
+  g, params, x, targets, lat_w, coef, ref = _small_grad_case(res, 3)
+  eng = engine.Engine(g, params, c_in=31, n_out=23, msg_steps=3, precision=prec, **mode)
   got, sums = _engine_grads(eng, x, targets, lat_w, coef, chunk_rows)
+  plan = _chunk_plan(eng)
   if chunk_rows:                                  # several receiver-aligned edge chunks
     assert len(eng._backward.chunks["m2g"]) > 3 and len(eng._backward.chunks["g2m"]) > 3
-  ref = _oracle_grads(g, params, x, targets, lat_w, coef)
+  if res == 2.0:
+    assert plan["heavy_receivers"] > 0
+    if chunk_rows:
+      assert plan["oversized"] > 0
+    else:                                         # a chunk holds all of a heavy sender's edges
+      assert plan["heavy_senders"] > 0
   assert set(got) == set(params)
   worst = _compare(got, ref, params, tol)
-  print(f"{prec}, chunk_rows={chunk_rows}: max per-tensor relative error {max(worst.values()):.3g}")
+  name, err = max(worst.items(), key=lambda kv: kv[1])
+  print(f"{res} deg, {prec}, chunk_rows={chunk_rows}, {mode or 'default mode'}: max per-tensor "
+        f"relative error {err:.3g} ({name[0]}:{name[1]}); chunk plan {plan}")
   dead = "mesh2grid_gnn/~_networks_builder/processor_nodes_0_mesh_nodes_mlp/~/linear_0"
   assert torch.count_nonzero(got[dead]["w"]) == 0
   again, sums2 = _engine_grads(eng, x, targets, lat_w, coef, chunk_rows)
@@ -269,6 +314,21 @@ def test_model_grads_against_fp64_autograd(prec, tol, chunk_rows):
   for name in got:
     for f in got[name]:
       assert torch.equal(got[name][f], again[name][f]), (name, f)
+  # the stage-wise forward of the gradient is gcb_forward: the same loss sums, bit for bit
+  w = torch.as_tensor(lat_w).to(DEV)
+  for b in range(x.shape[1]):
+    eng.pack_inputs(torch.as_tensor(x[:, b, :].T.copy()).to(DEV))
+    eng.step()
+    step_sums = torch.empty(23, dtype=torch.float64, device=DEV)
+    eng.output_loss(torch.as_tensor(targets[:, b, :].T.copy()).to(DEV), w, channel_sums=step_sums)
+    assert torch.equal(step_sums, sums[b]), b
+
+
+def test_gradients_need_the_pregathered_edge_layers():
+  g, params, _ = _cases.small_case(c_in=31, n_out=23, msg_steps=3)
+  eng = engine.Engine(g, params, c_in=31, n_out=23, msg_steps=3, pregather=False)
+  with pytest.raises(NotImplementedError, match="pregather"):
+    eng.grads_begin()
 
 
 def test_graphcast_loss_and_grads_surface():
@@ -372,59 +432,3 @@ def test_config1_grads_against_fp32_autograd():
   worst = _compare(got, ref, params, 1e-4)
   print(f"config 1: max per-tensor relative error {max(worst.values()):.3g}")
 
-
-def test_full_size_directional_derivative_and_peak_memory():
-  """0.25 deg / 37 levels, one gradient on one H100: along u = g / |g| the central difference of the
-  device loss agrees with |g|; the peak device memory is reported."""
-  if torch.cuda.get_device_properties(0).total_memory < 75e9:
-    pytest.skip("needs an 80 GB GPU")
-  from graphcast_b200 import graphcast, synthetic
-  task = graphcast.TASK
-  lat, lon = synthetic.grid_coords(0.25)
-  g = graph_lib.cached_static_graph(grid_lat=lat, grid_lon=lon, mesh_size=6,
-                                    radius_query_fraction_edge_length=0.6)
-  c_in, n_out = synthetic.num_input_channels(task), graphcast.num_outputs(task)
-  params = graphcast.init_params(graphcast.ModelConfig(0.25, 6, 512, 16, 1, 0.6), task, c_in, seed=1)
-  gen = torch.Generator(device=DEV).manual_seed(0)
-  planes = torch.randn(c_in, g.num_grid_nodes, device=DEV, generator=gen)
-  targets = torch.randn(n_out, g.num_grid_nodes, device=DEV, generator=gen)
-  lat_w = torch.as_tensor(_lat_weight(lat)).to(DEV)
-  kappa = np.random.default_rng(1).uniform(0.5, 2.0, n_out) / (n_out * g.num_grid_nodes)
-  kappa_d = torch.as_tensor(kappa).to(DEV)
-
-  def device_loss(eng):
-    sums = torch.empty(n_out, dtype=torch.float64, device=DEV)
-    eng.pack_inputs(planes)
-    eng.step()
-    eng.output_loss(targets, lat_w, channel_sums=sums)
-    return float((sums * kappa_d).sum())
-
-  eng = engine.Engine(g, params, c_in=c_in, n_out=n_out, msg_steps=16, precision="bf16x3")
-  torch.cuda.synchronize()
-  torch.cuda.reset_peak_memory_stats()
-  eng.grads_begin()
-  sums = torch.empty(n_out, dtype=torch.float64, device=DEV)
-  eng.pack_inputs(planes)
-  eng.loss_and_grads_element(targets, lat_w, torch.as_tensor(2 * kappa).to(DEV), channel_sums=sums)
-  grads = {k: {f: t.double().cpu().numpy() for f, t in v.items()} for k, v in eng.grads().items()}
-  torch.cuda.synchronize()
-  peak = torch.cuda.max_memory_allocated()
-  loss = float((sums * kappa_d).sum())
-  del eng
-  torch.cuda.empty_cache()
-  gnorm = np.sqrt(sum(float((a ** 2).sum()) for v in grads.values() for a in v.values()))
-  eps = 1e-2 * loss / gnorm
-  shifted = []
-  for sign in (1.0, -1.0):
-    p = {k: {f: (np.asarray(a, np.float64) + sign * eps * grads[k][f] / gnorm).astype(np.float32)
-             for f, a in v.items()} for k, v in params.items()}
-    e = engine.Engine(g, p, c_in=c_in, n_out=n_out, msg_steps=16, precision="bf16x3")
-    shifted.append(device_loss(e))
-    del e
-    torch.cuda.empty_cache()
-  fd = (shifted[0] - shifted[1]) / (2 * eps)
-  rel = abs(fd - gnorm) / gnorm
-  print(f"0.25 deg: loss {loss:.6g}, |g| {gnorm:.6g}, central difference {fd:.6g} (relative {rel:.3g}), "
-        f"eps {eps:.3g}; peak device memory {peak / 2**30:.1f} GiB on "
-        f"{torch.cuda.get_device_name(0)}")
-  assert rel <= 1e-2

@@ -151,7 +151,8 @@ def _stats(task, seed=0):
 
   def stats(lo, hi):
     ds = xs.Dataset(coords={"level": levels})
-    for name in set(task.input_variables) | set(task.target_variables) | set(task.forcing_variables):
+    # sorted: the draws go to the same variables in every process (set order follows string hashing)
+    for name in sorted(set(task.input_variables) | set(task.target_variables) | set(task.forcing_variables)):
       if name in graphcast.variables.ALL_ATMOSPHERIC_VARS:
         ds[name] = xs.DataArray(rng.uniform(lo, hi, len(levels)).astype(np.float32), ("level",))
       else:
