@@ -121,6 +121,13 @@ EXPORTS = {
     "gcb_image_rows_pack": (C.c_int, [_fp, _fp, C.c_int64, _fp, _fp]),
     "gcb_image_rows_unpack": (C.c_int, [_fp, C.c_int64, _fp, C.c_int64, _fp]),
     "gcb_pack_weight_host": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp]),
+    "gcb_pack_weight": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                  C.c_int32, _fp, _fp, _fp]),
+    "gcb_sum_squares": (C.c_int, [_fp, C.c_int64, _fp, C.c_int64, _fp, _fp]),
+    "gcb_sum_squares_workspace_bytes": (C.c_int64, []),
+    "gcb_adamw_step": (C.c_int, [_fp, _fp, _fp, _fp, C.c_int64, C.c_int64, C.c_int64, C.c_double,
+                                 C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _fp,
+                                 C.c_double, _fp]),
     "gcb_layer_forward": (C.c_int, [C.POINTER(LayerDesc), _fp]),
     "gcb_segment_sum": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, _fp, C.c_int32, C.c_int32, _fp]),
     "gcb_segment_sum_heavy": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, _fp, C.c_int32, _fp,

@@ -57,7 +57,7 @@ class _MlpInfo:
 class Backward:
   """Gradient workspace and launch sequence of one Engine (created on the first loss_and_grads)."""
 
-  def __init__(self, eng, params, chunk_rows: int = 1 << 19):
+  def __init__(self, eng, chunk_rows: int = 1 << 19):
     if not eng.pregather:
       raise NotImplementedError("parameter gradients need the pre-gathered edge layers (pregather=True)")
     # The engine owns this workspace: a weak reference, so that dropping the engine frees both at
@@ -92,7 +92,7 @@ class Backward:
                             [D] * 3, True, D, D, m.proc_e_mesh_split[k]) for k in range(eng.msg_steps)]
     self.proc_n = [_MlpInfo(_stem("mesh_gnn", f"processor_nodes_{k}_", "mesh_nodes"), m.proc_n_mesh[k],
                             [D] * 2, True, D, D) for k in range(eng.msg_steps)]
-    self.params = params
+    self.shapes = eng.param_shapes
     self._all = list(self.mlps.values()) + self.proc_e + self.proc_n
     for info in self._all:
       self._pack_transposed(info)
@@ -146,57 +146,48 @@ class Backward:
       g0 = g1
     return out
 
-  def _pack(self, w: np.ndarray, k_pad: int, n_pad: int,
-            out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """The packed image of w [k, n] zero padded to [k_pad, n_pad], on the device (into `out`)."""
-    w = np.ascontiguousarray(w, np.float32)
-    nbytes = self.lib.gcb_packed_weight_bytes(k_pad, n_pad)
-    img = np.empty([nbytes], np.uint8)
-    _native.check(self.lib.gcb_pack_weight_host(w.ctypes.data, w.shape[0], w.shape[1], k_pad, n_pad,
-                                                img.ctypes.data), "gcb_pack_weight_host")
-    if out is not None:
-      return out.copy_(torch.from_numpy(img))
-    return torch.as_tensor(img).to(self.dev)
+  def _pack_t(self, info: _MlpInfo, key: str, w: int, ld: int, k: int, n: int, n_cols: int) -> None:
+    """info.t[key] = the packed image of the transpose of the device fp32 matrix at address w (rows of
+    `ld` floats), of padded shape [k, n] (n_cols real columns), written in place when it exists."""
+    if key not in info.t:
+      info.t[key] = torch.empty([self.lib.gcb_packed_weight_bytes(k, n)], dtype=torch.uint8,
+                                device=self.dev)
+    self.eng.pack_weight(w, ld, True, k, n_cols, k, n, info.t[key])
 
   def _pack_transposed(self, info: _MlpInfo) -> None:
-    """Packs the transposed weights of one MLP, into the existing buffers when there are some."""
-    p = self.params
-
-    def pack(key, w, k_pad, n_pad):
-      info.t[key] = self._pack(w, k_pad, n_pad, info.t.get(key))
-    w1 = np.asarray(p[f"{info.stem}_mlp/~/linear_1"]["w"], np.float32)       # [512, n1_valid]
-    pack("w1", w1.T, info.n1, D)                                               # [n1, 512]
-    w0 = np.asarray(p[f"{info.stem}_mlp/~/linear_0"]["w"], np.float32)
-    if len(info.k_segs) >= 2 and w0.shape[0] == len(info.k_segs) * D:
+    """Packs the transposed weights of one MLP on the device, from the engine's zero-padded fp32 weight
+    buffers (so they follow every reload, from host or device): w1^T [n1, 512], and w0^T per 512-row
+    block of the first layer."""
+    w = info.w
+    self._pack_t(info, "w1", w.w1_f32, info.n1, info.n1, D, D)
+    k0 = self.shapes[f"{info.stem}_mlp/~/linear_0"]["w"][0]
+    if len(info.k_segs) >= 2 and k0 == len(info.k_segs) * D:
       for s in range(len(info.k_segs)):
-        pack(f"w0_{s}", w0[s * D:(s + 1) * D].T, D, D)                         # block s, transposed
-    elif w0.shape[0] == D:
-      pack("w0_0", w0.T, D, D)
+        self._pack_t(info, f"w0_{s}", w.w0_f32 + 4 * s * D * D, D, D, D, D)   # block s, transposed
+    elif k0 == D:
+      self._pack_t(info, "w0_0", w.w0_f32, D, D, D, D)
     if "w0_in" in info.t:                                  # the grid embedder's input transpose
-      pack("w0_in", w0.T, D, self.n_in_t)
+      self._pack_t(info, "w0_in", w.w0_f32, D, D, self.n_in_t, self.eng.c_in_pad)
 
-  def load_params(self, params, stems) -> None:
-    """The engine's weights were rewritten (Engine.load_params): repacks the transposed weights of
-    the MLPs whose module path stem is in `stems`, in place."""
-    self.params = params
+  def repack(self, stems=None) -> None:
+    """The engine's weights were rewritten (Engine.load_params / load_params_device): repacks the
+    transposed weights of the MLPs whose module path stem is in `stems` (None: all), in place."""
     for info in self._all:
-      if info.stem in stems:
+      if stems is None or info.stem in stems:
         self._pack_transposed(info)
 
   def input_transposed(self):
     """(packed [512, n] transpose of the grid embedder's first layer, n): the dX product of the grid
-    inputs (backprop through time), n = 256 | 512 >= c_in_pad.  Packed on first use, so the one-step
-    gradient never holds it."""
+    inputs (backprop through time), n = 256 | 512 >= c_in_pad.  Packed on first use, from the
+    engine's current weights, so the one-step gradient never holds it."""
     info = self.mlps["enc_grid"]
     if "w0_in" not in info.t:
       cin = self.eng.c_in_pad
       if cin > 2 * 256:
         raise NotImplementedError(f"input gradients support at most 512 padded input channels, "
                                   f"not {cin}")
-      n = 256 if cin <= 256 else 512
-      w0 = np.asarray(self.params[f"{info.stem}_mlp/~/linear_0"]["w"], np.float32)   # [c_in + 3, 512]
-      info.t["w0_in"] = self._pack(w0.T, D, n)
-      self.n_in_t = n
+      self.n_in_t = 256 if cin <= 256 else 512
+      self._pack_t(info, "w0_in", info.w.w0_f32, D, D, self.n_in_t, cin)   # [512, c_in_pad]
     return info.t["w0_in"], self.n_in_t
 
   def _alloc_grads(self, info: _MlpInfo) -> None:
@@ -525,26 +516,42 @@ class Backward:
     return dx
 
   # -- result ----------------------------------------------------------------------------------------
-  def grads(self) -> Dict[str, Dict[str, torch.Tensor]]:
-    """Device fp32 gradients keyed and shaped like the params; parameters the step never reads (the
-    mesh2grid mesh-node MLP) get zeros."""
+  def _accumulators(self) -> Dict[str, Dict[str, torch.Tensor]]:
+    """The valid slices of the gradient accumulators (views), keyed and shaped like the params; the
+    parameters the step never reads (the mesh2grid mesh-node MLP) are absent."""
     out: Dict[str, Dict[str, torch.Tensor]] = {}
     for info in self._all:
-      p = self.params
       l0, l1 = f"{info.stem}_mlp/~/linear_0", f"{info.stem}_mlp/~/linear_1"
-      k_real = np.asarray(p[l0]["w"]).shape[0]
+      k_real = self.shapes[l0]["w"][0]
       g = info.g
       if len(info.k_segs) == 1:
         w0 = g["w0"][:k_real]
       else:
         w0 = g["w0"]
       n = info.n1_valid
-      out[l0] = {"w": w0.clone(), "b": g["b0"].clone()}
-      out[l1] = {"w": g["w1"][:, :n].clone(), "b": g["b1"][:n].clone()}
+      out[l0] = {"w": w0, "b": g["b0"]}
+      out[l1] = {"w": g["w1"][:, :n], "b": g["b1"][:n]}
       if info.ln:
-        out[f"{info.stem}_layer_norm"] = {"scale": g["scale"].clone(), "offset": g["offset"].clone()}
-    for name, fields in self.params.items():
-      if name not in out:
-        out[name] = {f: torch.zeros(np.asarray(a).shape, dtype=torch.float32, device=self.dev)
-                     for f, a in fields.items()}
+        out[f"{info.stem}_layer_norm"] = {"scale": g["scale"], "offset": g["offset"]}
     return out
+
+  def grads(self) -> Dict[str, Dict[str, torch.Tensor]]:
+    """Device fp32 gradients keyed and shaped like the params; parameters the step never reads (the
+    mesh2grid mesh-node MLP) get zeros."""
+    out = {name: {f: t.clone() for f, t in fields.items()}
+           for name, fields in self._accumulators().items()}
+    for name, fields in self.shapes.items():
+      if name not in out:
+        out[name] = {f: torch.zeros(shape, dtype=torch.float32, device=self.dev)
+                     for f, shape in fields.items()}
+    return out
+
+  def grads_into(self, out) -> None:
+    """The gradients of `grads` copied into the device tensors out[name][field]."""
+    acc = self._accumulators()
+    for name, fields in self.shapes.items():
+      for f in fields:
+        if name in acc:
+          out[name][f].copy_(acc[name][f])
+        else:
+          out[name][f].zero_()

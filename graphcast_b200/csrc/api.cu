@@ -6,6 +6,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -15,6 +16,7 @@
 #include "mlp_tc.cuh"
 #include "mlp_chain.cuh"
 #include "backward_kernels.cuh"
+#include "optim_kernels.cuh"
 
 namespace {
 
@@ -580,6 +582,65 @@ int gcb_pack_weight_host(const float* w, int32_t k_rows, int32_t n_cols, int32_t
             lo[off] = lv;
           }
     }
+  return GCB_OK;
+}
+
+int gcb_pack_weight(const float* w, int32_t ld, int32_t transpose, int32_t k_rows, int32_t n_cols,
+                    int32_t k, int32_t n, void* dst, float* dst_f32, void* stream) {
+  GCB_CHECK_ARG(w != nullptr && dst != nullptr, "null pointer");
+  GCB_CHECK_ARG(k > 0 && k % 16 == 0 && n > 0 && n % 256 == 0, "k must be a multiple of 16, n of 256");
+  GCB_CHECK_ARG(k_rows <= k && n_cols <= n && k_rows >= 0 && n_cols >= 0, "real shape exceeds padded shape");
+  GCB_CHECK_ARG(ld >= (transpose ? k_rows : n_cols), "ld smaller than a source row");
+  GCB_CHECK_ARG(aligned16(dst), "dst unaligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  dim3 grid(static_cast<unsigned>(k / 16), static_cast<unsigned>(n / 256));
+  gcb::pack_weight_kernel<<<grid, 256, 0, st>>>(w, ld, transpose ? 1 : 0, k_rows, n_cols, n,
+                                                static_cast<uint16_t*>(dst), dst_f32);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int64_t gcb_sum_squares_workspace_bytes(void) {
+  return static_cast<int64_t>(gcb::kSumGroups) * static_cast<int64_t>(sizeof(double));
+}
+
+int gcb_sum_squares(const float* x, int64_t n, void* workspace, int64_t workspace_bytes, double* out,
+                    void* stream) {
+  GCB_CHECK_ARG(workspace && out && (x || n == 0), "null pointer");
+  GCB_CHECK_ARG(n >= 0, "n < 0");
+  GCB_CHECK_ARG(workspace_bytes >= gcb_sum_squares_workspace_bytes(), "workspace too small");
+  GCB_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 7u) == 0 &&
+                (reinterpret_cast<uintptr_t>(out) & 7u) == 0, "unaligned fp64 buffer");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  double* partial = static_cast<double*>(workspace);
+  gcb::sum_squares_kernel<<<gcb::kSumGroups, 256, 0, st>>>(x, n, partial);
+  GCB_CUDA(cudaGetLastError());
+  gcb::sum_partials_kernel<<<1, 256, 0, st>>>(partial, out);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int gcb_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, int64_t n_decay, int64_t t,
+                   double learning_rate, double b1, double b2, double eps, double eps_root,
+                   double weight_decay, const double* sumsq, double max_norm, void* stream) {
+  GCB_CHECK_ARG((p && g && m && v) || n == 0, "null pointer");
+  GCB_CHECK_ARG(n >= 0 && n_decay >= 0 && n_decay <= n, "n_decay out of [0, n]");
+  GCB_CHECK_ARG(t >= 1, "the step count t starts at 1");
+  GCB_CHECK_ARG(b1 >= 0.0 && b1 < 1.0 && b2 >= 0.0 && b2 < 1.0, "b1, b2 must lie in [0, 1)");
+  GCB_CHECK_ARG(!(max_norm > 0.0) || sumsq != nullptr, "clipping needs the sum of squares");
+  if (n == 0) return GCB_OK;
+  gcb::AdamWArgs a;
+  a.lr = learning_rate; a.b1 = b1; a.b2 = b2; a.eps = eps; a.eps_root = eps_root;
+  a.weight_decay = weight_decay; a.max_norm = max_norm > 0.0 ? max_norm : 0.0;
+  a.bc1 = 1.0 - pow(b1, static_cast<double>(t));
+  a.bc2 = 1.0 - pow(b2, static_cast<double>(t));
+  a.n = n; a.n_decay = n_decay;
+  const int vec4 = (aligned16(p) && aligned16(g) && aligned16(m) && aligned16(v)) ? 1 : 0;
+  const long long work = vec4 ? (n + 3) / 4 : n;
+  const long long blocks = std::min<long long>((work + 255) / 256, 16LL * sm_count_cached());
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  gcb::adamw_kernel<<<static_cast<unsigned>(blocks), 256, 0, st>>>(p, g, m, v, sumsq, a, vec4);
+  GCB_CUDA(cudaGetLastError());
   return GCB_OK;
 }
 

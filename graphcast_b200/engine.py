@@ -118,7 +118,14 @@ class Engine:
     self._upload_weights(params)
     self._alloc_workspace()
     self.launches_per_step = 0
-    self._params = params                 # host dict: transposed weights of the backward pass
+    self.param_shapes = {name: {f: tuple(np.shape(a)) for f, a in fields.items()}
+                         for name, fields in params.items()}
+    # The host dict of the weights (see `params`).  After load_params_device it is stale until read,
+    # and so are the host copies by which load_params skips unchanged groups.
+    self._host_params = params
+    self._params_stale = False
+    self._copies_stale = False
+    self.weights_version = 0              # counts the reloads (load_params, load_params_device)
     self._backward = None                 # gradient workspace, created by the first loss_and_grads
 
   # -- helpers -------------------------------------------------------------------
@@ -199,15 +206,42 @@ class Engine:
         wp.ctypes.data, k_pad, n_pad, k_pad, n_pad, img.ctypes.data), "gcb_pack_weight_host")
     return img, wp
 
-  def _upload_group(self, key, build, params, sources) -> dict:
+  def pack_weight(self, w: int, ld: int, transpose: bool, k_rows: int, n_cols: int, k: int, n: int,
+                  img: torch.Tensor, f32: Optional[torch.Tensor] = None) -> None:
+    """gcb_pack_weight on the current stream: the device fp32 matrix at address w (rows of `ld`
+    floats, read transposed with `transpose`) -> the packed image `img` of padded shape [k, n] and,
+    optionally, the zero-padded fp32 copy `f32` [k, n]."""
+    _native.check(self._lib.gcb_pack_weight(w, ld, 1 if transpose else 0, k_rows, n_cols, k, n,
+                                            img.data_ptr(), self._ptr(f32), self._stream()),
+                  "gcb_pack_weight")
+
+  def _pack_linear_device(self, w: torch.Tensor, seg_real, seg_pad, img: torch.Tensor,
+                          f32: torch.Tensor) -> None:
+    """The device twin of _pack_linear, into the existing buffers: one launch per padded segment
+    (one in all for the unpadded multi-segment layers)."""
+    k_real, n_real = w.shape
+    n_pad = f32.shape[1]
+    if list(seg_real) == list(seg_pad):
+      seg_real = seg_pad = [k_real]
+    src = dst = 0
+    for real, pad in zip(seg_real, seg_pad):
+      self.pack_weight(w.data_ptr() + 4 * src * n_real, n_real, False, real, n_real, pad, n_pad,
+                       img[4 * dst * n_pad:], f32[dst:])
+      src += real
+      dst += pad
+
+  def _upload_group(self, key, build, device_build, read, params, sources) -> dict:
     """Uploads the host arrays build(self, params) of one group of weight buffers and remembers how
-    to rebuild them in place (load_params).  sources: the (module, field) parameters they are made of.
-    `build` takes the engine as an argument rather than closing over it: the engine keeps `build`, and
-    a cycle would keep a dropped engine's device memory alive until the garbage collector ran."""
+    to rebuild them in place: from host arrays (load_params) and, with device_build(self, params,
+    bufs), from device tensors (load_params_device).  read(self, bufs) -> {(module, field): device
+    tensor} recovers the parameters the buffers hold (the `params` refresh).  sources: the (module,
+    field) parameters they are made of.  The callables take the engine as an argument rather than
+    closing over it: the engine keeps them, and a cycle would keep a dropped engine's device memory
+    alive until the garbage collector ran."""
     bufs = {name: self._dev(a, torch.uint8 if a.dtype == np.uint8 else torch.float32)
             for name, a in build(self, params).items()}
     copies = [np.array(params[n][f], np.float32) for n, f in sources]
-    self._weights[key] = (build, bufs, sources, copies)
+    self._weights[key] = (build, device_build, read, bufs, sources, copies)
     return bufs
 
   def _make_mlp(self, params, stem: str, seg_real, seg_pad, n1_real: int,
@@ -239,10 +273,30 @@ class Engine:
         out["ln_scale"] = pad(get(params, ln, "scale"), n1_pad)
         out["ln_offset"] = pad(get(params, ln, "offset"), n1_pad)
       return out
+
+    def device_build(eng, params, bufs):      # the padding of every buffer stays zero
+      eng._pack_linear_device(params[l0]["w"], seg_real, seg_pad, bufs["w0_packed"], bufs["w0_f32"])
+      eng._pack_linear_device(params[l1]["w"], [LATENT], [LATENT], bufs["w1_packed"], bufs["w1_f32"])
+      bufs["b0"].copy_(params[l0]["b"])
+      bufs["b1"][:n1_real].copy_(params[l1]["b"])
+      if layer_norm:
+        bufs["ln_scale"][:n1_real].copy_(params[ln]["scale"])
+        bufs["ln_offset"][:n1_real].copy_(params[ln]["offset"])
+
+    def read(eng, bufs):
+      w0, rows, dst = bufs["w0_f32"], [], 0
+      for real, padded in zip(seg_real, seg_pad):
+        rows.append(w0[dst:dst + real])
+        dst += padded
+      out = {(l0, "w"): torch.cat(rows), (l0, "b"): bufs["b0"],
+             (l1, "w"): bufs["w1_f32"][:, :n1_real], (l1, "b"): bufs["b1"][:n1_real]}
+      if layer_norm:
+        out[(ln, "scale")], out[(ln, "offset")] = bufs["ln_scale"][:n1_real], bufs["ln_offset"][:n1_real]
+      return out
     sources = [(l0, "w"), (l0, "b"), (l1, "w"), (l1, "b")]
     if layer_norm:
       sources += [(ln, "scale"), (ln, "offset")]
-    bufs = self._upload_group(stem, build, params, sources)
+    bufs = self._upload_group(stem, build, device_build, read, params, sources)
     mlp = _native.Mlp()
     for name, t in bufs.items():
       setattr(mlp, name, self._ptr(t))
@@ -263,7 +317,14 @@ class Engine:
       for name, block in (("we", w0[:D]), ("ws", w0[D:2 * D]), ("wr", w0[2 * D:])):
         out[f"{name}_packed"], out[f"{name}_f32"] = eng._pack_linear(block, [D], [D], D)
       return out
-    bufs = self._upload_group((stem, "split"), build, params, [(l0, "w")])
+
+    def device_build(eng, params, bufs):      # row block i: a pointer offset into w0
+      w0 = params[l0]["w"]
+      for i, name in enumerate(("we", "ws", "wr")):
+        eng.pack_weight(w0.data_ptr() + 4 * i * D * D, D, False, D, D, D, D, bufs[f"{name}_packed"],
+                        bufs[f"{name}_f32"])
+    bufs = self._upload_group((stem, "split"), build, device_build, lambda eng, bufs: {}, params,
+                              [(l0, "w")])
     sp = _native.MlpSplit()
     for name, t in bufs.items():
       setattr(sp, name, self._ptr(t))
@@ -276,18 +337,11 @@ class Engine:
     same, so the recorded step graph stays valid and device memory does not grow.  Groups whose
     arrays equal what was loaded last are not repacked.  Raises ValueError on a missing parameter or
     a shape mismatch, before anything is written."""
-    for name, fields in self._params.items():
-      for f, a in fields.items():
-        try:
-          b = params[name][f]
-        except KeyError:
-          raise ValueError(f"missing parameter {name}:{f}") from None
-        if np.shape(b) != np.shape(a):
-          raise ValueError(f"{name}:{f} has shape {np.shape(b)}, the engine holds {np.shape(a)}")
+    self._check_params(params, lambda b: np.shape(b))
     changed = set()
-    for key, (build, bufs, sources, copies) in self._weights.items():
+    for key, (build, _, _, bufs, sources, copies) in self._weights.items():
       new = [np.asarray(params[n][f], np.float32) for n, f in sources]
-      if all(np.array_equal(a, c) for a, c in zip(new, copies)):
+      if not self._copies_stale and all(np.array_equal(a, c) for a, c in zip(new, copies)):
         continue
       with self._on_device():
         for name, a in build(self, params).items():
@@ -295,10 +349,67 @@ class Engine:
       for c, a in zip(copies, new):
         c[...] = a
       changed.add(key if isinstance(key, str) else key[0])
-    self._params = params
+    self._host_params, self._params_stale, self._copies_stale = params, False, False
+    self.weights_version += 1
     if self._backward is not None:
       with self._on_device():
-        self._backward.load_params(params, changed)
+        self._backward.repack(changed)
+
+  def load_params_device(self, params: Mapping[str, Mapping[str, torch.Tensor]]) -> None:
+    """load_params from device tensors: `params` shaped like the params, contiguous fp32 tensors on
+    this engine's device (views into one flat buffer are fine).  Rewrites the same buffers on the
+    device, on the current stream and without a host synchronisation: the packed images and fp32
+    copies through gcb_pack_weight, the padded biases and LayerNorm vectors, the split blocks and the
+    backward pass's transposed weights.  Pointers stay the same and nothing is allocated.  Raises
+    ValueError on a missing parameter or a shape, dtype or device mismatch, before anything is
+    written.  Afterwards `params` and the host copies of load_params are stale: the next read of
+    `params` refreshes it from the device, and the next load_params repacks every group."""
+    def shape(t):
+      if not (isinstance(t, torch.Tensor) and t.dtype == torch.float32 and t.device == self.device
+              and t.is_contiguous()):
+        raise ValueError(f"load_params_device takes contiguous float32 tensors on {self.device}")
+      return tuple(t.shape)
+    self._check_params(params, shape)
+    with self._on_device():
+      for build, device_build, _, bufs, _, _ in self._weights.values():
+        device_build(self, params, bufs)
+      if self._backward is not None:
+        self._backward.repack()
+    self._params_stale = self._copies_stale = True
+    self.weights_version += 1
+
+  def _check_params(self, params, shape) -> None:
+    for name, fields in self.param_shapes.items():
+      for f, want in fields.items():
+        try:
+          b = params[name][f]
+        except KeyError:
+          raise ValueError(f"missing parameter {name}:{f}") from None
+        if shape(b) != want:
+          raise ValueError(f"{name}:{f} has shape {shape(b)}, the engine holds {want}")
+
+  @property
+  def params(self) -> Mapping[str, Mapping[str, np.ndarray]]:
+    """The host dict of the weights the engine holds: the dict of the last load_params (or of the
+    constructor), or, after load_params_device, a refresh from the engine's fp32 weight buffers, made
+    on first read with one device-to-host copy.  Parameters the step never reads (the mesh2grid
+    mesh-node MLP) keep their last host values."""
+    if self._params_stale:
+      held = {}
+      for _, _, read, bufs, _, _ in self._weights.values():
+        held.update(read(self, bufs))
+      keys = sorted(held)
+      with self._on_device():
+        flat = torch.cat([held[k].reshape(-1) for k in keys]).cpu().numpy()
+      new = {name: dict(fields) for name, fields in self._host_params.items()}
+      off = 0
+      for name, f in keys:
+        shape = self.param_shapes[name][f]
+        size = int(np.prod(shape))
+        new[name][f] = flat[off:off + size].reshape(shape)
+        off += size
+      self._host_params, self._params_stale = new, False
+    return self._host_params
 
   def _upload_weights(self, params) -> None:
     m = self._model
@@ -537,8 +648,8 @@ class Engine:
       from graphcast_b200 import backward
       self._backward = None
       with self._on_device():
-        self._backward = (backward.Backward(self, self._params, chunk_rows) if chunk_rows
-                          else backward.Backward(self, self._params))
+        self._backward = (backward.Backward(self, chunk_rows) if chunk_rows
+                          else backward.Backward(self))
     self._backward.prec = _native.PRECISIONS[self.precision]
     self._backward.zero_grads()
 
@@ -622,6 +733,13 @@ class Engine:
   def grads(self):
     """The accumulated gradients: device fp32 tensors keyed and shaped like the params."""
     return self._backward.grads()
+
+  def grads_into(self, out: Mapping[str, Mapping[str, torch.Tensor]]) -> None:
+    """The accumulated gradients copied into `out`, device tensors keyed and shaped like the params
+    (e.g. views into an optimiser's flat buffer): the valid slices of the accumulators, no copy in
+    between; zeros for the parameters the step never reads."""
+    with self._on_device():
+      self._backward.grads_into(out)
 
   def feedback(self, plan, add_plane_index=None, in_scale: Optional[torch.Tensor] = None) -> "Feedback":
     """Backprop-through-time state of one batch element for a feedback.FeedbackPlan (host) of this

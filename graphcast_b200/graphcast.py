@@ -154,11 +154,14 @@ class GraphCast(Predictor):
     self._fuse, self._chain_lag, self._image_residual = fuse, chain_lag, image_residual
     self._deep_chains = deep_chains
     self._device = device
+    self._engine: Optional[engine_lib.Engine] = None
     self._params = params
+    # Where the gradients of _loss_and_grads / _bptt_grads go: None = host numpy dicts (the public
+    # loss_and_grads), else a callable(engine) that takes them on the device (optim.AdamW).
+    self._grad_sink = None
     self._num_outputs = num_outputs(task_config)
     self._initialized = False
     self._static_graph: Optional[graph_lib.StaticGraph] = None
-    self._engine: Optional[engine_lib.Engine] = None
     self._planes_in: Optional[torch.Tensor] = None
     self._planes_out: Optional[torch.Tensor] = None
     # Host->device staging: two input-plane buffers filled on a dedicated copy stream, so
@@ -176,6 +179,16 @@ class GraphCast(Predictor):
     self._channel_sums: Optional[torch.Tensor] = None
 
   # -- parameters ------------------------------------------------------------------
+  @property
+  def _params(self):
+    """The host parameters: while an engine exists, the engine's (Engine.params, which follows
+    device reloads); otherwise those of the constructor or the last set_params."""
+    return self._engine.params if self._engine is not None else self._host_params
+
+  @_params.setter
+  def _params(self, params) -> None:
+    self._host_params = params
+
   def set_params(self, params: Mapping[str, Mapping[str, np.ndarray]]) -> None:
     """New weights.  An engine that exists already is reloaded in place (Engine.load_params) when
     the shapes match: no graph upload, no new workspace.  Otherwise it is dropped and the next call
@@ -268,9 +281,15 @@ class GraphCast(Predictor):
                grad_coef=coef)
     loss, diagnostics = losses.losses_from_channel_sums(
         self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
-    grads = {name: {f: t.cpu().numpy() for f, t in fields.items()}
-             for name, fields in self._engine.grads().items()}
-    return loss, diagnostics, grads
+    return loss, diagnostics, self._export_grads()
+
+  def _export_grads(self):
+    """The engine's accumulated gradients as host numpy dicts, or, with a _grad_sink, whatever the
+    sink returns after taking them on the device."""
+    if self._grad_sink is not None:
+      return self._grad_sink(self._engine)
+    return {name: {f: t.cpu().numpy() for f, t in fields.items()}
+            for name, fields in self._engine.grads().items()}
 
   def _stash_step(self, stash: "StepStash") -> None:
     """Keeps the input and target planes of the last `_call` (with targets) in pinned host memory."""
@@ -315,8 +334,7 @@ class GraphCast(Predictor):
                         add_plane_index=norm.add_plane_index)
         eng.loss_and_grads_element(tgt, lat_weight, coef_dev, channel_sums=scratch, feedback=fb,
                                    input_grad=t > 0, **affine)
-    return {name: {f: t.cpu().numpy() for f, t in fields.items()}
-            for name, fields in eng.grads().items()}
+    return self._export_grads()
 
   def _loss(self, inputs, targets, forcings, norm: Optional[FusedNormalization], predictions: bool):
     finish, preds, sums = self._device_loss(inputs, targets, forcings, norm, predictions)

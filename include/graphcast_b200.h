@@ -157,6 +157,38 @@ int64_t gcb_packed_weight_bytes(int32_t k, int32_t n);
 int gcb_pack_weight_host(const float* w, int32_t k_rows, int32_t n_cols, int32_t k, int32_t n,
                          void* dst);
 
+/* Device packing, byte-identical to gcb_pack_weight_host (padding included): the logical W[k_rows,
+ * n_cols] is w[r * ld + c] (device fp32), or w[c * ld + r] with `transpose` (the transposed weights
+ * of the backward pass), so row blocks and transposes of a larger matrix are packed through a
+ * pointer offset and `ld` without a copy.  dst: gcb_packed_weight_bytes(k, n) bytes, 16-byte
+ * aligned.  dst_f32 (optional, NULL = none): also the zero-padded fp32 [k, n] copy of W, row-major
+ * (the engine's fp32 weight buffers).  One launch on `stream`. */
+int gcb_pack_weight(const float* w, int32_t ld, int32_t transpose, int32_t k_rows, int32_t n_cols,
+                    int32_t k, int32_t n, void* dst, float* dst_f32, void* stream);
+
+/* ---- optimiser (graphcast_b200/optim.py) ---------------------------------------------------
+ * out[0] = sum of x[i]^2 over a flat fp32 buffer of n elements, in fp64 (the squares are exact), on
+ * the device.  A fixed split of the elements into groups and fixed-order reductions, no atomics:
+ * bit-identical run to run and on any device.  workspace: gcb_sum_squares_workspace_bytes() bytes,
+ * 8-byte aligned.  Two launches on `stream`. */
+int gcb_sum_squares(const float* x, int64_t n, void* workspace, int64_t workspace_bytes, double* out,
+                    void* stream);
+int64_t gcb_sum_squares_workspace_bytes(void);
+
+/* One fused pass of optax's clip_by_global_norm(max_norm) -> adamw over flat fp32 buffers p, g, m, v
+ * of n elements (p, m, v updated in place, g read only), in fp64 arithmetic from the fp32 state:
+ *   c = 1 if |g| < max_norm else max_norm / |g|,  |g| = sqrt(*sumsq)  (max_norm <= 0: c = 1)
+ *   m = b1 m + (1 - b1) c g;   v = b2 v + (1 - b2) (c g)^2
+ *   u = (m / (1 - b1^t)) / (sqrt(v / (1 - b2^t) + eps_root) + eps) + [i < n_decay] weight_decay p
+ *   p = p - learning_rate u
+ * t >= 1 is the step count after this update (optax's incremented count).  Elements [0, n_decay)
+ * are weight-decayed (the optimiser orders its flat buffer so that the mask is one split index).
+ * sumsq: device fp64 (gcb_sum_squares of g), read on the device -- no host synchronisation.
+ * Elementwise and deterministic.  One launch on `stream`. */
+int gcb_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, int64_t n_decay, int64_t t,
+                   double learning_rate, double b1, double b2, double eps, double eps_root,
+                   double weight_decay, const double* sumsq, double max_norm, void* stream);
+
 /* CTAs per thread-block cluster of the tensor-core layer kernel (1, 2 or 4; default
  * 2).  The CTAs of a cluster process consecutive row tiles in lockstep and receive
  * each weight tile once from L2 through TMA multicast.  Process-wide tuning knob. */
