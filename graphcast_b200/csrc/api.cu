@@ -107,6 +107,22 @@ struct ProfScope {
   }
 };
 
+// An external A segment: an operand image, or an fp32 table (gathered, fan-in summed).
+int validate_segment(const gcb_segment& g) {
+  GCB_CHECK_ARG(g.k > 0 && g.k % 16 == 0, "segment k must be a positive multiple of 16");
+  GCB_CHECK_ARG(g.k / 16 <= INT16_MAX, "segment k too large");   // SegInfo::ksteps
+  if (g.img != nullptr) {
+    GCB_CHECK_ARG(aligned16(g.img), "segment image unaligned");
+    return GCB_OK;
+  }
+  GCB_CHECK_ARG(g.table != nullptr && aligned16(g.table), "segment table null/unaligned");
+  GCB_CHECK_ARG(g.k_valid > 0 && g.k_valid <= g.k && g.k_valid % 4 == 0,
+                "segment k_valid must be a multiple of 4 and <= k");
+  GCB_CHECK_ARG(g.ld % 4 == 0 && g.ld >= g.k_valid, "segment ld must be a multiple of 4 and >= k_valid");
+  GCB_CHECK_ARG(g.fan >= 1, "segment fan must be >= 1");
+  return GCB_OK;
+}
+
 int validate_layer(const gcb_layer_desc* d) {
   GCB_CHECK_ARG(d != nullptr, "null descriptor");
   GCB_CHECK_ARG(d->rows >= 0, "rows < 0");
@@ -118,18 +134,8 @@ int validate_layer(const gcb_layer_desc* d) {
                   "out_img requires n = n_valid = 512");
   int ksteps = 0;
   for (int s = 0; s < d->nseg; ++s) {
-    const gcb_segment& g = d->seg[s];
-    GCB_CHECK_ARG(g.k > 0 && g.k % 16 == 0, "segment k must be a positive multiple of 16");
-    ksteps += g.k / 16;
-    if (g.img != nullptr) {
-      GCB_CHECK_ARG(aligned16(g.img), "segment image unaligned");
-      continue;
-    }
-    GCB_CHECK_ARG(g.table != nullptr && aligned16(g.table), "segment table null/unaligned");
-    GCB_CHECK_ARG(g.k_valid > 0 && g.k_valid <= g.k && g.k_valid % 4 == 0,
-                  "segment k_valid must be a multiple of 4 and <= k");
-    GCB_CHECK_ARG(g.ld % 4 == 0 && g.ld >= g.k_valid, "segment ld must be a multiple of 4 and >= k_valid");
-    GCB_CHECK_ARG(g.fan >= 1, "segment fan must be >= 1");
+    if (int rc = validate_segment(d->seg[s])) return rc;
+    ksteps += d->seg[s].k / 16;
   }
   GCB_CHECK_ARG(ksteps <= gcb::kMaxKSteps, "K too large");
   GCB_CHECK_ARG(d->bias != nullptr, "bias is null");
@@ -159,29 +165,25 @@ int validate_layer(const gcb_layer_desc* d) {
 
 int g_cluster_size = 2;   // CTAs per cluster sharing the weight stream (1, 2 or 4)
 
-template <bool kSplit, bool kSwish, bool kLN>
-int launch_tc_variant(const gcb_layer_desc& d, cudaStream_t stream) {
-  using Cfg = gcb::TcConfig<kSplit, kLN>;
-  auto kernel = gcb::mlp_layer_tc_kernel<kSplit, kSwish, kLN>;
+// Launches the persistent kernel kKernel (kThreads threads per CTA, clusters of csize CTAs)
+// on `clusters` clusters, or as many as are resident at once if that is fewer, with `smem`
+// bytes of dynamic shared memory.  smem_max (>= smem) is the kernel's opt-in size, set once
+// per device; residency is queried at that size once per device and cluster size.
+template <auto kKernel, typename... Args>
+int launch_persistent(int smem_max, int smem, int csize, int clusters, cudaStream_t stream, const Args&... args) {
   static bool attr_set[64] = {false};
   static int max_clusters[64][5] = {{0}};
   int dev = 0;
   GCB_CUDA(cudaGetDevice(&dev));
   GCB_CHECK_ARG(dev >= 0 && dev < 64, "device index out of range");
   if (!attr_set[dev]) {
-    GCB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  Cfg::kSmemBytes));
+    GCB_CUDA(cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
     attr_set[dev] = true;
   }
-  const int csize = g_cluster_size;
-  // A consumer warpgroup holds the accumulator of one 256-column unit only: LayerNorm over a
-  // 512-wide row needs the N-split schedule, where each CTA of the pair owns one half.
-  if (kLN && d.n == 512 && csize != 2)
-    return fail(GCB_ERR_INVALID, "LayerNorm with n = 512 needs the cluster size 2 (N-split) schedule");
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.blockDim = dim3(gcb::kThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+  cfg.dynamicSmemBytes = smem_max;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -190,22 +192,34 @@ int launch_tc_variant(const gcb_layer_desc& d, cudaStream_t stream) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  if (max_clusters[dev][csize] == 0) {
+  int& resident = max_clusters[dev][csize];
+  if (resident == 0) {
     cfg.gridDim = dim3(sm_count_cached() / csize * csize);
     int nc = 0;
-    GCB_CUDA(cudaOccupancyMaxActiveClusters(&nc, kernel, &cfg));
+    GCB_CUDA(cudaOccupancyMaxActiveClusters(&nc, kKernel, &cfg));
     if (nc <= 0) return fail(GCB_ERR_CUDA, "no resident cluster fits on this device");
-    max_clusters[dev][csize] = nc;
+    resident = nc;
   }
+  cfg.dynamicSmemBytes = smem;
+  cfg.gridDim = dim3(std::min(clusters, resident) * csize);
+  GCB_CUDA(cudaLaunchKernelEx(&cfg, kKernel, args...));
+  return GCB_OK;
+}
+
+template <bool kSplit, bool kSwish, bool kLN>
+int launch_tc_variant(const gcb_layer_desc& d, cudaStream_t stream) {
+  constexpr int smem = gcb::TcConfig<kSplit, kLN>::kSmemBytes;
+  const int csize = g_cluster_size;
+  // A consumer warpgroup holds the accumulator of one 256-column unit only: LayerNorm over a
+  // 512-wide row needs the N-split schedule, where each CTA of the pair owns one half.
+  if (kLN && d.n == 512 && csize != 2)
+    return fail(GCB_ERR_INVALID, "LayerNorm with n = 512 needs the cluster size 2 (N-split) schedule");
   const int tiles = (d.rows + gcb::kTileM - 1) / gcb::kTileM;
   // N-split schedule (n = 512, cluster of 2): one tile per cluster at a time; otherwise
   // every CTA of the cluster has its own tile.
   const bool nsplit = (csize == 2 && d.n == 512);
-  int clusters = nsplit ? tiles : (tiles + csize - 1) / csize;
-  if (clusters > max_clusters[dev][csize]) clusters = max_clusters[dev][csize];
-  cfg.gridDim = dim3(clusters * csize);
-  GCB_CUDA(cudaLaunchKernelEx(&cfg, kernel, d));
-  return GCB_OK;
+  const int clusters = nsplit ? tiles : (tiles + csize - 1) / csize;
+  return launch_persistent<gcb::mlp_layer_tc_kernel<kSplit, kSwish, kLN>>(smem, smem, csize, clusters, stream, d);
 }
 
 template <bool kSplit>
@@ -240,7 +254,7 @@ struct ChainShape {
   int maxdist = 1;     // largest (consumer layer - producer layer)
   int nslots = 2;
   bool pre = false;
-  bool big = false;    // more than 4 parameter vectors
+  int vecs = 0;        // bias / LayerNorm parameter vectors
 };
 
 int validate_chain(const gcb_chain_desc* d, ChainShape* shape) {
@@ -251,7 +265,6 @@ int validate_chain(const gcb_chain_desc* d, ChainShape* shape) {
                 "chains run on the tensor-core path only (BF16X3 / BF16)");
   GCB_CHECK_ARG(d->lag >= 0 && d->lag <= 2, "lag must be 0 (default), 1 or 2");
   ChainShape sh;
-  int vecs = 0;
   for (int l = 0; l < d->nlayers; ++l) {
     const gcb_chain_layer& g = d->layer[l];
     GCB_CHECK_ARG(g.nseg >= 1 && g.nseg <= 3, "nseg must be 1..3");
@@ -262,17 +275,7 @@ int validate_chain(const gcb_chain_desc* d, ChainShape* shape) {
         if (l - from > sh.maxdist) sh.maxdist = l - from;
         continue;
       }
-      const gcb_segment& sg = g.seg[s];
-      GCB_CHECK_ARG(sg.k > 0 && sg.k % 16 == 0, "segment k must be a positive multiple of 16");
-      if (sg.img != nullptr) {
-        GCB_CHECK_ARG(aligned16(sg.img), "segment image unaligned");
-        continue;
-      }
-      GCB_CHECK_ARG(sg.table != nullptr && aligned16(sg.table), "segment table null/unaligned");
-      GCB_CHECK_ARG(sg.k_valid > 0 && sg.k_valid <= sg.k && sg.k_valid % 4 == 0,
-                    "segment k_valid must be a multiple of 4 and <= k");
-      GCB_CHECK_ARG(sg.ld % 4 == 0 && sg.ld >= sg.k_valid, "segment ld must be a multiple of 4 and >= k_valid");
-      GCB_CHECK_ARG(sg.fan >= 1, "segment fan must be >= 1");
+      if (int rc = validate_segment(g.seg[s])) return rc;
     }
     GCB_CHECK_ARG(g.w_packed != nullptr && aligned16(g.w_packed), "w_packed null/unaligned");
     GCB_CHECK_ARG((g.ln_scale == nullptr) == (g.ln_offset == nullptr), "ln_scale/ln_offset mismatch");
@@ -308,11 +311,10 @@ int validate_chain(const gcb_chain_desc* d, ChainShape* shape) {
                       "pre_add table null/unaligned");
       sh.pre = true;
     }
-    vecs += (g.bias ? 1 : 0) + (g.ln_scale ? 2 : 0);
+    sh.vecs += (g.bias ? 1 : 0) + (g.ln_scale ? 2 : 0);
     if (g.keep) ++sh.nq;
   }
-  GCB_CHECK_ARG(vecs <= 8, "too many bias / LayerNorm vectors for one chain (at most 8)");
-  sh.big = vecs > 4;
+  GCB_CHECK_ARG(sh.vecs <= gcb::kChainParamVecs, "too many bias / LayerNorm vectors for one chain (at most 8)");
   const int lag = d->lag > 0 ? d->lag : 1;
   GCB_CHECK_ARG(d->order == 0 || (d->order == 1 && d->nlayers >= 3),
                 "order must be 0, or 1 for chains of at least 3 layers");
@@ -328,58 +330,15 @@ int validate_chain(const gcb_chain_desc* d, ChainShape* shape) {
   return GCB_OK;
 }
 
-template <bool kSplit, bool kPre, bool kBig>
+template <bool kSplit, bool kPre>
 int launch_chain_variant(const gcb_chain_desc& d, const ChainShape& sh, cudaStream_t stream) {
-  using Cfg = gcb::ChainConfig<kSplit, kPre, kBig>;
-  auto kernel = gcb::mlp_chain_tc_kernel<kSplit, kPre, kBig>;
-  static bool attr_set[64] = {false};
-  static int max_clusters[64] = {0};
-  int dev = 0;
-  GCB_CUDA(cudaGetDevice(&dev));
-  GCB_CHECK_ARG(dev >= 0 && dev < 64, "device index out of range");
-  if (!attr_set[dev]) {
-    GCB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set[dev] = true;
-    // The scratch ring is accessed with the L2 evict_last policy.  Experiment switch: with
-    // GCB_L2_PERSIST_MB > 0 those lines also get a persisting set-aside of that size (capped at the
-    // device's cudaDevAttrMaxPersistingL2CacheSize); the default is no set-aside.
-    static bool l2_set[64] = {false};
-    if (!l2_set[dev]) {
-      l2_set[dev] = true;
-      int max_persist = 0;
-      cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, dev);
-      long long want = 0;
-      if (const char* e = getenv("GCB_L2_PERSIST_MB")) want = atoll(e) * (1ll << 20);
-      if (want > max_persist) want = max_persist;
-      if (want > 0 && cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, static_cast<size_t>(want)) != cudaSuccess)
-        cudaGetLastError();
-    }
-  }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.blockDim = dim3(gcb::kThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (max_clusters[dev] == 0) {
-    cfg.gridDim = dim3(sm_count_cached() / 2 * 2);
-    int nc = 0;
-    GCB_CUDA(cudaOccupancyMaxActiveClusters(&nc, kernel, &cfg));
-    if (nc <= 0) return fail(GCB_ERR_CUDA, "no resident cluster fits on this device");
-    if (nc > sm_count_cached() / 2) nc = sm_count_cached() / 2;   // the scratch is sized for SMs / 2
-    max_clusters[dev] = nc;
-  }
+  using Cfg = gcb::ChainConfig<kSplit>;
+  // The parameter area ends the dynamic shared memory: request only the vectors of this chain.
+  const int smem = Cfg::kSmemBytes - (gcb::kChainParamVecs - sh.vecs) * gcb::kMaxN * 4;
   const int tiles = (d.rows + gcb::kTileM - 1) / gcb::kTileM;
-  int clusters = tiles < max_clusters[dev] ? tiles : max_clusters[dev];
-  cfg.gridDim = dim3(clusters * 2);
-  GCB_CUDA(cudaLaunchKernelEx(&cfg, kernel, d, sh.nq, sh.nslots));
-  return GCB_OK;
+  const int clusters = std::min(tiles, sm_count_cached() / 2);   // the scratch is sized for SMs / 2
+  return launch_persistent<gcb::mlp_chain_tc_kernel<kSplit, kPre>>(Cfg::kSmemBytes, smem, 2, clusters, stream, d,
+                                                                   sh.nq, sh.nslots);
 }
 
 struct StepCtx {
@@ -710,17 +669,9 @@ int gcb_chain_forward(const gcb_chain_desc* d, void* stream) {
     // (a residual_img that is also a segment of the chain is read from HBM once: not counted again)
   }
   ProfScope prof(st, GCB_KIND_CHAIN_TC, flops, bytes);
-  const int variant = (d->precision == GCB_PREC_BF16X3 ? 4 : 0) | (sh.pre ? 2 : 0) | (sh.big ? 1 : 0);
-  switch (variant) {
-    case 7: return launch_chain_variant<true, true, true>(*d, sh, st);
-    case 6: return launch_chain_variant<true, true, false>(*d, sh, st);
-    case 5: return launch_chain_variant<true, false, true>(*d, sh, st);
-    case 4: return launch_chain_variant<true, false, false>(*d, sh, st);
-    case 3: return launch_chain_variant<false, true, true>(*d, sh, st);
-    case 2: return launch_chain_variant<false, true, false>(*d, sh, st);
-    case 1: return launch_chain_variant<false, false, true>(*d, sh, st);
-    default: return launch_chain_variant<false, false, false>(*d, sh, st);
-  }
+  if (d->precision == GCB_PREC_BF16X3)
+    return sh.pre ? launch_chain_variant<true, true>(*d, sh, st) : launch_chain_variant<true, false>(*d, sh, st);
+  return sh.pre ? launch_chain_variant<false, true>(*d, sh, st) : launch_chain_variant<false, false>(*d, sh, st);
 }
 
 int gcb_segment_sum(const float* msg, int32_t ld_msg, const int32_t* row_ptr, int32_t num_nodes,
@@ -1695,7 +1646,7 @@ int gcb_debug_trace(long long* device_buffer) {
 }
 
 int gcb_debug_flags(int flags) {
-  GCB_CUDA(cudaMemcpyToSymbol(gcb::g_dbg_flags, &flags, sizeof(flags)));
+  GCB_CHECK_ARG(flags == 0, "this build has no experiment switches");
   return GCB_OK;
 }
 

@@ -42,35 +42,13 @@ namespace gcb {
 constexpr int kChainSlotsMax = 5;
 constexpr int kScratchTileBytes = (kMaxN / kKStep) * GCB_A_IMAGE_BLOCK;   // 32 x 8448 = 270336
 constexpr int kChainTailBytes = 3072;
+constexpr int kChainParamVecs = 8;          // [512]-float parameter vectors (biases, LayerNorm scale / offset)
 
-// kBig: room for 8 instead of 4 [512]-float parameter vectors (biases, LayerNorm scale / offset):
-// chains of two MLPs; costs 8 KB of shared memory (one operand stage in some variants).
-template <bool kSplit, bool kPre, bool kBig>
-struct ChainConfig {
-  static constexpr int kParamVecs = kBig ? 8 : 4;
-  static constexpr int kAStageBytes = kSplit ? 2 * kAPartBytes : kAPartBytes;
-  static constexpr int kBStageBytes = kSplit ? 2 * kBPartBytes : kBPartBytes;
-  static constexpr int kStageBytes = kAStageBytes + kBStageBytes;
-  static constexpr int kParamBytes = kParamVecs * kMaxN * 4;
-  static constexpr int kFixedBytes = kParamBytes + kLnxBytes + kChainTailBytes;
-  static constexpr int kFit = (kSmemLimit - kFixedBytes) / kStageBytes;
-#ifdef GCB_FORCE_STAGES          // experiment: sensitivity of a launch to the ring depth
-  static constexpr int kStages = GCB_FORCE_STAGES < kFit ? GCB_FORCE_STAGES : kFit;
-#else
-  static constexpr int kStages = kFit < 12 ? kFit : 12;
-#endif
-  static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
-  static_assert(kStages >= 4, "operand ring too shallow");
-};
-
-struct ChainSeg {
-  const float* table;
-  const int32_t* idx;
-  const uint8_t* img;
-  int ld, k_valid, fan, ksteps;
-  int src_q;          // >= 0: scratch ring q (result of an earlier layer); else external
-  int pad_;
-};
+// stages | LayerNorm exchange | tail | parameters.  The ring is sized for kChainParamVecs
+// parameter vectors, and a launch requests only the vectors its chain uses, which the
+// parameter area at the end lets it leave out.
+template <bool kSplit>
+using ChainConfig = StageRing<kSplit, kLnxBytes + kChainTailBytes + kChainParamVecs * kMaxN * 4>;
 
 // kKindLN*: LayerNorm without residual / with an fp32 residual / with an operand-image residual
 enum { kKindPlain = 0, kKindSwish = 1, kKindLN = 2, kKindLNRes = 3, kKindLNImg = 4 };
@@ -253,25 +231,25 @@ __device__ __forceinline__ void chain_epilogue(float (&acc)[128], uint2 (&buf)[1
   }
 }
 
-template <bool kSplit, bool kPre, bool kBig>
+template <bool kSplit, bool kPre>
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, const int nslots) {
-  using Cfg = ChainConfig<kSplit, kPre, kBig>;
+  using Cfg = ChainConfig<kSplit>;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* stage_base = smem;
-  float* s_param = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes);
-  float2* s_lnx = reinterpret_cast<float2*>(s_param + Cfg::kParamBytes / 4);   // [2][128]
+  float2* s_lnx = reinterpret_cast<float2*>(smem + Cfg::kStages * Cfg::kStageBytes);   // [2][128]
   uint8_t* tail = reinterpret_cast<uint8_t*>(s_lnx) + kLnxBytes;
+  float* s_param = reinterpret_cast<float*>(tail + kChainTailBytes);   // the chain's vectors only
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);          // [12]
   uint64_t* empty_bar = full_bar + 12;                             // [12]
   uint64_t* lnx_bar = empty_bar + 12;                              // [2 warpgroups][2]
   uint64_t* h_full_bar = lnx_bar + 4;                              // [GCB_MAX_CHAIN][kChainSlotsMax]
   uint64_t* h_free_bar = h_full_bar + GCB_MAX_CHAIN * kChainSlotsMax;
   ChainLayer* s_layer = reinterpret_cast<ChainLayer*>(h_free_bar + GCB_MAX_CHAIN * kChainSlotsMax);  // [4]
-  ChainSeg* s_seg = reinterpret_cast<ChainSeg*>(s_layer + GCB_MAX_CHAIN);            // [4][3]
+  SegInfo* s_seg = reinterpret_cast<SegInfo*>(s_layer + GCB_MAX_CHAIN);              // [4][3]
   PreAddInfo* s_pre = reinterpret_cast<PreAddInfo*>(s_seg + GCB_MAX_CHAIN * 3);      // [4][2]
   static_assert((2 * 12 + 4 + 2 * GCB_MAX_CHAIN * kChainSlotsMax) * 8 +
-                    GCB_MAX_CHAIN * (sizeof(ChainLayer) + 3 * sizeof(ChainSeg) + 2 * sizeof(PreAddInfo))
+                    GCB_MAX_CHAIN * (sizeof(ChainLayer) + 3 * sizeof(SegInfo) + 2 * sizeof(PreAddInfo))
                     <= kChainTailBytes, "tail region too small");
 
   const int warp = threadIdx.x >> 5;
@@ -353,13 +331,13 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
       if (gl.keep) { cl.keep_q = q; q_of_layer[l] = q; ++q; }
       int ks = 0, has_table = 0;
       for (int s = 0; s < gl.nseg; ++s) {
-        ChainSeg& cs = s_seg[l * 3 + s];
+        SegInfo& cs = s_seg[l * 3 + s];
         const int from = gl.seg_from[s];
         cs.table = gl.seg[s].table; cs.idx = gl.seg[s].idx;
         cs.img = static_cast<const uint8_t*>(gl.seg[s].img);
         cs.ld = gl.seg[s].ld; cs.k_valid = gl.seg[s].k_valid; cs.fan = gl.seg[s].fan;
-        cs.ksteps = (from >= 0 ? kMaxN : gl.seg[s].k) / kKStep;
-        cs.src_q = from >= 0 ? q_of_layer[from] : -1;
+        cs.ksteps = static_cast<int16_t>((from >= 0 ? kMaxN : gl.seg[s].k) / kKStep);
+        cs.src_q = static_cast<int16_t>(from >= 0 ? q_of_layer[from] : -1);
         if (from >= 0) { cs.img = nullptr; ++consumers[from]; }
         else if (cs.img == nullptr) has_table = 1;
         ks += cs.ksteps;
@@ -415,7 +393,7 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
           const bool tr = tracing(tu);
           long long blocked = 0, hwait = 0;
           for (int s = 0; s < nseg; ++s) {
-            const ChainSeg sg = s_seg[l * 3 + s];
+            const SegInfo sg = s_seg[l * 3 + s];
             const uint8_t* a_ptr = nullptr;
             bool a_copy = false;
             const bool a_scratch = sg.src_q >= 0;
@@ -477,49 +455,18 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
           const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
           const int nseg = s_layer[l].nseg;
           for (int s = 0; any_table && s < nseg; ++s) {
-            const ChainSeg sg = s_seg[l * 3 + s];
+            const SegInfo sg = s_seg[l * 3 + s];
             const bool is_tab = sg.src_q < 0 && sg.img == nullptr;
             int src[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              src[i] = -1;
-              if (is_tab) {
-                const long long grow = static_cast<long long>(tile) * kTileM + rg + 16 * i;
-                if (grow < rows_total) src[i] = sg.idx ? __ldg(sg.idx + grow) : static_cast<int>(grow);
-              }
-            }
+            table_rows(src, is_tab, sg, tile, rg, rows_total);
             for (int k = 0; k < sg.ksteps; ++k) {
               float4 cur[8];
               if (is_tab) {
-                const int koff = k * kKStep + sub * 4;
-                const bool kvalid = koff < sg.k_valid;
 #pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-                  if (kvalid && src[i] >= 0) {
-                    const float* p = sg.table + static_cast<long long>(src[i]) * sg.fan * sg.ld + koff;
-                    a = __ldg(reinterpret_cast<const float4*>(p));
-                    for (int j = 1; j < sg.fan; ++j) {
-                      const float4 t = __ldg(reinterpret_cast<const float4*>(p + static_cast<long long>(j) * sg.ld));
-                      a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
-                    }
-                  }
-                  cur[i] = a;
-                }
+                for (int i = 0; i < 8; ++i) cur[i] = load_table_row(sg, src[i], k * kKStep + sub * 4);
               }
               ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-              if (is_tab) {
-                uint8_t* a_hi = stage_base + stage * Cfg::kStageBytes;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  uint2 hi, lo;
-                  ptx::split_bf16x4(cur[i], hi, lo);
-                  const uint32_t off = sts_off + (rg + 16 * i) * 16;
-                  *reinterpret_cast<uint2*>(a_hi + off) = hi;
-                  if (kSplit) *reinterpret_cast<uint2*>(a_hi + kAPartBytes + off) = lo;
-                }
-                ptx::fence_proxy_async_smem();
-              }
+              if (is_tab) store_table_kstep<kSplit>(stage_base + stage * Cfg::kStageBytes, cur, sts_off, rg);
               __syncwarp();
               if (lane == 0) ptx::mbar_arrive(&full_bar[stage]);
               if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
@@ -649,32 +596,9 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         e.mean[0] = e.mean[1] = 0.f;
         e.rstd[0] = e.rstd[1] = 1.f;
         if (is_ln) {
-          // Each CTA computes (mean, M2) of its 256 columns of a row, hands them to the partner
-          // through distributed shared memory, and both combine them (Chan's parallel update).
           float shift[2], s1[2], s2[2];
           row_shifted_sums(acc, s_bias != nullptr ? s_bias + col_base : nullptr, kUnitN, shift, s1, s2);
-          const uint32_t lb = ln_count & 1, par = (ln_count >> 1) & 1;
-          uint64_t* bar = &lnx_bar[eg * 2 + lb];
-          float mh[2], m2h[2];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            mh[h] = shift[h] + s1[h] * (1.0f / kUnitN);
-            m2h[h] = fmaxf(s2[h] - s1[h] * s1[h] * (1.0f / kUnitN), 0.f);
-            if (q == 0)
-              ptx::st_async_f32x2(ptx::mapa(ptx::smem_addr(&s_lnx[lb * kTileM + lr0 + 8 * h]), peer),
-                                  mh[h], m2h[h], ptx::mapa(ptx::smem_addr(bar), peer));
-          }
-          if (lead) ptx::mbar_arrive_expect_tx(bar, 64 * 8);
-          ptx::mbar_wait(bar, par);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const float2 other = s_lnx[lb * kTileM + lr0 + 8 * h];
-            const float delta = other.x - mh[h];
-            e.mean[h] = 0.5f * (mh[h] + other.x);
-            const float var = (m2h[h] + other.y + delta * delta * (0.5f * kUnitN)) * (1.0f / (2 * kUnitN));
-            e.rstd[h] = rsqrtf(var + 1e-5f);
-          }
-          ++ln_count;
+          ln_pair_stats(shift, s1, s2, s_lnx, &lnx_bar[eg * 2], ln_count, lr0, peer, lead, e.mean, e.rstd);
           if (lead && eg == 0) trace(u, 4);
         }
         // One column loop per layer kind, chosen once per unit.

@@ -60,25 +60,34 @@ constexpr int kConsumerWarps = 8;                 // warps 4-11: two warpgroups 
 constexpr int kProducerWarps = 2;                 // warps 2-3
 static_assert(2 * kAPartBytes == GCB_A_IMAGE_BLOCK, "A image block must match the stage layout");
 
-// Shared-memory budget: everything the variant does not need goes to pipeline stages.
-// LayerNorm variants never stage gathered addends (only the 2 KB statistics exchange
-// aliases that region); the others carry no LayerNorm scale / offset.
+// Shared-memory budget: everything a kernel variant does not need for its fixed regions goes
+// to the operand ring (StageRing).
 constexpr int kSmemLimit = 227 * 1024;            // opt-in dynamic shared memory per CTA
 constexpr int kTailBytes = 1024;                  // barriers, segment tables
 constexpr int kLnxBytes = 2 * kTileM * 8;         // [2][128] (mean, M2) pairs
 
-template <bool kSplit, bool kLN>
-struct TcConfig {
+// The operand ring of a kernel variant whose other shared-memory regions take kFixed bytes:
+// as many stages as the rest of kSmemLimit holds, at most 12 (the tails hold 2 x 12 stage
+// barriers), at least 4.
+template <bool kSplit, int kFixed>
+struct StageRing {
   static constexpr int kAStageBytes = kSplit ? 2 * kAPartBytes : kAPartBytes;
   static constexpr int kBStageBytes = kSplit ? 2 * kBPartBytes : kBPartBytes;
   static constexpr int kStageBytes = kAStageBytes + kBStageBytes;
-  static constexpr int kParamBytes = (kLN ? 3 : 1) * kMaxN * 4;   // bias (, ln scale, ln offset)
-  static constexpr int kGRegionBytes = kLN ? kLnxBytes : kGBytes;
-  static constexpr int kFixedBytes = kParamBytes + kGRegionBytes + kTailBytes;
+  static constexpr int kFixedBytes = kFixed;
   static constexpr int kFit = (kSmemLimit - kFixedBytes) / kStageBytes;
-  static constexpr int kStages = kFit < 12 ? kFit : 12;           // tail holds 2*12+8 barriers
+  static constexpr int kStages = kFit < 12 ? kFit : 12;
   static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
   static_assert(kStages >= 4, "operand ring too shallow");
+};
+
+// Layer kernel: stages | bias (, LayerNorm scale, offset) | addend buffers | tail.  LayerNorm
+// variants never stage gathered addends (only the 2 KB statistics exchange takes that region);
+// the others carry no LayerNorm scale / offset.
+template <bool kSplit, bool kLN, int kParam = (kLN ? 3 : 1) * kMaxN * 4, int kGRegion = kLN ? kLnxBytes : kGBytes>
+struct TcConfig : StageRing<kSplit, kParam + kGRegion + kTailBytes> {
+  static constexpr int kParamBytes = kParam;
+  static constexpr int kGRegionBytes = kGRegion;
 };
 
 // Register split between warpgroup 0 (TMA, idle and producer warps) and the two consumer
@@ -113,8 +122,6 @@ __device__ __forceinline__ float swish_f(float x) {
 constexpr int kTraceTiles = 64;
 constexpr int kTraceEvents = 16;
 __device__ long long* g_trace = nullptr;
-// Debug-only experiment switches (gcb_debug_flags); 0 in production.
-__device__ int g_dbg_flags = 0;
 
 __device__ __forceinline__ void trace(uint32_t unit, int ev) {
   if (g_trace != nullptr && blockIdx.x == 0 && unit < kTraceTiles)
@@ -139,7 +146,10 @@ struct SegInfo {
   const float* table;
   const int32_t* idx;
   const uint8_t* img;
-  int ld, k_valid, fan, ksteps;
+  int ld, k_valid, fan;
+  // 16 bits keep the struct at 40 bytes; at 48 the layer kernel spills more.
+  int16_t ksteps;
+  int16_t src_q;      // chain kernel: >= 0 = scratch ring q (result of an earlier layer); else -1
 };
 struct PreAddInfo {
   const float* table;
@@ -244,6 +254,88 @@ __device__ __forceinline__ void row_shifted_sums(const float (&acc)[128], const 
   }
 }
 
+// LayerNorm statistics of this thread's two rows when the row's 512 columns are split over the
+// two CTAs of a cluster (N-split): each CTA computes (mean, M2) of its 256 columns from the
+// shifted sums, hands them to the partner through distributed shared memory (s_lnx and
+// wg_bar = this warpgroup's two lnx_bar, alternating with ln_count), and both combine them
+// (Chan's parallel update).
+__device__ __forceinline__ void ln_pair_stats(const float (&shift)[2], const float (&s1)[2], const float (&s2)[2],
+                                              float2* s_lnx, uint64_t* wg_bar, uint32_t& ln_count, int lr0,
+                                              uint32_t peer, bool lead, float (&mean)[2], float (&rstd)[2]) {
+  const uint32_t lb = ln_count & 1, par = (ln_count >> 1) & 1;
+  uint64_t* bar = &wg_bar[lb];
+  float mh[2], m2h[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    mh[h] = shift[h] + s1[h] * (1.0f / kUnitN);
+    m2h[h] = fmaxf(s2[h] - s1[h] * s1[h] * (1.0f / kUnitN), 0.f);
+    if ((threadIdx.x & 3) == 0)
+      ptx::st_async_f32x2(ptx::mapa(ptx::smem_addr(&s_lnx[lb * kTileM + lr0 + 8 * h]), peer),
+                          mh[h], m2h[h], ptx::mapa(ptx::smem_addr(bar), peer));
+  }
+  if (lead) ptx::mbar_arrive_expect_tx(bar, 64 * 8);
+  ptx::mbar_wait(bar, par);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float2 other = s_lnx[lb * kTileM + lr0 + 8 * h];
+    const float delta = other.x - mh[h];
+    mean[h] = 0.5f * (mh[h] + other.x);
+    const float var = (m2h[h] + other.y + delta * delta * (0.5f * kUnitN)) * (1.0f / (2 * kUnitN));
+    rstd[h] = rsqrtf(var + 1e-5f);
+  }
+  ++ln_count;
+}
+
+// ---- producer helpers (fp32-table A segments, shared with mlp_chain.cuh) -----------
+// Producer thread t64 (of 64) converts the float4 sub = t64 % 4 of the 16-wide K-step for the
+// 8 tile rows rg + 16i (rg = t64 / 4).
+
+// Source rows of the thread's 8 tile rows of `tile`: through sg.idx if given, -1 past the end
+// (and everywhere unless `active`; sg is not read then).
+__device__ __forceinline__ void table_rows(int (&src)[8], bool active, const SegInfo& sg, uint32_t tile,
+                                           int rg, long long rows_total) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    src[i] = -1;
+    if (active) {
+      const long long grow = static_cast<long long>(tile) * kTileM + rg + 16 * i;
+      const int32_t* ip = sg.idx;
+      if (grow < rows_total) src[i] = ip ? __ldg(ip + grow) : static_cast<int>(grow);
+    }
+  }
+}
+
+// One row's float4 at element koff of a K-step: the sum over the sg.fan consecutive table rows
+// from source row sr; zero for sr < 0 and past k_valid.
+__device__ __forceinline__ float4 load_table_row(const SegInfo& sg, int sr, int koff) {
+  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (koff < sg.k_valid && sr >= 0) {
+    const float* p = sg.table + static_cast<long long>(sr) * sg.fan * sg.ld + koff;
+    a = __ldg(reinterpret_cast<const float4*>(p));
+    for (int j = 1; j < sg.fan; ++j) {
+      const float4 t = __ldg(reinterpret_cast<const float4*>(p + static_cast<long long>(j) * sg.ld));
+      a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
+    }
+  }
+  return a;
+}
+
+// Splits the 8 rows to bf16 hi (| lo) and stores them into the A operand of a stage (K-major
+// core-matrix layout; sts_off = the thread's K-chunk / 8-byte offset), then makes the stores
+// visible to the wgmma operand fetches (async proxy).
+template <bool kSplit>
+__device__ __forceinline__ void store_table_kstep(uint8_t* a_hi, const float4 (&v)[8], uint32_t sts_off, int rg) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    uint2 hi, lo;
+    ptx::split_bf16x4(v[i], hi, lo);
+    const uint32_t off = sts_off + (rg + 16 * i) * 16;
+    *reinterpret_cast<uint2*>(a_hi + off) = hi;
+    if (kSplit) *reinterpret_cast<uint2*>(a_hi + kAPartBytes + off) = lo;
+  }
+  ptx::fence_proxy_async_smem();
+}
+
 // Adds the staged pre-activation addends of one 32-column chunk (rows of this thread).
 __device__ __forceinline__ void add_staged_chunk(float (&acc)[128], int j0, const float* gbuf, int lr0) {
   const int q = threadIdx.x & 3;
@@ -333,6 +425,8 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
   SegInfo* s_seg = reinterpret_cast<SegInfo*>(lnx_bar + 4);               // [3]
   PreAddInfo* s_pre = reinterpret_cast<PreAddInfo*>(s_seg + 3);           // [2]
   KStepInfo* ks_info = reinterpret_cast<KStepInfo*>(s_pre + 2);           // [kMaxKSteps]
+  static_assert((2 * 12 + 8) * 8 + 3 * sizeof(SegInfo) + 2 * sizeof(PreAddInfo) + kMaxKSteps * sizeof(KStepInfo)
+                    <= kTailBytes, "tail region too small");
   // [2][128] LayerNorm statistics received from the partner CTA (N-split).  Aliases the
   // addend buffers, which LayerNorm layers never use (pre_add excludes LayerNorm).
   float2* s_lnx = reinterpret_cast<float2*>(s_g);
@@ -350,14 +444,13 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
     ksteps += d.seg[s].k / kKStep;
     a_is_img = a_is_img && (d.seg[s].img != nullptr);
   }
-  const int dbg = g_dbg_flags;
-  uint8_t* const out_img = (dbg & 2) ? nullptr : static_cast<uint8_t*>(d.out_img);
+  uint8_t* const out_img = static_cast<uint8_t*>(d.out_img);
   // Descriptor fields used inside hot loops, hoisted into registers once.
   const long long rows_total = d.rows;
   const int nseg = d.nseg;
   const int n_pre = d.n_pre_add;               // gathered pre-activation addends (0..2)
-  float* const out_ptr = (dbg & 2) ? nullptr : d.out;
-  float* const outy_ptr = (dbg & 2) ? nullptr : d.out_y;
+  float* const out_ptr = d.out;
+  float* const outy_ptr = d.out_y;
   const float* const res_ptr = d.residual;
   const long long ld_out = d.ld_out, ld_outy = d.ld_out_y, ld_res = d.ld_res;
   // Cluster schedule: the CTAs of a cluster walk the K-steps of `csize` consecutive
@@ -371,9 +464,6 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
   const uint32_t tile_off = nsplit ? 0u : crank;             // my tile = base + tile_off
   const int units_per_tile = nsplit ? 1 : n_halves;          // units this CTA runs per tile
   const uint16_t cmask = static_cast<uint16_t>((1u << csize) - 1u);
-  // (experiment, debug flag 4) N-split pair without A multicast: each CTA streams the whole
-  // block itself and recycles its stages on its own MMAs only.
-  const bool decouple = nsplit && (dbg & 4);
   const bool gather_mode = !kLN && n_pre > 0;
 
   // ---- one-time setup ---------------------------------------------------------
@@ -393,7 +483,8 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
       s_seg[s].ld = d.seg[s].ld;
       s_seg[s].k_valid = d.seg[s].k_valid;
       s_seg[s].fan = d.seg[s].fan;
-      s_seg[s].ksteps = d.seg[s].k / kKStep;
+      s_seg[s].ksteps = static_cast<int16_t>(d.seg[s].k / kKStep);
+      s_seg[s].src_q = -1;
     }
     for (int s = 0; s < n_pre; ++s) {
       s_pre[s].table = d.pre_add[s].table;
@@ -411,7 +502,7 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
       // 1 TMA lane (+ the producer warps unless A comes from images only)
       ptx::mbar_init(&full_bar[s], a_is_img ? 1 : 1 + kProducerWarps);
       // every consumer warp of every CTA that shares the stage
-      ptx::mbar_init(&empty_bar[s], (decouple ? 1 : csize) * kConsumerWarps);
+      ptx::mbar_init(&empty_bar[s], csize * kConsumerWarps);
     }
     for (int b = 0; b < 2; ++b) {
       ptx::mbar_init(&g_full_bar[b], kProducerWarps);     // every producer warp
@@ -454,12 +545,8 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
             // Same tile in both CTAs of an N-split pair: each fetches half of every block and
             // multicasts it to both.
             const uint8_t* a_ptr = sg.img + static_cast<size_t>(tile) * sg.ksteps * GCB_A_IMAGE_BLOCK +
-                                   (nsplit && !decouple ? crank * a_half : 0u);
+                                   (nsplit ? crank * a_half : 0u);
             const uint32_t tx = b_bytes + (a_copy ? a_bytes : 0u);
-            // (experiment, debug flag 16) L2 prefetch of the same block of my next tile
-            const bool pf_next = (dbg & 16) && uh == units_per_tile - 1 &&
-                                 tile + tile_stride < static_cast<uint32_t>(num_tiles);
-            const size_t pf_off = static_cast<size_t>(tile_stride) * sg.ksteps * GCB_A_IMAGE_BLOCK;
             for (int k = 0; k < sg.ksteps; ++k) {
               const long long w0 = tr ? clock64() : 0;
               ptx::mbar_wait(&empty_bar[stage], phase ^ 1);   // free in every CTA of the cluster
@@ -467,9 +554,8 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
               uint8_t* a_dst = stage_base + stage * Cfg::kStageBytes;
               if (ptx::elect_one()) {
                 ptx::mbar_arrive_expect_tx(&full_bar[stage], tx);
-                if (pf_next && a_copy) ptx::bulk_prefetch_l2(a_ptr + pf_off, nsplit ? a_half : a_bytes);
                 if (a_copy) {
-                  if (nsplit && !decouple) ptx::bulk_g2s_multicast(a_dst + crank * a_half, a_ptr, a_half, &full_bar[stage], cmask);
+                  if (nsplit) ptx::bulk_g2s_multicast(a_dst + crank * a_half, a_ptr, a_half, &full_bar[stage], cmask);
                   else ptx::bulk_g2s(a_dst, a_ptr, a_bytes, &full_bar[stage]);
                 }
                 if (b_own) {
@@ -504,17 +590,7 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
             // Source row of each of my 8 tile rows, per segment (-1 = out of range).
             int src[3][8];
 #pragma unroll
-            for (int s = 0; s < 3; ++s) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                src[s][i] = -1;
-                if (s < nseg) {
-                  const long long grow = static_cast<long long>(tile) * kTileM + rg + 16 * i;
-                  const int32_t* ip = s_seg[s].idx;
-                  if (grow < rows_total) src[s][i] = ip ? __ldg(ip + grow) : static_cast<int>(grow);
-                }
-              }
-            }
+            for (int s = 0; s < 3; ++s) table_rows(src[s], s < nseg, s_seg[s], tile, rg, rows_total);
             float4 cur[8];
             bool have_cur = false, cur_img = false;
             uint32_t cur_it = 0;
@@ -527,40 +603,17 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
               const bool img_step = mine && ks_info[ks].is_img;   // TMA brings the data: arrive only
               if (mine && !img_step) {
                 const int s = ks_info[ks].seg;
-                const int koff = ks_info[ks].koff + sub * 4;
                 const SegInfo sg = s_seg[s];
-                const bool kvalid = koff < sg.k_valid;
+                const int koff = ks_info[ks].koff + sub * 4;
 #pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-                  const int sr = (s == 0) ? src[0][i] : (s == 1 ? src[1][i] : src[2][i]);
-                  if (kvalid && sr >= 0) {
-                    const float* p = sg.table + static_cast<long long>(sr) * sg.fan * sg.ld + koff;
-                    a = __ldg(reinterpret_cast<const float4*>(p));
-                    for (int j = 1; j < sg.fan; ++j) {
-                      const float4 t = __ldg(reinterpret_cast<const float4*>(p + static_cast<long long>(j) * sg.ld));
-                      a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
-                    }
-                  }
-                  nxt[i] = a;
-                }
+                for (int i = 0; i < 8; ++i)
+                  nxt[i] = load_table_row(sg, (s == 0) ? src[0][i] : (s == 1 ? src[1][i] : src[2][i]), koff);
               }
               if (have_cur) {
                 const uint32_t stage = cur_it % Cfg::kStages;
                 const uint32_t phase = (cur_it / Cfg::kStages) & 1;
                 ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t* a_hi = stage_base + stage * Cfg::kStageBytes;
-                if (!cur_img) {
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) {
-                    uint2 hi, lo;
-                    ptx::split_bf16x4(cur[i], hi, lo);
-                    const uint32_t off = sts_off + (rg + 16 * i) * 16;
-                    *reinterpret_cast<uint2*>(a_hi + off) = hi;
-                    if (kSplit) *reinterpret_cast<uint2*>(a_hi + kAPartBytes + off) = lo;
-                  }
-                }
-                ptx::fence_proxy_async_smem();
+                if (!cur_img) store_table_kstep<kSplit>(stage_base + stage * Cfg::kStageBytes, cur, sts_off, rg);
                 __syncwarp();
                 if (lane == 0) ptx::mbar_arrive(&full_bar[stage]);
                 have_cur = false;
@@ -591,7 +644,7 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
     const int lr0 = eg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile rows lr0, lr0 + 8
     const int n_valid = d.n_valid;
     const bool lead = lane == 0 && (warp & 3) == 0;
-    const uint32_t rel_mask = (csize == 1 || decouple) ? 0u : cmask;
+    const uint32_t rel_mask = csize == 1 ? 0u : cmask;
     // The image holds residual + y when an fp32 output is written, y otherwise.
     const bool img_res = res_ptr != nullptr && (out_ptr != nullptr || outy_ptr != nullptr);
     uint32_t stage = 0, phase = 0, g_count = 0, ln_count = 0, u = 0;
@@ -613,32 +666,7 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
           float shift[2], s1[2], s2[2];
           row_shifted_sums(acc, s_bias + col_base, ncols, shift, s1, s2);
           if (nsplit) {
-            // LayerNorm over a row whose two halves live in the two CTAs of the cluster: each
-            // CTA computes (mean, M2) of its 256 columns, hands them to the partner through
-            // distributed shared memory, and both combine them (Chan's parallel update).
-            const uint32_t lb = ln_count & 1, par = (ln_count >> 1) & 1;
-            uint64_t* bar = &lnx_bar[eg * 2 + lb];
-            const uint32_t peer = crank ^ 1u;
-            float mh[2], m2h[2];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              mh[h] = shift[h] + s1[h] * (1.0f / kUnitN);
-              m2h[h] = fmaxf(s2[h] - s1[h] * s1[h] * (1.0f / kUnitN), 0.f);
-              if (q == 0)
-                ptx::st_async_f32x2(ptx::mapa(ptx::smem_addr(&s_lnx[lb * kTileM + lr0 + 8 * h]), peer),
-                                    mh[h], m2h[h], ptx::mapa(ptx::smem_addr(bar), peer));
-            }
-            if (lead) ptx::mbar_arrive_expect_tx(bar, 64 * 8);
-            ptx::mbar_wait(bar, par);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const float2 other = s_lnx[lb * kTileM + lr0 + 8 * h];
-              const float delta = other.x - mh[h];
-              mean[h] = 0.5f * (mh[h] + other.x);
-              const float var = (m2h[h] + other.y + delta * delta * (0.5f * kUnitN)) * (1.0f / (2 * kUnitN));
-              rstd[h] = rsqrtf(var + 1e-5f);
-            }
-            ++ln_count;
+            ln_pair_stats(shift, s1, s2, s_lnx, &lnx_bar[eg * 2], ln_count, lr0, crank ^ 1u, lead, mean, rstd);
           } else {
             const float inv_n = 1.0f / static_cast<float>(ncols);
 #pragma unroll

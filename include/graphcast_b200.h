@@ -596,17 +596,17 @@ int gcb_profile_begin(void);
 int gcb_profile_end(int32_t capacity, int32_t* kinds, float* ms, double* flops, double* bytes,
                     int32_t* count);
 
-/* Debug: timeline trace of CTA 0 of the tensor-core layer kernel.  `device_buffer`
- * (64 tiles x 8 events of int64 clock64 values; NULL disables) receives, per tile:
- * [0] MMA: accumulator free  [1] MMA: first operands landed  [2] MMA: last commit issued
- * [3] epilogue: accumulator ready  [4] epilogue: LayerNorm statistics done
- * [5] epilogue: tile stored. */
+/* Debug: timeline trace of CTA 0 of the tensor-core layer and chain kernels.  `device_buffer`
+ * (64 units x 16 events of int64; NULL disables) receives, per unit, clock64 stamps of
+ * consumer warp 4 unless a count:
+ * [0] unit start  [1] first full barrier passed  [2] h_free passed (chain)  [3] MMAs retired
+ * [4] LayerNorm statistics combined  [5] epilogue stored  [6] hand-over done (chain)
+ * [7] cycles the TMA warp waited on empty barriers  [8] cycles it waited on h_full (chain)
+ * [9] K-steps  [11] layer (chain). */
 int gcb_debug_trace(long long* device_buffer);
 
-/* Debug only: experiment switches of the tensor-core kernel for performance attribution
- * (0 = production behaviour).  2: skip all global stores of the epilogue (results are NOT
- * produced); 4: N-split pairs stream the whole A block per CTA instead of multicasting halves
- * (same results); 16: L2-prefetch the A blocks of the next tile (same results). */
+/* Kept for ABI compatibility: this build has no kernel experiment switches.  Returns GCB_OK
+ * for 0 and GCB_ERR_INVALID for any other value; touches no CUDA state. */
 int gcb_debug_flags(int flags);
 
 /* Device self-test of the tensor-core layer against the FP32_SIMT arm on random

@@ -80,6 +80,14 @@ def test_layer_validation_rejects_bad_descriptors():
     _native.check(-1, "x")
 
 
+def test_debug_flags_accepts_only_zero():
+  """The build has no kernel experiment switches: 0 is accepted, anything else is an error."""
+  lib = _native.lib()
+  assert lib.gcb_debug_flags(0) == 0
+  with pytest.raises(ValueError, match="no experiment switches"):
+    _native.check(lib.gcb_debug_flags(2), "gcb_debug_flags")
+
+
 def test_struct_layouts_match_the_header():
   """ctypes mirrors vs the C structs: sizes computed by a C compiler from the header itself."""
   import subprocess

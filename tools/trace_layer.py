@@ -2,8 +2,7 @@
 
   python tools/trace_layer.py            # six layer shapes, 1184 tiles
   python tools/trace_layer.py big        # two image-fed shapes at 3.0M rows (HBM resident)
-  python tools/trace_layer.py flags      # attribution sweep over gcb_debug_flags (2, 4, 16)
-  python tools/trace_layer.py cluster    # cluster 1 vs 2, with / without global stores
+  python tools/trace_layer.py cluster    # cluster 1 vs 2
 
 Columns: cycles (clock64) of consumer warp 4 for the first units of CTA 0 (wait for the first
 operands, MMA phase and its cycles per K-step against the tensor-pipe ideal, LayerNorm statistics,
@@ -72,26 +71,14 @@ def run(rows, k, n, ln, act, csize, out_y=False, residual=False, idx=False, pre=
           f"next unit+{t[i+1,0]-r[0]:7d} | tma_blocked={r[7]}")
 
 import sys
-big = len(sys.argv) > 1 and sys.argv[1] in ("big", "flags", "cluster")
+big = len(sys.argv) > 1 and sys.argv[1] in ("big", "cluster")
 if len(sys.argv) > 1 and sys.argv[1] == "cluster":
   for cs in (1, 2):
-    for fl in (0, 2):
-      print("== cluster", cs, "flags", fl)
-      lib.gcb_debug_flags(fl)
-      run(132 * 128 * 160, 512, 512, False, True, cs, img_in=True, img_out=True)
-      run(132 * 128 * 160, 512, 512, True, False, cs, img_in=True)
-  lib.gcb_debug_flags(0)
+    print("== cluster", cs)
+    run(132 * 128 * 160, 512, 512, False, True, cs, img_in=True, img_out=True)
+    run(132 * 128 * 160, 512, 512, True, False, cs, img_in=True)
   sys.exit(0)
 rows = 132 * 128 * (160 if big else 8)
-if len(sys.argv) > 1 and sys.argv[1] == "flags":
-  # attribution sweep: 2 no global stores | 4 N-split pair without A multicast | 16 L2 prefetch
-  for fl in (0, 2, 4, 16, 2 | 4):
-    print(f"==== debug flags {fl}")
-    lib.gcb_debug_flags(fl)
-    run(rows, 512, 512, False, True, 2, img_in=True, img_out=True)
-    run(rows, 512, 512, True, False, 2, img_in=True)
-  lib.gcb_debug_flags(0)
-  sys.exit(0)
 for cs in (2,):
   run(rows, 512, 512, False, True, cs, img_in=True, img_out=True)
   run(rows, 512, 512, True, False, cs, img_in=True)
