@@ -19,6 +19,7 @@ GCB_MAX_MSG_STEPS = 64
 PREC_BF16X3, PREC_BF16, PREC_FP32_SIMT = 0, 1, 2
 PRECISIONS = {"bf16x3": PREC_BF16X3, "bf16": PREC_BF16, "fp32_simt": PREC_FP32_SIMT}
 ACT_NONE, ACT_SWISH = 0, 1
+BCAST_NONE, BCAST_LAT, BCAST_LAT_LON = 0, 1, 2
 
 _fp = C.c_void_p   # device pointers are passed as raw addresses
 
@@ -148,6 +149,10 @@ EXPORTS = {
                                                 C.c_int32, _fp, _fp, _fp, _fp, C.c_int32, _fp]),
     "gcb_input_grad": (C.c_int, [_fp, C.c_int32, C.c_int64, C.c_int32, _fp, _fp, _fp, C.c_int32,
                                  _fp]),
+    "gcb_output_cotangent_grad_feedback": (C.c_int, [C.c_int32, C.c_int64, _fp, _fp, _fp, _fp,
+                                                     C.c_int32, _fp, _fp, _fp, _fp, C.c_int32, _fp]),
+    "gcb_broadcast_grad_sum": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, _fp, C.c_int32, _fp,
+                                         C.c_int32, _fp]),
     "gcb_weight_grad_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
     "gcb_weight_grad": (C.c_int, [_fp, C.c_int32, C.c_int32, _fp, C.c_int32, _fp, C.c_int32,
                                   C.c_int64, C.c_int32, C.c_int32, C.c_int32, _fp, C.c_int64, _fp,

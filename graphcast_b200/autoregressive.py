@@ -154,16 +154,32 @@ class Predictor(graphcast.Predictor):
     forcings = xs.from_xarray(forcings)
     if targets.sizes["time"] == 1:
       return self._predictor.loss_and_grads(inputs, targets, forcings, **kwargs)
+    model, norm_of = self._checkpointed_parts(inputs, targets, forcings, "loss_and_grads")
+    loss, diagnostics, stash, first, lat_weight, coef = self._checkpointed_loss(
+        model, norm_of, inputs, targets, forcings)
+    plan = feedback.FeedbackPlan(first["inputs"], first["targets"], first["forcings"])
+    grads = model._bptt_grads(stash, plan, first["norm"], lat_weight, coef)
+    return loss, diagnostics, grads
+
+  def _checkpointed_parts(self, inputs, targets, forcings, what: str):
+    """(GraphCast, norm_of) for a gradient over several target times, with its refusals."""
     if not self._gradient_checkpointing:
       raise NotImplementedError(
-          "loss_and_grads over several target times (backprop through time) recomputes every step "
+          f"{what} over several target times (backprop through time) recomputes every step "
           "from its saved inputs: construct autoregressive.Predictor with gradient_checkpointing=True")
     parts = self._device_parts()
     if parts is None:
       raise NotImplementedError("backprop through time needs a GraphCast predictor, directly or inside "
                                 "InputsAndResiduals (the fused normalisation)")
-    model, norm_of = parts
     self._validate(inputs, targets, forcings)
+    return parts
+
+  @staticmethod
+  def _checkpointed_loss(model, norm_of, inputs, targets, forcings):
+    """The forward of a gradient over several target times: the device path of `loss`, which also
+    keeps every step's input and target planes in pinned host memory (graphcast.StepStash).  Returns
+    (loss, diagnostics, stash, first step's {inputs, targets, forcings, norm}, latitude weights,
+    loss-derivative coefficients 2 kappa / (batch * steps))."""
     records, first = [], {}
     stash = None
 
@@ -185,15 +201,65 @@ class Predictor(graphcast.Predictor):
     sums = torch.stack([s for _, s in records]).cpu().numpy()      # the one read-back
     records = [finish(sums[t]) for t, (finish, _) in enumerate(records)]
     loss, diagnostics = _mean_over_time([l for l, _ in records], [d for _, d in records])
-
-    plan = feedback.FeedbackPlan(first["inputs"], first["targets"], first["forcings"])
-    num_steps, batch = len(records), stash.batch
     slabs = model_utils.channel_layout(first["targets"])
     kappa = losses.channel_kappa(slabs, model.engine.num_grid, graphcast.LOSS_PER_VARIABLE_WEIGHTS)
     lat_weight = model._lat_weight(first["targets"], model.engine.device)
-    grads = model._bptt_grads(stash, plan, first["norm"], lat_weight,
-                              2.0 * kappa / (batch * num_steps))
-    return loss, diagnostics, grads
+    return (loss, diagnostics, stash, first, lat_weight,
+            2.0 * kappa / (stash.batch * len(records)))
+
+  def loss_and_input_grads(self, inputs, targets, forcings, **kwargs):
+    """(loss, diagnostics, input_grads, forcing_grads): `loss` and `diagnostics` exactly as `loss`
+    returns them, the gradients of loss.mean() with respect to every variable of `inputs` and
+    `forcings` (GraphCast.loss_and_input_grads).  One target time delegates to the inner predictor;
+    several differentiate through the fed-back predictions and forcings as loss_and_grads does
+    (gradient_checkpointing=True), over every input channel (feedback.FeedbackPlan.all_channels): the
+    inputs collect every step's contributions, the forcings of target time t those of step t and of
+    the last input frame of step t + 1."""
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    forcings = xs.from_xarray(forcings)
+    if targets.sizes["time"] == 1:
+      return self._predictor.loss_and_input_grads(inputs, targets, forcings, **kwargs)
+    model, norm_of = self._checkpointed_parts(inputs, targets, forcings, "input gradients")
+    loss, diagnostics, stash, first, lat_weight, coef = self._checkpointed_loss(
+        model, norm_of, inputs, targets, forcings)
+    plan = feedback.FeedbackPlan.all_channels(first["inputs"], first["targets"], first["forcings"])
+    input_grads, forcing_grads = model._input_grads(stash, plan, first["norm"], inputs, forcings,
+                                                    lat_weight=lat_weight, coef=coef)
+    return loss, diagnostics, input_grads, forcing_grads
+
+  def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
+    """(predictions, input_grads, forcing_grads): `predictions` as __call__ returns them, the gradients
+    of sum(cotangents * predictions) over all target times with respect to every variable of `inputs`
+    and `forcings` (GraphCast.input_vjp), through the fed-back predictions and forcings.  One target
+    time delegates to the inner predictor; several need gradient_checkpointing=True."""
+    inputs, targets_template = xs.from_xarray(inputs), xs.from_xarray(targets_template)
+    forcings, cotangents = xs.from_xarray(forcings), xs.from_xarray(cotangents)
+    if targets_template.sizes["time"] == 1:
+      return self._predictor.input_vjp(inputs, targets_template, forcings, cotangents, **kwargs)
+    model, norm_of = self._checkpointed_parts(inputs, targets_template, forcings, "input gradients")
+    first = {}
+    stash = None
+
+    def step(rng, inputs, targets_template, forcings):
+      nonlocal stash
+      norm = norm_of(inputs, targets_template, forcings)
+      predictions = model._call(inputs, targets_template, forcings, norm=norm)
+      if stash is None:
+        stash = graphcast.StepStash(model.engine.device)
+        first.update(inputs=inputs, targets=targets_template, forcings=forcings, norm=norm)
+      stash.save(model._planes_in)
+      return predictions
+
+    chunks = list(rollout.chunked_prediction_generator(
+        step, rng=None, inputs=inputs, targets_template=targets_template, num_steps_per_chunk=1,
+        forcings=forcings))
+    predictions = xs.concat_time(chunks)
+    plan = feedback.FeedbackPlan.all_channels(first["inputs"], first["targets"], first["forcings"])
+    cot = [model._cotangent_planes(cotangents.isel(time=slice(t, t + 1)), first["targets"],
+                                   stash.batch) for t in range(len(stash.steps))]
+    input_grads, forcing_grads = model._input_grads(stash, plan, first["norm"], inputs, forcings,
+                                                    cotangents=cot)
+    return predictions, input_grads, forcing_grads
 
 
 def _mean_over_time(step_losses, step_diagnostics):

@@ -117,6 +117,10 @@ class Backward:
     self.ws_rows = torch.empty([max(self.lib.gcb_rowwise_workspace_bytes(D), 16)], dtype=torch.uint8, device=dev)
     nb = self.lib.gcb_weight_grad_workspace_bytes(D, D)     # the largest single call: k = n = 512
     self.ws_wg = torch.empty([nb], dtype=torch.uint8, device=dev)
+    # element(param_grads=False): the column sums of the row-wise kernels land here, never in info.g
+    self.param_grads = True
+    self.sink = {f: torch.zeros([D], dtype=torch.float32, device=dev)
+                 for f in ("b0", "b1", "scale", "offset")}
 
   # -- setup ---------------------------------------------------------------------------------
   def _i32(self, a):
@@ -275,7 +279,7 @@ class Backward:
     w = info.w
     h = self.empty(rows)
     self.layer(rows, segs, w0 or w.w0_packed, w.b0, _native.ACT_NONE, out_y=h, pre=pre)
-    g = info.g
+    g = info.g if self.param_grads else self.sink
     ws = self.ws_rows
     if info.ln:
       a = self.empty(rows)
@@ -295,7 +299,8 @@ class Backward:
       _native.check(self.lib.gcb_layernorm_backward(
           dy.data_ptr(), dy.shape[1], None, 0, None, rows, info.n1, None, 0, ws.data_ptr(),
           ws.numel(), g["b1"].data_ptr(), None, None, 1, self._st()), "gcb_layernorm_backward")
-    self.wgrad(self.tab(h), dz, rows, g["w1"], n=info.n1, swish=True)     # dW1 = swish(h)^T dz
+    if self.param_grads:
+      self.wgrad(self.tab(h), dz, rows, g["w1"], n=info.n1, swish=True)     # dW1 = swish(h)^T dz
     da = self.empty(rows)
     self.layer(rows, [self.tab(dz, info.n1)], info.t["w1"], self.zero_bias, out_y=da)
     dh = self.empty(rows)
@@ -303,11 +308,12 @@ class Backward:
         da.data_ptr(), D, h.data_ptr(), D, rows, D, dh.data_ptr(), D, ws.data_ptr(), ws.numel(),
         g["b0"].data_ptr(), 1, self._st()), "gcb_swish_backward")
     del da, h
-    off = 0
-    for s in (dw_segs if dw_segs is not None else segs):
-      k = s[2]
-      self.wgrad(s, dh, rows, g["w0"][off:off + k])
-      off += k
+    if self.param_grads:
+      off = 0
+      for s in (dw_segs if dw_segs is not None else segs):
+        k = s[2]
+        self.wgrad(s, dh, rows, g["w0"][off:off + k])
+        off += k
     return dh
 
   def seg_sum_sender(self, name: str, dh: torch.Tensor, num_nodes: int) -> torch.Tensor:
@@ -350,9 +356,10 @@ class Backward:
     del ps, pr
     s = self.seg_sum_sender(snd_name, dh, n_s)
     r = rcv_sum(dh)
-    w0 = info.g["w0"]
-    self.wgrad(v_s, s, n_s, w0[D:2 * D])
-    self.wgrad(v_r, r, n_r, w0[2 * D:3 * D])
+    if self.param_grads:
+      w0 = info.g["w0"]
+      self.wgrad(v_s, s, n_s, w0[D:2 * D])
+      self.wgrad(v_r, r, n_r, w0[2 * D:3 * D])
     return dh, s, r
 
   def bipartite_backward(self, name: str, info: _MlpInfo, enc: _MlpInfo, feat_t: torch.Tensor,
@@ -385,25 +392,42 @@ class Backward:
       _native.check(self.lib.gcb_segment_sum_heavy(
           dh.data_ptr(), D, rp.data_ptr(), g1 - g0, heavy.data_ptr() if n_heavy else None, n_heavy,
           r_tab[g0:g1].data_ptr(), D, D, self._st()), "gcb_segment_sum_heavy")
-      de = self.empty(n)
-      self.layer(n, [self.tab(dh)], info.t["w0_0"], self.zero_bias, out_y=de)
-      del dh
-      self.mlp_backward(enc, n, [f], de)
-      del de
+      if self.param_grads:                  # the edge embedder's backward: parameters only
+        de = self.empty(n)
+        self.layer(n, [self.tab(dh)], info.t["w0_0"], self.zero_bias, out_y=de)
+        del dh
+        self.mlp_backward(enc, n, [f], de)
+        del de
+      else:
+        del dh
     del ps, pr
-    w0 = info.g["w0"]
-    self.wgrad(v_s, s_tab, n_s, w0[D:2 * D])
-    self.wgrad(v_r, r_tab, n_r, w0[2 * D:3 * D])
+    if self.param_grads:
+      w0 = info.g["w0"]
+      self.wgrad(v_s, s_tab, n_s, w0[D:2 * D])
+      self.wgrad(v_r, r_tab, n_r, w0[2 * D:3 * D])
     return s_tab, r_tab
 
   # -- one batch element ---------------------------------------------------------------------------
   def element(self, grid_in_img: torch.Tensor, g_out: torch.Tensor, snaps: dict,
-              dgrid_in: bool = False) -> Optional[torch.Tensor]:
+              dgrid_in: bool = False, param_grads: bool = True) -> Optional[torch.Tensor]:
     """Accumulates the parameter gradients of one batch element whose loss derivative with respect
     to the decoder output is g_out [Ng, 256] (gcb_output_loss_grad) and whose forward left `snaps`
     (whose entries are dropped as they are consumed).  dgrid_in: also return the derivative with
     respect to the packed grid inputs, dh_enc_grid W0^T [Ng, n] (see input_transposed; columns >=
-    c_in + 3 are zero)."""
+    c_in + 3 are zero).
+
+    param_grads=False (with dgrid_in: the input gradient alone) leaves the accumulators untouched and
+    skips what only the parameters need: every gcb_weight_grad, the backward passes of the three edge
+    embedders and of the mesh-node encoder, and the de product of the first processor step.  The
+    row-wise kernels' column sums go to scratch.  The recomputes and the dX products that remain are
+    the same launches on the same operands, so dx is bit-identical to that of param_grads=True."""
+    self.param_grads = bool(param_grads)
+    try:
+      return self._element(grid_in_img, g_out, snaps, dgrid_in)
+    finally:
+      self.param_grads = True
+
+  def _element(self, grid_in_img, g_out, snaps, dgrid_in):
     eng, m = self.eng, self.m
     ng, nm = m.num_grid, m.num_mesh
     K = eng.msg_steps
@@ -456,11 +480,14 @@ class Backward:
           efo, m.e_mesh, e_k, dm, "mesh", v_k, nm, eng.mesh_snd, v_k, nm, eng.mesh_rcv,
           lambda d: self.seg_sum_receiver(d, eng.mesh_row_ptr, nm))
       del dm
-      de = self.empty(m.e_mesh)              # de_k = de_{k+1} + dH W_e^T  (e' = e + m)
-      if de_next is None:
-        self.layer(m.e_mesh, [tab(dH)], efo.t["w0_0"], self.zero_bias, out_y=de)
+      if k == 0 and not self.param_grads:    # de_0 feeds the mesh edge embedder's parameters only
+        de = None
       else:
-        self.layer(m.e_mesh, [tab(dH)], efo.t["w0_0"], self.zero_bias, residual=de_next, out=de)
+        de = self.empty(m.e_mesh)            # de_k = de_{k+1} + dH W_e^T  (e' = e + m)
+        if de_next is None:
+          self.layer(m.e_mesh, [tab(dH)], efo.t["w0_0"], self.zero_bias, out_y=de)
+        else:
+          self.layer(m.e_mesh, [tab(dH)], efo.t["w0_0"], self.zero_bias, residual=de_next, out=de)
       del dH
       de_next = de
       # dv_k = dv_{k+1} + dh_n W0a^T + S W_s^T + R W_r^T
@@ -473,7 +500,8 @@ class Backward:
       del dh_n, S, R, dv2
       snaps["v"][k + 1] = snaps["agg"][k] = snaps["e"][k] = None
     # mesh edge embedder: e0 = MLP(edge features)
-    self.mlp_backward(mp["enc_e_mesh"], m.e_mesh, [feat(eng.mesh_feat)], de_next)
+    if self.param_grads:
+      self.mlp_backward(mp["enc_e_mesh"], m.e_mesh, [feat(eng.mesh_feat)], de_next)
     del de_next, e0
 
     # ---- encoder: vg1 = vg0 + MLP([vg0]);  vm1 = vm0 + MLP([vm0 | agg1]);
@@ -512,7 +540,8 @@ class Backward:
       dx = self.empty(ng, n)
       self.layer(ng, [tab(dh)], w0t, self.zero_bias, out_y=dx, n=n)
     del dh, dvg0
-    self.mlp_backward(mp["enc_mesh"], nm, [mesh_in], dvm0)
+    if self.param_grads:
+      self.mlp_backward(mp["enc_mesh"], nm, [mesh_in], dvm0)
     return dx
 
   # -- result ----------------------------------------------------------------------------------------

@@ -65,3 +65,9 @@ class Bfloat16Cast(graphcast.Predictor):
 
   def loss_and_grads(self, inputs, targets, forcings, **kwargs):
     return self._predictor.loss_and_grads(inputs, targets, forcings, **kwargs)
+
+  def loss_and_input_grads(self, inputs, targets, forcings, **kwargs):
+    return self._predictor.loss_and_input_grads(inputs, targets, forcings, **kwargs)
+
+  def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
+    return self._predictor.input_vjp(inputs, targets_template, forcings, cotangents, **kwargs)

@@ -881,6 +881,58 @@ int gcb_input_grad(const float* dx, int32_t ld_dx, int64_t n_nodes, int32_t n_ro
   return GCB_OK;
 }
 
+int gcb_output_cotangent_grad_feedback(int32_t n_out, int64_t n_nodes, const float* scale,
+                                       const float* cot, const float* a_next,
+                                       const int32_t* dpred_row, int32_t n_rows,
+                                       const int32_t* resid_channel, const int32_t* carry_row,
+                                       float* a_out, float* g, int32_t ld_g, void* stream) {
+  GCB_CHECK_ARG(cot && g, "null pointer");
+  GCB_CHECK_ARG(n_out > 0 && ld_g >= n_out && n_nodes >= 0, "bad shape");
+  GCB_CHECK_ARG(a_next == nullptr || dpred_row != nullptr, "a_next needs dpred_row");
+  GCB_CHECK_ARG(n_rows >= 0 && (n_rows == 0 || (a_out && resid_channel)), "rows need a_out and resid_channel");
+  const int c_tiles = (n_out + 31) / 32, r_tiles = (n_rows + 31) / 32;
+  GCB_CHECK_ARG(c_tiles + r_tiles <= 65535, "too many channels / rows");
+  if (n_nodes == 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // algorithmic bytes: the cotangent read and g written, the rows written and the feedback rows read once
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * n_nodes * (n_out * (2.0 + (a_next ? 1.0 : 0.0)) + n_rows * (a_next ? 2.0 : 1.0)));
+  dim3 grid(static_cast<unsigned>((n_nodes + 31) / 32), static_cast<unsigned>(c_tiles + r_tiles));
+  gcb::output_cotangent_grad_feedback_kernel<<<grid, 256, 0, st>>>(
+      n_out, n_nodes, scale, cot, a_next, dpred_row, n_rows, resid_channel, carry_row, a_out, g, ld_g,
+      c_tiles);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int gcb_broadcast_grad_sum(const float* a, int32_t n_lat, int32_t n_lon, int32_t n_rows,
+                           const int32_t* rows, int32_t mode, float* out, int32_t accumulate,
+                           void* stream) {
+  GCB_CHECK_ARG(a && rows && out, "null pointer");
+  GCB_CHECK_ARG(n_lat > 0 && n_lon > 0 && n_rows >= 0 && n_rows <= 65535, "bad shape");
+  GCB_CHECK_ARG(mode == GCB_BCAST_NONE || mode == GCB_BCAST_LAT || mode == GCB_BCAST_LAT_LON,
+                "mode must be GCB_BCAST_NONE, GCB_BCAST_LAT or GCB_BCAST_LAT_LON");
+  if (n_rows == 0) return GCB_OK;
+  const long long n_nodes = static_cast<long long>(n_lat) * n_lon;
+  const long long width = mode == GCB_BCAST_NONE ? n_nodes : (mode == GCB_BCAST_LAT ? n_lon : 1);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * n_rows * (static_cast<double>(n_nodes) + width * (accumulate ? 2.0 : 1.0)));
+  const int acc = accumulate ? 1 : 0;
+  if (mode == GCB_BCAST_LAT_LON) {
+    gcb::broadcast_grad_sum_kernel<gcb::kBcastLatLon><<<dim3(1, n_rows), 256, 0, st>>>(
+        a, n_lat, n_lon, rows, out, acc);
+  } else {
+    dim3 grid(static_cast<unsigned>((width + 255) / 256), static_cast<unsigned>(n_rows));
+    if (mode == GCB_BCAST_LAT)
+      gcb::broadcast_grad_sum_kernel<gcb::kBcastLat><<<grid, 256, 0, st>>>(a, n_lat, n_lon, rows, out, acc);
+    else
+      gcb::broadcast_grad_sum_kernel<gcb::kBcastNone><<<grid, 256, 0, st>>>(a, n_lat, n_lon, rows, out, acc);
+  }
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
 int64_t gcb_weight_grad_workspace_bytes(int32_t k, int32_t n) {
   if (k <= 0 || n <= 0) return -1;
   return static_cast<int64_t>(gcb::kWgSlices) * k * n * static_cast<int64_t>(sizeof(float));

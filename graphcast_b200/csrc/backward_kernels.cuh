@@ -543,4 +543,108 @@ input_grad_kernel(const float* __restrict__ dx, int ld_dx, long long n_nodes, in
   }
 }
 
+// ---- input gradients of a vector-Jacobian product ---------------------------------------------------
+// The seed of J = sum cot * pred over the physical predictions pred = y * scale + (offset | add), with
+// the feedback of output_loss_grad_feedback_kernel: d[c, node] = cot[c, node] + a_next[dpred_row[c], node]
+// (the second term when a_next != NULL and dpred_row[c] >= 0; fp64, rounded once) is dJ/dpred.
+// Blocks with blockIdx.y < c_tiles: g[node, c] = (float)(scale[c] * d), node-major through the 32 x 32
+// shared-memory transpose.  The other blocks: rows r of a_out, channel-major,
+//   a_out[r, node] = (c = resid_channel[r]) >= 0 ? (float)d[c, node] : 0  (+ a_next[carry_row[r], node])
+__device__ __forceinline__ double cotangent_d(int c, long long node, long long n_nodes,
+                                              const float* __restrict__ cot,
+                                              const float* __restrict__ a_next,
+                                              const int* __restrict__ dpred_row) {
+  double d = static_cast<double>(cot[static_cast<long long>(c) * n_nodes + node]);
+  const int q = a_next ? dpred_row[c] : -1;
+  if (q >= 0) d += static_cast<double>(a_next[static_cast<long long>(q) * n_nodes + node]);
+  return d;
+}
+
+__global__ void __launch_bounds__(256)
+output_cotangent_grad_feedback_kernel(int n_out, long long n_nodes, const float* __restrict__ scale,
+                                      const float* __restrict__ cot, const float* __restrict__ a_next,
+                                      const int* __restrict__ dpred_row, int n_rows,
+                                      const int* __restrict__ resid_channel,
+                                      const int* __restrict__ carry_row, float* __restrict__ a_out,
+                                      float* __restrict__ g, int ld_g, int c_tiles) {
+  const long long node0 = static_cast<long long>(blockIdx.x) * 32;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  if (static_cast<int>(blockIdx.y) < c_tiles) {
+    __shared__ float tile[32][33];
+    const int c0 = blockIdx.y * 32;
+    for (int r = ty; r < 32; r += 8) {
+      const int c = c0 + r;
+      const long long node = node0 + tx;
+      float v = 0.f;
+      if (c < n_out && node < n_nodes) {
+        const double sc = scale ? static_cast<double>(scale[c]) : 1.0;
+        v = static_cast<float>(sc * cotangent_d(c, node, n_nodes, cot, a_next, dpred_row));
+      }
+      tile[r][tx] = v;
+    }
+    __syncthreads();
+    for (int r = ty; r < 32; r += 8) {
+      const long long node = node0 + r;
+      const int c = c0 + tx;
+      if (c < n_out && node < n_nodes) g[node * ld_g + c] = tile[tx][r];
+    }
+    return;
+  }
+  const int r0 = (static_cast<int>(blockIdx.y) - c_tiles) * 32;
+  for (int q = ty; q < 32; q += 8) {
+    const int r = r0 + q;
+    const long long node = node0 + tx;
+    if (r >= n_rows || node >= n_nodes) continue;
+    const int c = resid_channel[r];
+    float v = c >= 0 ? static_cast<float>(cotangent_d(c, node, n_nodes, cot, a_next, dpred_row)) : 0.f;
+    const int k = (a_next && carry_row) ? carry_row[r] : -1;
+    if (k >= 0) v = __fadd_rn(v, a_next[static_cast<long long>(k) * n_nodes + node]);
+    a_out[static_cast<long long>(r) * n_nodes + node] = v;
+  }
+}
+
+// Transpose of the host broadcast of a variable that lacks lat and / or lon (model_utils
+// .variable_to_planes): for row i of the list, the plane a[rows[i]] [n_lat, n_lon] summed over lat
+// (kMode 1: out [n_rows, n_lon]), over lat and lon (kMode 2: out [n_rows]) or not at all (kMode 0: out
+// [n_rows, n_lat * n_lon]).  fp64 sums in a fixed order, one rounding per output element, optionally
+// added to out (accumulate: out = (float)(out + sum)).
+constexpr int kBcastNone = 0, kBcastLat = 1, kBcastLatLon = 2;
+
+template <int kMode>
+__global__ void __launch_bounds__(256)
+broadcast_grad_sum_kernel(const float* __restrict__ a, int n_lat, int n_lon,
+                          const int* __restrict__ rows, float* __restrict__ out, int accumulate) {
+  const long long n_nodes = static_cast<long long>(n_lat) * n_lon;
+  const int i = blockIdx.y;
+  const float* src = a + static_cast<long long>(rows[i]) * n_nodes;
+  if constexpr (kMode == kBcastLatLon) {
+    __shared__ double part[256];
+    double s = 0.0;
+    for (long long j = threadIdx.x; j < n_nodes; j += 256) s += static_cast<double>(__ldg(src + j));
+    part[threadIdx.x] = s;
+    __syncthreads();
+    for (int w = 128; w > 0; w >>= 1) {
+      if (static_cast<int>(threadIdx.x) < w) part[threadIdx.x] += part[threadIdx.x + w];
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+      float* p = out + i;
+      *p = static_cast<float>(accumulate ? static_cast<double>(*p) + part[0] : part[0]);
+    }
+  } else {
+    const long long width = kMode == kBcastLat ? n_lon : n_nodes;
+    const long long j = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+    if (j >= width) return;
+    double s;
+    if constexpr (kMode == kBcastLat) {
+      s = 0.0;
+      for (int la = 0; la < n_lat; ++la) s += static_cast<double>(__ldg(src + static_cast<long long>(la) * n_lon + j));
+    } else {
+      s = static_cast<double>(__ldg(src + j));
+    }
+    float* p = out + static_cast<long long>(i) * width + j;
+    *p = static_cast<float>(accumulate ? static_cast<double>(*p) + s : s);
+  }
+}
+
 }  // namespace gcb

@@ -637,12 +637,17 @@ class Engine:
     weights, sender CSRs, accumulators) is created by the first call, so inference never holds it.
     chunk_rows: edges per chunk of the grid2mesh / mesh2grid edge-MLP backward passes (default 2^19;
     the peak memory of the backward pass scales with it)."""
+    self._grad_workspace(chunk_rows, "parameter gradients")
+    self._backward.zero_grads()
+
+  def _grad_workspace(self, chunk_rows: Optional[int], what: str) -> None:
+    """The checks of every gradient and the gradient workspace, created on first use."""
     if self.num_grid_owned:
       raise NotImplementedError(
-          "parameter gradients are not available in the node-partitioned engine: each rank holds "
+          f"{what} are not available in the node-partitioned engine: each rank holds "
           "only its own grid rows; compute them with a single-GPU GraphCast")
     if self.precision not in ("bf16x3", "bf16"):
-      raise NotImplementedError(f"parameter gradients support the tensor-core precisions 'bf16x3' "
+      raise NotImplementedError(f"{what} support the tensor-core precisions 'bf16x3' "
                                 f"and 'bf16', not {self.precision!r}")
     if self._backward is None or (chunk_rows and chunk_rows != self._backward.chunk_rows):
       from graphcast_b200 import backward
@@ -651,7 +656,6 @@ class Engine:
         self._backward = (backward.Backward(self, chunk_rows) if chunk_rows
                           else backward.Backward(self))
     self._backward.prec = _native.PRECISIONS[self.precision]
-    self._backward.zero_grads()
 
   def loss_and_grads_element(self, targets_planes: torch.Tensor, lat_weight: torch.Tensor,
                              coef: torch.Tensor, *, channel_sums: torch.Tensor,
@@ -730,6 +734,86 @@ class Engine:
             dx.data_ptr(), dx.shape[1], self.num_grid, n_rows, fb.rows.data_ptr(),
             self._ptr(fb.in_scale), a_out.data_ptr(), 1, self._stream()), "gcb_input_grad")
 
+  # -- input gradients (loss_and_input_grads, input_vjp) ---------------------------------------------
+  def input_grads_begin(self) -> None:
+    """The gradient workspace of `input_grads_element`, with the checks of grads_begin; the parameter
+    accumulators are neither zeroed nor touched."""
+    self._grad_workspace(None, "input gradients")
+
+  def input_grads_element(self, fb: "Feedback", operands: dict, *,
+                          lat_weight: Optional[torch.Tensor] = None, coef: Optional[torch.Tensor] = None,
+                          channel_sums: Optional[torch.Tensor] = None,
+                          planes_out: Optional[torch.Tensor] = None,
+                          grid_in: Optional[torch.Tensor] = None) -> None:
+    """One step of one batch element of an input gradient: the step stage by stage from `grid_in`
+    (default: the packed grid_in_img), the seed, and the backward pass without parameter gradients
+    (Backward.element(param_grads=False)).  Afterwards fb.a [fb.n_rows, Ng] is the derivative with
+    respect to this step's input planes (physical units) on fb's rows, fb.a of the following step
+    having been consumed by the seed.
+
+    With channel_sums the forward's loss sums go there (output_loss); with planes_out its predictions
+    (unpack_outputs), as the step and unpack of __call__ would give them.  Both are optional: a
+    recomputed step of a rollout needs neither.
+
+    The seed is either the loss of loss_and_grads_element (operands["targets_planes"], lat_weight,
+    coef = 2 kappa / (batch * steps): gcb_output_loss_grad_feedback) or, with
+    operands["cotangent"] [n_out, Ng], J = sum cotangent * prediction
+    (gcb_output_cotangent_grad_feedback).  `operands` also holds the affine keywords of output_loss
+    (scale, offset, add_planes, add_plane_index).  The seed is their last reader: the dict is cleared
+    after it, so that planes the caller no longer references are free during the backward pass."""
+    if self._backward is None:
+      raise RuntimeError("call input_grads_begin() first")
+    affine = {k: operands[k] for k in ("scale", "offset", "add_planes", "add_plane_index")
+              if k in operands}
+    targets_planes, cotangent = operands.get("targets_planes"), operands.get("cotangent")
+    operands.clear()
+    grid_in = self.grid_in_img if grid_in is None else grid_in
+    snaps = self._forward_snapshots(grid_in)
+    g_out = torch.zeros([self.num_grid, 256], dtype=torch.float32, device=self.device)
+    a_out = torch.empty([fb.n_rows, self.num_grid], dtype=torch.float32, device=self.device)
+    with self._on_device():
+      if planes_out is not None:
+        self.unpack_outputs(planes_out, **affine)
+      if channel_sums is not None:
+        self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
+      if cotangent is None:
+        n_lat = lat_weight.shape[0]
+        _native.check(self._lib.gcb_output_loss_grad_feedback(
+            self.grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat,
+            self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
+            self._ptr(affine.get("add_planes")), self._ptr(affine.get("add_plane_index")),
+            targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), self._ptr(fb.a),
+            fb.dpred_row.data_ptr(), fb.n_rows, fb.resid_channel.data_ptr(), fb.carry_row.data_ptr(),
+            a_out.data_ptr(), g_out.data_ptr(), 256, self._stream()), "gcb_output_loss_grad_feedback")
+      else:
+        if tuple(cotangent.shape) != (self.n_out, self.num_grid) or not cotangent.is_contiguous():
+          raise ValueError(f"cotangent must be a contiguous [{self.n_out}, {self.num_grid}] tensor")
+        _native.check(self._lib.gcb_output_cotangent_grad_feedback(
+            self.n_out, self.num_grid, self._ptr(affine.get("scale")), cotangent.data_ptr(),
+            self._ptr(fb.a), fb.dpred_row.data_ptr(), fb.n_rows, fb.resid_channel.data_ptr(),
+            fb.carry_row.data_ptr(), a_out.data_ptr(), g_out.data_ptr(), 256, self._stream()),
+            "gcb_output_cotangent_grad_feedback")
+      # the following step's rows, the planes, targets and cotangent are consumed: release them
+      fb.a = a_out
+      affine = targets_planes = cotangent = None
+      dx = self._backward.element(grid_in, g_out, snaps, dgrid_in=True, param_grads=False)
+      _native.check(self._lib.gcb_input_grad(
+          dx.data_ptr(), dx.shape[1], self.num_grid, fb.n_rows, fb.rows.data_ptr(),
+          self._ptr(fb.in_scale), a_out.data_ptr(), 1, self._stream()), "gcb_input_grad")
+
+  def broadcast_grad_sum(self, a: torch.Tensor, n_lat: int, rows: torch.Tensor, mode: int,
+                         out: torch.Tensor, accumulate: bool) -> None:
+    """gcb_broadcast_grad_sum on the current stream: the planes a[rows] ([*, Ng] fp32) reduced into
+    `out` ([len(rows), Ng | n_lon | 1]) over the axes of `mode` (_native.BCAST_*)."""
+    n_lon = self.num_grid // n_lat
+    width = (self.num_grid, n_lon, 1)[mode]
+    if out.numel() != rows.numel() * width or not out.is_contiguous() or out.dtype != torch.float32:
+      raise ValueError(f"out must be a contiguous float32 tensor of {rows.numel() * width} elements")
+    with self._on_device():
+      _native.check(self._lib.gcb_broadcast_grad_sum(
+          a.data_ptr(), n_lat, n_lon, rows.numel(), rows.data_ptr(), mode, out.data_ptr(),
+          1 if accumulate else 0, self._stream()), "gcb_broadcast_grad_sum")
+
   def grads(self):
     """The accumulated gradients: device fp32 tensors keyed and shaped like the params."""
     return self._backward.grads()
@@ -749,7 +833,7 @@ class Engine:
       raise ValueError(f"feedback plan of {plan.c_in} -> {plan.n_out} channels, engine "
                        f"{self.c_in} -> {self.n_out}")
     if self._backward is None:
-      raise RuntimeError("call grads_begin() first")
+      raise RuntimeError("call grads_begin() or input_grads_begin() first")
     with self._on_device():
       self._backward.input_transposed()
     if add_plane_index is not None and isinstance(add_plane_index, torch.Tensor):

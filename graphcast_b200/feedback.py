@@ -13,6 +13,10 @@ rollout.py:581-604) on that layout is a fixed map of channels:
 Backprop through time (autoregressive.Predictor.loss_and_grads) runs that map backwards.  The ROWS of
 the plan are the input channels that depend on the parameters: every frame of every time-dependent
 input variable that is also a target, frame-major (row k * n_fed + i is frame k of fed-back channel i).
+
+Input gradients (loss_and_input_grads / input_vjp) run it backwards over every channel:
+FeedbackPlan.all_channels has the rows 0..c_in-1 (row r = channel r), and `VariableRows` maps the rows
+back to the variables of the inputs and forcings Datasets.
 """
 
 from __future__ import annotations
@@ -99,6 +103,29 @@ class FeedbackPlan:
     self.n_frames, self.n_fed = n_frames, n_fed
     self.next_from_input, self.next_from_pred = next_from_input, next_from_pred
     self.rows, self.dpred_row, self.carry_row = rows, dpred_row, carry_row
+    self.all_rows = False
+
+  @classmethod
+  def all_channels(cls, inputs: xs.Dataset, targets: xs.Dataset,
+                   forcings: xs.Dataset) -> "FeedbackPlan":
+    """The plan whose rows are all c_in channels (row r = channel r), for gradients with respect to
+    the inputs and forcings.  dpred_row, carry_row and resid_channel keep their meaning and follow
+    next_from_input / next_from_pred: frame k + 1 -> frame k, static -> static, forcings slab -> the
+    last input frame of the same forcing variable, frame 0 -> -1.  Every channel feeds at most one
+    channel of the next step, so a single carry row per row suffices."""
+    plan = cls(inputs, targets, forcings)
+    c_in = plan.c_in
+    carry_row = np.full([c_in], -1, np.int64)
+    src = np.nonzero(plan.next_from_input >= 0)[0]
+    if np.unique(plan.next_from_input[src]).size != src.size:
+      raise ValueError("an input channel feeds several channels of the next step")
+    carry_row[plan.next_from_input[src]] = src
+    dpred_row = np.full([plan.n_out], -1, np.int64)
+    pred = np.nonzero(plan.next_from_pred >= 0)[0]
+    dpred_row[plan.next_from_pred[pred]] = pred
+    plan.rows, plan.dpred_row, plan.carry_row = np.arange(c_in, dtype=np.int64), dpred_row, carry_row
+    plan.all_rows = True
+    return plan
 
   @property
   def n_rows(self) -> int:
@@ -116,6 +143,10 @@ class FeedbackPlan:
     if add_plane_index is None:
       return out
     add = np.asarray(add_plane_index, np.int64)
+    if self.all_rows:                     # every channel is a row: any residual channel has its row
+      c = np.nonzero(add >= 0)[0]
+      out[add[c]] = c
+      return out
     last = self.last_frame_channel()
     fed = self.dpred_row >= 0
     if not np.array_equal(add[fed], last[fed]):
@@ -135,3 +166,74 @@ class FeedbackPlan:
     out[pred] = predictions[self.next_from_pred[pred]]
     out[self.n_in:] = next_forcings
     return out
+
+
+class VariableRows:
+  """Where one variable of the inputs or forcings Dataset sits in the rows of an all-channel plan and
+  how its gradient is formed from them: rows [start, start + count) of a step (the forcings of target
+  time t in step t), summed over the axes the packing broadcast the variable to.
+
+  mode     0: the variable has lat and lon, 1: it lacks lat (summed over lat), 2: it lacks both
+           (summed over lat and lon); these are gcb_broadcast_grad_sum's modes
+  batched  the variable has a batch dim; a batch-free one is summed over the batch elements
+  forcing  a variable of the forcings Dataset: its rows are those of every step's forcings slab
+  timed    a forcing with a time dim: one slab per target time (else the steps' slabs are summed)"""
+
+  def __init__(self, slab: model_utils.ChannelSlab, var: xs.DataArray, forcing: bool):
+    self.name, self.start, self.count = slab.name, slab.start, slab.count
+    self.stack_dims, self.stack_sizes = slab.stack_dims, slab.stack_sizes
+    self.var_dims = tuple(var.dims)
+    self.batched = "batch" in var.dims
+    has_lat, has_lon = "lat" in var.dims, "lon" in var.dims
+    if has_lat and not has_lon:
+      raise NotImplementedError(f"{slab.name}: input gradients of a variable with lat but no lon")
+    self.mode = 0 if has_lat else (1 if has_lon else 2)
+    self.forcing = forcing
+    self.timed = forcing and "time" in var.dims
+    self.key = ("forcings" if forcing else "inputs", slab.name)   # forcings share inputs' names
+
+  def plane_shape(self, n_lat: int, n_lon: int) -> tuple:
+    """Shape of the reduced plane of one row: (n_lat, n_lon), (n_lon,) or ()."""
+    return ((n_lat, n_lon), (n_lon,), ())[self.mode]
+
+  def reduce(self, a: np.ndarray, n_lat: int, n_lon: int) -> np.ndarray:
+    """The numpy statement of gcb_broadcast_grad_sum for this variable: a [c_in, n_lat * n_lon] (the
+    gradient of one step's planes) -> [count, *plane_shape], in float64."""
+    x = np.asarray(a[self.start:self.start + self.count], np.float64).reshape(self.count, n_lat, n_lon)
+    return x if self.mode == 0 else (x.sum(axis=1) if self.mode == 1 else x.sum(axis=(1, 2)))
+
+  def to_variable(self, g: np.ndarray, n_lat: int, n_lon: int) -> xs.DataArray:
+    """g: [batch]? ([time] for a timed forcing) [count, *plane_shape] -> the gradient as a DataArray with
+    the variable's dims, in its order.  A timed forcing's per-step slab has a time dim of size 1, whose
+    place the time axis of g takes."""
+    lead = ["batch"] if self.batched else []
+    if self.timed:
+      lead.append("time")
+    stack = [d for d in self.stack_dims if not (self.timed and d == "time")]
+    sizes = [s for d, s in zip(self.stack_dims, self.stack_sizes) if not (self.timed and d == "time")]
+    spatial = [("lat", "lon"), ("lon",), ()][self.mode]
+    arr = np.asarray(g).reshape(list(g.shape[:len(lead)]) + sizes + list(self.plane_shape(n_lat, n_lon)))
+    dims = lead + stack + list(spatial)
+    return xs.DataArray(np.ascontiguousarray(np.transpose(arr, [dims.index(d) for d in self.var_dims])),
+                        self.var_dims)
+
+
+def variable_rows(inputs: xs.Dataset, forcings: xs.Dataset) -> list:
+  """VariableRows of every variable of `inputs` and of `forcings` (one target time's slab layout), in
+  channel order."""
+  in_slabs = model_utils.channel_layout(inputs)
+  n_in = sum(s.count for s in in_slabs)
+  step = forcings.isel(time=slice(0, 1)) if "time" in forcings.sizes else forcings
+  f_slabs = model_utils.channel_layout(step, start=n_in)
+  return ([VariableRows(s, inputs.data_vars[s.name], False) for s in in_slabs] +
+          [VariableRows(s, forcings.data_vars[s.name], True) for s in f_slabs])
+
+
+def grads_to_datasets(rows: list, grads: dict, inputs: xs.Dataset, forcings: xs.Dataset,
+                      n_lat: int, n_lon: int):
+  """(input_grads, forcing_grads): Datasets with the variables, dims and coords of `inputs` and
+  `forcings`, from grads[VariableRows.key] as VariableRows.to_variable takes them."""
+  out_in, out_f = xs.Dataset(coords=inputs.coords), xs.Dataset(coords=forcings.coords)
+  for v in rows:
+    (out_f if v.forcing else out_in)[v.name] = v.to_variable(grads[v.key], n_lat, n_lon)
+  return out_in, out_f

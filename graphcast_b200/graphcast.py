@@ -32,6 +32,7 @@ import numpy as np
 import torch
 
 from graphcast_b200 import engine as engine_lib
+from graphcast_b200 import feedback
 from graphcast_b200 import graph as graph_lib
 from graphcast_b200 import losses
 from graphcast_b200 import model_utils
@@ -104,6 +105,18 @@ class Predictor(abc.ABC):
     """Returns (loss, diagnostics, grads): `loss` / `diagnostics` as `loss` returns them, `grads`
     the gradient of loss.mean() (the mean over the batch) with respect to the parameters."""
     raise NotImplementedError(f"{type(self).__name__} does not implement parameter gradients")
+
+  def loss_and_input_grads(self, inputs, targets, forcings, **optional_kwargs):
+    """Returns (loss, diagnostics, input_grads, forcing_grads): `loss` / `diagnostics` as `loss`
+    returns them, the gradients of loss.mean() with respect to every variable of `inputs` and
+    `forcings`, as float32 Datasets shaped like them."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement input gradients")
+
+  def input_vjp(self, inputs, targets_template, forcings, cotangents, **optional_kwargs):
+    """Returns (predictions, input_grads, forcing_grads): the predictions of __call__ and the
+    gradients of sum(cotangents * predictions) with respect to every variable of `inputs` and
+    `forcings`; `cotangents` is shaped like `targets_template`."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement input gradients")
 
 
 # Per-variable weights of GraphCast's loss (reference graphcast.py:341-356); others weigh 1.
@@ -283,6 +296,154 @@ class GraphCast(Predictor):
         self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
     return loss, diagnostics, self._export_grads()
 
+  def loss_and_input_grads(self, inputs, targets, forcings, **unused_kwargs):
+    """(loss, diagnostics, input_grads, forcing_grads) for one target time.
+
+    `loss` and `diagnostics` are exactly what `loss()` returns for the same call.  `input_grads` and
+    `forcing_grads` are the gradient of loss.mean() (the scalar of loss_and_grads) with respect to
+    every data variable of `inputs` and of `forcings`: float32 Datasets with their variables, dims and
+    coords, in the variables' physical units.  A variable the packing broadcast over batch, lat or lon
+    gets the sum over those axes.  The backward pass is Backward.element(param_grads=False) in the
+    model's precision, seeded and carried over every input channel (feedback.FeedbackPlan
+    .all_channels); the parameter gradients are neither computed nor touched."""
+    return self._loss_and_input_grads(inputs, targets, forcings, norm=None)
+
+  def input_vjp(self, inputs, targets_template, forcings, cotangents, **unused_kwargs):
+    """(predictions, input_grads, forcing_grads) for one target time: `predictions` is what __call__
+    returns, bit for bit; the gradients (as in loss_and_input_grads) are those of
+    J = sum over variables, batch, time, level, lat and lon of cotangents * predictions, with
+    `cotangents` a Dataset shaped like `targets_template`."""
+    return self._input_vjp(inputs, targets_template, forcings, cotangents, norm=None)
+
+  def _loss_and_input_grads(self, inputs, targets, forcings, norm: Optional[FusedNormalization]):
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    forcings = xs.from_xarray(forcings)
+    if targets.sizes.get("time", 1) != 1:
+      raise NotImplementedError("input gradients of GraphCast cover one target time (several: "
+                                "autoregressive.Predictor with gradient_checkpointing=True)")
+    batch = dict(inputs.sizes).get("batch", 1)
+    slabs = model_utils.channel_layout(targets)
+    num_grid = inputs.sizes["lat"] * inputs.sizes["lon"]
+    coef = 2.0 * losses.channel_kappa(slabs, num_grid, LOSS_PER_VARIABLE_WEIGHTS) / batch
+    run = self._one_step_input_grads(inputs, targets, forcings, norm, targets=targets, coef=coef)
+    loss, diagnostics = losses.losses_from_channel_sums(
+        self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
+    return (loss, diagnostics) + run.finish()
+
+  def _input_vjp(self, inputs, targets_template, forcings, cotangents,
+                 norm: Optional[FusedNormalization]):
+    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
+    targets_template = xs.from_xarray(targets_template)
+    if targets_template.sizes.get("time", 1) != 1:
+      raise NotImplementedError("input gradients of GraphCast cover one target time (several: "
+                                "autoregressive.Predictor with gradient_checkpointing=True)")
+    holder = {}
+    run = self._one_step_input_grads(inputs, targets_template, forcings, norm, cotangents=cotangents,
+                                     predictions=holder)
+    return (holder["predictions"],) + run.finish()
+
+  def _one_step_input_grads(self, inputs, template, forcings, norm, *, targets=None, coef=None,
+                            cotangents=None, predictions=None) -> "_InputGradRun":
+    """One target time: `_call` stages the planes once and, for every batch element, runs the
+    stage-wise forward, the seed and the backward pass of Engine.input_grads_element in place of its
+    step (no second forward, no host round trip).  With `targets` the loss sums land in
+    self._channel_sums as in `loss`; with `cotangents`, predictions["predictions"] receives the
+    predictions, unpacked from that forward as __call__ unpacks its step's.  Returns the run, whose
+    finish() gives (input_grads, forcing_grads)."""
+    state = {}
+
+    def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
+      eng = self._engine
+      if "run" not in state:
+        plan = feedback.FeedbackPlan.all_channels(inputs, template, forcings)
+        state["run"] = _InputGradRun(self, plan, norm, inputs, forcings, 1, state["batch"],
+                                     release_staging=False)
+        if cotangents is not None:
+          state["cot"] = self._cotangent_planes(cotangents, template, state["run"].batch)
+        if coef is not None:
+          state["coef"] = torch.as_tensor(np.asarray(coef, np.float64)).to(eng.device)
+      operands = dict(affine)
+      if targets is not None:
+        operands["targets_planes"] = planes_tgt
+        kw = dict(lat_weight=self._lat_weight(targets, eng.device), coef=state["coef"],
+                  channel_sums=channel_sums)
+      else:
+        seed = torch.empty([eng.n_out, eng.num_grid], dtype=torch.float32, device=eng.device)
+        seed.copy_(state["cot"][b])
+        operands["cotangent"] = seed
+        kw = {}
+      state["run"].element(b, 0, operands, planes_out=planes_out, **kw)
+
+    state["batch"] = dict(inputs.sizes).get("batch", 1)
+    out = self._call(inputs, template, forcings, norm=norm, targets=targets,
+                     predictions=predictions is not None, element=element)
+    if predictions is not None:
+      predictions["predictions"] = out
+    return state["run"]
+
+  def _cotangent_planes(self, cotangents, template: xs.Dataset, batch: int) -> torch.Tensor:
+    """[batch, n_out, Ng] float32 host planes of a cotangent Dataset shaped like the one-step
+    `template`, in the predictions' channel order."""
+    cotangents = xs.from_xarray(cotangents)
+    slabs = self._check_template(template, self._engine.n_out)
+    if set(cotangents.keys()) != set(template.keys()):
+      raise ValueError(f"cotangents have the variables {sorted(cotangents.keys())}, the predictions "
+                       f"{sorted(template.keys())}")
+    n_lat, n_lon = template.sizes["lat"], template.sizes["lon"]
+    sizes = {"batch": batch, "lat": n_lat, "lon": n_lon}
+    out = torch.empty([batch, self._engine.n_out, n_lat * n_lon], dtype=torch.float32)
+    for s in slabs:
+      v = cotangents.data_vars[s.name]
+      if tuple(v.shape) != tuple(template.data_vars[s.name].shape):
+        raise ValueError(f"cotangent {s.name} has shape {tuple(v.shape)}, the prediction "
+                         f"{tuple(template.data_vars[s.name].shape)}")
+      src = model_utils.variable_to_planes(v.transpose(*template.data_vars[s.name].dims), sizes)
+      out[:, s.start:s.start + s.count] = torch.as_tensor(
+          np.asarray(src, np.float32)).reshape(batch, s.count, n_lat * n_lon)
+    return out
+
+  def _input_grads(self, stash: "StepStash", plan, norm: Optional[FusedNormalization],
+                   inputs: xs.Dataset, forcings: xs.Dataset, *, lat_weight=None, coef=None,
+                   cotangents=None):
+    """Gradients with respect to the inputs and forcings of the steps `stash` holds (several target
+    times): for every batch element, last step first, the step's planes are uploaded again, packed
+    and differentiated by Engine.input_grads_element with the all-channel feedback `plan` of the
+    following step.  The seed is the loss (lat_weight, coef; the stash holds the target planes) or,
+    with `cotangents` (per step [batch, n_out, Ng] host planes), J = sum cotangents * predictions.
+    Returns (input_grads, forcing_grads) Datasets shaped like `inputs` and `forcings`."""
+    run = _InputGradRun(self, plan, norm, inputs, forcings, len(stash.steps), stash.batch,
+                        release_staging=True)
+    eng = self._engine
+    dev = eng.device
+    coef_dev = None if coef is None else torch.as_tensor(np.asarray(coef, np.float64)).to(dev)
+    compute = torch.cuda.current_stream(dev)
+    for b in range(run.batch):
+      for t in range(run.num_steps - 1, -1, -1):
+        saved, done = stash.steps[t]
+        compute.wait_event(done)
+        # The step's planes and seed live in `operands` only: the engine drops them after the seed,
+        # so the backward pass reuses their 2.9 GB (0.25 degree).
+        operands = {"planes": torch.empty([eng.c_in, eng.num_grid], dtype=torch.float32, device=dev)}
+        operands["planes"].copy_(saved[0][b], non_blocking=True)
+        if norm is None:
+          eng.pack_inputs(operands.pop("planes"))
+        else:
+          eng.pack_inputs(operands["planes"], mean=norm.in_mean, scale=norm.in_scale)
+          operands.update(scale=norm.out_scale, offset=norm.out_offset,
+                          add_planes=operands.pop("planes"), add_plane_index=norm.add_plane_index)
+        seed = torch.empty([eng.n_out, eng.num_grid], dtype=torch.float32, device=dev)
+        if cotangents is None:
+          seed.copy_(saved[1][b], non_blocking=True)
+          operands["targets_planes"] = seed
+          kw = dict(lat_weight=lat_weight, coef=coef_dev)
+        else:
+          seed.copy_(cotangents[t][b])
+          operands["cotangent"] = seed
+          kw = {}
+        del seed
+        run.element(b, t, operands, **kw)
+    return run.finish()
+
   def _export_grads(self):
     """The engine's accumulated gradients as host numpy dicts, or, with a _grad_sink, whatever the
     sink returns after taking them on the device."""
@@ -295,6 +456,24 @@ class GraphCast(Predictor):
     """Keeps the input and target planes of the last `_call` (with targets) in pinned host memory."""
     stash.save(self._planes_in, self._planes_tgt)
 
+  def _release_staging(self) -> None:
+    """Before a backward pass that reads its steps from a StepStash: the rollout's staging buffers are
+    not needed any more, their memory goes to the backward pass."""
+    self._planes_bufs, self._target_bufs, self._buf_free = [None, None], [None, None], [None, None]
+    self._planes_in = self._planes_tgt = None
+    # Return the rollout's cached blocks to the driver, so that the backward pass allocates from an
+    # unfragmented pool: at 0.25 degree it peaks within a few GiB of an 80 GB card's capacity, and a
+    # second call would otherwise find its 1 GiB tables only in the gaps the first one left.
+    torch.cuda.empty_cache()
+
+  def _release_idle_staging(self) -> None:
+    """Inside a `_call`: drops the staging slot the call does not use (the one the next call would
+    stage into), for a backward pass that runs inside the call.  Its blocks stay in the allocator's
+    cache, where the backward pass's rows of the same size reuse them: emptying the cache here would
+    cost 0.5 s at 0.25 degree."""
+    idle = self._call_index % 2
+    self._planes_bufs[idle] = self._target_bufs[idle] = self._buf_free[idle] = None
+
   def _bptt_grads(self, stash: "StepStash", plan, norm: Optional[FusedNormalization],
                   lat_weight: torch.Tensor, coef: np.ndarray):
     """Parameter gradients of the multi-step loss whose steps `stash` holds (backprop through time,
@@ -306,13 +485,7 @@ class GraphCast(Predictor):
     eng.grads_begin()
     fb = eng.feedback(plan, None if norm is None else norm.add_plane_index,
                       None if norm is None else norm.in_scale)
-    # The rollout's staging buffers are not needed any more: their memory goes to the backward pass.
-    self._planes_bufs, self._target_bufs, self._buf_free = [None, None], [None, None], [None, None]
-    self._planes_in = self._planes_tgt = None
-    # Return the rollout's cached blocks to the driver, so that the backward pass allocates from an
-    # unfragmented pool: at 0.25 degree it peaks within a few GiB of an 80 GB card's capacity, and a
-    # second call would otherwise find its 1 GiB tables only in the gaps the first one left.
-    torch.cuda.empty_cache()
+    self._release_staging()
     planes = torch.empty([eng.c_in, eng.num_grid], dtype=torch.float32, device=dev)
     tgt = torch.empty([eng.n_out, eng.num_grid], dtype=torch.float32, device=dev)
     scratch = torch.empty([eng.n_out], dtype=torch.float64, device=dev)
@@ -380,13 +553,16 @@ class GraphCast(Predictor):
 
   def _call(self, inputs, targets_template, forcings, norm: Optional[FusedNormalization],
             targets: Optional[xs.Dataset] = None, predictions: bool = True,
-            grad_coef: Optional[np.ndarray] = None):
+            grad_coef: Optional[np.ndarray] = None, element=None):
     """The step for every batch element.  With `targets` (shaped like the template, usually the
     same Dataset) the outputs go through gcb_output_loss instead of the plain unpack: the loss sums
     land in a new [batch, n_out] fp64 device tensor, self._channel_sums, and the predictions are
     returned only when `predictions` is set (else None).  With `grad_coef` ([n_out] coefficients
     2 kappa / batch of the loss derivative) every element also runs the backward pass, which
-    accumulates the parameter gradients in the engine (Engine.loss_and_grads_element)."""
+    accumulates the parameter gradients in the engine (Engine.loss_and_grads_element).  With
+    `element`, element(b, planes_in[b], target planes or None, prediction planes or None, channel sums
+    or None, affine keywords) replaces the step of every batch element after its inputs are packed
+    (the input gradients of one target time)."""
     inputs = xs.from_xarray(inputs)
     forcings = xs.from_xarray(forcings)
     targets_template = xs.from_xarray(targets_template)
@@ -466,6 +642,18 @@ class GraphCast(Predictor):
       planes_out = torch.empty([batch, eng.n_out, eng.num_grid], dtype=torch.float32,
                                device=eng.device)
     for b in range(batch):
+      if element is not None:
+        if norm is None:
+          eng.pack_inputs(planes_in[b])
+        else:
+          eng.pack_inputs(planes_in[b], mean=norm.in_mean, scale=norm.in_scale)
+        affine = {} if norm is None else dict(
+            scale=norm.out_scale, offset=norm.out_offset, add_planes=planes_in[b],
+            add_plane_index=norm.add_plane_index)
+        element(b, planes_in[b], None if targets is None else planes_tgt[b],
+                None if planes_out is None else planes_out[b],
+                None if targets is None else channel_sums[b], affine)
+        continue
       if targets is not None:
         affine = {} if norm is None else dict(
             scale=norm.out_scale, offset=norm.out_offset, add_planes=planes_in[b],
@@ -579,6 +767,80 @@ def init_params(model_config: ModelConfig, task_config: TaskConfig, c_in: int,
   add(g, "processor_nodes_0_", "mesh_nodes", D, D)
   add(g, "decoder_nodes_", "grid_nodes", D, n_out, layer_norm=False)
   return params
+
+
+class _InputGradRun:
+  """The backward pass of one input-gradient call (GraphCast._input_grads / _one_step_input_grads):
+  the all-channel feedback of `plan`, and the per-variable results.  release_staging: the steps come
+  from a StepStash and every staging buffer goes; else the backward pass runs inside `_call`, which
+  keeps the slot it staged into.  After step t of batch element b
+  (element(b, t, ...)) the rows of its forcings slab, and after step 0 those of the inputs, are
+  reduced on the device (gcb_broadcast_grad_sum: the transpose of the broadcast over lat / lon,
+  batch-free variables summed over the batch in order) before the previous step consumes `a`.
+  Batched inputs are reduced into a buffer allocated after the element's backward pass and copied
+  without a synchronisation into pinned host memory (torch's caching host allocator: allocated on the
+  first call, reused after), so that the 0.25 degree inputs' 1.9 GB never coexist with a backward pass
+  and cross PCIe at full speed; finish() synchronises once.  The returned arrays are views of it."""
+
+  def __init__(self, model: GraphCast, plan, norm: Optional[FusedNormalization], inputs: xs.Dataset,
+               forcings: xs.Dataset, num_steps: int, batch: int, release_staging: bool):
+    eng = self.eng = model.engine
+    eng.input_grads_begin()
+    self.fb = eng.feedback(plan, None if norm is None else norm.add_plane_index,
+                           None if norm is None else norm.in_scale)
+    if release_staging:
+      model._release_staging()
+    else:
+      model._release_idle_staging()
+    self.inputs, self.forcings = inputs, forcings
+    self.num_steps, self.batch = num_steps, batch
+    self.n_lat, self.n_lon = inputs.sizes["lat"], inputs.sizes["lon"]
+    self.var_rows = feedback.variable_rows(inputs, forcings)
+    dev = eng.device
+    self.dev_bufs, self.host, self.rows = {}, {}, {}
+    for v in self.var_rows:
+      if v.forcing or not v.batched:
+        shape = ([batch] if v.batched else []) + ([num_steps] if v.timed else []) + [v.count, self._width(v)]
+        self.dev_bufs[v.key] = torch.zeros(shape, dtype=torch.float32, device=dev)
+      else:
+        self.host[v.key] = torch.empty([batch, v.count, self._width(v)], dtype=torch.float32,
+                                       pin_memory=True)
+      self.rows[v.key] = torch.arange(v.start, v.start + v.count, dtype=torch.int32, device=dev)
+
+  def _width(self, v) -> int:
+    return (self.eng.num_grid, self.n_lon, 1)[v.mode]
+
+  def element(self, b: int, t: int, operands: dict, **kw) -> None:
+    """Step t of batch element b (t = num_steps - 1 first): Engine.input_grads_element, then the
+    reductions of the rows that are complete."""
+    if t == self.num_steps - 1:
+      self.fb.a = None
+    self.eng.input_grads_element(self.fb, operands, **kw)
+    for v in self.var_rows:
+      if v.forcing or t == 0:
+        self._reduce(v, b, t)
+    if t == 0:
+      self.fb.a = None
+
+  def _reduce(self, v, b: int, t: int) -> None:
+    eng, fb = self.eng, self.fb
+    if v.key in self.host:                 # a batched input
+      out = torch.empty([v.count, self._width(v)], dtype=torch.float32, device=eng.device)
+      eng.broadcast_grad_sum(fb.a, self.n_lat, self.rows[v.key], v.mode, out, False)
+      self.host[v.key][b].copy_(out, non_blocking=True)   # stream-ordered before out's reuse
+      return
+    out = self.dev_bufs[v.key][b] if v.batched else self.dev_bufs[v.key]
+    out = out[t] if v.timed else out
+    accumulate = (not v.batched and b > 0) or (v.forcing and not v.timed and t < self.num_steps - 1)
+    eng.broadcast_grad_sum(fb.a, self.n_lat, self.rows[v.key], v.mode, out, accumulate)
+
+  def finish(self):
+    """(input_grads, forcing_grads) Datasets shaped like the inputs and forcings."""
+    grads = {key: buf.cpu().numpy() for key, buf in self.dev_bufs.items()}   # synchronises
+    torch.cuda.current_stream(self.eng.device).synchronize()
+    grads.update({key: t.numpy() for key, t in self.host.items()})
+    return feedback.grads_to_datasets(self.var_rows, grads, self.inputs, self.forcings, self.n_lat,
+                                      self.n_lon)
 
 
 class StepStash:

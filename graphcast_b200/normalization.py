@@ -246,6 +246,30 @@ class InputsAndResiduals(graphcast.Predictor):
     consts = self._fused_constants(inputs, targets, forcings, torch.device(device))
     return self._predictor._loss_and_grads(inputs, targets, forcings, norm=consts)
 
+  def _fused_for(self, inputs, targets, forcings, what: str):
+    if not self._fuses():
+      raise NotImplementedError(f"{what} need a GraphCast predictor directly inside "
+                                "InputsAndResiduals (the fused normalisation)")
+    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
+    targets = xs.from_xarray(targets)
+    device = self._predictor._device or f"cuda:{torch.cuda.current_device()}"
+    return inputs, targets, forcings, self._fused_constants(inputs, targets, forcings,
+                                                            torch.device(device))
+
+  def loss_and_input_grads(self, inputs, targets, forcings, **kwargs):
+    """(loss, diagnostics, input_grads, forcing_grads) of `loss` (GraphCast.loss_and_input_grads):
+    the gradients are in the physical units of the inputs and forcings, through the normalisation of
+    the inputs, the residual add and the target normalisation.  GraphCast only."""
+    inputs, targets, forcings, consts = self._fused_for(inputs, targets, forcings, "input gradients")
+    return self._predictor._loss_and_input_grads(inputs, targets, forcings, norm=consts)
+
+  def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
+    """(predictions, input_grads, forcing_grads) of the un-normalised predictions of __call__
+    (GraphCast.input_vjp).  GraphCast only."""
+    inputs, targets_template, forcings, consts = self._fused_for(inputs, targets_template, forcings,
+                                                                 "input gradients")
+    return self._predictor._input_vjp(inputs, targets_template, forcings, cotangents, norm=consts)
+
   def loss(self, inputs, targets, forcings, **kwargs):
     """The loss computed on normalised inputs and targets (targets that are also inputs as
     normalised residuals against the last input frame)."""

@@ -317,6 +317,36 @@ int gcb_input_grad(const float* dx, int32_t ld_dx, int64_t n_nodes, int32_t n_ro
                    const int32_t* channel, const float* scale, float* a, int32_t accumulate,
                    void* stream);
 
+/* ---- input gradients of a vector-Jacobian product (GraphCast.input_vjp) ----------------------------
+ * The seed of J = sum over channels and nodes of cot * pred, pred = y * scale + (offset | add) the
+ * physical prediction: the row arguments of gcb_output_loss_grad_feedback, with the cotangent
+ * cot [n_out, n_nodes] (channel-major fp32) in place of the targets, latitude weights and coef.
+ *   d[c, node]     = cot[c, node] + a_next[dpred_row[c], node]   (second term when a_next != NULL and
+ *                                                                 dpred_row[c] >= 0; fp64)
+ *   g[node, c]     = (float)(scale[c] * d)                        (scale NULL = 1)
+ *   a_out[r, node] = c >= 0 ? (float)d[c, node] : 0, c = resid_channel[r]
+ *                  + a_next[carry_row[r], node]                   when carry_row[r] >= 0
+ * No y is read: J is linear in the prediction.  Deterministic, no atomics. */
+int gcb_output_cotangent_grad_feedback(int32_t n_out, int64_t n_nodes, const float* scale,
+                                       const float* cot, const float* a_next,
+                                       const int32_t* dpred_row, int32_t n_rows,
+                                       const int32_t* resid_channel, const int32_t* carry_row,
+                                       float* a_out, float* g, int32_t ld_g, void* stream);
+
+/* Transpose of the broadcast by which a variable lacking lat and / or lon fills its input planes:
+ * for i < n_rows, the plane a[rows[i]] ([n_lat, n_lon] of a row-major [*, n_lat * n_lon] fp32 array)
+ * reduced into row i of out,
+ *   GCB_BCAST_NONE     out [n_rows, n_lat * n_lon]  a copy
+ *   GCB_BCAST_LAT      out [n_rows, n_lon]          summed over lat
+ *   GCB_BCAST_LAT_LON  out [n_rows]                 summed over lat and lon
+ * with fp64 sums in a fixed order and one rounding per element; accumulate = 1 adds the sum to out
+ * (out = (float)((double)out + sum)), e.g. to sum a batch-free variable over the batch elements in
+ * order.  Deterministic, no atomics. */
+enum { GCB_BCAST_NONE = 0, GCB_BCAST_LAT = 1, GCB_BCAST_LAT_LON = 2 };
+int gcb_broadcast_grad_sum(const float* a, int32_t n_lat, int32_t n_lon, int32_t n_rows,
+                           const int32_t* rows, int32_t mode, float* out, int32_t accumulate,
+                           void* stream);
+
 /* Weight gradient of one hk.Linear (utils/legacy/deep_typed_graph_net.py:205-247):
  *   dw[0:k, 0:n] (+)= sum_{r < rows} X[r, 0:k]^T G[r, 0:n]          (dw dense, row stride n)
  * X is an fp32 table (x, ld_x; columns >= k_valid read as 0) or, when x_img != NULL, an operand image
@@ -590,7 +620,8 @@ typedef enum {
   GCB_KIND_WGRAD = 9,       /* gcb_weight_grad (both of its launches) */
   GCB_KIND_ROWWISE_BWD = 10 /* gcb_layernorm_backward, gcb_swish_backward, gcb_output_loss_grad,
                              * gcb_segment_sum_sorted, gcb_gather_add, gcb_swish_rows,
-                             * gcb_output_loss_grad_feedback, gcb_input_grad */
+                             * gcb_output_loss_grad_feedback, gcb_input_grad,
+                             * gcb_output_cotangent_grad_feedback, gcb_broadcast_grad_sum */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
 int gcb_profile_end(int32_t capacity, int32_t* kinds, float* ms, double* flops, double* bytes,
