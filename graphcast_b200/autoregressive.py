@@ -25,6 +25,9 @@ target time is supported.  The gradient reaches a step's inputs through the resi
 target normalisation of InputsAndResiduals, the frame shift and the grid embedder; see
 graphcast_b200/feedback.py and DESIGN.md section 3.5.
 
+`input_jvp` (the tangent-linear forecast, `jax.jvp` of the unroll) runs forward with the rollout: each
+step's tangent planes are fed on the device from the step before, so it needs no checkpointing.
+
 Not provided: input noise (a training-side feature)."""
 
 from __future__ import annotations
@@ -260,6 +263,49 @@ class Predictor(graphcast.Predictor):
     input_grads, forcing_grads = model._input_grads(stash, plan, first["norm"], inputs, forcings,
                                                     cotangents=cot)
     return predictions, input_grads, forcing_grads
+
+  def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
+                **kwargs):
+    """(predictions, prediction_tangents): `predictions` as __call__ returns them, their derivative
+    along the tangents of the inputs and of the forcings of every target time (GraphCast.input_jvp),
+    through the fed-back predictions and forcings.  One target time delegates to the inner predictor.
+    Several run forward with the rollout, step by step (no gradient_checkpointing needed, nothing kept
+    per step): each step's tangent planes are fed on the device from the step before, by the rollout's
+    channel map (feedback.FeedbackPlan.feed_index), its forcings slab from forcing_tangents."""
+    inputs, targets_template = xs.from_xarray(inputs), xs.from_xarray(targets_template)
+    forcings = xs.from_xarray(forcings)
+    if targets_template.sizes["time"] == 1:
+      return self._predictor.input_jvp(inputs, targets_template, forcings, input_tangents,
+                                       forcing_tangents, **kwargs)
+    parts = self._device_parts()
+    if parts is None:
+      raise NotImplementedError("input_jvp over several target times needs a GraphCast predictor, "
+                                "directly or inside InputsAndResiduals (the fused normalisation)")
+    self._validate(inputs, targets_template, forcings)
+    model, norm_of = parts
+    num_steps = targets_template.sizes["time"]
+    one = lambda ds: ds.isel(time=slice(0, 1))
+    run = graphcast._TangentRun(inputs, forcings, input_tangents, forcing_tangents, num_steps,
+                                feedback.FeedbackPlan(inputs, one(targets_template), one(forcings)))
+    tangents = []
+
+    def step(rng, inputs, targets_template, forcings):
+      norm = norm_of(inputs, targets_template, forcings)
+      predictions, step_tangents = model._input_jvp(inputs, targets_template, forcings, run, norm)
+      tangents.append(step_tangents)
+      return predictions
+
+    chunks = list(rollout.chunked_prediction_generator(
+        step, rng=None, inputs=inputs, targets_template=targets_template, num_steps_per_chunk=1,
+        forcings=forcings))
+    # the tangents of each step with the coordinates the rollout gives its predictions
+    timed = []
+    for chunk, step_tangents in zip(chunks, tangents):
+      ds = xs.Dataset(coords=chunk.coords)
+      for name in step_tangents.keys():
+        ds[name] = step_tangents.data_vars[name]
+      timed.append(ds)
+    return xs.concat_time(chunks), xs.concat_time(timed)
 
 
 def _mean_over_time(step_losses, step_diagnostics):

@@ -19,6 +19,10 @@ SURVEY.md appendix A:
   * inputs (grid features, mesh zeros + structural, edge features) are constants: their MLPs get dW,
     never dX.
 
+The tangent-linear model (input_jvp) walks the same graph in forward order with the same helpers
+(Backward.tangent): each stage of the stage-wise forward is followed by its tangent, every MLP's tangent
+formed at its recomputed h and z (mlp_jvp; gcb_layernorm_jvp for the LayerNorm).
+
 All arithmetic is in libgraphcast_b200.so; this module only sequences the launches and owns the
 buffers.  Allocation is lazy: nothing here exists until the first loss_and_grads call.
 """
@@ -112,6 +116,7 @@ class Backward:
                             m.num_grid),
     }
     self.iota = self._i32(np.arange(max(m.num_grid, m.num_mesh)))
+    self._edge_iota = None
     self.zero_bias = torch.zeros([D], dtype=torch.float32, device=dev)
     self.prec = _native.PRECISIONS[eng.precision]
     self.ws_rows = torch.empty([max(self.lib.gcb_rowwise_workspace_bytes(D), 16)], dtype=torch.uint8, device=dev)
@@ -543,6 +548,166 @@ class Backward:
     if self.param_grads:
       self.mlp_backward(mp["enc_mesh"], nm, [mesh_in], dvm0)
     return dx
+
+  # -- tangent-linear model (Engine.input_jvp_element) ------------------------------------------------
+  def w0_block(self, info: _MlpInfo, s: int) -> int:
+    """Address of the packed image of the 512-row block s of an MLP's first layer (the image is K-step
+    major, so a row block is a contiguous slice)."""
+    return info.w.w0_packed + s * self.lib.gcb_packed_weight_bytes(D, D)
+
+  def mlp_jvp(self, info: _MlpInfo, rows: int, segs, dsegs, *, pre=None, dpre=(), w0=None,
+              dw0=None, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Tangent of one MLP y = LN(swish(X W0 + b0) W1 + b1) at the recomputed forward (h, z as
+    mlp_backward forms them), along the layer-0 input tangents `dsegs` with the weight dw0 (default:
+    that of the primal, w0) and the pre-gathered addends `dpre`; with no dsegs the addends alone are the
+    pre-activation tangent.  Returns residual + dy (LayerNorm MLPs) or dy [rows, n1] (the decoder)."""
+    w = info.w
+    w0 = w0 or w.w0_packed
+    if dsegs:
+      dh = self.empty(rows)
+      self.layer(rows, dsegs, dw0 or w0, self.zero_bias, out_y=dh, pre=list(dpre) or None)
+    else:
+      dh = None
+      for table, idx in dpre:
+        dh = self.gather_add(table, idx, rows, dh)
+    h = self.empty(rows)
+    self.layer(rows, segs, w0, w.b0, _native.ACT_NONE, out_y=h, pre=pre)
+    ws = self.ws_rows
+    da = self.empty(rows)                    # swish'(h) dh: the Jacobian of swish is diagonal
+    _native.check(self.lib.gcb_swish_backward(
+        dh.data_ptr(), D, h.data_ptr(), D, rows, D, da.data_ptr(), D, ws.data_ptr(), ws.numel(),
+        self.sink["b0"].data_ptr(), 0, self._st()), "gcb_swish_backward")
+    del dh
+    if not info.ln:
+      dy = self.empty(rows, info.n1)
+      self.layer(rows, [self.tab(da)], w.w1_packed, self.zero_bias, out_y=dy, n=info.n1,
+                 n_valid=info.n1_valid)
+      return dy
+    a = self.empty(rows)
+    _native.check(self.lib.gcb_swish_rows(h.data_ptr(), D, rows, D, a.data_ptr(), D, self._st()),
+                  "gcb_swish_rows")
+    del h
+    z = self.empty(rows)
+    self.layer(rows, [self.tab(a)], w.w1_packed, w.b1, out_y=z)
+    del a
+    dz = self.empty(rows)
+    self.layer(rows, [self.tab(da)], w.w1_packed, self.zero_bias, out_y=dz)
+    del da
+    out = self.empty(rows)
+    _native.check(self.lib.gcb_layernorm_jvp(
+        z.data_ptr(), D, dz.data_ptr(), D, w.ln_scale, rows, D, self._ptr(residual), D,
+        out.data_ptr(), D, self._st()), "gcb_layernorm_jvp")
+    return out
+
+  @staticmethod
+  def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
+    return None if t is None else t.data_ptr()
+
+  def bipartite_jvp(self, name: str, info: _MlpInfo, enc: _MlpInfo, feat_t: torch.Tensor,
+                    snd: torch.Tensor, rcv: torch.Tensor, v_s, n_s: int, v_r, n_r: int,
+                    dv_s: torch.Tensor, dv_r: Optional[torch.Tensor]) -> torch.Tensor:
+    """Tangent of the receiver sums of a grid2mesh / mesh2grid edge MLP m = MLP([e | v_s[snd] |
+    v_r[rcv]]) with e = MLP(edge features) (no tangent), chunk by chunk (self.chunks): dagg [n_r, 512],
+    from the sender and (when dv_r is given) receiver node tangents."""
+    sp = info.split
+    ps = self.projection(n_s, v_s, sp.ws_packed)
+    pr = self.projection(n_r, v_r, sp.wr_packed)
+    dps = self.projection(n_s, self.tab(dv_s), sp.ws_packed)
+    dpr = None if dv_r is None else self.projection(n_r, self.tab(dv_r), sp.wr_packed)
+    dagg = self.empty(n_r)
+    for r0, r1, g0, g1, rp, heavy, n_heavy, _ in self.chunks[name]:
+      n = r1 - r0
+      f = self.tab(feat_t[r0:r1], 16, 4, 4)                 # 16-byte rows: the view stays aligned
+      snd_c, rcv_c = snd[r0:r1].clone(), rcv[r0:r1].clone()  # index arrays from an aligned base
+      e = self.fwd_mlp(enc, n, [f])
+      dpre = [(dps, snd_c)] + ([] if dpr is None else [(dpr, rcv_c)])
+      dm = self.mlp_jvp(info, n, [self.tab(e)], [], pre=[(ps, snd_c), (pr, rcv_c)], dpre=dpre,
+                        w0=sp.we_packed)
+      del e
+      _native.check(self.lib.gcb_segment_sum_heavy(
+          dm.data_ptr(), D, rp.data_ptr(), g1 - g0, heavy.data_ptr() if n_heavy else None, n_heavy,
+          dagg[g0:g1].data_ptr(), D, D, self._st()), "gcb_segment_sum_heavy")
+      del dm
+    return dagg
+
+  def tangent(self, grid_in_img: torch.Tensor, dgrid_in_img: torch.Tensor) -> torch.Tensor:
+    """One step stage by stage (Engine.run_stage, from the packed inputs grid_in_img) and, interleaved
+    with it, its tangent along the packed input tangent dgrid_in_img (an operand image of [Ng,
+    c_in_pad] whose structural columns are zero): returns dy [Ng, 256], the tangent of the decoder
+    output (n_out valid columns).  Each stage's tangent runs right after the stage, from the engine's
+    buffers and copies of that stage's inputs alone; the tangent state is fp32 tables.  Exactly zero
+    tangents are not formed: the mesh-node encoder, the three edge embedders, e_0 of the processor,
+    and the v_m0 and edge terms of the grid2mesh edge MLP."""
+    eng, m = self.eng, self.m
+    ng, nm = m.num_grid, m.num_mesh
+    K = eng.msg_steps
+    mp = self.mlps
+    img, tab = self.img, self.tab
+    cin = eng.c_in_pad
+
+    # ---- encoder: vg0 = MLP(grid_in);  m1 = MLP([e1 | vg0[snd] | vm0[rcv]]);  agg1 = sum m1;
+    #      vm1 = vm0 + MLP([vm0 | agg1]);  vg1 = vg0 + MLP([vg0]).  agg1 is read from the engine.
+    eng.run_stage("encode", grid_in=grid_in_img)
+    grid_in = img(grid_in_img, cin)
+    info = mp["enc_grid"]
+    dvg0 = self.mlp_jvp(info, ng, [grid_in], [img(dgrid_in_img, cin)])
+    vg0 = self.fwd_mlp(info, ng, [grid_in])
+    vm0 = self.fwd_mlp(mp["enc_mesh"], nm, [img(eng.mesh_in_img, cin)])
+    dagg = self.bipartite_jvp("g2m", mp["proc_e_g2m"], mp["enc_e_g2m"], eng.g2m_feat, eng.g2m_snd,
+                              eng.g2m_rcv, tab(vg0), ng, tab(vm0), nm, dvg0, None)
+    info = mp["proc_n_mesh_g2m"]                 # vm0 has no tangent: block 1 of W0 alone
+    dv = self.mlp_jvp(info, nm, [tab(vm0), img(eng.mesh_agg_img)], [tab(dagg)],
+                      dw0=self.w0_block(info, 1))
+    del dagg, vm0
+    dvg = self.mlp_jvp(mp["proc_n_grid_g2m"], ng, [tab(vg0)], [tab(dvg0)], residual=dvg0)
+    del dvg0, vg0
+
+    # ---- processor:  m = MLP([e | v[snd] | v[rcv]]);  v' = v + MLP([v | agg]);  e' = e + m.
+    #      v_k and e_k are copied before step k, agg_k read after it.
+    eng.run_stage("process_embed")
+    de = None
+    for k in range(K):
+      v_k = eng.mesh_lat_img.clone()
+      if k == 0:
+        e_k = tab(self.fwd_mlp(mp["enc_e_mesh"], m.e_mesh, [tab(eng.mesh_feat, 16, 4, 4)]))
+      else:
+        e_k = img(eng.mesh_edge_img.clone())
+      eng.run_stage("process_step", k)
+      nfo, efo = self.proc_n[k], self.proc_e[k]
+      sp = efo.split
+      ps, pr = self.projection(nm, img(v_k), sp.ws_packed), self.projection(nm, img(v_k), sp.wr_packed)
+      dps = self.projection(nm, tab(dv), sp.ws_packed)
+      dpr = self.projection(nm, tab(dv), sp.wr_packed)
+      dpre = [(dps, eng.mesh_snd), (dpr, eng.mesh_rcv)]
+      dm = self.mlp_jvp(efo, m.e_mesh, [e_k], [] if de is None else [tab(de)],
+                        pre=[(ps, eng.mesh_snd), (pr, eng.mesh_rcv)], dpre=dpre, w0=sp.we_packed)
+      del ps, pr, dps, dpr, e_k
+      dagg = self.seg_sum_receiver(dm, eng.mesh_row_ptr, nm)
+      if k < K - 1:                              # the last step's edge update is never read
+        de = dm if de is None else self.gather_add(dm, self.edge_iota(), m.e_mesh, de)
+      del dm
+      dv = self.mlp_jvp(nfo, nm, [img(v_k), img(eng.mesh_agg_img)], [tab(dv), tab(dagg)],
+                        residual=dv)
+      del dagg, v_k
+    del de
+
+    # ---- decoder: m3 = MLP([e3 | v[snd] | vg1[rcv]]);  agg3 = fan-in-3 sum;
+    #      vg2 = vg1 + MLP([vg1 | agg3]);  out = MLP(vg2).  agg3 and vg2 are read from the engine.
+    v_k, vg1 = eng.mesh_lat_img.clone(), eng.grid_lat_img.clone()
+    eng.run_stage("decode", grid_in=grid_in_img)
+    dagg = self.bipartite_jvp("m2g", mp["proc_e_m2g"], mp["enc_e_m2g"], eng.m2g_feat, eng.m2g_snd,
+                              eng.m2g_rcv, img(v_k), nm, img(vg1), ng, dv, dvg)
+    del v_k, dv
+    dvg = self.mlp_jvp(mp["proc_n_grid_m2g"], ng, [img(vg1), img(eng.grid_agg_img)],
+                       [tab(dvg), tab(dagg)], residual=dvg)
+    del vg1, dagg
+    return self.mlp_jvp(mp["dec_grid"], ng, [img(eng.grid_lat_img)], [tab(dvg)])
+
+  def edge_iota(self) -> torch.Tensor:
+    """0..E_mesh-1 (the identity gather of the edge-tangent update e' = e + m), made on first use."""
+    if self._edge_iota is None:
+      self._edge_iota = self._i32(np.arange(self.m.e_mesh))
+    return self._edge_iota
 
   # -- result ----------------------------------------------------------------------------------------
   def _accumulators(self) -> Dict[str, Dict[str, torch.Tensor]]:

@@ -71,3 +71,8 @@ class Bfloat16Cast(graphcast.Predictor):
 
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
     return self._predictor.input_vjp(inputs, targets_template, forcings, cotangents, **kwargs)
+
+  def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
+                **kwargs):
+    return self._predictor.input_jvp(inputs, targets_template, forcings, input_tangents,
+                                     forcing_tangents, **kwargs)

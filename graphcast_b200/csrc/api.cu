@@ -1045,6 +1045,23 @@ int gcb_swish_backward(const float* da, int32_t ld_da, const float* h, int32_t l
                         workspace_bytes, sums, 1, accumulate, stream);
 }
 
+int gcb_layernorm_jvp(const float* z, int32_t ld_z, const float* dz, int32_t ld_dz, const float* scale,
+                      int64_t rows, int32_t n, const float* residual, int32_t ld_res, float* out,
+                      int32_t ld_out, void* stream) {
+  GCB_CHECK_ARG(z && dz && scale && out, "null pointer");
+  GCB_CHECK_ARG(n == 512, "the LayerNorm tangent needs n = 512");
+  GCB_CHECK_ARG(rows >= 0 && ld_z >= n && ld_dz >= n && ld_out >= n && (!residual || ld_res >= n),
+                "rows < 0 or leading dimension < n");
+  if (rows == 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * static_cast<double>(rows) * n * (3.0 + (residual ? 1.0 : 0.0)));
+  gcb::layernorm_jvp_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, st>>>(
+      z, ld_z, dz, ld_dz, scale, rows, residual, ld_res, out, ld_out);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
 int gcb_segment_sum_sorted(const float* msg, int32_t ld_msg, const int32_t* order,
                            const int32_t* ptr, int32_t num_nodes, const int32_t* heavy,
                            int32_t num_heavy, float* out, int32_t ld_out, int32_t width, void* stream) {

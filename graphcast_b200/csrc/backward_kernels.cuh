@@ -202,6 +202,25 @@ slices_reduce_kernel(const float* __restrict__ partial, int slices, long long st
 constexpr int kRowSlices = 256;
 enum RowMode { kRowLayerNorm = 0, kRowCopy = 1, kRowSwish = 2 };
 
+// The LayerNorm statistics (eps 1e-5) of one n = 32 * kCols row held by a warp, lane owning v[j] =
+// column lane + 32 j: its mean and 1 / sqrt(var + eps), with fixed butterfly sums.
+template <int kCols>
+__device__ __forceinline__ void ln_row_stats(const float* v, float& mean, float& rstd) {
+  constexpr int n = kCols * 32;
+  mean = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) mean += v[j];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mean += __shfl_xor_sync(0xffffffffu, mean, o);
+  mean *= (1.0f / n);
+  float var = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) { const float t = v[j] - mean; var += t * t; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) var += __shfl_xor_sync(0xffffffffu, var, o);
+  rstd = rsqrtf(var * (1.0f / n) + 1e-5f);
+}
+
 template <int kMode, int kCols>   // kCols = n / 32 (8 or 16)
 __global__ void __launch_bounds__(256)
 rowwise_backward_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z, int ld_z,
@@ -227,18 +246,8 @@ rowwise_backward_kernel(const float* __restrict__ dy, int ld_dy, const float* __
     if (kMode == kRowLayerNorm) {
 #pragma unroll
       for (int j = 0; j < kCols; ++j) v[j] = z[r * ld_z + lane + 32 * j];
-      float mean = 0.f;
-#pragma unroll
-      for (int j = 0; j < kCols; ++j) mean += v[j];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) mean += __shfl_xor_sync(0xffffffffu, mean, o);
-      mean *= (1.0f / n);
-      float var = 0.f;
-#pragma unroll
-      for (int j = 0; j < kCols; ++j) { const float t = v[j] - mean; var += t * t; }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) var += __shfl_xor_sync(0xffffffffu, var, o);
-      const float rstd = rsqrtf(var * (1.0f / n) + 1e-5f);
+      float mean, rstd;
+      ln_row_stats<kCols>(v, mean, rstd);
       float mg = 0.f, mgz = 0.f;
 #pragma unroll
       for (int j = 0; j < kCols; ++j) {
@@ -290,6 +299,52 @@ rowwise_backward_kernel(const float* __restrict__ dy, int ld_dy, const float* __
       partial[(static_cast<long long>(blockIdx.x) * kSums + q) * n + c] = static_cast<float>(t);
     }
     __syncthreads();
+  }
+}
+
+// ---- tangent-linear model ------------------------------------------------------------------------
+// Tangent of hk.LayerNorm at the pre-LayerNorm z along dz, one warp per row of n = 512 (lane owns
+// columns lane + 32 j), 8 rows per block:
+//   out = (residual ? residual : 0) + scale * (rstd * (dz - mean(dz) - zhat * mean(zhat * dz)))
+// zhat = (z - mu) * rstd, mu and rstd from ln_row_stats as rowwise_backward_kernel forms them.  The
+// Jacobian is symmetric, so with unit scale this is that kernel's dz for dy = dz.  Row-wise: no column
+// sums, no atomics.
+__global__ void __launch_bounds__(256)
+layernorm_jvp_kernel(const float* __restrict__ z, int ld_z, const float* __restrict__ dz, int ld_dz,
+                     const float* __restrict__ scale, long long rows, const float* __restrict__ residual,
+                     int ld_res, float* __restrict__ out, int ld_out) {
+  constexpr int kCols = 16, n = 512;
+  const int lane = threadIdx.x & 31;
+  const long long r = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  if (r >= rows) return;
+  float v[kCols], d[kCols];
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) {
+    v[j] = z[r * ld_z + lane + 32 * j];
+    d[j] = dz[r * ld_dz + lane + 32 * j];
+  }
+  float mean, rstd;
+  ln_row_stats<kCols>(v, mean, rstd);
+  float md = 0.f, mdz = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) {
+    v[j] = (v[j] - mean) * rstd;                       // z-hat
+    md += d[j];
+    mdz += d[j] * v[j];
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    md += __shfl_xor_sync(0xffffffffu, md, o);
+    mdz += __shfl_xor_sync(0xffffffffu, mdz, o);
+  }
+  md *= (1.0f / n);
+  mdz *= (1.0f / n);
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) {
+    const int c = lane + 32 * j;
+    float o = scale[c] * (rstd * (d[j] - md - v[j] * mdz));
+    if (residual) o = residual[r * ld_res + c] + o;
+    out[r * ld_out + c] = o;
   }
 }
 

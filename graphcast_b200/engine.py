@@ -801,6 +801,46 @@ class Engine:
           dx.data_ptr(), dx.shape[1], self.num_grid, fb.n_rows, fb.rows.data_ptr(),
           self._ptr(fb.in_scale), a_out.data_ptr(), 1, self._stream()), "gcb_input_grad")
 
+  # -- tangent-linear model (input_jvp) -----------------------------------------------------------------
+  def input_jvp_element(self, tangent_planes: torch.Tensor, tangent_out: torch.Tensor, *,
+                        in_scale: Optional[torch.Tensor] = None,
+                        planes_out: Optional[torch.Tensor] = None,
+                        grid_in: Optional[torch.Tensor] = None, **affine) -> None:
+    """One step of one batch element of the tangent-linear forecast (call input_grads_begin() first):
+    the step stage by stage from `grid_in` (default: the packed grid_in_img) interleaved with its
+    tangent (Backward.tangent) along tangent_planes [c_in, Ng], the tangent of this step's input planes
+    in physical units.  They are packed as pack_inputs packs the planes, without the mean (in_scale:
+    the input normalisation's scale) and with zero structural features.  tangent_out [n_out, Ng]
+    receives the tangent of the physical predictions: the decoder tangent times affine["scale"] plus,
+    through the residual add, tangent_planes[affine["add_plane_index"]] (gcb_unpack_grid_outputs
+    without the offset).  With planes_out, the predictions as unpack_outputs gives them from the same
+    forward.  `affine`: the keywords of unpack_outputs (scale, offset, add_planes, add_plane_index)."""
+    if self._backward is None:
+      raise RuntimeError("call input_grads_begin() first")
+    for name, t, rows in (("tangent_planes", tangent_planes, self.c_in),
+                          ("tangent_out", tangent_out, self.n_out)):
+      if (tuple(t.shape) != (rows, self.num_grid) or t.dtype != torch.float32
+          or not t.is_contiguous() or t.device != self.device):
+        raise ValueError(f"{name} must be a contiguous float32 [{rows}, {self.num_grid}] tensor on "
+                         f"{self.device}")
+    grid_in = self.grid_in_img if grid_in is None else grid_in
+    dgrid_in = self._image(self.num_grid, self.c_in_pad)
+    no_static = torch.zeros([self.num_grid, 3], dtype=torch.float32, device=self.device)
+    add_index = affine.get("add_plane_index")
+    with self._on_device():
+      _native.check(self._lib.gcb_pack_grid_image(
+          tangent_planes.data_ptr(), self.c_in, self.num_grid, None, self._ptr(in_scale),
+          no_static.data_ptr(), 3, self.c_in_pad, dgrid_in.data_ptr(), self._stream()),
+          "gcb_pack_grid_image")
+      dy = self._backward.tangent(grid_in, dgrid_in)
+      del dgrid_in
+      if planes_out is not None:
+        self.unpack_outputs(planes_out, **affine)
+      _native.check(self._lib.gcb_unpack_grid_outputs(
+          dy.data_ptr(), dy.shape[1], self.n_out, self.num_grid, self._ptr(affine.get("scale")), None,
+          None if add_index is None else tangent_planes.data_ptr(), self._ptr(add_index),
+          tangent_out.data_ptr(), self._stream()), "gcb_unpack_grid_outputs")
+
   def broadcast_grad_sum(self, a: torch.Tensor, n_lat: int, rows: torch.Tensor, mode: int,
                          out: torch.Tensor, accumulate: bool) -> None:
     """gcb_broadcast_grad_sum on the current stream: the planes a[rows] ([*, Ng] fp32) reduced into

@@ -155,6 +155,16 @@ class FeedbackPlan:
     out[self.dpred_row[c]] = c
     return out
 
+  def feed_index(self) -> np.ndarray:
+    """[n_in] int32: the row of [this step's planes (c_in rows) | its predictions (n_out rows)] that
+    becomes input channel j of the next step (next_from_input, else c_in + next_from_pred).  The
+    forcings slab, channels n_in.., is the next target time's, given.  The gather index of the tangent
+    feed between the steps of input_jvp."""
+    src, pred = self.next_from_input[:self.n_in], self.next_from_pred[:self.n_in]
+    if not np.all((src >= 0) | (pred >= 0)):
+      raise ValueError("an input channel is neither carried nor predicted")
+    return np.where(src >= 0, src, self.c_in + pred).astype(np.int32)
+
   def next_planes(self, planes: np.ndarray, predictions: np.ndarray,
                   next_forcings: np.ndarray) -> np.ndarray:
     """The next step's planes [c_in, ...] from this step's planes [c_in, ...], its predictions
@@ -227,6 +237,40 @@ def variable_rows(inputs: xs.Dataset, forcings: xs.Dataset) -> list:
   f_slabs = model_utils.channel_layout(step, start=n_in)
   return ([VariableRows(s, inputs.data_vars[s.name], False) for s in in_slabs] +
           [VariableRows(s, forcings.data_vars[s.name], True) for s in f_slabs])
+
+
+def check_tangents(tangents: Optional[xs.Dataset], like: xs.Dataset, what: str) -> None:
+  """ValueError unless every variable of `tangents` (None: none) has a namesake in `like` with the
+  same dims, in any order, and the same sizes."""
+  if tangents is None:
+    return
+  for name in sorted(tangents.keys()):
+    if name not in like.data_vars:
+      raise ValueError(f"{what}: unknown variable {name!r}, expected one of {sorted(like.keys())}")
+    v, ref = tangents.data_vars[name], like.data_vars[name]
+    if set(v.dims) != set(ref.dims) or tuple(v.transpose(*ref.dims).shape) != tuple(ref.shape):
+      raise ValueError(f"{what}: {name} has dims {tuple(v.dims)} and shape {tuple(v.shape)}, the "
+                       f"variable {tuple(ref.dims)} and {tuple(ref.shape)}")
+
+
+def tangent_planes(tangents: Optional[xs.Dataset], like: xs.Dataset,
+                   sizes: dict) -> np.ndarray:
+  """[batch, channels, lat * lon] float32 planes of a tangent Dataset (check_tangents), packed exactly
+  as GraphCast stages `like`: channel_layout(like) order, model_utils.variable_to_planes broadcasting
+  a variable over the batch, lat and lon it lacks.  Variables `tangents` leaves out (all of them for
+  None) get zero planes."""
+  batch, n_lat, n_lon = sizes["batch"], sizes["lat"], sizes["lon"]
+  slabs = model_utils.channel_layout(like)
+  out = np.zeros([batch, sum(s.count for s in slabs), n_lat * n_lon], np.float32)
+  for s in slabs:
+    if tangents is None or s.name not in tangents.data_vars:
+      continue
+    v = tangents.data_vars[s.name].transpose(*like.data_vars[s.name].dims)
+    p = model_utils.variable_to_planes(v, sizes)
+    p = p.detach().cpu().numpy() if xs._is_torch(p) else np.asarray(p)
+    out[:, s.start:s.start + s.count] = np.broadcast_to(
+        p, (batch, s.count, n_lat, n_lon)).reshape(batch, s.count, n_lat * n_lon)
+  return out
 
 
 def grads_to_datasets(rows: list, grads: dict, inputs: xs.Dataset, forcings: xs.Dataset,

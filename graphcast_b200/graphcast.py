@@ -31,6 +31,7 @@ from typing import Any, Dict, List, Mapping, Optional, Tuple
 import numpy as np
 import torch
 
+from graphcast_b200 import _native
 from graphcast_b200 import engine as engine_lib
 from graphcast_b200 import feedback
 from graphcast_b200 import graph as graph_lib
@@ -116,6 +117,13 @@ class Predictor(abc.ABC):
     """Returns (predictions, input_grads, forcing_grads): the predictions of __call__ and the
     gradients of sum(cotangents * predictions) with respect to every variable of `inputs` and
     `forcings`; `cotangents` is shaped like `targets_template`."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement input gradients")
+
+  def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
+                **optional_kwargs):
+    """Returns (predictions, prediction_tangents): the predictions of __call__ and their derivative
+    along the tangents of the inputs and forcings (Datasets with some of their variables, each shaped
+    like its namesake; a variable left out is held fixed), shaped like the predictions."""
     raise NotImplementedError(f"{type(self).__name__} does not implement input gradients")
 
 
@@ -314,6 +322,51 @@ class GraphCast(Predictor):
     J = sum over variables, batch, time, level, lat and lon of cotangents * predictions, with
     `cotangents` a Dataset shaped like `targets_template`."""
     return self._input_vjp(inputs, targets_template, forcings, cotangents, norm=None)
+
+  def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
+                **unused_kwargs):
+    """(predictions, prediction_tangents) for one target time: `predictions` is what __call__ returns,
+    bit for bit; `prediction_tangents` (float32, shaped like it) is d(predictions)/d eps at eps = 0 for
+    the inputs + eps * input_tangents and forcings + eps * forcing_tangents, what jax.jvp of the
+    predictor gives.  The tangent Datasets hold variables of `inputs` / `forcings` with their dims and
+    shapes, in physical units; a variable left out (every forcing for forcing_tangents=None) is held
+    fixed.  An unknown variable or a wrong shape raises ValueError before anything runs.  The tangent
+    runs forward with the step, stage by stage (Backward.tangent), in the model's precision."""
+    run = self._one_step_tangents(inputs, targets_template, forcings, input_tangents,
+                                  forcing_tangents)
+    return self._input_jvp(inputs, targets_template, forcings, run, norm=None)
+
+  @staticmethod
+  def _one_step_tangents(inputs, targets_template, forcings, input_tangents,
+                         forcing_tangents) -> "_TangentRun":
+    """The checked and packed tangents of an input_jvp of one target time."""
+    if xs.from_xarray(targets_template).sizes.get("time", 1) != 1:
+      raise NotImplementedError("input_jvp of GraphCast covers one target time (several: "
+                                "autoregressive.Predictor)")
+    return _TangentRun(xs.from_xarray(inputs), xs.from_xarray(forcings), input_tangents,
+                       forcing_tangents, num_steps=1)
+
+  def _input_jvp(self, inputs, targets_template, forcings, run: "_TangentRun",
+                 norm: Optional[FusedNormalization]):
+    """input_jvp of one step, the tangent planes carried by `run` (from the step before, in a
+    rollout).  `_call` stages the planes once and, for every batch element, runs the stage-wise
+    forward and its tangent (Engine.input_jvp_element) in place of its step."""
+    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
+    targets_template = xs.from_xarray(targets_template)
+    state = {}
+
+    def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
+      eng = self._engine
+      if "out" not in state:
+        eng.input_grads_begin()
+        self._release_idle_staging()
+        state["out"] = torch.empty([run.batch, eng.n_out, eng.num_grid], dtype=torch.float32,
+                                   device=eng.device)
+      run.element(eng, b, state["out"][b], planes_out, norm, affine)
+
+    predictions = self._call(inputs, targets_template, forcings, norm=norm, element=element)
+    run.step += 1
+    return predictions, self._planes_to_dataset(state["out"], targets_template, run.n_lat, run.n_lon)
 
   def _loss_and_input_grads(self, inputs, targets, forcings, norm: Optional[FusedNormalization]):
     inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
@@ -841,6 +894,67 @@ class _InputGradRun:
     grads.update({key: t.numpy() for key, t in self.host.items()})
     return feedback.grads_to_datasets(self.var_rows, grads, self.inputs, self.forcings, self.n_lat,
                                       self.n_lon)
+
+
+class _TangentRun:
+  """The tangent planes of one input_jvp call (GraphCast._input_jvp, autoregressive.Predictor
+  .input_jvp).  The tangent Datasets are checked and packed into host planes on construction, before
+  anything runs on the device.  Per batch element a device buffer [c_in + n_out, Ng] holds the tangent
+  of the current step's input planes in its first c_in rows.  After a step that has a successor, the
+  prediction tangents are copied into its last n_out rows and the next step's first n_in rows are
+  gathered from the buffer by FeedbackPlan.feed_index (gcb_gather_rows: every such row is a copy of one
+  row of the two sources); the forcings slab comes from the forcing tangents of that target time.  The
+  tangent planes stay on the device from step to step, and nothing is kept per step."""
+
+  def __init__(self, inputs: xs.Dataset, forcings: xs.Dataset, input_tangents, forcing_tangents,
+               num_steps: int, plan=None):
+    input_tangents = None if input_tangents is None else xs.from_xarray(input_tangents)
+    forcing_tangents = None if forcing_tangents is None else xs.from_xarray(forcing_tangents)
+    feedback.check_tangents(input_tangents, inputs, "input_tangents")
+    feedback.check_tangents(forcing_tangents, forcings, "forcing_tangents")
+    self.batch = dict(inputs.sizes).get("batch", 1)
+    self.n_lat, self.n_lon = inputs.sizes["lat"], inputs.sizes["lon"]
+    self.sizes = {"batch": self.batch, "lat": self.n_lat, "lon": self.n_lon}
+    if num_steps > 1 and (self.n_lat * self.n_lon) % 4:
+      raise NotImplementedError("input_jvp over several target times needs a multiple of 4 grid "
+                                "nodes (the tangent feed gathers 16-byte rows)")
+    self.input_planes = torch.from_numpy(feedback.tangent_planes(input_tangents, inputs, self.sizes))
+    self.forcings, self.forcing_tangents = forcings, forcing_tangents
+    self.num_steps, self.step = num_steps, 0
+    self.feed = None if plan is None else torch.from_numpy(plan.feed_index())
+    self.carry = [None] * self.batch
+    self._slab = (-1, None)
+
+  def _forcing_planes(self, t: int) -> torch.Tensor:
+    """[batch, c_in - n_in, Ng] host tangent planes of the forcings of target time t."""
+    if self._slab[0] != t:
+      at = lambda ds: ds.isel(time=slice(t, t + 1)) if "time" in ds.sizes else ds
+      tangents = None if self.forcing_tangents is None else at(self.forcing_tangents)
+      self._slab = (t, torch.from_numpy(feedback.tangent_planes(tangents, at(self.forcings),
+                                                                self.sizes)))
+    return self._slab[1]
+
+  def element(self, eng, b: int, tangent_out: torch.Tensor, planes_out: Optional[torch.Tensor],
+              norm: Optional[FusedNormalization], affine: dict) -> None:
+    """This step of batch element b: Engine.input_jvp_element, then the feed of the next step."""
+    c_in, n_in, ng = eng.c_in, self.input_planes.shape[1], eng.num_grid
+    buf, self.carry[b] = self.carry[b], None
+    if buf is None:
+      buf = torch.empty([c_in + eng.n_out, ng], dtype=torch.float32, device=eng.device)
+      buf[:n_in].copy_(self.input_planes[b])
+    buf[n_in:c_in].copy_(self._forcing_planes(self.step)[b])
+    eng.input_jvp_element(buf[:c_in], tangent_out, in_scale=None if norm is None else norm.in_scale,
+                          planes_out=planes_out, **affine)
+    if self.step + 1 < self.num_steps:
+      if self.feed.device != eng.device:
+        self.feed = self.feed.to(eng.device)
+      buf[c_in:].copy_(tangent_out)
+      nxt = torch.empty_like(buf)
+      with eng._on_device():
+        _native.check(eng._lib.gcb_gather_rows(buf.data_ptr(), ng, self.feed.data_ptr(), n_in,
+                                               nxt.data_ptr(), ng, ng, eng._stream()),
+                      "gcb_gather_rows")
+      self.carry[b] = nxt
 
 
 class StepStash:

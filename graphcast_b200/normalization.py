@@ -270,6 +270,17 @@ class InputsAndResiduals(graphcast.Predictor):
                                                                  "input gradients")
     return self._predictor._input_vjp(inputs, targets_template, forcings, cotangents, norm=consts)
 
+  def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
+                **kwargs):
+    """(predictions, prediction_tangents) of the un-normalised predictions of __call__
+    (GraphCast.input_jvp): the tangents are in physical units, through the normalisation of the inputs
+    and the residual add.  GraphCast only."""
+    run = graphcast.GraphCast._one_step_tangents(inputs, targets_template, forcings, input_tangents,
+                                                 forcing_tangents)
+    inputs, targets_template, forcings, consts = self._fused_for(inputs, targets_template, forcings,
+                                                                 "input gradients")
+    return self._predictor._input_jvp(inputs, targets_template, forcings, run, norm=consts)
+
   def loss(self, inputs, targets, forcings, **kwargs):
     """The loss computed on normalised inputs and targets (targets that are also inputs as
     normalised residuals against the last input frame)."""

@@ -378,6 +378,17 @@ int gcb_swish_backward(const float* da, int32_t ld_da, const float* h, int32_t l
                        int32_t n, float* dh, int32_t ld_dh, void* workspace, int64_t workspace_bytes,
                        float* dbias, int32_t accumulate, void* stream);
 
+/* Tangent-linear model (GraphCast.input_jvp): the forward-mode derivative of hk.LayerNorm (eps 1e-5)
+ * at the pre-LayerNorm z [rows, 512] along dz, n = 512:
+ *   out = (residual ? residual : 0) + scale * rstd * (dz - mean(dz) - zhat * mean(zhat * dz))
+ * zhat = (z - mu) * rstd, with mu and rstd recomputed from z exactly as gcb_layernorm_backward forms
+ * them (the Jacobian is symmetric: with unit scale, out is gcb_layernorm_backward's dz for dy = dz).
+ * `residual` (may be NULL) is the tangent of the residual stream the MLP output is added to.  Row-wise,
+ * no column sums, no atomics, deterministic; out may not alias z, dz or residual. */
+int gcb_layernorm_jvp(const float* z, int32_t ld_z, const float* dz, int32_t ld_dz, const float* scale,
+                      int64_t rows, int32_t n, const float* residual, int32_t ld_res, float* out,
+                      int32_t ld_out, void* stream);
+
 /* Backward of a gather v[senders] (jax_gather, utils/typed_graph_net.py:124-125,431-445):
  *   out[i, 0:512] = sum_{j in [ptr[i], ptr[i+1])} msg[order[j], 0:512]
  * (order / ptr: the sender CSR of an edge set, host-built), summed in j order; the rows listed in
@@ -621,7 +632,8 @@ typedef enum {
   GCB_KIND_ROWWISE_BWD = 10 /* gcb_layernorm_backward, gcb_swish_backward, gcb_output_loss_grad,
                              * gcb_segment_sum_sorted, gcb_gather_add, gcb_swish_rows,
                              * gcb_output_loss_grad_feedback, gcb_input_grad,
-                             * gcb_output_cotangent_grad_feedback, gcb_broadcast_grad_sum */
+                             * gcb_output_cotangent_grad_feedback, gcb_broadcast_grad_sum,
+                             * gcb_layernorm_jvp */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
 int gcb_profile_end(int32_t capacity, int32_t* kinds, float* ms, double* flops, double* bytes,
