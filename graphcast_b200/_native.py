@@ -50,6 +50,14 @@ class MlpSplit(C.Structure):
               ("wr_packed", _fp), ("wr_f32", _fp)]
 
 
+class NoiseSegment(C.Structure):
+  _fields_ = [("src", _fp), ("dst", _fp), ("n", C.c_int64), ("offset", C.c_int64),
+              ("stream", C.c_uint32)]
+
+
+GCB_NOISE_MAX_SEGMENTS = 64
+
+
 class Mlp(C.Structure):
   _fields_ = [("w0_packed", _fp), ("w0_f32", _fp), ("b0", _fp),
               ("w1_packed", _fp), ("w1_f32", _fp), ("b1", _fp),
@@ -129,6 +137,8 @@ EXPORTS = {
     "gcb_adamw_step": (C.c_int, [_fp, _fp, _fp, _fp, C.c_int64, C.c_int64, C.c_int64, C.c_double,
                                  C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _fp,
                                  C.c_double, _fp]),
+    "gcb_add_gaussian_noise": (C.c_int, [C.POINTER(NoiseSegment), C.c_int32, C.c_uint64, C.c_uint32,
+                                         C.c_float, _fp]),
     "gcb_layer_forward": (C.c_int, [C.POINTER(LayerDesc), _fp]),
     "gcb_segment_sum": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, _fp, C.c_int32, C.c_int32, _fp]),
     "gcb_segment_sum_heavy": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, _fp, C.c_int32, _fp,

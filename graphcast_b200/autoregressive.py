@@ -28,15 +28,26 @@ graphcast_b200/feedback.py and DESIGN.md section 3.5.
 `input_jvp` (the tangent-linear forecast, `jax.jvp` of the unroll) runs forward with the rollout: each
 step's tangent planes are fed on the device from the step before, so it needs no checkpointing.
 
-Not provided: input noise (a training-side feature)."""
+Input noise (`noise_level`, :63-86 and :238-249) applies where the reference applies it: in `loss`,
+`loss_and_grads` and `loss_and_input_grads` with several target times, once, to the time-dependent
+inputs (those that are targets or forcings) before the unroll, each variable with noise of its own
+shape, in physical units.  `__call__`, `input_vjp`, `input_jvp` and every one-step call are
+noise-free.  The noise is drawn on the device by gcb_add_gaussian_noise, a counter-based generator
+(Philox4x32-10 and Box-Muller) keyed by `rng` (an int seed, or a uint32 [2] array laid out as
+jax.random.PRNGKey's key), and a variable's noise depends only on the key, the variable's name and the
+element index.  JAX's threefry draws are not reproduced.  `noisy_inputs` returns the noised Dataset, and
+the loss and its gradients are exactly those of the noiseless path on it; the input gradients are
+returned with respect to the caller's inputs (the derivative of x + noise with respect to x is 1)."""
 
 from __future__ import annotations
 
-from typing import Optional
+import zlib
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
 
+from graphcast_b200 import _native
 from graphcast_b200 import feedback
 from graphcast_b200 import graphcast
 from graphcast_b200 import losses
@@ -51,8 +62,12 @@ class Predictor(graphcast.Predictor):
 
   def __init__(self, predictor: graphcast.Predictor, noise_level: Optional[float] = None,
                gradient_checkpointing: bool = False):
-    if noise_level:
-      raise NotImplementedError("input noise is a training-time feature")
+    if noise_level is not None:
+      noise_level = float(noise_level)
+      if not np.isfinite(noise_level):
+        raise ValueError(f"noise_level must be finite, not {noise_level}")
+    # None and 0 turn the noise off (the reference's `if self._noise_level:`)
+    self._noise_level = noise_level or None
     # The multi-step gradient recomputes every step from its saved inputs (the reference's hk.remat
     # per step); without checkpointing it would hold every step's activations, which is not offered.
     self._gradient_checkpointing = bool(gradient_checkpointing)
@@ -100,13 +115,72 @@ class Predictor(graphcast.Predictor):
       return lambda i, t, f: p._device_loss(i, t, f, True)
     return None
 
-  def loss(self, inputs, targets, forcings, **kwargs):
-    """The mean over target times of the per-step losses of the underlying predictor."""
+  def noisy_inputs(self, inputs, targets, forcings, rng, *, _noise_fold: int = 0) -> xs.Dataset:
+    """The inputs the multi-step loss unrolls from: with noise and several target times, the constant
+    inputs unchanged and every time-dependent input (noise_plan) as a new float32 tensor x + noise on
+    the device of the GraphCast at the bottom of the stack; otherwise `inputs` itself.  The caller's
+    arrays are not modified."""
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    forcings = xs.from_xarray(forcings)
+    if targets.sizes["time"] == 1 or not self._noise_level:
+      return inputs
+    self._validate(inputs, targets, forcings)
+    return self._noised(inputs, targets, forcings, rng, _noise_fold)
+
+  def _noised(self, inputs: xs.Dataset, targets: xs.Dataset, forcings: xs.Dataset, rng,
+              fold: int) -> xs.Dataset:
+    """noisy_inputs after its checks (several target times); `inputs` itself without noise."""
+    if not self._noise_level:
+      return inputs
+    if rng is None:
+      raise ValueError("input noise needs an rng: pass rng= (an int seed, or a uint32 [2] key)")
+    seed = rng_seed(rng)
+    if not 0 <= int(fold) < 2**32:
+      raise ValueError(f"the noise fold must lie in [0, 2**32), not {fold}")
+    plan = noise_plan(inputs, targets, forcings)
+    model = graphcast.innermost_graphcast(self)
+    if model is None:
+      raise NotImplementedError("input noise is drawn on the device of the GraphCast at the bottom of "
+                                f"the predictor stack; {type(self._predictor).__name__} holds none")
+    dev = model.compute_device()
+    out = inputs.copy()
+    segments = []
+    with torch.cuda.device(dev):
+      for name, stream in plan:
+        v = inputs.data_vars[name]
+        if isinstance(v.data, torch.Tensor):
+          caller = v.data.detach()
+          src = caller.to(device=dev, dtype=torch.float32).contiguous()
+          # noised in place when that made a copy, else into a new tensor
+          copied = src.untyped_storage().data_ptr() != caller.untyped_storage().data_ptr()
+          dst = src if copied else torch.empty_like(src)
+        else:                                     # uploaded once, then noised in place
+          src = torch.from_numpy(np.ascontiguousarray(v.data, np.float32)).to(dev)
+          dst = src
+        segments.append((src, dst, stream))
+        out[name] = v.copy(dst)
+      lib = _native.lib()
+      st = torch.cuda.current_stream(dev).cuda_stream
+      for k in range(0, len(segments), _native.GCB_NOISE_MAX_SEGMENTS):
+        chunk = segments[k:k + _native.GCB_NOISE_MAX_SEGMENTS]
+        table = (_native.NoiseSegment * len(chunk))()
+        for entry, (src, dst, stream) in zip(table, chunk):
+          entry.src, entry.dst, entry.n, entry.offset, entry.stream = (
+              src.data_ptr(), dst.data_ptr(), dst.numel(), 0, stream)
+        _native.check(lib.gcb_add_gaussian_noise(table, len(chunk), seed, int(fold),
+                                                 float(self._noise_level), st),
+                      "gcb_add_gaussian_noise")
+    return out
+
+  def loss(self, inputs, targets, forcings, rng=None, *, _noise_fold: int = 0, **kwargs):
+    """The mean over target times of the per-step losses of the underlying predictor; with noise,
+    those of the inputs noised by `rng` (noisy_inputs)."""
     inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
     forcings = xs.from_xarray(forcings)
     if targets.sizes["time"] == 1:
       return self._predictor.loss(inputs, targets, forcings, **kwargs)
     self._validate(inputs, targets, forcings)
+    inputs = self._noised(inputs, targets, forcings, rng, _noise_fold)
     device_step = self._device_step()
     records = []
 
@@ -142,7 +216,7 @@ class Predictor(graphcast.Predictor):
       return p._predictor, norm_of
     return None
 
-  def loss_and_grads(self, inputs, targets, forcings, **kwargs):
+  def loss_and_grads(self, inputs, targets, forcings, rng=None, *, _noise_fold: int = 0, **kwargs):
     """(loss, diagnostics, grads): `loss` and `diagnostics` exactly as `loss` returns them, `grads`
     the gradient of loss.mean() (the mean over the batch) with respect to the parameters.
 
@@ -152,14 +226,15 @@ class Predictor(graphcast.Predictor):
     forward is the device path of `loss`, which also keeps every step's input and target planes in
     pinned host memory; the backward pass then recomputes each step from them, last step first, and
     carries dL/d(inputs) from step to step (feedback.FeedbackPlan, gcb_output_loss_grad_feedback,
-    gcb_input_grad)."""
+    gcb_input_grad).  With noise, all of this runs on noisy_inputs(inputs, targets, forcings, rng),
+    whose tensors are released before the backward pass."""
     inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
     forcings = xs.from_xarray(forcings)
     if targets.sizes["time"] == 1:
       return self._predictor.loss_and_grads(inputs, targets, forcings, **kwargs)
     model, norm_of = self._checkpointed_parts(inputs, targets, forcings, "loss_and_grads")
     loss, diagnostics, stash, first, lat_weight, coef = self._checkpointed_loss(
-        model, norm_of, inputs, targets, forcings)
+        model, norm_of, self._noised(inputs, targets, forcings, rng, _noise_fold), targets, forcings)
     plan = feedback.FeedbackPlan(first["inputs"], first["targets"], first["forcings"])
     grads = model._bptt_grads(stash, plan, first["norm"], lat_weight, coef)
     return loss, diagnostics, grads
@@ -182,7 +257,9 @@ class Predictor(graphcast.Predictor):
     """The forward of a gradient over several target times: the device path of `loss`, which also
     keeps every step's input and target planes in pinned host memory (graphcast.StepStash).  Returns
     (loss, diagnostics, stash, first step's {inputs, targets, forcings, norm}, latitude weights,
-    loss-derivative coefficients 2 kappa / (batch * steps))."""
+    loss-derivative coefficients 2 kappa / (batch * steps)).  first["inputs"] is the layout of step 0's
+    inputs only (_layout): the stash holds their values, and the tensors of noised inputs (1.9 GB at
+    0.25 degree) must not outlive the forward."""
     records, first = [], {}
     stash = None
 
@@ -193,7 +270,7 @@ class Predictor(graphcast.Predictor):
       records.append((finish, sums))
       if stash is None:
         stash = graphcast.StepStash(model.engine.device)
-        first.update(inputs=inputs, targets=targets_template, forcings=forcings, norm=norm)
+        first.update(inputs=_layout(inputs), targets=targets_template, forcings=forcings, norm=norm)
       model._stash_step(stash)
       return predictions
 
@@ -210,21 +287,23 @@ class Predictor(graphcast.Predictor):
     return (loss, diagnostics, stash, first, lat_weight,
             2.0 * kappa / (stash.batch * len(records)))
 
-  def loss_and_input_grads(self, inputs, targets, forcings, **kwargs):
+  def loss_and_input_grads(self, inputs, targets, forcings, rng=None, *, _noise_fold: int = 0,
+                           **kwargs):
     """(loss, diagnostics, input_grads, forcing_grads): `loss` and `diagnostics` exactly as `loss`
     returns them, the gradients of loss.mean() with respect to every variable of `inputs` and
     `forcings` (GraphCast.loss_and_input_grads).  One target time delegates to the inner predictor;
     several differentiate through the fed-back predictions and forcings as loss_and_grads does
     (gradient_checkpointing=True), over every input channel (feedback.FeedbackPlan.all_channels): the
     inputs collect every step's contributions, the forcings of target time t those of step t and of
-    the last input frame of step t + 1."""
+    the last input frame of step t + 1.  With noise, the gradients are taken at noisy_inputs(inputs,
+    targets, forcings, rng) and returned with respect to `inputs`."""
     inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
     forcings = xs.from_xarray(forcings)
     if targets.sizes["time"] == 1:
       return self._predictor.loss_and_input_grads(inputs, targets, forcings, **kwargs)
     model, norm_of = self._checkpointed_parts(inputs, targets, forcings, "input gradients")
     loss, diagnostics, stash, first, lat_weight, coef = self._checkpointed_loss(
-        model, norm_of, inputs, targets, forcings)
+        model, norm_of, self._noised(inputs, targets, forcings, rng, _noise_fold), targets, forcings)
     plan = feedback.FeedbackPlan.all_channels(first["inputs"], first["targets"], first["forcings"])
     input_grads, forcing_grads = model._input_grads(stash, plan, first["norm"], inputs, forcings,
                                                     lat_weight=lat_weight, coef=coef)
@@ -306,6 +385,49 @@ class Predictor(graphcast.Predictor):
         ds[name] = step_tangents.data_vars[name]
       timed.append(ds)
     return xs.concat_time(chunks), xs.concat_time(timed)
+
+
+def rng_seed(rng) -> int:
+  """The 64-bit seed of an `rng`: an int in [0, 2**64), or a uint32 array of shape (2,) laid out as
+  jax.random.PRNGKey(seed) lays out its key, [seed >> 32, seed & 0xffffffff]."""
+  if isinstance(rng, (bool, np.bool_)):
+    raise ValueError("rng must be an int seed or a uint32 [2] key, not a bool")
+  if isinstance(rng, (int, np.integer)):
+    if not 0 <= int(rng) < 2**64:
+      raise ValueError(f"an int rng must lie in [0, 2**64), not {rng}")
+    return int(rng)
+  key = np.asarray(rng)
+  if key.shape != (2,) or key.dtype != np.uint32:
+    raise ValueError(f"rng must be an int seed or a uint32 array of shape (2,), not {key.dtype} "
+                     f"{key.shape}")
+  return (int(key[0]) << 32) | int(key[1])
+
+
+def noise_plan(inputs: xs.Dataset, targets: xs.Dataset, forcings: xs.Dataset) -> List[Tuple[str, int]]:
+  """(name, stream) of every input the noise applies to, in the order of `inputs`: the time-dependent
+  inputs, which are targets or forcings (reference :238-242; the others are the constant inputs).
+  stream = crc32 of the name, so that a variable's noise does not depend on which others are present;
+  two variables with the same stream raise ValueError."""
+  plan, seen = [], {}
+  for name in inputs.keys():
+    if name not in targets and name not in forcings:
+      continue
+    stream = zlib.crc32(name.encode())
+    if stream in seen:
+      raise ValueError(f"input variables {seen[stream]} and {name} have the same noise stream "
+                       f"{stream:#010x} (crc32 of the name): rename one of them")
+    seen[stream] = name
+    plan.append((name, stream))
+  return plan
+
+
+def _layout(ds: xs.Dataset) -> xs.Dataset:
+  """`ds` with each variable's data replaced by a zero-stride array of its shape: the names, dims,
+  shapes and coords that the backward pass's channel plans read, without the values."""
+  out = ds.copy()
+  for name, v in ds.data_vars.items():
+    out[name] = v.copy(np.broadcast_to(np.float32(0), v.shape))
+  return out
 
 
 def _mean_over_time(step_losses, step_diagnostics):

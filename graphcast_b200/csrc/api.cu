@@ -17,6 +17,7 @@
 #include "mlp_chain.cuh"
 #include "backward_kernels.cuh"
 #include "optim_kernels.cuh"
+#include "noise_kernels.cuh"
 
 namespace {
 
@@ -599,6 +600,55 @@ int gcb_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, int6
   const long long blocks = std::min<long long>((work + 255) / 256, 16LL * sm_count_cached());
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   gcb::adamw_kernel<<<static_cast<unsigned>(blocks), 256, 0, st>>>(p, g, m, v, sumsq, a, vec4);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int gcb_add_gaussian_noise(const gcb_noise_segment* segments, int32_t n_segments, uint64_t seed,
+                           uint32_t fold, float sigma, void* stream) {
+  GCB_CHECK_ARG(n_segments >= 0 && n_segments <= GCB_NOISE_MAX_SEGMENTS,
+                "n_segments out of [0, GCB_NOISE_MAX_SEGMENTS]");
+  GCB_CHECK_ARG(segments != nullptr || n_segments == 0, "null segments");
+  GCB_CHECK_ARG(isfinite(sigma), "sigma must be finite");
+  static_assert(GCB_NOISE_MAX_SEGMENTS == gcb::kMaxNoiseSegments, "segment capacity");
+  gcb::NoiseArgs a;
+  memset(&a, 0, sizeof(a));
+  a.key0 = static_cast<unsigned>(seed & 0xffffffffu);
+  a.key1 = static_cast<unsigned>(seed >> 32);
+  a.fold = fold;
+  a.sigma = sigma;
+  long long items = 0, bytes = 0;
+  for (int32_t i = 0; i < n_segments; ++i) {
+    const gcb_noise_segment& s = segments[i];
+    GCB_CHECK_ARG(s.n >= 0 && s.offset >= 0 && s.offset <= INT64_MAX - s.n, "segment n / offset out of range");
+    if (s.n == 0) continue;
+    GCB_CHECK_ARG(s.dst != nullptr, "null dst");
+    const uintptr_t d = reinterpret_cast<uintptr_t>(s.dst), r = reinterpret_cast<uintptr_t>(s.src);
+    GCB_CHECK_ARG((d & 3u) == 0 && (r & 3u) == 0, "src / dst not 4-byte aligned");
+    const uintptr_t span = static_cast<uintptr_t>(s.n) * sizeof(float);
+    GCB_CHECK_ARG(s.src == nullptr || s.src == s.dst || r + span <= d || d + span <= r,
+                  "src and dst overlap without being equal");
+    gcb::NoiseSeg& g = a.seg[a.nseg++];
+    g.src = s.src;
+    g.dst = s.dst;
+    g.n = s.n;
+    g.offset = s.offset;
+    g.stream = s.stream;
+    g.group0 = s.offset / 4;
+    g.begin = items;
+    items += (s.offset + s.n - 1) / 4 - g.group0 + 1;
+    // dst + (4 j - offset) is 16-byte aligned for every j iff dst - offset (in floats) is
+    const long long phase = static_cast<long long>((d / 4) & 3u) - (s.offset & 3);
+    const long long phase_src = static_cast<long long>((r / 4) & 3u) - (s.offset & 3);
+    g.vec4 = (phase & 3) == 0 && (s.src == nullptr || (phase_src & 3) == 0);
+    bytes += (s.src ? 8LL : 4LL) * s.n;
+  }
+  a.items = items;
+  if (items == 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long blocks = std::min<long long>((items + 255) / 256, 16LL * sm_count_cached());
+  ProfScope prof(st, GCB_KIND_NOISE, 0.0, static_cast<double>(bytes));
+  gcb::gaussian_noise_kernel<<<static_cast<unsigned>(blocks), 256, 0, st>>>(a);
   GCB_CUDA(cudaGetLastError());
   return GCB_OK;
 }

@@ -237,6 +237,13 @@ class GraphCast(Predictor):
       raise RuntimeError("GraphCast has not been called yet")
     return self._engine
 
+  def compute_device(self) -> torch.device:
+    """The device the model runs on: its engine's, or the one the next call builds its engine on."""
+    if self._engine is not None:
+      return self._engine.device
+    return torch.device(self._device if self._device is not None
+                        else f"cuda:{torch.cuda.current_device()}")
+
   # -- lazy initialisation (reference _maybe_init :368-378) -------------------------
   def _maybe_init(self, sample_inputs: xs.Dataset, c_in: int) -> None:
     if not self._initialized:
@@ -769,6 +776,15 @@ class GraphCast(Predictor):
       da = xs.DataArray(piece, ("batch",) + s.stack_dims + ("lat", "lon"))
       out[s.name] = da.transpose(*s.var_dims)
     return out
+
+
+def innermost_graphcast(predictor) -> Optional[GraphCast]:
+  """The GraphCast at the bottom of a predictor stack (autoregressive.Predictor, InputsAndResiduals,
+  Bfloat16Cast wrappers hold it as `_predictor`), or None."""
+  p = predictor
+  while p is not None and not isinstance(p, GraphCast):
+    p = getattr(p, "_predictor", None)
+  return p
 
 
 def init_params(model_config: ModelConfig, task_config: TaskConfig, c_in: int,

@@ -11,9 +11,14 @@ flat fp32 master weights and moments in one pass, and Engine.load_params_device 
 weights from the master weights on the device.  Nothing goes through the host but the loss and the
 norm that `step` returns.
 
+The input noise of an autoregressive.Predictor(noise_level=...) is keyed per step: `step(..., rng=None)`
+draws with (seed, fold = count), so each step gets fresh noise, a run is reproducible from the
+constructor's `seed`, and a run resumed with load_state() replays its noise exactly; an explicit `rng`
+(an int seed or a uint32 [2] key, as autoregressive.Predictor.loss_and_grads takes it) uses fold 0.
+
 Differences from optax: the master weights are fp32 whatever the predictor's precision, the gradient
-is the one the kernels compute (see GraphCast.loss_and_grads), and `step` takes no rng and returns no
-next state.  GraphCast was trained with b1 = 0.9, b2 = 0.95, weight decay 0.1 and clipping at global
+is the one the kernels compute (see GraphCast.loss_and_grads), and `step` returns no next state.
+GraphCast was trained with b1 = 0.9, b2 = 0.95, weight decay 0.1 and clipping at global
 norm 32 (the paper's supplement); those are the defaults here.
 """
 
@@ -26,6 +31,7 @@ import numpy as np
 import torch
 
 from graphcast_b200 import _native
+from graphcast_b200 import autoregressive
 from graphcast_b200 import graphcast
 
 
@@ -77,15 +83,12 @@ class FlatLayout:
 
 
 def _graphcast_of(predictor) -> graphcast.GraphCast:
-  """The GraphCast at the bottom of a predictor stack (autoregressive.Predictor, InputsAndResiduals,
-  Bfloat16Cast wrappers hold it as `_predictor`)."""
-  p = predictor
-  while not isinstance(p, graphcast.GraphCast):
-    p = getattr(p, "_predictor", None)
-    if p is None:
-      raise NotImplementedError(
-          f"optim.AdamW trains a GraphCast predictor, directly or inside autoregressive.Predictor, "
-          f"InputsAndResiduals or Bfloat16Cast; {type(predictor).__name__} holds none")
+  """The GraphCast at the bottom of a predictor stack (graphcast.innermost_graphcast)."""
+  p = graphcast.innermost_graphcast(predictor)
+  if p is None:
+    raise NotImplementedError(
+        f"optim.AdamW trains a GraphCast predictor, directly or inside autoregressive.Predictor, "
+        f"InputsAndResiduals or Bfloat16Cast; {type(predictor).__name__} holds none")
   return p
 
 
@@ -105,7 +108,7 @@ class AdamW:
   def __init__(self, predictor, learning_rate: Union[float, Callable[[int], float]] = 1e-4, *,
                b1: float = 0.9, b2: float = 0.95, eps: float = 1e-8, eps_root: float = 0.0,
                weight_decay: float = 0.1, mask: Optional[Callable[[str, str], bool]] = None,
-               max_grad_norm: Optional[float] = 32.0):
+               max_grad_norm: Optional[float] = 32.0, seed: int = 0):
     if not callable(learning_rate):
       learning_rate = float(learning_rate)
       if not np.isfinite(learning_rate) or learning_rate < 0:
@@ -120,6 +123,7 @@ class AdamW:
       raise ValueError("mask must be None or a callable(module, field) -> bool")
     if max_grad_norm is not None and not np.isfinite(float(max_grad_norm)):
       raise ValueError(f"max_grad_norm must be None or a finite float, not {max_grad_norm}")
+    self.seed = autoregressive.rng_seed(seed)
     self._predictor = predictor
     self._model = _graphcast_of(predictor)
     self._lr = learning_rate
@@ -140,11 +144,7 @@ class AdamW:
     params = model._params
     if params is None:
       raise ValueError("GraphCast has no parameters: pass params= or call set_params()")
-    if model._engine is not None:
-      device = model._engine.device
-    else:
-      device = torch.device(model._device if model._device is not None
-                            else f"cuda:{torch.cuda.current_device()}")
+    device = model.compute_device()
     self.layout = FlatLayout.of(params, self._mask)
     lib = _native.lib()
     p = torch.from_numpy(self.layout.flatten(params)).to(device)
@@ -200,10 +200,18 @@ class AdamW:
     eng.load_params_device(self._p_views)
     self._synced = (weakref.ref(eng), eng.weights_version)
 
-  def step(self, inputs, targets, forcings):
+  def step(self, inputs, targets, forcings, rng=None):
     """One training step on a batch: returns (loss, diagnostics, grad_norm), `loss` and `diagnostics`
     exactly as predictor.loss_and_grads returns them at the current weights, grad_norm the global
-    norm of the gradient before clipping.  Raises NotImplementedError where loss_and_grads does."""
+    norm of the gradient before clipping.  Raises NotImplementedError where loss_and_grads does.
+
+    rng: the key of the input noise of an autoregressive.Predictor with noise_level (used with several
+    target times only).  None draws with the optimiser's seed and the step count as the fold, so every
+    step gets fresh noise and a run resumed from state() replays it; an explicit rng uses fold 0."""
+    kwargs = {}
+    if isinstance(self._predictor, autoregressive.Predictor):
+      kwargs = (dict(rng=self.seed, _noise_fold=self._count) if rng is None
+                else dict(rng=rng, _noise_fold=0))
     self._ensure_state()
     model = self._model
     self._sync_engine()
@@ -217,7 +225,7 @@ class AdamW:
       taken.append(eng)
     model._grad_sink = sink
     try:
-      loss, diagnostics, _ = self._predictor.loss_and_grads(inputs, targets, forcings)
+      loss, diagnostics, _ = self._predictor.loss_and_grads(inputs, targets, forcings, **kwargs)
     finally:
       model._grad_sink = None
     if not taken:

@@ -189,6 +189,32 @@ int gcb_adamw_step(float* p, const float* g, float* m, float* v, int64_t n, int6
                    double learning_rate, double b1, double b2, double eps, double eps_root,
                    double weight_decay, const double* sumsq, double max_norm, void* stream);
 
+/* ---- input noise (autoregressive.Predictor(noise_level=...)) -------------------------------
+ * One segment of gcb_add_gaussian_noise: n fp32 elements, dst[k] being element offset + k of
+ * stream `stream`.  src == NULL writes the noise alone; src == dst noises in place (any other
+ * overlap is not allowed).  src and dst are 4-byte aligned. */
+typedef struct {
+  const float* src;
+  float* dst;
+  int64_t n;
+  int64_t offset;     /* >= 0: element index of dst[0] in the stream */
+  uint32_t stream;
+} gcb_noise_segment;
+
+#define GCB_NOISE_MAX_SEGMENTS 64
+
+/* dst[k] = fl32(src[k] + fl32(sigma * z(seed, fold, stream, offset + k))) in fp32 for every segment
+ * (src == NULL: fl32(sigma * z) alone), z a standard normal drawn by a counter-based generator:
+ * Philox4x32-10 with key (seed & 0xffffffff, seed >> 32) and counter (j & 0xffffffff, j >> 32, stream,
+ * fold), j = i / 4, gives words w0..w3; u_k = (w_k + 0.5) 2^-32 (fp64); Box-Muller in fp64,
+ * z0 = r cos(2 pi u1), z1 = r sin(2 pi u1), r = sqrt(-2 ln u0), z2 and z3 from (u2, u3) the same way,
+ * each rounded to fp32 once; element i takes z_{i mod 4}.  The draw of an element depends on
+ * (seed, fold, stream, i) only: not on the launch, the device, the segments or pointer alignment.
+ * segments: a host array of 0..GCB_NOISE_MAX_SEGMENTS entries; sigma finite.  One launch on
+ * `stream`; deterministic. */
+int gcb_add_gaussian_noise(const gcb_noise_segment* segments, int32_t n_segments, uint64_t seed,
+                           uint32_t fold, float sigma, void* stream);
+
 /* CTAs per thread-block cluster of the tensor-core layer kernel (1, 2 or 4; default
  * 2).  The CTAs of a cluster process consecutive row tiles in lockstep and receive
  * each weight tile once from L2 through TMA multicast.  Process-wide tuning knob. */
@@ -629,11 +655,12 @@ typedef enum {
   GCB_KIND_LAYER_SIMT = 4, GCB_KIND_ROWS_TO_IMAGE = 5, GCB_KIND_CHAIN_TC = 6, GCB_KIND_GATHER = 7,
   GCB_KIND_LOSS = 8,        /* gcb_output_loss (both of its launches) */
   GCB_KIND_WGRAD = 9,       /* gcb_weight_grad (both of its launches) */
-  GCB_KIND_ROWWISE_BWD = 10 /* gcb_layernorm_backward, gcb_swish_backward, gcb_output_loss_grad,
+  GCB_KIND_ROWWISE_BWD = 10,/* gcb_layernorm_backward, gcb_swish_backward, gcb_output_loss_grad,
                              * gcb_segment_sum_sorted, gcb_gather_add, gcb_swish_rows,
                              * gcb_output_loss_grad_feedback, gcb_input_grad,
                              * gcb_output_cotangent_grad_feedback, gcb_broadcast_grad_sum,
                              * gcb_layernorm_jvp */
+  GCB_KIND_NOISE = 11       /* gcb_add_gaussian_noise */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
 int gcb_profile_end(int32_t capacity, int32_t* kinds, float* ms, double* flops, double* bytes,
