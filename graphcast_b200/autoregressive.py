@@ -356,6 +356,30 @@ class Predictor(graphcast.Predictor):
     if targets_template.sizes["time"] == 1:
       return self._predictor.input_jvp(inputs, targets_template, forcings, input_tangents,
                                        forcing_tangents, **kwargs)
+    return self._tangent_rollout(inputs, targets_template, forcings, input_tangents,
+                                 forcing_tangents, directions=False)
+
+  def batched_input_jvp(self, inputs, targets_template, forcings, input_tangents,
+                        forcing_tangents=None, *, directions_per_pass=None, **kwargs):
+    """input_jvp along K tangent directions at once (GraphCast.batched_input_jvp), over every target
+    time: the tangent Datasets carry a leading "direction" dim, and so do prediction_tangents.  One
+    target time delegates to the inner predictor.  Several run the rollout once per pass of
+    directions_per_pass directions (None: all), feeding every direction's tangent planes on the device
+    with one gather per step (feedback.FeedbackPlan.feed_index(K))."""
+    inputs, targets_template = xs.from_xarray(inputs), xs.from_xarray(targets_template)
+    forcings = xs.from_xarray(forcings)
+    if targets_template.sizes["time"] == 1:
+      return self._predictor.batched_input_jvp(inputs, targets_template, forcings, input_tangents,
+                                               forcing_tangents,
+                                               directions_per_pass=directions_per_pass, **kwargs)
+    one_pass = lambda it, ft: self._tangent_rollout(inputs, targets_template, forcings, it, ft,
+                                                    directions=True)
+    return graphcast.batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
+                                 directions_per_pass)
+
+  def _tangent_rollout(self, inputs, targets_template, forcings, input_tangents, forcing_tangents,
+                       directions: bool):
+    """input_jvp (batched_input_jvp with `directions`) over several target times."""
     parts = self._device_parts()
     if parts is None:
       raise NotImplementedError("input_jvp over several target times needs a GraphCast predictor, "
@@ -365,7 +389,8 @@ class Predictor(graphcast.Predictor):
     num_steps = targets_template.sizes["time"]
     one = lambda ds: ds.isel(time=slice(0, 1))
     run = graphcast._TangentRun(inputs, forcings, input_tangents, forcing_tangents, num_steps,
-                                feedback.FeedbackPlan(inputs, one(targets_template), one(forcings)))
+                                feedback.FeedbackPlan(inputs, one(targets_template), one(forcings)),
+                                directions=directions)
     tangents = []
 
     def step(rng, inputs, targets_template, forcings):
@@ -381,6 +406,8 @@ class Predictor(graphcast.Predictor):
     timed = []
     for chunk, step_tangents in zip(chunks, tangents):
       ds = xs.Dataset(coords=chunk.coords)
+      if directions:
+        ds.coords[feedback.DIRECTION] = step_tangents.coords[feedback.DIRECTION]
       for name in step_tangents.keys():
         ds[name] = step_tangents.data_vars[name]
       timed.append(ds)

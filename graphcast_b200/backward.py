@@ -19,9 +19,11 @@ SURVEY.md appendix A:
   * inputs (grid features, mesh zeros + structural, edge features) are constants: their MLPs get dW,
     never dX.
 
-The tangent-linear model (input_jvp) walks the same graph in forward order with the same helpers
-(Backward.tangent): each stage of the stage-wise forward is followed by its tangent, every MLP's tangent
-formed at its recomputed h and z (mlp_jvp; gcb_layernorm_jvp for the LayerNorm).
+The tangent-linear model (input_jvp, batched_input_jvp) walks the same graph in forward order with the
+same helpers (Backward.tangent): each stage of the stage-wise forward is followed by its tangent, every
+MLP's tangent formed at its recomputed h and z (mlp_jvp; gcb_swish_jvp and gcb_layernorm_jvp_dirs for
+the two nonlinearities).  Several tangent directions share that walk: their state is stacked
+direction-major, so every tangent GEMM runs once over all of them and h and z are recomputed once.
 
 All arithmetic is in libgraphcast_b200.so; this module only sequences the launches and owns the
 buffers.  Allocation is lazy: nothing here exists until the first loss_and_grads call.
@@ -109,14 +111,18 @@ class Backward:
     # boundaries (for mesh2grid: grid nodes, 3 edges each), so that every receiver sum is complete
     # inside its chunk; the sender sums of the chunks are added in chunk order.
     self.chunk_rows = int(chunk_rows)
-    self.chunks = {
-        "m2g": self._chunks(np.arange(0, 3 * m.num_grid + 1, 3, dtype=np.int64),
-                            eng.exec_senders["m2g"], m.num_mesh),
-        "g2m": self._chunks(eng.exec_row_ptr["g2m"].astype(np.int64), eng.exec_senders["g2m"],
-                            m.num_grid),
+    self._chunk_src = {
+        "m2g": (np.arange(0, 3 * m.num_grid + 1, 3, dtype=np.int64), eng.exec_senders["m2g"],
+                m.num_mesh),
+        "g2m": (eng.exec_row_ptr["g2m"].astype(np.int64), eng.exec_senders["g2m"], m.num_grid),
     }
+    self.chunks = {name: self._chunks(*src, self.chunk_rows) for name, src in self._chunk_src.items()}
     self.iota = self._i32(np.arange(max(m.num_grid, m.num_mesh)))
     self._edge_iota = None
+    # the tangent of several directions (tangent(dirs=...)): their K-fold gather indices and chunks
+    self.dirs = 1
+    self._kfold, self._kfold_dirs = {}, 1
+    self._tangent_chunks = {}
     self.zero_bias = torch.zeros([D], dtype=torch.float32, device=dev)
     self.prec = _native.PRECISIONS[eng.precision]
     self.ws_rows = torch.empty([max(self.lib.gcb_rowwise_workspace_bytes(D), 16)], dtype=torch.uint8, device=dev)
@@ -136,22 +142,24 @@ class Backward:
     return (self._i32(order), self._i32(ptr),
             self._i32(heavy if heavy.size else np.zeros([1], np.int32)), int(heavy.size))
 
-  def _chunks(self, row_ptr: np.ndarray, senders: np.ndarray, n_senders: int):
-    """Receiver-aligned chunks of a bipartite edge set: (r0, r1, g0, g1, local receiver row_ptr,
-    local heavy receivers, count, sender CSR of the chunk's edges)."""
+  def _chunks(self, row_ptr: np.ndarray, senders: np.ndarray, n_senders: int, chunk_rows: int,
+              csr: bool = True):
+    """Receiver-aligned chunks of at most chunk_rows edges (at least one receiver) of a bipartite edge
+    set: (r0, r1, g0, g1, local receiver row_ptr, local heavy receivers, count, sender CSR of the
+    chunk's edges, or None without `csr`)."""
     out = []
     n_rcv = row_ptr.shape[0] - 1
     g0 = 0
     while g0 < n_rcv:
       # the last receiver whose edges still fit (at least one receiver per chunk)
-      g1 = int(np.searchsorted(row_ptr, row_ptr[g0] + self.chunk_rows, side="right")) - 1
+      g1 = int(np.searchsorted(row_ptr, row_ptr[g0] + chunk_rows, side="right")) - 1
       g1 = min(max(g1, g0 + 1), n_rcv)
       r0, r1 = int(row_ptr[g0]), int(row_ptr[g1])
       rp = row_ptr[g0:g1 + 1] - row_ptr[g0]
       heavy = np.nonzero(np.diff(rp) > 256)[0].astype(np.int32)
       out.append((r0, r1, g0, g1, self._i32(rp),
                   self._i32(heavy if heavy.size else np.zeros([1], np.int32)), int(heavy.size),
-                  self._csr(senders[r0:r1], n_senders)))
+                  self._csr(senders[r0:r1], n_senders) if csr else None))
       g0 = g1
     return out
 
@@ -550,6 +558,52 @@ class Backward:
     return dx
 
   # -- tangent-linear model (Engine.input_jvp_element) ------------------------------------------------
+  # The tangent state of `dirs` directions is stacked direction-major: a table of n rows per direction
+  # holds direction k in rows [k * dir_stride(n), k * dir_stride(n) + n), the stride rounded up to the
+  # 128-row tiles of the operand images.  The last direction is not padded, so that one direction is
+  # exactly the table of n rows.  The pad rows between directions are never read into a valid row: the
+  # GEMMs and row-wise kernels treat every row on its own, and the segment sums and unpacks run per
+  # direction.
+  @staticmethod
+  def dir_stride(rows: int) -> int:
+    return (rows + 127) // 128 * 128
+
+  def dir_rows(self, rows: int) -> int:
+    """Rows of a stacked tangent table of self.dirs directions of `rows` rows each."""
+    return (self.dirs - 1) * self.dir_stride(rows) + rows
+
+  def kfold(self, idx: torch.Tensor, n_src: int, key) -> torch.Tensor:
+    """The gather index `idx` (into a table of n_src rows per direction) for self.dirs directions:
+    idx + k * dir_stride(n_src) in the rows of direction k of a stacked table of len(idx) rows per
+    direction, 0 in the pad rows.  Built on first use per `key` and kept while the direction count
+    stays the same."""
+    if self.dirs == 1:
+      return idx
+    if self._kfold_dirs != self.dirs:
+      self._kfold, self._kfold_dirs = {}, self.dirs
+    out = self._kfold.get(key)
+    if out is None:
+      n, s_src, s = idx.shape[0], self.dir_stride(n_src), self.dir_stride(idx.shape[0])
+      out = torch.zeros([self.dir_rows(n)], dtype=torch.int32, device=self.dev)
+      for k in range(self.dirs):
+        out[k * s:k * s + n] = idx + k * s_src
+      self._kfold[key] = out
+    return out
+
+  def tangent_chunks(self, name: str):
+    """The receiver-aligned chunks of a bipartite edge set for the tangent of self.dirs directions: those
+    of the backward pass for one direction, else chunks of chunk_rows // dirs edges (built on first
+    use, without the sender CSR), so that the stacked temporaries stay the size of one direction's.
+    Every receiver's sum is complete inside its chunk, so the results do not depend on the chunking."""
+    if self.dirs == 1:
+      return self.chunks[name]
+    key = (name, self.dirs)
+    if key not in self._tangent_chunks:
+      row_ptr, senders, n_senders = self._chunk_src[name]
+      self._tangent_chunks[key] = self._chunks(row_ptr, senders, n_senders,
+                                               max(self.chunk_rows // self.dirs, 1), csr=False)
+    return self._tangent_chunks[key]
+
   def w0_block(self, info: _MlpInfo, s: int) -> int:
     """Address of the packed image of the 512-row block s of an MLP's first layer (the image is K-step
     major, so a row block is a contiguous slice)."""
@@ -558,29 +612,30 @@ class Backward:
   def mlp_jvp(self, info: _MlpInfo, rows: int, segs, dsegs, *, pre=None, dpre=(), w0=None,
               dw0=None, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Tangent of one MLP y = LN(swish(X W0 + b0) W1 + b1) at the recomputed forward (h, z as
-    mlp_backward forms them), along the layer-0 input tangents `dsegs` with the weight dw0 (default:
-    that of the primal, w0) and the pre-gathered addends `dpre`; with no dsegs the addends alone are the
-    pre-activation tangent.  Returns residual + dy (LayerNorm MLPs) or dy [rows, n1] (the decoder)."""
+    mlp_backward forms them, once for all directions), along the layer-0 input tangents `dsegs` with the
+    weight dw0 (default: that of the primal, w0) and the pre-gathered addends `dpre` (K-fold indices);
+    with no dsegs the addends alone are the pre-activation tangent.  Tangents are stacked tables of
+    self.dirs directions of `rows` rows.  Returns residual + dy (LayerNorm MLPs) or dy [., n1] (the
+    decoder)."""
     w = info.w
     w0 = w0 or w.w0_packed
+    nd, stride, rk = self.dirs, self.dir_stride(rows), self.dir_rows(rows)
     if dsegs:
-      dh = self.empty(rows)
-      self.layer(rows, dsegs, dw0 or w0, self.zero_bias, out_y=dh, pre=list(dpre) or None)
+      dh = self.empty(rk)
+      self.layer(rk, dsegs, dw0 or w0, self.zero_bias, out_y=dh, pre=list(dpre) or None)
     else:
       dh = None
       for table, idx in dpre:
-        dh = self.gather_add(table, idx, rows, dh)
+        dh = self.gather_add(table, idx, rk, dh)
     h = self.empty(rows)
     self.layer(rows, segs, w0, w.b0, _native.ACT_NONE, out_y=h, pre=pre)
-    ws = self.ws_rows
-    da = self.empty(rows)                    # swish'(h) dh: the Jacobian of swish is diagonal
-    _native.check(self.lib.gcb_swish_backward(
-        dh.data_ptr(), D, h.data_ptr(), D, rows, D, da.data_ptr(), D, ws.data_ptr(), ws.numel(),
-        self.sink["b0"].data_ptr(), 0, self._st()), "gcb_swish_backward")
+    da = dh                                  # swish'(h) dh in place: the Jacobian of swish is diagonal
+    _native.check(self.lib.gcb_swish_jvp(h.data_ptr(), D, rows, D, dh.data_ptr(), D, stride, nd,
+                                         da.data_ptr(), D, self._st()), "gcb_swish_jvp")
     del dh
     if not info.ln:
-      dy = self.empty(rows, info.n1)
-      self.layer(rows, [self.tab(da)], w.w1_packed, self.zero_bias, out_y=dy, n=info.n1,
+      dy = self.empty(rk, info.n1)
+      self.layer(rk, [self.tab(da)], w.w1_packed, self.zero_bias, out_y=dy, n=info.n1,
                  n_valid=info.n1_valid)
       return dy
     a = self.empty(rows)
@@ -590,54 +645,75 @@ class Backward:
     z = self.empty(rows)
     self.layer(rows, [self.tab(a)], w.w1_packed, w.b1, out_y=z)
     del a
-    dz = self.empty(rows)
-    self.layer(rows, [self.tab(da)], w.w1_packed, self.zero_bias, out_y=dz)
+    dz = self.empty(rk)
+    self.layer(rk, [self.tab(da)], w.w1_packed, self.zero_bias, out_y=dz)
     del da
-    out = self.empty(rows)
-    _native.check(self.lib.gcb_layernorm_jvp(
-        z.data_ptr(), D, dz.data_ptr(), D, w.ln_scale, rows, D, self._ptr(residual), D,
-        out.data_ptr(), D, self._st()), "gcb_layernorm_jvp")
+    out = self.empty(rk)
+    _native.check(self.lib.gcb_layernorm_jvp_dirs(
+        z.data_ptr(), D, dz.data_ptr(), D, w.ln_scale, rows, D, stride, nd, self._ptr(residual), D,
+        out.data_ptr(), D, self._st()), "gcb_layernorm_jvp_dirs")
     return out
 
   @staticmethod
   def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
+  def receiver_sums(self, dm: torch.Tensor, rows: int, row_ptr: torch.Tensor, n_nodes: int,
+                    out: torch.Tensor, out_stride: int, heavy=None, n_heavy: int = 0) -> None:
+    """gcb_segment_sum_heavy of every direction of the stacked edge tangent dm (`rows` rows per
+    direction) into n_nodes rows of every direction of the stacked node table `out` (a view starting at
+    direction 0's first row, out_stride rows per direction), one launch per direction."""
+    s_in, s_out = self.dir_stride(rows), out_stride
+    for k in range(self.dirs):
+      _native.check(self.lib.gcb_segment_sum_heavy(
+          dm[k * s_in:].data_ptr(), D, row_ptr.data_ptr(), n_nodes,
+          heavy.data_ptr() if n_heavy else None, n_heavy, out[k * s_out:].data_ptr(), D, D,
+          self._st()), "gcb_segment_sum_heavy")
+
   def bipartite_jvp(self, name: str, info: _MlpInfo, enc: _MlpInfo, feat_t: torch.Tensor,
                     snd: torch.Tensor, rcv: torch.Tensor, v_s, n_s: int, v_r, n_r: int,
                     dv_s: torch.Tensor, dv_r: Optional[torch.Tensor]) -> torch.Tensor:
     """Tangent of the receiver sums of a grid2mesh / mesh2grid edge MLP m = MLP([e | v_s[snd] |
-    v_r[rcv]]) with e = MLP(edge features) (no tangent), chunk by chunk (self.chunks): dagg [n_r, 512],
-    from the sender and (when dv_r is given) receiver node tangents."""
+    v_r[rcv]]) with e = MLP(edge features) (no tangent), chunk by chunk (tangent_chunks): dagg (n_r
+    rows per direction), from the stacked sender and (when dv_r is given) receiver node tangents."""
     sp = info.split
     ps = self.projection(n_s, v_s, sp.ws_packed)
     pr = self.projection(n_r, v_r, sp.wr_packed)
-    dps = self.projection(n_s, self.tab(dv_s), sp.ws_packed)
-    dpr = None if dv_r is None else self.projection(n_r, self.tab(dv_r), sp.wr_packed)
-    dagg = self.empty(n_r)
-    for r0, r1, g0, g1, rp, heavy, n_heavy, _ in self.chunks[name]:
+    dps = self.projection(self.dir_rows(n_s), self.tab(dv_s), sp.ws_packed)
+    dpr = None if dv_r is None else self.projection(self.dir_rows(n_r), self.tab(dv_r), sp.wr_packed)
+    dagg = self.empty(self.dir_rows(n_r))
+    for i, (r0, r1, g0, g1, rp, heavy, n_heavy, _) in enumerate(self.tangent_chunks(name)):
       n = r1 - r0
       f = self.tab(feat_t[r0:r1], 16, 4, 4)                 # 16-byte rows: the view stays aligned
       snd_c, rcv_c = snd[r0:r1].clone(), rcv[r0:r1].clone()  # index arrays from an aligned base
       e = self.fwd_mlp(enc, n, [f])
-      dpre = [(dps, snd_c)] + ([] if dpr is None else [(dpr, rcv_c)])
+      dpre = [(dps, self.kfold(snd_c, n_s, (name, i, "snd")))]
+      if dpr is not None:
+        dpre.append((dpr, self.kfold(rcv_c, n_r, (name, i, "rcv"))))
       dm = self.mlp_jvp(info, n, [self.tab(e)], [], pre=[(ps, snd_c), (pr, rcv_c)], dpre=dpre,
                         w0=sp.we_packed)
       del e
-      _native.check(self.lib.gcb_segment_sum_heavy(
-          dm.data_ptr(), D, rp.data_ptr(), g1 - g0, heavy.data_ptr() if n_heavy else None, n_heavy,
-          dagg[g0:g1].data_ptr(), D, D, self._st()), "gcb_segment_sum_heavy")
+      self.receiver_sums(dm, n, rp, g1 - g0, dagg[g0:], self.dir_stride(n_r), heavy, n_heavy)
       del dm
     return dagg
 
-  def tangent(self, grid_in_img: torch.Tensor, dgrid_in_img: torch.Tensor) -> torch.Tensor:
+  def tangent(self, grid_in_img: torch.Tensor, dgrid_in_img: torch.Tensor, dirs: int = 1) -> torch.Tensor:
     """One step stage by stage (Engine.run_stage, from the packed inputs grid_in_img) and, interleaved
-    with it, its tangent along the packed input tangent dgrid_in_img (an operand image of [Ng,
-    c_in_pad] whose structural columns are zero): returns dy [Ng, 256], the tangent of the decoder
-    output (n_out valid columns).  Each stage's tangent runs right after the stage, from the engine's
-    buffers and copies of that stage's inputs alone; the tangent state is fp32 tables.  Exactly zero
-    tangents are not formed: the mesh-node encoder, the three edge embedders, e_0 of the processor,
-    and the v_m0 and edge terms of the grid2mesh edge MLP."""
+    with it, its tangent along `dirs` directions at once: dgrid_in_img is the stacked operand image of
+    the packed input tangents ([Ng, c_in_pad] per direction, dir_stride(Ng) rows apart, structural
+    columns zero).  Returns dy, the stacked tangents of the decoder output ([Ng, 256] per direction,
+    n_out valid columns).  Each stage's tangent runs right after the stage, from the engine's buffers
+    and copies of that stage's inputs alone; the tangent state is stacked fp32 tables, and every MLP's
+    h and z are recomputed once for all directions.  Exactly zero tangents are not formed: the
+    mesh-node encoder, the three edge embedders, e_0 of the processor, and the v_m0 and edge terms of
+    the grid2mesh edge MLP."""
+    self.dirs = int(dirs)
+    try:
+      return self._tangent(grid_in_img, dgrid_in_img)
+    finally:
+      self.dirs = 1
+
+  def _tangent(self, grid_in_img, dgrid_in_img):
     eng, m = self.eng, self.m
     ng, nm = m.num_grid, m.num_mesh
     K = eng.msg_steps
@@ -666,6 +742,8 @@ class Backward:
     #      v_k and e_k are copied before step k, agg_k read after it.
     eng.run_stage("process_embed")
     de = None
+    snd_k, rcv_k = (self.kfold(eng.mesh_snd, nm, ("mesh", "snd")),
+                    self.kfold(eng.mesh_rcv, nm, ("mesh", "rcv")))
     for k in range(K):
       v_k = eng.mesh_lat_img.clone()
       if k == 0:
@@ -676,15 +754,16 @@ class Backward:
       nfo, efo = self.proc_n[k], self.proc_e[k]
       sp = efo.split
       ps, pr = self.projection(nm, img(v_k), sp.ws_packed), self.projection(nm, img(v_k), sp.wr_packed)
-      dps = self.projection(nm, tab(dv), sp.ws_packed)
-      dpr = self.projection(nm, tab(dv), sp.wr_packed)
-      dpre = [(dps, eng.mesh_snd), (dpr, eng.mesh_rcv)]
+      dps = self.projection(self.dir_rows(nm), tab(dv), sp.ws_packed)
+      dpr = self.projection(self.dir_rows(nm), tab(dv), sp.wr_packed)
+      dpre = [(dps, snd_k), (dpr, rcv_k)]
       dm = self.mlp_jvp(efo, m.e_mesh, [e_k], [] if de is None else [tab(de)],
                         pre=[(ps, eng.mesh_snd), (pr, eng.mesh_rcv)], dpre=dpre, w0=sp.we_packed)
       del ps, pr, dps, dpr, e_k
-      dagg = self.seg_sum_receiver(dm, eng.mesh_row_ptr, nm)
+      dagg = self.empty(self.dir_rows(nm))
+      self.receiver_sums(dm, m.e_mesh, eng.mesh_row_ptr, nm, dagg, self.dir_stride(nm))
       if k < K - 1:                              # the last step's edge update is never read
-        de = dm if de is None else self.gather_add(dm, self.edge_iota(), m.e_mesh, de)
+        de = dm if de is None else self.gather_add(dm, self.edge_iota(), self.dir_rows(m.e_mesh), de)
       del dm
       dv = self.mlp_jvp(nfo, nm, [img(v_k), img(eng.mesh_agg_img)], [tab(dv), tab(dagg)],
                         residual=dv)
@@ -704,9 +783,11 @@ class Backward:
     return self.mlp_jvp(mp["dec_grid"], ng, [img(eng.grid_lat_img)], [tab(dvg)])
 
   def edge_iota(self) -> torch.Tensor:
-    """0..E_mesh-1 (the identity gather of the edge-tangent update e' = e + m), made on first use."""
-    if self._edge_iota is None:
-      self._edge_iota = self._i32(np.arange(self.m.e_mesh))
+    """0..dir_rows(E_mesh)-1 (the identity gather of the edge-tangent update e' = e + m over every
+    direction), made on first use."""
+    n = self.dir_rows(self.m.e_mesh)
+    if self._edge_iota is None or self._edge_iota.shape[0] != n:
+      self._edge_iota = self._i32(np.arange(n))
     return self._edge_iota
 
   # -- result ----------------------------------------------------------------------------------------

@@ -76,3 +76,9 @@ class Bfloat16Cast(graphcast.Predictor):
                 **kwargs):
     return self._predictor.input_jvp(inputs, targets_template, forcings, input_tangents,
                                      forcing_tangents, **kwargs)
+
+  def batched_input_jvp(self, inputs, targets_template, forcings, input_tangents,
+                        forcing_tangents=None, *, directions_per_pass=None, **kwargs):
+    return self._predictor.batched_input_jvp(inputs, targets_template, forcings, input_tangents,
+                                             forcing_tangents, directions_per_pass=directions_per_pass,
+                                             **kwargs)

@@ -1112,6 +1112,44 @@ int gcb_layernorm_jvp(const float* z, int32_t ld_z, const float* dz, int32_t ld_
   return GCB_OK;
 }
 
+int gcb_swish_jvp(const float* h, int32_t ld_h, int64_t rows, int32_t n, const float* dh, int32_t ld_dh,
+                  int64_t dir_stride, int32_t dirs, float* da, int32_t ld_da, void* stream) {
+  GCB_CHECK_ARG(h && dh && da, "null pointer");
+  GCB_CHECK_ARG(n > 0 && n % 4 == 0 && ld_h % 4 == 0 && ld_dh % 4 == 0 && ld_da % 4 == 0 &&
+                    ld_h >= n && ld_dh >= n && ld_da >= n && aligned16(h) && aligned16(dh) &&
+                    aligned16(da),
+                "n / leading dimensions must be multiples of 4 with 16-byte rows");
+  GCB_CHECK_ARG(rows >= 0 && dirs >= 1 && (dirs == 1 || dir_stride >= rows),
+                "rows < 0, dirs < 1 or dir_stride < rows");
+  if (rows == 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0, 4.0 * static_cast<double>(rows) * n * (1.0 + 2.0 * dirs));
+  const long long total = rows * (n / 4);
+  gcb::swish_jvp_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
+      h, ld_h, rows, n / 4, dh, ld_dh, dir_stride, dirs, da, ld_da);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int gcb_layernorm_jvp_dirs(const float* z, int32_t ld_z, const float* dz, int32_t ld_dz,
+                           const float* scale, int64_t rows, int32_t n, int64_t dir_stride,
+                           int32_t dirs, const float* residual, int32_t ld_res, float* out,
+                           int32_t ld_out, void* stream) {
+  GCB_CHECK_ARG(z && dz && scale && out, "null pointer");
+  GCB_CHECK_ARG(n == 512, "the LayerNorm tangent needs n = 512");
+  GCB_CHECK_ARG(rows >= 0 && ld_z >= n && ld_dz >= n && ld_out >= n && (!residual || ld_res >= n),
+                "rows < 0 or leading dimension < n");
+  GCB_CHECK_ARG(dirs >= 1 && (dirs == 1 || dir_stride >= rows), "dirs < 1 or dir_stride < rows");
+  if (rows == 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * static_cast<double>(rows) * n * (1.0 + dirs * (2.0 + (residual ? 1.0 : 0.0))));
+  gcb::layernorm_jvp_dirs_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, st>>>(
+      z, ld_z, dz, ld_dz, scale, rows, dir_stride, dirs, residual, ld_res, out, ld_out);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
 int gcb_segment_sum_sorted(const float* msg, int32_t ld_msg, const int32_t* order,
                            const int32_t* ptr, int32_t num_nodes, const int32_t* heavy,
                            int32_t num_heavy, float* out, int32_t ld_out, int32_t width, void* stream) {

@@ -303,25 +303,50 @@ rowwise_backward_kernel(const float* __restrict__ dy, int ld_dy, const float* __
 }
 
 // ---- tangent-linear model ------------------------------------------------------------------------
+// The LayerNorm tangent of one row (n = 512, lane owns columns lane + 32 j) from zhat v, rstd and the
+// row sums md_sum = sum dz and mdz_sum = sum zhat * dz:
+//   out = [residual +] scale * (rstd * (dz - md_sum / n - zhat * (mdz_sum / n)))
+// with every rounding pinned by an intrinsic, so that each kernel applying it gives the same bits.  The
+// roundings are those layernorm_jvp_kernel was first compiled to, which input_jvp's results have been
+// since: md_sum / n folded into one fma with dz, mdz_sum / n rounded once, and the residual of column
+// 0 (j = 0) added to the rounded product, that of every other column fused with it into one fma.
+__device__ __forceinline__ void ln_jvp_apply(const float (&d)[16], const float (&v)[16], float rstd,
+                                             float md_sum, float mdz_sum, const float (&sc)[16],
+                                             const float* __restrict__ res_row, float* __restrict__ out_row,
+                                             int lane) {
+  const float mdz = __fmul_rn(mdz_sum, 1.0f / 512);
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int c = lane + 32 * j;
+    const float t = __fmul_rn(rstd, __fmaf_rn(v[j], -mdz, __fmaf_rn(md_sum, -1.0f / 512, d[j])));
+    float o;
+    if (!res_row) o = __fmul_rn(t, sc[j]);
+    else if (j == 0) o = __fadd_rn(__fmul_rn(t, sc[j]), res_row[c]);
+    else o = __fmaf_rn(t, sc[j], res_row[c]);
+    out_row[c] = o;
+  }
+}
+
 // Tangent of hk.LayerNorm at the pre-LayerNorm z along dz, one warp per row of n = 512 (lane owns
 // columns lane + 32 j), 8 rows per block:
 //   out = (residual ? residual : 0) + scale * (rstd * (dz - mean(dz) - zhat * mean(zhat * dz)))
 // zhat = (z - mu) * rstd, mu and rstd from ln_row_stats as rowwise_backward_kernel forms them.  The
 // Jacobian is symmetric, so with unit scale this is that kernel's dz for dy = dz.  Row-wise: no column
-// sums, no atomics.
+// sums, no atomics.  The output arithmetic is ln_jvp_apply.
 __global__ void __launch_bounds__(256)
 layernorm_jvp_kernel(const float* __restrict__ z, int ld_z, const float* __restrict__ dz, int ld_dz,
                      const float* __restrict__ scale, long long rows, const float* __restrict__ residual,
                      int ld_res, float* __restrict__ out, int ld_out) {
-  constexpr int kCols = 16, n = 512;
+  constexpr int kCols = 16;
   const int lane = threadIdx.x & 31;
   const long long r = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
   if (r >= rows) return;
-  float v[kCols], d[kCols];
+  float v[kCols], d[kCols], sc[kCols];
 #pragma unroll
   for (int j = 0; j < kCols; ++j) {
     v[j] = z[r * ld_z + lane + 32 * j];
     d[j] = dz[r * ld_dz + lane + 32 * j];
+    sc[j] = scale[lane + 32 * j];
   }
   float mean, rstd;
   ln_row_stats<kCols>(v, mean, rstd);
@@ -337,14 +362,82 @@ layernorm_jvp_kernel(const float* __restrict__ z, int ld_z, const float* __restr
     md += __shfl_xor_sync(0xffffffffu, md, o);
     mdz += __shfl_xor_sync(0xffffffffu, mdz, o);
   }
-  md *= (1.0f / n);
-  mdz *= (1.0f / n);
+  ln_jvp_apply(d, v, rstd, md, mdz, sc, residual ? residual + r * ld_res : nullptr, out + r * ld_out,
+               lane);
+}
+
+// ---- several tangent directions (batched_input_jvp) -----------------------------------------------
+// The tangent tables of `dirs` directions are stacked direction-major: row r of direction k is row
+// k * stride + r.  Each kernel reads the primal row once and applies it to the dirs tangent rows with,
+// per element, exactly the arithmetic of its one-direction counterpart, so every direction is bit for
+// bit what that kernel gives it alone.
+
+// da[k] = swish'(h) * dh[k], swish'(h) = sg * (1 + h * (1 - sg)), sg = 1 / (1 + exp(-h)): the dz of
+// rowwise_backward_kernel<kRowSwish> without its column sums.  One thread per 4 columns of a row; da
+// may alias dh (each thread reads its dh before it writes the same da).
+__global__ void __launch_bounds__(256)
+swish_jvp_kernel(const float* __restrict__ h, int ld_h, long long rows, int n4,
+                 const float* dh, int ld_dh, long long stride, int dirs, float* da, int ld_da) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= rows * n4) return;
+  const long long r = i / n4;
+  const int c = static_cast<int>(i - r * n4) * 4;
+  const float4 hv = *reinterpret_cast<const float4*>(h + r * ld_h + c);
+  const float hq[4] = {hv.x, hv.y, hv.z, hv.w};
+  float f[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float sg = 1.0f / (1.0f + expf(-hq[q]));
+    f[q] = sg * (1.0f + hq[q] * (1.0f - sg));
+  }
+  for (int k = 0; k < dirs; ++k) {
+    const long long rk = k * stride + r;
+    const float4 d = *reinterpret_cast<const float4*>(dh + rk * ld_dh + c);
+    *reinterpret_cast<float4*>(da + rk * ld_da + c) =
+        make_float4(d.x * f[0], d.y * f[1], d.z * f[2], d.w * f[3]);
+  }
+}
+
+// layernorm_jvp_kernel for dirs directions: the statistics and zhat of z's row once, then per direction
+//   out[k] = (residual ? residual[k] : 0) + scale * (rstd * (dz[k] - mean(dz[k]) - zhat * mean(zhat * dz[k])))
+// One warp per row of n = 512, 8 rows per block.
+__global__ void __launch_bounds__(256)
+layernorm_jvp_dirs_kernel(const float* __restrict__ z, int ld_z, const float* __restrict__ dz,
+                          int ld_dz, const float* __restrict__ scale, long long rows, long long stride,
+                          int dirs, const float* __restrict__ residual, int ld_res,
+                          float* __restrict__ out, int ld_out) {
+  constexpr int kCols = 16;
+  const int lane = threadIdx.x & 31;
+  const long long r = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  if (r >= rows) return;
+  float v[kCols], sc[kCols];
 #pragma unroll
   for (int j = 0; j < kCols; ++j) {
-    const int c = lane + 32 * j;
-    float o = scale[c] * (rstd * (d[j] - md - v[j] * mdz));
-    if (residual) o = residual[r * ld_res + c] + o;
-    out[r * ld_out + c] = o;
+    v[j] = z[r * ld_z + lane + 32 * j];
+    sc[j] = scale[lane + 32 * j];
+  }
+  float mean, rstd;
+  ln_row_stats<kCols>(v, mean, rstd);
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) v[j] = (v[j] - mean) * rstd;     // z-hat
+  for (int k = 0; k < dirs; ++k) {
+    const long long rk = k * stride + r;
+    float d[kCols];
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) d[j] = dz[rk * ld_dz + lane + 32 * j];
+    float md = 0.f, mdz = 0.f;
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) {
+      md += d[j];
+      mdz += d[j] * v[j];
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      md += __shfl_xor_sync(0xffffffffu, md, o);
+      mdz += __shfl_xor_sync(0xffffffffu, mdz, o);
+    }
+    ln_jvp_apply(d, v, rstd, md, mdz, sc, residual ? residual + rk * ld_res : nullptr,
+                 out + rk * ld_out, lane);
   }
 }
 

@@ -801,7 +801,7 @@ class Engine:
           dx.data_ptr(), dx.shape[1], self.num_grid, fb.n_rows, fb.rows.data_ptr(),
           self._ptr(fb.in_scale), a_out.data_ptr(), 1, self._stream()), "gcb_input_grad")
 
-  # -- tangent-linear model (input_jvp) -----------------------------------------------------------------
+  # -- tangent-linear model (input_jvp, batched_input_jvp) --------------------------------------------
   def input_jvp_element(self, tangent_planes: torch.Tensor, tangent_out: torch.Tensor, *,
                         in_scale: Optional[torch.Tensor] = None,
                         planes_out: Optional[torch.Tensor] = None,
@@ -809,37 +809,48 @@ class Engine:
     """One step of one batch element of the tangent-linear forecast (call input_grads_begin() first):
     the step stage by stage from `grid_in` (default: the packed grid_in_img) interleaved with its
     tangent (Backward.tangent) along tangent_planes [c_in, Ng], the tangent of this step's input planes
-    in physical units.  They are packed as pack_inputs packs the planes, without the mean (in_scale:
-    the input normalisation's scale) and with zero structural features.  tangent_out [n_out, Ng]
-    receives the tangent of the physical predictions: the decoder tangent times affine["scale"] plus,
-    through the residual add, tangent_planes[affine["add_plane_index"]] (gcb_unpack_grid_outputs
-    without the offset).  With planes_out, the predictions as unpack_outputs gives them from the same
+    in physical units, or along several directions at once, tangent_planes [K, c_in, Ng] (each
+    direction's planes contiguous).  They are packed as pack_inputs packs the planes, without the mean
+    (in_scale: the input normalisation's scale) and with zero structural features, each direction into
+    its slice of one stacked image.  tangent_out [n_out, Ng] ([K, n_out, Ng]) receives the tangent of
+    the physical predictions: the decoder tangent times affine["scale"] plus, through the residual add,
+    tangent_planes[affine["add_plane_index"]] (gcb_unpack_grid_outputs without the offset), unpacked
+    per direction.  With planes_out, the predictions as unpack_outputs gives them from the same
     forward.  `affine`: the keywords of unpack_outputs (scale, offset, add_planes, add_plane_index)."""
     if self._backward is None:
       raise RuntimeError("call input_grads_begin() first")
+    single = tangent_planes.dim() == 2
+    dirs = 1 if single else tangent_planes.shape[0]
     for name, t, rows in (("tangent_planes", tangent_planes, self.c_in),
                           ("tangent_out", tangent_out, self.n_out)):
-      if (tuple(t.shape) != (rows, self.num_grid) or t.dtype != torch.float32
-          or not t.is_contiguous() or t.device != self.device):
-        raise ValueError(f"{name} must be a contiguous float32 [{rows}, {self.num_grid}] tensor on "
-                         f"{self.device}")
+      lead = () if single else (dirs,)
+      if (tuple(t.shape) != lead + (rows, self.num_grid) or t.dtype != torch.float32
+          or t.stride()[-2:] != (self.num_grid, 1) or t.device != self.device or dirs < 1):
+        raise ValueError(f"{name} must be a float32 {list(lead + (rows, self.num_grid))} tensor on "
+                         f"{self.device} with contiguous [{rows}, {self.num_grid}] planes per direction")
+    planes = [tangent_planes] if single else list(tangent_planes.unbind(0))
+    outs = [tangent_out] if single else list(tangent_out.unbind(0))
     grid_in = self.grid_in_img if grid_in is None else grid_in
-    dgrid_in = self._image(self.num_grid, self.c_in_pad)
+    stride = self._backward.dir_stride(self.num_grid)
+    dgrid_in = self._image((dirs - 1) * stride + self.num_grid, self.c_in_pad)
+    img_stride = self._lib.gcb_a_image_bytes(stride, self.c_in_pad)
     no_static = torch.zeros([self.num_grid, 3], dtype=torch.float32, device=self.device)
     add_index = affine.get("add_plane_index")
     with self._on_device():
-      _native.check(self._lib.gcb_pack_grid_image(
-          tangent_planes.data_ptr(), self.c_in, self.num_grid, None, self._ptr(in_scale),
-          no_static.data_ptr(), 3, self.c_in_pad, dgrid_in.data_ptr(), self._stream()),
-          "gcb_pack_grid_image")
-      dy = self._backward.tangent(grid_in, dgrid_in)
+      for k, p in enumerate(planes):
+        _native.check(self._lib.gcb_pack_grid_image(
+            p.data_ptr(), self.c_in, self.num_grid, None, self._ptr(in_scale), no_static.data_ptr(), 3,
+            self.c_in_pad, dgrid_in.data_ptr() + k * img_stride, self._stream()),
+            "gcb_pack_grid_image")
+      dy = self._backward.tangent(grid_in, dgrid_in, dirs)
       del dgrid_in
       if planes_out is not None:
         self.unpack_outputs(planes_out, **affine)
-      _native.check(self._lib.gcb_unpack_grid_outputs(
-          dy.data_ptr(), dy.shape[1], self.n_out, self.num_grid, self._ptr(affine.get("scale")), None,
-          None if add_index is None else tangent_planes.data_ptr(), self._ptr(add_index),
-          tangent_out.data_ptr(), self._stream()), "gcb_unpack_grid_outputs")
+      for k, (p, out) in enumerate(zip(planes, outs)):
+        _native.check(self._lib.gcb_unpack_grid_outputs(
+            dy[k * stride:].data_ptr(), dy.shape[1], self.n_out, self.num_grid,
+            self._ptr(affine.get("scale")), None, None if add_index is None else p.data_ptr(),
+            self._ptr(add_index), out.data_ptr(), self._stream()), "gcb_unpack_grid_outputs")
 
   def broadcast_grad_sum(self, a: torch.Tensor, n_lat: int, rows: torch.Tensor, mode: int,
                          out: torch.Tensor, accumulate: bool) -> None:

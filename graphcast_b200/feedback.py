@@ -155,15 +155,28 @@ class FeedbackPlan:
     out[self.dpred_row[c]] = c
     return out
 
-  def feed_index(self) -> np.ndarray:
+  def feed_index(self, directions: int = 1) -> np.ndarray:
     """[n_in] int32: the row of [this step's planes (c_in rows) | its predictions (n_out rows)] that
     becomes input channel j of the next step (next_from_input, else c_in + next_from_pred).  The
     forcings slab, channels n_in.., is the next target time's, given.  The gather index of the tangent
-    feed between the steps of input_jvp."""
+    feed between the steps of input_jvp.
+
+    directions > 1: the K-fold index of the feed of that many directions at once (batched_input_jvp),
+    whose buffer stacks them as [directions, c_in + n_out] rows.  Direction k's first n_in rows read
+    feed_index() + k (c_in + n_out); the rows between them (the forcings slab and the predictions of
+    every direction but the last) are copied through unchanged, as the next step overwrites them:
+    [(directions - 1) (c_in + n_out) + n_in] in all, so that one gather feeds every direction."""
     src, pred = self.next_from_input[:self.n_in], self.next_from_pred[:self.n_in]
     if not np.all((src >= 0) | (pred >= 0)):
       raise ValueError("an input channel is neither carried nor predicted")
-    return np.where(src >= 0, src, self.c_in + pred).astype(np.int32)
+    one = np.where(src >= 0, src, self.c_in + pred).astype(np.int32)
+    if directions == 1:
+      return one
+    width = self.c_in + self.n_out
+    out = np.arange((directions - 1) * width + self.n_in, dtype=np.int32)
+    for k in range(directions):
+      out[k * width:k * width + self.n_in] = one + k * width
+    return out
 
   def next_planes(self, planes: np.ndarray, predictions: np.ndarray,
                   next_forcings: np.ndarray) -> np.ndarray:
@@ -239,29 +252,80 @@ def variable_rows(inputs: xs.Dataset, forcings: xs.Dataset) -> list:
           [VariableRows(s, forcings.data_vars[s.name], True) for s in f_slabs])
 
 
-def check_tangents(tangents: Optional[xs.Dataset], like: xs.Dataset, what: str) -> None:
+DIRECTION = "direction"
+
+
+def check_tangents(tangents: Optional[xs.Dataset], like: xs.Dataset, what: str,
+                   directions: bool = False) -> Optional[int]:
   """ValueError unless every variable of `tangents` (None: none) has a namesake in `like` with the
-  same dims, in any order, and the same sizes."""
+  same dims, in any order, and the same sizes.  With `directions`, every variable instead has a leading
+  "direction" dim followed by those dims, of one size K >= 1 for all of them; returns K (None for no
+  variables)."""
   if tangents is None:
-    return
+    return None
+  dirs = None
   for name in sorted(tangents.keys()):
     if name not in like.data_vars:
       raise ValueError(f"{what}: unknown variable {name!r}, expected one of {sorted(like.keys())}")
     v, ref = tangents.data_vars[name], like.data_vars[name]
+    if directions:
+      if not v.dims or v.dims[0] != DIRECTION:
+        raise ValueError(f"{what}: {name} has dims {tuple(v.dims)}; a tangent of several directions "
+                         f"needs the leading dim {DIRECTION!r}")
+      k = v.shape[0]
+      if k < 1:
+        raise ValueError(f"{what}: {name} has no directions")
+      if dirs is not None and k != dirs:
+        raise ValueError(f"{what}: {name} has {k} directions, other variables {dirs}")
+      dirs = k
+      v = v.isel({DIRECTION: 0})
     if set(v.dims) != set(ref.dims) or tuple(v.transpose(*ref.dims).shape) != tuple(ref.shape):
       raise ValueError(f"{what}: {name} has dims {tuple(v.dims)} and shape {tuple(v.shape)}, the "
                        f"variable {tuple(ref.dims)} and {tuple(ref.shape)}")
+  return dirs
+
+
+def check_direction_tangents(input_tangents: Optional[xs.Dataset], inputs: xs.Dataset,
+                             forcing_tangents: Optional[xs.Dataset], forcings: xs.Dataset):
+  """(K, direction labels) of the tangents of a batched_input_jvp, after check_tangents(directions=True)
+  of both Datasets: ValueError unless they agree on K and have at least one variable.  The labels are
+  input_tangents' "direction" coordinate when it has one, else 0..K-1."""
+  k_in = check_tangents(input_tangents, inputs, "input_tangents", directions=True)
+  k_f = check_tangents(forcing_tangents, forcings, "forcing_tangents", directions=True)
+  if k_in is not None and k_f is not None and k_in != k_f:
+    raise ValueError(f"input_tangents have {k_in} directions, forcing_tangents {k_f}")
+  dirs = k_in if k_in is not None else k_f
+  if dirs is None:
+    raise ValueError("the tangents have no variables, so no direction dim: give at least one")
+  labels = np.arange(dirs)
+  coord = None if input_tangents is None else input_tangents.coords.get(DIRECTION)
+  if coord is not None and coord[0] == (DIRECTION,) and np.asarray(coord[1]).shape == (dirs,):
+    labels = np.asarray(coord[1])
+  return dirs, labels
 
 
 def tangent_planes(tangents: Optional[xs.Dataset], like: xs.Dataset,
-                   sizes: dict) -> np.ndarray:
+                   sizes: dict, directions: Optional[int] = None) -> np.ndarray:
   """[batch, channels, lat * lon] float32 planes of a tangent Dataset (check_tangents), packed exactly
   as GraphCast stages `like`: channel_layout(like) order, model_utils.variable_to_planes broadcasting
   a variable over the batch, lat and lon it lacks.  Variables `tangents` leaves out (all of them for
-  None) get zero planes."""
+  None) get zero planes.  With `directions` = K (a Dataset of check_tangents(directions=True)):
+  [K, batch, channels, lat * lon], direction k packed as the Dataset's slice k alone would be."""
   batch, n_lat, n_lon = sizes["batch"], sizes["lat"], sizes["lon"]
   slabs = model_utils.channel_layout(like)
-  out = np.zeros([batch, sum(s.count for s in slabs), n_lat * n_lon], np.float32)
+  lead = () if directions is None else (directions,)
+  out = np.zeros(lead + (batch, sum(s.count for s in slabs), n_lat * n_lon), np.float32)
+  if directions is None:
+    _fill_planes(tangents, like, sizes, slabs, out)
+  else:                                           # each direction packed in place, no stacking copy
+    for k in range(directions):
+      _fill_planes(None if tangents is None else tangents.isel({DIRECTION: k}), like, sizes, slabs,
+                   out[k])
+  return out
+
+
+def _fill_planes(tangents, like, sizes, slabs, out: np.ndarray) -> None:
+  batch, n_lat, n_lon = sizes["batch"], sizes["lat"], sizes["lon"]
   for s in slabs:
     if tangents is None or s.name not in tangents.data_vars:
       continue
@@ -270,7 +334,6 @@ def tangent_planes(tangents: Optional[xs.Dataset], like: xs.Dataset,
     p = p.detach().cpu().numpy() if xs._is_torch(p) else np.asarray(p)
     out[:, s.start:s.start + s.count] = np.broadcast_to(
         p, (batch, s.count, n_lat, n_lon)).reshape(batch, s.count, n_lat * n_lon)
-  return out
 
 
 def grads_to_datasets(rows: list, grads: dict, inputs: xs.Dataset, forcings: xs.Dataset,

@@ -126,6 +126,13 @@ class Predictor(abc.ABC):
     like its namesake; a variable left out is held fixed), shaped like the predictions."""
     raise NotImplementedError(f"{type(self).__name__} does not implement input gradients")
 
+  def batched_input_jvp(self, inputs, targets_template, forcings, input_tangents,
+                        forcing_tangents=None, *, directions_per_pass=None, **optional_kwargs):
+    """Returns (predictions, prediction_tangents): input_jvp along K tangent directions at once, the
+    tangent Datasets' variables carrying a leading "direction" dim of size K; prediction_tangents has
+    the same leading dim.  directions_per_pass: directions that share one forward (None: all)."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement input gradients")
+
 
 # Per-variable weights of GraphCast's loss (reference graphcast.py:341-356); others weigh 1.
 LOSS_PER_VARIABLE_WEIGHTS = {
@@ -343,15 +350,43 @@ class GraphCast(Predictor):
                                   forcing_tangents)
     return self._input_jvp(inputs, targets_template, forcings, run, norm=None)
 
+  def batched_input_jvp(self, inputs, targets_template, forcings, input_tangents,
+                        forcing_tangents=None, *, directions_per_pass=None, **unused_kwargs):
+    """(predictions, prediction_tangents) of input_jvp along K tangent directions at once, for one
+    target time: what jax.vmap of jax.jvp over the directions gives.
+
+    Every variable of input_tangents / forcing_tangents has a leading "direction" dim of size K >= 1,
+    followed by its namesake's dims and shape; a variable left out (every forcing for
+    forcing_tangents=None) is held fixed in every direction.  A missing direction dim, K differing
+    between variables or Datasets, an unknown variable or a wrong shape raise ValueError before anything
+    runs, and every refusal of input_jvp applies.  `predictions` is what __call__ returns, bit for bit;
+    `prediction_tangents` (float32) has a leading "direction" dim followed by the predictions' dims, its
+    coordinate input_tangents' "direction" coordinate when it has one, else 0..K-1.  Direction k is
+    bit for bit input_jvp along direction k alone, for any K and directions_per_pass.
+
+    The directions share one stage-wise forward: their tangent state is stacked direction-major
+    (Backward.tangent), so every tangent GEMM streams its weights once for all of them and every MLP's
+    h and z are recomputed once.  directions_per_pass = g (None: K) runs ceil(K / g) such passes, for
+    memory.  Measured on an 80 GB H100 (DESIGN.md section 8): at 0.25 degree / 37 levels a pass peaks
+    at 57.4 GiB for one direction and 68.7-69.6 GiB for two, 11.3-12.2 GiB per direction, so at most
+    2 directions fit per pass; at 1 degree / 13 levels 16 directions peak at 17.6 GiB (T = 4), about
+    0.8 GiB per direction, so about 90 fit."""
+    def one_pass(it, ft):
+      run = self._one_step_tangents(inputs, targets_template, forcings, it, ft, directions=True)
+      return self._input_jvp(inputs, targets_template, forcings, run, norm=None)
+    return batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
+                       directions_per_pass)
+
   @staticmethod
   def _one_step_tangents(inputs, targets_template, forcings, input_tangents,
-                         forcing_tangents) -> "_TangentRun":
-    """The checked and packed tangents of an input_jvp of one target time."""
+                         forcing_tangents, directions: bool = False) -> "_TangentRun":
+    """The checked and packed tangents of an input_jvp (with `directions`: batched_input_jvp) of one
+    target time."""
     if xs.from_xarray(targets_template).sizes.get("time", 1) != 1:
       raise NotImplementedError("input_jvp of GraphCast covers one target time (several: "
                                 "autoregressive.Predictor)")
     return _TangentRun(xs.from_xarray(inputs), xs.from_xarray(forcings), input_tangents,
-                       forcing_tangents, num_steps=1)
+                       forcing_tangents, num_steps=1, directions=directions)
 
   def _input_jvp(self, inputs, targets_template, forcings, run: "_TangentRun",
                  norm: Optional[FusedNormalization]):
@@ -367,13 +402,17 @@ class GraphCast(Predictor):
       if "out" not in state:
         eng.input_grads_begin()
         self._release_idle_staging()
-        state["out"] = torch.empty([run.batch, eng.n_out, eng.num_grid], dtype=torch.float32,
-                                   device=eng.device)
-      run.element(eng, b, state["out"][b], planes_out, norm, affine)
+        state["out"] = torch.empty([run.dirs, run.batch, eng.n_out, eng.num_grid],
+                                   dtype=torch.float32, device=eng.device)
+      run.element(eng, b, state["out"][:, b], planes_out, norm, affine)
 
     predictions = self._call(inputs, targets_template, forcings, norm=norm, element=element)
     run.step += 1
-    return predictions, self._planes_to_dataset(state["out"], targets_template, run.n_lat, run.n_lon)
+    if not run.directions:
+      return predictions, self._planes_to_dataset(state["out"][0], targets_template, run.n_lat,
+                                                  run.n_lon)
+    return predictions, self._planes_to_dataset(state["out"], targets_template, run.n_lat, run.n_lon,
+                                                directions=run.labels)
 
   def _loss_and_input_grads(self, inputs, targets, forcings, norm: Optional[FusedNormalization]):
     inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
@@ -766,16 +805,49 @@ class GraphCast(Predictor):
     return slabs
 
   def _planes_to_dataset(self, planes_out: torch.Tensor, template: xs.Dataset,
-                         n_lat: int, n_lon: int) -> xs.Dataset:
-    slabs = self._check_template(template, planes_out.shape[1])
-    batch = planes_out.shape[0]
+                         n_lat: int, n_lon: int, directions=None) -> xs.Dataset:
+    """planes_out [batch, n_out, Ng] -> a Dataset shaped like `template`.  With `directions` (labels),
+    planes_out [K, batch, n_out, Ng] -> variables with a leading "direction" dim, labelled so."""
+    lead, lead_dims = planes_out.shape[:-2], ("batch",)
+    if directions is not None:
+      lead_dims = (feedback.DIRECTION, "batch")
+    slabs = self._check_template(template, planes_out.shape[-2])
     out = xs.Dataset(coords=template.coords)
+    if directions is not None:
+      out.coords[feedback.DIRECTION] = ((feedback.DIRECTION,), np.asarray(directions))
     for s in slabs:
-      piece = planes_out[:, s.start:s.start + s.count]
-      piece = piece.reshape((batch,) + s.stack_sizes + (n_lat, n_lon))
-      da = xs.DataArray(piece, ("batch",) + s.stack_dims + ("lat", "lon"))
-      out[s.name] = da.transpose(*s.var_dims)
+      piece = planes_out[..., s.start:s.start + s.count, :]
+      piece = piece.reshape(tuple(lead) + s.stack_sizes + (n_lat, n_lon))
+      da = xs.DataArray(piece, lead_dims + s.stack_dims + ("lat", "lon"))
+      out[s.name] = da.transpose(*lead_dims[:-1], *s.var_dims)
     return out
+
+
+def batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents, directions_per_pass):
+  """batched_input_jvp of a predictor stack: checks the tangents (feedback.check_direction_tangents)
+  and directions_per_pass before anything runs, then runs one_pass(input_tangents, forcing_tangents)
+  -> (predictions, prediction_tangents) on ceil(K / directions_per_pass) consecutive slices of the
+  directions and joins the tangents along "direction".  The predictions are those of the first pass."""
+  inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
+  it = None if input_tangents is None else xs.from_xarray(input_tangents)
+  ft = None if forcing_tangents is None else xs.from_xarray(forcing_tangents)
+  dirs, labels = feedback.check_direction_tangents(it, inputs, ft, forcings)
+  per = dirs if directions_per_pass is None else directions_per_pass
+  if isinstance(per, bool) or not isinstance(per, (int, np.integer)) or per < 1:
+    raise ValueError(f"directions_per_pass must be None or an int >= 1, not {directions_per_pass!r}")
+  at = lambda ds, sl: None if ds is None else ds.isel({feedback.DIRECTION: sl})
+  predictions, parts = None, []
+  for k0 in range(0, dirs, int(per)):
+    sl = slice(k0, min(k0 + int(per), dirs))
+    p, t = one_pass(at(it, sl), at(ft, sl))
+    predictions = p if predictions is None else predictions
+    parts.append(t)
+  out = xs.Dataset(coords=parts[0].coords)
+  out.coords[feedback.DIRECTION] = ((feedback.DIRECTION,), np.asarray(labels))
+  for name, v in parts[0].data_vars.items():
+    data = v.data if len(parts) == 1 else torch.cat([t.data_vars[name].data for t in parts], dim=0)
+    out[name] = xs.DataArray(data, v.dims)
+  return predictions, out
 
 
 def innermost_graphcast(predictor) -> Optional[GraphCast]:
@@ -913,63 +985,78 @@ class _InputGradRun:
 
 
 class _TangentRun:
-  """The tangent planes of one input_jvp call (GraphCast._input_jvp, autoregressive.Predictor
-  .input_jvp).  The tangent Datasets are checked and packed into host planes on construction, before
-  anything runs on the device.  Per batch element a device buffer [c_in + n_out, Ng] holds the tangent
-  of the current step's input planes in its first c_in rows.  After a step that has a successor, the
-  prediction tangents are copied into its last n_out rows and the next step's first n_in rows are
-  gathered from the buffer by FeedbackPlan.feed_index (gcb_gather_rows: every such row is a copy of one
-  row of the two sources); the forcings slab comes from the forcing tangents of that target time.  The
-  tangent planes stay on the device from step to step, and nothing is kept per step."""
+  """The tangent planes of one input_jvp or batched_input_jvp call (GraphCast._input_jvp,
+  autoregressive.Predictor.input_jvp).  The tangent Datasets are checked and packed into host planes
+  on construction, before anything runs on the device.  Per batch element a device buffer [dirs,
+  c_in + n_out, Ng] holds the tangent of the current step's input planes of every direction in its
+  first c_in rows (dirs = 1 for input_jvp, K with `directions`).  After a step that has a successor,
+  the prediction tangents are copied into the last n_out rows and the next step's first n_in rows of
+  every direction are gathered from the buffer by one gcb_gather_rows with FeedbackPlan.feed_index
+  (dirs) (every such row is a copy of one row of the two sources); the forcings slab comes from the
+  forcing tangents of that target time.  The tangent planes stay on the device from step to step, and
+  nothing is kept per step."""
 
   def __init__(self, inputs: xs.Dataset, forcings: xs.Dataset, input_tangents, forcing_tangents,
-               num_steps: int, plan=None):
+               num_steps: int, plan=None, directions: bool = False):
     input_tangents = None if input_tangents is None else xs.from_xarray(input_tangents)
     forcing_tangents = None if forcing_tangents is None else xs.from_xarray(forcing_tangents)
-    feedback.check_tangents(input_tangents, inputs, "input_tangents")
-    feedback.check_tangents(forcing_tangents, forcings, "forcing_tangents")
+    self.directions = directions
+    if directions:
+      self.dirs, self.labels = feedback.check_direction_tangents(input_tangents, inputs,
+                                                                 forcing_tangents, forcings)
+    else:
+      feedback.check_tangents(input_tangents, inputs, "input_tangents")
+      feedback.check_tangents(forcing_tangents, forcings, "forcing_tangents")
+      self.dirs, self.labels = 1, None
     self.batch = dict(inputs.sizes).get("batch", 1)
     self.n_lat, self.n_lon = inputs.sizes["lat"], inputs.sizes["lon"]
     self.sizes = {"batch": self.batch, "lat": self.n_lat, "lon": self.n_lon}
     if num_steps > 1 and (self.n_lat * self.n_lon) % 4:
       raise NotImplementedError("input_jvp over several target times needs a multiple of 4 grid "
                                 "nodes (the tangent feed gathers 16-byte rows)")
-    self.input_planes = torch.from_numpy(feedback.tangent_planes(input_tangents, inputs, self.sizes))
+    self.input_planes = self._planes(input_tangents, inputs)
     self.forcings, self.forcing_tangents = forcings, forcing_tangents
     self.num_steps, self.step = num_steps, 0
-    self.feed = None if plan is None else torch.from_numpy(plan.feed_index())
+    self.feed = None if plan is None else torch.from_numpy(plan.feed_index(self.dirs))
     self.carry = [None] * self.batch
     self._slab = (-1, None)
 
+  def _planes(self, tangents, like) -> torch.Tensor:
+    """[dirs, batch, channels, Ng] host planes of a tangent Dataset (feedback.tangent_planes)."""
+    if self.directions:
+      return torch.from_numpy(feedback.tangent_planes(tangents, like, self.sizes, self.dirs))
+    return torch.from_numpy(feedback.tangent_planes(tangents, like, self.sizes)).unsqueeze(0)
+
   def _forcing_planes(self, t: int) -> torch.Tensor:
-    """[batch, c_in - n_in, Ng] host tangent planes of the forcings of target time t."""
+    """[dirs, batch, c_in - n_in, Ng] host tangent planes of the forcings of target time t."""
     if self._slab[0] != t:
       at = lambda ds: ds.isel(time=slice(t, t + 1)) if "time" in ds.sizes else ds
       tangents = None if self.forcing_tangents is None else at(self.forcing_tangents)
-      self._slab = (t, torch.from_numpy(feedback.tangent_planes(tangents, at(self.forcings),
-                                                                self.sizes)))
+      self._slab = (t, self._planes(tangents, at(self.forcings)))
     return self._slab[1]
 
   def element(self, eng, b: int, tangent_out: torch.Tensor, planes_out: Optional[torch.Tensor],
               norm: Optional[FusedNormalization], affine: dict) -> None:
-    """This step of batch element b: Engine.input_jvp_element, then the feed of the next step."""
-    c_in, n_in, ng = eng.c_in, self.input_planes.shape[1], eng.num_grid
+    """This step of batch element b (tangent_out [dirs, n_out, Ng]): Engine.input_jvp_element, then the
+    feed of the next step."""
+    c_in, n_in, ng = eng.c_in, self.input_planes.shape[2], eng.num_grid
     buf, self.carry[b] = self.carry[b], None
     if buf is None:
-      buf = torch.empty([c_in + eng.n_out, ng], dtype=torch.float32, device=eng.device)
-      buf[:n_in].copy_(self.input_planes[b])
-    buf[n_in:c_in].copy_(self._forcing_planes(self.step)[b])
-    eng.input_jvp_element(buf[:c_in], tangent_out, in_scale=None if norm is None else norm.in_scale,
-                          planes_out=planes_out, **affine)
+      buf = torch.empty([self.dirs, c_in + eng.n_out, ng], dtype=torch.float32, device=eng.device)
+      buf[:, :n_in].copy_(self.input_planes[:, b])
+    buf[:, n_in:c_in].copy_(self._forcing_planes(self.step)[:, b])
+    eng.input_jvp_element(buf[:, :c_in], tangent_out,
+                          in_scale=None if norm is None else norm.in_scale, planes_out=planes_out,
+                          **affine)
     if self.step + 1 < self.num_steps:
       if self.feed.device != eng.device:
         self.feed = self.feed.to(eng.device)
-      buf[c_in:].copy_(tangent_out)
+      buf[:, c_in:].copy_(tangent_out)
       nxt = torch.empty_like(buf)
       with eng._on_device():
-        _native.check(eng._lib.gcb_gather_rows(buf.data_ptr(), ng, self.feed.data_ptr(), n_in,
-                                               nxt.data_ptr(), ng, ng, eng._stream()),
-                      "gcb_gather_rows")
+        _native.check(eng._lib.gcb_gather_rows(buf.data_ptr(), ng, self.feed.data_ptr(),
+                                               self.feed.shape[0], nxt.data_ptr(), ng, ng,
+                                               eng._stream()), "gcb_gather_rows")
       self.carry[b] = nxt
 
 

@@ -281,6 +281,18 @@ class InputsAndResiduals(graphcast.Predictor):
                                                                  "input gradients")
     return self._predictor._input_jvp(inputs, targets_template, forcings, run, norm=consts)
 
+  def batched_input_jvp(self, inputs, targets_template, forcings, input_tangents,
+                        forcing_tangents=None, *, directions_per_pass=None, **kwargs):
+    """input_jvp along K tangent directions at once (GraphCast.batched_input_jvp), through the
+    normalisation of the inputs and the residual add.  GraphCast only."""
+    def one_pass(it, ft):
+      run = graphcast.GraphCast._one_step_tangents(inputs, targets_template, forcings, it, ft,
+                                                   directions=True)
+      ins, tt, fs, consts = self._fused_for(inputs, targets_template, forcings, "input gradients")
+      return self._predictor._input_jvp(ins, tt, fs, run, norm=consts)
+    return graphcast.batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
+                                 directions_per_pass)
+
   def loss(self, inputs, targets, forcings, **kwargs):
     """The loss computed on normalised inputs and targets (targets that are also inputs as
     normalised residuals against the last input frame)."""

@@ -415,6 +415,23 @@ int gcb_layernorm_jvp(const float* z, int32_t ld_z, const float* dz, int32_t ld_
                       int64_t rows, int32_t n, const float* residual, int32_t ld_res, float* out,
                       int32_t ld_out, void* stream);
 
+/* Several tangent directions at one primal (GraphCast.batched_input_jvp).  The tangent operands hold
+ * `dirs` (>= 1) tables of `rows` rows stacked direction-major: row r of direction k is row
+ * k * dir_stride + r (dir_stride >= rows; ignored for dirs = 1).  The primal row is read once and
+ * applied to every direction, with per element exactly the arithmetic of the one-direction kernel, so
+ * each direction is bit for bit what that kernel gives it alone.  Row-wise, deterministic.
+ *
+ * gcb_swish_jvp: da[k] = swish'(h) * dh[k], the dh of gcb_swish_backward (its argument da being
+ * dh[k] here) without the column sums.  n a multiple of 4, 16-byte rows; da may alias dh.
+ * gcb_layernorm_jvp_dirs: out[k] = gcb_layernorm_jvp(z, dz[k], scale, residual[k]), the residual (may be
+ * NULL) stacked like dz; out may not alias z, dz or residual. */
+int gcb_swish_jvp(const float* h, int32_t ld_h, int64_t rows, int32_t n, const float* dh, int32_t ld_dh,
+                  int64_t dir_stride, int32_t dirs, float* da, int32_t ld_da, void* stream);
+int gcb_layernorm_jvp_dirs(const float* z, int32_t ld_z, const float* dz, int32_t ld_dz,
+                           const float* scale, int64_t rows, int32_t n, int64_t dir_stride,
+                           int32_t dirs, const float* residual, int32_t ld_res, float* out,
+                           int32_t ld_out, void* stream);
+
 /* Backward of a gather v[senders] (jax_gather, utils/typed_graph_net.py:124-125,431-445):
  *   out[i, 0:512] = sum_{j in [ptr[i], ptr[i+1])} msg[order[j], 0:512]
  * (order / ptr: the sender CSR of an edge set, host-built), summed in j order; the rows listed in
@@ -659,7 +676,7 @@ typedef enum {
                              * gcb_segment_sum_sorted, gcb_gather_add, gcb_swish_rows,
                              * gcb_output_loss_grad_feedback, gcb_input_grad,
                              * gcb_output_cotangent_grad_feedback, gcb_broadcast_grad_sum,
-                             * gcb_layernorm_jvp */
+                             * gcb_layernorm_jvp, gcb_swish_jvp, gcb_layernorm_jvp_dirs */
   GCB_KIND_NOISE = 11       /* gcb_add_gaussian_noise */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
