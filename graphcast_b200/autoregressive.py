@@ -319,6 +319,45 @@ class Predictor(graphcast.Predictor):
     if targets_template.sizes["time"] == 1:
       return self._predictor.input_vjp(inputs, targets_template, forcings, cotangents, **kwargs)
     model, norm_of = self._checkpointed_parts(inputs, targets_template, forcings, "input gradients")
+    predictions, stash, first, plan = self._vjp_forward(model, norm_of, inputs, targets_template,
+                                                        forcings)
+    cot = [model._cotangent_planes(cotangents.isel(time=slice(t, t + 1)), first["targets"],
+                                   stash.batch) for t in range(len(stash.steps))]
+    input_grads, forcing_grads = model._input_grads(stash, plan, first["norm"], inputs, forcings,
+                                                    cotangents=cot)
+    return predictions, input_grads, forcing_grads
+
+  def batched_input_vjp(self, inputs, targets_template, forcings, cotangents, *,
+                        directions_per_pass=None, **kwargs):
+    """input_vjp of K cotangents at once (GraphCast.batched_input_vjp), over every target time: each
+    variable of `cotangents` has a leading "direction" dim followed by the shape of its
+    targets_template namesake, and so do both gradient Datasets.  One target time delegates to the inner
+    predictor; several need gradient_checkpointing=True.  The checkpointed rollout forward runs once
+    per call and keeps every step's planes (graphcast.StepStash); each pass of directions_per_pass
+    directions (None: all) then differentiates every step from that stash, its cotangents sharing each
+    step's recompute and backward pass."""
+    inputs, targets_template = xs.from_xarray(inputs), xs.from_xarray(targets_template)
+    forcings, cotangents = xs.from_xarray(forcings), xs.from_xarray(cotangents)
+    if targets_template.sizes["time"] == 1:
+      return self._predictor.batched_input_vjp(inputs, targets_template, forcings, cotangents,
+                                               directions_per_pass=directions_per_pass, **kwargs)
+    model, norm_of = self._checkpointed_parts(inputs, targets_template, forcings, "input gradients")
+    state = {}
+
+    def one_pass(cot, first):
+      if not state:                        # the forward, once, after every check has passed
+        state["forward"] = self._vjp_forward(model, norm_of, inputs, targets_template, forcings)
+      predictions, stash, first, plan = state["forward"]
+      planes = [model._direction_cotangent_planes(cot.isel(time=slice(t, t + 1)), first["targets"],
+                                                  stash.batch) for t in range(len(stash.steps))]
+      return (predictions,) + model._input_grads(stash, plan, first["norm"], inputs, forcings,
+                                                 cotangents=planes, directions=True)
+    return graphcast.batched_vjp(one_pass, targets_template, cotangents, directions_per_pass)
+
+  def _vjp_forward(self, model, norm_of, inputs, targets_template, forcings):
+    """The forward of input_vjp over several target times: the rollout, keeping every step's input
+    planes in pinned host memory.  Returns (predictions, graphcast.StepStash, first step's {inputs,
+    targets, forcings, norm}, the all-channel feedback.FeedbackPlan)."""
     first = {}
     stash = None
 
@@ -335,13 +374,8 @@ class Predictor(graphcast.Predictor):
     chunks = list(rollout.chunked_prediction_generator(
         step, rng=None, inputs=inputs, targets_template=targets_template, num_steps_per_chunk=1,
         forcings=forcings))
-    predictions = xs.concat_time(chunks)
     plan = feedback.FeedbackPlan.all_channels(first["inputs"], first["targets"], first["forcings"])
-    cot = [model._cotangent_planes(cotangents.isel(time=slice(t, t + 1)), first["targets"],
-                                   stash.batch) for t in range(len(stash.steps))]
-    input_grads, forcing_grads = model._input_grads(stash, plan, first["norm"], inputs, forcings,
-                                                    cotangents=cot)
-    return predictions, input_grads, forcing_grads
+    return xs.concat_time(chunks), stash, first, plan
 
   def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
                 **kwargs):

@@ -24,6 +24,9 @@ same helpers (Backward.tangent): each stage of the stage-wise forward is followe
 MLP's tangent formed at its recomputed h and z (mlp_jvp; gcb_swish_jvp and gcb_layernorm_jvp_dirs for
 the two nonlinearities).  Several tangent directions share that walk: their state is stacked
 direction-major, so every tangent GEMM runs once over all of them and h and z are recomputed once.
+Several cotangents (batched_input_vjp) share the backward walk the same way: element(dirs=K) stacks the
+gradient state like the tangent's, runs every dX product once over all directions, and differentiates
+the two nonlinearities with gcb_layernorm_backward_dirs and gcb_swish_jvp.
 
 All arithmetic is in libgraphcast_b200.so; this module only sequences the launches and owns the
 buffers.  Allocation is lazy: nothing here exists until the first loss_and_grads call.
@@ -288,8 +291,14 @@ class Backward:
                    w0=None, dw_segs=None) -> torch.Tensor:
     """Backward of one MLP at the recomputed forward; accumulates its parameter gradients and returns
     dh [rows, 512], the gradient of the first layer's pre-activation (incl. pre-gathered addends).
-    dw_segs: the layer-0 inputs whose weight blocks get X^T dh (default: all of `segs`)."""
+    dw_segs: the layer-0 inputs whose weight blocks get X^T dh (default: all of `segs`).
+
+    With self.dirs > 1 (no parameter gradients), dy and dh are stacked tables of that many directions
+    of `rows` rows (dir_rows): h and z are recomputed once, the dX products run once over every
+    direction, and the two nonlinearities are gcb_layernorm_backward_dirs and gcb_swish_jvp, whose
+    results are those of the one-direction kernels without the column sums."""
     w = info.w
+    nd, stride, rk = self.dirs, self.dir_stride(rows), self.dir_rows(rows)
     h = self.empty(rows)
     self.layer(rows, segs, w0 or w.w0_packed, w.b0, _native.ACT_NONE, out_y=h, pre=pre)
     g = info.g if self.param_grads else self.sink
@@ -301,25 +310,36 @@ class Backward:
       z = self.empty(rows)
       self.layer(rows, [self.tab(a)], w.w1_packed, w.b1, out_y=z)
       del a
-      dz = self.empty(rows)
-      _native.check(self.lib.gcb_layernorm_backward(
-          dy.data_ptr(), dy.shape[1], z.data_ptr(), D, w.ln_scale, rows, D, dz.data_ptr(), D,
-          ws.data_ptr(), ws.numel(), g["b1"].data_ptr(), g["scale"].data_ptr(),
-          g["offset"].data_ptr(), 1, self._st()), "gcb_layernorm_backward")
+      dz = self.empty(rk)
+      if nd == 1:
+        _native.check(self.lib.gcb_layernorm_backward(
+            dy.data_ptr(), dy.shape[1], z.data_ptr(), D, w.ln_scale, rows, D, dz.data_ptr(), D,
+            ws.data_ptr(), ws.numel(), g["b1"].data_ptr(), g["scale"].data_ptr(),
+            g["offset"].data_ptr(), 1, self._st()), "gcb_layernorm_backward")
+      else:
+        _native.check(self.lib.gcb_layernorm_backward_dirs(
+            dy.data_ptr(), dy.shape[1], z.data_ptr(), D, w.ln_scale, rows, D, stride, nd,
+            dz.data_ptr(), D, self._st()), "gcb_layernorm_backward_dirs")
       del z
     else:
       dz = dy
-      _native.check(self.lib.gcb_layernorm_backward(
-          dy.data_ptr(), dy.shape[1], None, 0, None, rows, info.n1, None, 0, ws.data_ptr(),
-          ws.numel(), g["b1"].data_ptr(), None, None, 1, self._st()), "gcb_layernorm_backward")
+      if nd == 1:                            # its column sums only (several directions: none)
+        _native.check(self.lib.gcb_layernorm_backward(
+            dy.data_ptr(), dy.shape[1], None, 0, None, rows, info.n1, None, 0, ws.data_ptr(),
+            ws.numel(), g["b1"].data_ptr(), None, None, 1, self._st()), "gcb_layernorm_backward")
     if self.param_grads:
       self.wgrad(self.tab(h), dz, rows, g["w1"], n=info.n1, swish=True)     # dW1 = swish(h)^T dz
-    da = self.empty(rows)
-    self.layer(rows, [self.tab(dz, info.n1)], info.t["w1"], self.zero_bias, out_y=da)
-    dh = self.empty(rows)
-    _native.check(self.lib.gcb_swish_backward(
-        da.data_ptr(), D, h.data_ptr(), D, rows, D, dh.data_ptr(), D, ws.data_ptr(), ws.numel(),
-        g["b0"].data_ptr(), 1, self._st()), "gcb_swish_backward")
+    da = self.empty(rk)
+    self.layer(rk, [self.tab(dz, info.n1)], info.t["w1"], self.zero_bias, out_y=da)
+    if nd == 1:
+      dh = self.empty(rows)
+      _native.check(self.lib.gcb_swish_backward(
+          da.data_ptr(), D, h.data_ptr(), D, rows, D, dh.data_ptr(), D, ws.data_ptr(), ws.numel(),
+          g["b0"].data_ptr(), 1, self._st()), "gcb_swish_backward")
+    else:                                    # swish'(h) da in place
+      dh = da
+      _native.check(self.lib.gcb_swish_jvp(h.data_ptr(), D, rows, D, da.data_ptr(), D, stride, nd,
+                                           dh.data_ptr(), D, self._st()), "gcb_swish_jvp")
     del da, h
     if self.param_grads:
       off = 0
@@ -329,19 +349,23 @@ class Backward:
         off += k
     return dh
 
-  def seg_sum_sender(self, name: str, dh: torch.Tensor, num_nodes: int) -> torch.Tensor:
-    order, ptr, heavy, n_heavy = self.csr[name]
-    out = self.empty(num_nodes)
-    _native.check(self.lib.gcb_segment_sum_sorted(
-        dh.data_ptr(), D, order.data_ptr(), ptr.data_ptr(), num_nodes, heavy.data_ptr(), n_heavy,
-        out.data_ptr(), D, D, self._st()), "gcb_segment_sum_sorted")
+  def sender_sums(self, dh: torch.Tensor, rows: int, csr, num_nodes: int) -> torch.Tensor:
+    """gcb_segment_sum_sorted (sender CSR `csr`) of every direction of the stacked edge table dh (`rows`
+    rows per direction) into a new stacked node table of num_nodes rows per direction, one launch per
+    direction."""
+    order, ptr, heavy, n_heavy = csr
+    out = self.empty(self.dir_rows(num_nodes))
+    s_in, s_out = self.dir_stride(rows), self.dir_stride(num_nodes)
+    for k in range(self.dirs):
+      _native.check(self.lib.gcb_segment_sum_sorted(
+          dh[k * s_in:].data_ptr(), D, order.data_ptr(), ptr.data_ptr(), num_nodes, heavy.data_ptr(),
+          n_heavy, out[k * s_out:].data_ptr(), D, D, self._st()), "gcb_segment_sum_sorted")
     return out
 
-  def seg_sum_receiver(self, dh: torch.Tensor, row_ptr, num_nodes: int, heavy=None, n_heavy=0):
-    out = self.empty(num_nodes)
-    _native.check(self.lib.gcb_segment_sum_heavy(
-        dh.data_ptr(), D, row_ptr.data_ptr(), num_nodes, heavy.data_ptr() if n_heavy else None,
-        n_heavy, out.data_ptr(), D, D, self._st()), "gcb_segment_sum_heavy")
+  def seg_sum_receiver(self, dh: torch.Tensor, rows: int, row_ptr, num_nodes: int, heavy=None,
+                       n_heavy=0):
+    out = self.empty(self.dir_rows(num_nodes))
+    self.receiver_sums(dh, rows, row_ptr, num_nodes, out, self.dir_stride(num_nodes), heavy, n_heavy)
     return out
 
   def gather_add(self, src: torch.Tensor, idx: torch.Tensor, n: int,
@@ -367,7 +391,7 @@ class Backward:
     pr = self.projection(n_r, v_r, sp.wr_packed)
     dh = self.mlp_backward(info, rows, [e_seg], dm, pre=[(ps, snd), (pr, rcv)], w0=sp.we_packed)
     del ps, pr
-    s = self.seg_sum_sender(snd_name, dh, n_s)
+    s = self.sender_sums(dh, rows, self.csr[snd_name], n_s)
     r = rcv_sum(dh)
     if self.param_grads:
       w0 = info.g["w0"]
@@ -381,30 +405,31 @@ class Backward:
     """Backward of a grid2mesh / mesh2grid edge MLP m = MLP([e | v_s[snd] | v_r[rcv]]) with
     e = MLP(edge features) and dm = dagg[rcv] (its edge residual is dead), chunk by chunk (see
     self.chunks): accumulates the parameter gradients of both MLPs and returns the node tables
-    (S [n_s, 512], R [n_r, 512]) of dH summed by sender / receiver."""
+    (S [n_s, 512], R [n_r, 512]) of dH summed by sender / receiver.
+
+    Several directions (self.dirs > 1, stacked dagg) use these same chunks, not tangent_chunks: S is
+    added chunk by chunk, so its bits depend on where the chunks fall, and direction k is to be what
+    one direction alone gives.  The stacked temporaries of a chunk therefore grow with the direction
+    count."""
     sp = info.split
     ps = self.projection(n_s, v_s, sp.ws_packed)
     pr = self.projection(n_r, v_r, sp.wr_packed)
-    s_tab, r_tab = None, self.empty(n_r)
-    for r0, r1, g0, g1, rp, heavy, n_heavy, csr in self.chunks[name]:
+    s_tab, r_tab = None, self.empty(self.dir_rows(n_r))
+    for i, (r0, r1, g0, g1, rp, heavy, n_heavy, csr) in enumerate(self.chunks[name]):
       n = r1 - r0
       f = self.tab(feat_t[r0:r1], 16, 4, 4)                 # 16-byte rows: the view stays aligned
       snd_c, rcv_c = snd[r0:r1].clone(), rcv[r0:r1].clone()  # index arrays from an aligned base
       e = self.fwd_mlp(enc, n, [f])
-      dm = self.gather_add(dagg, rcv_c, n)
+      dm = self.gather_add(dagg, self.kfold(rcv_c, n_r, (name, "backward", i, "rcv")),
+                           self.dir_rows(n))
       dh = self.mlp_backward(info, n, [self.tab(e)], dm, pre=[(ps, snd_c), (pr, rcv_c)],
                              w0=sp.we_packed)
       del dm, e, snd_c, rcv_c
-      order, ptr, sh, n_sh = csr
-      s_c = self.empty(n_s)
-      _native.check(self.lib.gcb_segment_sum_sorted(
-          dh.data_ptr(), D, order.data_ptr(), ptr.data_ptr(), n_s, sh.data_ptr(), n_sh,
-          s_c.data_ptr(), D, D, self._st()), "gcb_segment_sum_sorted")
-      s_tab = s_c if s_tab is None else self.gather_add(s_c, self.iota, n_s, s_tab)
+      s_c = self.sender_sums(dh, n, csr, n_s)
+      s_tab = s_c if s_tab is None else self.gather_add(
+          s_c, self.kfold(self.iota[:n_s], n_s, ("iota", n_s)), self.dir_rows(n_s), s_tab)
       del s_c
-      _native.check(self.lib.gcb_segment_sum_heavy(
-          dh.data_ptr(), D, rp.data_ptr(), g1 - g0, heavy.data_ptr() if n_heavy else None, n_heavy,
-          r_tab[g0:g1].data_ptr(), D, D, self._st()), "gcb_segment_sum_heavy")
+      self.receiver_sums(dh, n, rp, g1 - g0, r_tab[g0:], self.dir_stride(n_r), heavy, n_heavy)
       if self.param_grads:                  # the edge embedder's backward: parameters only
         de = self.empty(n)
         self.layer(n, [self.tab(dh)], info.t["w0_0"], self.zero_bias, out_y=de)
@@ -422,7 +447,8 @@ class Backward:
 
   # -- one batch element ---------------------------------------------------------------------------
   def element(self, grid_in_img: torch.Tensor, g_out: torch.Tensor, snaps: dict,
-              dgrid_in: bool = False, param_grads: bool = True) -> Optional[torch.Tensor]:
+              dgrid_in: bool = False, param_grads: bool = True,
+              dirs: int = 1) -> Optional[torch.Tensor]:
     """Accumulates the parameter gradients of one batch element whose loss derivative with respect
     to the decoder output is g_out [Ng, 256] (gcb_output_loss_grad) and whose forward left `snaps`
     (whose entries are dropped as they are consumed).  dgrid_in: also return the derivative with
@@ -433,12 +459,20 @@ class Backward:
     skips what only the parameters need: every gcb_weight_grad, the backward passes of the three edge
     embedders and of the mesh-node encoder, and the de product of the first processor step.  The
     row-wise kernels' column sums go to scratch.  The recomputes and the dX products that remain are
-    the same launches on the same operands, so dx is bit-identical to that of param_grads=True."""
-    self.param_grads = bool(param_grads)
+    the same launches on the same operands, so dx is bit-identical to that of param_grads=True.
+
+    dirs = K > 1 (param_grads=False only) differentiates K cotangents at once: g_out is the stacked
+    table of K directions of Ng rows (dir_rows), and so is dx.  The gradient state is stacked like the
+    tangent's, so every dX product is one GEMM over all directions and every MLP's h and z, the
+    embedder recomputes and the sender / receiver projections are formed once; the segment sums run
+    per direction.  Direction k is bit for bit what g_out's direction k alone gives."""
+    if dirs > 1 and param_grads:
+      raise ValueError("several directions are supported without parameter gradients only")
+    self.param_grads, self.dirs = bool(param_grads), int(dirs)
     try:
       return self._element(grid_in_img, g_out, snaps, dgrid_in)
     finally:
-      self.param_grads = True
+      self.param_grads, self.dirs = True, 1
 
   def _element(self, grid_in_img, g_out, snaps, dgrid_in):
     eng, m = self.eng, self.m
@@ -447,17 +481,18 @@ class Backward:
     mp = self.mlps
     img, tab = self.img, self.tab
     feat = lambda t: tab(t, 16, 4, 4)
+    rk = self.dir_rows                       # rows of a stacked table (n rows for one direction)
 
     # ---- decoder: out = MLP(vg2);  vg2 = vg1 + MLP([vg1 | agg3]);  m3 = MLP([e3 | v[snd] | vg1[rcv]])
     dh = self.mlp_backward(mp["dec_grid"], ng, [img(snaps["vg2"])], g_out)
-    dvg2 = self.empty(ng)
-    self.layer(ng, [tab(dh)], mp["dec_grid"].t["w0_0"], self.zero_bias, out_y=dvg2)
+    dvg2 = self.empty(rk(ng))
+    self.layer(rk(ng), [tab(dh)], mp["dec_grid"].t["w0_0"], self.zero_bias, out_y=dvg2)
     info = mp["proc_n_grid_m2g"]
     dh = self.mlp_backward(info, ng, [img(snaps["vg1"]), img(snaps["agg3"])], dvg2)
-    dvg1 = self.empty(ng)
-    self.layer(ng, [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dvg2, out=dvg1)
-    dagg3 = self.empty(ng)
-    self.layer(ng, [tab(dh)], info.t["w0_1"], self.zero_bias, out_y=dagg3)
+    dvg1 = self.empty(rk(ng))
+    self.layer(rk(ng), [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dvg2, out=dvg1)
+    dagg3 = self.empty(rk(ng))
+    self.layer(rk(ng), [tab(dh)], info.t["w0_1"], self.zero_bias, out_y=dagg3)
     del dh, dvg2
     info = mp["proc_e_m2g"]
     S, R = self.bipartite_backward("m2g", info, mp["enc_e_m2g"], eng.m2g_feat, dagg3, eng.m2g_snd,
@@ -465,24 +500,25 @@ class Backward:
     del dagg3
     # snapshots are released as soon as the backward pass is past their stage
     snaps["vg2"] = snaps["agg3"] = snaps["vg1"] = None
-    dvg1_new = self.empty(ng)
-    self.layer(ng, [tab(R)], info.t["w0_2"], self.zero_bias, residual=dvg1, out=dvg1_new)
+    dvg1_new = self.empty(rk(ng))
+    self.layer(rk(ng), [tab(R)], info.t["w0_2"], self.zero_bias, residual=dvg1, out=dvg1_new)
     dvg1 = dvg1_new
-    dv = self.empty(nm)
-    self.layer(nm, [tab(S)], info.t["w0_1"], self.zero_bias, out_y=dv)
+    dv = self.empty(rk(nm))
+    self.layer(rk(nm), [tab(S)], info.t["w0_1"], self.zero_bias, out_y=dv)
     del S, R
 
     # ---- processor, last step first:  m = MLP([e | v[snd] | v[rcv]]);  v' = v + MLP([v | agg]);
     #      e' = e + m
     de_next = None
+    rcv_k = self.kfold(eng.mesh_rcv, nm, ("mesh", "rcv"))
     for k in range(K - 1, -1, -1):
       v_k = img(snaps["v"][k])
       agg_k = img(snaps["agg"][k])
       nfo, efo = self.proc_n[k], self.proc_e[k]
       dh_n = self.mlp_backward(nfo, nm, [v_k, agg_k], dv)
-      dagg = self.empty(nm)
-      self.layer(nm, [tab(dh_n)], nfo.t["w0_1"], self.zero_bias, out_y=dagg)
-      dm = self.gather_add(dagg, eng.mesh_rcv, m.e_mesh, de_next)
+      dagg = self.empty(rk(nm))
+      self.layer(rk(nm), [tab(dh_n)], nfo.t["w0_1"], self.zero_bias, out_y=dagg)
+      dm = self.gather_add(dagg, rcv_k, rk(m.e_mesh), de_next)
       del dagg
       if k == 0:
         e0 = self.fwd_mlp(mp["enc_e_mesh"], m.e_mesh, [feat(eng.mesh_feat)])
@@ -491,24 +527,25 @@ class Backward:
         e_k = img(snaps["e"][k])
       dH, S, R = self.edge_backward(
           efo, m.e_mesh, e_k, dm, "mesh", v_k, nm, eng.mesh_snd, v_k, nm, eng.mesh_rcv,
-          lambda d: self.seg_sum_receiver(d, eng.mesh_row_ptr, nm))
+          lambda d: self.seg_sum_receiver(d, m.e_mesh, eng.mesh_row_ptr, nm))
       del dm
       if k == 0 and not self.param_grads:    # de_0 feeds the mesh edge embedder's parameters only
         de = None
       else:
-        de = self.empty(m.e_mesh)            # de_k = de_{k+1} + dH W_e^T  (e' = e + m)
+        de = self.empty(rk(m.e_mesh))        # de_k = de_{k+1} + dH W_e^T  (e' = e + m)
         if de_next is None:
-          self.layer(m.e_mesh, [tab(dH)], efo.t["w0_0"], self.zero_bias, out_y=de)
+          self.layer(rk(m.e_mesh), [tab(dH)], efo.t["w0_0"], self.zero_bias, out_y=de)
         else:
-          self.layer(m.e_mesh, [tab(dH)], efo.t["w0_0"], self.zero_bias, residual=de_next, out=de)
+          self.layer(rk(m.e_mesh), [tab(dH)], efo.t["w0_0"], self.zero_bias, residual=de_next,
+                     out=de)
       del dH
       de_next = de
       # dv_k = dv_{k+1} + dh_n W0a^T + S W_s^T + R W_r^T
-      dv_new = self.empty(nm)
-      self.layer(nm, [tab(dh_n)], nfo.t["w0_0"], self.zero_bias, residual=dv, out=dv_new)
-      dv2 = self.empty(nm)
-      self.layer(nm, [tab(S)], efo.t["w0_1"], self.zero_bias, residual=dv_new, out=dv2)
-      self.layer(nm, [tab(R)], efo.t["w0_2"], self.zero_bias, residual=dv2, out=dv_new)
+      dv_new = self.empty(rk(nm))
+      self.layer(rk(nm), [tab(dh_n)], nfo.t["w0_0"], self.zero_bias, residual=dv, out=dv_new)
+      dv2 = self.empty(rk(nm))
+      self.layer(rk(nm), [tab(S)], efo.t["w0_1"], self.zero_bias, residual=dv_new, out=dv2)
+      self.layer(rk(nm), [tab(R)], efo.t["w0_2"], self.zero_bias, residual=dv2, out=dv_new)
       dv = dv_new
       del dh_n, S, R, dv2
       snaps["v"][k + 1] = snaps["agg"][k] = snaps["e"][k] = None
@@ -525,40 +562,40 @@ class Backward:
     vm0 = self.fwd_mlp(mp["enc_mesh"], nm, [mesh_in])
     info = mp["proc_n_grid_g2m"]
     dh = self.mlp_backward(info, ng, [tab(vg0)], dvg1)
-    dvg0 = self.empty(ng)
-    self.layer(ng, [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dvg1, out=dvg0)
+    dvg0 = self.empty(rk(ng))
+    self.layer(rk(ng), [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dvg1, out=dvg0)
     del dh, dvg1
     info = mp["proc_n_mesh_g2m"]
     dh = self.mlp_backward(info, nm, [tab(vm0), img(snaps["agg1"])], dv)
-    dvm0 = self.empty(nm)
-    self.layer(nm, [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dv, out=dvm0)
-    dagg1 = self.empty(nm)
-    self.layer(nm, [tab(dh)], info.t["w0_1"], self.zero_bias, out_y=dagg1)
+    dvm0 = self.empty(rk(nm))
+    self.layer(rk(nm), [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dv, out=dvm0)
+    dagg1 = self.empty(rk(nm))
+    self.layer(rk(nm), [tab(dh)], info.t["w0_1"], self.zero_bias, out_y=dagg1)
     del dh, dv
     info = mp["proc_e_g2m"]
     S, R = self.bipartite_backward("g2m", info, mp["enc_e_g2m"], eng.g2m_feat, dagg1, eng.g2m_snd,
                                    eng.g2m_rcv, tab(vg0), ng, tab(vm0), nm)
     del dagg1
-    t = self.empty(ng)
-    self.layer(ng, [tab(S)], info.t["w0_1"], self.zero_bias, residual=dvg0, out=t)
+    t = self.empty(rk(ng))
+    self.layer(rk(ng), [tab(S)], info.t["w0_1"], self.zero_bias, residual=dvg0, out=t)
     dvg0 = t
-    t = self.empty(nm)
-    self.layer(nm, [tab(R)], info.t["w0_2"], self.zero_bias, residual=dvm0, out=t)
+    t = self.empty(rk(nm))
+    self.layer(rk(nm), [tab(R)], info.t["w0_2"], self.zero_bias, residual=dvm0, out=t)
     dvm0 = t
     del S, R, vg0, vm0
     dh = self.mlp_backward(mp["enc_grid"], ng, [grid_in], dvg0)
     dx = None
     if dgrid_in:
       w0t, n = self.input_transposed()
-      dx = self.empty(ng, n)
-      self.layer(ng, [tab(dh)], w0t, self.zero_bias, out_y=dx, n=n)
+      dx = self.empty(rk(ng), n)
+      self.layer(rk(ng), [tab(dh)], w0t, self.zero_bias, out_y=dx, n=n)
     del dh, dvg0
     if self.param_grads:
       self.mlp_backward(mp["enc_mesh"], nm, [mesh_in], dvm0)
     return dx
 
   # -- tangent-linear model (Engine.input_jvp_element) ------------------------------------------------
-  # The tangent state of `dirs` directions is stacked direction-major: a table of n rows per direction
+  # The tangent (or, in element(dirs=K), gradient) state of `dirs` directions is stacked direction-major: a table of n rows per direction
   # holds direction k in rows [k * dir_stride(n), k * dir_stride(n) + n), the stride rounded up to the
   # 128-row tiles of the operand images.  The last direction is not padded, so that one direction is
   # exactly the table of n rows.  The pad rows between directions are never read into a valid row: the
@@ -576,7 +613,9 @@ class Backward:
     """The gather index `idx` (into a table of n_src rows per direction) for self.dirs directions:
     idx + k * dir_stride(n_src) in the rows of direction k of a stacked table of len(idx) rows per
     direction, 0 in the pad rows.  Built on first use per `key` and kept while the direction count
-    stays the same."""
+    stays the same.  The key names the index and, for a bipartite chunk, the chunk set it belongs to
+    ("tangent" | "backward"): with several directions the two sets differ, so chunk i of one is not
+    chunk i of the other."""
     if self.dirs == 1:
       return idx
     if self._kfold_dirs != self.dirs:
@@ -687,9 +726,9 @@ class Backward:
       f = self.tab(feat_t[r0:r1], 16, 4, 4)                 # 16-byte rows: the view stays aligned
       snd_c, rcv_c = snd[r0:r1].clone(), rcv[r0:r1].clone()  # index arrays from an aligned base
       e = self.fwd_mlp(enc, n, [f])
-      dpre = [(dps, self.kfold(snd_c, n_s, (name, i, "snd")))]
+      dpre = [(dps, self.kfold(snd_c, n_s, (name, "tangent", i, "snd")))]
       if dpr is not None:
-        dpre.append((dpr, self.kfold(rcv_c, n_r, (name, i, "rcv"))))
+        dpre.append((dpr, self.kfold(rcv_c, n_r, (name, "tangent", i, "rcv"))))
       dm = self.mlp_jvp(info, n, [self.tab(e)], [], pre=[(ps, snd_c), (pr, rcv_c)], dpre=dpre,
                         w0=sp.we_packed)
       del e

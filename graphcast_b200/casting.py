@@ -72,6 +72,11 @@ class Bfloat16Cast(graphcast.Predictor):
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
     return self._predictor.input_vjp(inputs, targets_template, forcings, cotangents, **kwargs)
 
+  def batched_input_vjp(self, inputs, targets_template, forcings, cotangents, *,
+                        directions_per_pass=None, **kwargs):
+    return self._predictor.batched_input_vjp(inputs, targets_template, forcings, cotangents,
+                                             directions_per_pass=directions_per_pass, **kwargs)
+
   def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
                 **kwargs):
     return self._predictor.input_jvp(inputs, targets_template, forcings, input_tangents,

@@ -1150,6 +1150,23 @@ int gcb_layernorm_jvp_dirs(const float* z, int32_t ld_z, const float* dz, int32_
   return GCB_OK;
 }
 
+int gcb_layernorm_backward_dirs(const float* dy, int32_t ld_dy, const float* z, int32_t ld_z,
+                                const float* scale, int64_t rows, int32_t n, int64_t dir_stride,
+                                int32_t dirs, float* dz, int32_t ld_dz, void* stream) {
+  GCB_CHECK_ARG(dy && z && scale && dz, "null pointer");
+  GCB_CHECK_ARG(n == 512, "the LayerNorm backward of several directions needs n = 512");
+  GCB_CHECK_ARG(rows >= 0 && ld_dy >= n && ld_z >= n && ld_dz >= n,
+                "rows < 0 or leading dimension < n");
+  GCB_CHECK_ARG(dirs >= 1 && (dirs == 1 || dir_stride >= rows), "dirs < 1 or dir_stride < rows");
+  if (rows == 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0, 4.0 * static_cast<double>(rows) * n * (1.0 + 2.0 * dirs));
+  gcb::layernorm_backward_dirs_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, st>>>(
+      dy, ld_dy, z, ld_z, scale, rows, dir_stride, dirs, dz, ld_dz);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
 int gcb_segment_sum_sorted(const float* msg, int32_t ld_msg, const int32_t* order,
                            const int32_t* ptr, int32_t num_nodes, const int32_t* heavy,
                            int32_t num_heavy, float* out, int32_t ld_out, int32_t width, void* stream) {

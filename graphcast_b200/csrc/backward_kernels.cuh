@@ -441,6 +441,70 @@ layernorm_jvp_dirs_kernel(const float* __restrict__ z, int ld_z, const float* __
   }
 }
 
+// ---- several cotangents (batched_input_vjp) -------------------------------------------------------
+// The dz of rowwise_backward_kernel<kRowLayerNorm, 16> for dirs stacked dy tables (row r of direction k
+// is row k * stride + r), without its column sums:
+//   dz[k] = rstd * (dy[k]*scale - mean(dy[k]*scale) - zhat * mean(dy[k]*scale*zhat))
+// One warp per row of n = 512 (lane owns columns lane + 32 j), 8 rows per block; z's row is read once.
+// Every rounding is pinned by an intrinsic to what rowwise_backward_kernel<kRowLayerNorm, 16> compiles
+// to (its SASS): the row sum s of z in column order then butterfly order, z - mean as fma(s, -1/n, z)
+// (the mean itself never rounded), the variance as a chain of fmas from 0, rstd = rsqrt(fma(var, 1/n,
+// 1e-5)), zhat = (z - mean) * rstd; g = dy * scale rounded, sum g added in column order, sum g * zhat
+// as a chain of fmas from 0; dz = rstd * fma(zhat, -mgz, fma(sum g, -1/n, g)) with mgz = (sum g * zhat)
+// / n rounded once.
+__global__ void __launch_bounds__(256)
+layernorm_backward_dirs_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z,
+                               int ld_z, const float* __restrict__ scale, long long rows,
+                               long long stride, int dirs, float* __restrict__ dz, int ld_dz) {
+  constexpr int kCols = 16;
+  constexpr float kInvN = 1.0f / (kCols * 32);
+  const int lane = threadIdx.x & 31;
+  const long long r = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  if (r >= rows) return;
+  float v[kCols], sc[kCols];
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) {
+    v[j] = z[r * ld_z + lane + 32 * j];
+    sc[j] = scale[lane + 32 * j];
+  }
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) s = __fadd_rn(s, v[j]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, o));
+  float var = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) {
+    v[j] = __fmaf_rn(s, -kInvN, v[j]);                 // z - mean
+    var = __fmaf_rn(v[j], v[j], var);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) var = __fadd_rn(var, __shfl_xor_sync(0xffffffffu, var, o));
+  const float rstd = rsqrtf(__fmaf_rn(var, kInvN, 1e-5f));
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) v[j] = __fmul_rn(v[j], rstd);     // z-hat
+  for (int k = 0; k < dirs; ++k) {
+    const long long rk = k * stride + r;
+    float g[kCols];
+    float mg = 0.f, mgz = 0.f;
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) {
+      g[j] = __fmul_rn(dy[rk * ld_dy + lane + 32 * j], sc[j]);
+      mg = __fadd_rn(mg, g[j]);
+      mgz = __fmaf_rn(v[j], g[j], mgz);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      mg = __fadd_rn(mg, __shfl_xor_sync(0xffffffffu, mg, o));
+      mgz = __fadd_rn(mgz, __shfl_xor_sync(0xffffffffu, mgz, o));
+    }
+    const float mgz_n = __fmul_rn(mgz, kInvN);
+#pragma unroll
+    for (int j = 0; j < kCols; ++j)
+      dz[rk * ld_dz + lane + 32 * j] = __fmul_rn(rstd, __fmaf_rn(v[j], -mgz_n, __fmaf_rn(mg, -kInvN, g[j])));
+  }
+}
+
 // ---- index operations ----------------------------------------------------------------------------
 // out[i, 0:512] = sum_{j in [ptr[i], ptr[i+1])} msg[order[j], 0:512], summed in j order.  Rows listed
 // in `heavy` (ascending node ids): one 128-thread block each (thread owns one float4 column); every

@@ -760,17 +760,31 @@ class Engine:
     operands["cotangent"] [n_out, Ng], J = sum cotangent * prediction
     (gcb_output_cotangent_grad_feedback).  `operands` also holds the affine keywords of output_loss
     (scale, offset, add_planes, add_plane_index).  The seed is their last reader: the dict is cleared
-    after it, so that planes the caller no longer references are free during the backward pass."""
+    after it, so that planes the caller no longer references are free during the backward pass.
+
+    Several cotangents at once (batched_input_vjp): operands["cotangent"] [K, n_out, Ng], contiguous.
+    fb.a is then [K, fb.n_rows, Ng], direction k's rows; the seed and gcb_input_grad run per direction,
+    the backward pass once for all of them (Backward.element(dirs=K)), and direction k is bit for bit
+    what its cotangent alone gives."""
     if self._backward is None:
       raise RuntimeError("call input_grads_begin() first")
     affine = {k: operands[k] for k in ("scale", "offset", "add_planes", "add_plane_index")
               if k in operands}
     targets_planes, cotangent = operands.get("targets_planes"), operands.get("cotangent")
     operands.clear()
+    single = cotangent is None or cotangent.dim() == 2
+    dirs = 1 if single else cotangent.shape[0]
+    if not single and (tuple(cotangent.shape) != (dirs, self.n_out, self.num_grid) or dirs < 1
+                       or not cotangent.is_contiguous()):
+      raise ValueError(f"cotangent must be a contiguous [K, {self.n_out}, {self.num_grid}] tensor")
     grid_in = self.grid_in_img if grid_in is None else grid_in
     snaps = self._forward_snapshots(grid_in)
-    g_out = torch.zeros([self.num_grid, 256], dtype=torch.float32, device=self.device)
-    a_out = torch.empty([fb.n_rows, self.num_grid], dtype=torch.float32, device=self.device)
+    stride = self._backward.dir_stride(self.num_grid)
+    g_out = torch.zeros([(dirs - 1) * stride + self.num_grid, 256], dtype=torch.float32,
+                        device=self.device)
+    a_out = torch.empty(([] if single else [dirs]) + [fb.n_rows, self.num_grid], dtype=torch.float32,
+                        device=self.device)
+    a_outs = [a_out] if single else list(a_out.unbind(0))
     with self._on_device():
       if planes_out is not None:
         self.unpack_outputs(planes_out, **affine)
@@ -786,20 +800,26 @@ class Engine:
             fb.dpred_row.data_ptr(), fb.n_rows, fb.resid_channel.data_ptr(), fb.carry_row.data_ptr(),
             a_out.data_ptr(), g_out.data_ptr(), 256, self._stream()), "gcb_output_loss_grad_feedback")
       else:
-        if tuple(cotangent.shape) != (self.n_out, self.num_grid) or not cotangent.is_contiguous():
+        if single and (tuple(cotangent.shape) != (self.n_out, self.num_grid)
+                       or not cotangent.is_contiguous()):
           raise ValueError(f"cotangent must be a contiguous [{self.n_out}, {self.num_grid}] tensor")
-        _native.check(self._lib.gcb_output_cotangent_grad_feedback(
-            self.n_out, self.num_grid, self._ptr(affine.get("scale")), cotangent.data_ptr(),
-            self._ptr(fb.a), fb.dpred_row.data_ptr(), fb.n_rows, fb.resid_channel.data_ptr(),
-            fb.carry_row.data_ptr(), a_out.data_ptr(), g_out.data_ptr(), 256, self._stream()),
-            "gcb_output_cotangent_grad_feedback")
+        cots = [cotangent] if single else list(cotangent.unbind(0))
+        a_next = [fb.a] if single else [None] * dirs if fb.a is None else list(fb.a.unbind(0))
+        for k in range(dirs):
+          _native.check(self._lib.gcb_output_cotangent_grad_feedback(
+              self.n_out, self.num_grid, self._ptr(affine.get("scale")), cots[k].data_ptr(),
+              self._ptr(a_next[k]), fb.dpred_row.data_ptr(), fb.n_rows, fb.resid_channel.data_ptr(),
+              fb.carry_row.data_ptr(), a_outs[k].data_ptr(), g_out[k * stride:].data_ptr(), 256,
+              self._stream()), "gcb_output_cotangent_grad_feedback")
+        del cots, a_next
       # the following step's rows, the planes, targets and cotangent are consumed: release them
       fb.a = a_out
       affine = targets_planes = cotangent = None
-      dx = self._backward.element(grid_in, g_out, snaps, dgrid_in=True, param_grads=False)
-      _native.check(self._lib.gcb_input_grad(
-          dx.data_ptr(), dx.shape[1], self.num_grid, fb.n_rows, fb.rows.data_ptr(),
-          self._ptr(fb.in_scale), a_out.data_ptr(), 1, self._stream()), "gcb_input_grad")
+      dx = self._backward.element(grid_in, g_out, snaps, dgrid_in=True, param_grads=False, dirs=dirs)
+      for k in range(dirs):
+        _native.check(self._lib.gcb_input_grad(
+            dx[k * stride:].data_ptr(), dx.shape[1], self.num_grid, fb.n_rows, fb.rows.data_ptr(),
+            self._ptr(fb.in_scale), a_outs[k].data_ptr(), 1, self._stream()), "gcb_input_grad")
 
   # -- tangent-linear model (input_jvp, batched_input_jvp) --------------------------------------------
   def input_jvp_element(self, tangent_planes: torch.Tensor, tangent_out: torch.Tensor, *,

@@ -225,11 +225,12 @@ class VariableRows:
     x = np.asarray(a[self.start:self.start + self.count], np.float64).reshape(self.count, n_lat, n_lon)
     return x if self.mode == 0 else (x.sum(axis=1) if self.mode == 1 else x.sum(axis=(1, 2)))
 
-  def to_variable(self, g: np.ndarray, n_lat: int, n_lon: int) -> xs.DataArray:
+  def to_variable(self, g: np.ndarray, n_lat: int, n_lon: int, directions: bool = False) -> xs.DataArray:
     """g: [batch]? ([time] for a timed forcing) [count, *plane_shape] -> the gradient as a DataArray with
     the variable's dims, in its order.  A timed forcing's per-step slab has a time dim of size 1, whose
-    place the time axis of g takes."""
-    lead = ["batch"] if self.batched else []
+    place the time axis of g takes.  directions: g has a leading axis of directions, and the result a
+    leading "direction" dim (one copy, as for one direction)."""
+    lead = ([DIRECTION] if directions else []) + (["batch"] if self.batched else [])
     if self.timed:
       lead.append("time")
     stack = [d for d in self.stack_dims if not (self.timed and d == "time")]
@@ -237,8 +238,9 @@ class VariableRows:
     spatial = [("lat", "lon"), ("lon",), ()][self.mode]
     arr = np.asarray(g).reshape(list(g.shape[:len(lead)]) + sizes + list(self.plane_shape(n_lat, n_lon)))
     dims = lead + stack + list(spatial)
-    return xs.DataArray(np.ascontiguousarray(np.transpose(arr, [dims.index(d) for d in self.var_dims])),
-                        self.var_dims)
+    var_dims = ((DIRECTION,) if directions else ()) + self.var_dims
+    return xs.DataArray(np.ascontiguousarray(np.transpose(arr, [dims.index(d) for d in var_dims])),
+                        var_dims)
 
 
 def variable_rows(inputs: xs.Dataset, forcings: xs.Dataset) -> list:
@@ -304,6 +306,47 @@ def check_direction_tangents(input_tangents: Optional[xs.Dataset], inputs: xs.Da
   return dirs, labels
 
 
+def check_direction_cotangents(cotangents: xs.Dataset, template: xs.Dataset):
+  """(K, direction labels) of the cotangents of a batched_input_vjp: ValueError unless they have the
+  variables of `template` and each has a leading "direction" dim of one size K >= 1 for all of them,
+  followed by its namesake's shape.  The variable-set and shape errors are input_vjp's.  The labels
+  are the cotangents' "direction" coordinate when they have one, else 0..K-1."""
+  if set(cotangents.keys()) != set(template.keys()):
+    raise ValueError(f"cotangents have the variables {sorted(cotangents.keys())}, the predictions "
+                     f"{sorted(template.keys())}")
+  dirs = None
+  for name in sorted(cotangents.keys()):
+    v = cotangents.data_vars[name]
+    if not v.dims or v.dims[0] != DIRECTION:
+      raise ValueError(f"cotangents: {name} has dims {tuple(v.dims)}; the cotangents of several "
+                       f"directions need the leading dim {DIRECTION!r}")
+    if v.shape[0] < 1:
+      raise ValueError(f"cotangents: {name} has no directions")
+    if dirs is not None and v.shape[0] != dirs:
+      raise ValueError(f"cotangents: {name} has {v.shape[0]} directions, other variables {dirs}")
+    dirs = v.shape[0]
+    shape, want = tuple(v.shape[1:]), tuple(template.data_vars[name].shape)
+    if shape != want:
+      raise ValueError(f"cotangent {name} has shape {shape}, the prediction {want}")
+  if dirs is None:
+    raise ValueError("the cotangents have no variables, so no direction dim")
+  labels = np.arange(dirs)
+  coord = cotangents.coords.get(DIRECTION)
+  if coord is not None and coord[0] == (DIRECTION,) and np.asarray(coord[1]).shape == (dirs,):
+    labels = np.asarray(coord[1])
+  return dirs, labels
+
+
+def direction_slices(dirs: int, directions_per_pass) -> list:
+  """The consecutive slices of `dirs` directions that share one pass, directions_per_pass (None: all)
+  each; ValueError unless it is None or an int >= 1."""
+  per = dirs if directions_per_pass is None else directions_per_pass
+  if isinstance(per, bool) or not isinstance(per, (int, np.integer)) or per < 1:
+    raise ValueError(f"directions_per_pass must be None or an int >= 1, not {directions_per_pass!r}")
+  per = int(per)
+  return [slice(k0, min(k0 + per, dirs)) for k0 in range(0, dirs, per)]
+
+
 def tangent_planes(tangents: Optional[xs.Dataset], like: xs.Dataset,
                    sizes: dict, directions: Optional[int] = None) -> np.ndarray:
   """[batch, channels, lat * lon] float32 planes of a tangent Dataset (check_tangents), packed exactly
@@ -337,10 +380,16 @@ def _fill_planes(tangents, like, sizes, slabs, out: np.ndarray) -> None:
 
 
 def grads_to_datasets(rows: list, grads: dict, inputs: xs.Dataset, forcings: xs.Dataset,
-                      n_lat: int, n_lon: int):
+                      n_lat: int, n_lon: int, directions: Optional[int] = None):
   """(input_grads, forcing_grads): Datasets with the variables, dims and coords of `inputs` and
-  `forcings`, from grads[VariableRows.key] as VariableRows.to_variable takes them."""
+  `forcings`, from grads[VariableRows.key] as VariableRows.to_variable takes them.  With `directions`
+  = K, grads[key] has a leading axis of K directions, and so has every variable ("direction" dim,
+  labelled 0..K-1)."""
   out_in, out_f = xs.Dataset(coords=inputs.coords), xs.Dataset(coords=forcings.coords)
+  if directions is not None:
+    for out in (out_in, out_f):
+      out.coords[DIRECTION] = ((DIRECTION,), np.arange(directions))
   for v in rows:
-    (out_f if v.forcing else out_in)[v.name] = v.to_variable(grads[v.key], n_lat, n_lon)
+    (out_f if v.forcing else out_in)[v.name] = v.to_variable(grads[v.key], n_lat, n_lon,
+                                                             directions=directions is not None)
   return out_in, out_f

@@ -133,6 +133,13 @@ class Predictor(abc.ABC):
     the same leading dim.  directions_per_pass: directions that share one forward (None: all)."""
     raise NotImplementedError(f"{type(self).__name__} does not implement input gradients")
 
+  def batched_input_vjp(self, inputs, targets_template, forcings, cotangents, *,
+                        directions_per_pass=None, **optional_kwargs):
+    """Returns (predictions, input_grads, forcing_grads): input_vjp of K cotangents at once, each
+    variable of `cotangents` carrying a leading "direction" dim of size K; both gradient Datasets have
+    the same leading dim.  directions_per_pass: directions that share one forward (None: all)."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement input gradients")
+
 
 # Per-variable weights of GraphCast's loss (reference graphcast.py:341-356); others weigh 1.
 LOSS_PER_VARIABLE_WEIGHTS = {
@@ -337,6 +344,38 @@ class GraphCast(Predictor):
     `cotangents` a Dataset shaped like `targets_template`."""
     return self._input_vjp(inputs, targets_template, forcings, cotangents, norm=None)
 
+  def batched_input_vjp(self, inputs, targets_template, forcings, cotangents, *,
+                        directions_per_pass=None, **unused_kwargs):
+    """(predictions, input_grads, forcing_grads) of input_vjp for K cotangents at once, for one target
+    time: what jax.vmap of the vjp function of jax.vjp over the cotangents gives.
+
+    Every variable of `cotangents` has a leading "direction" dim of size K >= 1, followed by the shape
+    of the `targets_template` variable of the same name; the variables are the template's.  A missing
+    direction dim, K differing between variables, a wrong variable set or shape and a bad
+    directions_per_pass raise ValueError before anything runs, and every refusal of input_vjp applies.
+    `predictions` is what __call__ returns, bit for bit; input_grads and forcing_grads (float32) are
+    shaped like `inputs` and `forcings` with a leading "direction" dim, its coordinate the cotangents'
+    "direction" coordinate when they have one, else 0..K-1.  Direction k is bit for bit input_vjp with
+    cotangent k alone, for any K and directions_per_pass.
+
+    The directions share one stage-wise forward and one backward walk (Backward.element(dirs=K)): the
+    gradient state is stacked direction-major, so every dX product streams its weights once for all of
+    them and every MLP's h and z, the embedder recomputes and the edge projections are formed once; the
+    seed, segment sums and input reductions run per direction.  directions_per_pass = g (None: K) runs
+    ceil(K / g) such passes, for memory: the stacked state, and the bipartite chunks' temporaries
+    (the chunks are those of one direction, whose boundaries the sender sums depend on), grow with the
+    directions of a pass.  Measured on an 80 GB H100 (DESIGN.md section 8): at 0.25 degree / 37 levels
+    input_vjp already peaks at 73.8 GiB, so run one direction per pass there (directions_per_pass=1),
+    which peaks as input_vjp does (but measured slower than K input_vjp calls there, 0.69x at T = 1); at
+    1 degree / 13 levels a pass peaks at 9.9 GiB for one direction and 33.9 GiB for 16, about 1.6 GiB per
+    further direction, so about 40 fit, and 8 directions take 1.71x less time than 8 input_vjp calls."""
+    if xs.from_xarray(targets_template).sizes.get("time", 1) != 1:
+      raise NotImplementedError("input gradients of GraphCast cover one target time (several: "
+                                "autoregressive.Predictor with gradient_checkpointing=True)")
+    one_pass = lambda cot, first: self._input_vjp(inputs, targets_template, forcings, cot, norm=None,
+                                                  directions=True, predictions=first)
+    return batched_vjp(one_pass, targets_template, cotangents, directions_per_pass)
+
   def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
                 **unused_kwargs):
     """(predictions, prediction_tangents) for one target time: `predictions` is what __call__ returns,
@@ -430,34 +469,45 @@ class GraphCast(Predictor):
     return (loss, diagnostics) + run.finish()
 
   def _input_vjp(self, inputs, targets_template, forcings, cotangents,
-                 norm: Optional[FusedNormalization]):
+                 norm: Optional[FusedNormalization], directions: bool = False,
+                 predictions: bool = True):
+    """input_vjp of one target time; with `directions`, batched_input_vjp of one pass, the cotangents
+    (checked) carrying a leading "direction" dim.  predictions=False: None in place of the predictions,
+    which are then not unpacked."""
     inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
     targets_template = xs.from_xarray(targets_template)
     if targets_template.sizes.get("time", 1) != 1:
       raise NotImplementedError("input gradients of GraphCast cover one target time (several: "
                                 "autoregressive.Predictor with gradient_checkpointing=True)")
-    holder = {}
+    holder = {"predictions": None}
     run = self._one_step_input_grads(inputs, targets_template, forcings, norm, cotangents=cotangents,
-                                     predictions=holder)
+                                     predictions=holder if predictions else None,
+                                     directions=directions)
     return (holder["predictions"],) + run.finish()
 
   def _one_step_input_grads(self, inputs, template, forcings, norm, *, targets=None, coef=None,
-                            cotangents=None, predictions=None) -> "_InputGradRun":
+                            cotangents=None, predictions=None,
+                            directions: bool = False) -> "_InputGradRun":
     """One target time: `_call` stages the planes once and, for every batch element, runs the
     stage-wise forward, the seed and the backward pass of Engine.input_grads_element in place of its
     step (no second forward, no host round trip).  With `targets` the loss sums land in
     self._channel_sums as in `loss`; with `cotangents`, predictions["predictions"] receives the
-    predictions, unpacked from that forward as __call__ unpacks its step's.  Returns the run, whose
-    finish() gives (input_grads, forcing_grads)."""
+    predictions, unpacked from that forward as __call__ unpacks its step's; with `directions`, the
+    cotangents have a leading "direction" dim and every direction shares that forward and backward
+    pass.  Returns the run, whose finish() gives (input_grads, forcing_grads)."""
     state = {}
 
     def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
       eng = self._engine
       if "run" not in state:
         plan = feedback.FeedbackPlan.all_channels(inputs, template, forcings)
+        dirs = None
+        if directions:
+          state["cot"] = self._direction_cotangent_planes(cotangents, template, state["batch"])
+          dirs = state["cot"].shape[0]
         state["run"] = _InputGradRun(self, plan, norm, inputs, forcings, 1, state["batch"],
-                                     release_staging=False)
-        if cotangents is not None:
+                                     release_staging=False, dirs=dirs)
+        if cotangents is not None and not directions:
           state["cot"] = self._cotangent_planes(cotangents, template, state["run"].batch)
         if coef is not None:
           state["coef"] = torch.as_tensor(np.asarray(coef, np.float64)).to(eng.device)
@@ -467,8 +517,9 @@ class GraphCast(Predictor):
         kw = dict(lat_weight=self._lat_weight(targets, eng.device), coef=state["coef"],
                   channel_sums=channel_sums)
       else:
-        seed = torch.empty([eng.n_out, eng.num_grid], dtype=torch.float32, device=eng.device)
-        seed.copy_(state["cot"][b])
+        cot = state["cot"][:, b] if directions else state["cot"][b]
+        seed = torch.empty(list(cot.shape), dtype=torch.float32, device=eng.device)
+        seed.copy_(cot)
         operands["cotangent"] = seed
         kw = {}
       state["run"].element(b, 0, operands, planes_out=planes_out, **kw)
@@ -480,9 +531,10 @@ class GraphCast(Predictor):
       predictions["predictions"] = out
     return state["run"]
 
-  def _cotangent_planes(self, cotangents, template: xs.Dataset, batch: int) -> torch.Tensor:
+  def _cotangent_planes(self, cotangents, template: xs.Dataset, batch: int,
+                        out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """[batch, n_out, Ng] float32 host planes of a cotangent Dataset shaped like the one-step
-    `template`, in the predictions' channel order."""
+    `template`, in the predictions' channel order (written into `out` when given)."""
     cotangents = xs.from_xarray(cotangents)
     slabs = self._check_template(template, self._engine.n_out)
     if set(cotangents.keys()) != set(template.keys()):
@@ -490,7 +542,8 @@ class GraphCast(Predictor):
                        f"{sorted(template.keys())}")
     n_lat, n_lon = template.sizes["lat"], template.sizes["lon"]
     sizes = {"batch": batch, "lat": n_lat, "lon": n_lon}
-    out = torch.empty([batch, self._engine.n_out, n_lat * n_lon], dtype=torch.float32)
+    if out is None:
+      out = torch.empty([batch, self._engine.n_out, n_lat * n_lon], dtype=torch.float32)
     for s in slabs:
       v = cotangents.data_vars[s.name]
       if tuple(v.shape) != tuple(template.data_vars[s.name].shape):
@@ -501,17 +554,31 @@ class GraphCast(Predictor):
           np.asarray(src, np.float32)).reshape(batch, s.count, n_lat * n_lon)
     return out
 
+  def _direction_cotangent_planes(self, cotangents, template: xs.Dataset, batch: int) -> torch.Tensor:
+    """[K, batch, n_out, Ng] float32 host planes of cotangents with a leading "direction" dim, direction
+    k packed as _cotangent_planes packs cotangent k alone."""
+    cotangents = xs.from_xarray(cotangents)
+    dirs = next(iter(cotangents.data_vars.values())).shape[0]
+    out = torch.empty([dirs, batch, self._engine.n_out, self._engine.num_grid], dtype=torch.float32)
+    for k in range(dirs):
+      self._cotangent_planes(cotangents.isel({feedback.DIRECTION: k}), template, batch, out=out[k])
+    return out
+
   def _input_grads(self, stash: "StepStash", plan, norm: Optional[FusedNormalization],
                    inputs: xs.Dataset, forcings: xs.Dataset, *, lat_weight=None, coef=None,
-                   cotangents=None):
+                   cotangents=None, directions: bool = False):
     """Gradients with respect to the inputs and forcings of the steps `stash` holds (several target
     times): for every batch element, last step first, the step's planes are uploaded again, packed
     and differentiated by Engine.input_grads_element with the all-channel feedback `plan` of the
     following step.  The seed is the loss (lat_weight, coef; the stash holds the target planes) or,
-    with `cotangents` (per step [batch, n_out, Ng] host planes), J = sum cotangents * predictions.
-    Returns (input_grads, forcing_grads) Datasets shaped like `inputs` and `forcings`."""
+    with `cotangents` (per step [batch, n_out, Ng] host planes), J = sum cotangents * predictions;
+    with `directions`, per step [K, batch, n_out, Ng] planes of K cotangents that share every step's
+    backward pass.  The stash is only read, so several calls can differentiate the same forward.
+    Returns (input_grads, forcing_grads) Datasets shaped like `inputs` and `forcings` (with a leading
+    "direction" dim for `directions`)."""
     run = _InputGradRun(self, plan, norm, inputs, forcings, len(stash.steps), stash.batch,
-                        release_staging=True)
+                        release_staging=True,
+                        dirs=cotangents[0].shape[0] if directions else None)
     eng = self._engine
     dev = eng.device
     coef_dev = None if coef is None else torch.as_tensor(np.asarray(coef, np.float64)).to(dev)
@@ -530,13 +597,14 @@ class GraphCast(Predictor):
           eng.pack_inputs(operands["planes"], mean=norm.in_mean, scale=norm.in_scale)
           operands.update(scale=norm.out_scale, offset=norm.out_offset,
                           add_planes=operands.pop("planes"), add_plane_index=norm.add_plane_index)
-        seed = torch.empty([eng.n_out, eng.num_grid], dtype=torch.float32, device=dev)
+        lead = [cotangents[t].shape[0]] if directions else []
+        seed = torch.empty(lead + [eng.n_out, eng.num_grid], dtype=torch.float32, device=dev)
         if cotangents is None:
           seed.copy_(saved[1][b], non_blocking=True)
           operands["targets_planes"] = seed
           kw = dict(lat_weight=lat_weight, coef=coef_dev)
         else:
-          seed.copy_(cotangents[t][b])
+          seed.copy_(cotangents[t][:, b] if directions else cotangents[t][b])
           operands["cotangent"] = seed
           kw = {}
         del seed
@@ -832,22 +900,53 @@ def batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents, di
   it = None if input_tangents is None else xs.from_xarray(input_tangents)
   ft = None if forcing_tangents is None else xs.from_xarray(forcing_tangents)
   dirs, labels = feedback.check_direction_tangents(it, inputs, ft, forcings)
-  per = dirs if directions_per_pass is None else directions_per_pass
-  if isinstance(per, bool) or not isinstance(per, (int, np.integer)) or per < 1:
-    raise ValueError(f"directions_per_pass must be None or an int >= 1, not {directions_per_pass!r}")
   at = lambda ds, sl: None if ds is None else ds.isel({feedback.DIRECTION: sl})
-  predictions, parts = None, []
-  for k0 in range(0, dirs, int(per)):
-    sl = slice(k0, min(k0 + int(per), dirs))
-    p, t = one_pass(at(it, sl), at(ft, sl))
+  return direction_passes(lambda sl: one_pass(at(it, sl), at(ft, sl)), dirs, labels,
+                          directions_per_pass)
+
+
+def batched_vjp(one_pass, targets_template, cotangents, directions_per_pass):
+  """batched_input_vjp of a predictor stack: checks the cotangents against the template
+  (feedback.check_direction_cotangents) and directions_per_pass before anything runs, then runs
+  one_pass(cotangents, first) -> (predictions, input_grads, forcing_grads) on consecutive slices of the
+  directions (direction_passes).  Only the first pass (first=True) need form the predictions: the later
+  ones' are dropped, so they need not hold a second copy on the device."""
+  cot = xs.from_xarray(cotangents)
+  dirs, labels = feedback.check_direction_cotangents(cot, xs.from_xarray(targets_template))
+  return direction_passes(lambda sl: one_pass(cot.isel({feedback.DIRECTION: sl}), sl.start == 0),
+                          dirs, labels, directions_per_pass)
+
+
+def direction_passes(one_pass, dirs: int, labels, directions_per_pass):
+  """The passes of a batched call of `dirs` directions: one_pass(sl) -> (predictions, *results) runs
+  on ceil(K / directions_per_pass) consecutive slices sl of the directions (feedback.direction_slices,
+  which checks directions_per_pass first), each result a Dataset with a leading "direction" dim.
+  Returns (predictions of the first pass, *each result joined along "direction" over the passes and
+  labelled `labels`)."""
+  predictions, parts = None, None
+  for sl in feedback.direction_slices(dirs, directions_per_pass):
+    p, *results = one_pass(sl)
     predictions = p if predictions is None else predictions
-    parts.append(t)
+    parts = [[r] for r in results] if parts is None else [a + [r] for a, r in zip(parts, results)]
+  return (predictions,) + tuple(join_directions(a, labels) for a in parts)
+
+
+def join_directions(parts, labels) -> xs.Dataset:
+  """Datasets with the same variables, each with a leading "direction" dim (consecutive slices of the
+  directions, in order), joined along it and labelled `labels`.  The data stay torch tensors or numpy
+  arrays, as the parts hold them."""
   out = xs.Dataset(coords=parts[0].coords)
   out.coords[feedback.DIRECTION] = ((feedback.DIRECTION,), np.asarray(labels))
   for name, v in parts[0].data_vars.items():
-    data = v.data if len(parts) == 1 else torch.cat([t.data_vars[name].data for t in parts], dim=0)
+    data = [p.data_vars[name].data for p in parts]
+    if len(data) == 1:
+      data = data[0]
+    elif isinstance(data[0], torch.Tensor):
+      data = torch.cat(data, dim=0)
+    else:
+      data = np.concatenate(data, axis=0)
     out[name] = xs.DataArray(data, v.dims)
-  return predictions, out
+  return out
 
 
 def innermost_graphcast(predictor) -> Optional[GraphCast]:
@@ -921,11 +1020,17 @@ class _InputGradRun:
   Batched inputs are reduced into a buffer allocated after the element's backward pass and copied
   without a synchronisation into pinned host memory (torch's caching host allocator: allocated on the
   first call, reused after), so that the 0.25 degree inputs' 1.9 GB never coexist with a backward pass
-  and cross PCIe at full speed; finish() synchronises once.  The returned arrays are views of it."""
+  and cross PCIe at full speed; finish() synchronises once.  The returned arrays are views of it.
+
+  dirs = K (batched_input_vjp): K cotangents share every step, fb.a is [K, n_rows, Ng], and every
+  result buffer has a leading axis of K directions, each reduced as one direction's would be."""
 
   def __init__(self, model: GraphCast, plan, norm: Optional[FusedNormalization], inputs: xs.Dataset,
-               forcings: xs.Dataset, num_steps: int, batch: int, release_staging: bool):
+               forcings: xs.Dataset, num_steps: int, batch: int, release_staging: bool,
+               dirs: Optional[int] = None):
     eng = self.eng = model.engine
+    self.dirs = dirs
+    lead = [] if dirs is None else [dirs]
     eng.input_grads_begin()
     self.fb = eng.feedback(plan, None if norm is None else norm.add_plane_index,
                            None if norm is None else norm.in_scale)
@@ -942,9 +1047,9 @@ class _InputGradRun:
     for v in self.var_rows:
       if v.forcing or not v.batched:
         shape = ([batch] if v.batched else []) + ([num_steps] if v.timed else []) + [v.count, self._width(v)]
-        self.dev_bufs[v.key] = torch.zeros(shape, dtype=torch.float32, device=dev)
+        self.dev_bufs[v.key] = torch.zeros(lead + shape, dtype=torch.float32, device=dev)
       else:
-        self.host[v.key] = torch.empty([batch, v.count, self._width(v)], dtype=torch.float32,
+        self.host[v.key] = torch.empty(lead + [batch, v.count, self._width(v)], dtype=torch.float32,
                                        pin_memory=True)
       self.rows[v.key] = torch.arange(v.start, v.start + v.count, dtype=torch.int32, device=dev)
 
@@ -964,16 +1069,27 @@ class _InputGradRun:
       self.fb.a = None
 
   def _reduce(self, v, b: int, t: int) -> None:
-    eng, fb = self.eng, self.fb
-    if v.key in self.host:                 # a batched input
-      out = torch.empty([v.count, self._width(v)], dtype=torch.float32, device=eng.device)
-      eng.broadcast_grad_sum(fb.a, self.n_lat, self.rows[v.key], v.mode, out, False)
-      self.host[v.key][b].copy_(out, non_blocking=True)   # stream-ordered before out's reuse
+    if self.dirs is None:
+      self._reduce_one(v, b, t, self.fb.a, self.host.get(v.key), self.dev_bufs.get(v.key))
       return
-    out = self.dev_bufs[v.key][b] if v.batched else self.dev_bufs[v.key]
+    for k in range(self.dirs):
+      host, dev = self.host.get(v.key), self.dev_bufs.get(v.key)
+      self._reduce_one(v, b, t, self.fb.a[k], None if host is None else host[k],
+                       None if dev is None else dev[k])
+
+  def _reduce_one(self, v, b: int, t: int, a: torch.Tensor, host: Optional[torch.Tensor],
+                  dev: Optional[torch.Tensor]) -> None:
+    """The rows of one direction's gradient a [n_rows, Ng] into its result buffer (host or dev)."""
+    eng = self.eng
+    if host is not None:                   # a batched input
+      out = torch.empty([v.count, self._width(v)], dtype=torch.float32, device=eng.device)
+      eng.broadcast_grad_sum(a, self.n_lat, self.rows[v.key], v.mode, out, False)
+      host[b].copy_(out, non_blocking=True)   # stream-ordered before out's reuse
+      return
+    out = dev[b] if v.batched else dev
     out = out[t] if v.timed else out
     accumulate = (not v.batched and b > 0) or (v.forcing and not v.timed and t < self.num_steps - 1)
-    eng.broadcast_grad_sum(fb.a, self.n_lat, self.rows[v.key], v.mode, out, accumulate)
+    eng.broadcast_grad_sum(a, self.n_lat, self.rows[v.key], v.mode, out, accumulate)
 
   def finish(self):
     """(input_grads, forcing_grads) Datasets shaped like the inputs and forcings."""
@@ -981,7 +1097,7 @@ class _InputGradRun:
     torch.cuda.current_stream(self.eng.device).synchronize()
     grads.update({key: t.numpy() for key, t in self.host.items()})
     return feedback.grads_to_datasets(self.var_rows, grads, self.inputs, self.forcings, self.n_lat,
-                                      self.n_lon)
+                                      self.n_lon, directions=self.dirs)
 
 
 class _TangentRun:

@@ -270,6 +270,16 @@ class InputsAndResiduals(graphcast.Predictor):
                                                                  "input gradients")
     return self._predictor._input_vjp(inputs, targets_template, forcings, cotangents, norm=consts)
 
+  def batched_input_vjp(self, inputs, targets_template, forcings, cotangents, *,
+                        directions_per_pass=None, **kwargs):
+    """input_vjp of K cotangents at once (GraphCast.batched_input_vjp), of the un-normalised
+    predictions.  GraphCast only."""
+    def one_pass(cot, first):
+      ins, tt, fs, consts = self._fused_for(inputs, targets_template, forcings, "input gradients")
+      return self._predictor._input_vjp(ins, tt, fs, cot, norm=consts, directions=True,
+                                        predictions=first)
+    return graphcast.batched_vjp(one_pass, targets_template, cotangents, directions_per_pass)
+
   def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
                 **kwargs):
     """(predictions, prediction_tangents) of the un-normalised predictions of __call__

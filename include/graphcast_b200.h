@@ -432,6 +432,16 @@ int gcb_layernorm_jvp_dirs(const float* z, int32_t ld_z, const float* dz, int32_
                            int32_t dirs, const float* residual, int32_t ld_res, float* out,
                            int32_t ld_out, void* stream);
 
+/* Several cotangents at one primal (GraphCast.batched_input_vjp), stacked as above: the LayerNorm
+ * backward of each direction,
+ *   dz[k] = rstd * (dy[k]*scale - mean(dy[k]*scale) - zhat*mean(dy[k]*scale*zhat)),
+ * n = 512, bit for bit the dz of gcb_layernorm_backward for dy[k] alone, without the column sums (the
+ * parameter gradients are not formed for several directions).  z's row and its statistics are formed
+ * once for all directions.  dz may not alias dy or z; its pad rows between directions are not written. */
+int gcb_layernorm_backward_dirs(const float* dy, int32_t ld_dy, const float* z, int32_t ld_z,
+                                const float* scale, int64_t rows, int32_t n, int64_t dir_stride,
+                                int32_t dirs, float* dz, int32_t ld_dz, void* stream);
+
 /* Backward of a gather v[senders] (jax_gather, utils/typed_graph_net.py:124-125,431-445):
  *   out[i, 0:512] = sum_{j in [ptr[i], ptr[i+1])} msg[order[j], 0:512]
  * (order / ptr: the sender CSR of an edge set, host-built), summed in j order; the rows listed in
@@ -676,7 +686,8 @@ typedef enum {
                              * gcb_segment_sum_sorted, gcb_gather_add, gcb_swish_rows,
                              * gcb_output_loss_grad_feedback, gcb_input_grad,
                              * gcb_output_cotangent_grad_feedback, gcb_broadcast_grad_sum,
-                             * gcb_layernorm_jvp, gcb_swish_jvp, gcb_layernorm_jvp_dirs */
+                             * gcb_layernorm_jvp, gcb_swish_jvp, gcb_layernorm_jvp_dirs,
+                             * gcb_layernorm_backward_dirs */
   GCB_KIND_NOISE = 11       /* gcb_add_gaussian_noise */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
