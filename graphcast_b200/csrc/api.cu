@@ -124,6 +124,8 @@ int validate_segment(const gcb_segment& g) {
   return GCB_OK;
 }
 
+int g_cluster_size = 2;   // CTAs per cluster sharing the weight stream (1, 2 or 4)
+
 int validate_layer(const gcb_layer_desc* d) {
   GCB_CHECK_ARG(d != nullptr, "null descriptor");
   GCB_CHECK_ARG(d->rows >= 0, "rows < 0");
@@ -144,8 +146,19 @@ int validate_layer(const gcb_layer_desc* d) {
   GCB_CHECK_ARG(d->out != nullptr || d->out_y != nullptr || d->out_img != nullptr, "no output");
   if (d->out) GCB_CHECK_ARG(aligned16(d->out) && d->ld_out % 4 == 0 && d->ld_out >= d->n_valid, "out unaligned");
   if (d->out_y) GCB_CHECK_ARG(aligned16(d->out_y) && d->ld_out_y % 4 == 0 && d->ld_out_y >= d->n_valid, "out_y unaligned");
-  if (d->residual) GCB_CHECK_ARG(aligned16(d->residual) && d->ld_res % 4 == 0, "residual unaligned");
+  if (d->residual) {
+    GCB_CHECK_ARG(aligned16(d->residual) && d->ld_res % 4 == 0, "residual unaligned");
+    GCB_CHECK_ARG(d->ld_res >= d->n_valid, "ld_res must be >= n_valid");
+    // The tensor-core epilogue adds the residual to the image only next to an fp32 output.
+    GCB_CHECK_ARG(d->out != nullptr || d->out_y != nullptr, "a residual needs out or out_y");
+  }
   GCB_CHECK_ARG(d->act == GCB_ACT_NONE || d->act == GCB_ACT_SWISH, "unknown activation");
+  // The tensor-core epilogue forms the LayerNorm statistics before the activation, and over
+  // 512 columns combines two 256-column halves of equal width (mlp_tc.cuh ln_pair_stats).
+  GCB_CHECK_ARG(!(d->act == GCB_ACT_SWISH && d->ln_scale != nullptr),
+                "a layer is swish OR LayerNorm, not both");
+  if (d->ln_scale != nullptr && d->n == 512)
+    GCB_CHECK_ARG(d->n_valid == 512, "LayerNorm with n = 512 needs n_valid = 512");
   GCB_CHECK_ARG(d->n_pre_add >= 0 && d->n_pre_add <= 2, "n_pre_add must be 0..2");
   if (d->n_pre_add > 0) {
     GCB_CHECK_ARG(d->ln_scale == nullptr, "pre_add cannot be combined with LayerNorm");
@@ -160,11 +173,13 @@ int validate_layer(const gcb_layer_desc* d) {
   } else {
     GCB_CHECK_ARG(d->precision == GCB_PREC_BF16X3 || d->precision == GCB_PREC_BF16, "unknown precision");
     GCB_CHECK_ARG(d->w_packed != nullptr && aligned16(d->w_packed), "w_packed null/unaligned");
+    // A consumer warpgroup holds the accumulator of one 256-column unit only: LayerNorm over a
+    // 512-wide row needs the N-split schedule, where each CTA of the pair owns one half.
+    if (d->ln_scale != nullptr && d->n == 512)
+      GCB_CHECK_ARG(g_cluster_size == 2, "LayerNorm with n = 512 needs the cluster size 2 (N-split) schedule");
   }
   return GCB_OK;
 }
-
-int g_cluster_size = 2;   // CTAs per cluster sharing the weight stream (1, 2 or 4)
 
 // Launches the persistent kernel kKernel (kThreads threads per CTA, clusters of csize CTAs)
 // on `clusters` clusters, or as many as are resident at once if that is fewer, with `smem`
@@ -210,11 +225,7 @@ int launch_persistent(int smem_max, int smem, int csize, int clusters, cudaStrea
 template <bool kSplit, bool kSwish, bool kLN>
 int launch_tc_variant(const gcb_layer_desc& d, cudaStream_t stream) {
   constexpr int smem = gcb::TcConfig<kSplit, kLN>::kSmemBytes;
-  const int csize = g_cluster_size;
-  // A consumer warpgroup holds the accumulator of one 256-column unit only: LayerNorm over a
-  // 512-wide row needs the N-split schedule, where each CTA of the pair owns one half.
-  if (kLN && d.n == 512 && csize != 2)
-    return fail(GCB_ERR_INVALID, "LayerNorm with n = 512 needs the cluster size 2 (N-split) schedule");
+  const int csize = g_cluster_size;     // validate_layer: 2 for LayerNorm over 512 columns
   const int tiles = (d.rows + gcb::kTileM - 1) / gcb::kTileM;
   // N-split schedule (n = 512, cluster of 2): one tile per cluster at a time; otherwise
   // every CTA of the cluster has its own tile.
@@ -225,8 +236,7 @@ int launch_tc_variant(const gcb_layer_desc& d, cudaStream_t stream) {
 
 template <bool kSplit>
 int launch_tc(const gcb_layer_desc& d, cudaStream_t stream) {
-  const bool swish = d.act == GCB_ACT_SWISH, ln = d.ln_scale != nullptr;
-  if (swish && ln) return launch_tc_variant<kSplit, true, true>(d, stream);
+  const bool swish = d.act == GCB_ACT_SWISH, ln = d.ln_scale != nullptr;   // not both (validate_layer)
   if (swish) return launch_tc_variant<kSplit, true, false>(d, stream);
   if (ln) return launch_tc_variant<kSplit, false, true>(d, stream);
   return launch_tc_variant<kSplit, false, false>(d, stream);

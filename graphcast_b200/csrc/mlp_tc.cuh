@@ -11,7 +11,7 @@
 //     distributed shared memory.  Consecutive units of a CTA are consecutive tiles.
 //   unsplit (n = 256, or cluster of 1 / 4): every CTA walks its own tiles (n/256 units per
 //     tile); the CTAs of a cluster share the weight stream by multicast.  LayerNorm over
-//     512 columns needs the N-split schedule (the launcher enforces it).
+//     512 columns needs the N-split schedule and n_valid = 512 (validate_layer enforces both).
 // Warp roles:
 //   warp 0        TMA lane: per K-step streams (a) 1/cluster of the pre-packed bf16 weight
 //                 tile with cp.async.bulk, multicast to every CTA of the cluster, and (b)
@@ -409,6 +409,8 @@ __device__ __forceinline__ uint32_t stage_addends(float* s_g, uint64_t* g_full_b
 template <bool kSplit, bool kSwish, bool kLN>
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
+  // row_shifted_sums takes the LayerNorm statistics of acc + bias, i.e. before any activation.
+  static_assert(!(kSwish && kLN), "a layer is swish or LayerNorm, not both");
   using Cfg = TcConfig<kSplit, kLN>;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* stage_base = smem;
@@ -645,7 +647,8 @@ mlp_layer_tc_kernel(const __grid_constant__ gcb_layer_desc d) {
     const int n_valid = d.n_valid;
     const bool lead = lane == 0 && (warp & 3) == 0;
     const uint32_t rel_mask = csize == 1 ? 0u : cmask;
-    // The image holds residual + y when an fp32 output is written, y otherwise.
+    // The image holds residual + y when an fp32 output is written, y otherwise (validate_layer
+    // refuses a residual with out_img alone).
     const bool img_res = res_ptr != nullptr && (out_ptr != nullptr || outy_ptr != nullptr);
     uint32_t stage = 0, phase = 0, g_count = 0, ln_count = 0, u = 0;
     float acc[128];

@@ -80,11 +80,15 @@ typedef struct {
 } gcb_pre_add;
 
 /* One fused linear layer over `rows` rows:
- *     z   = concat(segments)                         [rows, K],  K = sum k
- *     y   = act(z @ W + bias + sum_p pre_add_p)      [rows, n]
- *     y   = LayerNorm(y) * ln_scale + ln_offset      (if ln_scale != NULL; eps 1e-5)
+ *     z   = concat(segments)                         [rows, K],  K = sum k <= 2048
+ *     y   = z @ W + bias + sum_p pre_add_p           [rows, n]
+ *     y   = swish(y)                                 (if act == GCB_ACT_SWISH)
+ *       or  LayerNorm(y) * ln_scale + ln_offset      (if ln_scale != NULL; eps 1e-5; statistics
+ *                                                     over the n_valid columns)
  *     out_y[r] = y[r]                                (if out_y  != NULL)
  *     out[r]   = (residual ? residual[r] : 0) + y[r] (if out    != NULL)
+ * A layer is swish OR LayerNorm, not both.  LayerNorm with n = 512 needs n_valid = 512 and the
+ * cluster size 2 (gcb_set_cluster_size) on the tensor-core precisions; with n = 256 any n_valid.
  * Replaces one hk.Linear (+ jax.nn.swish | + hk.LayerNorm + residual add) of
  * build_mlp_with_maybe_layer_norm (utils/legacy/deep_typed_graph_net.py:205-247),
  * the concat of jraph.concatenated_args, and the residuals of _process_step
@@ -101,11 +105,11 @@ typedef struct {
   const float* ln_scale;  /* [n] or NULL */
   const float* ln_offset; /* [n] or NULL (required iff ln_scale) */
   int32_t act;          /* gcb_activation */
-  const float* residual; int32_t ld_res;
+  const float* residual; int32_t ld_res;  /* ld_res >= n_valid; needs out or out_y */
   float* out;   int32_t ld_out;
   float* out_y; int32_t ld_out_y;
   int32_t precision;    /* gcb_precision */
-  int32_t n_pre_add;    /* 0..2; requires ln_scale == NULL and n_valid % 32 == 0 */
+  int32_t n_pre_add;    /* 0..2; requires ln_scale == NULL and n_valid == n */
   gcb_pre_add pre_add[2];
   /* Operand images.  The "A image" of a [rows, k] fp32 matrix is its bf16 hi/lo split
    * stored tile by tile in the exact shared-memory layout of the tensor-core A operand:
@@ -217,7 +221,11 @@ int gcb_add_gaussian_noise(const gcb_noise_segment* segments, int32_t n_segments
 
 /* CTAs per thread-block cluster of the tensor-core layer kernel (1, 2 or 4; default
  * 2).  The CTAs of a cluster process consecutive row tiles in lockstep and receive
- * each weight tile once from L2 through TMA multicast.  Process-wide tuning knob. */
+ * each weight tile once from L2 through TMA multicast.  Process-wide tuning knob; the
+ * results are bit-identical at every size.  The chain kernel always runs clusters of 2.
+ * Sizes 1 and 4 refuse LayerNorm layers with n = 512 (see gcb_layer_desc), so they serve
+ * gcb_forward with fuse = 1 (whose layer-by-layer launches carry no such layer) but not
+ * fuse = 0, nor the forward recompute of the backward passes (graphcast_b200/backward.py). */
 int gcb_set_cluster_size(int32_t ctas);
 
 /* Launch one fused layer. */

@@ -80,6 +80,62 @@ def test_layer_validation_rejects_bad_descriptors():
     _native.check(-1, "x")
 
 
+def test_layer_refusals_name_the_unsupported_case():
+  """Layers the kernels cannot compute are refused by the argument checks: status -1, and
+  gcb_last_error says why.  The pointers are dummies and rows = 0, so a descriptor that passed the
+  checks would return 0 without a launch."""
+  lib = _native.lib()
+
+  def layer(n=512, n_valid=512, ks=(512,), act=_native.ACT_NONE, ln=False, ld_res=None,
+            prec=_native.PREC_BF16X3):
+    d = _native.LayerDesc()
+    d.rows, d.n, d.n_valid, d.nseg = 0, n, n_valid, len(ks)
+    for i, k in enumerate(ks):
+      d.seg[i].table, d.seg[i].ld, d.seg[i].k, d.seg[i].k_valid, d.seg[i].fan = 256, k, k, k, 1
+    d.w_packed, d.w_f32, d.bias, d.out, d.ld_out = 256, 256, 256, 256, 512
+    d.act = act
+    if ln:
+      d.ln_scale = d.ln_offset = 256
+    if ld_res is not None:
+      d.residual, d.ld_res = 256, ld_res
+    d.precision = prec
+    return d
+
+  def refused(d, why):
+    assert lib.gcb_layer_forward(C.byref(d), None) == -1
+    assert why in lib.gcb_last_error(), lib.gcb_last_error()
+
+  def accepted(d):
+    assert lib.gcb_layer_forward(C.byref(d), None) == 0, lib.gcb_last_error()
+
+  refused(layer(ks=(1024, 512, 528)), b"K too large")           # 129 K-steps: 2048 is the limit
+  accepted(layer(ks=(1024, 512, 512)))
+  for prec in (_native.PREC_BF16X3, _native.PREC_BF16, _native.PREC_FP32_SIMT):
+    # the tensor-core epilogue takes the LayerNorm statistics before the activation
+    refused(layer(act=_native.ACT_SWISH, ln=True, prec=prec), b"swish OR LayerNorm")
+    refused(layer(act=_native.ACT_SWISH, ln=True, n=256, n_valid=256, prec=prec), b"swish OR LayerNorm")
+    # ... and over 512 columns combines two 256-column halves of equal width
+    for n_valid in (508, 474, 256, 200):
+      refused(layer(n_valid=n_valid, ln=True, prec=prec), b"needs n_valid = 512")
+    refused(layer(n_valid=474, ld_res=472, prec=prec), b"ld_res must be >= n_valid")
+    d = layer(ld_res=512, prec=prec)    # the tensor-core epilogue adds it to out_img only beside out
+    d.out, d.out_img = None, 256
+    refused(d, b"a residual needs out or out_y")
+    d.out_y, d.ld_out_y = 256, 512
+    accepted(d)
+  for bad in (0, 3, 8, -1):
+    assert lib.gcb_set_cluster_size(bad) == -1
+    assert b"cluster size must be 1, 2 or 4" in lib.gcb_last_error()
+  try:
+    for cs in (1, 4):     # one 256-column accumulator per warpgroup: LayerNorm over 512 needs the pair
+      assert lib.gcb_set_cluster_size(cs) == 0
+      refused(layer(ln=True), b"needs the cluster size 2")
+      accepted(layer(ln=True, n=256, n_valid=227))
+      accepted(layer(ln=True, prec=_native.PREC_FP32_SIMT))     # no clusters on the SIMT arm
+  finally:
+    assert lib.gcb_set_cluster_size(2) == 0
+
+
 def test_debug_flags_accepts_only_zero():
   """The build has no kernel experiment switches: 0 is accepted, anything else is an error."""
   lib = _native.lib()
