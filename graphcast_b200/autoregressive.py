@@ -253,25 +253,37 @@ class Predictor(graphcast.Predictor):
     return parts
 
   @staticmethod
-  def _checkpointed_loss(model, norm_of, inputs, targets, forcings):
+  def _checkpointed_loss(model, norm_of, inputs, targets, forcings, tangent_run=None):
     """The forward of a gradient over several target times: the device path of `loss`, which also
     keeps every step's input and target planes in pinned host memory (graphcast.StepStash).  Returns
     (loss, diagnostics, stash, first step's {inputs, targets, forcings, norm}, latitude weights,
     loss-derivative coefficients 2 kappa / (batch * steps)).  first["inputs"] is the layout of step 0's
     inputs only (_layout): the stash holds their values, and the tensors of noised inputs (1.9 GB at
-    0.25 degree) must not outlive the forward."""
+    0.25 degree) must not outlive the forward.
+
+    With tangent_run (a graphcast._TangentRun of one direction: loss_and_input_hvp), every step also
+    carries the input tangent planes on the device (GraphCast._device_loss_tangent) and keeps them in
+    pinned host memory too: first["tangents"] is that StepStash."""
     records, first = [], {}
     stash = None
 
     def step(rng, inputs, targets_template, forcings):
       nonlocal stash
       norm = norm_of(inputs, targets_template, forcings)
-      finish, predictions, sums = model._device_loss(inputs, targets_template, forcings, norm, True)
+      if tangent_run is None:
+        finish, predictions, sums = model._device_loss(inputs, targets_template, forcings, norm, True)
+      else:
+        finish, predictions, sums, tangent = model._device_loss_tangent(
+            inputs, targets_template, forcings, norm, tangent_run)
       records.append((finish, sums))
       if stash is None:
         stash = graphcast.StepStash(model.engine.device)
         first.update(inputs=_layout(inputs), targets=targets_template, forcings=forcings, norm=norm)
+        if tangent_run is not None:
+          first["tangents"] = graphcast.StepStash(model.engine.device)
       model._stash_step(stash)
+      if tangent_run is not None:
+        first["tangents"].save(tangent)
       return predictions
 
     for _ in rollout.chunked_prediction_generator(
@@ -308,6 +320,37 @@ class Predictor(graphcast.Predictor):
     input_grads, forcing_grads = model._input_grads(stash, plan, first["norm"], inputs, forcings,
                                                     lat_weight=lat_weight, coef=coef)
     return loss, diagnostics, input_grads, forcing_grads
+
+  def loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
+                         rng=None, *, _noise_fold: int = 0, **kwargs):
+    """(loss, diagnostics, input_grads, forcing_grads, input_hvp, forcing_hvp): those of
+    loss_and_input_grads, bit for bit, and H v, H the Hessian of loss.mean() with respect to every
+    variable of `inputs` and `forcings` and v the tangents (GraphCast.loss_and_input_hvp; the forcing
+    tangents cover every target time).  One target time delegates to the inner predictor.  Several
+    need gradient_checkpointing=True: one rollout computes the loss of `loss`, keeps every step's input
+    and target planes and carries the input tangent planes on the device (as input_jvp does), keeping
+    them too; then, last step first, each step is recomputed with its tangent and differentiated with
+    the gradient and its tangent stacked (Engine.input_hvp_element), the pair carried from step to step
+    over every input channel.  With noise, everything is taken at noisy_inputs(inputs, targets,
+    forcings, rng)."""
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    forcings = xs.from_xarray(forcings)
+    if targets.sizes["time"] == 1:
+      return self._predictor.loss_and_input_hvp(inputs, targets, forcings, input_tangents,
+                                                forcing_tangents, **kwargs)
+    model, norm_of = self._checkpointed_parts(inputs, targets, forcings, "input gradients")
+    one = lambda ds: ds.isel(time=slice(0, 1))
+    run = graphcast._TangentRun(inputs, forcings, input_tangents, forcing_tangents,
+                                targets.sizes["time"],
+                                feedback.FeedbackPlan(inputs, one(targets), one(forcings)))
+    loss, diagnostics, stash, first, lat_weight, coef = self._checkpointed_loss(
+        model, norm_of, self._noised(inputs, targets, forcings, rng, _noise_fold), targets, forcings,
+        tangent_run=run)
+    del run
+    plan = feedback.FeedbackPlan.all_channels(first["inputs"], first["targets"], first["forcings"])
+    return (loss, diagnostics) + model._input_grads(stash, plan, first["norm"], inputs, forcings,
+                                                    lat_weight=lat_weight, coef=coef,
+                                                    tangents=first["tangents"])
 
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
     """(predictions, input_grads, forcing_grads): `predictions` as __call__ returns them, the gradients

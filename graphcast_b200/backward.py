@@ -133,6 +133,9 @@ class Backward:
     self.ws_wg = torch.empty([nb], dtype=torch.uint8, device=dev)
     # element(param_grads=False): the column sums of the row-wise kernels land here, never in info.g
     self.param_grads = True
+    # element(hvp=...): the tangent snapshots of the forward (tangent(snaps=...)); the walk then carries
+    # the gradient (direction 0) and its tangent (direction 1)
+    self.hvp = None
     self.sink = {f: torch.zeros([D], dtype=torch.float32, device=dev)
                  for f in ("b0", "b1", "scale", "offset")}
 
@@ -288,7 +291,7 @@ class Backward:
     return y
 
   def mlp_backward(self, info: _MlpInfo, rows: int, segs, dy: torch.Tensor, *, pre=None,
-                   w0=None, dw_segs=None) -> torch.Tensor:
+                   w0=None, dw_segs=None, tan=None) -> torch.Tensor:
     """Backward of one MLP at the recomputed forward; accumulates its parameter gradients and returns
     dh [rows, 512], the gradient of the first layer's pre-activation (incl. pre-gathered addends).
     dw_segs: the layer-0 inputs whose weight blocks get X^T dh (default: all of `segs`).
@@ -296,11 +299,18 @@ class Backward:
     With self.dirs > 1 (no parameter gradients), dy and dh are stacked tables of that many directions
     of `rows` rows (dir_rows): h and z are recomputed once, the dX products run once over every
     direction, and the two nonlinearities are gcb_layernorm_backward_dirs and gcb_swish_jvp, whose
-    results are those of the one-direction kernels without the column sums."""
+    results are those of the one-direction kernels without the column sums.
+
+    In a Hessian-vector product (self.hvp set, two directions: the gradient and its tangent), `tan` =
+    (dsegs, dpre, dw0) is the tangent of the layer-0 input as mlp_jvp takes it (one direction, plain
+    gather indices): h-dot = dsegs W0 + the gathered addends, z-dot = W1 (swish'(h) h-dot), and the two
+    nonlinearities are gcb_layernorm_backward_jvp and gcb_swish_backward_jvp."""
     w = info.w
+    w0 = w0 or w.w0_packed
     nd, stride, rk = self.dirs, self.dir_stride(rows), self.dir_rows(rows)
     h = self.empty(rows)
-    self.layer(rows, segs, w0 or w.w0_packed, w.b0, _native.ACT_NONE, out_y=h, pre=pre)
+    self.layer(rows, segs, w0, w.b0, _native.ACT_NONE, out_y=h, pre=pre)
+    hd = None if self.hvp is None else self._hdot(rows, w0, tan)
     g = info.g if self.param_grads else self.sink
     ws = self.ws_rows
     if info.ln:
@@ -311,7 +321,18 @@ class Backward:
       self.layer(rows, [self.tab(a)], w.w1_packed, w.b1, out_y=z)
       del a
       dz = self.empty(rk)
-      if nd == 1:
+      if hd is not None:                     # z-dot = W1 (swish'(h) h-dot)
+        ad = self.empty(rows)
+        _native.check(self.lib.gcb_swish_jvp(h.data_ptr(), D, rows, D, hd.data_ptr(), D, rows, 1,
+                                             ad.data_ptr(), D, self._st()), "gcb_swish_jvp")
+        zd = self.empty(rows)
+        self.layer(rows, [self.tab(ad)], w.w1_packed, self.zero_bias, out_y=zd)
+        del ad
+        _native.check(self.lib.gcb_layernorm_backward_jvp(
+            dy.data_ptr(), dy.shape[1], z.data_ptr(), D, zd.data_ptr(), D, w.ln_scale, rows, D, stride,
+            dz.data_ptr(), D, self._st()), "gcb_layernorm_backward_jvp")
+        del zd
+      elif nd == 1:
         _native.check(self.lib.gcb_layernorm_backward(
             dy.data_ptr(), dy.shape[1], z.data_ptr(), D, w.ln_scale, rows, D, dz.data_ptr(), D,
             ws.data_ptr(), ws.numel(), g["b1"].data_ptr(), g["scale"].data_ptr(),
@@ -331,7 +352,13 @@ class Backward:
       self.wgrad(self.tab(h), dz, rows, g["w1"], n=info.n1, swish=True)     # dW1 = swish(h)^T dz
     da = self.empty(rk)
     self.layer(rk, [self.tab(dz, info.n1)], info.t["w1"], self.zero_bias, out_y=da)
-    if nd == 1:
+    if hd is not None:                       # [swish'(h) da; d/dt of it] in place
+      dh = da
+      _native.check(self.lib.gcb_swish_backward_jvp(
+          h.data_ptr(), D, hd.data_ptr(), D, rows, D, da.data_ptr(), D, stride, dh.data_ptr(), D,
+          self._st()), "gcb_swish_backward_jvp")
+      del hd
+    elif nd == 1:
       dh = self.empty(rows)
       _native.check(self.lib.gcb_swish_backward(
           da.data_ptr(), D, h.data_ptr(), D, rows, D, dh.data_ptr(), D, ws.data_ptr(), ws.numel(),
@@ -348,6 +375,20 @@ class Backward:
         self.wgrad(s, dh, rows, g["w0"][off:off + k])
         off += k
     return dh
+
+  def _hdot(self, rows: int, w0, tan) -> torch.Tensor:
+    """h-dot [rows, 512] of an MLP's first layer from tan = (dsegs, dpre, dw0) (see mlp_backward):
+    dsegs W0 (dw0: the weight of those segments, default w0) plus the gathered addends dpre, or the
+    addends alone; zeros when the layer input has no tangent."""
+    dsegs, dpre, dw0 = tan if tan is not None else ([], (), None)
+    if dsegs:
+      hd = self.empty(rows)
+      self.layer(rows, dsegs, dw0 or w0, self.zero_bias, out_y=hd, pre=list(dpre) or None)
+      return hd
+    hd = None
+    for table, idx in dpre:
+      hd = self.gather_add(table, idx, rows, hd)
+    return hd if hd is not None else torch.zeros([max(rows, 1), D], dtype=torch.float32, device=self.dev)
 
   def sender_sums(self, dh: torch.Tensor, rows: int, csr, num_nodes: int) -> torch.Tensor:
     """gcb_segment_sum_sorted (sender CSR `csr`) of every direction of the stacked edge table dh (`rows`
@@ -383,14 +424,22 @@ class Backward:
 
   def edge_backward(self, info: _MlpInfo, rows: int, e_seg, dm: torch.Tensor, snd_name: str,
                     v_s, n_s: int, snd: torch.Tensor, v_r, n_r: int, rcv: torch.Tensor,
-                    rcv_sum) -> tuple:
+                    rcv_sum, tan=None) -> tuple:
     """Backward of a pre-gathered edge MLP m = MLP([e | v_s[snd] | v_r[rcv]]): accumulates its
-    parameter gradients, returns (dH, S, R)."""
+    parameter gradients, returns (dH, S, R).  tan (Hessian-vector products): (edge tangent segments,
+    sender node tangent table, receiver node tangent table)."""
     sp = info.split
     ps = self.projection(n_s, v_s, sp.ws_packed)
     pr = self.projection(n_r, v_r, sp.wr_packed)
-    dh = self.mlp_backward(info, rows, [e_seg], dm, pre=[(ps, snd), (pr, rcv)], w0=sp.we_packed)
-    del ps, pr
+    t = None
+    if tan is not None:
+      de_segs, dv_s, dv_r = tan
+      dps = self.projection(n_s, self.tab(dv_s), sp.ws_packed)
+      dpr = self.projection(n_r, self.tab(dv_r), sp.wr_packed)
+      t = (de_segs, [(dps, snd), (dpr, rcv)], None)
+    dh = self.mlp_backward(info, rows, [e_seg], dm, pre=[(ps, snd), (pr, rcv)], w0=sp.we_packed,
+                           tan=t)
+    del ps, pr, t
     s = self.sender_sums(dh, rows, self.csr[snd_name], n_s)
     r = rcv_sum(dh)
     if self.param_grads:
@@ -401,7 +450,7 @@ class Backward:
 
   def bipartite_backward(self, name: str, info: _MlpInfo, enc: _MlpInfo, feat_t: torch.Tensor,
                          dagg: torch.Tensor, snd: torch.Tensor, rcv: torch.Tensor, v_s, n_s: int,
-                         v_r, n_r: int) -> tuple:
+                         v_r, n_r: int, tan=None) -> tuple:
     """Backward of a grid2mesh / mesh2grid edge MLP m = MLP([e | v_s[snd] | v_r[rcv]]) with
     e = MLP(edge features) and dm = dagg[rcv] (its edge residual is dead), chunk by chunk (see
     self.chunks): accumulates the parameter gradients of both MLPs and returns the node tables
@@ -410,10 +459,17 @@ class Backward:
     Several directions (self.dirs > 1, stacked dagg) use these same chunks, not tangent_chunks: S is
     added chunk by chunk, so its bits depend on where the chunks fall, and direction k is to be what
     one direction alone gives.  The stacked temporaries of a chunk therefore grow with the direction
-    count."""
+    count.
+
+    tan (Hessian-vector products): the node tangent tables (sender, receiver or None); the edge
+    embedder's output has no tangent."""
     sp = info.split
     ps = self.projection(n_s, v_s, sp.ws_packed)
     pr = self.projection(n_r, v_r, sp.wr_packed)
+    dps = dpr = None
+    if tan is not None:
+      dps = self.projection(n_s, self.tab(tan[0]), sp.ws_packed)
+      dpr = None if tan[1] is None else self.projection(n_r, self.tab(tan[1]), sp.wr_packed)
     s_tab, r_tab = None, self.empty(self.dir_rows(n_r))
     for i, (r0, r1, g0, g1, rp, heavy, n_heavy, csr) in enumerate(self.chunks[name]):
       n = r1 - r0
@@ -422,9 +478,12 @@ class Backward:
       e = self.fwd_mlp(enc, n, [f])
       dm = self.gather_add(dagg, self.kfold(rcv_c, n_r, (name, "backward", i, "rcv")),
                            self.dir_rows(n))
+      t = None
+      if dps is not None:
+        t = ([], [(dps, snd_c)] + ([] if dpr is None else [(dpr, rcv_c)]), None)
       dh = self.mlp_backward(info, n, [self.tab(e)], dm, pre=[(ps, snd_c), (pr, rcv_c)],
-                             w0=sp.we_packed)
-      del dm, e, snd_c, rcv_c
+                             w0=sp.we_packed, tan=t)
+      del dm, e, snd_c, rcv_c, t
       s_c = self.sender_sums(dh, n, csr, n_s)
       s_tab = s_c if s_tab is None else self.gather_add(
           s_c, self.kfold(self.iota[:n_s], n_s, ("iota", n_s)), self.dir_rows(n_s), s_tab)
@@ -438,7 +497,7 @@ class Backward:
         del de
       else:
         del dh
-    del ps, pr
+    del ps, pr, dps, dpr
     if self.param_grads:
       w0 = info.g["w0"]
       self.wgrad(v_s, s_tab, n_s, w0[D:2 * D])
@@ -448,7 +507,7 @@ class Backward:
   # -- one batch element ---------------------------------------------------------------------------
   def element(self, grid_in_img: torch.Tensor, g_out: torch.Tensor, snaps: dict,
               dgrid_in: bool = False, param_grads: bool = True,
-              dirs: int = 1) -> Optional[torch.Tensor]:
+              dirs: int = 1, hvp: Optional[dict] = None) -> Optional[torch.Tensor]:
     """Accumulates the parameter gradients of one batch element whose loss derivative with respect
     to the decoder output is g_out [Ng, 256] (gcb_output_loss_grad) and whose forward left `snaps`
     (whose entries are dropped as they are consumed).  dgrid_in: also return the derivative with
@@ -465,14 +524,23 @@ class Backward:
     table of K directions of Ng rows (dir_rows), and so is dx.  The gradient state is stacked like the
     tangent's, so every dX product is one GEMM over all directions and every MLP's h and z, the
     embedder recomputes and the sender / receiver projections are formed once; the segment sums run
-    per direction.  Direction k is bit for bit what g_out's direction k alone gives."""
+    per direction.  Direction k is bit for bit what g_out's direction k alone gives.
+
+    hvp (Hessian-vector products, dirs = 2, param_grads=False): the tangent snapshots of
+    tangent(snaps=...), entries dropped as they are consumed.  Direction 0 of g_out is the loss seed,
+    direction 1 its tangent; the walk is the same, every MLP also forms h-dot and z-dot from the
+    snapshots and differentiates its two nonlinearities with gcb_layernorm_backward_jvp and
+    gcb_swish_backward_jvp, so direction 1 of dx is the tangent of direction 0, and direction 0 is bit
+    for bit what g_out's direction 0 alone gives."""
     if dirs > 1 and param_grads:
       raise ValueError("several directions are supported without parameter gradients only")
-    self.param_grads, self.dirs = bool(param_grads), int(dirs)
+    if hvp is not None and (dirs != 2 or param_grads):
+      raise ValueError("a Hessian-vector product runs two directions without parameter gradients")
+    self.param_grads, self.dirs, self.hvp = bool(param_grads), int(dirs), hvp
     try:
       return self._element(grid_in_img, g_out, snaps, dgrid_in)
     finally:
-      self.param_grads, self.dirs = True, 1
+      self.param_grads, self.dirs, self.hvp = True, 1, None
 
   def _element(self, grid_in_img, g_out, snaps, dgrid_in):
     eng, m = self.eng, self.m
@@ -482,13 +550,18 @@ class Backward:
     img, tab = self.img, self.tab
     feat = lambda t: tab(t, 16, 4, 4)
     rk = self.dir_rows                       # rows of a stacked table (n rows for one direction)
+    T = self.hvp                             # tangent snapshots (Hessian-vector products) or None
+    tan = (lambda *segs, dw0=None: None) if T is None else (
+        lambda *segs, dw0=None: ([tab(t) for t in segs], (), dw0))
 
     # ---- decoder: out = MLP(vg2);  vg2 = vg1 + MLP([vg1 | agg3]);  m3 = MLP([e3 | v[snd] | vg1[rcv]])
-    dh = self.mlp_backward(mp["dec_grid"], ng, [img(snaps["vg2"])], g_out)
+    dh = self.mlp_backward(mp["dec_grid"], ng, [img(snaps["vg2"])], g_out,
+                           tan=tan(*(() if T is None else (T.pop("vg2"),))))
     dvg2 = self.empty(rk(ng))
     self.layer(rk(ng), [tab(dh)], mp["dec_grid"].t["w0_0"], self.zero_bias, out_y=dvg2)
     info = mp["proc_n_grid_m2g"]
-    dh = self.mlp_backward(info, ng, [img(snaps["vg1"]), img(snaps["agg3"])], dvg2)
+    dh = self.mlp_backward(info, ng, [img(snaps["vg1"]), img(snaps["agg3"])], dvg2,
+                           tan=tan(*(() if T is None else (T["vg1"], T.pop("agg3")))))
     dvg1 = self.empty(rk(ng))
     self.layer(rk(ng), [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dvg2, out=dvg1)
     dagg3 = self.empty(rk(ng))
@@ -496,7 +569,8 @@ class Backward:
     del dh, dvg2
     info = mp["proc_e_m2g"]
     S, R = self.bipartite_backward("m2g", info, mp["enc_e_m2g"], eng.m2g_feat, dagg3, eng.m2g_snd,
-                                   eng.m2g_rcv, img(snaps["v"][K]), nm, img(snaps["vg1"]), ng)
+                                   eng.m2g_rcv, img(snaps["v"][K]), nm, img(snaps["vg1"]), ng,
+                                   tan=None if T is None else (T["v"][K], T.pop("vg1")))
     del dagg3
     # snapshots are released as soon as the backward pass is past their stage
     snaps["vg2"] = snaps["agg3"] = snaps["vg1"] = None
@@ -515,7 +589,8 @@ class Backward:
       v_k = img(snaps["v"][k])
       agg_k = img(snaps["agg"][k])
       nfo, efo = self.proc_n[k], self.proc_e[k]
-      dh_n = self.mlp_backward(nfo, nm, [v_k, agg_k], dv)
+      dh_n = self.mlp_backward(nfo, nm, [v_k, agg_k], dv,
+                               tan=tan(*(() if T is None else (T["v"][k], T["agg"][k]))))
       dagg = self.empty(rk(nm))
       self.layer(rk(nm), [tab(dh_n)], nfo.t["w0_1"], self.zero_bias, out_y=dagg)
       dm = self.gather_add(dagg, rcv_k, rk(m.e_mesh), de_next)
@@ -527,7 +602,8 @@ class Backward:
         e_k = img(snaps["e"][k])
       dH, S, R = self.edge_backward(
           efo, m.e_mesh, e_k, dm, "mesh", v_k, nm, eng.mesh_snd, v_k, nm, eng.mesh_rcv,
-          lambda d: self.seg_sum_receiver(d, m.e_mesh, eng.mesh_row_ptr, nm))
+          lambda d: self.seg_sum_receiver(d, m.e_mesh, eng.mesh_row_ptr, nm),
+          tan=None if T is None else ([] if k == 0 else [tab(T["e"][k])], T["v"][k], T["v"][k]))
       del dm
       if k == 0 and not self.param_grads:    # de_0 feeds the mesh edge embedder's parameters only
         de = None
@@ -549,6 +625,8 @@ class Backward:
       dv = dv_new
       del dh_n, S, R, dv2
       snaps["v"][k + 1] = snaps["agg"][k] = snaps["e"][k] = None
+      if T is not None:
+        T["v"][k + 1] = T["agg"][k] = T["e"][k] = None
     # mesh edge embedder: e0 = MLP(edge features)
     if self.param_grads:
       self.mlp_backward(mp["enc_e_mesh"], m.e_mesh, [feat(eng.mesh_feat)], de_next)
@@ -561,12 +639,14 @@ class Backward:
     vg0 = self.fwd_mlp(mp["enc_grid"], ng, [grid_in])
     vm0 = self.fwd_mlp(mp["enc_mesh"], nm, [mesh_in])
     info = mp["proc_n_grid_g2m"]
-    dh = self.mlp_backward(info, ng, [tab(vg0)], dvg1)
+    dh = self.mlp_backward(info, ng, [tab(vg0)], dvg1,
+                           tan=tan(*(() if T is None else (T["vg0"],))))
     dvg0 = self.empty(rk(ng))
     self.layer(rk(ng), [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dvg1, out=dvg0)
     del dh, dvg1
     info = mp["proc_n_mesh_g2m"]
-    dh = self.mlp_backward(info, nm, [tab(vm0), img(snaps["agg1"])], dv)
+    dh = self.mlp_backward(info, nm, [tab(vm0), img(snaps["agg1"])], dv,   # vm0 has no tangent
+                           tan=None if T is None else tan(T.pop("agg1"), dw0=self.w0_block(info, 1)))
     dvm0 = self.empty(rk(nm))
     self.layer(rk(nm), [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dv, out=dvm0)
     dagg1 = self.empty(rk(nm))
@@ -574,7 +654,8 @@ class Backward:
     del dh, dv
     info = mp["proc_e_g2m"]
     S, R = self.bipartite_backward("g2m", info, mp["enc_e_g2m"], eng.g2m_feat, dagg1, eng.g2m_snd,
-                                   eng.g2m_rcv, tab(vg0), ng, tab(vm0), nm)
+                                   eng.g2m_rcv, tab(vg0), ng, tab(vm0), nm,
+                                   tan=None if T is None else (T.pop("vg0"), None))
     del dagg1
     t = self.empty(rk(ng))
     self.layer(rk(ng), [tab(S)], info.t["w0_1"], self.zero_bias, residual=dvg0, out=t)
@@ -583,7 +664,8 @@ class Backward:
     self.layer(rk(nm), [tab(R)], info.t["w0_2"], self.zero_bias, residual=dvm0, out=t)
     dvm0 = t
     del S, R, vg0, vm0
-    dh = self.mlp_backward(mp["enc_grid"], ng, [grid_in], dvg0)
+    dh = self.mlp_backward(mp["enc_grid"], ng, [grid_in], dvg0,
+                           tan=None if T is None else ([img(T.pop("grid_in"), eng.c_in_pad)], (), None))
     dx = None
     if dgrid_in:
       w0t, n = self.input_transposed()
@@ -736,7 +818,8 @@ class Backward:
       del dm
     return dagg
 
-  def tangent(self, grid_in_img: torch.Tensor, dgrid_in_img: torch.Tensor, dirs: int = 1) -> torch.Tensor:
+  def tangent(self, grid_in_img: torch.Tensor, dgrid_in_img: torch.Tensor, dirs: int = 1,
+              snaps: Optional[dict] = None, tsnaps: Optional[dict] = None) -> torch.Tensor:
     """One step stage by stage (Engine.run_stage, from the packed inputs grid_in_img) and, interleaved
     with it, its tangent along `dirs` directions at once: dgrid_in_img is the stacked operand image of
     the packed input tangents ([Ng, c_in_pad] per direction, dir_stride(Ng) rows apart, structural
@@ -745,14 +828,20 @@ class Backward:
     and copies of that stage's inputs alone; the tangent state is stacked fp32 tables, and every MLP's
     h and z are recomputed once for all directions.  Exactly zero tangents are not formed: the
     mesh-node encoder, the three edge embedders, e_0 of the processor, and the v_m0 and edge terms of
-    the grid2mesh edge MLP."""
+    the grid2mesh edge MLP.
+
+    With `snaps` and `tsnaps` (dicts, one direction; Hessian-vector products) they receive what
+    element(hvp=tsnaps) reads: snaps the primal copies of Engine._forward_snapshots, tsnaps the tangent
+    tables v-dot_k (k = 0..K), e-dot_k (k = 1..K-1), agg-dot_k, and the v-dot / agg-dot of the grid
+    and mesh nodes around the encoder and decoder (vg0, agg1, vg1, agg3, vg2), and the packed input
+    tangent image (grid_in).  Without them nothing more is kept or launched."""
     self.dirs = int(dirs)
     try:
-      return self._tangent(grid_in_img, dgrid_in_img)
+      return self._tangent(grid_in_img, dgrid_in_img, snaps, tsnaps)
     finally:
       self.dirs = 1
 
-  def _tangent(self, grid_in_img, dgrid_in_img):
+  def _tangent(self, grid_in_img, dgrid_in_img, snaps=None, ts=None):
     eng, m = self.eng, self.m
     ng, nm = m.num_grid, m.num_mesh
     K = eng.msg_steps
@@ -763,6 +852,11 @@ class Backward:
     # ---- encoder: vg0 = MLP(grid_in);  m1 = MLP([e1 | vg0[snd] | vm0[rcv]]);  agg1 = sum m1;
     #      vm1 = vm0 + MLP([vm0 | agg1]);  vg1 = vg0 + MLP([vg0]).  agg1 is read from the engine.
     eng.run_stage("encode", grid_in=grid_in_img)
+    keep = ts is not None
+    if keep:
+      snaps.update(v=[], agg=[], e=[None], vg1=eng.grid_lat_img.clone(), agg1=eng.mesh_agg_img.clone())
+      snaps["v"].append(eng.mesh_lat_img.clone())
+      ts.update(v=[], agg=[], e=[None], grid_in=dgrid_in_img)
     grid_in = img(grid_in_img, cin)
     info = mp["enc_grid"]
     dvg0 = self.mlp_jvp(info, ng, [grid_in], [img(dgrid_in_img, cin)])
@@ -773,8 +867,13 @@ class Backward:
     info = mp["proc_n_mesh_g2m"]                 # vm0 has no tangent: block 1 of W0 alone
     dv = self.mlp_jvp(info, nm, [tab(vm0), img(eng.mesh_agg_img)], [tab(dagg)],
                       dw0=self.w0_block(info, 1))
+    if keep:
+      ts.update(vg0=dvg0, agg1=dagg)
+      ts["v"].append(dv)
     del dagg, vm0
     dvg = self.mlp_jvp(mp["proc_n_grid_g2m"], ng, [tab(vg0)], [tab(dvg0)], residual=dvg0)
+    if keep:
+      ts["vg1"] = dvg
     del dvg0, vg0
 
     # ---- processor:  m = MLP([e | v[snd] | v[rcv]]);  v' = v + MLP([v | agg]);  e' = e + m.
@@ -790,6 +889,13 @@ class Backward:
       else:
         e_k = img(eng.mesh_edge_img.clone())
       eng.run_stage("process_step", k)
+      if keep:
+        snaps["v"].append(eng.mesh_lat_img.clone())
+        snaps["agg"].append(eng.mesh_agg_img.clone())
+        if k < K - 1:
+          snaps["e"].append(eng.mesh_edge_img.clone())
+        if k > 0:
+          ts["e"].append(de)
       nfo, efo = self.proc_n[k], self.proc_e[k]
       sp = efo.split
       ps, pr = self.projection(nm, img(v_k), sp.ws_packed), self.projection(nm, img(v_k), sp.wr_packed)
@@ -804,8 +910,12 @@ class Backward:
       if k < K - 1:                              # the last step's edge update is never read
         de = dm if de is None else self.gather_add(dm, self.edge_iota(), self.dir_rows(m.e_mesh), de)
       del dm
+      if keep:
+        ts["agg"].append(dagg)
       dv = self.mlp_jvp(nfo, nm, [img(v_k), img(eng.mesh_agg_img)], [tab(dv), tab(dagg)],
                         residual=dv)
+      if keep:
+        ts["v"].append(dv)
       del dagg, v_k
     del de
 
@@ -813,11 +923,15 @@ class Backward:
     #      vg2 = vg1 + MLP([vg1 | agg3]);  out = MLP(vg2).  agg3 and vg2 are read from the engine.
     v_k, vg1 = eng.mesh_lat_img.clone(), eng.grid_lat_img.clone()
     eng.run_stage("decode", grid_in=grid_in_img)
+    if keep:
+      snaps.update(vg2=eng.grid_lat_img.clone(), agg3=eng.grid_agg_img.clone())
     dagg = self.bipartite_jvp("m2g", mp["proc_e_m2g"], mp["enc_e_m2g"], eng.m2g_feat, eng.m2g_snd,
                               eng.m2g_rcv, img(v_k), nm, img(vg1), ng, dv, dvg)
     del v_k, dv
     dvg = self.mlp_jvp(mp["proc_n_grid_m2g"], ng, [img(vg1), img(eng.grid_agg_img)],
                        [tab(dvg), tab(dagg)], residual=dvg)
+    if keep:
+      ts.update(agg3=dagg, vg2=dvg)
     del vg1, dagg
     return self.mlp_jvp(mp["dec_grid"], ng, [img(eng.grid_lat_img)], [tab(dvg)])
 

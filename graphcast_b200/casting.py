@@ -69,6 +69,11 @@ class Bfloat16Cast(graphcast.Predictor):
   def loss_and_input_grads(self, inputs, targets, forcings, **kwargs):
     return self._predictor.loss_and_input_grads(inputs, targets, forcings, **kwargs)
 
+  def loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
+                         **kwargs):
+    return self._predictor.loss_and_input_hvp(inputs, targets, forcings, input_tangents,
+                                              forcing_tangents, **kwargs)
+
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
     return self._predictor.input_vjp(inputs, targets_template, forcings, cotangents, **kwargs)
 

@@ -505,6 +505,141 @@ layernorm_backward_dirs_kernel(const float* __restrict__ dy, int ld_dy, const fl
   }
 }
 
+// ---- Hessian-vector products (loss_and_input_hvp) ---------------------------------------------------
+// The backward pass of the gradient (direction 0) coupled with its tangent (direction 1), stacked as
+// above with two directions, at the primal h / z and their tangents hdot / zdot (one table each).
+// Direction 0 is bit for bit what swish_jvp_kernel / layernorm_backward_dirs_kernel give it alone;
+// direction 1 is its derivative along the tangent, in fp32.
+
+// dh = s'(h) da, dhdot = s'(h) dadot + s''(h) hdot da, with s'(h) = sg (1 + h (1 - sg)) rounded as
+// swish_jvp_kernel compiles it and s''(h) = sg (1 - sg) (2 + h (1 - 2 sg)).  One thread per 4 columns of
+// a row; dh may alias da (each thread reads both directions of da before it writes dh).
+__global__ void __launch_bounds__(256)
+swish_backward_jvp_kernel(const float* __restrict__ h, int ld_h, const float* __restrict__ hdot,
+                          int ld_hdot, long long rows, int n4, const float* da, int ld_da,
+                          long long stride, float* dh, int ld_dh) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= rows * n4) return;
+  const long long r = i / n4;
+  const int c = static_cast<int>(i - r * n4) * 4;
+  const float4 hv = *reinterpret_cast<const float4*>(h + r * ld_h + c);
+  const float4 tv = *reinterpret_cast<const float4*>(hdot + r * ld_hdot + c);
+  const float4 a0 = *reinterpret_cast<const float4*>(da + r * ld_da + c);
+  const float4 a1 = *reinterpret_cast<const float4*>(da + (stride + r) * ld_da + c);
+  const float hq[4] = {hv.x, hv.y, hv.z, hv.w}, tq[4] = {tv.x, tv.y, tv.z, tv.w};
+  const float d0[4] = {a0.x, a0.y, a0.z, a0.w}, d1[4] = {a1.x, a1.y, a1.z, a1.w};
+  float o0[4], o1[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float sg = 1.0f / (1.0f + expf(-hq[q]));
+    const float om = __fsub_rn(1.0f, sg);
+    const float f = __fmul_rn(sg, __fmaf_rn(hq[q], om, 1.0f));
+    const float f2 = sg * om * (2.0f + hq[q] * (1.0f - 2.0f * sg));
+    o0[q] = __fmul_rn(d0[q], f);
+    o1[q] = d1[q] * f + f2 * tq[q] * d0[q];
+  }
+  *reinterpret_cast<float4*>(dh + r * ld_dh + c) = make_float4(o0[0], o0[1], o0[2], o0[3]);
+  *reinterpret_cast<float4*>(dh + (stride + r) * ld_dh + c) = make_float4(o1[0], o1[1], o1[2], o1[3]);
+}
+
+// The LayerNorm backward of layernorm_backward_dirs_kernel for [dy; dydot] (direction 0: its dz, with
+// its pinned roundings) and the tangent of that dz along zdot (direction 1).  With r = rstd, zhat =
+// (z - mu) r, g = dy*scale, m = mean(g*zhat):
+//   rdot    = -r^2 mean(zhat*zdot)
+//   zhatdot = r (zdot - mean(zdot) - zhat mean(zhat*zdot))
+//   gdot    = dydot*scale,  mdot = mean(gdot*zhat + g*zhatdot)
+//   dzdot   = rdot (g - mean(g) - zhat m) + r (gdot - mean(gdot) - zhatdot m - zhat mdot)
+// One warp per row of n = 512 (lane owns columns lane + 32 j), 8 rows per block; z's row is read once.
+__global__ void __launch_bounds__(256)
+layernorm_backward_jvp_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z,
+                              int ld_z, const float* __restrict__ zdot, int ld_zdot,
+                              const float* __restrict__ scale, long long rows, long long stride,
+                              float* __restrict__ dz, int ld_dz) {
+  constexpr int kCols = 16;
+  constexpr float kInvN = 1.0f / (kCols * 32);
+  const int lane = threadIdx.x & 31;
+  const long long r = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  if (r >= rows) return;
+  float v[kCols], sc[kCols];
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) {
+    v[j] = z[r * ld_z + lane + 32 * j];
+    sc[j] = scale[lane + 32 * j];
+  }
+  // the primal statistics and direction 0: layernorm_backward_dirs_kernel's arithmetic
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) s = __fadd_rn(s, v[j]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, o));
+  float var = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) {
+    v[j] = __fmaf_rn(s, -kInvN, v[j]);                 // z - mean
+    var = __fmaf_rn(v[j], v[j], var);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) var = __fadd_rn(var, __shfl_xor_sync(0xffffffffu, var, o));
+  const float rstd = rsqrtf(__fmaf_rn(var, kInvN, 1e-5f));
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) v[j] = __fmul_rn(v[j], rstd);     // z-hat
+  float g[kCols];
+  float mg = 0.f, mgz = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) {
+    g[j] = __fmul_rn(dy[r * ld_dy + lane + 32 * j], sc[j]);
+    mg = __fadd_rn(mg, g[j]);
+    mgz = __fmaf_rn(v[j], g[j], mgz);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mg = __fadd_rn(mg, __shfl_xor_sync(0xffffffffu, mg, o));
+    mgz = __fadd_rn(mgz, __shfl_xor_sync(0xffffffffu, mgz, o));
+  }
+  const float mgz_n = __fmul_rn(mgz, kInvN);
+#pragma unroll
+  for (int j = 0; j < kCols; ++j)
+    dz[r * ld_dz + lane + 32 * j] = __fmul_rn(rstd, __fmaf_rn(v[j], -mgz_n, __fmaf_rn(mg, -kInvN, g[j])));
+  // direction 1: the tangent
+  float zd[kCols];
+  float mzd = 0.f, mvz = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) {
+    zd[j] = zdot[r * ld_zdot + lane + 32 * j];
+    mzd += zd[j];
+    mvz += v[j] * zd[j];
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mzd += __shfl_xor_sync(0xffffffffu, mzd, o);
+    mvz += __shfl_xor_sync(0xffffffffu, mvz, o);
+  }
+  mzd *= kInvN;
+  mvz *= kInvN;
+  const float rdot = -rstd * rstd * mvz;
+  float gd[kCols];
+  float mgd = 0.f, mdot = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) {
+    zd[j] = rstd * (zd[j] - mzd - v[j] * mvz);         // zhat-dot
+    gd[j] = dy[(stride + r) * ld_dy + lane + 32 * j] * sc[j];
+    mgd += gd[j];
+    mdot += gd[j] * v[j] + g[j] * zd[j];
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mgd += __shfl_xor_sync(0xffffffffu, mgd, o);
+    mdot += __shfl_xor_sync(0xffffffffu, mdot, o);
+  }
+  mgd *= kInvN;
+  mdot *= kInvN;
+  const float mg_n = mg * kInvN;
+#pragma unroll
+  for (int j = 0; j < kCols; ++j)
+    dz[(stride + r) * ld_dz + lane + 32 * j] =
+        rdot * (g[j] - mg_n - v[j] * mgz_n) + rstd * (gd[j] - mgd - zd[j] * mgz_n - v[j] * mdot);
+}
+
 // ---- index operations ----------------------------------------------------------------------------
 // out[i, 0:512] = sum_{j in [ptr[i], ptr[i+1])} msg[order[j], 0:512], summed in j order.  Rows listed
 // in `heavy` (ascending node ids): one 128-thread block each (thread owns one float4 column); every

@@ -119,6 +119,13 @@ class Predictor(abc.ABC):
     `forcings`; `cotangents` is shaped like `targets_template`."""
     raise NotImplementedError(f"{type(self).__name__} does not implement input gradients")
 
+  def loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
+                         **optional_kwargs):
+    """Returns (loss, diagnostics, input_grads, forcing_grads, input_hvp, forcing_hvp): those of
+    loss_and_input_grads, and the Hessian of loss.mean() with respect to the inputs and forcings times
+    the tangents (Datasets as input_jvp takes them), shaped like `inputs` and `forcings`."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement Hessian-vector products")
+
   def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
                 **optional_kwargs):
     """Returns (predictions, prediction_tangents): the predictions of __call__ and their derivative
@@ -337,6 +344,26 @@ class GraphCast(Predictor):
     .all_channels); the parameter gradients are neither computed nor touched."""
     return self._loss_and_input_grads(inputs, targets, forcings, norm=None)
 
+  def loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
+                         **unused_kwargs):
+    """(loss, diagnostics, input_grads, forcing_grads, input_hvp, forcing_hvp) for one target time:
+    what jax.jvp(jax.grad(loss), (x,), (v,)) gives, with the loss and gradient of loss_and_input_grads.
+
+    `loss`, `diagnostics`, `input_grads` and `forcing_grads` are bit for bit what loss_and_input_grads
+    returns.  `input_hvp` and `forcing_hvp` (float32, shaped like `inputs` and `forcings`, physical
+    units) are H v, H the Hessian of loss.mean() with respect to every variable of the inputs and
+    forcings and v = (input_tangents, forcing_tangents); the tangents are Datasets as input_jvp takes
+    them, a variable left out (every forcing for forcing_tangents=None) being zero.  Variables the
+    packing broadcast are summed as in loss_and_input_grads.  Every refusal of loss_and_input_grads and
+    of input_jvp's tangents applies, before anything runs.
+
+    The forward runs stage by stage with its tangent (Backward.tangent), keeping the tangent state the
+    backward walk reads; the gradient and its tangent then share one backward walk
+    (Backward.element(hvp=...)), forward-over-reverse: one forward, one tangent and one two-direction
+    backward pass in place of the two gradients of a central difference."""
+    return self._loss_and_input_grads(inputs, targets, forcings, norm=None,
+                                      tangents=(input_tangents, forcing_tangents))
+
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **unused_kwargs):
     """(predictions, input_grads, forcing_grads) for one target time: `predictions` is what __call__
     returns, bit for bit; the gradients (as in loss_and_input_grads) are those of
@@ -453,17 +480,22 @@ class GraphCast(Predictor):
     return predictions, self._planes_to_dataset(state["out"], targets_template, run.n_lat, run.n_lon,
                                                 directions=run.labels)
 
-  def _loss_and_input_grads(self, inputs, targets, forcings, norm: Optional[FusedNormalization]):
+  def _loss_and_input_grads(self, inputs, targets, forcings, norm: Optional[FusedNormalization],
+                            tangents=None):
+    """loss_and_input_grads of one target time; with tangents = (input_tangents, forcing_tangents),
+    loss_and_input_hvp."""
     inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
     forcings = xs.from_xarray(forcings)
     if targets.sizes.get("time", 1) != 1:
       raise NotImplementedError("input gradients of GraphCast cover one target time (several: "
                                 "autoregressive.Predictor with gradient_checkpointing=True)")
+    tangent = None if tangents is None else hvp_tangent_planes(inputs, forcings, *tangents)
     batch = dict(inputs.sizes).get("batch", 1)
     slabs = model_utils.channel_layout(targets)
     num_grid = inputs.sizes["lat"] * inputs.sizes["lon"]
     coef = 2.0 * losses.channel_kappa(slabs, num_grid, LOSS_PER_VARIABLE_WEIGHTS) / batch
-    run = self._one_step_input_grads(inputs, targets, forcings, norm, targets=targets, coef=coef)
+    run = self._one_step_input_grads(inputs, targets, forcings, norm, targets=targets, coef=coef,
+                                     tangent_planes=tangent)
     loss, diagnostics = losses.losses_from_channel_sums(
         self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
     return (loss, diagnostics) + run.finish()
@@ -486,15 +518,17 @@ class GraphCast(Predictor):
     return (holder["predictions"],) + run.finish()
 
   def _one_step_input_grads(self, inputs, template, forcings, norm, *, targets=None, coef=None,
-                            cotangents=None, predictions=None,
-                            directions: bool = False) -> "_InputGradRun":
+                            cotangents=None, predictions=None, directions: bool = False,
+                            tangent_planes: Optional[torch.Tensor] = None) -> "_InputGradRun":
     """One target time: `_call` stages the planes once and, for every batch element, runs the
     stage-wise forward, the seed and the backward pass of Engine.input_grads_element in place of its
     step (no second forward, no host round trip).  With `targets` the loss sums land in
     self._channel_sums as in `loss`; with `cotangents`, predictions["predictions"] receives the
     predictions, unpacked from that forward as __call__ unpacks its step's; with `directions`, the
     cotangents have a leading "direction" dim and every direction shares that forward and backward
-    pass.  Returns the run, whose finish() gives (input_grads, forcing_grads)."""
+    pass; with `tangent_planes` ([batch, c_in, Ng] host planes of the input tangents, with `targets`)
+    every element runs Engine.input_hvp_element.  Returns the run, whose finish() gives (input_grads,
+    forcing_grads), with tangent_planes followed by (input_hvp, forcing_hvp)."""
     state = {}
 
     def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
@@ -506,12 +540,15 @@ class GraphCast(Predictor):
           state["cot"] = self._direction_cotangent_planes(cotangents, template, state["batch"])
           dirs = state["cot"].shape[0]
         state["run"] = _InputGradRun(self, plan, norm, inputs, forcings, 1, state["batch"],
-                                     release_staging=False, dirs=dirs)
+                                     release_staging=False, dirs=dirs,
+                                     hvp=tangent_planes is not None)
         if cotangents is not None and not directions:
           state["cot"] = self._cotangent_planes(cotangents, template, state["run"].batch)
         if coef is not None:
           state["coef"] = torch.as_tensor(np.asarray(coef, np.float64)).to(eng.device)
       operands = dict(affine)
+      if tangent_planes is not None:
+        operands["tangent_planes"] = tangent_planes[b].to(eng.device)
       if targets is not None:
         operands["targets_planes"] = planes_tgt
         kw = dict(lat_weight=self._lat_weight(targets, eng.device), coef=state["coef"],
@@ -566,7 +603,7 @@ class GraphCast(Predictor):
 
   def _input_grads(self, stash: "StepStash", plan, norm: Optional[FusedNormalization],
                    inputs: xs.Dataset, forcings: xs.Dataset, *, lat_weight=None, coef=None,
-                   cotangents=None, directions: bool = False):
+                   cotangents=None, directions: bool = False, tangents: Optional["StepStash"] = None):
     """Gradients with respect to the inputs and forcings of the steps `stash` holds (several target
     times): for every batch element, last step first, the step's planes are uploaded again, packed
     and differentiated by Engine.input_grads_element with the all-channel feedback `plan` of the
@@ -575,10 +612,13 @@ class GraphCast(Predictor):
     with `directions`, per step [K, batch, n_out, Ng] planes of K cotangents that share every step's
     backward pass.  The stash is only read, so several calls can differentiate the same forward.
     Returns (input_grads, forcing_grads) Datasets shaped like `inputs` and `forcings` (with a leading
-    "direction" dim for `directions`)."""
+    "direction" dim for `directions`).  With `tangents` (a StepStash of each step's input tangent planes
+    [batch, c_in, Ng], loss seed only) every step runs Engine.input_hvp_element, and (input_hvp,
+    forcing_hvp) follow the gradients."""
     run = _InputGradRun(self, plan, norm, inputs, forcings, len(stash.steps), stash.batch,
                         release_staging=True,
-                        dirs=cotangents[0].shape[0] if directions else None)
+                        dirs=cotangents[0].shape[0] if directions else None,
+                        hvp=tangents is not None)
     eng = self._engine
     dev = eng.device
     coef_dev = None if coef is None else torch.as_tensor(np.asarray(coef, np.float64)).to(dev)
@@ -597,6 +637,12 @@ class GraphCast(Predictor):
           eng.pack_inputs(operands["planes"], mean=norm.in_mean, scale=norm.in_scale)
           operands.update(scale=norm.out_scale, offset=norm.out_offset,
                           add_planes=operands.pop("planes"), add_plane_index=norm.add_plane_index)
+        if tangents is not None:
+          (host_tangent,), tangent_done = tangents.steps[t]
+          compute.wait_event(tangent_done)
+          operands["tangent_planes"] = torch.empty([eng.c_in, eng.num_grid], dtype=torch.float32,
+                                                   device=dev)
+          operands["tangent_planes"].copy_(host_tangent[b], non_blocking=True)
         lead = [cotangents[t].shape[0]] if directions else []
         seed = torch.empty(lead + [eng.n_out, eng.num_grid], dtype=torch.float32, device=dev)
         if cotangents is None:
@@ -695,6 +741,39 @@ class GraphCast(Predictor):
     finish = lambda sums: losses.losses_from_channel_sums(sums, slabs, num_grid,
                                                           LOSS_PER_VARIABLE_WEIGHTS)
     return finish, preds, self._channel_sums
+
+  def _device_loss_tangent(self, inputs, targets, forcings, norm: Optional[FusedNormalization],
+                           run: "_TangentRun"):
+    """_device_loss with the tangent planes of `run` carried through the step (the forward of
+    loss_and_input_hvp over several target times): every batch element runs the stage-wise forward with
+    its tangent (_TangentRun.element, which also feeds the next step's tangent planes), then
+    output_loss on that forward, which is the step _device_loss runs.  Returns (finish, predictions,
+    channel_sums, this step's input tangent planes [batch, c_in, Ng] on the device)."""
+    targets = xs.from_xarray(targets)
+    state = {}
+
+    def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
+      eng = self._engine
+      if "planes" not in state:
+        eng.input_grads_begin()
+        state["planes"] = torch.empty([run.batch, eng.c_in, eng.num_grid], dtype=torch.float32,
+                                      device=eng.device)
+        state["lat_weight"] = self._lat_weight(targets, eng.device)
+      tangent_out = torch.empty([run.dirs, eng.n_out, eng.num_grid], dtype=torch.float32,
+                                device=eng.device)
+      run.element(eng, b, tangent_out, None, norm, affine,
+                  keep=lambda p: state["planes"][b].copy_(p[0]))
+      eng.output_loss(planes_tgt, state["lat_weight"], channel_sums=channel_sums,
+                      planes_out=planes_out, **affine)
+
+    preds = self._call(inputs, targets, forcings, norm=norm, targets=targets, predictions=True,
+                       element=element)
+    run.step += 1
+    slabs = model_utils.channel_layout(targets)
+    num_grid = self._engine.num_grid
+    finish = lambda sums: losses.losses_from_channel_sums(sums, slabs, num_grid,
+                                                          LOSS_PER_VARIABLE_WEIGHTS)
+    return finish, preds, self._channel_sums, state["planes"]
 
   def _lat_weight(self, targets: xs.Dataset, device) -> torch.Tensor:
     """Normalised latitude weights of the targets' grid (float32, on the device), cached."""
@@ -891,6 +970,21 @@ class GraphCast(Predictor):
     return out
 
 
+def hvp_tangent_planes(inputs: xs.Dataset, forcings: xs.Dataset, input_tangents,
+                       forcing_tangents) -> torch.Tensor:
+  """[batch, c_in, Ng] float32 host planes of the tangent of a Hessian-vector product, inputs then
+  forcings, packed as GraphCast stages the planes (feedback.tangent_planes), after input_jvp's checks."""
+  input_tangents = None if input_tangents is None else xs.from_xarray(input_tangents)
+  forcing_tangents = None if forcing_tangents is None else xs.from_xarray(forcing_tangents)
+  feedback.check_tangents(input_tangents, inputs, "input_tangents")
+  feedback.check_tangents(forcing_tangents, forcings, "forcing_tangents")
+  sizes = {"batch": dict(inputs.sizes).get("batch", 1), "lat": inputs.sizes["lat"],
+           "lon": inputs.sizes["lon"]}
+  return torch.from_numpy(np.concatenate(
+      [feedback.tangent_planes(input_tangents, inputs, sizes),
+       feedback.tangent_planes(forcing_tangents, forcings, sizes)], axis=1))
+
+
 def batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents, directions_per_pass):
   """batched_input_jvp of a predictor stack: checks the tangents (feedback.check_direction_tangents)
   and directions_per_pass before anything runs, then runs one_pass(input_tangents, forcing_tangents)
@@ -1023,12 +1117,18 @@ class _InputGradRun:
   and cross PCIe at full speed; finish() synchronises once.  The returned arrays are views of it.
 
   dirs = K (batched_input_vjp): K cotangents share every step, fb.a is [K, n_rows, Ng], and every
-  result buffer has a leading axis of K directions, each reduced as one direction's would be."""
+  result buffer has a leading axis of K directions, each reduced as one direction's would be.
+
+  hvp (loss_and_input_hvp): every step runs Engine.input_hvp_element, the two directions are the
+  gradient and its derivative along the tangent, and finish() gives (input_grads, forcing_grads,
+  input_hvp, forcing_hvp)."""
 
   def __init__(self, model: GraphCast, plan, norm: Optional[FusedNormalization], inputs: xs.Dataset,
                forcings: xs.Dataset, num_steps: int, batch: int, release_staging: bool,
-               dirs: Optional[int] = None):
+               dirs: Optional[int] = None, hvp: bool = False):
     eng = self.eng = model.engine
+    self.hvp, self.zero_targets = hvp, None
+    dirs = 2 if hvp else dirs
     self.dirs = dirs
     lead = [] if dirs is None else [dirs]
     eng.input_grads_begin()
@@ -1061,7 +1161,13 @@ class _InputGradRun:
     reductions of the rows that are complete."""
     if t == self.num_steps - 1:
       self.fb.a = None
-    self.eng.input_grads_element(self.fb, operands, **kw)
+    if self.hvp:
+      if self.zero_targets is None:
+        self.zero_targets = torch.zeros([self.eng.n_out, self.eng.num_grid], dtype=torch.float32,
+                                        device=self.eng.device)
+      self.eng.input_hvp_element(self.fb, operands, zero_targets=self.zero_targets, **kw)
+    else:
+      self.eng.input_grads_element(self.fb, operands, **kw)
     for v in self.var_rows:
       if v.forcing or t == 0:
         self._reduce(v, b, t)
@@ -1096,6 +1202,10 @@ class _InputGradRun:
     grads = {key: buf.cpu().numpy() for key, buf in self.dev_bufs.items()}   # synchronises
     torch.cuda.current_stream(self.eng.device).synchronize()
     grads.update({key: t.numpy() for key, t in self.host.items()})
+    if self.hvp:
+      return tuple(ds for k in range(2) for ds in feedback.grads_to_datasets(
+          self.var_rows, {key: g[k] for key, g in grads.items()}, self.inputs, self.forcings,
+          self.n_lat, self.n_lon))
     return feedback.grads_to_datasets(self.var_rows, grads, self.inputs, self.forcings, self.n_lat,
                                       self.n_lon, directions=self.dirs)
 
@@ -1152,15 +1262,18 @@ class _TangentRun:
     return self._slab[1]
 
   def element(self, eng, b: int, tangent_out: torch.Tensor, planes_out: Optional[torch.Tensor],
-              norm: Optional[FusedNormalization], affine: dict) -> None:
+              norm: Optional[FusedNormalization], affine: dict, keep=None) -> None:
     """This step of batch element b (tangent_out [dirs, n_out, Ng]): Engine.input_jvp_element, then the
-    feed of the next step."""
+    feed of the next step.  keep(planes): called with this step's input tangent planes [dirs, c_in, Ng]
+    (a device view, valid until the next step's feed) before the step runs."""
     c_in, n_in, ng = eng.c_in, self.input_planes.shape[2], eng.num_grid
     buf, self.carry[b] = self.carry[b], None
     if buf is None:
       buf = torch.empty([self.dirs, c_in + eng.n_out, ng], dtype=torch.float32, device=eng.device)
       buf[:, :n_in].copy_(self.input_planes[:, b])
     buf[:, n_in:c_in].copy_(self._forcing_planes(self.step)[:, b])
+    if keep is not None:
+      keep(buf[:, :c_in])
     eng.input_jvp_element(buf[:, :c_in], tangent_out,
                           in_scale=None if norm is None else norm.in_scale, planes_out=planes_out,
                           **affine)

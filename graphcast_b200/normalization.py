@@ -263,6 +263,14 @@ class InputsAndResiduals(graphcast.Predictor):
     inputs, targets, forcings, consts = self._fused_for(inputs, targets, forcings, "input gradients")
     return self._predictor._loss_and_input_grads(inputs, targets, forcings, norm=consts)
 
+  def loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
+                         **kwargs):
+    """loss_and_input_grads and the Hessian-vector product of its loss (GraphCast.loss_and_input_hvp),
+    with respect to the inputs and forcings in their physical units.  GraphCast only."""
+    inputs, targets, forcings, consts = self._fused_for(inputs, targets, forcings, "input gradients")
+    return self._predictor._loss_and_input_grads(inputs, targets, forcings, norm=consts,
+                                                 tangents=(input_tangents, forcing_tangents))
+
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
     """(predictions, input_grads, forcing_grads) of the un-normalised predictions of __call__
     (GraphCast.input_vjp).  GraphCast only."""

@@ -450,6 +450,25 @@ int gcb_layernorm_backward_dirs(const float* dy, int32_t ld_dy, const float* z, 
                                 const float* scale, int64_t rows, int32_t n, int64_t dir_stride,
                                 int32_t dirs, float* dz, int32_t ld_dz, void* stream);
 
+/* Hessian-vector products (GraphCast.loss_and_input_hvp): the backward pass of the gradient coupled
+ * with its tangent, stacked as above with two directions, [d; ddot] (row r of direction 1 is row
+ * dir_stride + r, dir_stride >= rows), at the primal rows and their tangent (one table each).
+ * Direction 0 is bit for bit what the one-direction kernel gives; direction 1 is its derivative along
+ * the primal tangent, in fp32.  Row-wise, deterministic.
+ *
+ * gcb_swish_backward_jvp: dh = swish'(h) da (bit for bit gcb_swish_jvp) and
+ *   dhdot = swish'(h) dadot + swish''(h) hdot da,  swish''(h) = sg (1 - sg) (2 + h (1 - 2 sg)).
+ *   n a multiple of 4, 16-byte rows; dh may alias da.
+ * gcb_layernorm_backward_jvp: dz = gcb_layernorm_backward_dirs(dy) (bit for bit) and its tangent along
+ *   zdot, the tangent of the pre-LayerNorm z (formulas in backward_kernels.cuh).  n = 512; dz may not
+ *   alias dy, z or zdot; z's row is read once. */
+int gcb_swish_backward_jvp(const float* h, int32_t ld_h, const float* hdot, int32_t ld_hdot,
+                           int64_t rows, int32_t n, const float* da, int32_t ld_da, int64_t dir_stride,
+                           float* dh, int32_t ld_dh, void* stream);
+int gcb_layernorm_backward_jvp(const float* dy, int32_t ld_dy, const float* z, int32_t ld_z,
+                               const float* zdot, int32_t ld_zdot, const float* scale, int64_t rows,
+                               int32_t n, int64_t dir_stride, float* dz, int32_t ld_dz, void* stream);
+
 /* Backward of a gather v[senders] (jax_gather, utils/typed_graph_net.py:124-125,431-445):
  *   out[i, 0:512] = sum_{j in [ptr[i], ptr[i+1])} msg[order[j], 0:512]
  * (order / ptr: the sender CSR of an edge set, host-built), summed in j order; the rows listed in
@@ -695,7 +714,8 @@ typedef enum {
                              * gcb_output_loss_grad_feedback, gcb_input_grad,
                              * gcb_output_cotangent_grad_feedback, gcb_broadcast_grad_sum,
                              * gcb_layernorm_jvp, gcb_swish_jvp, gcb_layernorm_jvp_dirs,
-                             * gcb_layernorm_backward_dirs */
+                             * gcb_layernorm_backward_dirs, gcb_swish_backward_jvp,
+                             * gcb_layernorm_backward_jvp */
   GCB_KIND_NOISE = 11       /* gcb_add_gaussian_noise */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
