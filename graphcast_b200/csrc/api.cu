@@ -325,6 +325,15 @@ int validate_chain(const gcb_chain_desc* d, ChainShape* shape) {
     sh.vecs += (g.bias ? 1 : 0) + (g.ln_scale ? 2 : 0);
     if (g.keep) ++sh.nq;
   }
+  // A kept layer's scratch slot is handed back for its next tile by the units that read it through
+  // seg_from (mlp_chain.cuh, h_free); without one, the first reuse of a slot would wait forever.
+  for (int l = 0; l < d->nlayers; ++l) {
+    if (!d->layer[l].keep) continue;
+    bool read = false;
+    for (int j = l + 1; j < d->nlayers; ++j)
+      for (int s = 0; s < d->layer[j].nseg; ++s) read = read || d->layer[j].seg_from[s] == l;
+    GCB_CHECK_ARG(read, "a kept layer must be read through seg_from by a later layer");
+  }
   GCB_CHECK_ARG(sh.vecs <= gcb::kChainParamVecs, "too many bias / LayerNorm vectors for one chain (at most 8)");
   const int lag = d->lag > 0 ? d->lag : 1;
   GCB_CHECK_ARG(d->order == 0 || (d->order == 1 && d->nlayers >= 3),

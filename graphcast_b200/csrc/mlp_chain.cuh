@@ -245,9 +245,9 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
   uint64_t* lnx_bar = empty_bar + 12;                              // [2 warpgroups][2]
   uint64_t* h_full_bar = lnx_bar + 4;                              // [GCB_MAX_CHAIN][kChainSlotsMax]
   uint64_t* h_free_bar = h_full_bar + GCB_MAX_CHAIN * kChainSlotsMax;
-  ChainLayer* s_layer = reinterpret_cast<ChainLayer*>(h_free_bar + GCB_MAX_CHAIN * kChainSlotsMax);  // [4]
-  SegInfo* s_seg = reinterpret_cast<SegInfo*>(s_layer + GCB_MAX_CHAIN);              // [4][3]
-  PreAddInfo* s_pre = reinterpret_cast<PreAddInfo*>(s_seg + GCB_MAX_CHAIN * 3);      // [4][2]
+  ChainLayer* s_layer = reinterpret_cast<ChainLayer*>(h_free_bar + GCB_MAX_CHAIN * kChainSlotsMax);  // [GCB_MAX_CHAIN]
+  SegInfo* s_seg = reinterpret_cast<SegInfo*>(s_layer + GCB_MAX_CHAIN);              // [GCB_MAX_CHAIN][3]
+  PreAddInfo* s_pre = reinterpret_cast<PreAddInfo*>(s_seg + GCB_MAX_CHAIN * 3);      // [GCB_MAX_CHAIN][2]
   static_assert((2 * 12 + 4 + 2 * GCB_MAX_CHAIN * kChainSlotsMax) * 8 +
                     GCB_MAX_CHAIN * (sizeof(ChainLayer) + 3 * sizeof(SegInfo) + 2 * sizeof(PreAddInfo))
                     <= kChainTailBytes, "tail region too small");

@@ -514,7 +514,10 @@ typedef struct {
   const void* w_packed; const float* bias;      /* bias may be NULL (= 0) */
   const float* ln_scale; const float* ln_offset;
   int32_t act;              /* gcb_activation; SWISH and LayerNorm are mutually exclusive here */
-  int32_t keep;             /* 1: later layers of the chain consume this layer's result */
+  int32_t keep;             /* 1: later layers of the chain consume this layer's result; at least
+                             * one of them must name it in seg_from (a scratch slot is reused only
+                             * after its seg_from readers are done with it), so a layer read only
+                             * through residual_keep, or not at all, is refused */
   const float* residual; int32_t ld_res;
   /* Alternative: the residual given as an operand image (x = hi + lo, two bf16: 2^-17 relative)
    * of the [rows, 512] stream -- typically the SAME buffer as out_img (updated in place) and as a
@@ -522,7 +525,8 @@ typedef struct {
    * fp32 master plus an image.  Excludes `residual` and `out`; LayerNorm layers only. */
   const void* residual_img;
   /* Or the kept result of an earlier layer of this chain: 0 = none, j + 1 = layer j (keep = 1).
-   * Excludes residual / residual_img / out.  (vg1 = vg0 + MLP(vg0) with vg0 never leaving the chip.) */
+   * Excludes residual / residual_img / out.  Layer j must also be a seg_from segment of some later
+   * layer (see keep).  (vg1 = vg0 + MLP(vg0) with vg0 never leaving the chip.) */
   int32_t residual_keep;
   float* out;   int32_t ld_out;      /* residual + y, fp32 (optional) */
   float* out_y; int32_t ld_out_y;    /* y alone, fp32 (optional) */

@@ -2,8 +2,11 @@
 layers one by one through gcb_layer_forward (same tiles, same products, same order of operations;
 only the hand-over of intermediate results changes: L2-resident scratch instead of HBM images),
 and within the usual tolerance of a torch fp64 reference.  Row counts give every cluster several
-tiles so that the scratch slots are reused and the pipeline fills and drains."""
+tiles so that the scratch slots are reused and the pipeline fills and drains.  The matrix at the end
+runs chains of 1 to 6 layers of every layer kind at every valid lag and order, from one row to many
+tiles per cluster; the refusals of gcb_chain_forward that need no GPU are in test_native_abi.py."""
 import ctypes as C
+import zlib
 
 import numpy as np
 import pytest
@@ -12,6 +15,7 @@ import torch
 import _cases
 from graphcast_b200 import _native, engine
 from oracle import gnn as oracle_gnn
+from test_gpu_layer import TOL, _image_values, _pack
 
 pytestmark = pytest.mark.gpu
 
@@ -455,3 +459,389 @@ def test_image_residual_step_stagewise_and_deep_chains(deep):
   torch.cuda.synchronize()
   assert n == eng.launches_per_step
   np.testing.assert_array_equal(eng.grid_out[:, :23].cpu().numpy(), y[:, 0])
+
+
+# ---- every chain shape against the layer kernel and float64 ---------------------------------------
+LD = 516     # row stride of the fp32 outputs and residuals: 4 padding columns that must stay untouched
+
+
+def _image_words(img, rows):
+  """(hi, lo) bf16 words of the operand image of a [rows, 512] matrix, as int16 [rows, 512] each."""
+  w = img.view(torch.int16).view(-1, 32, 2, 2, 1056)[..., :1024]          # tile, K-step, hi|lo, chunk
+  return [w[:, :, p].reshape(-1, 32, 2, 128, 8).permute(0, 3, 1, 2, 4).reshape(-1, 512)[:rows]
+          for p in (0, 1)]
+
+
+class _Chain:
+  """One chain on seeded device data; the same layers run one by one through gcb_layer_forward (at
+  cluster size 2, each kept result an operand image in HBM); and a float64 reference of every layer,
+  formed from the inputs that layer read.
+
+  A spec has `layers` (below) and `order`, the unit order of its default launch.  Per layer:
+    segs   ("img", k[, name]): the operand image of a random [rows, k] matrix; a named one is a
+           latent stream that residuals and outputs of the same name update in place
+           ("tab", table_rows, k_valid, k_pad, use_idx, fan): an fp32 table (table_rows None: rows)
+           ("keep", j): the kept result of layer j
+    kind   "plain", "swish" or "ln";  bias (default True; False: bias = NULL);  keep
+    out, out_y  fp32 outputs;  out_img: True, or the name of an image segment to update in place
+    res    "fp32", "inplace" (out == residual), ("img", name) or ("keep", j)
+    pre    gathered pre-activation addends, (table_rows, use_idx) each (table_rows None: rows)"""
+
+  def __init__(self, spec, rows, seed):
+    lib = self.lib = _native.lib()
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    randn = lambda *shape: torch.randn(*shape, generator=g, device=DEV)
+    index = lambda n: torch.randint(0, n, (rows,), generator=g, device=DEV, dtype=torch.int32)
+    self.rows, self.layers, self.order = rows, spec["layers"], spec["order"]
+    self.images = {}                 # name -> pristine image of an in-place latent stream
+    self.params = []
+    for s in self.layers:
+      p = {"segs": [], "vals": [], "alive": []}
+      widths = []
+      for sg in s["segs"]:
+        if sg[0] == "keep":
+          p["segs"].append(sg[1])
+          p["vals"].append(sg[1])
+          widths.append((512, 512))
+          continue
+        seg = _native.Segment()
+        if sg[0] == "img":
+          k, name = sg[1], (sg[2] if len(sg) > 2 else None)
+          img = self.images.get(name)
+          if img is None:
+            x = randn(rows, k)
+            img = torch.zeros(lib.gcb_a_image_bytes(rows, k), dtype=torch.uint8, device=DEV)
+            _native.check(lib.gcb_rows_to_image(x.data_ptr(), k, 1, rows, k, img.data_ptr(), _stream()),
+                          "rows_to_image")
+            if name is not None:
+              self.images[name] = img
+          seg.img, seg.k, seg.k_valid, seg.fan = img.data_ptr(), k, k, 1
+          p["segs"].append((seg, name, img))
+          p["vals"].append(_image_values(img, rows, k).double())
+          widths.append((k, k))
+          continue
+        _, trows, kv, kp, use_idx, fan = sg
+        trows = rows if trows is None else trows
+        table = randn(trows * fan, kv + 4)
+        seg.table, seg.ld, seg.k, seg.k_valid, seg.fan = table.data_ptr(), kv + 4, kp, kv, fan
+        src = torch.arange(rows, device=DEV)
+        if use_idx:
+          idx = index(trows)
+          seg.idx, src = idx.data_ptr(), idx.long()
+          p["alive"].append(idx)
+        p["segs"].append((seg, None, table))
+        p["vals"].append(table.view(trows, fan, kv + 4)[src][:, :, :kv].double().sum(1))
+        widths.append((kv, kp))
+      k_real, k_pad = sum(kv for kv, _ in widths), sum(kp for _, kp in widths)
+      p["w"] = randn(k_real, 512) / np.sqrt(k_real)
+      wp = torch.zeros(k_pad, 512, device=DEV)
+      src = dst = 0
+      for kv, kp in widths:
+        wp[dst:dst + kv] = p["w"][src:src + kv]
+        src, dst = src + kv, dst + kp
+      p["w_img"], _ = _pack(lib, wp.cpu().numpy(), k_pad, 512, DEV)
+      p["bias"] = 0.1 * randn(512) if s.get("bias", True) else None
+      p["zero_bias"] = torch.zeros(512, device=DEV)
+      p["scale"], p["offset"] = 1 + 0.1 * randn(512), 0.1 * randn(512)
+      p["adds"] = []
+      for trows, use_idx in s.get("pre", ()):
+        trows = rows if trows is None else trows
+        t = randn(trows, LD)
+        idx = index(trows) if use_idx else None
+        p["adds"].append((t, idx, t[idx.long() if use_idx else torch.arange(rows, device=DEV), :512].double()))
+      if s.get("res") in ("fp32", "inplace"):
+        r = torch.full((rows + 1, LD), float("nan"), device=DEV)
+        r[:rows, :512] = randn(rows, 512)
+        p["res"] = r
+      self.params.append(p)
+    self.maxdist = 1      # largest distance from a kept layer to a layer that reads it
+    for l, s in enumerate(self.layers):
+      reads = [sg[1] for sg in s["segs"] if sg[0] == "keep"]
+      if isinstance(s.get("res"), tuple) and s["res"][0] == "keep":
+        reads.append(s["res"][1])
+      self.maxdist = max([self.maxdist] + [l - j for j in reads])
+    self.nq = sum(1 for s in self.layers if s.get("keep"))
+
+  def nslots(self, lag, order):
+    return max(lag, 1) * self.maxdist + (1 if order == 0 else 0)
+
+  def valid(self, lag, order):
+    return (order == 0 or len(self.layers) >= 3) and self.nslots(lag, order) <= 5
+
+  def scratch_need(self, lag, order):
+    return (self.lib.gcb_sm_count(0) // 2) * self.nq * self.nslots(lag, order) * 32 * 8448
+
+  def _nan(self):
+    return torch.full((self.rows + 1, LD), float("nan"), device=DEV)
+
+  def _img(self):
+    return torch.full((self.lib.gcb_a_image_bytes(self.rows, 512),), 0xFF, dtype=torch.uint8, device=DEV)
+
+  def _common(self, d, s, p):
+    d.w_packed = p["w_img"].data_ptr()
+    if s["kind"] == "ln":
+      d.ln_scale, d.ln_offset = p["scale"].data_ptr(), p["offset"].data_ptr()
+    d.act = _native.ACT_SWISH if s["kind"] == "swish" else _native.ACT_NONE
+    d.n_pre_add = len(p["adds"])
+    for i, (t, idx, _) in enumerate(p["adds"]):
+      d.pre_add[i].table, d.pre_add[i].ld = t.data_ptr(), LD
+      d.pre_add[i].idx = idx.data_ptr() if idx is not None else None
+
+  def run_chain(self, prec, lag, order, short=0):
+    """One gcb_chain_forward with scratch_bytes = the need - short: (status, {(layer, output): buffer})."""
+    work = {name: img.clone() for name, img in self.images.items()}
+    ch = _native.ChainDesc()
+    ch.rows, ch.nlayers, ch.precision, ch.lag, ch.order = (self.rows, len(self.layers), _native.PRECISIONS[prec],
+                                                          lag, order)
+    scratch = None
+    if self.nq:
+      need = self.scratch_need(lag, order)
+      scratch = torch.empty(need, dtype=torch.uint8, device=DEV)
+      ch.scratch, ch.scratch_bytes = scratch.data_ptr(), need - short
+    outs = {}
+    for l, (s, p) in enumerate(zip(self.layers, self.params)):
+      cl = ch.layer[l]
+      cl.nseg = len(p["segs"])
+      for i in range(3):
+        cl.seg_from[i] = -1
+      for i, sg in enumerate(p["segs"]):
+        if isinstance(sg, int):
+          cl.seg_from[i], cl.seg[i].k = sg, 512
+        else:
+          cl.seg[i] = sg[0]
+          if sg[1] is not None:
+            cl.seg[i].img = work[sg[1]].data_ptr()
+      self._common(cl, s, p)
+      cl.bias = p["bias"].data_ptr() if p["bias"] is not None else None
+      cl.keep = 1 if s.get("keep") else 0
+      res = s.get("res")
+      if res == "fp32":
+        cl.residual, cl.ld_res = p["res"].data_ptr(), LD
+      elif res == "inplace":
+        outs[l, "out"] = p["res"].clone()
+        cl.residual, cl.ld_res = outs[l, "out"].data_ptr(), LD
+        cl.out, cl.ld_out = outs[l, "out"].data_ptr(), LD
+      elif res is not None and res[0] == "img":
+        cl.residual_img = work[res[1]].data_ptr()
+      elif res is not None:
+        cl.residual_keep = res[1] + 1
+      if s.get("out") and res != "inplace":
+        outs[l, "out"] = self._nan()
+        cl.out, cl.ld_out = outs[l, "out"].data_ptr(), LD
+      if s.get("out_y"):
+        outs[l, "out_y"] = self._nan()
+        cl.out_y, cl.ld_out_y = outs[l, "out_y"].data_ptr(), LD
+      if s.get("out_img"):
+        outs[l, "img"] = work[s["out_img"]] if isinstance(s["out_img"], str) else self._img()
+        cl.out_img = outs[l, "img"].data_ptr()
+    rc = self.lib.gcb_chain_forward(C.byref(ch), _stream())
+    torch.cuda.synchronize()
+    return rc, outs
+
+  def run_layers(self, prec):
+    """The same layers through gcb_layer_forward: {(layer, output): buffer}, and per layer the fp32
+    residual it added (an image residual decoded) or None."""
+    rows = self.rows
+    outs, resid = {}, []
+    for l, (s, p) in enumerate(zip(self.layers, self.params)):
+      d = _native.LayerDesc()
+      d.rows, d.n, d.n_valid, d.nseg = rows, 512, 512, len(p["segs"])
+      for i, sg in enumerate(p["segs"]):
+        if isinstance(sg, int):
+          d.seg[i].img, d.seg[i].k, d.seg[i].k_valid, d.seg[i].fan = outs[sg, "img"].data_ptr(), 512, 512, 1
+        else:
+          d.seg[i] = sg[0]
+      self._common(d, s, p)
+      d.bias = (p["bias"] if p["bias"] is not None else p["zero_bias"]).data_ptr()
+      d.precision = _native.PRECISIONS[prec]
+      res, r = s.get("res"), None
+      if res in ("fp32", "inplace"):
+        r = p["res"]
+      elif res is not None:      # hi + lo is exact in fp32: the value the chain adds
+        r = _image_values(self.images[res[1]] if res[0] == "img" else outs[res[1], "img"], rows, 512).contiguous()
+      resid.append(r)
+      if r is not None:
+        d.residual, d.ld_res = r.data_ptr(), r.shape[1]
+      if s.get("out") or res == "inplace":
+        outs[l, "out"] = self._nan()
+        d.out, d.ld_out = outs[l, "out"].data_ptr(), LD
+      if s.get("out_y") or (r is not None and not (s.get("out") or res == "inplace")):
+        outs[l, "out_y"] = self._nan()      # the layer kernel adds a residual only beside out / out_y
+        d.out_y, d.ld_out_y = outs[l, "out_y"].data_ptr(), LD
+      if s.get("keep") or s.get("out_img"):
+        outs[l, "img"] = self._img()
+        d.out_img = outs[l, "img"].data_ptr()
+      _native.check(self.lib.gcb_layer_forward(C.byref(d), _stream()), f"layer {l}")
+    torch.cuda.synchronize()
+    return outs, resid
+
+  def reference(self, l, lbl, resid):
+    """float64 (y, residual + y) of layer l from the inputs it read."""
+    s, p = self.layers[l], self.params[l]
+    z = torch.cat([_image_values(lbl[v, "img"], self.rows, 512).double() if isinstance(v, int) else v
+                   for v in p["vals"]], 1)
+    pre = z @ p["w"].double()
+    if p["bias"] is not None:
+      pre += p["bias"].double()
+    for _, _, a in p["adds"]:
+      pre += a
+    y = pre * torch.sigmoid(pre) if s["kind"] == "swish" else pre
+    if s["kind"] == "ln":
+      y = torch.nn.functional.layer_norm(y, (512,), p["scale"].double(), p["offset"].double(), 1e-5)
+    r = resid[l]
+    return y, (y + r[:self.rows, :512].double() if r is not None else y)
+
+  def snapshot(self, outs):
+    """Every output of a chain launch: fp32 buffers whole, images as full-tile bytes + row values."""
+    full = (self.rows // 128) * 32 * 8448
+    snap = {}
+    for key, t in outs.items():
+      snap[key] = [t.clone()] if key[1] != "img" else [t[:full].clone(), _image_values(t, self.rows, 512)]
+    return snap
+
+
+def _same(a, b):
+  """Bit equality of fp32 or byte tensors (NaN padding included)."""
+  if a.dtype == torch.float32:
+    return torch.equal(a.view(torch.int32), b.view(torch.int32))
+  return torch.equal(a, b)
+
+
+# Specs.  Every kept layer is read through seg_from (gcb_chain_forward refuses it otherwise).
+_CHAINS = {
+    "1_plain_out_out_y": dict(order=0, layers=[
+        dict(segs=[("img", 512), ("tab", None, 508, 512, False, 1)], kind="plain", out=True, out_y=True)]),
+    "1_layernorm_in_place_residual": dict(order=0, layers=[
+        dict(segs=[("tab", 400, 512, 512, True, 1), ("tab", None, 256, 256, False, 3)], kind="ln",
+             res="inplace", out_y=True, out_img=True)]),
+    "2_gathers_fan3_two_addends": dict(order=0, layers=[
+        dict(segs=[("img", 512), ("tab", 300, 512, 512, True, 3), ("tab", None, 4, 16, False, 1)],
+             kind="swish", keep=True, pre=[(700, True), (None, False)]),
+        dict(segs=[("keep", 0)], kind="ln", res="fp32", out=True, out_y=True, out_img=True)]),
+    "2_plain_one_addend": dict(order=0, layers=[
+        dict(segs=[("img", 512)], kind="plain", keep=True, out=True, out_y=True, pre=[(500, True)]),
+        dict(segs=[("keep", 0)], kind="swish", out_img=True)]),
+    "3_two_scratch_and_image": dict(order=1, layers=[
+        dict(segs=[("img", 256)], kind="swish", keep=True, out_img=True),
+        dict(segs=[("keep", 0)], kind="plain", keep=True, out=True),
+        dict(segs=[("keep", 1), ("keep", 0), ("img", 512)], kind="ln", res="fp32", out=True, out_img=True)]),
+    "3_same_kept_layer_twice": dict(order=1, layers=[
+        dict(segs=[("tab", None, 508, 512, False, 1)], kind="swish", keep=True),
+        dict(segs=[("keep", 0)], kind="swish", keep=True),
+        dict(segs=[("keep", 1), ("img", 512), ("keep", 1)], kind="plain", out_y=True)]),
+    "4_node_block": dict(order=1, layers=[      # the processor's node MLP + next edge MLP's projections
+        dict(segs=[("img", 512, "v"), ("img", 512)], kind="swish", keep=True),
+        dict(segs=[("keep", 0)], kind="ln", res=("img", "v"), out_img="v", keep=True),
+        dict(segs=[("keep", 1)], kind="plain", bias=False, out=True),
+        dict(segs=[("keep", 1)], kind="plain", bias=False, out=True)]),
+    "4_embedder_edge_block": dict(order=1, layers=[   # edge embedder MLP -> edge MLP, e1 = e0 + m
+        dict(segs=[("tab", None, 4, 16, False, 1)], kind="swish", keep=True),
+        dict(segs=[("keep", 0)], kind="ln", keep=True),
+        dict(segs=[("keep", 1)], kind="swish", keep=True, pre=[(3000, True), (2000, True)]),
+        dict(segs=[("keep", 2)], kind="ln", res=("keep", 1), out_y=True, out_img=True)]),
+    "2_node_update_in_place": dict(order=0, layers=[
+        dict(segs=[("img", 512, "x"), ("img", 512)], kind="swish", keep=True),
+        dict(segs=[("keep", 0)], kind="ln", res=("img", "x"), out_img="x", out_y=True)]),
+    "5_residual_keep_distance3_8_vectors": dict(order=1, layers=[
+        dict(segs=[("img", 512)], kind="swish", keep=True),
+        dict(segs=[("keep", 0)], kind="ln", keep=True, out=True),
+        dict(segs=[("keep", 1)], kind="swish", keep=True),
+        dict(segs=[("keep", 2)], kind="plain", bias=False, keep=True),
+        dict(segs=[("keep", 3)], kind="ln", res=("keep", 1), out_y=True, out_img=True)]),
+    "6_distance5": dict(order=1, layers=[
+        dict(segs=[("tab", None, 64, 64, False, 1)], kind="swish", keep=True),
+        dict(segs=[("keep", 0)], kind="plain", bias=False, keep=True, out_y=True),
+        dict(segs=[("keep", 1)], kind="plain", bias=False, keep=True),
+        dict(segs=[("keep", 2)], kind="swish", keep=True),
+        dict(segs=[("keep", 3)], kind="plain", bias=False, keep=True),
+        dict(segs=[("keep", 4), ("keep", 0)], kind="ln", res="fp32", out=True, out_y=True, out_img=True)]),
+    "2_layernorm_without_bias": dict(order=0, layers=[
+        dict(segs=[("tab", 900, 512, 512, True, 1)], kind="ln", bias=False, keep=True),
+        dict(segs=[("keep", 0)], kind="ln", bias=False, res="fp32", out=True)]),
+}
+
+
+def _chain_rows(which):
+  """1, 127, 129; one tile per cluster and a second one for cluster 0; and 3 x 5 (the most slots a
+  ring has) tiles per cluster plus a ragged one, so that every cluster rewrites every slot of every
+  ring at least twice."""
+  clusters = _native.lib().gcb_sm_count(0) // 2
+  return {"one_more_tile": clusters * 128 + 1, "slots_reused": 3 * 5 * clusters * 128 + 77}.get(which, which)
+
+
+@pytest.mark.parametrize("prec", ["bf16x3", "bf16"])
+@pytest.mark.parametrize("rows", [1, 127, 129, "one_more_tile", "slots_reused"])
+@pytest.mark.parametrize("name", sorted(_CHAINS))
+def test_chain_matches_the_layer_kernel_and_fp64(name, rows, prec):
+  """A chain equals the same layers run one by one through gcb_layer_forward bit for bit (decoded
+  image values where the chain adds an image residual: hi + lo is exact in fp32, only the sign of a
+  zero may differ), every layer is within the layer kernel's tolerance of float64, fp32 outputs
+  leave the row past the end and the padding columns untouched, and every valid (lag, order) and
+  cluster size gives the same bytes.  The scratch the chain needs is accepted, 16 bytes less is not."""
+  rows = _chain_rows(rows)
+  c = _Chain(_CHAINS[name], rows, seed=zlib.crc32(name.encode()))
+  rc, got = c.run_chain(prec, 1, c.order)
+  _native.check(rc, "chain")
+  lbl, resid = c.run_layers(prec)
+  rel = lambda got, want: float((got.double() - want).abs().max() / want.abs().max())
+  errs = []
+  for l, s in enumerate(c.layers):
+    y, want = c.reference(l, lbl, resid)
+    checks = []       # (relative error against float64, tolerance)
+    image_res = s["kind"] == "ln" and isinstance(s.get("res"), tuple)
+    for key, ref in (("out", want), ("out_y", y)):
+      if (l, key) not in got:
+        continue
+      t = got[l, key]
+      assert _same(t[:rows, :512], lbl[l, key][:rows, :512]), f"layer {l} {key} differs from the layer kernel"
+      assert torch.isnan(t[rows]).all() and torch.isnan(t[:, 512:]).all(), f"layer {l} {key} written outside"
+      checks.append((rel(t[:rows, :512], ref), TOL[prec]))
+    lbl_vals = _image_values(lbl[l, "img"], rows, 512) if (l, "img") in lbl else None
+    if (l, "img") in got:
+      img = got[l, "img"]
+      vals = _image_values(img, rows, 512)
+      assert torch.equal(vals, lbl_vals), f"layer {l} image values differ from the layer kernel"
+      if not image_res:
+        full = (rows // 128) * 32 * 8448
+        assert torch.equal(img[:full], lbl[l, "img"][:full]), f"layer {l} image bytes differ"
+      checks.append((rel(vals, want), TOL[prec] + 2 ** -16))    # + the image's hi + lo rounding
+    elif s.get("keep"):   # kept only: the result as the layer kernel hands it over
+      checks.append((rel(lbl_vals, want), TOL[prec] + 2 ** -16))
+    if image_res and (l, "out_y") in got:
+      # the image of x = (y + 0) + (hi + lo) split into bf16 hi and lo, both rounded to nearest even
+      x = (got[l, "out_y"][:rows, :512] + 0.0) + resid[l]
+      hi = x.to(torch.bfloat16)
+      lo = (x - hi.float()).to(torch.bfloat16)
+      whi, wlo = _image_words(got[l, "img"], rows)
+      assert torch.equal(whi, hi.view(torch.int16)) and torch.equal(wlo, lo.view(torch.int16)), f"layer {l}"
+    for err, tol in checks:
+      assert err < tol, f"layer {l}: relative error {err:.3e} vs float64 (tolerance {tol:.1e})"
+    errs.append(max(err for err, _ in checks))
+  print(f"chain vs float64 {name} {prec} rows={rows}: per-layer errors " + " ".join(f"{e:.2e}" for e in errs))
+  # every valid schedule, and the cluster size, give the same bytes
+  want = c.snapshot(got)
+
+  def same_as_default(outs, what):
+    for key, parts in c.snapshot(outs).items():
+      assert all(_same(a, b) for a, b in zip(parts, want[key])), f"{what}: {key} differs"
+
+  for lag in (0, 1, 2):
+    for order in (0, 1):
+      if c.valid(lag, order) and (lag, order) != (1, c.order):
+        rc, outs = c.run_chain(prec, lag, order)
+        _native.check(rc, f"lag {lag} order {order}")
+        same_as_default(outs, f"lag {lag} order {order}")
+      elif not c.valid(lag, order):
+        assert c.run_chain(prec, lag, order)[0] == -1
+  lib = c.lib
+  try:
+    for cs in (1, 4):
+      _native.check(lib.gcb_set_cluster_size(cs), "gcb_set_cluster_size")
+      rc, outs = c.run_chain(prec, 1, c.order)
+      _native.check(rc, f"cluster size {cs}")
+      same_as_default(outs, f"cluster size {cs}")
+  finally:
+    assert lib.gcb_set_cluster_size(2) == 0
+  if c.nq:
+    assert c.run_chain(prec, 1, c.order, short=16)[0] == -1
+    assert b"scratch too small" in lib.gcb_last_error()

@@ -136,6 +136,94 @@ def test_layer_refusals_name_the_unsupported_case():
     assert lib.gcb_set_cluster_size(2) == 0
 
 
+def test_chain_refusals_name_the_unsupported_case():
+  """Chains the kernel cannot run are refused by gcb_chain_forward's argument checks, as layers are
+  above: rows = 0 and dummy pointers, so an accepted descriptor returns 0 without a launch.  The
+  scratch is far larger than any chain needs (the need depends on the SM count, which a machine
+  without a GPU takes to be 132)."""
+  lib = _native.lib()
+  LN = dict(ln_scale=256, ln_offset=256)
+
+  def chain(*layers, lag=1, order=0):
+    """layers: gcb_chain_layer fields per layer, and `reads`: its seg_from entries (-1: an external
+    fp32 table of 512 columns).  Every layer is plain with a bias and an fp32 `out` unless told
+    otherwise."""
+    d = _native.ChainDesc()
+    d.rows, d.nlayers, d.precision, d.lag, d.order = 0, len(layers), _native.PREC_BF16X3, lag, order
+    d.scratch, d.scratch_bytes = 256, 1 << 40
+    for cl, spec in zip(d.layer, layers):
+      spec = dict(spec)
+      reads = spec.pop("reads", (-1,))
+      cl.nseg = len(reads)
+      for s in range(3):
+        cl.seg_from[s] = reads[s] if s < len(reads) else -1
+      for s, j in enumerate(reads):
+        cl.seg[s].k = 512
+        if j < 0:
+          cl.seg[s].table, cl.seg[s].ld, cl.seg[s].k_valid, cl.seg[s].fan = 256, 512, 512, 1
+      cl.w_packed, cl.bias, cl.out, cl.ld_out = 256, 256, 256, 512
+      for name, value in spec.items():
+        setattr(cl, name, value)
+    return d
+
+  def line(n, **kw):
+    """n layers, layer l reading layer l - 1 and the last also layer 0: distance n - 1."""
+    layers = [dict(keep=1)] + [dict(reads=(l - 1,), keep=1) for l in range(1, n - 1)]
+    return chain(*layers, dict(reads=(n - 2, 0) if n > 2 else (n - 2,)), **kw)
+
+  def refused(d, why):
+    assert lib.gcb_chain_forward(C.byref(d), None) == -1
+    assert why in lib.gcb_last_error(), lib.gcb_last_error()
+
+  def accepted(d):
+    assert lib.gcb_chain_forward(C.byref(d), None) == 0, lib.gcb_last_error()
+
+  swish_kept = dict(act=_native.ACT_SWISH, out=None, keep=1)
+  # A kept layer's scratch slot is released for reuse only by its seg_from readers.
+  no_reader = b"a kept layer must be read through seg_from by a later layer"
+  refused(chain(dict(keep=1)), no_reader)
+  refused(chain(dict(keep=1, out=None)), no_reader)
+  refused(chain(swish_kept, dict(LN, out=None, out_y=256, ld_out_y=512, residual_keep=1)), no_reader)
+  accepted(chain(swish_kept, dict(LN, reads=(0,), out=None, out_y=256, ld_out_y=512, residual_keep=1)))
+  refused(chain(swish_kept, dict(reads=(0,), keep=1)), no_reader)
+  accepted(chain(swish_kept, dict(reads=(0,))))
+  # slots per ring: lag x distance (+ 1 in ascending order), at most 5
+  too_far = b"lag x distance too large"
+  refused(line(4, lag=2, order=0), too_far)
+  refused(line(4, lag=2, order=1), too_far)
+  accepted(line(3, lag=2, order=1))
+  refused(line(6, lag=1, order=0), too_far)
+  accepted(line(6, lag=1, order=1))
+  accepted(line(6, lag=0, order=1))
+  accepted(line(5, lag=1, order=0))
+  refused(line(6, lag=3, order=1), b"lag must be 0 (default), 1 or 2")
+  refused(chain(*[dict()] * 7), b"nlayers must be 1..GCB_MAX_CHAIN")
+  # at most 8 bias / LayerNorm parameter vectors
+  refused(chain(dict(LN, keep=1), dict(LN, reads=(0,), keep=1), dict(LN, reads=(1,))),
+          b"too many bias / LayerNorm vectors")
+  accepted(chain(dict(LN, keep=1), dict(LN, reads=(0,), keep=1), dict(LN, reads=(1,), bias=None)))
+  # the descending order needs 3 layers
+  refused(line(2, order=1), b"order must be 0, or 1 for chains of at least 3 layers")
+  accepted(line(2, order=0))
+  accepted(line(3, order=1))
+  # residuals on LayerNorm layers only; swish layers deliver operand images only
+  refused(chain(dict(residual=256, ld_res=512)), b"residual needs a LayerNorm layer")
+  refused(chain(dict(residual_img=256, out=None, out_y=256, ld_out_y=512)), b"residual needs a LayerNorm layer")
+  accepted(chain(dict(LN, residual=256, ld_res=512)))
+  refused(chain(dict(act=_native.ACT_SWISH)), b"a swish chain layer delivers operand images only")
+  refused(chain(dict(act=_native.ACT_SWISH, out=None, out_y=256, ld_out_y=512)),
+          b"a swish chain layer delivers operand images only")
+  accepted(chain(dict(act=_native.ACT_SWISH, out=None, out_img=256)))
+  refused(chain(dict(LN, act=_native.ACT_SWISH, out=None, out_img=256)), b"swish OR LayerNorm")
+  # residual_keep names an earlier kept layer
+  bad_keep = b"residual_keep must name an earlier kept layer"
+  rk = dict(LN, out=None, out_y=256, ld_out_y=512)
+  refused(chain(dict(act=_native.ACT_SWISH, out=None, out_img=256), dict(rk, residual_keep=1)), bad_keep)
+  refused(chain(dict(rk, residual_keep=2), dict(keep=1), dict(reads=(1,))), bad_keep)
+  refused(chain(swish_kept, dict(rk, reads=(0,), residual_keep=2)), bad_keep)
+  refused(chain(swish_kept, dict(rk, reads=(0,), residual_keep=1, out=256)), bad_keep)
+
+
 def test_debug_flags_accepts_only_zero():
   """The build has no kernel experiment switches: 0 is accepted, anything else is an error."""
   lib = _native.lib()
