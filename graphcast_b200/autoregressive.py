@@ -261,9 +261,10 @@ class Predictor(graphcast.Predictor):
     inputs only (_layout): the stash holds their values, and the tensors of noised inputs (1.9 GB at
     0.25 degree) must not outlive the forward.
 
-    With tangent_run (a graphcast._TangentRun of one direction: loss_and_input_hvp), every step also
-    carries the input tangent planes on the device (GraphCast._device_loss_tangent) and keeps them in
-    pinned host memory too: first["tangents"] is that StepStash."""
+    With tangent_run (a graphcast._TangentRun of one direction: loss_and_input_hvp; of K directions:
+    a pass of batched_loss_and_input_hvp), every step also carries the input tangent planes of every
+    direction on the device (GraphCast._device_loss_tangent) and keeps them in pinned host memory too:
+    first["tangents"] is that StepStash."""
     records, first = [], {}
     stash = None
 
@@ -351,6 +352,43 @@ class Predictor(graphcast.Predictor):
     return (loss, diagnostics) + model._input_grads(stash, plan, first["norm"], inputs, forcings,
                                                     lat_weight=lat_weight, coef=coef,
                                                     tangents=first["tangents"])
+
+  def batched_loss_and_input_hvp(self, inputs, targets, forcings, input_tangents,
+                                 forcing_tangents=None, rng=None, *, directions_per_pass=None,
+                                 _noise_fold: int = 0, **kwargs):
+    """loss_and_input_hvp along K tangent directions at once (GraphCast.batched_loss_and_input_hvp),
+    over every target time: the tangent Datasets carry a leading "direction" dim (the forcing tangents
+    cover every target time), and so do input_hvp and forcing_hvp; the loss, diagnostics and gradients
+    are bit for bit those of loss_and_input_grads.  One target time delegates to the inner predictor.
+    Several need gradient_checkpointing=True: each pass of directions_per_pass directions (None: all)
+    is what loss_and_input_hvp runs, with every step's K tangents carried on the device and stashed
+    together, and each step's recompute and backward walk shared by the gradient and its K tangents.
+    With noise, everything is taken at noisy_inputs(inputs, targets, forcings, rng), the same noise in
+    every pass."""
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    forcings = xs.from_xarray(forcings)
+    if targets.sizes["time"] == 1:
+      return self._predictor.batched_loss_and_input_hvp(inputs, targets, forcings, input_tangents,
+                                                        forcing_tangents,
+                                                        directions_per_pass=directions_per_pass,
+                                                        **kwargs)
+    model, norm_of = self._checkpointed_parts(inputs, targets, forcings, "input gradients")
+    one = lambda ds: ds.isel(time=slice(0, 1))
+
+    def one_pass(it, ft):
+      run = graphcast._TangentRun(inputs, forcings, it, ft, targets.sizes["time"],
+                                  feedback.FeedbackPlan(inputs, one(targets), one(forcings)),
+                                  directions=True)
+      loss, diagnostics, stash, first, lat_weight, coef = self._checkpointed_loss(
+          model, norm_of, self._noised(inputs, targets, forcings, rng, _noise_fold), targets,
+          forcings, tangent_run=run)
+      del run
+      plan = feedback.FeedbackPlan.all_channels(first["inputs"], first["targets"], first["forcings"])
+      return (loss, diagnostics) + model._input_grads(stash, plan, first["norm"], inputs, forcings,
+                                                      lat_weight=lat_weight, coef=coef,
+                                                      tangents=first["tangents"])
+    return graphcast.batched_hvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
+                                 directions_per_pass)
 
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
     """(predictions, input_grads, forcing_grads): `predictions` as __call__ returns them, the gradients

@@ -124,7 +124,9 @@ class Backward:
     self._edge_iota = None
     # the tangent of several directions (tangent(dirs=...)): their K-fold gather indices and chunks
     self.dirs = 1
-    self._kfold, self._kfold_dirs = {}, 1
+    # kfold's indices: {fold count: {key: index}}, the two fold counts used last (a Hessian-vector
+    # product's walk reads K-fold and (1 + K)-fold indices in one pass)
+    self._kfold = {}
     self._tangent_chunks = {}
     self.zero_bias = torch.zeros([D], dtype=torch.float32, device=dev)
     self.prec = _native.PRECISIONS[eng.precision]
@@ -133,9 +135,9 @@ class Backward:
     self.ws_wg = torch.empty([nb], dtype=torch.uint8, device=dev)
     # element(param_grads=False): the column sums of the row-wise kernels land here, never in info.g
     self.param_grads = True
-    # element(hvp=...): the tangent snapshots of the forward (tangent(snaps=...)); the walk then carries
-    # the gradient (direction 0) and its tangent (direction 1)
-    self.hvp = None
+    # element(hvp=...): the tangent snapshots of the forward (tangent(snaps=...)) of self.tdirs = K
+    # directions; the walk then carries the gradient (direction 0) and its K tangents (directions 1..K)
+    self.hvp, self.tdirs = None, 0
     self.sink = {f: torch.zeros([D], dtype=torch.float32, device=dev)
                  for f in ("b0", "b1", "scale", "offset")}
 
@@ -301,10 +303,12 @@ class Backward:
     direction, and the two nonlinearities are gcb_layernorm_backward_dirs and gcb_swish_jvp, whose
     results are those of the one-direction kernels without the column sums.
 
-    In a Hessian-vector product (self.hvp set, two directions: the gradient and its tangent), `tan` =
-    (dsegs, dpre, dw0) is the tangent of the layer-0 input as mlp_jvp takes it (one direction, plain
-    gather indices): h-dot = dsegs W0 + the gathered addends, z-dot = W1 (swish'(h) h-dot), and the two
-    nonlinearities are gcb_layernorm_backward_jvp and gcb_swish_backward_jvp."""
+    In a Hessian-vector product (self.hvp set, 1 + K directions: the gradient and its tangents along K
+    primal tangents, K = self.tdirs), `tan` = (dsegs, dpre, dw0) is the tangent of the layer-0 input as
+    mlp_jvp takes it (stacked tables of K directions, K-fold gather indices): h-dot = dsegs W0 + the
+    gathered addends, z-dot = W1 (swish'(h) h-dot), each one GEMM over the K directions, and the two
+    nonlinearities are gcb_layernorm_backward_jvp_dirs and gcb_swish_backward_jvp_dirs, which form the
+    primal terms once for all K."""
     w = info.w
     w0 = w0 or w.w0_packed
     nd, stride, rk = self.dirs, self.dir_stride(rows), self.dir_rows(rows)
@@ -321,16 +325,18 @@ class Backward:
       self.layer(rows, [self.tab(a)], w.w1_packed, w.b1, out_y=z)
       del a
       dz = self.empty(rk)
-      if hd is not None:                     # z-dot = W1 (swish'(h) h-dot)
-        ad = self.empty(rows)
-        _native.check(self.lib.gcb_swish_jvp(h.data_ptr(), D, rows, D, hd.data_ptr(), D, rows, 1,
+      if hd is not None:                     # z-dot = W1 (swish'(h) h-dot), K directions
+        nt = self.tdirs
+        rt = self.dir_rows(rows, nt)
+        ad = self.empty(rt)
+        _native.check(self.lib.gcb_swish_jvp(h.data_ptr(), D, rows, D, hd.data_ptr(), D, stride, nt,
                                              ad.data_ptr(), D, self._st()), "gcb_swish_jvp")
-        zd = self.empty(rows)
-        self.layer(rows, [self.tab(ad)], w.w1_packed, self.zero_bias, out_y=zd)
+        zd = self.empty(rt)
+        self.layer(rt, [self.tab(ad)], w.w1_packed, self.zero_bias, out_y=zd)
         del ad
-        _native.check(self.lib.gcb_layernorm_backward_jvp(
+        _native.check(self.lib.gcb_layernorm_backward_jvp_dirs(
             dy.data_ptr(), dy.shape[1], z.data_ptr(), D, zd.data_ptr(), D, w.ln_scale, rows, D, stride,
-            dz.data_ptr(), D, self._st()), "gcb_layernorm_backward_jvp")
+            dz.data_ptr(), D, nt, self._st()), "gcb_layernorm_backward_jvp_dirs")
         del zd
       elif nd == 1:
         _native.check(self.lib.gcb_layernorm_backward(
@@ -352,11 +358,11 @@ class Backward:
       self.wgrad(self.tab(h), dz, rows, g["w1"], n=info.n1, swish=True)     # dW1 = swish(h)^T dz
     da = self.empty(rk)
     self.layer(rk, [self.tab(dz, info.n1)], info.t["w1"], self.zero_bias, out_y=da)
-    if hd is not None:                       # [swish'(h) da; d/dt of it] in place
+    if hd is not None:                       # [swish'(h) da; its K tangents] in place
       dh = da
-      _native.check(self.lib.gcb_swish_backward_jvp(
+      _native.check(self.lib.gcb_swish_backward_jvp_dirs(
           h.data_ptr(), D, hd.data_ptr(), D, rows, D, da.data_ptr(), D, stride, dh.data_ptr(), D,
-          self._st()), "gcb_swish_backward_jvp")
+          self.tdirs, self._st()), "gcb_swish_backward_jvp_dirs")
       del hd
     elif nd == 1:
       dh = self.empty(rows)
@@ -377,18 +383,20 @@ class Backward:
     return dh
 
   def _hdot(self, rows: int, w0, tan) -> torch.Tensor:
-    """h-dot [rows, 512] of an MLP's first layer from tan = (dsegs, dpre, dw0) (see mlp_backward):
-    dsegs W0 (dw0: the weight of those segments, default w0) plus the gathered addends dpre, or the
-    addends alone; zeros when the layer input has no tangent."""
+    """h-dot of an MLP's first layer, a stacked table of self.tdirs directions of `rows` rows, from
+    tan = (dsegs, dpre, dw0) (see mlp_backward): dsegs W0 (dw0: the weight of those segments, default
+    w0) plus the gathered addends dpre, or the addends alone; zeros when the layer input has no
+    tangent."""
     dsegs, dpre, dw0 = tan if tan is not None else ([], (), None)
+    rt = self.dir_rows(rows, self.tdirs)
     if dsegs:
-      hd = self.empty(rows)
-      self.layer(rows, dsegs, dw0 or w0, self.zero_bias, out_y=hd, pre=list(dpre) or None)
+      hd = self.empty(rt)
+      self.layer(rt, dsegs, dw0 or w0, self.zero_bias, out_y=hd, pre=list(dpre) or None)
       return hd
     hd = None
     for table, idx in dpre:
-      hd = self.gather_add(table, idx, rows, hd)
-    return hd if hd is not None else torch.zeros([max(rows, 1), D], dtype=torch.float32, device=self.dev)
+      hd = self.gather_add(table, idx, rt, hd)
+    return hd if hd is not None else torch.zeros([max(rt, 1), D], dtype=torch.float32, device=self.dev)
 
   def sender_sums(self, dh: torch.Tensor, rows: int, csr, num_nodes: int) -> torch.Tensor:
     """gcb_segment_sum_sorted (sender CSR `csr`) of every direction of the stacked edge table dh (`rows`
@@ -427,16 +435,20 @@ class Backward:
                     rcv_sum, tan=None) -> tuple:
     """Backward of a pre-gathered edge MLP m = MLP([e | v_s[snd] | v_r[rcv]]): accumulates its
     parameter gradients, returns (dH, S, R).  tan (Hessian-vector products): (edge tangent segments,
-    sender node tangent table, receiver node tangent table)."""
+    sender node tangent table, receiver node tangent table), stacked tables of self.tdirs directions;
+    their projections are gathered with K-fold indices keyed (snd_name, "snd" | "rcv"), those of
+    tangent()."""
     sp = info.split
     ps = self.projection(n_s, v_s, sp.ws_packed)
     pr = self.projection(n_r, v_r, sp.wr_packed)
     t = None
     if tan is not None:
       de_segs, dv_s, dv_r = tan
-      dps = self.projection(n_s, self.tab(dv_s), sp.ws_packed)
-      dpr = self.projection(n_r, self.tab(dv_r), sp.wr_packed)
-      t = (de_segs, [(dps, snd), (dpr, rcv)], None)
+      nt = self.tdirs
+      dps = self.projection(self.dir_rows(n_s, nt), self.tab(dv_s), sp.ws_packed)
+      dpr = self.projection(self.dir_rows(n_r, nt), self.tab(dv_r), sp.wr_packed)
+      t = (de_segs, [(dps, self.kfold(snd, n_s, (snd_name, "snd"), nt)),
+                     (dpr, self.kfold(rcv, n_r, (snd_name, "rcv"), nt))], None)
     dh = self.mlp_backward(info, rows, [e_seg], dm, pre=[(ps, snd), (pr, rcv)], w0=sp.we_packed,
                            tan=t)
     del ps, pr, t
@@ -461,15 +473,18 @@ class Backward:
     one direction alone gives.  The stacked temporaries of a chunk therefore grow with the direction
     count.
 
-    tan (Hessian-vector products): the node tangent tables (sender, receiver or None); the edge
-    embedder's output has no tangent."""
+    tan (Hessian-vector products): the node tangent tables (sender, receiver or None), stacked tables
+    of self.tdirs directions; the edge embedder's output has no tangent.  Their projections are
+    gathered in a chunk with K-fold indices of that chunk (keys (name, "hvp", i, ...))."""
     sp = info.split
     ps = self.projection(n_s, v_s, sp.ws_packed)
     pr = self.projection(n_r, v_r, sp.wr_packed)
     dps = dpr = None
+    nt = self.tdirs
     if tan is not None:
-      dps = self.projection(n_s, self.tab(tan[0]), sp.ws_packed)
-      dpr = None if tan[1] is None else self.projection(n_r, self.tab(tan[1]), sp.wr_packed)
+      dps = self.projection(self.dir_rows(n_s, nt), self.tab(tan[0]), sp.ws_packed)
+      dpr = None if tan[1] is None else self.projection(self.dir_rows(n_r, nt), self.tab(tan[1]),
+                                                        sp.wr_packed)
     s_tab, r_tab = None, self.empty(self.dir_rows(n_r))
     for i, (r0, r1, g0, g1, rp, heavy, n_heavy, csr) in enumerate(self.chunks[name]):
       n = r1 - r0
@@ -480,7 +495,8 @@ class Backward:
                            self.dir_rows(n))
       t = None
       if dps is not None:
-        t = ([], [(dps, snd_c)] + ([] if dpr is None else [(dpr, rcv_c)]), None)
+        t = ([], [(dps, self.kfold(snd_c, n_s, (name, "hvp", i, "snd"), nt))] + (
+            [] if dpr is None else [(dpr, self.kfold(rcv_c, n_r, (name, "hvp", i, "rcv"), nt))]), None)
       dh = self.mlp_backward(info, n, [self.tab(e)], dm, pre=[(ps, snd_c), (pr, rcv_c)],
                              w0=sp.we_packed, tan=t)
       del dm, e, snd_c, rcv_c, t
@@ -526,21 +542,25 @@ class Backward:
     embedder recomputes and the sender / receiver projections are formed once; the segment sums run
     per direction.  Direction k is bit for bit what g_out's direction k alone gives.
 
-    hvp (Hessian-vector products, dirs = 2, param_grads=False): the tangent snapshots of
-    tangent(snaps=...), entries dropped as they are consumed.  Direction 0 of g_out is the loss seed,
-    direction 1 its tangent; the walk is the same, every MLP also forms h-dot and z-dot from the
-    snapshots and differentiates its two nonlinearities with gcb_layernorm_backward_jvp and
-    gcb_swish_backward_jvp, so direction 1 of dx is the tangent of direction 0, and direction 0 is bit
-    for bit what g_out's direction 0 alone gives."""
+    hvp (Hessian-vector products, dirs = 1 + K with K >= 1, param_grads=False): the tangent snapshots
+    of tangent(dirs=K, snaps=...), stacked tables of K directions, entries dropped as they are consumed.
+    Direction 0 of g_out is the loss seed, direction j its tangent along primal tangent j - 1; the walk
+    is the same, every MLP also forms h-dot and z-dot of the K tangents from the snapshots (one GEMM
+    each over the K directions) and differentiates its two nonlinearities with
+    gcb_layernorm_backward_jvp_dirs and gcb_swish_backward_jvp_dirs, so direction j of dx is the
+    tangent of direction 0 along tangent j - 1.  Direction 0 is bit for bit what g_out's direction 0
+    alone gives, and direction j what the K = 1 walk gives for tangent j - 1 and seed direction j."""
     if dirs > 1 and param_grads:
       raise ValueError("several directions are supported without parameter gradients only")
-    if hvp is not None and (dirs != 2 or param_grads):
-      raise ValueError("a Hessian-vector product runs two directions without parameter gradients")
+    if hvp is not None and (dirs < 2 or param_grads):
+      raise ValueError("a Hessian-vector product runs 1 + K directions (K >= 1) without parameter "
+                       "gradients")
     self.param_grads, self.dirs, self.hvp = bool(param_grads), int(dirs), hvp
+    self.tdirs = 0 if hvp is None else int(dirs) - 1
     try:
       return self._element(grid_in_img, g_out, snaps, dgrid_in)
     finally:
-      self.param_grads, self.dirs, self.hvp = True, 1, None
+      self.param_grads, self.dirs, self.hvp, self.tdirs = True, 1, None, 0
 
   def _element(self, grid_in_img, g_out, snaps, dgrid_in):
     eng, m = self.eng, self.m
@@ -687,28 +707,33 @@ class Backward:
   def dir_stride(rows: int) -> int:
     return (rows + 127) // 128 * 128
 
-  def dir_rows(self, rows: int) -> int:
-    """Rows of a stacked tangent table of self.dirs directions of `rows` rows each."""
-    return (self.dirs - 1) * self.dir_stride(rows) + rows
+  def dir_rows(self, rows: int, dirs: Optional[int] = None) -> int:
+    """Rows of a stacked tangent table of `dirs` (default self.dirs) directions of `rows` rows each."""
+    return ((self.dirs if dirs is None else dirs) - 1) * self.dir_stride(rows) + rows
 
-  def kfold(self, idx: torch.Tensor, n_src: int, key) -> torch.Tensor:
-    """The gather index `idx` (into a table of n_src rows per direction) for self.dirs directions:
-    idx + k * dir_stride(n_src) in the rows of direction k of a stacked table of len(idx) rows per
-    direction, 0 in the pad rows.  Built on first use per `key` and kept while the direction count
-    stays the same.  The key names the index and, for a bipartite chunk, the chunk set it belongs to
-    ("tangent" | "backward"): with several directions the two sets differ, so chunk i of one is not
-    chunk i of the other."""
-    if self.dirs == 1:
+  def kfold(self, idx: torch.Tensor, n_src: int, key, folds: Optional[int] = None) -> torch.Tensor:
+    """The gather index `idx` (into a table of n_src rows per direction) for `folds` (default
+    self.dirs) directions: idx + k * dir_stride(n_src) in the rows of direction k of a stacked table of
+    len(idx) rows per direction, 0 in the pad rows.  Built on first use per (folds, key) and kept while
+    the fold count is one of the two used last (a Hessian-vector product's walk reads K-fold and
+    (1 + K)-fold indices in one pass, and its tangent forward K-fold ones).  The key names the index
+    and, for a bipartite chunk, the chunk set it belongs to ("tangent" | "backward" | "hvp"): with
+    several directions the sets differ, so chunk i of one is not chunk i of the other."""
+    folds = self.dirs if folds is None else int(folds)
+    if folds == 1:
       return idx
-    if self._kfold_dirs != self.dirs:
-      self._kfold, self._kfold_dirs = {}, self.dirs
-    out = self._kfold.get(key)
+    cache = self._kfold.pop(folds, None)
+    cache = {} if cache is None else cache
+    self._kfold[folds] = cache               # most recently used last
+    while len(self._kfold) > 2:
+      del self._kfold[next(iter(self._kfold))]
+    out = cache.get(key)
     if out is None:
       n, s_src, s = idx.shape[0], self.dir_stride(n_src), self.dir_stride(idx.shape[0])
-      out = torch.zeros([self.dir_rows(n)], dtype=torch.int32, device=self.dev)
-      for k in range(self.dirs):
+      out = torch.zeros([self.dir_rows(n, folds)], dtype=torch.int32, device=self.dev)
+      for k in range(folds):
         out[k * s:k * s + n] = idx + k * s_src
-      self._kfold[key] = out
+      cache[key] = out
     return out
 
   def tangent_chunks(self, name: str):
@@ -830,11 +855,13 @@ class Backward:
     mesh-node encoder, the three edge embedders, e_0 of the processor, and the v_m0 and edge terms of
     the grid2mesh edge MLP.
 
-    With `snaps` and `tsnaps` (dicts, one direction; Hessian-vector products) they receive what
-    element(hvp=tsnaps) reads: snaps the primal copies of Engine._forward_snapshots, tsnaps the tangent
-    tables v-dot_k (k = 0..K), e-dot_k (k = 1..K-1), agg-dot_k, and the v-dot / agg-dot of the grid
-    and mesh nodes around the encoder and decoder (vg0, agg1, vg1, agg3, vg2), and the packed input
-    tangent image (grid_in).  Without them nothing more is kept or launched."""
+    With `snaps` and `tsnaps` (dicts; Hessian-vector products, any number of directions) they receive
+    what element(dirs=1 + dirs, hvp=tsnaps) reads: snaps the primal copies of
+    Engine._forward_snapshots, tsnaps the tangent tables v-dot_k (k = 0..K), e-dot_k (k = 1..K-1),
+    agg-dot_k, and the v-dot / agg-dot of the grid and mesh nodes around the encoder and decoder (vg0,
+    agg1, vg1, agg3, vg2), and the packed input tangent image (grid_in).  The tangent tables are the
+    stacked tables of `dirs` directions the forward forms anyway: keeping them costs no copy, and their
+    memory grows with the directions.  Without them nothing more is kept or launched."""
     self.dirs = int(dirs)
     try:
       return self._tangent(grid_in_img, dgrid_in_img, snaps, tsnaps)

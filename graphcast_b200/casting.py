@@ -74,6 +74,12 @@ class Bfloat16Cast(graphcast.Predictor):
     return self._predictor.loss_and_input_hvp(inputs, targets, forcings, input_tangents,
                                               forcing_tangents, **kwargs)
 
+  def batched_loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
+                                 *, directions_per_pass=None, **kwargs):
+    return self._predictor.batched_loss_and_input_hvp(inputs, targets, forcings, input_tangents,
+                                                      forcing_tangents,
+                                                      directions_per_pass=directions_per_pass, **kwargs)
+
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
     return self._predictor.input_vjp(inputs, targets_template, forcings, cotangents, **kwargs)
 

@@ -1186,21 +1186,51 @@ int gcb_layernorm_backward_dirs(const float* dy, int32_t ld_dy, const float* z, 
   return GCB_OK;
 }
 
-int gcb_swish_backward_jvp(const float* h, int32_t ld_h, const float* hdot, int32_t ld_hdot,
-                           int64_t rows, int32_t n, const float* da, int32_t ld_da, int64_t dir_stride,
-                           float* dh, int32_t ld_dh, void* stream) {
+int gcb_swish_backward_jvp_dirs(const float* h, int32_t ld_h, const float* hdot, int32_t ld_hdot,
+                                int64_t rows, int32_t n, const float* da, int32_t ld_da,
+                                int64_t dir_stride, float* dh, int32_t ld_dh, int32_t tangents,
+                                void* stream) {
   GCB_CHECK_ARG(h && hdot && da && dh, "null pointer");
   GCB_CHECK_ARG(n > 0 && n % 4 == 0 && ld_h % 4 == 0 && ld_hdot % 4 == 0 && ld_da % 4 == 0 &&
                     ld_dh % 4 == 0 && ld_h >= n && ld_hdot >= n && ld_da >= n && ld_dh >= n &&
                     aligned16(h) && aligned16(hdot) && aligned16(da) && aligned16(dh),
                 "n / leading dimensions must be multiples of 4 with 16-byte rows");
   GCB_CHECK_ARG(rows >= 0 && dir_stride >= rows, "rows < 0 or dir_stride < rows");
+  GCB_CHECK_ARG(tangents >= 1, "tangents < 1");
   if (rows == 0) return GCB_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0, 4.0 * static_cast<double>(rows) * n * 6.0);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * static_cast<double>(rows) * n * (3.0 + 3.0 * tangents));
   const long long total = rows * (n / 4);
   gcb::swish_backward_jvp_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
-      h, ld_h, hdot, ld_hdot, rows, n / 4, da, ld_da, dir_stride, dh, ld_dh);
+      h, ld_h, hdot, ld_hdot, rows, n / 4, da, ld_da, dir_stride, tangents, dh, ld_dh);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int gcb_swish_backward_jvp(const float* h, int32_t ld_h, const float* hdot, int32_t ld_hdot,
+                           int64_t rows, int32_t n, const float* da, int32_t ld_da, int64_t dir_stride,
+                           float* dh, int32_t ld_dh, void* stream) {
+  return gcb_swish_backward_jvp_dirs(h, ld_h, hdot, ld_hdot, rows, n, da, ld_da, dir_stride, dh, ld_dh,
+                                     1, stream);
+}
+
+int gcb_layernorm_backward_jvp_dirs(const float* dy, int32_t ld_dy, const float* z, int32_t ld_z,
+                                    const float* zdot, int32_t ld_zdot, const float* scale,
+                                    int64_t rows, int32_t n, int64_t dir_stride, float* dz,
+                                    int32_t ld_dz, int32_t tangents, void* stream) {
+  GCB_CHECK_ARG(dy && z && zdot && scale && dz, "null pointer");
+  GCB_CHECK_ARG(n == 512, "the LayerNorm backward tangent needs n = 512");
+  GCB_CHECK_ARG(rows >= 0 && ld_dy >= n && ld_z >= n && ld_zdot >= n && ld_dz >= n,
+                "rows < 0 or leading dimension < n");
+  GCB_CHECK_ARG(dir_stride >= rows, "dir_stride < rows");
+  GCB_CHECK_ARG(tangents >= 1, "tangents < 1");
+  if (rows == 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * static_cast<double>(rows) * n * (3.0 + 3.0 * tangents));
+  gcb::layernorm_backward_jvp_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, st>>>(
+      dy, ld_dy, z, ld_z, zdot, ld_zdot, scale, rows, dir_stride, tangents, dz, ld_dz);
   GCB_CUDA(cudaGetLastError());
   return GCB_OK;
 }
@@ -1208,18 +1238,8 @@ int gcb_swish_backward_jvp(const float* h, int32_t ld_h, const float* hdot, int3
 int gcb_layernorm_backward_jvp(const float* dy, int32_t ld_dy, const float* z, int32_t ld_z,
                                const float* zdot, int32_t ld_zdot, const float* scale, int64_t rows,
                                int32_t n, int64_t dir_stride, float* dz, int32_t ld_dz, void* stream) {
-  GCB_CHECK_ARG(dy && z && zdot && scale && dz, "null pointer");
-  GCB_CHECK_ARG(n == 512, "the LayerNorm backward tangent needs n = 512");
-  GCB_CHECK_ARG(rows >= 0 && ld_dy >= n && ld_z >= n && ld_zdot >= n && ld_dz >= n,
-                "rows < 0 or leading dimension < n");
-  GCB_CHECK_ARG(dir_stride >= rows, "dir_stride < rows");
-  if (rows == 0) return GCB_OK;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0, 4.0 * static_cast<double>(rows) * n * 6.0);
-  gcb::layernorm_backward_jvp_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, st>>>(
-      dy, ld_dy, z, ld_z, zdot, ld_zdot, scale, rows, dir_stride, dz, ld_dz);
-  GCB_CUDA(cudaGetLastError());
-  return GCB_OK;
+  return gcb_layernorm_backward_jvp_dirs(dy, ld_dy, z, ld_z, zdot, ld_zdot, scale, rows, n, dir_stride,
+                                         dz, ld_dz, 1, stream);
 }
 
 int gcb_segment_sum_sorted(const float* msg, int32_t ld_msg, const int32_t* order,

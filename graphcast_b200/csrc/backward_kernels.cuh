@@ -505,56 +505,68 @@ layernorm_backward_dirs_kernel(const float* __restrict__ dy, int ld_dy, const fl
   }
 }
 
-// ---- Hessian-vector products (loss_and_input_hvp) ---------------------------------------------------
-// The backward pass of the gradient (direction 0) coupled with its tangent (direction 1), stacked as
-// above with two directions, at the primal h / z and their tangents hdot / zdot (one table each).
-// Direction 0 is bit for bit what swish_jvp_kernel / layernorm_backward_dirs_kernel give it alone;
-// direction 1 is its derivative along the tangent, in fp32.
+// ---- Hessian-vector products (loss_and_input_hvp, batched_loss_and_input_hvp) ---------------------
+// The backward pass of the gradient (direction 0) coupled with its tangents along K primal tangents
+// (directions 1..K), stacked as above with 1 + K directions, at the primal h / z and their tangents
+// hdot / zdot (stacked tables of K directions at the same stride).  Direction 0 is bit for bit what
+// swish_jvp_kernel / layernorm_backward_dirs_kernel give it alone; direction j is its derivative along
+// tangent j - 1, in fp32, with the same roundings whatever K is (pinned below to the sequence the
+// one-tangent kernel compiled to), so direction j is bit for bit the K = 1 launch on (0, j, j - 1).
+// The primal terms (s', s'', the row statistics, z-hat, g) are formed once per element / row.
 
-// dh = s'(h) da, dhdot = s'(h) dadot + s''(h) hdot da, with s'(h) = sg (1 + h (1 - sg)) rounded as
-// swish_jvp_kernel compiles it and s''(h) = sg (1 - sg) (2 + h (1 - 2 sg)).  One thread per 4 columns of
-// a row; dh may alias da (each thread reads both directions of da before it writes dh).
+// dh = s'(h) da, dhdot_j = s'(h) dadot_j + s''(h) hdot_j da, with s'(h) = sg (1 + h (1 - sg)) rounded
+// as swish_jvp_kernel compiles it and s''(h) = sg (1 - sg) (2 + h (1 - 2 sg)).  One thread per 4 columns
+// of a row; dh may alias da (each thread reads direction j of da before it writes direction j of dh,
+// and no other thread touches those columns).
 __global__ void __launch_bounds__(256)
 swish_backward_jvp_kernel(const float* __restrict__ h, int ld_h, const float* __restrict__ hdot,
                           int ld_hdot, long long rows, int n4, const float* da, int ld_da,
-                          long long stride, float* dh, int ld_dh) {
+                          long long stride, int tangents, float* dh, int ld_dh) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= rows * n4) return;
   const long long r = i / n4;
   const int c = static_cast<int>(i - r * n4) * 4;
   const float4 hv = *reinterpret_cast<const float4*>(h + r * ld_h + c);
-  const float4 tv = *reinterpret_cast<const float4*>(hdot + r * ld_hdot + c);
   const float4 a0 = *reinterpret_cast<const float4*>(da + r * ld_da + c);
-  const float4 a1 = *reinterpret_cast<const float4*>(da + (stride + r) * ld_da + c);
-  const float hq[4] = {hv.x, hv.y, hv.z, hv.w}, tq[4] = {tv.x, tv.y, tv.z, tv.w};
-  const float d0[4] = {a0.x, a0.y, a0.z, a0.w}, d1[4] = {a1.x, a1.y, a1.z, a1.w};
-  float o0[4], o1[4];
+  const float hq[4] = {hv.x, hv.y, hv.z, hv.w}, d0[4] = {a0.x, a0.y, a0.z, a0.w};
+  float f[4], f2[4], o0[4];
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     const float sg = 1.0f / (1.0f + expf(-hq[q]));
     const float om = __fsub_rn(1.0f, sg);
-    const float f = __fmul_rn(sg, __fmaf_rn(hq[q], om, 1.0f));
-    const float f2 = sg * om * (2.0f + hq[q] * (1.0f - 2.0f * sg));
-    o0[q] = __fmul_rn(d0[q], f);
-    o1[q] = d1[q] * f + f2 * tq[q] * d0[q];
+    f[q] = __fmul_rn(sg, __fmaf_rn(hq[q], om, 1.0f));
+    f2[q] = __fmul_rn(__fmul_rn(sg, om),
+                      __fmaf_rn(hq[q], __fsub_rn(1.0f, __fadd_rn(sg, sg)), 2.0f));
+    o0[q] = __fmul_rn(d0[q], f[q]);
   }
   *reinterpret_cast<float4*>(dh + r * ld_dh + c) = make_float4(o0[0], o0[1], o0[2], o0[3]);
-  *reinterpret_cast<float4*>(dh + (stride + r) * ld_dh + c) = make_float4(o1[0], o1[1], o1[2], o1[3]);
+  for (int t = 0; t < tangents; ++t) {
+    const long long rt = static_cast<long long>(t) * stride + r;
+    const float4 tv = *reinterpret_cast<const float4*>(hdot + rt * ld_hdot + c);
+    const float4 a1 = *reinterpret_cast<const float4*>(da + (stride + rt) * ld_da + c);
+    const float tq[4] = {tv.x, tv.y, tv.z, tv.w}, d1[4] = {a1.x, a1.y, a1.z, a1.w};
+    float o1[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q)            // s'(h) dadot + (s''(h) hdot) da
+      o1[q] = __fmaf_rn(d1[q], f[q], __fmul_rn(__fmul_rn(f2[q], tq[q]), d0[q]));
+    *reinterpret_cast<float4*>(dh + (stride + rt) * ld_dh + c) = make_float4(o1[0], o1[1], o1[2], o1[3]);
+  }
 }
 
-// The LayerNorm backward of layernorm_backward_dirs_kernel for [dy; dydot] (direction 0: its dz, with
-// its pinned roundings) and the tangent of that dz along zdot (direction 1).  With r = rstd, zhat =
-// (z - mu) r, g = dy*scale, m = mean(g*zhat):
+// The LayerNorm backward of layernorm_backward_dirs_kernel for [dy; dydot_1..K] (direction 0: its dz,
+// with its pinned roundings) and the tangents of that dz along zdot_1..K (directions 1..K).  With r =
+// rstd, zhat = (z - mu) r, g = dy*scale, m = mean(g*zhat), per tangent:
 //   rdot    = -r^2 mean(zhat*zdot)
 //   zhatdot = r (zdot - mean(zdot) - zhat mean(zhat*zdot))
 //   gdot    = dydot*scale,  mdot = mean(gdot*zhat + g*zhatdot)
 //   dzdot   = rdot (g - mean(g) - zhat m) + r (gdot - mean(gdot) - zhatdot m - zhat mdot)
-// One warp per row of n = 512 (lane owns columns lane + 32 j), 8 rows per block; z's row is read once.
+// One warp per row of n = 512 (lane owns columns lane + 32 j), 8 rows per block; z's row is read once,
+// the statistics, zhat, g and (g - mean(g) - zhat m) are formed once for every tangent.
 __global__ void __launch_bounds__(256)
 layernorm_backward_jvp_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z,
                               int ld_z, const float* __restrict__ zdot, int ld_zdot,
                               const float* __restrict__ scale, long long rows, long long stride,
-                              float* __restrict__ dz, int ld_dz) {
+                              int tangents, float* __restrict__ dz, int ld_dz) {
   constexpr int kCols = 16;
   constexpr float kInvN = 1.0f / (kCols * 32);
   const int lane = threadIdx.x & 31;
@@ -583,7 +595,7 @@ layernorm_backward_jvp_kernel(const float* __restrict__ dy, int ld_dy, const flo
   const float rstd = rsqrtf(__fmaf_rn(var, kInvN, 1e-5f));
 #pragma unroll
   for (int j = 0; j < kCols; ++j) v[j] = __fmul_rn(v[j], rstd);     // z-hat
-  float g[kCols];
+  float g[kCols], a[kCols];
   float mg = 0.f, mgz = 0.f;
 #pragma unroll
   for (int j = 0; j < kCols; ++j) {
@@ -598,46 +610,51 @@ layernorm_backward_jvp_kernel(const float* __restrict__ dy, int ld_dy, const flo
   }
   const float mgz_n = __fmul_rn(mgz, kInvN);
 #pragma unroll
-  for (int j = 0; j < kCols; ++j)
-    dz[r * ld_dz + lane + 32 * j] = __fmul_rn(rstd, __fmaf_rn(v[j], -mgz_n, __fmaf_rn(mg, -kInvN, g[j])));
-  // direction 1: the tangent
-  float zd[kCols];
-  float mzd = 0.f, mvz = 0.f;
-#pragma unroll
   for (int j = 0; j < kCols; ++j) {
-    zd[j] = zdot[r * ld_zdot + lane + 32 * j];
-    mzd += zd[j];
-    mvz += v[j] * zd[j];
+    a[j] = __fmaf_rn(v[j], -mgz_n, __fmaf_rn(mg, -kInvN, g[j]));     // g - mean(g) - zhat m
+    dz[r * ld_dz + lane + 32 * j] = __fmul_rn(rstd, a[j]);
   }
+  const float rr = __fmul_rn(rstd, rstd);
+  // directions 1..K: the tangents.  mean(x) = sum(x) / 512 is folded into an fma with -1/512 where the
+  // mean is subtracted (exact: a power of two).
+  for (int t = 0; t < tangents; ++t) {
+    const long long rt = static_cast<long long>(t) * stride + r;
+    float zd[kCols];
+    float mzd = 0.f, mvz = 0.f;
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    mzd += __shfl_xor_sync(0xffffffffu, mzd, o);
-    mvz += __shfl_xor_sync(0xffffffffu, mvz, o);
+    for (int j = 0; j < kCols; ++j) {
+      zd[j] = zdot[rt * ld_zdot + lane + 32 * j];
+      mzd = __fadd_rn(mzd, zd[j]);
+      mvz = __fmaf_rn(v[j], zd[j], mvz);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      mzd = __fadd_rn(mzd, __shfl_xor_sync(0xffffffffu, mzd, o));
+      mvz = __fadd_rn(mvz, __shfl_xor_sync(0xffffffffu, mvz, o));
+    }
+    mvz = __fmul_rn(mvz, kInvN);
+    const float nrdot = __fmul_rn(mvz, rr);                          // -rdot
+    float gd[kCols];
+    float mgd = 0.f, mdot = 0.f;
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) {
+      zd[j] = __fmul_rn(rstd, __fmaf_rn(v[j], -mvz, __fmaf_rn(mzd, -kInvN, zd[j])));   // zhat-dot
+      gd[j] = __fmul_rn(dy[(stride + rt) * ld_dy + lane + 32 * j], sc[j]);
+      mgd = __fadd_rn(mgd, gd[j]);
+      mdot = __fadd_rn(mdot, __fmaf_rn(v[j], gd[j], __fmul_rn(g[j], zd[j])));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      mgd = __fadd_rn(mgd, __shfl_xor_sync(0xffffffffu, mgd, o));
+      mdot = __fadd_rn(mdot, __shfl_xor_sync(0xffffffffu, mdot, o));
+    }
+    mdot = __fmul_rn(mdot, kInvN);
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) {
+      const float b = __fmaf_rn(v[j], -mdot, __fmaf_rn(-mgz_n, zd[j], __fmaf_rn(mgd, -kInvN, gd[j])));
+      dz[(stride + rt) * ld_dz + lane + 32 * j] = __fmaf_rn(rstd, b, -__fmul_rn(nrdot, a[j]));
+    }
   }
-  mzd *= kInvN;
-  mvz *= kInvN;
-  const float rdot = -rstd * rstd * mvz;
-  float gd[kCols];
-  float mgd = 0.f, mdot = 0.f;
-#pragma unroll
-  for (int j = 0; j < kCols; ++j) {
-    zd[j] = rstd * (zd[j] - mzd - v[j] * mvz);         // zhat-dot
-    gd[j] = dy[(stride + r) * ld_dy + lane + 32 * j] * sc[j];
-    mgd += gd[j];
-    mdot += gd[j] * v[j] + g[j] * zd[j];
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    mgd += __shfl_xor_sync(0xffffffffu, mgd, o);
-    mdot += __shfl_xor_sync(0xffffffffu, mdot, o);
-  }
-  mgd *= kInvN;
-  mdot *= kInvN;
-  const float mg_n = mg * kInvN;
-#pragma unroll
-  for (int j = 0; j < kCols; ++j)
-    dz[(stride + r) * ld_dz + lane + 32 * j] =
-        rdot * (g[j] - mg_n - v[j] * mgz_n) + rstd * (gd[j] - mgd - zd[j] * mgz_n - v[j] * mdot);
 }
 
 // ---- index operations ----------------------------------------------------------------------------

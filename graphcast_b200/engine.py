@@ -829,54 +829,65 @@ class Engine:
                         zero_targets: Optional[torch.Tensor] = None) -> None:
     """One step of one batch element of a Hessian-vector product of the loss (call input_grads_begin()
     first).  operands: "targets_planes", "tangent_planes" [c_in, Ng] (the tangent v of this step's
-    input planes, physical units) and the affine keywords of output_loss.  fb.a is None or
-    [2, fb.n_rows, Ng] of the following step: direction 0 its gradient, direction 1 that gradient's
-    derivative along v; afterwards it is this step's.  channel_sums and planes_out as in
-    input_grads_element; zero_targets: a zero [n_out, Ng] float32 plane for the seed's tangent, shared
+    input planes, physical units) or [K, c_in, Ng] (K tangents v_1..v_K, each direction's planes
+    contiguous; batched_loss_and_input_hvp) and the affine keywords of output_loss.  fb.a is None or
+    [1 + K, fb.n_rows, Ng] of the following step: direction 0 its gradient, direction j that gradient's
+    derivative along v_j; afterwards it is this step's.  channel_sums and planes_out as in
+    input_grads_element; zero_targets: a zero [n_out, Ng] float32 plane for the seed's tangents, shared
     by the elements of a call (None: one is allocated here).
 
-    The step runs stage by stage with its tangent (Backward.tangent), keeping the primal and tangent
+    The step runs stage by stage with its K tangents (Backward.tangent(dirs=K)), each packed into its
+    slice of one stacked image as input_jvp_element packs them, keeping the primal and tangent
     snapshots.  Direction 0 of the seed is input_grads_element's loss seed.  The seed is affine in
-    (y, the add planes, fb.a), so direction 1 is the same kernel on their tangents with zero targets:
-    y-dot, add_planes = v (so that t_norm = -v[add] / scale), no offset and fb.a's direction 1.  Both
-    directions then share one backward walk (Backward.element(dirs=2, hvp=...)), and gcb_input_grad runs
-    per direction.  Direction 0 is bit for bit what input_grads_element gives."""
+    (y, the add planes, fb.a), so direction j is the same kernel on their tangents along v_j with zero
+    targets: y-dot_j, add_planes = v_j (so that t_norm = -v_j[add] / scale), no offset and fb.a's
+    direction j.  All 1 + K directions then share one backward walk (Backward.element(dirs=1 + K,
+    hvp=...)), and gcb_input_grad runs per direction.  Direction 0 is bit for bit what
+    input_grads_element gives, and direction j what the [c_in, Ng] call gives along v_j alone."""
     if self._backward is None:
       raise RuntimeError("call input_grads_begin() first")
     affine = {k: operands[k] for k in ("scale", "offset", "add_planes", "add_plane_index")
               if k in operands}
     targets_planes, tangent = operands["targets_planes"], operands["tangent_planes"]
     operands.clear()
-    if (tuple(tangent.shape) != (self.c_in, self.num_grid) or tangent.dtype != torch.float32
-        or not tangent.is_contiguous()):
-      raise ValueError(f"tangent_planes must be a contiguous float32 [{self.c_in}, {self.num_grid}] tensor")
+    single = tangent.dim() == 2
+    nt = 1 if single else tangent.shape[0]
+    lead = () if single else (nt,)
+    if (tuple(tangent.shape) != lead + (self.c_in, self.num_grid) or tangent.dtype != torch.float32
+        or tangent.stride()[-2:] != (self.num_grid, 1) or nt < 1):
+      raise ValueError(f"tangent_planes must be a float32 {list(lead + (self.c_in, self.num_grid))} "
+                       f"tensor with contiguous [{self.c_in}, {self.num_grid}] planes per direction")
+    planes = [tangent] if single else list(tangent.unbind(0))
     grid_in = self.grid_in_img if grid_in is None else grid_in
     stride = self._backward.dir_stride(self.num_grid)
     no_static = torch.zeros([self.num_grid, 3], dtype=torch.float32, device=self.device)
-    dgrid_in = self._image(self.num_grid, self.c_in_pad)
+    dgrid_in = self._image((nt - 1) * stride + self.num_grid, self.c_in_pad)
+    img_stride = self._lib.gcb_a_image_bytes(stride, self.c_in_pad)
     n_lat = lat_weight.shape[0]
     add_index = affine.get("add_plane_index")
     with self._on_device():
-      _native.check(self._lib.gcb_pack_grid_image(
-          tangent.data_ptr(), self.c_in, self.num_grid, None, self._ptr(fb.in_scale),
-          no_static.data_ptr(), 3, self.c_in_pad, dgrid_in.data_ptr(), self._stream()),
-          "gcb_pack_grid_image")
+      for k, p in enumerate(planes):
+        _native.check(self._lib.gcb_pack_grid_image(
+            p.data_ptr(), self.c_in, self.num_grid, None, self._ptr(fb.in_scale),
+            no_static.data_ptr(), 3, self.c_in_pad, dgrid_in.data_ptr() + k * img_stride,
+            self._stream()), "gcb_pack_grid_image")
       del no_static
       snaps, tsnaps = {}, {}
-      dy = self._backward.tangent(grid_in, dgrid_in, 1, snaps=snaps, tsnaps=tsnaps)
+      dy = self._backward.tangent(grid_in, dgrid_in, nt, snaps=snaps, tsnaps=tsnaps)
       del dgrid_in
       if planes_out is not None:
         self.unpack_outputs(planes_out, **affine)
       if channel_sums is not None:
         self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
-      g_out = torch.zeros([stride + self.num_grid, 256], dtype=torch.float32, device=self.device)
-      a_out = torch.empty([2, fb.n_rows, self.num_grid], dtype=torch.float32, device=self.device)
-      a_next = [None, None] if fb.a is None else list(fb.a.unbind(0))
+      g_out = torch.zeros([nt * stride + self.num_grid, 256], dtype=torch.float32, device=self.device)
+      a_out = torch.empty([1 + nt, fb.n_rows, self.num_grid], dtype=torch.float32, device=self.device)
+      a_next = [None] * (1 + nt) if fb.a is None else list(fb.a.unbind(0))
       if zero_targets is None:
         zero_targets = torch.zeros([self.n_out, self.num_grid], dtype=torch.float32,
                                    device=self.device)
-      seeds = ((self.grid_out, affine.get("offset"), affine.get("add_planes"), targets_planes),
-               (dy, None, None if add_index is None else tangent, zero_targets))
+      seeds = [(self.grid_out, affine.get("offset"), affine.get("add_planes"), targets_planes)]
+      seeds += [(dy[k * stride:], None, None if add_index is None else p, zero_targets)
+                for k, p in enumerate(planes)]
       for k, (y, offset, add, targets) in enumerate(seeds):
         _native.check(self._lib.gcb_output_loss_grad_feedback(
             y.data_ptr(), y.shape[1], self.n_out, n_lat, self.num_grid // n_lat,
@@ -885,14 +896,14 @@ class Engine:
             fb.dpred_row.data_ptr(), fb.n_rows, fb.resid_channel.data_ptr(), fb.carry_row.data_ptr(),
             a_out[k].data_ptr(), g_out[k * stride:].data_ptr(), 256, self._stream()),
             "gcb_output_loss_grad_feedback")
-      # the following step's rows, the planes, targets and tangent are consumed: release them
+      # the following step's rows, the planes, targets and tangents are consumed: release them
       fb.a = a_out
-      del seeds, y, offset, add, targets, a_next, zero_targets, dy
+      del seeds, y, offset, add, targets, a_next, zero_targets, dy, planes, p
       affine = targets_planes = tangent = None
-      dx = self._backward.element(grid_in, g_out, snaps, dgrid_in=True, param_grads=False, dirs=2,
-                                  hvp=tsnaps)
+      dx = self._backward.element(grid_in, g_out, snaps, dgrid_in=True, param_grads=False,
+                                  dirs=1 + nt, hvp=tsnaps)
       del g_out, snaps, tsnaps
-      for k in range(2):
+      for k in range(1 + nt):
         _native.check(self._lib.gcb_input_grad(
             dx[k * stride:].data_ptr(), dx.shape[1], self.num_grid, fb.n_rows, fb.rows.data_ptr(),
             self._ptr(fb.in_scale), a_out[k].data_ptr(), 1, self._stream()), "gcb_input_grad")

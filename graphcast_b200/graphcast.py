@@ -126,6 +126,14 @@ class Predictor(abc.ABC):
     the tangents (Datasets as input_jvp takes them), shaped like `inputs` and `forcings`."""
     raise NotImplementedError(f"{type(self).__name__} does not implement Hessian-vector products")
 
+  def batched_loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
+                                 *, directions_per_pass=None, **optional_kwargs):
+    """Returns (loss, diagnostics, input_grads, forcing_grads, input_hvp, forcing_hvp):
+    loss_and_input_hvp along K tangent directions at once, the tangent Datasets' variables carrying a
+    leading "direction" dim of size K; input_hvp and forcing_hvp have the same leading dim, the loss and
+    gradients none.  directions_per_pass: directions that share one forward (None: all)."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement Hessian-vector products")
+
   def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
                 **optional_kwargs):
     """Returns (predictions, prediction_tangents): the predictions of __call__ and their derivative
@@ -364,6 +372,40 @@ class GraphCast(Predictor):
     return self._loss_and_input_grads(inputs, targets, forcings, norm=None,
                                       tangents=(input_tangents, forcing_tangents))
 
+  def batched_loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
+                                 *, directions_per_pass=None, **unused_kwargs):
+    """(loss, diagnostics, input_grads, forcing_grads, input_hvp, forcing_hvp) of loss_and_input_hvp
+    along K tangent directions at once, for one target time: what jax.vmap over the tangents of
+    jax.jvp(jax.grad(loss), (x,), (v,)) gives.
+
+    Every variable of input_tangents / forcing_tangents has a leading "direction" dim of size K >= 1,
+    followed by its namesake's dims and shape; a variable left out (every forcing for
+    forcing_tangents=None) is zero in every direction.  A missing direction dim, K differing between
+    variables or Datasets, an unknown variable or a wrong shape and a bad directions_per_pass raise
+    ValueError before anything runs, and every refusal of loss_and_input_hvp applies.  `loss`,
+    `diagnostics`, `input_grads` and `forcing_grads` are bit for bit what loss_and_input_grads returns
+    (no direction dim); input_hvp and forcing_hvp (float32) are shaped like `inputs` and `forcings` with
+    a leading "direction" dim, its coordinate input_tangents' "direction" coordinate when it has one,
+    else 0..K-1.  Direction k is bit for bit loss_and_input_hvp along tangent k alone, for any K and
+    directions_per_pass.
+
+    The directions share one stage-wise forward with their K tangents and one backward walk of 1 + K
+    directions, the gradient and its K tangents (Backward.element(dirs=1 + K, hvp=...)): every GEMM
+    streams its weights once for all of them, and every MLP's h and z recomputes, the embedder
+    recomputes and the edge projections are formed once; the two coupled nonlinearities form their
+    primal terms once per element.  directions_per_pass = g (None: K) runs ceil(K / g) such passes,
+    each what a g-direction call runs, for memory: the kept tangent tables and the stacked gradient
+    state grow with the directions of a pass.  The loss, diagnostics and gradients are the first
+    pass's (every pass forms the same bits).  Measured on an 80 GB H100 at 1 degree / 13 levels
+    (DESIGN.md section 8): a pass peaks at 15.4 GiB for one direction and 56.0 GiB for 8, about 5.8 GiB
+    per further direction (3.5 GiB of it the kept tangent tables), so about 11 directions fit per pass
+    (16 do not); 8 directions take 1.87x (T = 1) and 2.02x (T = 4) less time than 8 loss_and_input_hvp
+    calls.  0.25 degree / 37 levels is not measured: one direction is not expected to fit there."""
+    one_pass = lambda it, ft: self._loss_and_input_grads(inputs, targets, forcings, norm=None,
+                                                         tangents=(it, ft), directions=True)
+    return batched_hvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
+                       directions_per_pass)
+
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **unused_kwargs):
     """(predictions, input_grads, forcing_grads) for one target time: `predictions` is what __call__
     returns, bit for bit; the gradients (as in loss_and_input_grads) are those of
@@ -481,15 +523,19 @@ class GraphCast(Predictor):
                                                 directions=run.labels)
 
   def _loss_and_input_grads(self, inputs, targets, forcings, norm: Optional[FusedNormalization],
-                            tangents=None):
+                            tangents=None, directions: bool = False):
     """loss_and_input_grads of one target time; with tangents = (input_tangents, forcing_tangents),
-    loss_and_input_hvp."""
+    loss_and_input_hvp; with `directions` too, batched_loss_and_input_hvp of one pass, the tangents
+    carrying a leading "direction" dim (hvp_direction_tangent_planes)."""
     inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
     forcings = xs.from_xarray(forcings)
     if targets.sizes.get("time", 1) != 1:
       raise NotImplementedError("input gradients of GraphCast cover one target time (several: "
                                 "autoregressive.Predictor with gradient_checkpointing=True)")
-    tangent = None if tangents is None else hvp_tangent_planes(inputs, forcings, *tangents)
+    tangent = None
+    if tangents is not None:
+      pack = hvp_direction_tangent_planes if directions else hvp_tangent_planes
+      tangent = pack(inputs, forcings, *tangents)
     batch = dict(inputs.sizes).get("batch", 1)
     slabs = model_utils.channel_layout(targets)
     num_grid = inputs.sizes["lat"] * inputs.sizes["lon"]
@@ -526,9 +572,10 @@ class GraphCast(Predictor):
     self._channel_sums as in `loss`; with `cotangents`, predictions["predictions"] receives the
     predictions, unpacked from that forward as __call__ unpacks its step's; with `directions`, the
     cotangents have a leading "direction" dim and every direction shares that forward and backward
-    pass; with `tangent_planes` ([batch, c_in, Ng] host planes of the input tangents, with `targets`)
-    every element runs Engine.input_hvp_element.  Returns the run, whose finish() gives (input_grads,
-    forcing_grads), with tangent_planes followed by (input_hvp, forcing_hvp)."""
+    pass; with `tangent_planes` ([batch, c_in, Ng] host planes of the input tangents, or [K, batch,
+    c_in, Ng] for K directions, with `targets`) every element runs Engine.input_hvp_element.  Returns
+    the run, whose finish() gives (input_grads, forcing_grads), with tangent_planes followed by
+    (input_hvp, forcing_hvp), these with a leading "direction" dim for K directions."""
     state = {}
 
     def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
@@ -541,13 +588,17 @@ class GraphCast(Predictor):
           dirs = state["cot"].shape[0]
         state["run"] = _InputGradRun(self, plan, norm, inputs, forcings, 1, state["batch"],
                                      release_staging=False, dirs=dirs,
-                                     hvp=tangent_planes is not None)
+                                     hvp=_hvp_directions(tangent_planes, 0))
         if cotangents is not None and not directions:
           state["cot"] = self._cotangent_planes(cotangents, template, state["run"].batch)
         if coef is not None:
           state["coef"] = torch.as_tensor(np.asarray(coef, np.float64)).to(eng.device)
       operands = dict(affine)
-      if tangent_planes is not None:
+      if tangent_planes is not None and tangent_planes.dim() == 4:    # [K, batch, c_in, Ng]
+        operands["tangent_planes"] = torch.empty(
+            [tangent_planes.shape[0], eng.c_in, eng.num_grid], dtype=torch.float32, device=eng.device)
+        operands["tangent_planes"].copy_(tangent_planes[:, b])
+      elif tangent_planes is not None:
         operands["tangent_planes"] = tangent_planes[b].to(eng.device)
       if targets is not None:
         operands["targets_planes"] = planes_tgt
@@ -613,12 +664,13 @@ class GraphCast(Predictor):
     backward pass.  The stash is only read, so several calls can differentiate the same forward.
     Returns (input_grads, forcing_grads) Datasets shaped like `inputs` and `forcings` (with a leading
     "direction" dim for `directions`).  With `tangents` (a StepStash of each step's input tangent planes
-    [batch, c_in, Ng], loss seed only) every step runs Engine.input_hvp_element, and (input_hvp,
-    forcing_hvp) follow the gradients."""
+    [batch, c_in, Ng], or [batch, K, c_in, Ng] for K directions; loss seed only) every step runs
+    Engine.input_hvp_element, and (input_hvp, forcing_hvp) follow the gradients, with a leading
+    "direction" dim for K directions."""
     run = _InputGradRun(self, plan, norm, inputs, forcings, len(stash.steps), stash.batch,
                         release_staging=True,
                         dirs=cotangents[0].shape[0] if directions else None,
-                        hvp=tangents is not None)
+                        hvp=None if tangents is None else _hvp_directions(tangents.steps[0][0][0], 1))
     eng = self._engine
     dev = eng.device
     coef_dev = None if coef is None else torch.as_tensor(np.asarray(coef, np.float64)).to(dev)
@@ -640,7 +692,7 @@ class GraphCast(Predictor):
         if tangents is not None:
           (host_tangent,), tangent_done = tangents.steps[t]
           compute.wait_event(tangent_done)
-          operands["tangent_planes"] = torch.empty([eng.c_in, eng.num_grid], dtype=torch.float32,
+          operands["tangent_planes"] = torch.empty(list(host_tangent[b].shape), dtype=torch.float32,
                                                    device=dev)
           operands["tangent_planes"].copy_(host_tangent[b], non_blocking=True)
         lead = [cotangents[t].shape[0]] if directions else []
@@ -748,7 +800,8 @@ class GraphCast(Predictor):
     loss_and_input_hvp over several target times): every batch element runs the stage-wise forward with
     its tangent (_TangentRun.element, which also feeds the next step's tangent planes), then
     output_loss on that forward, which is the step _device_loss runs.  Returns (finish, predictions,
-    channel_sums, this step's input tangent planes [batch, c_in, Ng] on the device)."""
+    channel_sums, this step's input tangent planes on the device: [batch, c_in, Ng] for a run of one
+    direction, [batch, K, c_in, Ng] for a run of K (`run.directions`))."""
     targets = xs.from_xarray(targets)
     state = {}
 
@@ -756,13 +809,14 @@ class GraphCast(Predictor):
       eng = self._engine
       if "planes" not in state:
         eng.input_grads_begin()
-        state["planes"] = torch.empty([run.batch, eng.c_in, eng.num_grid], dtype=torch.float32,
-                                      device=eng.device)
+        lead = [run.dirs] if run.directions else []
+        state["planes"] = torch.empty([run.batch] + lead + [eng.c_in, eng.num_grid],
+                                      dtype=torch.float32, device=eng.device)
         state["lat_weight"] = self._lat_weight(targets, eng.device)
       tangent_out = torch.empty([run.dirs, eng.n_out, eng.num_grid], dtype=torch.float32,
                                 device=eng.device)
       run.element(eng, b, tangent_out, None, norm, affine,
-                  keep=lambda p: state["planes"][b].copy_(p[0]))
+                  keep=lambda p: state["planes"][b].copy_(p if run.directions else p[0]))
       eng.output_loss(planes_tgt, state["lat_weight"], channel_sums=channel_sums,
                       planes_out=planes_out, **affine)
 
@@ -985,6 +1039,50 @@ def hvp_tangent_planes(inputs: xs.Dataset, forcings: xs.Dataset, input_tangents,
        feedback.tangent_planes(forcing_tangents, forcings, sizes)], axis=1))
 
 
+def hvp_direction_tangent_planes(inputs: xs.Dataset, forcings: xs.Dataset, input_tangents,
+                                 forcing_tangents) -> torch.Tensor:
+  """[K, batch, c_in, Ng] float32 host planes of the K tangents of a batched_loss_and_input_hvp, after
+  batched_input_jvp's checks (feedback.check_direction_tangents): direction k is what
+  hvp_tangent_planes packs for tangent k alone."""
+  it = None if input_tangents is None else xs.from_xarray(input_tangents)
+  ft = None if forcing_tangents is None else xs.from_xarray(forcing_tangents)
+  dirs, _ = feedback.check_direction_tangents(it, inputs, ft, forcings)
+  sizes = {"batch": dict(inputs.sizes).get("batch", 1), "lat": inputs.sizes["lat"],
+           "lon": inputs.sizes["lon"]}
+  return torch.from_numpy(np.concatenate(
+      [feedback.tangent_planes(it, inputs, sizes, dirs),
+       feedback.tangent_planes(ft, forcings, sizes, dirs)], axis=2))
+
+
+def _hvp_directions(planes: Optional[torch.Tensor], axis: int) -> Optional[Tuple[int, bool]]:
+  """(K, directions) of the tangent planes of a Hessian-vector product: the planes of one tangent have
+  no direction axis (K = 1, no "direction" dim in the results), those of K tangents one at `axis`
+  ([K, batch, c_in, Ng] host planes: 0; [batch, K, c_in, Ng] stashed planes: 1)."""
+  if planes is None:
+    return None
+  return (1, False) if planes.dim() == 3 else (int(planes.shape[axis]), True)
+
+
+def batched_hvp(one_pass, inputs, forcings, input_tangents, forcing_tangents, directions_per_pass):
+  """batched_loss_and_input_hvp of a predictor stack: checks the tangents
+  (feedback.check_direction_tangents) and directions_per_pass before anything runs, then runs
+  one_pass(input_tangents, forcing_tangents) -> (loss, diagnostics, input_grads, forcing_grads,
+  input_hvp, forcing_hvp) on consecutive slices of the directions (direction_passes) and joins the
+  Hessian-vector products along "direction".  The loss, diagnostics and gradients are the first
+  pass's."""
+  inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
+  it = None if input_tangents is None else xs.from_xarray(input_tangents)
+  ft = None if forcing_tangents is None else xs.from_xarray(forcing_tangents)
+  dirs, labels = feedback.check_direction_tangents(it, inputs, ft, forcings)
+  at = lambda ds, sl: None if ds is None else ds.isel({feedback.DIRECTION: sl})
+
+  def pass_of(sl):
+    out = one_pass(at(it, sl), at(ft, sl))
+    return (out[:4],) + tuple(out[4:])
+  first, input_hvp, forcing_hvp = direction_passes(pass_of, dirs, labels, directions_per_pass)
+  return first + (input_hvp, forcing_hvp)
+
+
 def batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents, directions_per_pass):
   """batched_input_jvp of a predictor stack: checks the tangents (feedback.check_direction_tangents)
   and directions_per_pass before anything runs, then runs one_pass(input_tangents, forcing_tangents)
@@ -1119,16 +1217,17 @@ class _InputGradRun:
   dirs = K (batched_input_vjp): K cotangents share every step, fb.a is [K, n_rows, Ng], and every
   result buffer has a leading axis of K directions, each reduced as one direction's would be.
 
-  hvp (loss_and_input_hvp): every step runs Engine.input_hvp_element, the two directions are the
-  gradient and its derivative along the tangent, and finish() gives (input_grads, forcing_grads,
-  input_hvp, forcing_hvp)."""
+  hvp = (K, directions) (loss_and_input_hvp: (1, False); batched_loss_and_input_hvp: (K, True)): every
+  step runs Engine.input_hvp_element, the 1 + K directions are the gradient and its derivatives along
+  the K tangents, and finish() gives (input_grads, forcing_grads) from direction 0 and (input_hvp,
+  forcing_hvp) from directions 1..K, these with a leading "direction" dim when `directions`."""
 
   def __init__(self, model: GraphCast, plan, norm: Optional[FusedNormalization], inputs: xs.Dataset,
                forcings: xs.Dataset, num_steps: int, batch: int, release_staging: bool,
-               dirs: Optional[int] = None, hvp: bool = False):
+               dirs: Optional[int] = None, hvp: Optional[Tuple[int, bool]] = None):
     eng = self.eng = model.engine
     self.hvp, self.zero_targets = hvp, None
-    dirs = 2 if hvp else dirs
+    dirs = 1 + hvp[0] if hvp else dirs
     self.dirs = dirs
     lead = [] if dirs is None else [dirs]
     eng.input_grads_begin()
@@ -1203,9 +1302,12 @@ class _InputGradRun:
     torch.cuda.current_stream(self.eng.device).synchronize()
     grads.update({key: t.numpy() for key, t in self.host.items()})
     if self.hvp:
-      return tuple(ds for k in range(2) for ds in feedback.grads_to_datasets(
-          self.var_rows, {key: g[k] for key, g in grads.items()}, self.inputs, self.forcings,
-          self.n_lat, self.n_lon))
+      nt, directions = self.hvp
+      at = lambda k: {key: g[k] for key, g in grads.items()}
+      return feedback.grads_to_datasets(self.var_rows, at(0), self.inputs, self.forcings, self.n_lat,
+                                        self.n_lon) + feedback.grads_to_datasets(
+          self.var_rows, at(slice(1, None)) if directions else at(1), self.inputs, self.forcings,
+          self.n_lat, self.n_lon, directions=nt if directions else None)
     return feedback.grads_to_datasets(self.var_rows, grads, self.inputs, self.forcings, self.n_lat,
                                       self.n_lon, directions=self.dirs)
 

@@ -271,6 +271,17 @@ class InputsAndResiduals(graphcast.Predictor):
     return self._predictor._loss_and_input_grads(inputs, targets, forcings, norm=consts,
                                                  tangents=(input_tangents, forcing_tangents))
 
+  def batched_loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
+                                 *, directions_per_pass=None, **kwargs):
+    """loss_and_input_hvp along K tangent directions at once (GraphCast.batched_loss_and_input_hvp),
+    with respect to the inputs and forcings in their physical units.  GraphCast only."""
+    def one_pass(it, ft):
+      ins, tgt, fs, consts = self._fused_for(inputs, targets, forcings, "input gradients")
+      return self._predictor._loss_and_input_grads(ins, tgt, fs, norm=consts, tangents=(it, ft),
+                                                   directions=True)
+    return graphcast.batched_hvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
+                                 directions_per_pass)
+
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
     """(predictions, input_grads, forcing_grads) of the un-normalised predictions of __call__
     (GraphCast.input_vjp).  GraphCast only."""

@@ -450,18 +450,30 @@ int gcb_layernorm_backward_dirs(const float* dy, int32_t ld_dy, const float* z, 
                                 const float* scale, int64_t rows, int32_t n, int64_t dir_stride,
                                 int32_t dirs, float* dz, int32_t ld_dz, void* stream);
 
-/* Hessian-vector products (GraphCast.loss_and_input_hvp): the backward pass of the gradient coupled
- * with its tangent, stacked as above with two directions, [d; ddot] (row r of direction 1 is row
- * dir_stride + r, dir_stride >= rows), at the primal rows and their tangent (one table each).
- * Direction 0 is bit for bit what the one-direction kernel gives; direction 1 is its derivative along
- * the primal tangent, in fp32.  Row-wise, deterministic.
+/* Hessian-vector products (GraphCast.loss_and_input_hvp, batched_loss_and_input_hvp): the backward
+ * pass of the gradient coupled with its tangents along K >= 1 primal tangents (`tangents`), stacked as
+ * above with 1 + K directions, [d; ddot_1; ...; ddot_K] (row r of direction k is row k * dir_stride + r,
+ * dir_stride >= rows), at the primal rows and their tangents, a stacked table of K directions at the
+ * same dir_stride (tangent j - 1 for direction j).  Direction 0 is bit for bit what the one-direction
+ * kernel gives; direction j is its derivative along tangent j - 1, in fp32, bit for bit what the
+ * K = 1 call gives on (direction 0, direction j, tangent j - 1).  The primal terms are formed once for
+ * all K.  Row-wise, deterministic; the pad rows between directions are not written.
  *
- * gcb_swish_backward_jvp: dh = swish'(h) da (bit for bit gcb_swish_jvp) and
- *   dhdot = swish'(h) dadot + swish''(h) hdot da,  swish''(h) = sg (1 - sg) (2 + h (1 - 2 sg)).
+ * gcb_swish_backward_jvp_dirs: dh = swish'(h) da (bit for bit gcb_swish_jvp) and
+ *   dhdot_j = swish'(h) dadot_j + swish''(h) hdot_j da,  swish''(h) = sg (1 - sg) (2 + h (1 - 2 sg)).
  *   n a multiple of 4, 16-byte rows; dh may alias da.
- * gcb_layernorm_backward_jvp: dz = gcb_layernorm_backward_dirs(dy) (bit for bit) and its tangent along
- *   zdot, the tangent of the pre-LayerNorm z (formulas in backward_kernels.cuh).  n = 512; dz may not
- *   alias dy, z or zdot; z's row is read once. */
+ * gcb_layernorm_backward_jvp_dirs: dz = gcb_layernorm_backward_dirs(dy) (bit for bit) and its tangents
+ *   along zdot_j, the tangents of the pre-LayerNorm z (formulas in backward_kernels.cuh).  n = 512; dz
+ *   may not alias dy, z or zdot; z's row is read once.
+ * gcb_swish_backward_jvp / gcb_layernorm_backward_jvp: the K = 1 calls (two directions, one tangent). */
+int gcb_swish_backward_jvp_dirs(const float* h, int32_t ld_h, const float* hdot, int32_t ld_hdot,
+                                int64_t rows, int32_t n, const float* da, int32_t ld_da,
+                                int64_t dir_stride, float* dh, int32_t ld_dh, int32_t tangents,
+                                void* stream);
+int gcb_layernorm_backward_jvp_dirs(const float* dy, int32_t ld_dy, const float* z, int32_t ld_z,
+                                    const float* zdot, int32_t ld_zdot, const float* scale,
+                                    int64_t rows, int32_t n, int64_t dir_stride, float* dz,
+                                    int32_t ld_dz, int32_t tangents, void* stream);
 int gcb_swish_backward_jvp(const float* h, int32_t ld_h, const float* hdot, int32_t ld_hdot,
                            int64_t rows, int32_t n, const float* da, int32_t ld_da, int64_t dir_stride,
                            float* dh, int32_t ld_dh, void* stream);
@@ -718,8 +730,8 @@ typedef enum {
                              * gcb_output_loss_grad_feedback, gcb_input_grad,
                              * gcb_output_cotangent_grad_feedback, gcb_broadcast_grad_sum,
                              * gcb_layernorm_jvp, gcb_swish_jvp, gcb_layernorm_jvp_dirs,
-                             * gcb_layernorm_backward_dirs, gcb_swish_backward_jvp,
-                             * gcb_layernorm_backward_jvp */
+                             * gcb_layernorm_backward_dirs, gcb_swish_backward_jvp(_dirs),
+                             * gcb_layernorm_backward_jvp(_dirs) */
   GCB_KIND_NOISE = 11       /* gcb_add_gaussian_noise */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
