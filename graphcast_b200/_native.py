@@ -93,6 +93,8 @@ class Model(C.Structure):
       ("chain_scratch", _fp),
       ("image_residual", C.c_int32), ("deep_chains", C.c_int32), ("proj_grid_b", _fp),
       ("chain_scratch_bytes", C.c_int64),
+      ("static_acc_g2m", _fp), ("static_acc_m2g", _fp), ("static_acc_mesh", _fp),
+      ("static_e0_img", _fp),
   ]
 
 
@@ -109,7 +111,8 @@ class ChainLayer(C.Structure):
               ("out", _fp), ("ld_out", C.c_int32),
               ("out_y", _fp), ("ld_out_y", C.c_int32),
               ("out_img", _fp),
-              ("n_pre_add", C.c_int32), ("pre_add", PreAdd * 2)]
+              ("n_pre_add", C.c_int32), ("pre_add", PreAdd * 2),
+              ("acc_table", _fp), ("ld_acc", C.c_int32), ("acc_out", C.c_int32)]
 
 
 class ChainDesc(C.Structure):
@@ -199,6 +202,7 @@ EXPORTS = {
     "gcb_forward":(C.c_int, [C.POINTER(Model), _fp, _fp, _fp, C.POINTER(C.c_int32)]),
     "gcb_forward_stage": (C.c_int, [C.POINTER(Model), C.c_int32, C.c_int32, _fp, _fp, _fp,
                                     C.POINTER(C.c_int32)]),
+    "gcb_forward_static": (C.c_int, [C.POINTER(Model), _fp, C.POINTER(C.c_int32)]),
     "gcb_chain_scratch_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "gcb_chain_forward": (C.c_int, [C.POINTER(ChainDesc), _fp]),
     "gcb_set_cluster_size": (C.c_int, [C.c_int32]),

@@ -265,6 +265,7 @@ struct ChainShape {
   int maxdist = 1;     // largest (consumer layer - producer layer)
   int nslots = 2;
   bool pre = false;
+  bool tab = false;    // some layer has acc_table or acc_out
   int vecs = 0;        // bias / LayerNorm parameter vectors
 };
 
@@ -278,7 +279,20 @@ int validate_chain(const gcb_chain_desc* d, ChainShape* shape) {
   ChainShape sh;
   for (int l = 0; l < d->nlayers; ++l) {
     const gcb_chain_layer& g = d->layer[l];
-    GCB_CHECK_ARG(g.nseg >= 1 && g.nseg <= 3, "nseg must be 1..3");
+    if (g.acc_table != nullptr) {
+      GCB_CHECK_ARG(g.nseg == 0 && g.w_packed == nullptr,
+                    "an acc_table layer has no segments and no weights (nseg = 0, w_packed = NULL)");
+      GCB_CHECK_ARG(g.ln_scale == nullptr && g.ln_offset == nullptr, "an acc_table layer cannot have LayerNorm");
+      GCB_CHECK_ARG(aligned16(g.acc_table) && g.ld_acc % 4 == 0 && g.ld_acc >= 512, "acc_table unaligned");
+    } else {
+      GCB_CHECK_ARG(g.nseg >= 1 && g.nseg <= 3, "nseg must be 1..3");
+    }
+    if (g.acc_table != nullptr || g.acc_out) sh.tab = true;
+    if (g.acc_out)
+      GCB_CHECK_ARG(g.acc_out == 1 && g.out && !g.bias && !g.ln_scale && g.act == GCB_ACT_NONE &&
+                        g.n_pre_add == 0 && !g.keep && !g.out_y && !g.out_img && !g.acc_table,
+                    "acc_out needs out and excludes bias, LayerNorm, swish, pre_add, keep, out_y, "
+                    "out_img and acc_table");
     for (int s = 0; s < g.nseg; ++s) {
       const int from = g.seg_from[s];
       if (from >= 0) {
@@ -288,7 +302,8 @@ int validate_chain(const gcb_chain_desc* d, ChainShape* shape) {
       }
       if (int rc = validate_segment(g.seg[s])) return rc;
     }
-    GCB_CHECK_ARG(g.w_packed != nullptr && aligned16(g.w_packed), "w_packed null/unaligned");
+    if (g.acc_table == nullptr)
+      GCB_CHECK_ARG(g.w_packed != nullptr && aligned16(g.w_packed), "w_packed null/unaligned");
     GCB_CHECK_ARG((g.ln_scale == nullptr) == (g.ln_offset == nullptr), "ln_scale/ln_offset mismatch");
     GCB_CHECK_ARG(g.act == GCB_ACT_NONE || g.act == GCB_ACT_SWISH, "unknown activation");
     GCB_CHECK_ARG(!(g.act == GCB_ACT_SWISH && g.ln_scale != nullptr),
@@ -350,15 +365,15 @@ int validate_chain(const gcb_chain_desc* d, ChainShape* shape) {
   return GCB_OK;
 }
 
-template <bool kSplit, bool kPre>
+template <bool kSplit, bool kPre, bool kTab>
 int launch_chain_variant(const gcb_chain_desc& d, const ChainShape& sh, cudaStream_t stream) {
   using Cfg = gcb::ChainConfig<kSplit>;
   // The parameter area ends the dynamic shared memory: request only the vectors of this chain.
   const int smem = Cfg::kSmemBytes - (gcb::kChainParamVecs - sh.vecs) * gcb::kMaxN * 4;
   const int tiles = (d.rows + gcb::kTileM - 1) / gcb::kTileM;
   const int clusters = std::min(tiles, sm_count_cached() / 2);   // the scratch is sized for SMs / 2
-  return launch_persistent<gcb::mlp_chain_tc_kernel<kSplit, kPre>>(Cfg::kSmemBytes, smem, 2, clusters, stream, d,
-                                                                   sh.nq, sh.nslots);
+  return launch_persistent<gcb::mlp_chain_tc_kernel<kSplit, kPre, kTab>>(Cfg::kSmemBytes, smem, 2, clusters,
+                                                                         stream, d, sh.nq, sh.nslots);
 }
 
 struct StepCtx {
@@ -730,7 +745,7 @@ int gcb_chain_forward(const gcb_chain_desc* d, void* stream) {
       kv += w;
       a_elems += w * (g.seg[s].img ? 1 : g.seg[s].fan);
     }
-    a_elems += 512.0 * g.n_pre_add;
+    a_elems += 512.0 * g.n_pre_add + (g.acc_table ? 512.0 : 0.0);   // an acc_table layer: no MMAs
     flops += 2.0 * rows * kv * 512;
     bytes += 4.0 * (rows * a_elems + kv * 512 +
                     rows * 512 * ((g.out ? 1 : 0) + (g.out_y ? 1 : 0) + (g.residual ? 1 : 0) +
@@ -738,9 +753,14 @@ int gcb_chain_forward(const gcb_chain_desc* d, void* stream) {
     // (a residual_img that is also a segment of the chain is read from HBM once: not counted again)
   }
   ProfScope prof(st, GCB_KIND_CHAIN_TC, flops, bytes);
+  if (sh.tab) {
+    if (d->precision == GCB_PREC_BF16X3)
+      return sh.pre ? launch_chain_variant<true, true, true>(*d, sh, st) : launch_chain_variant<true, false, true>(*d, sh, st);
+    return sh.pre ? launch_chain_variant<false, true, true>(*d, sh, st) : launch_chain_variant<false, false, true>(*d, sh, st);
+  }
   if (d->precision == GCB_PREC_BF16X3)
-    return sh.pre ? launch_chain_variant<true, true>(*d, sh, st) : launch_chain_variant<true, false>(*d, sh, st);
-  return sh.pre ? launch_chain_variant<false, true>(*d, sh, st) : launch_chain_variant<false, false>(*d, sh, st);
+    return sh.pre ? launch_chain_variant<true, true, false>(*d, sh, st) : launch_chain_variant<true, false, false>(*d, sh, st);
+  return sh.pre ? launch_chain_variant<false, true, false>(*d, sh, st) : launch_chain_variant<false, false, false>(*d, sh, st);
 }
 
 int gcb_segment_sum(const float* msg, int32_t ld_msg, const int32_t* row_ptr, int32_t num_nodes,
@@ -1568,6 +1588,14 @@ struct Chain {
     l.ld_res = l.ld_out = l.ld_out_y = 512;
     return l;
   }
+  // first linear of an edge MLP whose edge-block product e @ W_e is the static table `acc`
+  // (gcb_model.static_acc_*): no MMAs, the epilogue adds bias and gathered addends as mlp0 would
+  gcb_chain_layer& mlp0_acc(const gcb_mlp& w, const float* acc) {
+    gcb_chain_layer& l = add();
+    l.acc_table = acc; l.ld_acc = 512;
+    l.bias = w.b0; l.act = GCB_ACT_SWISH; l.keep = 1;
+    return l;
+  }
   // node-level projection of the kept result of layer `from` (no bias, no activation)
   gcb_chain_layer& proj(int from, const void* w_packed, float* out) {
     gcb_chain_layer& l = add();
@@ -1581,6 +1609,11 @@ struct Chain {
     return rc;
   }
 };
+
+// The static-edge cache is present (gcb_forward_static has filled it).
+bool static_cached(const gcb_model* m) {
+  return m->static_acc_g2m && m->static_acc_m2g && m->static_acc_mesh && m->static_e0_img;
+}
 
 void set_pre(gcb_chain_layer& l, const float* ps, const int32_t* snd, const float* pr, const int32_t* rcv) {
   l.n_pre_add = 2;
@@ -1612,12 +1645,19 @@ int mega_encode(StepCtx& c, const void* grid_in_img) {
     if ((rc = ch.run(c))) return rc;
   }
   {  // e1 = LN.MLP(edge feats);  m1 = LN.MLP([e1 | vg0[snd] | vm0[rcv]]) -> edge_b
-    Chain ch(m, m->e_g2m, 1);
-    s[0] = seg(m->g2m_feat, nullptr, 4, 16, 4);
-    ch.mlp0(m->enc_e_g2m, 1, s);
-    ch.mlp1(m->enc_e_g2m).keep = 1;
-    set_pre(ch.mlp0_from(m->proc_e_g2m, ch.last(), m->proc_e_g2m_split.we_packed),
-            m->proj_grid, m->g2m_snd, m->proj_mesh_a, m->g2m_rcv);
+    // (with the static-edge cache, e1 @ W_e is read from it and e1 is not formed)
+    const bool cached = static_cached(m);
+    Chain ch(m, m->e_g2m, cached ? 0 : 1);
+    gcb_chain_layer* l0 = nullptr;
+    if (cached) {
+      l0 = &ch.mlp0_acc(m->proc_e_g2m, m->static_acc_g2m);
+    } else {
+      s[0] = seg(m->g2m_feat, nullptr, 4, 16, 4);
+      ch.mlp0(m->enc_e_g2m, 1, s);
+      ch.mlp1(m->enc_e_g2m).keep = 1;
+      l0 = &ch.mlp0_from(m->proc_e_g2m, ch.last(), m->proc_e_g2m_split.we_packed);
+    }
+    set_pre(*l0, m->proj_grid, m->g2m_snd, m->proj_mesh_a, m->g2m_rcv);
     ch.mlp1(m->proc_e_g2m).out = m->edge_b;
     if ((rc = ch.run(c))) return rc;
   }
@@ -1656,7 +1696,17 @@ int mega_process_step(StepCtx& c, int k) {
   gcb_segment s[3];
   const int D = 512;
   const bool last = (k == m->msg_steps - 1);
-  if (k == 0) {
+  if (k == 0 && static_cached(m)) {
+    // m = LN.MLP([e0 | v[snd] | v[rcv]]) with e0 @ W_e from the static-edge cache;  e1 = e0 + m
+    // with e0 read from its cached image
+    Chain ch(m, m->e_mesh, 0);
+    set_pre(ch.mlp0_acc(m->proc_e_mesh[0], m->static_acc_mesh),
+            m->proj_mesh_a, m->mesh_snd, m->proj_mesh_b, m->mesh_rcv);
+    gcb_chain_layer& l1 = ch.mlp1(m->proc_e_mesh[0]);
+    l1.out_y = m->mesh_msg;
+    if (!last) { l1.residual_img = m->static_e0_img; l1.out_img = m->mesh_edge_img; }
+    if ((rc = ch.run(c))) return rc;
+  } else if (k == 0) {
     // e0 = LN.MLP(edge feats);  m = LN.MLP([e0 | v[snd] | v[rcv]]);  e1 = e0 + m  (e0 stays on chip)
     Chain ch(m, m->e_mesh, 1);
     s[0] = seg(m->mesh_feat, nullptr, 4, 16, 4);
@@ -1708,12 +1758,19 @@ int mega_decode(StepCtx& c, float* grid_out) {
   const int D = 512;
   GCB_CHECK_ARG(m->e_m2g == 3 * m->num_grid, "mesh2grid must have fan-in 3");
   {  // e3 = LN.MLP(edge feats);  m3 = LN.MLP([e3 | v[snd] | vg1[rcv]]) -> edge_b
-    Chain ch(m, m->e_m2g, 1);
-    s[0] = seg(m->m2g_feat, nullptr, 4, 16, 4);
-    ch.mlp0(m->enc_e_m2g, 1, s);
-    ch.mlp1(m->enc_e_m2g).keep = 1;
-    set_pre(ch.mlp0_from(m->proc_e_m2g, ch.last(), m->proc_e_m2g_split.we_packed),
-            m->proj_mesh_a, m->m2g_snd, m->proj_grid_b, m->m2g_rcv);
+    // (with the static-edge cache, e3 @ W_e is read from it and e3 is not formed)
+    const bool cached = static_cached(m);
+    Chain ch(m, m->e_m2g, cached ? 0 : 1);
+    gcb_chain_layer* l0 = nullptr;
+    if (cached) {
+      l0 = &ch.mlp0_acc(m->proc_e_m2g, m->static_acc_m2g);
+    } else {
+      s[0] = seg(m->m2g_feat, nullptr, 4, 16, 4);
+      ch.mlp0(m->enc_e_m2g, 1, s);
+      ch.mlp1(m->enc_e_m2g).keep = 1;
+      l0 = &ch.mlp0_from(m->proc_e_m2g, ch.last(), m->proc_e_m2g_split.we_packed);
+    }
+    set_pre(*l0, m->proj_mesh_a, m->m2g_snd, m->proj_grid_b, m->m2g_rcv);
     ch.mlp1(m->proc_e_m2g).out = m->edge_b;
     if ((rc = ch.run(c))) return rc;
   }
@@ -1843,6 +1900,21 @@ int stage_decode(StepCtx& c, float* grid_out) {
   return run_mlp(c, m->dec_grid, ng, 1, s, o);
 }
 
+// The static-edge cache of one graph: [edge embedder MLP -> edge block W_e of the first edge-MLP
+// layer] over the static edge features.  The last layer stores its raw accumulator (acc_out), which
+// the step's acc_table layer then takes as the accumulator its MMAs would have produced: the same
+// K-steps in the same order on the same operands.  e_img, if set, receives the embedded edges.
+int static_edge_chain(StepCtx& c, int rows, const float* feat, const gcb_mlp& enc, const void* we,
+                      float* acc, void* e_img) {
+  gcb_segment s = seg(feat, nullptr, 4, 16, 4);
+  Chain ch(c.m, rows, 1);
+  ch.mlp0(enc, 1, &s);
+  gcb_chain_layer& e = ch.mlp1(enc);
+  e.keep = 1; e.out_img = e_img;
+  ch.proj(ch.last(), we, acc).acc_out = 1;
+  return ch.run(c);
+}
+
 int forward_eager(const gcb_model* m, const void* grid_in_img, float* grid_out, void* stream,
                   int32_t* launches) {
   int rc = check_model(m);
@@ -1880,6 +1952,24 @@ int gcb_forward_stage(const gcb_model* m, int32_t stage, int32_t step, const voi
   }
   if (launches) *launches = c.launches;
   return rc;
+}
+
+int gcb_forward_static(const gcb_model* m, void* stream, int32_t* launches) {
+  GCB_CHECK_ARG(m != nullptr, "null model");
+  int rc = check_model(m);
+  if (rc) return rc;
+  GCB_CHECK_ARG(mega(m), "the static-edge cache needs the deep-chain path (image_residual, fuse, "
+                         "pregather, deep_chains, a tensor-core precision, one GPU)");
+  GCB_CHECK_ARG(static_cached(m), "static_acc_g2m / static_acc_m2g / static_acc_mesh / static_e0_img is null");
+  StepCtx c{m, static_cast<cudaStream_t>(stream), 0};
+  if ((rc = static_edge_chain(c, m->e_g2m, m->g2m_feat, m->enc_e_g2m, m->proc_e_g2m_split.we_packed,
+                              m->static_acc_g2m, nullptr))) return rc;
+  if ((rc = static_edge_chain(c, m->e_m2g, m->m2g_feat, m->enc_e_m2g, m->proc_e_m2g_split.we_packed,
+                              m->static_acc_m2g, nullptr))) return rc;
+  if ((rc = static_edge_chain(c, m->e_mesh, m->mesh_feat, m->enc_e_mesh, m->proc_e_mesh_split[0].we_packed,
+                              m->static_acc_mesh, m->static_e0_img))) return rc;
+  if (launches) *launches = c.launches;
+  return GCB_OK;
 }
 
 int gcb_set_cluster_size(int32_t ctas) {

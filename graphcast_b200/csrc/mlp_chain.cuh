@@ -50,8 +50,9 @@ constexpr int kChainParamVecs = 8;          // [512]-float parameter vectors (bi
 template <bool kSplit>
 using ChainConfig = StageRing<kSplit, kLnxBytes + kChainTailBytes + kChainParamVecs * kMaxN * 4>;
 
-// kKindLN*: LayerNorm without residual / with an fp32 residual / with an operand-image residual
-enum { kKindPlain = 0, kKindSwish = 1, kKindLN = 2, kKindLNRes = 3, kKindLNImg = 4 };
+// kKindLN*: LayerNorm without residual / with an fp32 residual / with an operand-image residual;
+// kKindAcc: the raw accumulator to `out` (gcb_chain_layer.acc_out)
+enum { kKindPlain = 0, kKindSwish = 1, kKindLN = 2, kKindLNRes = 3, kKindLNImg = 4, kKindAcc = 5 };
 
 struct ChainLayer {
   const uint8_t* w;
@@ -66,6 +67,12 @@ struct ChainLayer {
   int keep_q;                            // scratch ring this layer writes, -1 = none
   int has_table;                         // some segment is an fp32 table (producer warps)
   int res_q;                             // residual = the kept result in scratch ring res_q, -1 = none
+};
+// Accumulator table of a layer (gcb_chain_layer.acc_table, or null), kTab variants only: kept apart
+// from ChainLayer so that the other variants keep their shared-memory layout and code.
+struct AccTableInfo {
+  const float* acc;
+  long long ld;
 };
 
 // ---- epilogue ----------------------------------------------------------------------------
@@ -141,6 +148,31 @@ __device__ __forceinline__ void epi_load_res_img(const ChainEpi& e, uint2 (&buf)
       const uint8_t* p = e.res_img + epi_img_off(c, jj, h);
       buf[half + 2 * jj + h] = make_uint2(ptx::ld_global_b32_pred(p, ok), ptx::ld_global_b32_pred(p + kAPartBytes, ok));
     }
+}
+
+// Accumulator of a table layer (gcb_chain_layer.acc_table): this thread's fragment, rows lr0 + 8h
+// and columns 8j + 2q (+1) of the unit, straight from the fp32 table (rows past the end: 0).
+// Fully unrolled, so every load targets a fixed accumulator register and all 64 are in flight at once.
+__device__ __forceinline__ void load_acc_table(float (&acc)[128], const float* const (&row)[2],
+                                               const bool (&ok)[2]) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint2 v = ptx::ld_global_nc_v2_pred(row[h] + 8 * j, ok[h], 0u);
+      acc[4 * j + 2 * h] = __uint_as_float(v.x);
+      acc[4 * j + 2 * h + 1] = __uint_as_float(v.y);
+    }
+}
+// kKindAcc: the accumulator itself to `out`, without the + 0 of an absent bias or residual, so that
+// a table built from it (acc_table) holds the accumulator's bits, the sign of a zero included.
+__device__ __forceinline__ void store_acc(const float (&acc)[128], const ChainEpi& e) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      ptx::st_global_v2_pred(e.out[h] + 8 * j, make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]),
+                             e.row_ok[h]);
 }
 
 // The column loop of one unit for one layer kind (kAdd: Plain / Swish with gathered addends).
@@ -231,7 +263,10 @@ __device__ __forceinline__ void chain_epilogue(float (&acc)[128], uint2 (&buf)[1
   }
 }
 
-template <bool kSplit, bool kPre>
+// kTab: the chain has table-accumulator (acc_table) or raw-accumulator (acc_out) layers.  Their code
+// is compiled only into the kTab variants, so that every other chain keeps the register allocation
+// and the loop code it had without them.
+template <bool kSplit, bool kPre, bool kTab>
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, const int nslots) {
   using Cfg = ChainConfig<kSplit>;
@@ -248,8 +283,10 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
   ChainLayer* s_layer = reinterpret_cast<ChainLayer*>(h_free_bar + GCB_MAX_CHAIN * kChainSlotsMax);  // [GCB_MAX_CHAIN]
   SegInfo* s_seg = reinterpret_cast<SegInfo*>(s_layer + GCB_MAX_CHAIN);              // [GCB_MAX_CHAIN][3]
   PreAddInfo* s_pre = reinterpret_cast<PreAddInfo*>(s_seg + GCB_MAX_CHAIN * 3);      // [GCB_MAX_CHAIN][2]
+  AccTableInfo* s_acc = reinterpret_cast<AccTableInfo*>(s_pre + GCB_MAX_CHAIN * 2);  // [GCB_MAX_CHAIN], kTab
   static_assert((2 * 12 + 4 + 2 * GCB_MAX_CHAIN * kChainSlotsMax) * 8 +
-                    GCB_MAX_CHAIN * (sizeof(ChainLayer) + 3 * sizeof(SegInfo) + 2 * sizeof(PreAddInfo))
+                    GCB_MAX_CHAIN * (sizeof(ChainLayer) + 3 * sizeof(SegInfo) + 2 * sizeof(PreAddInfo) +
+                                     sizeof(AccTableInfo))
                     <= kChainTailBytes, "tail region too small");
 
   const int warp = threadIdx.x >> 5;
@@ -316,10 +353,12 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
       cl.residual = gl.residual; cl.out = gl.out; cl.out_y = gl.out_y;
       cl.out_img = static_cast<uint8_t*>(gl.out_img);
       cl.res_img = static_cast<const uint8_t*>(gl.residual_img);
+      if constexpr (kTab) { s_acc[l].acc = gl.acc_table; s_acc[l].ld = gl.ld_acc; }
       cl.ld_res = gl.ld_res; cl.ld_out = gl.ld_out; cl.ld_outy = gl.ld_out_y;
       cl.nseg = gl.nseg; cl.n_pre = gl.n_pre_add;
       cl.res_q = gl.residual_keep > 0 ? q_of_layer[gl.residual_keep - 1] : -1;
-      cl.kind = gl.ln_scale != nullptr
+      cl.kind = (kTab && gl.acc_out) ? kKindAcc
+                : gl.ln_scale != nullptr
                     ? (gl.residual != nullptr
                            ? kKindLNRes
                            : ((gl.residual_img != nullptr || gl.residual_keep > 0) ? kKindLNImg : kKindLN))
@@ -496,11 +535,16 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         const ChainLayer& cl = s_layer[l];
         const int kind = cl.kind;
         const float* const s_bias = cl.bias_off >= 0 ? s_param + cl.bias_off : nullptr;
-        if (eg == 0 && ti + 1 < T && (cl.residual != nullptr || cl.res_img != nullptr)) {
-          // Pull the residual of this layer's NEXT tile into L2 now (a whole step ahead).
+        if (eg == 0 && ti + 1 < T && (cl.residual != nullptr || cl.res_img != nullptr || (kTab && s_acc[l].acc != nullptr))) {
+          // Pull the residual (or the accumulator table) of this layer's NEXT tile into L2 now (a
+          // whole step ahead).
           const uint32_t ntile = tile + ncl;
           const int pr = (warp & 3) * 32 + lane;      // 128 threads: one row each
-          if (cl.residual != nullptr) {
+          if (kTab && s_acc[l].acc != nullptr) {
+            const AccTableInfo at = s_acc[l];
+            const long long nrow = static_cast<long long>(ntile) * kTileM + pr;
+            if (nrow < rows_total) ptx::bulk_prefetch_l2(at.acc + nrow * at.ld + col_base, kUnitN * 4);
+          } else if (cl.residual != nullptr) {
             const long long nrow = static_cast<long long>(ntile) * kTileM + pr;
             if (nrow < rows_total) ptx::bulk_prefetch_l2(cl.residual + nrow * cl.ld_res + col_base, kUnitN * 4);
           } else if (pr < kUnitN / kKStep) {
@@ -509,7 +553,7 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
                                   GCB_A_IMAGE_BLOCK);
           }
         }
-        const bool is_ln = kind >= kKindLN;
+        const bool is_ln = kind >= kKindLN && (!kTab || kind <= kKindLNImg);   // kKindAcc needs kTab
         const bool want_pre = kPre && !is_ln && cl.n_pre > 0;
         const int keep_q = cl.keep_q;
         // Epilogue state of this unit (ChainEpi).  Pointers of absent outputs are formed from
@@ -569,6 +613,16 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         if (want_pre) epi_load_pre(e, buf, 0, true);
         else if (kind == kKindLNRes) epi_load_res(e, buf, 0, 0, true);
         else if (kind == kKindLNImg) epi_load_res_img(e, buf, 0, 0, true);
+        const bool acc_tab = kTab && s_acc[l].acc != nullptr;
+        if (acc_tab) {
+          // No MMAs to hide the loads behind: the table rows go out together with chunk 0's inputs,
+          // before the h_free wait.
+          const long long grow0 = static_cast<long long>(tile) * kTileM + lr0;
+          const AccTableInfo at = s_acc[l];
+          const float* row[2] = {at.acc + grow0 * at.ld + col_base + 2 * q,
+                                 at.acc + (grow0 + 8) * at.ld + col_base + 2 * q};
+          load_acc_table(acc, row, e.row_ok);
+        }
         if (lead && eg == 0) trace(u, 0);
         if (keep_q >= 0) {
           // previous readers of this slot (tile ti - nslots) are done in both CTAs
@@ -576,8 +630,10 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
                          (static_cast<uint32_t>(ti / nslots) & 1u) ^ 1u);
         }
         if (lead && eg == 0) { trace(u, 2); trace_val(u, 9, cl.ksteps); }
-        mma_unit<kSplit, Cfg::kStages, Cfg::kStageBytes, Cfg::kAStageBytes>(
-            acc, stage_base, full_bar, empty_bar, stage, phase, cl.ksteps, eg * 64 * 16, cmask, u);
+        // A table layer has no segments: no stage was filled for it, and no scratch slot is read.
+        if (!acc_tab)
+          mma_unit<kSplit, Cfg::kStages, Cfg::kStageBytes, Cfg::kAStageBytes>(
+              acc, stage_base, full_bar, empty_bar, stage, phase, cl.ksteps, eg * 64 * 16, cmask, u);
         if (lane == 0) {
           // Every scratch slot this unit read is reusable (in both CTAs) once these MMAs retired.
           // The slot's readers are bulk copies that have completed (their bytes were counted on
@@ -613,6 +669,8 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
           chain_epilogue<kKindLN, false>(acc, buf, e, keep_policy);
         } else if (kind == kKindLNRes) {
           chain_epilogue<kKindLNRes, false>(acc, buf, e, keep_policy);
+        } else if (kTab && kind == kKindAcc) {
+          store_acc(acc, e);
         } else {
           chain_epilogue<kKindLNImg, false>(acc, buf, e, keep_policy);
         }

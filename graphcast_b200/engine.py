@@ -52,7 +52,7 @@ class Engine:
                device: Optional[torch.device] = None, pregather: bool = True,
                fuse: bool = True, chain_lag: int = 0, image_residual: bool = True,
                deep_chains: bool = True, num_grid_owned: int = 0, num_mesh_owned: int = 0,
-               reorder_mesh: bool = False):
+               reorder_mesh: bool = False, static_cache: bool = True):
     if precision not in _native.PRECISIONS:
       raise ValueError(f"unknown precision {precision!r}; expected one of "
                        f"{sorted(_native.PRECISIONS)}")
@@ -83,6 +83,16 @@ class Engine:
     # deep_chains (with image_residual): [edge embedder -> edge MLP] and [node MLP -> next
     # projections] as single launches; see gcb_model.deep_chains.
     self.deep_chains = bool(deep_chains)
+    # static_cache (deep-chain path only): the weight-only edge terms -- the embedded edges' product
+    # with the first edge-MLP layer's edge block, per graph, and the embedded mesh edges e0 -- are
+    # computed once per weight version and precision (gcb_forward_static) instead of every step.
+    # Built by step() when absent or stale and no gradient workspace exists; released by every
+    # gradient, tangent and HVP path before it builds its workspace.
+    self.static_cache = bool(static_cache)
+    self._static = None                   # {name: tensor} of the cache, or None
+    self._static_key = None               # (weights_version, precision) the cache was built for
+    self._static_events = None            # CUDA events around the last build
+    self.static_cache_builds = 0
     self.c_in_pad = _ceil(c_in + 3, 16)
     self.c_in_valid = _ceil(c_in + 3, 4)
     g = static_graph
@@ -351,6 +361,7 @@ class Engine:
       changed.add(key if isinstance(key, str) else key[0])
     self._host_params, self._params_stale, self._copies_stale = params, False, False
     self.weights_version += 1
+    self._static_detach()                 # stale until the next step() rebuilds it
     if self._backward is not None:
       with self._on_device():
         self._backward.repack(changed)
@@ -377,6 +388,7 @@ class Engine:
         self._backward.repack()
     self._params_stale = self._copies_stale = True
     self.weights_version += 1
+    self._static_detach()
 
   def _check_params(self, params, shape) -> None:
     for name, fields in self.param_shapes.items():
@@ -504,7 +516,78 @@ class Engine:
           self.grid_agg_img, self.grid_out]
     if self.pregather:
       ts += [self.proj_grid, self.proj_mesh_a, self.proj_mesh_b]
+    if self._static is not None:
+      ts += list(self._static.values())
     return sum(t.numel() * t.element_size() for t in ts)
+
+  # -- static-edge cache (gcb_forward_static) ------------------------------------------------
+  def _static_eligible(self) -> bool:
+    """The deep-chain path runs (the C side's condition for gcb_model.deep_chains)."""
+    return (self.static_cache and self.image_residual and self.fuse and self.pregather and
+            self.deep_chains and self.precision in ("bf16x3", "bf16") and
+            not (self.num_grid_owned or self.num_mesh_owned))
+
+  def _static_detach(self) -> None:
+    """The step stops reading the cache (its tables are kept for a rebuild in place)."""
+    m = self._model
+    m.static_acc_g2m = m.static_acc_m2g = m.static_acc_mesh = m.static_e0_img = None
+    self._static_key = None
+
+  def release_static_cache(self) -> None:
+    """Frees the static-edge cache; the next step() builds it again."""
+    self._static_detach()
+    self._static = None
+
+  def _ensure_static_cache(self, stream: torch.cuda.Stream) -> None:
+    """Builds the static-edge cache on `stream` when the step can use it and it is absent or stale."""
+    if not self._static_eligible():
+      if self._static is not None:
+        self.release_static_cache()
+      return
+    if self._backward is not None:
+      # A gradient workspace exists: the steps are most likely the forward of the next gradient,
+      # tangent or HVP call, which frees the cache again before its backward pass, so a build would
+      # cost 10 GiB (0.25 degree) next to the workspace for a few steps.  Inference gets the cache
+      # back after release_gradient_workspace().
+      return
+    key = (self.weights_version, self.precision)
+    if self._static is not None and self._static_key == key:
+      return
+    m = self._model
+    self._static_detach()
+    if self._static is None:
+      f = lambda rows: torch.empty([max(rows, 1), LATENT], dtype=torch.float32, device=self.device)
+      self._static = {"acc_g2m": f(m.e_g2m), "acc_m2g": f(m.e_m2g), "acc_mesh": f(m.e_mesh),
+                      "e0_img": self._image(m.e_mesh)}
+      cur = torch.cuda.current_stream(self.device)
+      if stream != cur:
+        # The tables were allocated, and the image zero-filled, on the current stream; the build
+        # and the steps that read them run on `stream`.
+        stream.wait_stream(cur)
+        for t in self._static.values():
+          t.record_stream(stream)
+    t = self._static
+    m.static_acc_g2m, m.static_acc_m2g = self._ptr(t["acc_g2m"]), self._ptr(t["acc_m2g"])
+    m.static_acc_mesh, m.static_e0_img = self._ptr(t["acc_mesh"]), self._ptr(t["e0_img"])
+    ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+    ev[0].record(stream)
+    try:
+      _native.check(self._lib.gcb_forward_static(C.byref(m), stream.cuda_stream, None),
+                    "gcb_forward_static")
+    except Exception:
+      self.release_static_cache()
+      raise
+    ev[1].record(stream)
+    self._static_events = ev
+    self._static_key = key
+    self.static_cache_builds += 1
+
+  def static_cache_build_ms(self) -> Optional[float]:
+    """Device time of the last static-edge cache build in ms (synchronises with it), or None."""
+    if self._static_events is None:
+      return None
+    self._static_events[1].synchronize()
+    return self._static_events[0].elapsed_time(self._static_events[1])
 
   # -- execution ---------------------------------------------------------------------
   def _stream(self) -> int:
@@ -518,6 +601,7 @@ class Engine:
   def set_precision(self, precision: str) -> None:
     self._model.precision = _native.PRECISIONS[precision]
     self.precision = precision
+    self._static_detach()                 # the cache holds products of the old precision
 
   def pack_inputs(self, planes: torch.Tensor, mean: Optional[torch.Tensor] = None,
                   scale: Optional[torch.Tensor] = None,
@@ -552,6 +636,7 @@ class Engine:
       self._step_stream.wait_stream(cur)
     st = self._step_stream if side else cur
     with self._on_device():
+      self._ensure_static_cache(st)
       _native.check(self._lib.gcb_forward(C.byref(self._model), grid_in.data_ptr(),
                                           grid_out.data_ptr(), st.cuda_stream, C.byref(n)),
                     "gcb_forward")
@@ -640,8 +725,17 @@ class Engine:
     self._grad_workspace(chunk_rows, "parameter gradients")
     self._backward.zero_grads()
 
+  def release_gradient_workspace(self) -> None:
+    """Frees the gradient workspace of the gradient, tangent and HVP paths, with the parameter
+    gradients it accumulated (the next such call builds it again).  While it exists, step() runs
+    without the static-edge cache."""
+    self._backward = None
+
   def _grad_workspace(self, chunk_rows: Optional[int], what: str) -> None:
-    """The checks of every gradient and the gradient workspace, created on first use."""
+    """The checks of every gradient and the gradient workspace, created on first use.  The static-edge
+    cache is released first: the derivative paths run the step without it, and at 0.25 degree their
+    peaks leave no room for it."""
+    self.release_static_cache()
     if self.num_grid_owned:
       raise NotImplementedError(
           f"{what} are not available in the node-partitioned engine: each rank holds "

@@ -191,7 +191,7 @@ class GraphCast(Predictor):
                params: Optional[Mapping[str, Mapping[str, np.ndarray]]] = None,
                precision: str = "bf16x3", device: Optional[Any] = None,
                pregather: bool = True, fuse: bool = True, chain_lag: int = 0,
-               image_residual: bool = True, deep_chains: bool = True):
+               image_residual: bool = True, deep_chains: bool = True, static_cache: bool = True):
     if model_config.latent_size != engine_lib.LATENT:
       raise ValueError(f"latent_size {model_config.latent_size} is not supported by the "
                        f"sm_90a kernels (only {engine_lib.LATENT})")
@@ -203,6 +203,9 @@ class GraphCast(Predictor):
     self._pregather = pregather
     self._fuse, self._chain_lag, self._image_residual = fuse, chain_lag, image_residual
     self._deep_chains = deep_chains
+    # Engine.static_cache: the weight-only edge terms of the step are computed once per weight
+    # version and precision (10.3 GiB at 0.25 degree), not every step.
+    self._static_cache = static_cache
     self._device = device
     self._engine: Optional[engine_lib.Engine] = None
     self._params = params
@@ -292,7 +295,7 @@ class GraphCast(Predictor):
           msg_steps=self._model_config.gnn_msg_steps, precision=self._precision,
           device=self._device, pregather=self._pregather, fuse=self._fuse,
           chain_lag=self._chain_lag, image_residual=self._image_residual,
-          deep_chains=self._deep_chains)
+          deep_chains=self._deep_chains, static_cache=self._static_cache)
     elif self._engine.c_in != c_in:
       raise ValueError(f"inputs+forcings stack to {c_in} channels but the model was "
                        f"built for {self._engine.c_in}")

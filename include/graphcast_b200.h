@@ -544,6 +544,15 @@ typedef struct {
   float* out_y; int32_t ld_out_y;    /* y alone, fp32 (optional) */
   void* out_img;                     /* residual + y as an operand image (optional) */
   int32_t n_pre_add; gcb_pre_add pre_add[2];
+  /* Accumulator from a table: the layer's A @ W is read from acc_table [rows, ld_acc] (fp32, 16-byte
+   * aligned, ld_acc >= 512 and a multiple of 4) instead of computed: nseg = 0, no w_packed, no
+   * LayerNorm.  Bias, gathered addends, activation, keep and outputs apply as usual.  For products
+   * that depend only on the weights and static inputs (gcb_forward_static). */
+  const float* acc_table; int32_t ld_acc;
+  /* 1: `out` receives the accumulator A @ W itself (no bias, activation, residual or + 0, so the sign
+   * of a zero is kept: the table an acc_table layer reproduces bit for bit).  Needs out; excludes
+   * bias, LayerNorm, swish, pre_add, keep, out_y, out_img and acc_table. */
+  int32_t acc_out;
 } gcb_chain_layer;
 
 typedef struct {
@@ -675,6 +684,21 @@ typedef struct {
   int32_t deep_chains;
   float* proj_grid_b;       /* [num_grid, 512]: receiver projection of the mesh2grid edge MLP */
   int64_t chain_scratch_bytes;
+  /* Static-edge cache of the deep-chain step (gcb_forward_static); all NULL = none.  The edge
+   * features are static, so the embedded edge latents and their product with the edge block W_e of
+   * the first edge-MLP layer depend only on the weights and the precision:
+   *   static_acc_g2m  [e_g2m, 512]   e1 @ W_e (grid2mesh), the accumulator without bias
+   *   static_acc_m2g  [e_m2g, 512]   the same for mesh2grid
+   *   static_acc_mesh [e_mesh, 512]  e0 @ W_e of processor step 0
+   *   static_e0_img   image [e_mesh, 512] of e0, the residual of processor step 0
+   * With all four set (and the deep-chain path active), those chains start from the tables and
+   * skip the edge embedder and the edge block of the first layer.  Results are bit-identical to
+   * the step without the cache, provided gcb_forward_static ran after the LAST write to any weight
+   * buffer or change of precision: the step does not check that the tables are current. */
+  float* static_acc_g2m;
+  float* static_acc_m2g;
+  float* static_acc_mesh;
+  void* static_e0_img;
 } gcb_model;
 
 /* Stage-wise execution of the same step: gcb_forward == ENCODE, PROCESS_EMBED, PROCESS_STEP for
@@ -703,6 +727,13 @@ int gcb_forward_stage(const gcb_model* m, int32_t stage, int32_t step, const voi
  * `launches` (host pointer, may be NULL) receives the number of kernels launched. */
 int gcb_forward(const gcb_model* m, const void* grid_in_img, float* grid_out, void* stream,
                 int32_t* launches);
+
+/* Fills the static-edge cache of `m` (the static_* buffers, which must be set) with three chain
+ * launches on `stream`: per graph [edge embedder MLP -> edge block of the first edge-MLP layer].
+ * Needs the deep-chain path (image_residual, fuse, pregather, deep_chains, a tensor-core precision,
+ * one GPU).  Run it again after every write to a weight buffer and every change of precision.
+ * Direct launches: never part of gcb_forward's recorded graph.  `launches` as in gcb_forward. */
+int gcb_forward_static(const gcb_model* m, void* stream, int32_t* launches);
 
 /* gcb_forward replays a CUDA graph of its launch sequence from the third call with the same
  * (model contents, buffers, stream) on: the first call runs the launches directly, the second

@@ -6,7 +6,10 @@ For an edge-MLP-shaped problem (image A operand + two gathered addends -> swish 
 fp32 + image outputs) and a node-MLP-shaped one it prints: NaN diagnostics, bitwise equality of
 the two paths, CUDA-event times, and the in-kernel timeline of cluster 0 / CTA 0 of the chain
 launch (cycles; per executed unit: barrier waits, MMA phase per K-step against the 768-cycle
-tensor-pipe ideal, LayerNorm statistics, epilogue stores, scratch hand-over)."""
+tensor-pipe ideal, LayerNorm statistics, epilogue stores, scratch hand-over).  The "edge-table" case
+is the edge problem with the first layer's accumulator read from a table (gcb_chain_layer.acc_table,
+filled by an acc_out chain) instead of computed: its layer-0 units have no MMAs, and their "columns"
+cycles include the wait for the table rows."""
 import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
@@ -33,7 +36,7 @@ def timed(fn, reps=5):
 IMG_RES = len(sys.argv) > 3 and sys.argv[3] == "img"
 
 
-def case(kind):
+def case(kind, table=False):
   g = torch.Generator().manual_seed(5)
   f = lambda *shape: torch.randn(*shape, generator=g)
   n_nodes = 40962
@@ -76,6 +79,19 @@ def case(kind):
     tc._fill_chain_layer(ch.layer[1], [None], [0], l1, act=False, keep=False, residual=res, out=o2,
                          out_y=y2, out_img=img2)
 
+  if table:
+    acc = nan()
+    tab = _native.ChainDesc()
+    tab.rows, tab.nlayers, tab.precision, tab.lag = rows, 1, 0, lag
+    tab.scratch, tab.scratch_bytes = scratch.data_ptr(), scratch.numel()
+    tc._fill_chain_layer(tab.layer[0], segs, [-1] * len(segs), l0, act=False, keep=False, out=acc)
+    tab.layer[0].bias, tab.layer[0].acc_out = None, 1
+    _native.check(lib.gcb_chain_forward(C.byref(tab), None), "acc_out chain")
+    cl = ch.layer[0]
+    cl.nseg, cl.w_packed, cl.seg_from[0] = 0, None, -1
+    cl.acc_table, cl.ld_acc = acc.data_ptr(), 512
+    kind += "-table"
+
   def fused():
     _native.check(lib.gcb_chain_forward(C.byref(ch), None), "chain")
 
@@ -105,21 +121,29 @@ def print_timeline(t):
   print("   u L | start  h_free  ops_ready  mma (per K-step / ideal) | ln_stats  columns  handed"
         " | next unit | tma: blocked h_full_wait")
   tot = np.zeros(8)
+  per_layer = {}
   for u in range(2, 14):
-    r = t[u]
+    r = t[u].copy()
+    if r[9] == 0:
+      r[1] = r[3]                        # a table unit: no MMAs, no operand barrier
     mma = r[3] - r[1]
     ln = r[4] - r[3] if r[4] > 0 else 0
     stored = r[5] - max(r[4], r[3])      # column loop
     handed = r[6] - r[5]                 # last store issued -> h_full arrives done
     nxt = t[u + 1, 0] - r[0]
     tot += [r[2] - r[0], r[1] - r[2], mma, ln + stored + handed, nxt, r[9], stored, handed]
+    per_layer.setdefault(int(r[11]), []).append((nxt, stored))
     print(f"  {u:2d} {r[11]} | {r[0]-base:8d} +{r[2]-r[0]:6d} +{r[1]-r[2]:6d} +{mma:7d} ({mma / max(r[9], 1):6.0f} / {IDEAL_KSTEP}) | "
           f"+{ln:6d} +{stored:7d} +{handed:6d} | +{nxt:7d} | {r[7]:7d} {r[8]:7d}")
   print(f"  units 2-13: h_free wait {tot[0]:.0f}, operand wait {tot[1]:.0f}, MMA {tot[2]:.0f} "
         f"({tot[2] / tot[5]:.0f} cycles per K-step vs {IDEAL_KSTEP}), epilogue + hand-over {tot[3]:.0f}, "
         f"unit to unit {tot[4]:.0f} cycles")
   print(f"  epilogue of units 2-13: column loop {tot[6]:.0f}, last store -> h_full arrive {tot[7]:.0f} cycles")
+  for l, v in sorted(per_layer.items()):
+    print(f"  layer {l}: {len(v)} units, mean unit to unit {np.mean([a for a, _ in v]):.0f} cycles, "
+          f"mean column loop {np.mean([b for _, b in v]):.0f} cycles")
 
 
 case("edge")
+case("edge", table=True)
 case("node")
