@@ -790,6 +790,8 @@ int segment_sum_launch(const float* msg, int32_t ld_msg, const int32_t* row_ptr,
   GCB_CHECK_ARG(num_heavy >= 0 && (num_heavy == 0 || heavy != nullptr), "heavy list is null");
   GCB_CHECK_ARG(width == 512, "segment_sum supports width 512");
   GCB_CHECK_ARG(ld_msg % 4 == 0 && ld_out % 4 == 0 && aligned16(msg) && aligned16(out), "unaligned");
+  GCB_CHECK_ARG(ld_msg >= width && ld_out >= width, "ld_msg and ld_out must be >= width");
+  GCB_CHECK_ARG(num_nodes >= 0, "num_nodes < 0");
   if (num_nodes == 0) return GCB_OK;
   const int warps_per_block = 8;
   long long blocks = (static_cast<long long>(num_nodes) + warps_per_block - 1) / warps_per_block;
@@ -1078,7 +1080,8 @@ int rowwise_launch(int mode, const float* dy, int32_t ld_dy, const float* z, int
                    const float* scale, int64_t rows, int32_t n, float* dz, int32_t ld_dz,
                    void* workspace, int64_t workspace_bytes, float* const* sums, int nsums,
                    int32_t accumulate, void* stream) {
-  GCB_CHECK_ARG(dy && workspace && rows >= 0, "null pointer");
+  GCB_CHECK_ARG(dy && workspace, "null pointer");
+  GCB_CHECK_ARG(rows >= 0, "rows < 0");
   GCB_CHECK_ARG(n == 256 || n == 512, "n must be 256 or 512");
   GCB_CHECK_ARG(ld_dy >= n && (!z || ld_z >= n) && (!dz || ld_dz >= n), "leading dimension < n");
   GCB_CHECK_ARG(workspace_bytes >= gcb_rowwise_workspace_bytes(n), "workspace too small");
@@ -1269,6 +1272,8 @@ int gcb_segment_sum_sorted(const float* msg, int32_t ld_msg, const int32_t* orde
   GCB_CHECK_ARG(num_heavy >= 0 && (num_heavy == 0 || heavy != nullptr), "heavy list is null");
   GCB_CHECK_ARG(width == 512, "segment_sum_sorted supports width 512");
   GCB_CHECK_ARG(ld_msg % 4 == 0 && ld_out % 4 == 0 && aligned16(msg) && aligned16(out), "unaligned");
+  GCB_CHECK_ARG(ld_msg >= width && ld_out >= width, "ld_msg and ld_out must be >= width");
+  GCB_CHECK_ARG(num_nodes >= 0, "num_nodes < 0");
   if (num_nodes == 0) return GCB_OK;
   long long light = (static_cast<long long>(num_nodes) + 7) / 8;
   const long long cap = static_cast<long long>(sm_count_cached()) * 16;

@@ -233,7 +233,8 @@ int gcb_layer_forward(const gcb_layer_desc* d, void* stream);
 
 /* out[i, :] = sum_{e in [row_ptr[i], row_ptr[i+1])} msg[e, :]   (width 512).
  * Deterministic receiver-sorted segmented sum; replaces jraph.segment_sum as
- * called from _node_update (utils/typed_graph_net.py:532-538). */
+ * called from _node_update (utils/typed_graph_net.py:532-538).  ld_msg and ld_out are multiples
+ * of 4 and >= width (16-byte rows that do not overlap), num_nodes >= 0; anything else is refused. */
 int gcb_segment_sum(const float* msg, int32_t ld_msg, const int32_t* row_ptr, int32_t num_nodes,
                     float* out, int32_t ld_out, int32_t width, void* stream);
 
@@ -486,7 +487,8 @@ int gcb_layernorm_backward_jvp(const float* dy, int32_t ld_dy, const float* z, i
  * (order / ptr: the sender CSR of an edge set, host-built), summed in j order; the rows listed in
  * `heavy` (ascending node ids; meant for the rows with many entries, e.g. the mesh nodes next to a
  * pole in mesh2grid) get one thread block each, every other row one warp.  The result does not
- * depend on the list.  Deterministic. */
+ * depend on the list.  Deterministic.  ld_msg and ld_out are multiples of 4 and >= width, num_nodes
+ * >= 0, as for gcb_segment_sum. */
 int gcb_segment_sum_sorted(const float* msg, int32_t ld_msg, const int32_t* order,
                            const int32_t* ptr, int32_t num_nodes, const int32_t* heavy,
                            int32_t num_heavy, float* out, int32_t ld_out, int32_t width, void* stream);

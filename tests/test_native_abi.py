@@ -224,6 +224,225 @@ def test_chain_refusals_name_the_unsupported_case():
   refused(chain(swish_kept, dict(rk, reads=(0,), residual_keep=1, out=256)), bad_keep)
 
 
+def _refuser(lib, fn):
+  """(refused, accepted) checkers of one entry point called with keyword overrides of its defaults."""
+  def refused(why, **kw):
+    assert fn(**kw) == -1, (why, kw)
+    assert why in lib.gcb_last_error(), (lib.gcb_last_error(), kw)
+
+  def accepted(**kw):
+    assert fn(**kw) == 0, (lib.gcb_last_error(), kw)
+  return refused, accepted
+
+
+def test_backward_kernel_refusals_name_the_unsupported_case():
+  """Refusals of the backward, tangent and HVP row kernels and the index operations: status -1, and
+  gcb_last_error says why.  The pointers are dummies and rows / nodes = 0: the direction kernels, the
+  index operations and gcb_swish_rows return without a launch once their checks pass, so the
+  accepted cases do no device work.  gcb_weight_grad and the column-sum kernels launch even at
+  rows = 0, so only their refusals are called here."""
+  lib = _native.lib()
+  P = 256                                   # a dummy, 16-byte aligned device address
+
+  def wgrad(x=P, ld_x=64, k_valid=64, x_img=None, swish=0, g=P, ld_g=64, rows=0, k=64, n=64,
+            prec=_native.PREC_BF16X3, ws=P, ws_bytes=None, dw=P, acc=0):
+    ws_bytes = lib.gcb_weight_grad_workspace_bytes(k, n) if ws_bytes is None else ws_bytes
+    return lib.gcb_weight_grad(x, ld_x, k_valid, x_img, swish, g, ld_g, rows, k, n, prec, ws, ws_bytes,
+                               dw, acc, None)
+
+  refused, _ = _refuser(lib, wgrad)
+  shape = b"k must be a multiple of 16, n of 64"
+  refused(shape, k=24, k_valid=24, ld_x=24)
+  refused(shape, n=96, ld_g=96)
+  refused(shape, n=0, ld_g=64)
+  refused(b"rows < 0", rows=-1)
+  refused(b"G must have 16-byte rows and ld_g >= n", ld_g=60)
+  refused(b"G must have 16-byte rows and ld_g >= n", ld_g=66)
+  table = b"x must have 16-byte rows, k_valid a multiple of 4 in (0, k]"
+  refused(table, k_valid=6, ld_x=8)
+  refused(table, k_valid=80, ld_x=80)
+  refused(table, k_valid=0)
+  refused(table, ld_x=60)
+  refused(table, ld_x=66)
+  refused(table, x=None)
+  refused(b"weight gradients support the tensor-core precisions only", prec=_native.PREC_FP32_SIMT)
+  refused(b"workspace too small", ws_bytes=lib.gcb_weight_grad_workspace_bytes(64, 64) - 1)
+  refused(b"workspace too small", k=64, n=128, ld_g=128, ws_bytes=lib.gcb_weight_grad_workspace_bytes(64, 64))
+  refused(b"x_img unaligned", x=None, x_img=P + 8)
+
+  nb = lambda n: lib.gcb_rowwise_workspace_bytes(n)
+
+  def ln_bwd(dy=P, ld_dy=512, z=P, ld_z=512, scale=P, rows=0, n=512, dz=P, ld_dz=512, ws=P,
+             ws_bytes=None, sums=(P, P, P)):
+    return lib.gcb_layernorm_backward(dy, ld_dy, z, ld_z, scale, rows, n, dz, ld_dz, ws,
+                                      nb(n) if ws_bytes is None else ws_bytes, *sums, 0, None)
+
+  refused, _ = _refuser(lib, ln_bwd)
+  refused(b"the LayerNorm backward needs n = 512", n=256, ld_dy=256, ld_z=256, ld_dz=256)
+  refused(b"n must be 256 or 512", n=384, ld_dy=384, ld_z=384, ld_dz=384)
+  refused(b"n must be 256 or 512", scale=None, z=None, n=128, ld_dy=128, ld_dz=128)
+  refused(b"rows < 0", rows=-1)
+  for ld in ("ld_dy", "ld_z", "ld_dz"):
+    refused(b"leading dimension < n", **{ld: 508})
+  refused(b"leading dimension < n", scale=None, z=None, n=256, ld_dy=256, ld_dz=252)
+  refused(b"workspace too small", ws_bytes=nb(512) - 1)
+  refused(b"the LayerNorm backward needs z and dz", dz=None)
+  refused(b"the LayerNorm backward needs z and dz", z=None)
+  refused(b"null column-sum output", sums=(P, None, P))
+  refused(b"null column-sum output", scale=None, z=None, sums=(None, None, None))
+  refused(b"null pointer", ws=None)
+
+  def swish_bwd(da=P, ld_da=256, h=P, ld_h=256, rows=0, n=256, dh=P, ld_dh=256, ws=P, ws_bytes=None,
+                dbias=P):
+    return lib.gcb_swish_backward(da, ld_da, h, ld_h, rows, n, dh, ld_dh, ws,
+                                  nb(n) if ws_bytes is None else ws_bytes, dbias, 0, None)
+
+  refused, _ = _refuser(lib, swish_bwd)
+  refused(b"n must be 256 or 512", n=128, ld_da=128, ld_h=128, ld_dh=128)
+  for ld in ("ld_da", "ld_h", "ld_dh"):
+    refused(b"leading dimension < n", **{ld: 252})
+  refused(b"null pointer", h=None)
+  refused(b"null pointer", dh=None)
+  refused(b"workspace too small", n=512, ld_da=512, ld_h=512, ld_dh=512, ws_bytes=nb(256))
+  refused(b"null column-sum output", dbias=None)
+
+  # ---- direction kernels: rows = 0 returns without a launch --------------------------------------
+  def swish_jvp(h=P, ld_h=256, rows=0, n=256, dh=P, ld_dh=256, stride=0, dirs=1, da=P, ld_da=256):
+    return lib.gcb_swish_jvp(h, ld_h, rows, n, dh, ld_dh, stride, dirs, da, ld_da, None)
+
+  refused, accepted = _refuser(lib, swish_jvp)
+  dirs_msg = b"rows < 0, dirs < 1 or dir_stride < rows"
+  refused(dirs_msg, dirs=0)
+  refused(dirs_msg, dirs=2, stride=-1)
+  refused(dirs_msg, rows=-1)
+  accepted(dirs=1, stride=-1)                     # ignored for one direction
+  accepted(dirs=3, stride=0)
+  ld_msg = b"n / leading dimensions must be multiples of 4 with 16-byte rows"
+  refused(ld_msg, n=254)
+  for ld in ("ld_h", "ld_dh", "ld_da"):
+    refused(ld_msg, **{ld: 252})
+    refused(ld_msg, **{ld: 258})
+  refused(ld_msg, dh=P + 4)
+  refused(b"null pointer", da=None)
+
+  def ln_jvp(z=P, ld_z=512, dz=P, ld_dz=512, scale=P, rows=0, n=512, res=None, ld_res=0, out=P,
+             ld_out=512):
+    return lib.gcb_layernorm_jvp(z, ld_z, dz, ld_dz, scale, rows, n, res, ld_res, out, ld_out, None)
+
+  refused, accepted = _refuser(lib, ln_jvp)
+  refused(b"the LayerNorm tangent needs n = 512", n=256, ld_z=256, ld_dz=256, ld_out=256)
+  for kw in (dict(ld_z=508), dict(ld_dz=508), dict(ld_out=508), dict(res=P, ld_res=508), dict(rows=-1)):
+    refused(b"rows < 0 or leading dimension < n", **kw)
+  refused(b"null pointer", scale=None)
+  accepted(res=P, ld_res=516)
+
+  def ln_jvp_dirs(z=P, ld_z=512, dz=P, ld_dz=512, scale=P, rows=0, n=512, stride=0, dirs=2, res=None,
+                  ld_res=0, out=P, ld_out=512):
+    return lib.gcb_layernorm_jvp_dirs(z, ld_z, dz, ld_dz, scale, rows, n, stride, dirs, res, ld_res,
+                                      out, ld_out, None)
+
+  refused, accepted = _refuser(lib, ln_jvp_dirs)
+  refused(b"the LayerNorm tangent needs n = 512", n=256, ld_z=256, ld_dz=256, ld_out=256)
+  refused(b"dirs < 1 or dir_stride < rows", dirs=0)
+  refused(b"dirs < 1 or dir_stride < rows", stride=-1)
+  refused(b"rows < 0 or leading dimension < n", ld_out=508)
+  refused(b"rows < 0 or leading dimension < n", res=P, ld_res=500)
+  accepted(dirs=1, stride=-1)
+  accepted(dirs=3, stride=5, res=P, ld_res=512)
+
+  def ln_bwd_dirs(dy=P, ld_dy=512, z=P, ld_z=512, scale=P, rows=0, n=512, stride=0, dirs=2, dz=P,
+                  ld_dz=512):
+    return lib.gcb_layernorm_backward_dirs(dy, ld_dy, z, ld_z, scale, rows, n, stride, dirs, dz, ld_dz,
+                                           None)
+
+  refused, accepted = _refuser(lib, ln_bwd_dirs)
+  refused(b"the LayerNorm backward of several directions needs n = 512", n=256, ld_dy=256, ld_z=256,
+          ld_dz=256)
+  refused(b"dirs < 1 or dir_stride < rows", dirs=0)
+  refused(b"dirs < 1 or dir_stride < rows", stride=-1)
+  for ld in ("ld_dy", "ld_z", "ld_dz"):
+    refused(b"rows < 0 or leading dimension < n", **{ld: 508})
+  refused(b"null pointer", scale=None)
+  accepted(dirs=1, stride=-1)
+  accepted(dirs=3, stride=7)
+
+  def swish_hvp(h=P, ld_h=256, hdot=P, ld_hdot=256, rows=0, n=256, da=P, ld_da=256, stride=0, dh=P,
+                ld_dh=256, tangents=1):
+    return lib.gcb_swish_backward_jvp_dirs(h, ld_h, hdot, ld_hdot, rows, n, da, ld_da, stride, dh, ld_dh,
+                                           tangents, None)
+
+  refused, accepted = _refuser(lib, swish_hvp)
+  refused(b"tangents < 1", tangents=0)
+  refused(b"rows < 0 or dir_stride < rows", stride=-1)
+  refused(b"rows < 0 or dir_stride < rows", rows=-1)
+  for ld in ("ld_h", "ld_hdot", "ld_da", "ld_dh"):
+    refused(ld_msg, **{ld: 252})
+  refused(ld_msg, n=6)
+  refused(b"null pointer", hdot=None)
+  accepted(tangents=3, stride=9)
+
+  def ln_hvp(dy=P, ld_dy=512, z=P, ld_z=512, zdot=P, ld_zdot=512, scale=P, rows=0, n=512, stride=0,
+             dz=P, ld_dz=512, tangents=1):
+    return lib.gcb_layernorm_backward_jvp_dirs(dy, ld_dy, z, ld_z, zdot, ld_zdot, scale, rows, n, stride,
+                                               dz, ld_dz, tangents, None)
+
+  refused, accepted = _refuser(lib, ln_hvp)
+  refused(b"the LayerNorm backward tangent needs n = 512", n=256, ld_dy=256, ld_z=256, ld_zdot=256,
+          ld_dz=256)
+  refused(b"tangents < 1", tangents=0)
+  refused(b"dir_stride < rows", stride=-1)
+  for ld in ("ld_dy", "ld_z", "ld_zdot", "ld_dz"):
+    refused(b"rows < 0 or leading dimension < n", **{ld: 508})
+  refused(b"null pointer", zdot=None)
+  accepted(tangents=3, stride=0)
+
+  def swish_rows(h=P, ld_h=256, rows=0, n=256, a=P, ld_a=256):
+    return lib.gcb_swish_rows(h, ld_h, rows, n, a, ld_a, None)
+
+  refused, accepted = _refuser(lib, swish_rows)
+  refused(ld_msg, ld_a=252)
+  refused(ld_msg, ld_h=258)
+  refused(ld_msg, n=0)
+  accepted(ld_h=260, ld_a=260)
+
+  def gather(src=P, ld_src=512, idx=P, n=0, add=None, ld_add=0, dst=P, ld_dst=512, width=512):
+    return lib.gcb_gather_add(src, ld_src, idx, n, add, ld_add, dst, ld_dst, width, None)
+
+  refused, accepted = _refuser(lib, gather)
+  gather_msg = b"width / leading dimensions must be multiples of 4 with 16-byte rows"
+  refused(gather_msg, width=6)
+  refused(gather_msg, ld_src=508)
+  refused(gather_msg, ld_dst=508)
+  refused(gather_msg, width=4, ld_dst=2)
+  refused(b"addend unaligned", add=P, ld_add=508)
+  accepted(width=4, ld_src=4, ld_dst=4)
+  accepted(width=252, ld_src=256, ld_dst=256, add=P, ld_add=252)
+
+  # ---- index operations: num_nodes = 0 returns without a launch ----------------------------------
+  def sorted_sum(msg=P, ld_msg=512, order=P, ptr=P, nodes=0, heavy=None, nheavy=0, out=P, ld_out=512,
+                 width=512):
+    return lib.gcb_segment_sum_sorted(msg, ld_msg, order, ptr, nodes, heavy, nheavy, out, ld_out, width,
+                                      None)
+
+  def receiver_sum(msg=P, ld_msg=512, ptr=P, nodes=0, heavy=None, nheavy=0, out=P, ld_out=512,
+                   width=512):
+    return lib.gcb_segment_sum_heavy(msg, ld_msg, ptr, nodes, heavy, nheavy, out, ld_out, width, None)
+
+  for fn in (sorted_sum, receiver_sum):
+    refused, accepted = _refuser(lib, fn)
+    # rows narrower than the 512 summed columns would overlap, and their writes race
+    refused(b"ld_msg and ld_out must be >= width", ld_out=508)
+    refused(b"ld_msg and ld_out must be >= width", ld_out=256)
+    refused(b"ld_msg and ld_out must be >= width", ld_msg=508)
+    refused(b"num_nodes < 0", nodes=-1)
+    refused(b"num_nodes < 0", nodes=-8)
+    refused(b"heavy list is null", nheavy=2)
+    refused(b"unaligned", ld_out=514)
+    refused(b"supports width 512", width=256, ld_msg=256, ld_out=256)
+    accepted(ld_msg=516, ld_out=516)
+    accepted(heavy=P, nheavy=3)
+
+
 def test_debug_flags_accepts_only_zero():
   """The build has no kernel experiment switches: 0 is accepted, anything else is an error."""
   lib = _native.lib()
