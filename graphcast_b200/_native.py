@@ -182,6 +182,10 @@ EXPORTS = {
                                 C.c_int32, _fp, C.c_int32, _fp]),
     "gcb_layernorm_jvp_dirs": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, _fp, C.c_int64, C.c_int32,
                                          C.c_int64, C.c_int32, _fp, C.c_int32, _fp, C.c_int32, _fp]),
+    "gcb_layernorm_jvp_params": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, _fp, C.c_int64, C.c_int32,
+                                           _fp, C.c_int32, _fp, _fp, _fp, C.c_int32, _fp]),
+    "gcb_output_loss_gn_seed": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp,
+                                          _fp, C.c_int32, _fp]),
     "gcb_layernorm_backward_dirs": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, _fp, C.c_int64,
                                               C.c_int32, C.c_int64, C.c_int32, _fp, C.c_int32, _fp]),
     "gcb_swish_backward_jvp": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, C.c_int64, C.c_int32, _fp,

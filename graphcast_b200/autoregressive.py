@@ -27,6 +27,8 @@ graphcast_b200/feedback.py and DESIGN.md section 3.5.
 
 `input_jvp` (the tangent-linear forecast, `jax.jvp` of the unroll) runs forward with the rollout: each
 step's tangent planes are fed on the device from the step before, so it needs no checkpointing.
+`param_jvp` (its derivative with respect to the parameters) runs the same rollout from zero input
+tangents, every step adding its weight-tangent terms.
 
 Input noise (`noise_level`, :63-86 and :238-249) applies where the reference applies it: in `loss`,
 `loss_and_grads` and `loss_and_input_grads` with several target times, once, to the time-dependent
@@ -492,20 +494,48 @@ class Predictor(graphcast.Predictor):
     return graphcast.batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
                                  directions_per_pass)
 
+  def param_jvp(self, inputs, targets_template, forcings, param_tangents, **kwargs):
+    """(predictions, prediction_tangents): `predictions` as __call__ returns them, their derivative
+    along the parameter tangents (GraphCast.param_jvp) over every target time.  One target time
+    delegates to the inner predictor.  Several run forward with the rollout, step by step, as input_jvp
+    does (no gradient_checkpointing needed, nothing kept per step): step t > 0 gets the fed-back
+    prediction tangent as its input tangent, plus its own weight-tangent terms."""
+    inputs, targets_template = xs.from_xarray(inputs), xs.from_xarray(targets_template)
+    forcings = xs.from_xarray(forcings)
+    if targets_template.sizes["time"] == 1:
+      return self._predictor.param_jvp(inputs, targets_template, forcings, param_tangents, **kwargs)
+    return self._tangent_rollout(inputs, targets_template, forcings, None, None, directions=False,
+                                 param_tangents=param_tangents)
+
+  def loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents, **kwargs):
+    """(loss, diagnostics, gnvp) of one target time (GraphCast.loss_and_param_gnvp), delegated to the
+    inner predictor; Gauss-Newton products over several target times are not provided."""
+    targets = xs.from_xarray(targets)
+    if targets.sizes["time"] != 1:
+      raise NotImplementedError("Gauss-Newton products cover one target time (several are not "
+                                "provided)")
+    return self._predictor.loss_and_param_gnvp(inputs, targets, forcings, param_tangents, **kwargs)
+
   def _tangent_rollout(self, inputs, targets_template, forcings, input_tangents, forcing_tangents,
-                       directions: bool):
-    """input_jvp (batched_input_jvp with `directions`) over several target times."""
+                       directions: bool, param_tangents=None):
+    """input_jvp (batched_input_jvp with `directions`, param_jvp with `param_tangents`) over several
+    target times."""
+    what = "input_jvp" if param_tangents is None else "param_jvp"
     parts = self._device_parts()
     if parts is None:
-      raise NotImplementedError("input_jvp over several target times needs a GraphCast predictor, "
+      raise NotImplementedError(f"{what} over several target times needs a GraphCast predictor, "
                                 "directly or inside InputsAndResiduals (the fused normalisation)")
     self._validate(inputs, targets_template, forcings)
     model, norm_of = parts
     num_steps = targets_template.sizes["time"]
     one = lambda ds: ds.isel(time=slice(0, 1))
-    run = graphcast._TangentRun(inputs, forcings, input_tangents, forcing_tangents, num_steps,
-                                feedback.FeedbackPlan(inputs, one(targets_template), one(forcings)),
-                                directions=directions)
+    plan = feedback.FeedbackPlan(inputs, one(targets_template), one(forcings))
+    if param_tangents is None:
+      run = graphcast._TangentRun(inputs, forcings, input_tangents, forcing_tangents, num_steps, plan,
+                                  directions=directions)
+    else:
+      run = model._param_tangent_run(inputs, targets_template, forcings, param_tangents, num_steps,
+                                     plan)
     tangents = []
 
     def step(rng, inputs, targets_template, forcings):

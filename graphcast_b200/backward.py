@@ -24,6 +24,9 @@ same helpers (Backward.tangent): each stage of the stage-wise forward is followe
 MLP's tangent formed at its recomputed h and z (mlp_jvp; gcb_swish_jvp and gcb_layernorm_jvp_dirs for
 the two nonlinearities).  Several tangent directions share that walk: their state is stacked
 direction-major, so every tangent GEMM runs once over all of them and h and z are recomputed once.
+Tangents along the parameters (param_jvp) walk the same graph with packed tangent weight images
+(weight_tangents): every layer with one adds its weight-tangent GEMM X W-dot + b-dot at the primal
+rows, and every LayerNorm scale-dot * zhat + offset-dot (gcb_layernorm_jvp_params).
 Several cotangents (batched_input_vjp) share the backward walk the same way: element(dirs=K) stacks the
 gradient state like the tangent's, runs every dX product once over all directions, and differentiates
 the two nonlinearities with gcb_layernorm_backward_dirs and gcb_swish_jvp.
@@ -61,6 +64,17 @@ class _MlpInfo:
     self.n1, self.n1_valid, self.split = n1, n1_valid, split
     self.g: Dict[str, torch.Tensor] = {}
     self.t: Dict[str, torch.Tensor] = {}     # transposed packed weights
+
+
+class _WeightTangent:
+  """The tangent of one MLP's parameters (param_jvp), packed as the engine packs its weights
+  (Backward.weight_tangents): the tangent weight images at the engine's precision with the primal's
+  padding, for a pre-gathered edge layer its split blocks (`split`: we / ws / wr) in place of w0, and the
+  padded tangent biases and LayerNorm vectors.  A layer with no tangent has w0 / split / w1 None (a
+  tangent bias alone comes with a zero weight image); a LayerNorm field with no tangent is None."""
+
+  def __init__(self):
+    self.w0 = self.split = self.b0 = self.w1 = self.b1 = self.scale = self.offset = None
 
 
 class Backward:
@@ -140,6 +154,8 @@ class Backward:
     self.hvp, self.tdirs = None, 0
     self.sink = {f: torch.zeros([D], dtype=torch.float32, device=dev)
                  for f in ("b0", "b1", "scale", "offset")}
+    # tangent(wts=...): the packed parameter tangents of param_jvp, {MLP stem: _WeightTangent}
+    self.wts: Dict[str, _WeightTangent] = {}
 
   # -- setup ---------------------------------------------------------------------------------
   def _i32(self, a):
@@ -193,6 +209,50 @@ class Backward:
       self._pack_t(info, "w0_0", w.w0_f32, D, D, D, D)
     if "w0_in" in info.t:                                  # the grid embedder's input transpose
       self._pack_t(info, "w0_in", w.w0_f32, D, D, self.n_in_t, self.eng.c_in_pad)
+
+  def weight_tangents(self, tangents) -> Dict[str, _WeightTangent]:
+    """Packs parameter tangents, device fp32 tensors keyed and shaped like the params (modules and
+    fields may be left out: zero), into tangent weight images on the current stream, with the padding
+    and split blocks of the engine's own (Engine._make_mlp, _make_split).  MLPs with no tangent at all
+    are absent, so their tangent GEMMs are skipped; the mesh2grid mesh-node MLP, which the step never
+    reads, is never packed.  The engine's weights are not touched."""
+    zeros = lambda *s: torch.zeros(list(s), dtype=torch.float32, device=self.dev)
+    image = lambda k, n: torch.zeros([self.lib.gcb_packed_weight_bytes(k, n)], dtype=torch.uint8,
+                                     device=self.dev)
+    out = {}
+    for info in self._all:
+      l0, l1 = f"{info.stem}_mlp/~/linear_0", f"{info.stem}_mlp/~/linear_1"
+      t0, t1 = tangents.get(l0, {}), tangents.get(l1, {})
+      tn = tangents.get(f"{info.stem}_layer_norm", {}) if info.ln else {}
+      if not (t0 or t1 or tn):
+        continue
+      wt = _WeightTangent()
+      if t0:
+        w = t0["w"] if "w" in t0 else zeros(*self.shapes[l0]["w"])
+        if info.split is not None:           # row blocks [edge | sender | receiver], each packed alone
+          wt.split = {}
+          for i, name in enumerate(("we", "ws", "wr")):
+            wt.split[name] = image(D, D)
+            self.eng.pack_weight(w.data_ptr() + 4 * i * D * D, D, False, D, D, D, D, wt.split[name])
+        else:
+          seg_real = [w.shape[0]] if len(info.k_segs) == 1 else info.k_segs
+          wt.w0 = image(sum(info.k_segs), D)
+          self.eng._pack_linear_device(w, seg_real, info.k_segs, wt.w0, zeros(sum(info.k_segs), D))
+        wt.b0 = t0["b"] if "b" in t0 else zeros(D)
+      if t1:
+        w = t1["w"] if "w" in t1 else zeros(*self.shapes[l1]["w"])
+        wt.w1 = image(D, info.n1)
+        self.eng._pack_linear_device(w, [D], [D], wt.w1, zeros(D, info.n1))
+        wt.b1 = zeros(info.n1)
+        if "b" in t1:
+          wt.b1[:info.n1_valid].copy_(t1["b"])
+      for f in ("scale", "offset"):
+        if f in tn:
+          v = zeros(info.n1)
+          v[:info.n1_valid].copy_(tn[f])
+          setattr(wt, f, v)
+      out[info.stem] = wt
+    return out
 
   def repack(self, stems=None) -> None:
     """The engine's weights were rewritten (Engine.load_params / load_params_device): repacks the
@@ -264,8 +324,9 @@ class Backward:
     d.precision = self.prec
     if pre is not None:
       d.n_pre_add = len(pre)
-      for i, (table, idx) in enumerate(pre):
-        d.pre_add[i].table, d.pre_add[i].idx, d.pre_add[i].ld = table.data_ptr(), idx.data_ptr(), D
+      for i, (table, idx) in enumerate(pre):             # idx None: row r adds row r of the table
+        d.pre_add[i].table, d.pre_add[i].idx = table.data_ptr(), None if idx is None else idx.data_ptr()
+        d.pre_add[i].ld = table.shape[1]
     _native.check(self.lib.gcb_layer_forward(C.byref(d), self._st()), "gcb_layer_forward")
 
   def empty(self, rows: int, cols: int = D) -> torch.Tensor:
@@ -762,27 +823,52 @@ class Backward:
     weight dw0 (default: that of the primal, w0) and the pre-gathered addends `dpre` (K-fold indices);
     with no dsegs the addends alone are the pre-activation tangent.  Tangents are stacked tables of
     self.dirs directions of `rows` rows.  Returns residual + dy (LayerNorm MLPs) or dy [., n1] (the
-    decoder)."""
+    decoder).
+
+    With a parameter tangent of this MLP in self.wts (param_jvp, one direction), each layer also gets
+    its weight-tangent term, one GEMM at the primal rows with the previous tangent as an identity
+    pre-gathered addend: h-dot = X-dot W0 + X W0-dot + b0-dot (for a pre-gathered edge layer X is the
+    edge segment and W0-dot its block we; the node blocks' terms come in dpre), z-dot = a-dot W1 +
+    a W1-dot + b1-dot, and the LayerNorm adds scale-dot * zhat + offset-dot (gcb_layernorm_jvp_params).
+    A layer without a tangent runs exactly what it runs without self.wts."""
     w = info.w
     w0 = w0 or w.w0_packed
+    wt = self.wts.get(info.stem)
+    t0 = None if wt is None else (wt.split["we"] if wt.split is not None else wt.w0)
     nd, stride, rk = self.dirs, self.dir_stride(rows), self.dir_rows(rows)
+    dh = None
     if dsegs:
       dh = self.empty(rk)
       self.layer(rk, dsegs, dw0 or w0, self.zero_bias, out_y=dh, pre=list(dpre) or None)
+      dpre = ()
+    if t0 is not None:                       # + X W0-dot + b0-dot (and the addends not yet added)
+      pre_t = list(dpre) + ([] if dh is None else [(dh, None)])
+      dht = self.empty(rows)
+      self.layer(rows, segs, t0, wt.b0, out_y=dht, pre=pre_t or None)
+      dh = dht
     else:
-      dh = None
       for table, idx in dpre:
         dh = self.gather_add(table, idx, rk, dh)
+      if dh is None:                         # neither the input nor the first layer has a tangent
+        dh = torch.zeros([max(rk, 1), D], dtype=torch.float32, device=self.dev)
     h = self.empty(rows)
     self.layer(rows, segs, w0, w.b0, _native.ACT_NONE, out_y=h, pre=pre)
     da = dh                                  # swish'(h) dh in place: the Jacobian of swish is diagonal
     _native.check(self.lib.gcb_swish_jvp(h.data_ptr(), D, rows, D, dh.data_ptr(), D, stride, nd,
                                          da.data_ptr(), D, self._st()), "gcb_swish_jvp")
     del dh
+    t1 = None if wt is None else wt.w1
     if not info.ln:
       dy = self.empty(rk, info.n1)
       self.layer(rk, [self.tab(da)], w.w1_packed, self.zero_bias, out_y=dy, n=info.n1,
                  n_valid=info.n1_valid)
+      if t1 is not None:                     # + a W1-dot + b1-dot (padded columns: zero weights)
+        a = self.empty(rows)
+        _native.check(self.lib.gcb_swish_rows(h.data_ptr(), D, rows, D, a.data_ptr(), D, self._st()),
+                      "gcb_swish_rows")
+        dyt = self.empty(rows, info.n1)
+        self.layer(rows, [self.tab(a)], t1, wt.b1, out_y=dyt, pre=[(dy, None)], n=info.n1)
+        dy = dyt
       return dy
     a = self.empty(rows)
     _native.check(self.lib.gcb_swish_rows(h.data_ptr(), D, rows, D, a.data_ptr(), D, self._st()),
@@ -790,15 +876,46 @@ class Backward:
     del h
     z = self.empty(rows)
     self.layer(rows, [self.tab(a)], w.w1_packed, w.b1, out_y=z)
-    del a
+    if t1 is None:
+      del a
     dz = self.empty(rk)
     self.layer(rk, [self.tab(da)], w.w1_packed, self.zero_bias, out_y=dz)
     del da
+    if t1 is not None:                       # + a W1-dot + b1-dot
+      dzt = self.empty(rows)
+      self.layer(rows, [self.tab(a)], t1, wt.b1, out_y=dzt, pre=[(dz, None)])
+      dz = dzt
+      del a
     out = self.empty(rk)
+    if wt is not None and (wt.scale is not None or wt.offset is not None):
+      _native.check(self.lib.gcb_layernorm_jvp_params(
+          z.data_ptr(), D, dz.data_ptr(), D, w.ln_scale, rows, D, self._ptr(residual), D,
+          self._ptr(wt.scale), self._ptr(wt.offset), out.data_ptr(), D, self._st()),
+          "gcb_layernorm_jvp_params")
+      return out
     _native.check(self.lib.gcb_layernorm_jvp_dirs(
         z.data_ptr(), D, dz.data_ptr(), D, w.ln_scale, rows, D, stride, nd, self._ptr(residual), D,
         out.data_ptr(), D, self._st()), "gcb_layernorm_jvp_dirs")
     return out
+
+  def proj_tangent(self, rows: int, v, dv: Optional[torch.Tensor], w_packed, tw_packed):
+    """Tangent of a node projection v W (a pre-gathered edge layer's sender or receiver block), a
+    stacked table of self.dirs directions of `rows` rows: dv W + v W-dot, each term only when its
+    tangent exists (dv, the image tw_packed of W-dot); None when neither does."""
+    out = None
+    if dv is not None:
+      out = self.projection(self.dir_rows(rows), self.tab(dv), w_packed)
+    if tw_packed is not None:
+      t = self.empty(rows)
+      self.layer(rows, [v], tw_packed, self.zero_bias, out_y=t,
+                 pre=None if out is None else [(out, None)])
+      out = t
+    return out
+
+  def _split_tangent(self, info: _MlpInfo, name: str):
+    """The image of the tangent of split block `name` (ws | wr) of an edge MLP, or None."""
+    wt = self.wts.get(info.stem)
+    return None if wt is None or wt.split is None else wt.split[name]
 
   @staticmethod
   def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -820,31 +937,35 @@ class Backward:
                     snd: torch.Tensor, rcv: torch.Tensor, v_s, n_s: int, v_r, n_r: int,
                     dv_s: torch.Tensor, dv_r: Optional[torch.Tensor]) -> torch.Tensor:
     """Tangent of the receiver sums of a grid2mesh / mesh2grid edge MLP m = MLP([e | v_s[snd] |
-    v_r[rcv]]) with e = MLP(edge features) (no tangent), chunk by chunk (tangent_chunks): dagg (n_r
-    rows per direction), from the stacked sender and (when dv_r is given) receiver node tangents."""
+    v_r[rcv]]) with e = MLP(edge features), chunk by chunk (tangent_chunks): dagg (n_r rows per
+    direction), from the stacked sender and (when dv_r is given) receiver node tangents.  e has a tangent
+    only through the edge embedder's parameters (self.wts), and so do the node blocks' W_s, W_r."""
     sp = info.split
     ps = self.projection(n_s, v_s, sp.ws_packed)
     pr = self.projection(n_r, v_r, sp.wr_packed)
-    dps = self.projection(self.dir_rows(n_s), self.tab(dv_s), sp.ws_packed)
-    dpr = None if dv_r is None else self.projection(self.dir_rows(n_r), self.tab(dv_r), sp.wr_packed)
+    dps = self.proj_tangent(n_s, v_s, dv_s, sp.ws_packed, self._split_tangent(info, "ws"))
+    dpr = self.proj_tangent(n_r, v_r, dv_r, sp.wr_packed, self._split_tangent(info, "wr"))
+    enc_t = enc.stem in self.wts
     dagg = self.empty(self.dir_rows(n_r))
     for i, (r0, r1, g0, g1, rp, heavy, n_heavy, _) in enumerate(self.tangent_chunks(name)):
       n = r1 - r0
       f = self.tab(feat_t[r0:r1], 16, 4, 4)                 # 16-byte rows: the view stays aligned
       snd_c, rcv_c = snd[r0:r1].clone(), rcv[r0:r1].clone()  # index arrays from an aligned base
       e = self.fwd_mlp(enc, n, [f])
+      de = self.mlp_jvp(enc, n, [f], []) if enc_t else None
       dpre = [(dps, self.kfold(snd_c, n_s, (name, "tangent", i, "snd")))]
       if dpr is not None:
         dpre.append((dpr, self.kfold(rcv_c, n_r, (name, "tangent", i, "rcv"))))
-      dm = self.mlp_jvp(info, n, [self.tab(e)], [], pre=[(ps, snd_c), (pr, rcv_c)], dpre=dpre,
-                        w0=sp.we_packed)
-      del e
+      dm = self.mlp_jvp(info, n, [self.tab(e)], [] if de is None else [self.tab(de)],
+                        pre=[(ps, snd_c), (pr, rcv_c)], dpre=dpre, w0=sp.we_packed)
+      del e, de
       self.receiver_sums(dm, n, rp, g1 - g0, dagg[g0:], self.dir_stride(n_r), heavy, n_heavy)
       del dm
     return dagg
 
   def tangent(self, grid_in_img: torch.Tensor, dgrid_in_img: torch.Tensor, dirs: int = 1,
-              snaps: Optional[dict] = None, tsnaps: Optional[dict] = None) -> torch.Tensor:
+              snaps: Optional[dict] = None, tsnaps: Optional[dict] = None,
+              wts: Optional[Dict[str, _WeightTangent]] = None) -> torch.Tensor:
     """One step stage by stage (Engine.run_stage, from the packed inputs grid_in_img) and, interleaved
     with it, its tangent along `dirs` directions at once: dgrid_in_img is the stacked operand image of
     the packed input tangents ([Ng, c_in_pad] per direction, dir_stride(Ng) rows apart, structural
@@ -861,12 +982,20 @@ class Backward:
     agg-dot_k, and the v-dot / agg-dot of the grid and mesh nodes around the encoder and decoder (vg0,
     agg1, vg1, agg3, vg2), and the packed input tangent image (grid_in).  The tangent tables are the
     stacked tables of `dirs` directions the forward forms anyway: keeping them costs no copy, and their
-    memory grows with the directions.  Without them nothing more is kept or launched."""
-    self.dirs = int(dirs)
+    memory grows with the directions.  Without them nothing more is kept or launched.
+
+    With `wts` (weight_tangents; param_jvp, one direction, no snapshots) the tangent is also along those
+    parameter tangents: every MLP with one adds its weight-tangent terms (mlp_jvp, proj_tangent), and
+    the tangents that are zero along the inputs alone are formed when their parameters have one: the
+    mesh-node encoder's (so the grid2mesh receiver block and the mesh-node residual get theirs), the
+    edge embedders' and with it e_0 of the processor."""
+    if wts and (dirs != 1 or tsnaps is not None):
+      raise ValueError("parameter tangents run one direction without snapshots")
+    self.dirs, self.wts = int(dirs), wts or {}
     try:
       return self._tangent(grid_in_img, dgrid_in_img, snaps, tsnaps)
     finally:
-      self.dirs = 1
+      self.dirs, self.wts = 1, {}
 
   def _tangent(self, grid_in_img, dgrid_in_img, snaps=None, ts=None):
     eng, m = self.eng, self.m
@@ -888,12 +1017,20 @@ class Backward:
     info = mp["enc_grid"]
     dvg0 = self.mlp_jvp(info, ng, [grid_in], [img(dgrid_in_img, cin)])
     vg0 = self.fwd_mlp(info, ng, [grid_in])
-    vm0 = self.fwd_mlp(mp["enc_mesh"], nm, [img(eng.mesh_in_img, cin)])
+    mesh_in = [img(eng.mesh_in_img, cin)]
+    vm0 = self.fwd_mlp(mp["enc_mesh"], nm, mesh_in)
+    # vm0 (from the static mesh inputs) has a tangent only through the mesh-node encoder's parameters
+    dvm0 = self.mlp_jvp(mp["enc_mesh"], nm, mesh_in, []) if mp["enc_mesh"].stem in self.wts else None
     dagg = self.bipartite_jvp("g2m", mp["proc_e_g2m"], mp["enc_e_g2m"], eng.g2m_feat, eng.g2m_snd,
-                              eng.g2m_rcv, tab(vg0), ng, tab(vm0), nm, dvg0, None)
-    info = mp["proc_n_mesh_g2m"]                 # vm0 has no tangent: block 1 of W0 alone
-    dv = self.mlp_jvp(info, nm, [tab(vm0), img(eng.mesh_agg_img)], [tab(dagg)],
-                      dw0=self.w0_block(info, 1))
+                              eng.g2m_rcv, tab(vg0), ng, tab(vm0), nm, dvg0, dvm0)
+    info = mp["proc_n_mesh_g2m"]
+    if dvm0 is None:                             # vm0 has no tangent: block 1 of W0 alone
+      dv = self.mlp_jvp(info, nm, [tab(vm0), img(eng.mesh_agg_img)], [tab(dagg)],
+                        dw0=self.w0_block(info, 1))
+    else:
+      dv = self.mlp_jvp(info, nm, [tab(vm0), img(eng.mesh_agg_img)], [tab(dvm0), tab(dagg)],
+                        residual=dvm0)
+      del dvm0
     if keep:
       ts.update(vg0=dvg0, agg1=dagg)
       ts["v"].append(dv)
@@ -912,7 +1049,10 @@ class Backward:
     for k in range(K):
       v_k = eng.mesh_lat_img.clone()
       if k == 0:
-        e_k = tab(self.fwd_mlp(mp["enc_e_mesh"], m.e_mesh, [tab(eng.mesh_feat, 16, 4, 4)]))
+        feat = [tab(eng.mesh_feat, 16, 4, 4)]
+        e_k = tab(self.fwd_mlp(mp["enc_e_mesh"], m.e_mesh, feat))
+        if mp["enc_e_mesh"].stem in self.wts:    # e_0 has a tangent through the embedder's parameters
+          de = self.mlp_jvp(mp["enc_e_mesh"], m.e_mesh, feat, [])
       else:
         e_k = img(eng.mesh_edge_img.clone())
       eng.run_stage("process_step", k)
@@ -926,8 +1066,8 @@ class Backward:
       nfo, efo = self.proc_n[k], self.proc_e[k]
       sp = efo.split
       ps, pr = self.projection(nm, img(v_k), sp.ws_packed), self.projection(nm, img(v_k), sp.wr_packed)
-      dps = self.projection(self.dir_rows(nm), tab(dv), sp.ws_packed)
-      dpr = self.projection(self.dir_rows(nm), tab(dv), sp.wr_packed)
+      dps = self.proj_tangent(nm, img(v_k), dv, sp.ws_packed, self._split_tangent(efo, "ws"))
+      dpr = self.proj_tangent(nm, img(v_k), dv, sp.wr_packed, self._split_tangent(efo, "wr"))
       dpre = [(dps, snd_k), (dpr, rcv_k)]
       dm = self.mlp_jvp(efo, m.e_mesh, [e_k], [] if de is None else [tab(de)],
                         pre=[(ps, eng.mesh_snd), (pr, eng.mesh_rcv)], dpre=dpre, w0=sp.we_packed)

@@ -98,3 +98,9 @@ class Bfloat16Cast(graphcast.Predictor):
     return self._predictor.batched_input_jvp(inputs, targets_template, forcings, input_tangents,
                                              forcing_tangents, directions_per_pass=directions_per_pass,
                                              **kwargs)
+
+  def param_jvp(self, inputs, targets_template, forcings, param_tangents, **kwargs):
+    return self._predictor.param_jvp(inputs, targets_template, forcings, param_tangents, **kwargs)
+
+  def loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents, **kwargs):
+    return self._predictor.loss_and_param_gnvp(inputs, targets, forcings, param_tangents, **kwargs)

@@ -926,6 +926,22 @@ int gcb_output_loss_grad(const float* y, int32_t ld_y, int32_t n_out, int32_t n_
   return GCB_OK;
 }
 
+int gcb_output_loss_gn_seed(const float* dy, int32_t ld_dy, int32_t n_out, int32_t n_lat,
+                            int32_t n_lon, const float* lat_weight, const double* coef, float* g,
+                            int32_t ld_g, void* stream) {
+  GCB_CHECK_ARG(dy && lat_weight && coef && g, "null pointer");
+  GCB_CHECK_ARG(n_out > 0 && ld_dy >= n_out && ld_g >= n_out, "ld_dy / ld_g too small");
+  GCB_CHECK_ARG(n_lat > 0 && n_lon > 0, "empty grid");
+  const long long n_nodes = static_cast<long long>(n_lat) * n_lon;
+  const long long total = n_nodes * n_out;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0, 4.0 * static_cast<double>(total) * 2.0);
+  gcb::output_loss_gn_seed_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
+      dy, ld_dy, n_out, n_lon, n_nodes, lat_weight, coef, g, ld_g);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
 int gcb_output_loss_grad_feedback(const float* y, int32_t ld_y, int32_t n_out, int32_t n_lat,
                                   int32_t n_lon, const float* scale, const float* offset,
                                   const float* add_planes, const int32_t* add_plane_index,
@@ -1188,6 +1204,26 @@ int gcb_layernorm_jvp_dirs(const float* z, int32_t ld_z, const float* dz, int32_
                  4.0 * static_cast<double>(rows) * n * (1.0 + dirs * (2.0 + (residual ? 1.0 : 0.0))));
   gcb::layernorm_jvp_dirs_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, st>>>(
       z, ld_z, dz, ld_dz, scale, rows, dir_stride, dirs, residual, ld_res, out, ld_out);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
+int gcb_layernorm_jvp_params(const float* z, int32_t ld_z, const float* dz, int32_t ld_dz,
+                             const float* scale, int64_t rows, int32_t n, const float* residual,
+                             int32_t ld_res, const float* dscale, const float* doffset, float* out,
+                             int32_t ld_out, void* stream) {
+  GCB_CHECK_ARG(z && dz && scale && out, "null pointer");
+  GCB_CHECK_ARG(n == 512, "the LayerNorm tangent needs n = 512");
+  GCB_CHECK_ARG(rows >= 0 && ld_z >= n && ld_dz >= n && ld_out >= n && (!residual || ld_res >= n),
+                "rows < 0 or leading dimension < n");
+  if (rows == 0) return GCB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const double params = (dscale ? 1.0 : 0.0) + (doffset ? 1.0 : 0.0);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * static_cast<double>(rows) * n * (3.0 + (residual ? 1.0 : 0.0) +
+                                                        (params > 0 ? 2.0 : 0.0)) + 4.0 * n * params);
+  gcb::layernorm_jvp_params_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, st>>>(
+      z, ld_z, dz, ld_dz, scale, rows, residual, ld_res, dscale, doffset, out, ld_out);
   GCB_CUDA(cudaGetLastError());
   return GCB_OK;
 }

@@ -829,10 +829,10 @@ class Engine:
             self._ptr(fb.in_scale), a_out.data_ptr(), 1, self._stream()), "gcb_input_grad")
 
   # -- input gradients (loss_and_input_grads, input_vjp) ---------------------------------------------
-  def input_grads_begin(self) -> None:
-    """The gradient workspace of `input_grads_element`, with the checks of grads_begin; the parameter
-    accumulators are neither zeroed nor touched."""
-    self._grad_workspace(None, "input gradients")
+  def input_grads_begin(self, what: str = "input gradients") -> None:
+    """The gradient workspace of `input_grads_element`, with the checks of grads_begin (`what` names
+    the call in their messages); the parameter accumulators are neither zeroed nor touched."""
+    self._grad_workspace(None, what)
 
   def input_grads_element(self, fb: "Feedback", operands: dict, *,
                           lat_weight: Optional[torch.Tensor] = None, coef: Optional[torch.Tensor] = None,
@@ -1006,7 +1006,8 @@ class Engine:
   def input_jvp_element(self, tangent_planes: torch.Tensor, tangent_out: torch.Tensor, *,
                         in_scale: Optional[torch.Tensor] = None,
                         planes_out: Optional[torch.Tensor] = None,
-                        grid_in: Optional[torch.Tensor] = None, **affine) -> None:
+                        grid_in: Optional[torch.Tensor] = None, weight_tangents=None,
+                        **affine) -> None:
     """One step of one batch element of the tangent-linear forecast (call input_grads_begin() first):
     the step stage by stage from `grid_in` (default: the packed grid_in_img) interleaved with its
     tangent (Backward.tangent) along tangent_planes [c_in, Ng], the tangent of this step's input planes
@@ -1017,11 +1018,17 @@ class Engine:
     the physical predictions: the decoder tangent times affine["scale"] plus, through the residual add,
     tangent_planes[affine["add_plane_index"]] (gcb_unpack_grid_outputs without the offset), unpacked
     per direction.  With planes_out, the predictions as unpack_outputs gives them from the same
-    forward.  `affine`: the keywords of unpack_outputs (scale, offset, add_planes, add_plane_index)."""
+    forward.  `affine`: the keywords of unpack_outputs (scale, offset, add_planes, add_plane_index).
+
+    weight_tangents (param_jvp, one direction): packed parameter tangents (weight_tangents()), along
+    which the step's tangent also runs (Backward.tangent(wts=...)); tangent_planes is then the input
+    tangent fed back from the step before (zeros for the first step)."""
     if self._backward is None:
       raise RuntimeError("call input_grads_begin() first")
     single = tangent_planes.dim() == 2
     dirs = 1 if single else tangent_planes.shape[0]
+    if weight_tangents is not None and dirs != 1:
+      raise ValueError("parameter tangents run one direction")
     for name, t, rows in (("tangent_planes", tangent_planes, self.c_in),
                           ("tangent_out", tangent_out, self.n_out)):
       lead = () if single else (dirs,)
@@ -1043,7 +1050,7 @@ class Engine:
             p.data_ptr(), self.c_in, self.num_grid, None, self._ptr(in_scale), no_static.data_ptr(), 3,
             self.c_in_pad, dgrid_in.data_ptr() + k * img_stride, self._stream()),
             "gcb_pack_grid_image")
-      dy = self._backward.tangent(grid_in, dgrid_in, dirs)
+      dy = self._backward.tangent(grid_in, dgrid_in, dirs, wts=weight_tangents)
       del dgrid_in
       if planes_out is not None:
         self.unpack_outputs(planes_out, **affine)
@@ -1052,6 +1059,52 @@ class Engine:
             dy[k * stride:].data_ptr(), dy.shape[1], self.n_out, self.num_grid,
             self._ptr(affine.get("scale")), None, None if add_index is None else p.data_ptr(),
             self._ptr(add_index), out.data_ptr(), self._stream()), "gcb_unpack_grid_outputs")
+
+  # -- parameter tangents (param_jvp, loss_and_param_gnvp) ---------------------------------------------
+  def weight_tangents(self, param_tangents: Mapping[str, Mapping[str, np.ndarray]]):
+    """Packs parameter tangents (host float32 arrays keyed and shaped like the params, modules and
+    fields optional) into tangent weight images on the device (Backward.weight_tangents), for
+    input_jvp_element and param_gnvp_element; call input_grads_begin() or grads_begin() first.  The
+    engine's weights and weights_version are not touched."""
+    if self._backward is None:
+      raise RuntimeError("call input_grads_begin() or grads_begin() first")
+    with self._on_device():
+      dev = {name: {f: torch.as_tensor(np.ascontiguousarray(a, np.float32)).to(self.device)
+                    for f, a in fields.items()} for name, fields in param_tangents.items()}
+      return self._backward.weight_tangents(dev)
+
+  def param_gnvp_element(self, targets_planes: torch.Tensor, lat_weight: torch.Tensor,
+                         coef: torch.Tensor, weight_tangents, *, channel_sums: torch.Tensor,
+                         **affine) -> None:
+    """One batch element of a Gauss-Newton product (call grads_begin() first): the step from the
+    packed grid_in_img with its tangent along the packed parameter tangents (Backward.tangent(wts=...),
+    zero input tangent), whose decoder tangent y-dot = J v seeds g = coef * lat_weight * y-dot
+    (gcb_output_loss_gn_seed: the loss Hessian with respect to y is that diagonal).  The step then runs
+    again stage by stage with the snapshots of loss_and_grads_element, whose loss sums go to
+    channel_sums, and the backward pass from g ADDS this element's J^T H J v to the gradient
+    accumulators.  Recomputing the step rather than keeping snapshots through the tangent keeps the
+    peak that of the larger of the two passes."""
+    if self._backward is None:
+      raise RuntimeError("call grads_begin() first")
+    grid_in = self.grid_in_img
+    n_lat = lat_weight.shape[0]
+    with self._on_device():
+      dgrid_in = self._image(self.num_grid, self.c_in_pad)
+      dy = self._backward.tangent(grid_in, dgrid_in, wts=weight_tangents)
+      del dgrid_in
+      g_out = torch.zeros([self.num_grid, 256], dtype=torch.float32, device=self.device)
+      _native.check(self._lib.gcb_output_loss_gn_seed(
+          dy.data_ptr(), dy.shape[1], self.n_out, n_lat, self.num_grid // n_lat, lat_weight.data_ptr(),
+          coef.data_ptr(), g_out.data_ptr(), 256, self._stream()), "gcb_output_loss_gn_seed")
+      del dy
+    # The tangent pass leaves its blocks cached in shapes the backward pass cannot reuse: at 0.25
+    # degree the backward pass peaks within a few GiB of an 80 GB card and would not find its 1 GiB
+    # tables in them.
+    torch.cuda.empty_cache()
+    snaps = self._forward_snapshots(grid_in)
+    self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
+    with self._on_device():
+      self._backward.element(grid_in, g_out, snaps)
 
   def broadcast_grad_sum(self, a: torch.Tensor, n_lat: int, rows: torch.Tensor, mode: int,
                          out: torch.Tensor, accumulate: bool) -> None:

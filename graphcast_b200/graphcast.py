@@ -155,6 +155,18 @@ class Predictor(abc.ABC):
     the same leading dim.  directions_per_pass: directions that share one forward (None: all)."""
     raise NotImplementedError(f"{type(self).__name__} does not implement input gradients")
 
+  def param_jvp(self, inputs, targets_template, forcings, param_tangents, **optional_kwargs):
+    """Returns (predictions, prediction_tangents): the predictions of __call__ and their derivative
+    along `param_tangents`, a dict shaped like the params ({module: {field: array}}, entries left out
+    being zero), shaped like the predictions: jax.jvp of the forecast with respect to the params."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement parameter tangents")
+
+  def loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents, **optional_kwargs):
+    """Returns (loss, diagnostics, gnvp): `loss` / `diagnostics` as `loss` returns them, `gnvp` the
+    generalised Gauss-Newton matrix of loss.mean() with respect to the params times `param_tangents`,
+    a dict shaped like the params."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement parameter tangents")
+
 
 # Per-variable weights of GraphCast's loss (reference graphcast.py:341-356); others weigh 1.
 LOSS_PER_VARIABLE_WEIGHTS = {
@@ -488,6 +500,97 @@ class GraphCast(Predictor):
     return batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
                        directions_per_pass)
 
+  def param_jvp(self, inputs, targets_template, forcings, param_tangents, **unused_kwargs):
+    """(predictions, prediction_tangents) for one target time: `predictions` is what __call__ returns,
+    bit for bit; `prediction_tangents` (float32, shaped like it, physical units) is d(predictions)/d eps
+    at eps = 0 for the params + eps * param_tangents, what jax.jvp of the predictor with respect to the
+    params gives (several target times: autoregressive.Predictor).
+
+    `param_tangents` is a dict shaped like the params, {module path: {field: array}} with each array
+    the shape of its parameter (cast to float32); a module or field left out is zero.  A non-mapping,
+    an unknown module or field and a wrong shape raise ValueError, and the fp32_simt precision
+    NotImplementedError, before anything runs.  The tangents are packed once per call into tangent
+    weight images at the model's precision (Engine.weight_tangents); the engine's weights are not
+    touched.  The tangent runs forward with the step, stage by stage (Backward.tangent(wts=...)):
+    every layer adds X W-dot + b-dot to the tangent of its input's term, every LayerNorm
+    scale-dot * zhat + offset-dot, and the mesh-node encoder, the edge embedders and the processor's
+    e_0 get the tangents their parameters give them.  A module with no tangent costs no extra GEMM."""
+    run = self._param_tangent_run(inputs, targets_template, forcings, param_tangents, num_steps=1)
+    return self._input_jvp(inputs, targets_template, forcings, run, norm=None)
+
+  def loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents, **unused_kwargs):
+    """(loss, diagnostics, gnvp) for one target time.
+
+    `loss` and `diagnostics` are bit for bit what `loss()` returns.  `gnvp` is G v = J^T H J v, the
+    generalised Gauss-Newton matrix of loss.mean() (the scalar of loss_and_grads) with respect to the
+    params times v = param_tangents (a dict as param_jvp takes it): J the Jacobian of the decoder output
+    y with respect to the params and H = diag(coef * lat_weight) the Hessian of the loss, a quadratic
+    in y.  It is a dict shaped like the params, float32 numpy arrays as loss_and_grads returns `grads`,
+    with exact zeros for the mesh2grid mesh-node MLP, which the step never reads; a batch averages over
+    its elements as loss_and_grads does.  Where the predictions equal the targets the residual term of
+    the Hessian vanishes, and G v is the full parameter Hessian times v.  Every refusal of param_jvp
+    and loss_and_grads applies, before anything runs.
+
+    Per batch element: the step with its tangent along v (param_jvp's forward), the seed
+    coef * lat_weight * y-dot (gcb_output_loss_gn_seed), then the parameter backward pass of
+    loss_and_grads from that seed, which recomputes the step with its snapshots."""
+    return self._loss_and_param_gnvp(inputs, targets, forcings, param_tangents, norm=None)
+
+  def _param_tangent_run(self, inputs, targets_template, forcings, param_tangents, num_steps: int,
+                         plan=None) -> "_TangentRun":
+    """The checked parameter tangents of a param_jvp of `num_steps` target times, as a _TangentRun of
+    zero input tangents; raises before anything runs."""
+    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
+    if num_steps == 1 and xs.from_xarray(targets_template).sizes.get("time", 1) != 1:
+      raise NotImplementedError("param_jvp of GraphCast covers one target time (several: "
+                                "autoregressive.Predictor)")
+    tangents = self._checked_param_tangents(param_tangents)
+    run = _TangentRun(inputs, forcings, None, None, num_steps=num_steps, plan=plan)
+    run.param_tangents = tangents
+    return run
+
+  def _checked_param_tangents(self, param_tangents) -> Dict[str, Dict[str, np.ndarray]]:
+    """param_tangents checked against the params (check_param_tangents) and the precision."""
+    if self._precision not in ("bf16x3", "bf16"):
+      raise NotImplementedError(f"parameter tangents support the tensor-core precisions 'bf16x3' and "
+                                f"'bf16', not {self._precision!r}")
+    if self._params is None:
+      raise ValueError("GraphCast has no parameters: pass params= or call set_params()")
+    return check_param_tangents(param_tangents, self._params)
+
+  def _loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents,
+                           norm: Optional[FusedNormalization]):
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    if targets.sizes.get("time", 1) != 1:
+      raise NotImplementedError("Gauss-Newton products cover one target time (several are not "
+                                "provided)")
+    tangents = self._checked_param_tangents(param_tangents)
+    batch = dict(inputs.sizes).get("batch", 1)
+    num_grid = inputs.sizes["lat"] * inputs.sizes["lon"]
+    slabs = model_utils.channel_layout(targets)
+    coef = 2.0 * losses.channel_kappa(slabs, num_grid, LOSS_PER_VARIABLE_WEIGHTS) / batch
+    state = {}
+
+    def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
+      eng = self._engine
+      if "wt" not in state:
+        eng.grads_begin()
+        self._release_idle_staging()
+        state["wt"] = eng.weight_tangents(tangents)
+        state["lat_weight"] = self._lat_weight(targets, eng.device)
+        state["coef"] = torch.as_tensor(np.asarray(coef, np.float64)).to(eng.device)
+      eng.param_gnvp_element(planes_tgt, state["lat_weight"], state["coef"], state["wt"],
+                             channel_sums=channel_sums, **affine)
+
+    self._call(inputs, targets, forcings, norm=norm, targets=targets, predictions=False,
+               element=element)
+    state.clear()
+    loss, diagnostics = losses.losses_from_channel_sums(
+        self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
+    gnvp = {name: {f: t.cpu().numpy() for f, t in fields.items()}
+            for name, fields in self._engine.grads().items()}
+    return loss, diagnostics, gnvp
+
   @staticmethod
   def _one_step_tangents(inputs, targets_template, forcings, input_tangents,
                          forcing_tangents, directions: bool = False) -> "_TangentRun":
@@ -511,7 +614,8 @@ class GraphCast(Predictor):
     def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
       eng = self._engine
       if "out" not in state:
-        eng.input_grads_begin()
+        eng.input_grads_begin("input gradients" if run.param_tangents is None
+                              else "parameter tangents")
         self._release_idle_staging()
         state["out"] = torch.empty([run.dirs, run.batch, eng.n_out, eng.num_grid],
                                    dtype=torch.float32, device=eng.device)
@@ -1027,6 +1131,34 @@ class GraphCast(Predictor):
     return out
 
 
+def check_param_tangents(param_tangents, params) -> Dict[str, Dict[str, np.ndarray]]:
+  """param_tangents (param_jvp, loss_and_param_gnvp) as float32 host arrays, after its checks against
+  `params`: a mapping of mappings whose modules and fields are those of the params and whose arrays
+  have their parameter's shape.  Raises ValueError otherwise."""
+  if not isinstance(param_tangents, Mapping):
+    raise ValueError(f"param_tangents must be a mapping {{module: {{field: array}}}} shaped like the "
+                     f"params, not {type(param_tangents).__name__}")
+  out = {}
+  for name, fields in param_tangents.items():
+    if name not in params:
+      raise ValueError(f"param_tangents has an unknown module {name!r}")
+    if not isinstance(fields, Mapping):
+      raise ValueError(f"param_tangents[{name!r}] must be a mapping {{field: array}}, not "
+                       f"{type(fields).__name__}")
+    for f, a in fields.items():
+      if f not in params[name]:
+        raise ValueError(f"param_tangents has an unknown field {name}:{f}")
+      try:
+        arr = np.asarray(a, dtype=np.float32)
+      except (TypeError, ValueError) as e:
+        raise ValueError(f"param_tangents {name}:{f} is not a float array: {e}") from None
+      want = tuple(np.shape(params[name][f]))
+      if arr.shape != want:
+        raise ValueError(f"param_tangents {name}:{f} has shape {arr.shape}, the parameter {want}")
+      out.setdefault(name, {})[f] = arr
+  return out
+
+
 def hvp_tangent_planes(inputs: xs.Dataset, forcings: xs.Dataset, input_tangents,
                        forcing_tangents) -> torch.Tensor:
   """[batch, c_in, Ng] float32 host planes of the tangent of a Hessian-vector product, inputs then
@@ -1351,6 +1483,8 @@ class _TangentRun:
     self.feed = None if plan is None else torch.from_numpy(plan.feed_index(self.dirs))
     self.carry = [None] * self.batch
     self._slab = (-1, None)
+    # param_jvp: the checked host parameter tangents, packed on the device by the first element
+    self.param_tangents, self.weight_tangents = None, None
 
   def _planes(self, tangents, like) -> torch.Tensor:
     """[dirs, batch, channels, Ng] host planes of a tangent Dataset (feedback.tangent_planes)."""
@@ -1379,9 +1513,11 @@ class _TangentRun:
     buf[:, n_in:c_in].copy_(self._forcing_planes(self.step)[:, b])
     if keep is not None:
       keep(buf[:, :c_in])
+    if self.param_tangents is not None and self.weight_tangents is None:
+      self.weight_tangents = eng.weight_tangents(self.param_tangents)
     eng.input_jvp_element(buf[:, :c_in], tangent_out,
                           in_scale=None if norm is None else norm.in_scale, planes_out=planes_out,
-                          **affine)
+                          weight_tangents=self.weight_tangents, **affine)
     if self.step + 1 < self.num_steps:
       if self.feed.device != eng.device:
         self.feed = self.feed.to(eng.device)

@@ -322,6 +322,35 @@ class InputsAndResiduals(graphcast.Predictor):
     return graphcast.batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
                                  directions_per_pass)
 
+  def param_jvp(self, inputs, targets_template, forcings, param_tangents, **kwargs):
+    """(predictions, prediction_tangents) of the un-normalised predictions of __call__ along
+    param_tangents (GraphCast.param_jvp): the tangents are in physical units, through the
+    un-normalisation of the outputs.  GraphCast only."""
+    self._refuse_unfused()
+    run = self._predictor._param_tangent_run(inputs, targets_template, forcings, param_tangents,
+                                             num_steps=1)
+    inputs, targets_template, forcings, consts = self._fused_for(inputs, targets_template, forcings,
+                                                                 "parameter gradients")
+    return self._predictor._input_jvp(inputs, targets_template, forcings, run, norm=consts)
+
+  def loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents, **kwargs):
+    """(loss, diagnostics, gnvp) of `loss` (GraphCast.loss_and_param_gnvp), with the normalisation
+    fused into the kernels as in `loss`.  GraphCast only."""
+    self._refuse_unfused()
+    if xs.from_xarray(targets).sizes.get("time", 1) != 1:
+      raise NotImplementedError("Gauss-Newton products cover one target time (several are not "
+                                "provided)")
+    self._predictor._checked_param_tangents(param_tangents)
+    inputs, targets, forcings, consts = self._fused_for(inputs, targets, forcings,
+                                                        "parameter gradients")
+    return self._predictor._loss_and_param_gnvp(inputs, targets, forcings, param_tangents,
+                                                norm=consts)
+
+  def _refuse_unfused(self) -> None:
+    if not self._fuses():
+      raise NotImplementedError("parameter gradients need a GraphCast predictor directly inside "
+                                "InputsAndResiduals (the fused normalisation)")
+
   def loss(self, inputs, targets, forcings, **kwargs):
     """The loss computed on normalised inputs and targets (targets that are also inputs as
     normalised residuals against the last input frame)."""

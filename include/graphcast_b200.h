@@ -318,6 +318,17 @@ int gcb_output_loss_grad(const float* y, int32_t ld_y, int32_t n_out, int32_t n_
                          const float* lat_weight, const double* coef, float* g, int32_t ld_g,
                          void* stream);
 
+/* Seed of a Gauss-Newton product (GraphCast.loss_and_param_gnvp): the loss above is a quadratic in the
+ * decoder output y with the diagonal Hessian coef[c] * lat_weight[node / n_lon], so the seed of the
+ * backward pass that forms J^T H J v is, from the decoder tangent dy = J v,
+ *   g[node, c] = coef[c] * lat_weight[node / n_lon] * dy[node, c],   c < n_out
+ * in fp64, rounded once: bit for bit gcb_output_loss_grad with y = dy, all-zero targets and NULL scale,
+ * offset and add planes, without the [n_out, n_nodes] target planes that call would read.  Columns
+ * >= n_out of g are not written.  Deterministic. */
+int gcb_output_loss_gn_seed(const float* dy, int32_t ld_dy, int32_t n_out, int32_t n_lat,
+                            int32_t n_lon, const float* lat_weight, const double* coef, float* g,
+                            int32_t ld_g, void* stream);
+
 /* ---- backprop through time (the multi-step loss of autoregressive.Predictor) ---------------------
  * A step's input planes P [c_in, n_nodes] feed the next step through the frame shift and the fed-back
  * predictions (weathernext/utils/autoregressive.py:114-125; the loss unroll :262-310).  A = dL/dP of a
@@ -440,6 +451,19 @@ int gcb_layernorm_jvp_dirs(const float* z, int32_t ld_z, const float* dz, int32_
                            const float* scale, int64_t rows, int32_t n, int64_t dir_stride,
                            int32_t dirs, const float* residual, int32_t ld_res, float* out,
                            int32_t ld_out, void* stream);
+
+/* Tangent with respect to the parameters as well (GraphCast.param_jvp): gcb_layernorm_jvp plus the
+ * tangents of the LayerNorm's own scale and offset,
+ *   out = (residual ? residual : 0) + scale * rstd * (dz - mean(dz) - zhat * mean(zhat * dz))
+ *         + dscale * zhat + doffset
+ * with mu, rstd and zhat formed exactly as gcb_layernorm_jvp forms them; the two parameter terms are
+ * added to that result in this order, each rounded once.  dscale and doffset ([512] each) may be NULL
+ * alone or together; with both NULL, out is bit for bit gcb_layernorm_jvp.  n = 512, row-wise,
+ * deterministic; out may not alias z, dz, residual, dscale or doffset. */
+int gcb_layernorm_jvp_params(const float* z, int32_t ld_z, const float* dz, int32_t ld_dz,
+                             const float* scale, int64_t rows, int32_t n, const float* residual,
+                             int32_t ld_res, const float* dscale, const float* doffset, float* out,
+                             int32_t ld_out, void* stream);
 
 /* Several cotangents at one primal (GraphCast.batched_input_vjp), stacked as above: the LayerNorm
  * backward of each direction,
@@ -764,7 +788,8 @@ typedef enum {
                              * gcb_output_cotangent_grad_feedback, gcb_broadcast_grad_sum,
                              * gcb_layernorm_jvp, gcb_swish_jvp, gcb_layernorm_jvp_dirs,
                              * gcb_layernorm_backward_dirs, gcb_swish_backward_jvp(_dirs),
-                             * gcb_layernorm_backward_jvp(_dirs) */
+                             * gcb_layernorm_backward_jvp(_dirs), gcb_layernorm_jvp_params,
+                             * gcb_output_loss_gn_seed */
   GCB_KIND_NOISE = 11       /* gcb_add_gaussian_noise */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
