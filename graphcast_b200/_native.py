@@ -198,6 +198,10 @@ EXPORTS = {
     "gcb_layernorm_backward_jvp_dirs": (C.c_int, [_fp, C.c_int32, _fp, C.c_int32, _fp, C.c_int32, _fp,
                                                   C.c_int64, C.c_int32, C.c_int64, _fp, C.c_int32,
                                                   C.c_int32, _fp]),
+    "gcb_layernorm_backward_jvp_params": (C.c_int, [_fp, C.c_int32, C.c_int64, _fp, C.c_int32, _fp,
+                                                    C.c_int32, _fp, _fp, C.c_int64, C.c_int32, _fp,
+                                                    C.c_int32, _fp, C.c_int64, _fp, _fp, _fp, _fp,
+                                                    _fp, _fp, C.c_int32, _fp]),
     "gcb_segment_sum_sorted": (C.c_int, [_fp, C.c_int32, _fp, _fp, C.c_int32, _fp, C.c_int32, _fp,
                                          C.c_int32, C.c_int32, _fp]),
     "gcb_swish_rows": (C.c_int, [_fp, C.c_int32, C.c_int64, C.c_int32, _fp, C.c_int32, _fp]),

@@ -516,6 +516,16 @@ class Predictor(graphcast.Predictor):
                                 "provided)")
     return self._predictor.loss_and_param_gnvp(inputs, targets, forcings, param_tangents, **kwargs)
 
+  def loss_and_param_hvp(self, inputs, targets, forcings, param_tangents, **kwargs):
+    """(loss, diagnostics, grads, hvp) of one target time (GraphCast.loss_and_param_hvp), delegated to
+    the inner predictor; parameter Hessian-vector products over several target times are not provided,
+    with or without gradient_checkpointing."""
+    targets = xs.from_xarray(targets)
+    if targets.sizes["time"] != 1:
+      raise NotImplementedError("parameter Hessian-vector products cover one target time (several "
+                                "are not provided)")
+    return self._predictor.loss_and_param_hvp(inputs, targets, forcings, param_tangents, **kwargs)
+
   def _tangent_rollout(self, inputs, targets_template, forcings, input_tangents, forcing_tangents,
                        directions: bool, param_tangents=None):
     """input_jvp (batched_input_jvp with `directions`, param_jvp with `param_tangents`) over several

@@ -30,6 +30,9 @@ rows, and every LayerNorm scale-dot * zhat + offset-dot (gcb_layernorm_jvp_param
 Several cotangents (batched_input_vjp) share the backward walk the same way: element(dirs=K) stacks the
 gradient state like the tangent's, runs every dX product once over all directions, and differentiates
 the two nonlinearities with gcb_layernorm_backward_dirs and gcb_swish_jvp.
+A parameter Hessian-vector product (loss_and_param_hvp) joins the two: the tangent along weight tangents keeps
+its snapshots, and the two-direction walk element(hvp=..., param_grads=True) accumulates the gradient and its
+tangent, with every layer's weight-tangent terms (mlp_backward, dx, wgrad_dot).
 
 All arithmetic is in libgraphcast_b200.so; this module only sequences the launches and owns the
 buffers.  Allocation is lazy: nothing here exists until the first loss_and_grads call.
@@ -71,10 +74,15 @@ class _WeightTangent:
   (Backward.weight_tangents): the tangent weight images at the engine's precision with the primal's
   padding, for a pre-gathered edge layer its split blocks (`split`: we / ws / wr) in place of w0, and the
   padded tangent biases and LayerNorm vectors.  A layer with no tangent has w0 / split / w1 None (a
-  tangent bias alone comes with a zero weight image); a LayerNorm field with no tangent is None."""
+  tangent bias alone comes with a zero weight image); a LayerNorm field with no tangent is None.
+  w0_f32 / w1_f32: the padded fp32 tangent weights the images were packed from; `t`: their transposed
+  images (Backward.pack_transposed_tangents, keyed as _MlpInfo.t), for the dX products of a parameter
+  Hessian-vector product."""
 
   def __init__(self):
     self.w0 = self.split = self.b0 = self.w1 = self.b1 = self.scale = self.offset = None
+    self.w0_f32 = self.w1_f32 = None
+    self.t: Dict[str, torch.Tensor] = {}
 
 
 class Backward:
@@ -156,6 +164,9 @@ class Backward:
                  for f in ("b0", "b1", "scale", "offset")}
     # tangent(wts=...): the packed parameter tangents of param_jvp, {MLP stem: _WeightTangent}
     self.wts: Dict[str, _WeightTangent] = {}
+    # element(hvp=..., param_grads=True, wts=...): a parameter Hessian-vector product, whose gradient
+    # tangents accumulate into info.gt (allocated by the first one, zero_hvp)
+    self.phvp = False
 
   # -- setup ---------------------------------------------------------------------------------
   def _i32(self, a):
@@ -187,8 +198,8 @@ class Backward:
       g0 = g1
     return out
 
-  def _pack_t(self, info: _MlpInfo, key: str, w: int, ld: int, k: int, n: int, n_cols: int) -> None:
-    """info.t[key] = the packed image of the transpose of the device fp32 matrix at address w (rows of
+  def _pack_t(self, info, key: str, w: int, ld: int, k: int, n: int, n_cols: int) -> None:
+    """info.t[key] (an _MlpInfo or _WeightTangent) = the packed image of the transpose of the device fp32 matrix at address w (rows of
     `ld` floats), of padded shape [k, n] (n_cols real columns), written in place when it exists."""
     if key not in info.t:
       info.t[key] = torch.empty([self.lib.gcb_packed_weight_bytes(k, n)], dtype=torch.uint8,
@@ -230,19 +241,19 @@ class Backward:
       if t0:
         w = t0["w"] if "w" in t0 else zeros(*self.shapes[l0]["w"])
         if info.split is not None:           # row blocks [edge | sender | receiver], each packed alone
-          wt.split = {}
+          wt.split, wt.w0_f32 = {}, w
           for i, name in enumerate(("we", "ws", "wr")):
             wt.split[name] = image(D, D)
             self.eng.pack_weight(w.data_ptr() + 4 * i * D * D, D, False, D, D, D, D, wt.split[name])
         else:
           seg_real = [w.shape[0]] if len(info.k_segs) == 1 else info.k_segs
-          wt.w0 = image(sum(info.k_segs), D)
-          self.eng._pack_linear_device(w, seg_real, info.k_segs, wt.w0, zeros(sum(info.k_segs), D))
+          wt.w0, wt.w0_f32 = image(sum(info.k_segs), D), zeros(sum(info.k_segs), D)
+          self.eng._pack_linear_device(w, seg_real, info.k_segs, wt.w0, wt.w0_f32)
         wt.b0 = t0["b"] if "b" in t0 else zeros(D)
       if t1:
         w = t1["w"] if "w" in t1 else zeros(*self.shapes[l1]["w"])
-        wt.w1 = image(D, info.n1)
-        self.eng._pack_linear_device(w, [D], [D], wt.w1, zeros(D, info.n1))
+        wt.w1, wt.w1_f32 = image(D, info.n1), zeros(D, info.n1)
+        self.eng._pack_linear_device(w, [D], [D], wt.w1, wt.w1_f32)
         wt.b1 = zeros(info.n1)
         if "b" in t1:
           wt.b1[:info.n1_valid].copy_(t1["b"])
@@ -253,6 +264,25 @@ class Backward:
           setattr(wt, f, v)
       out[info.stem] = wt
     return out
+
+  def pack_transposed_tangents(self, wts: Dict[str, _WeightTangent]) -> None:
+    """The transposed images of packed parameter tangents (weight_tangents), packed on the device as
+    _pack_transposed packs the primal ones: W1-dot^T and W0-dot^T per 512-row block (for a pre-gathered
+    edge layer: we, ws, wr), so that a parameter Hessian-vector product's dX products can add their
+    dY W-dot^T terms.  Layers without a tangent get none."""
+    for info in self._all:
+      wt = wts.get(info.stem)
+      if wt is None:
+        continue
+      if wt.w1_f32 is not None:
+        self._pack_t(wt, "w1", wt.w1_f32.data_ptr(), info.n1, info.n1, D, D)
+      if wt.w0_f32 is not None:
+        k0 = self.shapes[f"{info.stem}_mlp/~/linear_0"]["w"][0]
+        if len(info.k_segs) >= 2 and k0 == len(info.k_segs) * D:
+          for s in range(len(info.k_segs)):
+            self._pack_t(wt, f"w0_{s}", wt.w0_f32.data_ptr() + 4 * s * D * D, D, D, D, D)
+        elif k0 == D:
+          self._pack_t(wt, "w0_0", wt.w0_f32.data_ptr(), D, D, D, D)
 
   def repack(self, stems=None) -> None:
     """The engine's weights were rewritten (Engine.load_params / load_params_device): repacks the
@@ -284,6 +314,15 @@ class Backward:
   def zero_grads(self) -> None:
     for info in self._all:
       for t in info.g.values():
+        t.zero_()
+
+  def zero_hvp(self) -> None:
+    """Zeroes (allocating on first use) the accumulators of a parameter Hessian-vector product, the
+    tangents of the gradient accumulators info.g, shaped like them."""
+    for info in self._all:
+      if not hasattr(info, "gt"):
+        info.gt = {f: torch.zeros_like(t) for f, t in info.g.items()}
+      for t in info.gt.values():
         t.zero_()
 
   # -- launch helpers ------------------------------------------------------------------------------
@@ -354,7 +393,7 @@ class Backward:
     return y
 
   def mlp_backward(self, info: _MlpInfo, rows: int, segs, dy: torch.Tensor, *, pre=None,
-                   w0=None, dw_segs=None, tan=None) -> torch.Tensor:
+                   w0=None, dw_segs=None, tan=None, xdot=None) -> torch.Tensor:
     """Backward of one MLP at the recomputed forward; accumulates its parameter gradients and returns
     dh [rows, 512], the gradient of the first layer's pre-activation (incl. pre-gathered addends).
     dw_segs: the layer-0 inputs whose weight blocks get X^T dh (default: all of `segs`).
@@ -369,14 +408,26 @@ class Backward:
     mlp_jvp takes it (stacked tables of K directions, K-fold gather indices): h-dot = dsegs W0 + the
     gathered addends, z-dot = W1 (swish'(h) h-dot), each one GEMM over the K directions, and the two
     nonlinearities are gcb_layernorm_backward_jvp_dirs and gcb_swish_backward_jvp_dirs, which form the
-    primal terms once for all K."""
+    primal terms once for all K.
+
+    A parameter Hessian-vector product (self.phvp: two directions, parameter gradients, the weight
+    tangents self.wts) runs that walk with K = 1 and every launch of direction 0 on the operands of the
+    one-direction walk, and also forms the tangents of the parameter gradients in info.gt: h-dot and
+    z-dot get the MLP's weight-tangent terms X W0-dot + b0-dot and a W1-dot + b1-dot; the LayerNorm is
+    gcb_layernorm_backward_jvp_params (its scale-dot, the sums of both directions); da-dot gets
+    dz W1-dot^T; dW-dot = X-dot^T g + X^T g-dot for each weight, with `xdot` the tangents of the layer-0
+    inputs aligned with dw_segs (default segs; None entries or xdot None: zero) and a-dot for layer 1;
+    the bias sums of both directions run in gcb_layernorm_backward's column-sum mode."""
     w = info.w
     w0 = w0 or w.w0_packed
     nd, stride, rk = self.dirs, self.dir_stride(rows), self.dir_rows(rows)
+    ph = self.phvp
+    wt = self.wts.get(info.stem) if ph else None
     h = self.empty(rows)
     self.layer(rows, segs, w0, w.b0, _native.ACT_NONE, out_y=h, pre=pre)
-    hd = None if self.hvp is None else self._hdot(rows, w0, tan)
+    hd = None if self.hvp is None else self._hdot(rows, w0, tan, segs, wt)
     g = info.g if self.param_grads else self.sink
+    ad = None
     ws = self.ws_rows
     if info.ln:
       a = self.empty(rows)
@@ -384,7 +435,8 @@ class Backward:
                     "gcb_swish_rows")
       z = self.empty(rows)
       self.layer(rows, [self.tab(a)], w.w1_packed, w.b1, out_y=z)
-      del a
+      if wt is None or wt.w1 is None:
+        del a
       dz = self.empty(rk)
       if hd is not None:                     # z-dot = W1 (swish'(h) h-dot), K directions
         nt = self.tdirs
@@ -394,10 +446,25 @@ class Backward:
                                              ad.data_ptr(), D, self._st()), "gcb_swish_jvp")
         zd = self.empty(rt)
         self.layer(rt, [self.tab(ad)], w.w1_packed, self.zero_bias, out_y=zd)
-        del ad
-        _native.check(self.lib.gcb_layernorm_backward_jvp_dirs(
-            dy.data_ptr(), dy.shape[1], z.data_ptr(), D, zd.data_ptr(), D, w.ln_scale, rows, D, stride,
-            dz.data_ptr(), D, nt, self._st()), "gcb_layernorm_backward_jvp_dirs")
+        if not ph:
+          ad = None
+        if wt is not None and wt.w1 is not None:   # + a W1-dot + b1-dot
+          zdt = self.empty(rows)
+          self.layer(rows, [self.tab(a)], wt.w1, wt.b1, out_y=zdt, pre=[(zd, None)])
+          zd = zdt
+          del a
+        if ph:
+          gt = info.gt
+          _native.check(self.lib.gcb_layernorm_backward_jvp_params(
+              dy.data_ptr(), dy.shape[1], stride, z.data_ptr(), D, zd.data_ptr(), D, w.ln_scale,
+              self._ptr(None if wt is None else wt.scale), rows, D, dz.data_ptr(), D, ws.data_ptr(),
+              ws.numel(), g["b1"].data_ptr(), g["scale"].data_ptr(), g["offset"].data_ptr(),
+              gt["b1"].data_ptr(), gt["scale"].data_ptr(), gt["offset"].data_ptr(), 1, self._st()),
+              "gcb_layernorm_backward_jvp_params")
+        else:
+          _native.check(self.lib.gcb_layernorm_backward_jvp_dirs(
+              dy.data_ptr(), dy.shape[1], z.data_ptr(), D, zd.data_ptr(), D, w.ln_scale, rows, D,
+              stride, dz.data_ptr(), D, nt, self._st()), "gcb_layernorm_backward_jvp_dirs")
         del zd
       elif nd == 1:
         _native.check(self.lib.gcb_layernorm_backward(
@@ -412,19 +479,33 @@ class Backward:
     else:
       dz = dy
       if nd == 1:                            # its column sums only (several directions: none)
-        _native.check(self.lib.gcb_layernorm_backward(
-            dy.data_ptr(), dy.shape[1], None, 0, None, rows, info.n1, None, 0, ws.data_ptr(),
-            ws.numel(), g["b1"].data_ptr(), None, None, 1, self._st()), "gcb_layernorm_backward")
+        self.col_sums(dy, rows, info.n1, g["b1"])
+      elif ph:                               # both directions' (a parameter HVP)
+        self.col_sums(dy, rows, info.n1, g["b1"])
+        self.col_sums(dy[stride:], rows, info.n1, info.gt["b1"])
+      if ph:                                 # a-dot = swish'(h) h-dot, for dW1-dot
+        ad = self.empty(rows)
+        _native.check(self.lib.gcb_swish_jvp(h.data_ptr(), D, rows, D, hd.data_ptr(), D, stride, 1,
+                                             ad.data_ptr(), D, self._st()), "gcb_swish_jvp")
     if self.param_grads:
       self.wgrad(self.tab(h), dz, rows, g["w1"], n=info.n1, swish=True)     # dW1 = swish(h)^T dz
+    if ph:                                   # dW1-dot = a-dot^T dz + swish(h)^T dz-dot
+      self.wgrad(self.tab(ad), dz, rows, info.gt["w1"], n=info.n1)
+      self.wgrad(self.tab(h), dz[stride:], rows, info.gt["w1"], n=info.n1, swish=True)
+      del ad
     da = self.empty(rk)
     self.layer(rk, [self.tab(dz, info.n1)], info.t["w1"], self.zero_bias, out_y=da)
+    if wt is not None and "w1" in wt.t:      # da-dot += dz W1-dot^T
+      self.add_dot_product(rows, dz, wt.t["w1"], da, k=info.n1)
     if hd is not None:                       # [swish'(h) da; its K tangents] in place
       dh = da
       _native.check(self.lib.gcb_swish_backward_jvp_dirs(
           h.data_ptr(), D, hd.data_ptr(), D, rows, D, da.data_ptr(), D, stride, dh.data_ptr(), D,
           self.tdirs, self._st()), "gcb_swish_backward_jvp_dirs")
       del hd
+      if ph:                                 # the bias sums of dh and dh-dot
+        self.col_sums(dh, rows, D, g["b0"])
+        self.col_sums(dh[stride:], rows, D, info.gt["b0"])
     elif nd == 1:
       dh = self.empty(rows)
       _native.check(self.lib.gcb_swish_backward(
@@ -437,27 +518,77 @@ class Backward:
     del da, h
     if self.param_grads:
       off = 0
-      for s in (dw_segs if dw_segs is not None else segs):
+      wsegs = dw_segs if dw_segs is not None else segs
+      if xdot is None and tan is not None and tan[2] is None and len(tan[0]) == len(wsegs):
+        xdot = tan[0]                        # the input tangents, one per segment
+      for i, s in enumerate(wsegs):
         k = s[2]
         self.wgrad(s, dh, rows, g["w0"][off:off + k])
+        if ph:                               # dW0-dot = X-dot^T dh + X^T dh-dot
+          self.wgrad_dot(s, None if xdot is None else xdot[i], dh, rows, info.gt["w0"][off:off + k])
         off += k
     return dh
 
-  def _hdot(self, rows: int, w0, tan) -> torch.Tensor:
+  def _hdot(self, rows: int, w0, tan, segs=None, wt: Optional[_WeightTangent] = None) -> torch.Tensor:
     """h-dot of an MLP's first layer, a stacked table of self.tdirs directions of `rows` rows, from
     tan = (dsegs, dpre, dw0) (see mlp_backward): dsegs W0 (dw0: the weight of those segments, default
     w0) plus the gathered addends dpre, or the addends alone; zeros when the layer input has no
-    tangent."""
+    tangent.  With a layer-0 weight tangent wt (a parameter HVP, one direction), + segs W0-dot + b0-dot
+    (for a pre-gathered edge layer, segs is the edge segment and W0-dot its block we)."""
     dsegs, dpre, dw0 = tan if tan is not None else ([], (), None)
     rt = self.dir_rows(rows, self.tdirs)
     if dsegs:
       hd = self.empty(rt)
       self.layer(rt, dsegs, dw0 or w0, self.zero_bias, out_y=hd, pre=list(dpre) or None)
-      return hd
-    hd = None
-    for table, idx in dpre:
-      hd = self.gather_add(table, idx, rt, hd)
+    else:
+      hd = None
+      for table, idx in dpre:
+        hd = self.gather_add(table, idx, rt, hd)
+    t0 = None if wt is None else (wt.split["we"] if wt.split is not None else wt.w0)
+    if t0 is not None:
+      hdt = self.empty(rows)
+      self.layer(rows, segs, t0, wt.b0, out_y=hdt, pre=None if hd is None else [(hd, None)])
+      return hdt
     return hd if hd is not None else torch.zeros([max(rt, 1), D], dtype=torch.float32, device=self.dev)
+
+  def col_sums(self, t: torch.Tensor, rows: int, n: int, out: torch.Tensor) -> None:
+    """out += the column sums of t's first `rows` rows (gcb_layernorm_backward's column-sum mode: the
+    row split and fp64 fold of every row-wise backward kernel's sums)."""
+    ws = self.ws_rows
+    _native.check(self.lib.gcb_layernorm_backward(
+        t.data_ptr(), t.shape[1], None, 0, None, rows, n, None, 0, ws.data_ptr(), ws.numel(),
+        out.data_ptr(), None, None, 1, self._st()), "gcb_layernorm_backward")
+
+  def add_dot_product(self, rows: int, src: torch.Tensor, img, out: torch.Tensor, k: int = D) -> None:
+    """A parameter HVP's dX product: direction 1 of the stacked out (= src W^T over both directions)
+    += direction 0 of src times the transposed tangent image img (dY W-dot^T), through one GEMM with
+    that direction as an identity addend."""
+    s = self.dir_stride(rows)
+    t = self.empty(rows)
+    self.layer(rows, [self.tab(src, k)], img, self.zero_bias, out_y=t, pre=[(out[s:s + rows], None)])
+    out[s:s + rows].copy_(t)
+
+  def dx(self, info: _MlpInfo, key: str, rows: int, src: torch.Tensor,
+         residual: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """A dX product of the walk, [residual +] src W^T over every direction with the transposed block
+    info.t[key]; in a parameter HVP, direction 1 also gets src_0 W-dot^T when that block has a
+    tangent."""
+    rows_k = self.dir_rows(rows)
+    out = self.empty(rows_k)
+    if residual is None:
+      self.layer(rows_k, [self.tab(src)], info.t[key], self.zero_bias, out_y=out)
+    else:
+      self.layer(rows_k, [self.tab(src)], info.t[key], self.zero_bias, residual=residual, out=out)
+    wt = self.wts.get(info.stem) if self.phvp else None
+    if wt is not None and key in wt.t:
+      self.add_dot_product(rows, src, wt.t[key], out)
+    return out
+
+  def wgrad_dot(self, x, xdot, g: torch.Tensor, rows: int, dw: torch.Tensor, *, n: int = D) -> None:
+    """dw += X-dot^T g_0 + X^T g_1 (g a stacked table of two directions; xdot None: zero)."""
+    if xdot is not None:
+      self.wgrad(xdot, g, rows, dw, n=n)
+    self.wgrad(x, g[self.dir_stride(rows):], rows, dw, n=n)
 
   def sender_sums(self, dh: torch.Tensor, rows: int, csr, num_nodes: int) -> torch.Tensor:
     """gcb_segment_sum_sorted (sender CSR `csr`) of every direction of the stacked edge table dh (`rows`
@@ -503,15 +634,15 @@ class Backward:
     ps = self.projection(n_s, v_s, sp.ws_packed)
     pr = self.projection(n_r, v_r, sp.wr_packed)
     t = None
-    if tan is not None:
+    if tan is not None:                      # in a parameter HVP the projections get v W-dot too
       de_segs, dv_s, dv_r = tan
       nt = self.tdirs
-      dps = self.projection(self.dir_rows(n_s, nt), self.tab(dv_s), sp.ws_packed)
-      dpr = self.projection(self.dir_rows(n_r, nt), self.tab(dv_r), sp.wr_packed)
+      dps = self.proj_tangent(n_s, v_s, dv_s, sp.ws_packed, self._split_tangent(info, "ws"), nt)
+      dpr = self.proj_tangent(n_r, v_r, dv_r, sp.wr_packed, self._split_tangent(info, "wr"), nt)
       t = (de_segs, [(dps, self.kfold(snd, n_s, (snd_name, "snd"), nt)),
                      (dpr, self.kfold(rcv, n_r, (snd_name, "rcv"), nt))], None)
     dh = self.mlp_backward(info, rows, [e_seg], dm, pre=[(ps, snd), (pr, rcv)], w0=sp.we_packed,
-                           tan=t)
+                           tan=t, xdot=None if t is None or not t[0] else t[0])
     del ps, pr, t
     s = self.sender_sums(dh, rows, self.csr[snd_name], n_s)
     r = rcv_sum(dh)
@@ -519,6 +650,10 @@ class Backward:
       w0 = info.g["w0"]
       self.wgrad(v_s, s, n_s, w0[D:2 * D])
       self.wgrad(v_r, r, n_r, w0[2 * D:3 * D])
+      if self.phvp:                          # the node blocks: v-dot^T S + v^T S-dot
+        gt = info.gt["w0"]
+        self.wgrad_dot(v_s, self.tab(tan[1]), s, n_s, gt[D:2 * D])
+        self.wgrad_dot(v_r, self.tab(tan[2]), r, n_r, gt[2 * D:3 * D])
     return dh, s, r
 
   def bipartite_backward(self, name: str, info: _MlpInfo, enc: _MlpInfo, feat_t: torch.Tensor,
@@ -542,33 +677,36 @@ class Backward:
     pr = self.projection(n_r, v_r, sp.wr_packed)
     dps = dpr = None
     nt = self.tdirs
-    if tan is not None:
-      dps = self.projection(self.dir_rows(n_s, nt), self.tab(tan[0]), sp.ws_packed)
-      dpr = None if tan[1] is None else self.projection(self.dir_rows(n_r, nt), self.tab(tan[1]),
-                                                        sp.wr_packed)
+    if tan is not None:                      # in a parameter HVP the projections get v W-dot too
+      dps = self.proj_tangent(n_s, v_s, tan[0], sp.ws_packed, self._split_tangent(info, "ws"), nt)
+      dpr = self.proj_tangent(n_r, v_r, tan[1], sp.wr_packed, self._split_tangent(info, "wr"), nt)
+    enc_t = self.phvp and enc.stem in self.wts
     s_tab, r_tab = None, self.empty(self.dir_rows(n_r))
     for i, (r0, r1, g0, g1, rp, heavy, n_heavy, csr) in enumerate(self.chunks[name]):
       n = r1 - r0
       f = self.tab(feat_t[r0:r1], 16, 4, 4)                 # 16-byte rows: the view stays aligned
       snd_c, rcv_c = snd[r0:r1].clone(), rcv[r0:r1].clone()  # index arrays from an aligned base
       e = self.fwd_mlp(enc, n, [f])
+      # the embedded edges' tangent (their embedder's parameters), recomputed as e is
+      de = self.weight_jvp(enc, n, [f]) if enc_t else None
       dm = self.gather_add(dagg, self.kfold(rcv_c, n_r, (name, "backward", i, "rcv")),
                            self.dir_rows(n))
       t = None
       if dps is not None:
-        t = ([], [(dps, self.kfold(snd_c, n_s, (name, "hvp", i, "snd"), nt))] + (
-            [] if dpr is None else [(dpr, self.kfold(rcv_c, n_r, (name, "hvp", i, "rcv"), nt))]), None)
+        t = ([] if de is None else [self.tab(de)],
+             [(dps, self.kfold(snd_c, n_s, (name, "hvp", i, "snd"), nt))] + (
+                 [] if dpr is None else [(dpr, self.kfold(rcv_c, n_r, (name, "hvp", i, "rcv"), nt))]),
+             None)
       dh = self.mlp_backward(info, n, [self.tab(e)], dm, pre=[(ps, snd_c), (pr, rcv_c)],
-                             w0=sp.we_packed, tan=t)
-      del dm, e, snd_c, rcv_c, t
+                             w0=sp.we_packed, tan=t, xdot=None if de is None else [self.tab(de)])
+      del dm, e, de, snd_c, rcv_c, t
       s_c = self.sender_sums(dh, n, csr, n_s)
       s_tab = s_c if s_tab is None else self.gather_add(
           s_c, self.kfold(self.iota[:n_s], n_s, ("iota", n_s)), self.dir_rows(n_s), s_tab)
       del s_c
       self.receiver_sums(dh, n, rp, g1 - g0, r_tab[g0:], self.dir_stride(n_r), heavy, n_heavy)
       if self.param_grads:                  # the edge embedder's backward: parameters only
-        de = self.empty(n)
-        self.layer(n, [self.tab(dh)], info.t["w0_0"], self.zero_bias, out_y=de)
+        de = self.dx(info, "w0_0", n, dh)
         del dh
         self.mlp_backward(enc, n, [f], de)
         del de
@@ -579,12 +717,17 @@ class Backward:
       w0 = info.g["w0"]
       self.wgrad(v_s, s_tab, n_s, w0[D:2 * D])
       self.wgrad(v_r, r_tab, n_r, w0[2 * D:3 * D])
+      if self.phvp:                          # the node blocks: v-dot^T S + v^T S-dot
+        gt = info.gt["w0"]
+        self.wgrad_dot(v_s, self.tab(tan[0]), s_tab, n_s, gt[D:2 * D])
+        self.wgrad_dot(v_r, None if tan[1] is None else self.tab(tan[1]), r_tab, n_r, gt[2 * D:3 * D])
     return s_tab, r_tab
 
   # -- one batch element ---------------------------------------------------------------------------
   def element(self, grid_in_img: torch.Tensor, g_out: torch.Tensor, snaps: dict,
               dgrid_in: bool = False, param_grads: bool = True,
-              dirs: int = 1, hvp: Optional[dict] = None) -> Optional[torch.Tensor]:
+              dirs: int = 1, hvp: Optional[dict] = None,
+              wts: Optional[Dict[str, _WeightTangent]] = None) -> Optional[torch.Tensor]:
     """Accumulates the parameter gradients of one batch element whose loss derivative with respect
     to the decoder output is g_out [Ng, 256] (gcb_output_loss_grad) and whose forward left `snaps`
     (whose entries are dropped as they are consumed).  dgrid_in: also return the derivative with
@@ -610,18 +753,34 @@ class Backward:
     each over the K directions) and differentiates its two nonlinearities with
     gcb_layernorm_backward_jvp_dirs and gcb_swish_backward_jvp_dirs, so direction j of dx is the
     tangent of direction 0 along tangent j - 1.  Direction 0 is bit for bit what g_out's direction 0
-    alone gives, and direction j what the K = 1 walk gives for tangent j - 1 and seed direction j."""
-    if dirs > 1 and param_grads:
-      raise ValueError("several directions are supported without parameter gradients only")
-    if hvp is not None and (dirs < 2 or param_grads):
-      raise ValueError("a Hessian-vector product runs 1 + K directions (K >= 1) without parameter "
-                       "gradients")
+    alone gives, and direction j what the K = 1 walk gives for tangent j - 1 and seed direction j.
+
+    hvp with param_grads (a parameter Hessian-vector product, loss_and_param_hvp): dirs = 2, the
+    snapshots of tangent(wts=wts, snaps=..., tsnaps=...) along the packed parameter tangents `wts`
+    (with pack_transposed_tangents), g_out's direction 1 the seed's tangent.  The walk above with K = 1
+    then also accumulates the parameter gradients (direction 0, bit for bit those of the one-direction
+    walk) and their tangents into info.gt (see mlp_backward), runs the parts that only the parameters
+    need on both directions (the edge embedders, the mesh-node encoder, the first step's de product), and
+    adds every weight tangent's terms: h-dot and z-dot get X W-dot + b-dot, every dX product of a layer
+    with a tangent dY_0 W-dot^T, and the node projections of the edge layers v W-dot."""
+    phvp = hvp is not None and param_grads
+    if phvp:
+      if dirs != 2:
+        raise ValueError("a parameter Hessian-vector product runs two directions")
+    else:
+      if dirs > 1 and param_grads:
+        raise ValueError("several directions are supported without parameter gradients only")
+      if hvp is not None and dirs < 2:
+        raise ValueError("a Hessian-vector product runs 1 + K directions (K >= 1) without parameter "
+                         "gradients")
     self.param_grads, self.dirs, self.hvp = bool(param_grads), int(dirs), hvp
     self.tdirs = 0 if hvp is None else int(dirs) - 1
+    self.phvp, self.wts = phvp, (wts or {}) if phvp else {}
     try:
       return self._element(grid_in_img, g_out, snaps, dgrid_in)
     finally:
       self.param_grads, self.dirs, self.hvp, self.tdirs = True, 1, None, 0
+      self.phvp, self.wts = False, {}
 
   def _element(self, grid_in_img, g_out, snaps, dgrid_in):
     eng, m = self.eng, self.m
@@ -638,15 +797,12 @@ class Backward:
     # ---- decoder: out = MLP(vg2);  vg2 = vg1 + MLP([vg1 | agg3]);  m3 = MLP([e3 | v[snd] | vg1[rcv]])
     dh = self.mlp_backward(mp["dec_grid"], ng, [img(snaps["vg2"])], g_out,
                            tan=tan(*(() if T is None else (T.pop("vg2"),))))
-    dvg2 = self.empty(rk(ng))
-    self.layer(rk(ng), [tab(dh)], mp["dec_grid"].t["w0_0"], self.zero_bias, out_y=dvg2)
+    dvg2 = self.dx(mp["dec_grid"], "w0_0", ng, dh)
     info = mp["proc_n_grid_m2g"]
     dh = self.mlp_backward(info, ng, [img(snaps["vg1"]), img(snaps["agg3"])], dvg2,
                            tan=tan(*(() if T is None else (T["vg1"], T.pop("agg3")))))
-    dvg1 = self.empty(rk(ng))
-    self.layer(rk(ng), [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dvg2, out=dvg1)
-    dagg3 = self.empty(rk(ng))
-    self.layer(rk(ng), [tab(dh)], info.t["w0_1"], self.zero_bias, out_y=dagg3)
+    dvg1 = self.dx(info, "w0_0", ng, dh, residual=dvg2)
+    dagg3 = self.dx(info, "w0_1", ng, dh)
     del dh, dvg2
     info = mp["proc_e_m2g"]
     S, R = self.bipartite_backward("m2g", info, mp["enc_e_m2g"], eng.m2g_feat, dagg3, eng.m2g_snd,
@@ -655,11 +811,8 @@ class Backward:
     del dagg3
     # snapshots are released as soon as the backward pass is past their stage
     snaps["vg2"] = snaps["agg3"] = snaps["vg1"] = None
-    dvg1_new = self.empty(rk(ng))
-    self.layer(rk(ng), [tab(R)], info.t["w0_2"], self.zero_bias, residual=dvg1, out=dvg1_new)
-    dvg1 = dvg1_new
-    dv = self.empty(rk(nm))
-    self.layer(rk(nm), [tab(S)], info.t["w0_1"], self.zero_bias, out_y=dv)
+    dvg1 = self.dx(info, "w0_2", ng, R, residual=dvg1)
+    dv = self.dx(info, "w0_1", nm, S)
     del S, R
 
     # ---- processor, last step first:  m = MLP([e | v[snd] | v[rcv]]);  v' = v + MLP([v | agg]);
@@ -672,8 +825,7 @@ class Backward:
       nfo, efo = self.proc_n[k], self.proc_e[k]
       dh_n = self.mlp_backward(nfo, nm, [v_k, agg_k], dv,
                                tan=tan(*(() if T is None else (T["v"][k], T["agg"][k]))))
-      dagg = self.empty(rk(nm))
-      self.layer(rk(nm), [tab(dh_n)], nfo.t["w0_1"], self.zero_bias, out_y=dagg)
+      dagg = self.dx(nfo, "w0_1", nm, dh_n)
       dm = self.gather_add(dagg, rcv_k, rk(m.e_mesh), de_next)
       del dagg
       if k == 0:
@@ -684,27 +836,20 @@ class Backward:
       dH, S, R = self.edge_backward(
           efo, m.e_mesh, e_k, dm, "mesh", v_k, nm, eng.mesh_snd, v_k, nm, eng.mesh_rcv,
           lambda d: self.seg_sum_receiver(d, m.e_mesh, eng.mesh_row_ptr, nm),
-          tan=None if T is None else ([] if k == 0 else [tab(T["e"][k])], T["v"][k], T["v"][k]))
+          tan=None if T is None else ([] if T["e"][k] is None else [tab(T["e"][k])], T["v"][k],
+                                      T["v"][k]))
       del dm
       if k == 0 and not self.param_grads:    # de_0 feeds the mesh edge embedder's parameters only
         de = None
-      else:
-        de = self.empty(rk(m.e_mesh))        # de_k = de_{k+1} + dH W_e^T  (e' = e + m)
-        if de_next is None:
-          self.layer(rk(m.e_mesh), [tab(dH)], efo.t["w0_0"], self.zero_bias, out_y=de)
-        else:
-          self.layer(rk(m.e_mesh), [tab(dH)], efo.t["w0_0"], self.zero_bias, residual=de_next,
-                     out=de)
+      else:                                  # de_k = de_{k+1} + dH W_e^T  (e' = e + m)
+        de = self.dx(efo, "w0_0", m.e_mesh, dH, residual=de_next)
       del dH
       de_next = de
       # dv_k = dv_{k+1} + dh_n W0a^T + S W_s^T + R W_r^T
-      dv_new = self.empty(rk(nm))
-      self.layer(rk(nm), [tab(dh_n)], nfo.t["w0_0"], self.zero_bias, residual=dv, out=dv_new)
-      dv2 = self.empty(rk(nm))
-      self.layer(rk(nm), [tab(S)], efo.t["w0_1"], self.zero_bias, residual=dv_new, out=dv2)
-      self.layer(rk(nm), [tab(R)], efo.t["w0_2"], self.zero_bias, residual=dv2, out=dv_new)
-      dv = dv_new
-      del dh_n, S, R, dv2
+      dv_new = self.dx(nfo, "w0_0", nm, dh_n, residual=dv)
+      dv2 = self.dx(efo, "w0_1", nm, S, residual=dv_new)
+      dv = self.dx(efo, "w0_2", nm, R, residual=dv2)
+      del dh_n, S, R, dv2, dv_new
       snaps["v"][k + 1] = snaps["agg"][k] = snaps["e"][k] = None
       if T is not None:
         T["v"][k + 1] = T["agg"][k] = T["e"][k] = None
@@ -722,31 +867,33 @@ class Backward:
     info = mp["proc_n_grid_g2m"]
     dh = self.mlp_backward(info, ng, [tab(vg0)], dvg1,
                            tan=tan(*(() if T is None else (T["vg0"],))))
-    dvg0 = self.empty(rk(ng))
-    self.layer(rk(ng), [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dvg1, out=dvg0)
+    dvg0 = self.dx(info, "w0_0", ng, dh, residual=dvg1)
     del dh, dvg1
     info = mp["proc_n_mesh_g2m"]
-    dh = self.mlp_backward(info, nm, [tab(vm0), img(snaps["agg1"])], dv,   # vm0 has no tangent
-                           tan=None if T is None else tan(T.pop("agg1"), dw0=self.w0_block(info, 1)))
-    dvm0 = self.empty(rk(nm))
-    self.layer(rk(nm), [tab(dh)], info.t["w0_0"], self.zero_bias, residual=dv, out=dvm0)
-    dagg1 = self.empty(rk(nm))
-    self.layer(rk(nm), [tab(dh)], info.t["w0_1"], self.zero_bias, out_y=dagg1)
+    dvm0_t = None if T is None else T.pop("vm0", None)   # v_m0's tangent (its encoder's parameters)
+    if dvm0_t is None:                       # vm0 has no tangent: block 1 of W0 alone
+      dh = self.mlp_backward(info, nm, [tab(vm0), img(snaps["agg1"])], dv,
+                             tan=None if T is None else tan(T["agg1"], dw0=self.w0_block(info, 1)),
+                             xdot=None if T is None else [None, tab(T["agg1"])])
+    else:
+      dh = self.mlp_backward(info, nm, [tab(vm0), img(snaps["agg1"])], dv,
+                             tan=tan(dvm0_t, T["agg1"]))
+    if T is not None:
+      del T["agg1"]
+    dvm0 = self.dx(info, "w0_0", nm, dh, residual=dv)
+    dagg1 = self.dx(info, "w0_1", nm, dh)
     del dh, dv
     info = mp["proc_e_g2m"]
     S, R = self.bipartite_backward("g2m", info, mp["enc_e_g2m"], eng.g2m_feat, dagg1, eng.g2m_snd,
                                    eng.g2m_rcv, tab(vg0), ng, tab(vm0), nm,
-                                   tan=None if T is None else (T.pop("vg0"), None))
-    del dagg1
-    t = self.empty(rk(ng))
-    self.layer(rk(ng), [tab(S)], info.t["w0_1"], self.zero_bias, residual=dvg0, out=t)
-    dvg0 = t
-    t = self.empty(rk(nm))
-    self.layer(rk(nm), [tab(R)], info.t["w0_2"], self.zero_bias, residual=dvm0, out=t)
-    dvm0 = t
+                                   tan=None if T is None else (T.pop("vg0"), dvm0_t))
+    del dagg1, dvm0_t
+    dvg0 = self.dx(info, "w0_1", ng, S, residual=dvg0)
+    dvm0 = self.dx(info, "w0_2", nm, R, residual=dvm0)
     del S, R, vg0, vm0
-    dh = self.mlp_backward(mp["enc_grid"], ng, [grid_in], dvg0,
-                           tan=None if T is None else ([img(T.pop("grid_in"), eng.c_in_pad)], (), None))
+    dh = self.mlp_backward(mp["enc_grid"], ng, [grid_in], dvg0,   # (a parameter HVP: zero input tangent)
+                           tan=None if T is None else ([img(T.pop("grid_in"), eng.c_in_pad)], (), None),
+                           xdot=[None])
     dx = None
     if dgrid_in:
       w0t, n = self.input_transposed()
@@ -898,13 +1045,15 @@ class Backward:
         out.data_ptr(), D, self._st()), "gcb_layernorm_jvp_dirs")
     return out
 
-  def proj_tangent(self, rows: int, v, dv: Optional[torch.Tensor], w_packed, tw_packed):
+  def proj_tangent(self, rows: int, v, dv: Optional[torch.Tensor], w_packed, tw_packed,
+                   dirs: Optional[int] = None):
     """Tangent of a node projection v W (a pre-gathered edge layer's sender or receiver block), a
-    stacked table of self.dirs directions of `rows` rows: dv W + v W-dot, each term only when its
-    tangent exists (dv, the image tw_packed of W-dot); None when neither does."""
+    stacked table of `dirs` (default self.dirs) directions of `rows` rows: dv W + v W-dot, each term
+    only when its tangent exists (dv, the image tw_packed of W-dot, one direction); None when neither
+    does."""
     out = None
     if dv is not None:
-      out = self.projection(self.dir_rows(rows), self.tab(dv), w_packed)
+      out = self.projection(self.dir_rows(rows, dirs), self.tab(dv), w_packed)
     if tw_packed is not None:
       t = self.empty(rows)
       self.layer(rows, [v], tw_packed, self.zero_bias, out_y=t,
@@ -984,13 +1133,16 @@ class Backward:
     stacked tables of `dirs` directions the forward forms anyway: keeping them costs no copy, and their
     memory grows with the directions.  Without them nothing more is kept or launched.
 
-    With `wts` (weight_tangents; param_jvp, one direction, no snapshots) the tangent is also along those
-    parameter tangents: every MLP with one adds its weight-tangent terms (mlp_jvp, proj_tangent), and
-    the tangents that are zero along the inputs alone are formed when their parameters have one: the
-    mesh-node encoder's (so the grid2mesh receiver block and the mesh-node residual get theirs), the
-    edge embedders' and with it e_0 of the processor."""
-    if wts and (dirs != 1 or tsnaps is not None):
-      raise ValueError("parameter tangents run one direction without snapshots")
+    With `wts` (weight_tangents; param_jvp and loss_and_param_hvp, one direction) the tangent is also
+    along those parameter tangents: every MLP with one adds its weight-tangent terms (mlp_jvp,
+    proj_tangent), and the tangents that are zero along the inputs alone are formed when their
+    parameters have one: the mesh-node encoder's (so the grid2mesh receiver block and the mesh-node
+    residual get theirs), the edge embedders' and with it e_0 of the processor.  With snapshots as well
+    (a parameter Hessian-vector product), tsnaps also keeps v-dot_m0 ("vm0") and e-dot_0 (e[0]) when they
+    exist; the embedded edges' tangents of the two bipartite graphs are not kept (the backward pass
+    recomputes them per chunk)."""
+    if wts and dirs != 1:
+      raise ValueError("parameter tangents run one direction")
     self.dirs, self.wts = int(dirs), wts or {}
     try:
       return self._tangent(grid_in_img, dgrid_in_img, snaps, tsnaps)
@@ -1030,6 +1182,8 @@ class Backward:
     else:
       dv = self.mlp_jvp(info, nm, [tab(vm0), img(eng.mesh_agg_img)], [tab(dvm0), tab(dagg)],
                         residual=dvm0)
+      if keep:
+        ts["vm0"] = dvm0
       del dvm0
     if keep:
       ts.update(vg0=dvg0, agg1=dagg)
@@ -1053,6 +1207,8 @@ class Backward:
         e_k = tab(self.fwd_mlp(mp["enc_e_mesh"], m.e_mesh, feat))
         if mp["enc_e_mesh"].stem in self.wts:    # e_0 has a tangent through the embedder's parameters
           de = self.mlp_jvp(mp["enc_e_mesh"], m.e_mesh, feat, [])
+          if keep:
+            ts["e"][0] = de
       else:
         e_k = img(eng.mesh_edge_img.clone())
       eng.run_stage("process_step", k)
@@ -1102,6 +1258,15 @@ class Backward:
     del vg1, dagg
     return self.mlp_jvp(mp["dec_grid"], ng, [img(eng.grid_lat_img)], [tab(dvg)])
 
+  def weight_jvp(self, info: _MlpInfo, rows: int, segs) -> torch.Tensor:
+    """The tangent of an MLP of constant inputs along its parameter tangent (self.wts), one direction
+    (mlp_jvp with no input tangent), inside a walk of any direction count."""
+    dirs, self.dirs = self.dirs, 1
+    try:
+      return self.mlp_jvp(info, rows, segs, [])
+    finally:
+      self.dirs = dirs
+
   def edge_iota(self) -> torch.Tensor:
     """0..dir_rows(E_mesh)-1 (the identity gather of the edge-tangent update e' = e + m over every
     direction), made on first use."""
@@ -1111,14 +1276,15 @@ class Backward:
     return self._edge_iota
 
   # -- result ----------------------------------------------------------------------------------------
-  def _accumulators(self) -> Dict[str, Dict[str, torch.Tensor]]:
-    """The valid slices of the gradient accumulators (views), keyed and shaped like the params; the
-    parameters the step never reads (the mesh2grid mesh-node MLP) are absent."""
+  def _accumulators(self, tangent: bool = False) -> Dict[str, Dict[str, torch.Tensor]]:
+    """The valid slices of the gradient accumulators (views; `tangent`: those of a parameter
+    Hessian-vector product, info.gt), keyed and shaped like the params; the parameters the step never
+    reads (the mesh2grid mesh-node MLP) are absent."""
     out: Dict[str, Dict[str, torch.Tensor]] = {}
     for info in self._all:
       l0, l1 = f"{info.stem}_mlp/~/linear_0", f"{info.stem}_mlp/~/linear_1"
       k_real = self.shapes[l0]["w"][0]
-      g = info.g
+      g = info.gt if tangent else info.g
       if len(info.k_segs) == 1:
         w0 = g["w0"][:k_real]
       else:
@@ -1130,11 +1296,12 @@ class Backward:
         out[f"{info.stem}_layer_norm"] = {"scale": g["scale"], "offset": g["offset"]}
     return out
 
-  def grads(self) -> Dict[str, Dict[str, torch.Tensor]]:
-    """Device fp32 gradients keyed and shaped like the params; parameters the step never reads (the
-    mesh2grid mesh-node MLP) get zeros."""
+  def grads(self, tangent: bool = False) -> Dict[str, Dict[str, torch.Tensor]]:
+    """Device fp32 gradients keyed and shaped like the params (`tangent`: the Hessian-vector products
+    accumulated by parameter HVPs, zero_hvp); parameters the step never reads (the mesh2grid mesh-node
+    MLP) get zeros."""
     out = {name: {f: t.clone() for f, t in fields.items()}
-           for name, fields in self._accumulators().items()}
+           for name, fields in self._accumulators(tangent).items()}
     for name, fields in self.shapes.items():
       if name not in out:
         out[name] = {f: torch.zeros(shape, dtype=torch.float32, device=self.dev)

@@ -104,3 +104,6 @@ class Bfloat16Cast(graphcast.Predictor):
 
   def loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents, **kwargs):
     return self._predictor.loss_and_param_gnvp(inputs, targets, forcings, param_tangents, **kwargs)
+
+  def loss_and_param_hvp(self, inputs, targets, forcings, param_tangents, **kwargs):
+    return self._predictor.loss_and_param_hvp(inputs, targets, forcings, param_tangents, **kwargs)

@@ -1301,6 +1301,42 @@ int gcb_layernorm_backward_jvp(const float* dy, int32_t ld_dy, const float* z, i
                                          dz, ld_dz, 1, stream);
 }
 
+int gcb_layernorm_backward_jvp_params(const float* dy, int32_t ld_dy, int64_t dir_stride,
+                                      const float* z, int32_t ld_z, const float* zdot, int32_t ld_zdot,
+                                      const float* scale, const float* scale_dot, int64_t rows,
+                                      int32_t n, float* dz, int32_t ld_dz, void* workspace,
+                                      int64_t workspace_bytes, float* dbias, float* dscale,
+                                      float* doffset, float* dbias_dot, float* dscale_dot,
+                                      float* doffset_dot, int32_t accumulate, void* stream) {
+  GCB_CHECK_ARG(dy && z && zdot && scale && dz && workspace, "null pointer");
+  GCB_CHECK_ARG(dbias && dscale && doffset && dbias_dot && dscale_dot && doffset_dot,
+                "null column-sum output");
+  GCB_CHECK_ARG(n == 512, "the LayerNorm backward tangent needs n = 512");
+  GCB_CHECK_ARG(rows >= 0, "rows < 0");
+  GCB_CHECK_ARG(ld_dy >= n && ld_z >= n && ld_zdot >= n && ld_dz >= n, "leading dimension < n");
+  GCB_CHECK_ARG(dir_stride >= rows, "dir_stride < rows");
+  GCB_CHECK_ARG(workspace_bytes >= gcb_rowwise_workspace_bytes(n), "workspace too small");
+  // direction 0: gcb_layernorm_backward itself (its kernel, split and sums)
+  float* sums[3] = {dbias, dscale, doffset};
+  const int status = rowwise_launch(gcb::kRowLayerNorm, dy, ld_dy, z, ld_z, scale, rows, n, dz, ld_dz,
+                                    workspace, workspace_bytes, sums, 3, accumulate, stream);
+  if (status != GCB_OK) return status;
+  // direction 1 and the tangent sums, over the same split; the workspace is reused in stream order
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0, 4.0 * static_cast<double>(rows) * n * 5.0);
+  float* partial = static_cast<float*>(workspace);
+  gcb::layernorm_backward_jvp_params_kernel<<<gcb::kRowSlices, 256, 0, st>>>(
+      dy, ld_dy, dir_stride, z, ld_z, zdot, ld_zdot, scale, scale_dot, rows, dz, ld_dz, partial);
+  GCB_CUDA(cudaGetLastError());
+  float* tsums[3] = {dbias_dot, dscale_dot, doffset_dot};
+  for (int q = 0; q < 3; ++q) {
+    gcb::slices_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(partial + q * n, gcb::kRowSlices,
+                                                               3LL * n, n, tsums[q], accumulate);
+    GCB_CUDA(cudaGetLastError());
+  }
+  return GCB_OK;
+}
+
 int gcb_segment_sum_sorted(const float* msg, int32_t ld_msg, const int32_t* order,
                            const int32_t* ptr, int32_t num_nodes, const int32_t* heavy,
                            int32_t num_heavy, float* out, int32_t ld_out, int32_t width, void* stream) {

@@ -724,6 +724,130 @@ layernorm_backward_jvp_kernel(const float* __restrict__ dy, int ld_dy, const flo
   }
 }
 
+// ---- Hessian-vector products with respect to the parameters (loss_and_param_hvp) ------------------
+// Direction 1 of layernorm_backward_jvp_kernel (one tangent, dy and dydot = rows [0, rows) and
+// [stride, stride + rows)) with the tangent of the scale as well, g-dot = dydot*scale + dy*scale_dot
+// (scale_dot NULL: dydot*scale, so that dzdot is that kernel's bits), and the tangents of the three
+// column sums of rowwise_backward_kernel<kRowLayerNorm, 16>:
+//   sum dzdot (bias), sum dydot*zhat + dy*zhatdot (scale), sum dydot (offset)
+// over rowwise_backward_kernel's row split: block b of kRowSlices owns a contiguous row range, its 8
+// warps stride through it keeping fp64 column sums, and the warps are folded in order into
+// partial[b][q][col].  Direction 0 (dz and its sums) is rowwise_backward_kernel's launch itself.
+__global__ void __launch_bounds__(256)
+layernorm_backward_jvp_params_kernel(const float* __restrict__ dy, int ld_dy, long long stride,
+                                     const float* __restrict__ z, int ld_z,
+                                     const float* __restrict__ zdot, int ld_zdot,
+                                     const float* __restrict__ scale,
+                                     const float* __restrict__ scale_dot, long long rows,
+                                     float* __restrict__ dz, int ld_dz, float* __restrict__ partial) {
+  constexpr int kCols = 16;
+  constexpr int n = kCols * 32;
+  constexpr float kInvN = 1.0f / n;
+  __shared__ double red[8][n];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long per = (rows + kRowSlices - 1) / kRowSlices;
+  const long long r_beg = min(rows, per * blockIdx.x), r_end = min(rows, r_beg + per);
+  double s0[kCols], s1[kCols], s2[kCols];
+#pragma unroll
+  for (int j = 0; j < kCols; ++j) s0[j] = s1[j] = s2[j] = 0.0;
+  for (long long r = r_beg + warp; r < r_end; r += 8) {
+    // the primal statistics, z-hat, g and a = g - mean(g) - zhat m: layernorm_backward_jvp_kernel's
+    float v[kCols];
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) v[j] = z[r * ld_z + lane + 32 * j];
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) s = __fadd_rn(s, v[j]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, o));
+    float var = 0.f;
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) {
+      v[j] = __fmaf_rn(s, -kInvN, v[j]);               // z - mean
+      var = __fmaf_rn(v[j], v[j], var);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) var = __fadd_rn(var, __shfl_xor_sync(0xffffffffu, var, o));
+    const float rstd = rsqrtf(__fmaf_rn(var, kInvN, 1e-5f));
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) v[j] = __fmul_rn(v[j], rstd);   // z-hat
+    float g[kCols], a[kCols];
+    float mg = 0.f, mgz = 0.f;
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) {
+      g[j] = __fmul_rn(dy[r * ld_dy + lane + 32 * j], scale[lane + 32 * j]);
+      mg = __fadd_rn(mg, g[j]);
+      mgz = __fmaf_rn(v[j], g[j], mgz);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      mg = __fadd_rn(mg, __shfl_xor_sync(0xffffffffu, mg, o));
+      mgz = __fadd_rn(mgz, __shfl_xor_sync(0xffffffffu, mgz, o));
+    }
+    const float mgz_n = __fmul_rn(mgz, kInvN);
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) a[j] = __fmaf_rn(v[j], -mgz_n, __fmaf_rn(mg, -kInvN, g[j]));
+    const float rr = __fmul_rn(rstd, rstd);
+    // the tangent: layernorm_backward_jvp_kernel's direction 1, g-dot with the scale's tangent term
+    const long long rt = stride + r;
+    float zd[kCols];
+    float mzd = 0.f, mvz = 0.f;
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) {
+      zd[j] = zdot[r * ld_zdot + lane + 32 * j];
+      mzd = __fadd_rn(mzd, zd[j]);
+      mvz = __fmaf_rn(v[j], zd[j], mvz);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      mzd = __fadd_rn(mzd, __shfl_xor_sync(0xffffffffu, mzd, o));
+      mvz = __fadd_rn(mvz, __shfl_xor_sync(0xffffffffu, mvz, o));
+    }
+    mvz = __fmul_rn(mvz, kInvN);
+    const float nrdot = __fmul_rn(mvz, rr);                          // -rdot
+    float mgd = 0.f, mdot = 0.f;
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) {
+      const int c = lane + 32 * j;
+      zd[j] = __fmul_rn(rstd, __fmaf_rn(v[j], -mvz, __fmaf_rn(mzd, -kInvN, zd[j])));   // zhat-dot
+      float gd = __fmul_rn(dy[rt * ld_dy + c], scale[c]);
+      if (scale_dot) gd = __fmaf_rn(dy[r * ld_dy + c], scale_dot[c], gd);
+      mgd = __fadd_rn(mgd, gd);
+      mdot = __fadd_rn(mdot, __fmaf_rn(v[j], gd, __fmul_rn(g[j], zd[j])));
+      g[j] = gd;                                                     // g is not read again
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      mgd = __fadd_rn(mgd, __shfl_xor_sync(0xffffffffu, mgd, o));
+      mdot = __fadd_rn(mdot, __shfl_xor_sync(0xffffffffu, mdot, o));
+    }
+    mdot = __fmul_rn(mdot, kInvN);
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) {
+      const int c = lane + 32 * j;
+      const float b = __fmaf_rn(v[j], -mdot, __fmaf_rn(-mgz_n, zd[j], __fmaf_rn(mgd, -kInvN, g[j])));
+      const float out = __fmaf_rn(rstd, b, -__fmul_rn(nrdot, a[j]));
+      dz[rt * ld_dz + c] = out;
+      const float d0 = dy[r * ld_dy + c], d1 = dy[rt * ld_dy + c];
+      s0[j] += out;                                                  // bias of the linear before it
+      s1[j] += static_cast<double>(d1) * v[j] + static_cast<double>(d0) * zd[j];   // LayerNorm scale
+      s2[j] += d1;                                                   // LayerNorm offset
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < 3; ++q) {
+#pragma unroll
+    for (int j = 0; j < kCols; ++j) red[warp][lane + 32 * j] = q == 0 ? s0[j] : (q == 1 ? s1[j] : s2[j]);
+    __syncthreads();
+    for (int c = threadIdx.x; c < n; c += 256) {
+      double t = 0.0;
+      for (int w = 0; w < 8; ++w) t += red[w][c];
+      partial[(static_cast<long long>(blockIdx.x) * 3 + q) * n + c] = static_cast<float>(t);
+    }
+    __syncthreads();
+  }
+}
+
 // ---- index operations ----------------------------------------------------------------------------
 // out[i, 0:512] = sum_{j in [ptr[i], ptr[i+1])} msg[order[j], 0:512], summed in j order.  Rows listed
 // in `heavy` (ascending node ids): one 128-thread block each (thread owns one float4 column); every

@@ -1061,17 +1061,22 @@ class Engine:
             self._ptr(add_index), out.data_ptr(), self._stream()), "gcb_unpack_grid_outputs")
 
   # -- parameter tangents (param_jvp, loss_and_param_gnvp) ---------------------------------------------
-  def weight_tangents(self, param_tangents: Mapping[str, Mapping[str, np.ndarray]]):
+  def weight_tangents(self, param_tangents: Mapping[str, Mapping[str, np.ndarray]],
+                      transposed: bool = False):
     """Packs parameter tangents (host float32 arrays keyed and shaped like the params, modules and
     fields optional) into tangent weight images on the device (Backward.weight_tangents), for
-    input_jvp_element and param_gnvp_element; call input_grads_begin() or grads_begin() first.  The
-    engine's weights and weights_version are not touched."""
+    input_jvp_element, param_gnvp_element and (with `transposed`: also their transposed images,
+    Backward.pack_transposed_tangents) param_hvp_element; call input_grads_begin() or grads_begin()
+    first.  The engine's weights and weights_version are not touched."""
     if self._backward is None:
       raise RuntimeError("call input_grads_begin() or grads_begin() first")
     with self._on_device():
       dev = {name: {f: torch.as_tensor(np.ascontiguousarray(a, np.float32)).to(self.device)
                     for f, a in fields.items()} for name, fields in param_tangents.items()}
-      return self._backward.weight_tangents(dev)
+      wts = self._backward.weight_tangents(dev)
+      if transposed:
+        self._backward.pack_transposed_tangents(wts)
+      return wts
 
   def param_gnvp_element(self, targets_planes: torch.Tensor, lat_weight: torch.Tensor,
                          coef: torch.Tensor, weight_tangents, *, channel_sums: torch.Tensor,
@@ -1105,6 +1110,58 @@ class Engine:
     self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
     with self._on_device():
       self._backward.element(grid_in, g_out, snaps)
+
+  # -- parameter Hessian-vector products (loss_and_param_hvp) -----------------------------------------
+  def param_hvp_begin(self) -> None:
+    """grads_begin() for loss_and_param_hvp: zeroes the gradient accumulators and those of the
+    Hessian-vector product (param_hvp)."""
+    self.grads_begin()
+    self._backward.zero_hvp()
+
+  def param_hvp_element(self, targets_planes: torch.Tensor, lat_weight: torch.Tensor,
+                        coef: torch.Tensor, weight_tangents, *, channel_sums: torch.Tensor,
+                        **affine) -> None:
+    """One batch element of a Hessian-vector product of the loss with respect to the parameters (call
+    param_hvp_begin() first; weight_tangents from weight_tangents(..., transposed=True)).
+
+    The step runs from the packed grid_in_img with its tangent along the parameter tangents v and a
+    zero input tangent (Backward.tangent(wts=..., snaps=..., tsnaps=...)), keeping the primal and
+    tangent snapshots; the loss sums of that forward go to channel_sums (output_loss).  The seed has
+    two directions: direction 0 is loss_and_grads_element's (gcb_output_loss_grad), direction 1 its
+    tangent.  Targets and the normalisation do not move with the parameters, so that tangent is
+    coef * lat_weight * y-dot (gcb_output_loss_gn_seed).  One coupled backward walk
+    (Backward.element(dirs=2, hvp=..., param_grads=True)) then ADDS this element's gradient to the
+    gradient accumulators, bit for bit as loss_and_grads_element does, and its H v to those of
+    param_hvp()."""
+    if self._backward is None:
+      raise RuntimeError("call param_hvp_begin() first")
+    bw = self._backward
+    grid_in = self.grid_in_img
+    n_lat = lat_weight.shape[0]
+    stride = bw.dir_stride(self.num_grid)
+    with self._on_device():
+      dgrid_in = self._image(self.num_grid, self.c_in_pad)
+      snaps, tsnaps = {}, {}
+      dy = bw.tangent(grid_in, dgrid_in, snaps=snaps, tsnaps=tsnaps, wts=weight_tangents)
+      del dgrid_in
+      self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
+      g_out = torch.zeros([stride + self.num_grid, 256], dtype=torch.float32, device=self.device)
+      _native.check(self._lib.gcb_output_loss_grad(
+          self.grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat,
+          self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
+          self._ptr(affine.get("add_planes")), self._ptr(affine.get("add_plane_index")),
+          targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), g_out.data_ptr(), 256,
+          self._stream()), "gcb_output_loss_grad")
+      _native.check(self._lib.gcb_output_loss_gn_seed(
+          dy.data_ptr(), dy.shape[1], self.n_out, n_lat, self.num_grid // n_lat, lat_weight.data_ptr(),
+          coef.data_ptr(), g_out[stride:].data_ptr(), 256, self._stream()), "gcb_output_loss_gn_seed")
+      del dy
+      bw.element(grid_in, g_out, snaps, dirs=2, hvp=tsnaps, wts=weight_tangents)
+
+  def param_hvp(self):
+    """The accumulated Hessian-vector products of param_hvp_element: device fp32 tensors keyed and
+    shaped like the params, zeros for the parameters the step never reads."""
+    return self._backward.grads(tangent=True)
 
   def broadcast_grad_sum(self, a: torch.Tensor, n_lat: int, rows: torch.Tensor, mode: int,
                          out: torch.Tensor, accumulate: bool) -> None:

@@ -167,6 +167,12 @@ class Predictor(abc.ABC):
     a dict shaped like the params."""
     raise NotImplementedError(f"{type(self).__name__} does not implement parameter tangents")
 
+  def loss_and_param_hvp(self, inputs, targets, forcings, param_tangents, **optional_kwargs):
+    """Returns (loss, diagnostics, grads, hvp): `loss` / `diagnostics` as `loss` returns them, `grads`
+    as loss_and_grads returns it, `hvp` the Hessian of loss.mean() with respect to the params times
+    `param_tangents`, a dict shaped like the params."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement parameter tangents")
+
 
 # Per-variable weights of GraphCast's loss (reference graphcast.py:341-356); others weigh 1.
 LOSS_PER_VARIABLE_WEIGHTS = {
@@ -535,6 +541,59 @@ class GraphCast(Predictor):
     coef * lat_weight * y-dot (gcb_output_loss_gn_seed), then the parameter backward pass of
     loss_and_grads from that seed, which recomputes the step with its snapshots."""
     return self._loss_and_param_gnvp(inputs, targets, forcings, param_tangents, norm=None)
+
+  def loss_and_param_hvp(self, inputs, targets, forcings, param_tangents, **unused_kwargs):
+    """(loss, diagnostics, grads, hvp) for one target time: what jax.jvp(jax.grad(loss), (params,),
+    (v,)) gives, with the loss and gradient of loss_and_grads.
+
+    `loss` and `diagnostics` are bit for bit what `loss()` returns, `grads` what loss_and_grads
+    returns.  `hvp` is H v, H the Hessian of loss.mean() (the scalar of loss_and_grads; a batch
+    averages over its elements) with respect to the params and v = param_tangents (a dict as param_jvp
+    takes it, modules and fields left out being zero): a dict shaped like the params, float32 numpy
+    arrays, with exact zeros for the mesh2grid mesh-node MLP, which the step never reads.  Unlike
+    loss_and_param_gnvp's G v it keeps the residual term, the loss residual times the network's second
+    derivatives.  Every refusal of param_jvp and loss_and_grads applies, before anything runs;
+    several target times raise NotImplementedError.
+
+    Per batch element (Engine.param_hvp_element): one forward with the tangent along v that keeps its
+    tangent tables, then one backward walk of two directions, the gradient and its tangent, which
+    accumulates both the parameter gradients and their tangents."""
+    return self._loss_and_param_hvp(inputs, targets, forcings, param_tangents, norm=None)
+
+  def _loss_and_param_hvp(self, inputs, targets, forcings, param_tangents,
+                          norm: Optional[FusedNormalization]):
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    if targets.sizes.get("time", 1) != 1:
+      raise NotImplementedError("parameter Hessian-vector products cover one target time (several "
+                                "are not provided)")
+    tangents = self._checked_param_tangents(param_tangents)
+    batch = dict(inputs.sizes).get("batch", 1)
+    num_grid = inputs.sizes["lat"] * inputs.sizes["lon"]
+    slabs = model_utils.channel_layout(targets)
+    coef = 2.0 * losses.channel_kappa(slabs, num_grid, LOSS_PER_VARIABLE_WEIGHTS) / batch
+    state = {}
+
+    def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
+      eng = self._engine
+      if "wt" not in state:
+        eng.param_hvp_begin()
+        self._release_idle_staging()
+        state["wt"] = eng.weight_tangents(tangents, transposed=True)
+        state["lat_weight"] = self._lat_weight(targets, eng.device)
+        state["coef"] = torch.as_tensor(np.asarray(coef, np.float64)).to(eng.device)
+      eng.param_hvp_element(planes_tgt, state["lat_weight"], state["coef"], state["wt"],
+                            channel_sums=channel_sums, **affine)
+
+    self._call(inputs, targets, forcings, norm=norm, targets=targets, predictions=False,
+               element=element)
+    state.clear()
+    loss, diagnostics = losses.losses_from_channel_sums(
+        self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
+    grads = {name: {f: t.cpu().numpy() for f, t in fields.items()}
+             for name, fields in self._engine.grads().items()}
+    hvp = {name: {f: t.cpu().numpy() for f, t in fields.items()}
+           for name, fields in self._engine.param_hvp().items()}
+    return loss, diagnostics, grads, hvp
 
   def _param_tangent_run(self, inputs, targets_template, forcings, param_tangents, num_steps: int,
                          plan=None) -> "_TangentRun":

@@ -346,6 +346,19 @@ class InputsAndResiduals(graphcast.Predictor):
     return self._predictor._loss_and_param_gnvp(inputs, targets, forcings, param_tangents,
                                                 norm=consts)
 
+  def loss_and_param_hvp(self, inputs, targets, forcings, param_tangents, **kwargs):
+    """(loss, diagnostics, grads, hvp) of `loss` (GraphCast.loss_and_param_hvp), with the
+    normalisation fused into the kernels as in `loss`.  GraphCast only."""
+    self._refuse_unfused()
+    if xs.from_xarray(targets).sizes.get("time", 1) != 1:
+      raise NotImplementedError("parameter Hessian-vector products cover one target time (several "
+                                "are not provided)")
+    self._predictor._checked_param_tangents(param_tangents)
+    inputs, targets, forcings, consts = self._fused_for(inputs, targets, forcings,
+                                                        "parameter gradients")
+    return self._predictor._loss_and_param_hvp(inputs, targets, forcings, param_tangents,
+                                               norm=consts)
+
   def _refuse_unfused(self) -> None:
     if not self._fuses():
       raise NotImplementedError("parameter gradients need a GraphCast predictor directly inside "

@@ -506,6 +506,29 @@ int gcb_layernorm_backward_jvp(const float* dy, int32_t ld_dy, const float* z, i
                                const float* zdot, int32_t ld_zdot, const float* scale, int64_t rows,
                                int32_t n, int64_t dir_stride, float* dz, int32_t ld_dz, void* stream);
 
+/* Hessian-vector products with respect to the parameters (GraphCast.loss_and_param_hvp): the LayerNorm
+ * backward of two directions [dy; dydot] (row r of direction 1 is row dir_stride + r, dir_stride >=
+ * rows) at z and its tangent zdot ([rows] rows, ld_zdot), with the parameter gradients and their
+ * tangents.  n = 512.
+ *   Direction 0: dz and the sums dbias += sum dz, dscale += sum dy*zhat, doffset += sum dy, bit for bit
+ *     gcb_layernorm_backward (the same launch: its row split, fp64 per-warp sums, ordered warp fold and
+ *     second-pass reduction).
+ *   Direction 1: dzdot, the tangent of dz along (dydot, zdot, scale_dot), where g = dy*scale has the
+ *     tangent dydot*scale + dy*scale_dot; scale_dot ([512]) may be NULL, and dzdot is then bit for bit
+ *     direction 1 of gcb_layernorm_backward_jvp.  Its sums, over the same row split:
+ *     dbias_dot += sum dzdot, dscale_dot += sum dydot*zhat + dy*zhatdot, doffset_dot += sum dydot.
+ * accumulate = 0 overwrites the six [512] outputs instead.  The offset's tangent does not enter the
+ * backward pass.  workspace: gcb_rowwise_workspace_bytes(512) bytes, reused by both directions in stream
+ * order.  dz may not alias dy, z or zdot; its pad rows between directions are not written.
+ * Deterministic. */
+int gcb_layernorm_backward_jvp_params(const float* dy, int32_t ld_dy, int64_t dir_stride,
+                                      const float* z, int32_t ld_z, const float* zdot, int32_t ld_zdot,
+                                      const float* scale, const float* scale_dot, int64_t rows,
+                                      int32_t n, float* dz, int32_t ld_dz, void* workspace,
+                                      int64_t workspace_bytes, float* dbias, float* dscale,
+                                      float* doffset, float* dbias_dot, float* dscale_dot,
+                                      float* doffset_dot, int32_t accumulate, void* stream);
+
 /* Backward of a gather v[senders] (jax_gather, utils/typed_graph_net.py:124-125,431-445):
  *   out[i, 0:512] = sum_{j in [ptr[i], ptr[i+1])} msg[order[j], 0:512]
  * (order / ptr: the sender CSR of an edge set, host-built), summed in j order; the rows listed in
@@ -789,7 +812,7 @@ typedef enum {
                              * gcb_layernorm_jvp, gcb_swish_jvp, gcb_layernorm_jvp_dirs,
                              * gcb_layernorm_backward_dirs, gcb_swish_backward_jvp(_dirs),
                              * gcb_layernorm_backward_jvp(_dirs), gcb_layernorm_jvp_params,
-                             * gcb_output_loss_gn_seed */
+                             * gcb_output_loss_gn_seed, gcb_layernorm_backward_jvp_params */
   GCB_KIND_NOISE = 11       /* gcb_add_gaussian_noise */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);

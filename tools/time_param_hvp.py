@@ -1,0 +1,87 @@
+"""Seconds per call and peak device memory of the parameter Hessian-vector product (loss_and_param_hvp)
+against the Gauss-Newton product (loss_and_param_gnvp) and the central difference it replaces (two
+loss_and_grads calls).
+
+  python tools/time_param_hvp.py [--reps 3]
+
+Case: InputsAndResiduals(GraphCast) at 1 deg / 13 levels (TASK_13), bf16x3, B = 1, T = 1, random
+tangents on every parameter and random targets.  After one warm-up of each, the calls alternate in one
+process, rep by rep, so that clock drift reaches all of them alike.  Times are CUDA events around one
+synchronised call: median, min and max of --reps; the peak is torch.cuda.max_memory_allocated over one
+more call of each.  The card name and power limit are read in the same run, and the SM clock is sampled
+while the calls run (bench.ClockSampler; nvidia-smi, read-only)."""
+import argparse
+import gc
+import os
+import sys
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
+
+from graphcast_b200 import graphcast, normalization, synthetic  # noqa: E402
+from test_gpu_loss import _stats  # noqa: E402
+from time_input_grads import _card, _peak  # noqa: E402
+from time_input_jvp import _random_like  # noqa: E402
+from bench import ClockSampler  # noqa: E402
+
+
+def _once(fn) -> float:
+  torch.cuda.synchronize()
+  start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+  start.record()
+  fn()
+  end.record()
+  torch.cuda.synchronize()
+  return start.elapsed_time(end) / 1e3
+
+
+def main():
+  ap = argparse.ArgumentParser()
+  ap.add_argument("--reps", type=int, default=3)
+  args = ap.parse_args()
+  print(f"card: {_card()}", flush=True)
+  task, resolution, mesh_size = graphcast.TASK_13, 1.0, 5
+  inputs, template, forcings = synthetic.make_example(task, resolution, batch=1, num_target_steps=1,
+                                                      seed=2)
+  rng = np.random.default_rng(3)
+  targets = _random_like(template, rng)
+  cfg = graphcast.ModelConfig(resolution, mesh_size, 512, 16, 1, 0.6)
+  params = graphcast.init_params(cfg, task, synthetic.num_input_channels(task), seed=1)
+  v = {n: {f: (rng.standard_normal(np.shape(a)) * (float(np.std(a)) or 0.1)).astype(np.float32)
+           for f, a in fs.items()} for n, fs in params.items()}
+  model = graphcast.GraphCast(cfg, task, params=params)
+  pred = normalization.InputsAndResiduals(model, *_stats(task, seed=1))
+  calls = {
+      "loss_and_param_hvp": lambda: pred.loss_and_param_hvp(inputs, targets, forcings, v),
+      "loss_and_param_gnvp": lambda: pred.loss_and_param_gnvp(inputs, targets, forcings, v),
+      "2 x loss_and_grads": lambda: (pred.loss_and_grads(inputs, targets, forcings),
+                                     pred.loss_and_grads(inputs, targets, forcings)),
+  }
+  for fn in calls.values():
+    fn()
+  clocks = ClockSampler()
+  clocks.start()
+  times = {what: [] for what in calls}
+  for _ in range(args.reps):
+    for what, fn in calls.items():
+      times[what].append(_once(fn))
+  clk = clocks.stop()
+  peaks = {}
+  for what, fn in calls.items():
+    gc.collect()
+    torch.cuda.empty_cache()
+    peaks[what] = _peak(fn)
+  for what, ts in times.items():
+    print(f"{what}: {np.median(ts):.3f} s [{min(ts):.3f}, {max(ts):.3f}] (median [min, max] of "
+          f"{args.reps}), peak {peaks[what]:.1f} GiB", flush=True)
+  h = np.median(times["loss_and_param_hvp"])
+  print(f"loss_and_param_hvp / loss_and_param_gnvp {h / np.median(times['loss_and_param_gnvp']):.2f}, "
+        f"/ 2 x loss_and_grads {h / np.median(times['2 x loss_and_grads']):.2f}; SM clock under load "
+        f"{clk['sm_mhz']} MHz ({clk.get('samples', 0)} samples, reasons {clk['reasons']})", flush=True)
+
+
+if __name__ == "__main__":
+  main()
