@@ -160,6 +160,9 @@ EXPORTS = {
     "gcb_output_loss_grad_feedback": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                 _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp,
                                                 C.c_int32, _fp, _fp, _fp, _fp, C.c_int32, _fp]),
+    "gcb_output_loss_gn_seed_feedback": (C.c_int, [_fp, C.c_int32, C.c_int32, C.c_int32, _fp, _fp,
+                                                   _fp, _fp, _fp, C.c_int32, _fp, _fp, _fp, _fp,
+                                                   C.c_int32, _fp]),
     "gcb_input_grad": (C.c_int, [_fp, C.c_int32, C.c_int64, C.c_int32, _fp, _fp, _fp, C.c_int32,
                                  _fp]),
     "gcb_output_cotangent_grad_feedback": (C.c_int, [C.c_int32, C.c_int64, _fp, _fp, _fp, _fp,

@@ -255,7 +255,8 @@ class Predictor(graphcast.Predictor):
     return parts
 
   @staticmethod
-  def _checkpointed_loss(model, norm_of, inputs, targets, forcings, tangent_run=None):
+  def _checkpointed_loss(model, norm_of, inputs, targets, forcings, tangent_run=None,
+                         keep_predictions: bool = False):
     """The forward of a gradient over several target times: the device path of `loss`, which also
     keeps every step's input and target planes in pinned host memory (graphcast.StepStash).  Returns
     (loss, diagnostics, stash, first step's {inputs, targets, forcings, norm}, latitude weights,
@@ -266,7 +267,9 @@ class Predictor(graphcast.Predictor):
     With tangent_run (a graphcast._TangentRun of one direction: loss_and_input_hvp; of K directions:
     a pass of batched_loss_and_input_hvp), every step also carries the input tangent planes of every
     direction on the device (GraphCast._device_loss_tangent) and keeps them in pinned host memory too:
-    first["tangents"] is that StepStash."""
+    first["tangents"] is that StepStash.  keep_predictions (a run of one direction along parameter
+    tangents: loss_and_param_gnvp): it keeps each step's prediction tangents [batch, n_out, Ng]
+    instead."""
     records, first = [], {}
     stash = None
 
@@ -277,7 +280,7 @@ class Predictor(graphcast.Predictor):
         finish, predictions, sums = model._device_loss(inputs, targets_template, forcings, norm, True)
       else:
         finish, predictions, sums, tangent = model._device_loss_tangent(
-            inputs, targets_template, forcings, norm, tangent_run)
+            inputs, targets_template, forcings, norm, tangent_run, keep_predictions)
       records.append((finish, sums))
       if stash is None:
         stash = graphcast.StepStash(model.engine.device)
@@ -507,14 +510,45 @@ class Predictor(graphcast.Predictor):
     return self._tangent_rollout(inputs, targets_template, forcings, None, None, directions=False,
                                  param_tangents=param_tangents)
 
-  def loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents, **kwargs):
-    """(loss, diagnostics, gnvp) of one target time (GraphCast.loss_and_param_gnvp), delegated to the
-    inner predictor; Gauss-Newton products over several target times are not provided."""
-    targets = xs.from_xarray(targets)
-    if targets.sizes["time"] != 1:
-      raise NotImplementedError("Gauss-Newton products cover one target time (several are not "
-                                "provided)")
-    return self._predictor.loss_and_param_gnvp(inputs, targets, forcings, param_tangents, **kwargs)
+  def loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents, rng=None, *,
+                          _noise_fold: int = 0, **kwargs):
+    """(loss, diagnostics, gnvp): `loss` and `diagnostics` exactly as `loss` returns them, `gnvp` the
+    generalised Gauss-Newton matrix of loss.mean() with respect to the params times v =
+    param_tangents (a dict as param_jvp takes it), a dict shaped like the params (float32 numpy, exact
+    zeros for the mesh2grid mesh-node MLP).  One target time delegates to the inner predictor
+    (GraphCast.loss_and_param_gnvp).
+
+    Several target times need gradient_checkpointing=True, and GraphCast directly or under a fused
+    InputsAndResiduals.  gnvp is then sum_t J_t^T Lambda_t J_t v: r_t the normalised residual of step t,
+    J_t = dr_t / d params through the whole rollout (fed-back predictions included) and Lambda_t =
+    diag(coef * lat_weight), coef = 2 kappa / (batch * steps), the Hessian of the loss in r_t.  It is
+    positive semi-definite, and where every step's targets equal the rollout's own predictions it is
+    the full Hessian of the multi-step loss times v.  The forward is the rollout of param_jvp with the
+    fused loss, which keeps every step's input and target planes and prediction tangents J_t v in pinned
+    host memory; the backward then walks the steps last first as loss_and_grads does, each seeded with
+    Lambda_t r-dot_t plus the feedback of the following step (gcb_output_loss_gn_seed_feedback).  With
+    noise, everything is taken at noisy_inputs(inputs, targets, forcings, rng)."""
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    forcings = xs.from_xarray(forcings)
+    if targets.sizes["time"] == 1:
+      return self._predictor.loss_and_param_gnvp(inputs, targets, forcings, param_tangents, **kwargs)
+    if not self._gradient_checkpointing:
+      raise NotImplementedError(
+          "Gauss-Newton products cover one target time without gradient checkpointing: over several "
+          "they recompute every step from its saved inputs; construct autoregressive.Predictor with "
+          "gradient_checkpointing=True")
+    model, norm_of = self._checkpointed_parts(inputs, targets, forcings, "Gauss-Newton products")
+    one = lambda ds: ds.isel(time=slice(0, 1))
+    run = model._param_tangent_run(inputs, targets, forcings, param_tangents, targets.sizes["time"],
+                                   feedback.FeedbackPlan(inputs, one(targets), one(forcings)))
+    loss, diagnostics, stash, first, lat_weight, coef = self._checkpointed_loss(
+        model, norm_of, self._noised(inputs, targets, forcings, rng, _noise_fold), targets, forcings,
+        tangent_run=run, keep_predictions=True)
+    del run
+    plan = feedback.FeedbackPlan(first["inputs"], first["targets"], first["forcings"])
+    gnvp = model._bptt_grads(stash, plan, first["norm"], lat_weight, coef,
+                             pred_tangents=first["tangents"])
+    return loss, diagnostics, gnvp
 
   def loss_and_param_hvp(self, inputs, targets, forcings, param_tangents, **kwargs):
     """(loss, diagnostics, grads, hvp) of one target time (GraphCast.loss_and_param_hvp), delegated to

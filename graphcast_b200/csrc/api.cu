@@ -971,6 +971,31 @@ int gcb_output_loss_grad_feedback(const float* y, int32_t ld_y, int32_t n_out, i
   return GCB_OK;
 }
 
+int gcb_output_loss_gn_seed_feedback(const float* pdot, int32_t n_out, int32_t n_lat, int32_t n_lon,
+                                     const float* scale, const float* lat_weight, const double* coef,
+                                     const float* a_next, const int32_t* dpred_row, int32_t n_rows,
+                                     const int32_t* resid_channel, const int32_t* carry_row,
+                                     float* a_out, float* g, int32_t ld_g, void* stream) {
+  GCB_CHECK_ARG(pdot && lat_weight && coef && g, "null pointer");
+  GCB_CHECK_ARG(n_out > 0 && ld_g >= n_out, "ld_g too small");
+  GCB_CHECK_ARG(n_lat > 0 && n_lon > 0, "empty grid");
+  GCB_CHECK_ARG(a_next == nullptr || dpred_row != nullptr, "a_next needs dpred_row");
+  GCB_CHECK_ARG(n_rows >= 0 && (n_rows == 0 || (a_out && resid_channel)), "rows need a_out and resid_channel");
+  const long long n_nodes = static_cast<long long>(n_lat) * n_lon;
+  const int c_tiles = (n_out + 31) / 32, r_tiles = (n_rows + 31) / 32;
+  GCB_CHECK_ARG(c_tiles + r_tiles <= 65535, "too many channels / rows");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // algorithmic bytes: the tangent read and g written, the rows written and the feedback rows read once
+  ProfScope prof(st, GCB_KIND_ROWWISE_BWD, 0.0,
+                 4.0 * n_nodes * (n_out * (2.0 + (a_next ? 1.0 : 0.0)) + n_rows * (a_next ? 2.0 : 1.0)));
+  dim3 grid(static_cast<unsigned>((n_nodes + 31) / 32), static_cast<unsigned>(c_tiles + r_tiles));
+  gcb::output_loss_gn_seed_feedback_kernel<<<grid, 256, 0, st>>>(
+      pdot, n_out, n_lon, n_nodes, scale, lat_weight, coef, a_next, dpred_row, n_rows, resid_channel,
+      carry_row, a_out, g, ld_g, c_tiles);
+  GCB_CUDA(cudaGetLastError());
+  return GCB_OK;
+}
+
 int gcb_input_grad(const float* dx, int32_t ld_dx, int64_t n_nodes, int32_t n_rows,
                    const int32_t* channel, const float* scale, float* a, int32_t accumulate,
                    void* stream) {

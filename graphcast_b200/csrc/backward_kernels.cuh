@@ -1068,6 +1068,84 @@ output_loss_grad_feedback_kernel(const float* __restrict__ y, int ld_y, int n_ou
   }
 }
 
+// The seed of a Gauss-Newton product over several target times.  The loss is a quadratic in the
+// normalised residual r = y - t_norm = (pred - target) / scale, so its Gauss-Newton cotangent is
+// coef[c] * w * d with d = pdot / scale (fp32, true division; scale NULL = 1) the tangent of r, pdot
+// [n_out, n_nodes] the channel-major tangent of the physical predictions.  With d in place of y - t_norm
+// this is output_loss_grad_feedback_kernel's arithmetic:
+//   g[node, c]     = coef[c] * w * d + scale[c] * a_next[dpred_row[c], node]   (fp64, rounded once)
+//   a_out[r, node] = c >= 0 ? (float)(coef[c] * w * d / scale[c] + a_next[dpred_row[c], node]) : 0
+//                    (+ a_next[carry_row[r], node] when carry_row[r] >= 0)
+// d is rounded as that kernel rounds y - t_norm with t_norm = +0, so with scale NULL both outputs are its
+// bits for y = pdot^T and all-zero targets.  The c-tile blocks transpose d and the feedback row through
+// the 32 x 32 shared-memory tiles; the row blocks read pdot channel-major as they write a_out.
+__device__ __forceinline__ float gn_residual_tangent(int c, long long node, long long n_nodes,
+                                                     const float* __restrict__ scale,
+                                                     const float* __restrict__ pdot) {
+  const float p = pdot[static_cast<long long>(c) * n_nodes + node];
+  return __fsub_rn(scale ? __fdiv_rn(p, scale[c]) : p, 0.f);
+}
+
+__global__ void __launch_bounds__(256)
+output_loss_gn_seed_feedback_kernel(const float* __restrict__ pdot, int n_out, int n_lon,
+                                    long long n_nodes, const float* __restrict__ scale,
+                                    const float* __restrict__ lat_weight, const double* __restrict__ coef,
+                                    const float* __restrict__ a_next, const int* __restrict__ dpred_row,
+                                    int n_rows, const int* __restrict__ resid_channel,
+                                    const int* __restrict__ carry_row, float* __restrict__ a_out,
+                                    float* __restrict__ g, int ld_g, int c_tiles) {
+  const long long node0 = static_cast<long long>(blockIdx.x) * 32;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  if (static_cast<int>(blockIdx.y) < c_tiles) {
+    __shared__ float tile[32][33];
+    __shared__ float tile_dp[32][33];
+    const int c0 = blockIdx.y * 32;
+    for (int r = ty; r < 32; r += 8) {
+      const int c = c0 + r;
+      const long long node = node0 + tx;
+      float d = 0.f, dp = 0.f;
+      if (c < n_out && node < n_nodes) {
+        d = gn_residual_tangent(c, node, n_nodes, scale, pdot);
+        const int q = a_next ? dpred_row[c] : -1;
+        if (q >= 0) dp = a_next[static_cast<long long>(q) * n_nodes + node];
+      }
+      tile[r][tx] = d;
+      tile_dp[r][tx] = dp;
+    }
+    __syncthreads();
+    for (int r = ty; r < 32; r += 8) {
+      const long long node = node0 + r;
+      const int c = c0 + tx;
+      if (c < n_out && node < n_nodes) {
+        const double d = static_cast<double>(tile[tx][r]);
+        double v = coef[c] * static_cast<double>(lat_weight[node / n_lon]) * d;
+        if (a_next && dpred_row[c] >= 0)
+          v += static_cast<double>(scale ? scale[c] : 1.f) * static_cast<double>(tile_dp[tx][r]);
+        g[node * ld_g + c] = static_cast<float>(v);
+      }
+    }
+    return;
+  }
+  const int r0 = (static_cast<int>(blockIdx.y) - c_tiles) * 32;
+  for (int q = ty; q < 32; q += 8) {
+    const int r = r0 + q;
+    const long long node = node0 + tx;
+    if (r >= n_rows || node >= n_nodes) continue;
+    float v = 0.f;
+    const int c = resid_channel[r];
+    if (c >= 0) {
+      const double d = static_cast<double>(gn_residual_tangent(c, node, n_nodes, scale, pdot));
+      const double gl = coef[c] * static_cast<double>(lat_weight[node / n_lon]) * d;
+      const int p = a_next ? dpred_row[c] : -1;
+      const double dp = p >= 0 ? static_cast<double>(a_next[static_cast<long long>(p) * n_nodes + node]) : 0.0;
+      v = static_cast<float>(gl / static_cast<double>(scale ? scale[c] : 1.f) + dp);
+    }
+    const int k = (a_next && carry_row) ? carry_row[r] : -1;
+    if (k >= 0) v = __fadd_rn(v, a_next[static_cast<long long>(k) * n_nodes + node]);
+    a_out[static_cast<long long>(r) * n_nodes + node] = v;
+  }
+}
+
 // Transpose of pack_grid_image_kernel's normalisation for a list of rows (normalization.py:113-146,
 // the input side of InputsAndResiduals): a[r, node] (+)= dx[node, channel[r]] / scale[channel[r]]
 // (true division; scale == NULL divides by 1).  dx is read node-major through a 32 x 32 shared tile,

@@ -805,15 +805,10 @@ class Engine:
 
   def _bptt_element(self, targets_planes, lat_weight, coef, channel_sums, grid_in, fb: "Feedback",
                     input_grad: bool, affine) -> None:
-    grid_in = self.grid_in_img if grid_in is None else grid_in
-    snaps = self._forward_snapshots(grid_in)
-    self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
-    g_out = torch.zeros([self.num_grid, 256], dtype=torch.float32, device=self.device)
-    n_rows = fb.n_rows if input_grad else 0
-    a_out = torch.empty([n_rows, self.num_grid], dtype=torch.float32, device=self.device) \
-        if n_rows else None
     n_lat = lat_weight.shape[0]
-    with self._on_device():
+
+    def seed(g_out, a_out, n_rows):
+      self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
       _native.check(self._lib.gcb_output_loss_grad_feedback(
           self.grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat,
           self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
@@ -821,6 +816,50 @@ class Engine:
           targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), self._ptr(fb.a),
           fb.dpred_row.data_ptr(), n_rows, fb.resid_channel.data_ptr(), fb.carry_row.data_ptr(),
           self._ptr(a_out), g_out.data_ptr(), 256, self._stream()), "gcb_output_loss_grad_feedback")
+    self._bptt_walk(grid_in, fb, input_grad, seed)
+
+  def param_gnvp_bptt_element(self, pred_tangent: torch.Tensor, lat_weight: torch.Tensor,
+                              coef: torch.Tensor, *, feedback: "Feedback", input_grad: bool,
+                              grid_in: Optional[torch.Tensor] = None,
+                              scale: Optional[torch.Tensor] = None) -> None:
+    """One step of one batch element of a Gauss-Newton product over several target times (call
+    grads_begin() first): loss_and_grads_element(feedback=...) with the Gauss-Newton seed in place of
+    the loss seed, and no loss.  pred_tangent [n_out, Ng] is this step's tangent of the physical
+    predictions along the parameter tangents, through the whole rollout before it (the stash of the
+    forward); scale the output normalisation's scale (None: 1).  The step runs again stage by stage
+    from `grid_in` with its snapshots, gcb_output_loss_gn_seed_feedback seeds coef * lat_weight *
+    pred_tangent / scale plus the feedback of the following step, and the backward pass ADDS this
+    step's J^T Lambda J v terms to the gradient accumulators; with input_grad, feedback.a becomes this
+    step's input-plane cotangent (gcb_input_grad).  No tangent runs here: J v is pred_tangent."""
+    if self._backward is None:
+      raise RuntimeError("call grads_begin() first")
+    if (tuple(pred_tangent.shape) != (self.n_out, self.num_grid) or pred_tangent.dtype != torch.float32
+        or not pred_tangent.is_contiguous() or pred_tangent.device != self.device):
+      raise ValueError(f"pred_tangent must be a contiguous float32 [{self.n_out}, {self.num_grid}] "
+                       f"tensor on {self.device}")
+    n_lat = lat_weight.shape[0]
+    fb = feedback
+
+    def seed(g_out, a_out, n_rows):
+      _native.check(self._lib.gcb_output_loss_gn_seed_feedback(
+          pred_tangent.data_ptr(), self.n_out, n_lat, self.num_grid // n_lat, self._ptr(scale),
+          lat_weight.data_ptr(), coef.data_ptr(), self._ptr(fb.a), fb.dpred_row.data_ptr(), n_rows,
+          fb.resid_channel.data_ptr(), fb.carry_row.data_ptr(), self._ptr(a_out), g_out.data_ptr(),
+          256, self._stream()), "gcb_output_loss_gn_seed_feedback")
+    self._bptt_walk(grid_in, fb, input_grad, seed)
+
+  def _bptt_walk(self, grid_in, fb: "Feedback", input_grad: bool, seed) -> None:
+    """The step of a backprop-through-time element: the recompute with snapshots, seed(g_out, a_out,
+    n_rows) (which reads fb.a), the backward pass with parameter gradients and, with input_grad, the
+    input gradient into fb.a."""
+    grid_in = self.grid_in_img if grid_in is None else grid_in
+    snaps = self._forward_snapshots(grid_in)
+    g_out = torch.zeros([self.num_grid, 256], dtype=torch.float32, device=self.device)
+    n_rows = fb.n_rows if input_grad else 0
+    a_out = torch.empty([n_rows, self.num_grid], dtype=torch.float32, device=self.device) \
+        if n_rows else None
+    with self._on_device():
+      seed(g_out, a_out, n_rows)
       fb.a = a_out                         # the following step's rows are consumed: release them
       dx = self._backward.element(grid_in, g_out, snaps, dgrid_in=bool(n_rows))
       if n_rows:

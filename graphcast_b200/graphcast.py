@@ -906,11 +906,17 @@ class GraphCast(Predictor):
     self._planes_bufs[idle] = self._target_bufs[idle] = self._buf_free[idle] = None
 
   def _bptt_grads(self, stash: "StepStash", plan, norm: Optional[FusedNormalization],
-                  lat_weight: torch.Tensor, coef: np.ndarray):
+                  lat_weight: torch.Tensor, coef: np.ndarray,
+                  pred_tangents: Optional["StepStash"] = None):
     """Parameter gradients of the multi-step loss whose steps `stash` holds (backprop through time,
     see autoregressive.Predictor.loss_and_grads).  For every batch element, last step first: the
     step's planes are uploaded again, packed and differentiated by Engine.loss_and_grads_element with
-    the feedback of the following step; the gradients accumulate in this fixed order."""
+    the feedback of the following step; the gradients accumulate in this fixed order.
+
+    With pred_tangents (a StepStash of each step's prediction tangents [batch, n_out, Ng] along the
+    parameter tangents; autoregressive.Predictor.loss_and_param_gnvp) the result is the Gauss-Newton
+    product instead: each step's tangent is uploaded in place of its target planes and seeds
+    Engine.param_gnvp_bptt_element, the rest of the walk unchanged."""
     eng = self._engine
     dev = eng.device
     eng.grads_begin()
@@ -928,7 +934,12 @@ class GraphCast(Predictor):
         (host_in, host_tgt), done = stash.steps[t]
         compute.wait_event(done)
         planes.copy_(host_in[b], non_blocking=True)
-        tgt.copy_(host_tgt[b], non_blocking=True)
+        if pred_tangents is None:
+          tgt.copy_(host_tgt[b], non_blocking=True)
+        else:
+          (host_tangent,), tangent_done = pred_tangents.steps[t]
+          compute.wait_event(tangent_done)
+          tgt.copy_(host_tangent[b], non_blocking=True)
         affine = {}
         if norm is None:
           eng.pack_inputs(planes)
@@ -936,8 +947,12 @@ class GraphCast(Predictor):
           eng.pack_inputs(planes, mean=norm.in_mean, scale=norm.in_scale)
           affine = dict(scale=norm.out_scale, offset=norm.out_offset, add_planes=planes,
                         add_plane_index=norm.add_plane_index)
-        eng.loss_and_grads_element(tgt, lat_weight, coef_dev, channel_sums=scratch, feedback=fb,
-                                   input_grad=t > 0, **affine)
+        if pred_tangents is None:
+          eng.loss_and_grads_element(tgt, lat_weight, coef_dev, channel_sums=scratch, feedback=fb,
+                                     input_grad=t > 0, **affine)
+        else:
+          eng.param_gnvp_bptt_element(tgt, lat_weight, coef_dev, feedback=fb, input_grad=t > 0,
+                                      scale=affine.get("scale"))
     return self._export_grads()
 
   def _loss(self, inputs, targets, forcings, norm: Optional[FusedNormalization], predictions: bool):
@@ -961,13 +976,14 @@ class GraphCast(Predictor):
     return finish, preds, self._channel_sums
 
   def _device_loss_tangent(self, inputs, targets, forcings, norm: Optional[FusedNormalization],
-                           run: "_TangentRun"):
+                           run: "_TangentRun", keep_predictions: bool = False):
     """_device_loss with the tangent planes of `run` carried through the step (the forward of
     loss_and_input_hvp over several target times): every batch element runs the stage-wise forward with
     its tangent (_TangentRun.element, which also feeds the next step's tangent planes), then
     output_loss on that forward, which is the step _device_loss runs.  Returns (finish, predictions,
     channel_sums, this step's input tangent planes on the device: [batch, c_in, Ng] for a run of one
-    direction, [batch, K, c_in, Ng] for a run of K (`run.directions`))."""
+    direction, [batch, K, c_in, Ng] for a run of K (`run.directions`)).  keep_predictions (a run of one
+    direction; loss_and_param_gnvp): this step's prediction tangents [batch, n_out, Ng] in their place."""
     targets = xs.from_xarray(targets)
     state = {}
 
@@ -976,13 +992,17 @@ class GraphCast(Predictor):
       if "planes" not in state:
         eng.input_grads_begin()
         lead = [run.dirs] if run.directions else []
-        state["planes"] = torch.empty([run.batch] + lead + [eng.c_in, eng.num_grid],
+        rows = eng.n_out if keep_predictions else eng.c_in
+        state["planes"] = torch.empty([run.batch] + lead + [rows, eng.num_grid],
                                       dtype=torch.float32, device=eng.device)
         state["lat_weight"] = self._lat_weight(targets, eng.device)
       tangent_out = torch.empty([run.dirs, eng.n_out, eng.num_grid], dtype=torch.float32,
                                 device=eng.device)
-      run.element(eng, b, tangent_out, None, norm, affine,
-                  keep=lambda p: state["planes"][b].copy_(p if run.directions else p[0]))
+      keep = None if keep_predictions else (
+          lambda p: state["planes"][b].copy_(p if run.directions else p[0]))
+      run.element(eng, b, tangent_out, None, norm, affine, keep=keep)
+      if keep_predictions:
+        state["planes"][b].copy_(tangent_out[0])
       eng.output_loss(planes_tgt, state["lat_weight"], channel_sums=channel_sums,
                       planes_out=planes_out, **affine)
 

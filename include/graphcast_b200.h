@@ -354,6 +354,26 @@ int gcb_output_loss_grad_feedback(const float* y, int32_t ld_y, int32_t n_out, i
                                   const int32_t* resid_channel, const int32_t* carry_row,
                                   float* a_out, float* g, int32_t ld_g, void* stream);
 
+/* Seed of a Gauss-Newton product over several target times (autoregressive.Predictor
+ * .loss_and_param_gnvp): the loss is a quadratic in the normalised residual r = (pred - target) / scale
+ * with the diagonal Hessian coef[c] * lat_weight, so from pdot [n_out, n_nodes] (channel-major fp32), the
+ * tangent J v of the physical predictions, the cotangent of r is coef * lat_weight * d with
+ *   d[c, node]     = pdot[c, node] / scale[c]                  (fp32, true division; scale NULL = 1)
+ * and the seed carries it with the feedback of gcb_output_loss_grad_feedback (same row arguments):
+ *   g[node, c]     = coef[c] * lat_weight * d + scale[c] * a_next[dpred_row[c], node]   (fp64, rounded once)
+ *   a_out[r, node] = c >= 0 ? (float)(coef[c] * lat_weight * d / scale[c] + a_next[dpred_row[c], node]) : 0,
+ *                    c = resid_channel[r]
+ *                  + a_next[carry_row[r], node]                when carry_row[r] >= 0
+ * One launch.  With scale NULL, g and a_out are bit for bit gcb_output_loss_grad_feedback with y = pdot^T,
+ * all-zero targets and NULL offset and add planes, without the target planes that call would read; with
+ * no a_next and n_rows = 0 too, g is bit for bit gcb_output_loss_gn_seed on dy = pdot^T.  Columns >= n_out
+ * of g are not written.  Deterministic, no atomics. */
+int gcb_output_loss_gn_seed_feedback(const float* pdot, int32_t n_out, int32_t n_lat, int32_t n_lon,
+                                     const float* scale, const float* lat_weight, const double* coef,
+                                     const float* a_next, const int32_t* dpred_row, int32_t n_rows,
+                                     const int32_t* resid_channel, const int32_t* carry_row,
+                                     float* a_out, float* g, int32_t ld_g, void* stream);
+
 /* Input gradient: the transpose of gcb_pack_grid_image's normalisation (normalization.py:113-146,
  * (x - mean) / scale) for a list of rows,
  *   a[r, node] = (accumulate ? a[r, node] : 0) + dx[node, channel[r]] / scale[channel[r]]
@@ -812,7 +832,8 @@ typedef enum {
                              * gcb_layernorm_jvp, gcb_swish_jvp, gcb_layernorm_jvp_dirs,
                              * gcb_layernorm_backward_dirs, gcb_swish_backward_jvp(_dirs),
                              * gcb_layernorm_backward_jvp(_dirs), gcb_layernorm_jvp_params,
-                             * gcb_output_loss_gn_seed, gcb_layernorm_backward_jvp_params */
+                             * gcb_output_loss_gn_seed, gcb_layernorm_backward_jvp_params,
+                             * gcb_output_loss_gn_seed_feedback */
   GCB_KIND_NOISE = 11       /* gcb_add_gaussian_noise */
 } gcb_kernel_kind;
 int gcb_profile_begin(void);
