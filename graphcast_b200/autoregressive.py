@@ -52,8 +52,6 @@ import torch
 from graphcast_b200 import _native
 from graphcast_b200 import feedback
 from graphcast_b200 import graphcast
-from graphcast_b200 import losses
-from graphcast_b200 import model_utils
 from graphcast_b200 import normalization
 from graphcast_b200 import rollout
 from graphcast_b200 import xarray_shim as xs
@@ -212,10 +210,7 @@ class Predictor(graphcast.Predictor):
     if isinstance(p, graphcast.GraphCast):
       return p, lambda i, t, f: None
     if isinstance(p, normalization.InputsAndResiduals) and p._fuses():
-      def norm_of(i, t, f):
-        device = p._predictor._device or f"cuda:{torch.cuda.current_device()}"
-        return p._fused_constants(i, t, f, torch.device(device))
-      return p._predictor, norm_of
+      return p._predictor, p._norm_of()
     return None
 
   def loss_and_grads(self, inputs, targets, forcings, rng=None, *, _noise_fold: int = 0, **kwargs):
@@ -299,11 +294,10 @@ class Predictor(graphcast.Predictor):
     sums = torch.stack([s for _, s in records]).cpu().numpy()      # the one read-back
     records = [finish(sums[t]) for t, (finish, _) in enumerate(records)]
     loss, diagnostics = _mean_over_time([l for l, _ in records], [d for _, d in records])
-    slabs = model_utils.channel_layout(first["targets"])
-    kappa = losses.channel_kappa(slabs, model.engine.num_grid, graphcast.LOSS_PER_VARIABLE_WEIGHTS)
+    _, coef = graphcast.loss_coefficients(first["targets"], model.engine.num_grid, stash.batch,
+                                          len(records))
     lat_weight = model._lat_weight(first["targets"], model.engine.device)
-    return (loss, diagnostics, stash, first, lat_weight,
-            2.0 * kappa / (stash.batch * len(records)))
+    return loss, diagnostics, stash, first, lat_weight, coef
 
   def loss_and_input_grads(self, inputs, targets, forcings, rng=None, *, _noise_fold: int = 0,
                            **kwargs):

@@ -22,7 +22,7 @@ runs in libgraphcast_b200.so.  HBM layout (fp32 unless noted):
 from __future__ import annotations
 
 import ctypes as C
-from typing import Mapping, Optional
+from typing import List, Mapping, Optional
 
 import numpy as np
 import torch
@@ -776,15 +776,64 @@ class Engine:
     snaps = self._forward_snapshots(grid_in)
     self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
     g_out = torch.zeros([self.num_grid, 256], dtype=torch.float32, device=self.device)
-    n_lat = lat_weight.shape[0]
     with self._on_device():
-      _native.check(self._lib.gcb_output_loss_grad(
-          self.grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat,
-          self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
-          self._ptr(affine.get("add_planes")), self._ptr(affine.get("add_plane_index")),
-          targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), g_out.data_ptr(), 256,
-          self._stream()), "gcb_output_loss_grad")
+      self._loss_seed(self.grid_out, targets_planes, lat_weight, coef, g_out, affine)
       self._backward.element(grid_in, g_out, snaps)
+
+  def _loss_seed(self, y: torch.Tensor, targets_planes: torch.Tensor, lat_weight: torch.Tensor,
+                 coef: torch.Tensor, g: torch.Tensor, affine: dict, fb: Optional["Feedback"] = None,
+                 a_next: Optional[torch.Tensor] = None, a_out: Optional[torch.Tensor] = None,
+                 n_rows: int = 0) -> None:
+    """The loss derivative seed of the decoder output y [Ng, ld] into the rows of g (row stride 256),
+    with `affine` the output normalisation (scale, offset, add_planes, add_plane_index; absent: none):
+    gcb_output_loss_grad, or with fb, gcb_output_loss_grad_feedback, which also carries a_next (the
+    following step's gradient on fb's rows, or None) into the seed and writes the residual and
+    frame-shift terms of n_rows rows to a_out."""
+    n_lat = lat_weight.shape[0]
+    head = (y.data_ptr(), y.shape[1], self.n_out, n_lat, self.num_grid // n_lat,
+            self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
+            self._ptr(affine.get("add_planes")), self._ptr(affine.get("add_plane_index")),
+            targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr())
+    if fb is None:
+      _native.check(self._lib.gcb_output_loss_grad(*head, g.data_ptr(), 256, self._stream()),
+                    "gcb_output_loss_grad")
+      return
+    _native.check(self._lib.gcb_output_loss_grad_feedback(
+        *head, self._ptr(a_next), fb.dpred_row.data_ptr(), n_rows, fb.resid_channel.data_ptr(),
+        fb.carry_row.data_ptr(), self._ptr(a_out), g.data_ptr(), 256, self._stream()),
+        "gcb_output_loss_grad_feedback")
+
+  def _gn_seed(self, dy: torch.Tensor, lat_weight: torch.Tensor, coef: torch.Tensor,
+               g: torch.Tensor) -> None:
+    """The Gauss-Newton seed coef * lat_weight * dy of the decoder tangent dy [Ng, ld] into the rows
+    of g (row stride 256): gcb_output_loss_gn_seed."""
+    n_lat = lat_weight.shape[0]
+    _native.check(self._lib.gcb_output_loss_gn_seed(
+        dy.data_ptr(), dy.shape[1], self.n_out, n_lat, self.num_grid // n_lat, lat_weight.data_ptr(),
+        coef.data_ptr(), g.data_ptr(), 256, self._stream()), "gcb_output_loss_gn_seed")
+
+  def _pack_tangents(self, planes: List[torch.Tensor], in_scale: Optional[torch.Tensor],
+                     stride: int) -> torch.Tensor:
+    """The stacked operand image of K tangent planes [c_in, Ng] (direction k from row k * stride),
+    each packed as pack_inputs packs the planes, without the mean (in_scale: the input normalisation's
+    scale) and with zero structural features."""
+    dgrid_in = self._image((len(planes) - 1) * stride + self.num_grid, self.c_in_pad)
+    img_stride = self._lib.gcb_a_image_bytes(stride, self.c_in_pad)
+    no_static = torch.zeros([self.num_grid, 3], dtype=torch.float32, device=self.device)
+    for k, p in enumerate(planes):
+      _native.check(self._lib.gcb_pack_grid_image(
+          p.data_ptr(), self.c_in, self.num_grid, None, self._ptr(in_scale), no_static.data_ptr(), 3,
+          self.c_in_pad, dgrid_in.data_ptr() + k * img_stride, self._stream()), "gcb_pack_grid_image")
+    return dgrid_in
+
+  def _input_grad_tail(self, dx: torch.Tensor, fb: "Feedback", a_outs, stride: int) -> None:
+    """gcb_input_grad of every direction k of the backward pass's input-image gradient dx (from row
+    k * stride) into a_outs[k] [fb.n_rows, Ng]: the derivative through the grid embedder, added to the
+    seed's terms there."""
+    for k, a in enumerate(a_outs):
+      _native.check(self._lib.gcb_input_grad(
+          dx[k * stride:].data_ptr(), dx.shape[1], self.num_grid, fb.n_rows, fb.rows.data_ptr(),
+          self._ptr(fb.in_scale), a.data_ptr(), 1, self._stream()), "gcb_input_grad")
 
   def _forward_snapshots(self, grid_in: torch.Tensor) -> dict:
     """The step stage by stage, with copies of what the backward pass reads."""
@@ -805,17 +854,10 @@ class Engine:
 
   def _bptt_element(self, targets_planes, lat_weight, coef, channel_sums, grid_in, fb: "Feedback",
                     input_grad: bool, affine) -> None:
-    n_lat = lat_weight.shape[0]
-
     def seed(g_out, a_out, n_rows):
       self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
-      _native.check(self._lib.gcb_output_loss_grad_feedback(
-          self.grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat,
-          self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
-          self._ptr(affine.get("add_planes")), self._ptr(affine.get("add_plane_index")),
-          targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), self._ptr(fb.a),
-          fb.dpred_row.data_ptr(), n_rows, fb.resid_channel.data_ptr(), fb.carry_row.data_ptr(),
-          self._ptr(a_out), g_out.data_ptr(), 256, self._stream()), "gcb_output_loss_grad_feedback")
+      self._loss_seed(self.grid_out, targets_planes, lat_weight, coef, g_out, affine, fb=fb,
+                      a_next=fb.a, a_out=a_out, n_rows=n_rows)
     self._bptt_walk(grid_in, fb, input_grad, seed)
 
   def param_gnvp_bptt_element(self, pred_tangent: torch.Tensor, lat_weight: torch.Tensor,
@@ -863,9 +905,7 @@ class Engine:
       fb.a = a_out                         # the following step's rows are consumed: release them
       dx = self._backward.element(grid_in, g_out, snaps, dgrid_in=bool(n_rows))
       if n_rows:
-        _native.check(self._lib.gcb_input_grad(
-            dx.data_ptr(), dx.shape[1], self.num_grid, n_rows, fb.rows.data_ptr(),
-            self._ptr(fb.in_scale), a_out.data_ptr(), 1, self._stream()), "gcb_input_grad")
+        self._input_grad_tail(dx, fb, [a_out], 0)
 
   # -- input gradients (loss_and_input_grads, input_vjp) ---------------------------------------------
   def input_grads_begin(self, what: str = "input gradients") -> None:
@@ -924,14 +964,8 @@ class Engine:
       if channel_sums is not None:
         self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
       if cotangent is None:
-        n_lat = lat_weight.shape[0]
-        _native.check(self._lib.gcb_output_loss_grad_feedback(
-            self.grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat,
-            self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
-            self._ptr(affine.get("add_planes")), self._ptr(affine.get("add_plane_index")),
-            targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), self._ptr(fb.a),
-            fb.dpred_row.data_ptr(), fb.n_rows, fb.resid_channel.data_ptr(), fb.carry_row.data_ptr(),
-            a_out.data_ptr(), g_out.data_ptr(), 256, self._stream()), "gcb_output_loss_grad_feedback")
+        self._loss_seed(self.grid_out, targets_planes, lat_weight, coef, g_out, affine, fb=fb,
+                        a_next=fb.a, a_out=a_out, n_rows=fb.n_rows)
       else:
         if single and (tuple(cotangent.shape) != (self.n_out, self.num_grid)
                        or not cotangent.is_contiguous()):
@@ -949,10 +983,7 @@ class Engine:
       fb.a = a_out
       affine = targets_planes = cotangent = None
       dx = self._backward.element(grid_in, g_out, snaps, dgrid_in=True, param_grads=False, dirs=dirs)
-      for k in range(dirs):
-        _native.check(self._lib.gcb_input_grad(
-            dx[k * stride:].data_ptr(), dx.shape[1], self.num_grid, fb.n_rows, fb.rows.data_ptr(),
-            self._ptr(fb.in_scale), a_outs[k].data_ptr(), 1, self._stream()), "gcb_input_grad")
+      self._input_grad_tail(dx, fb, a_outs, stride)
 
   # -- Hessian-vector products (loss_and_input_hvp) ---------------------------------------------------
   def input_hvp_element(self, fb: "Feedback", operands: dict, *, lat_weight: torch.Tensor,
@@ -993,18 +1024,9 @@ class Engine:
     planes = [tangent] if single else list(tangent.unbind(0))
     grid_in = self.grid_in_img if grid_in is None else grid_in
     stride = self._backward.dir_stride(self.num_grid)
-    no_static = torch.zeros([self.num_grid, 3], dtype=torch.float32, device=self.device)
-    dgrid_in = self._image((nt - 1) * stride + self.num_grid, self.c_in_pad)
-    img_stride = self._lib.gcb_a_image_bytes(stride, self.c_in_pad)
-    n_lat = lat_weight.shape[0]
     add_index = affine.get("add_plane_index")
     with self._on_device():
-      for k, p in enumerate(planes):
-        _native.check(self._lib.gcb_pack_grid_image(
-            p.data_ptr(), self.c_in, self.num_grid, None, self._ptr(fb.in_scale),
-            no_static.data_ptr(), 3, self.c_in_pad, dgrid_in.data_ptr() + k * img_stride,
-            self._stream()), "gcb_pack_grid_image")
-      del no_static
+      dgrid_in = self._pack_tangents(planes, fb.in_scale, stride)
       snaps, tsnaps = {}, {}
       dy = self._backward.tangent(grid_in, dgrid_in, nt, snaps=snaps, tsnaps=tsnaps)
       del dgrid_in
@@ -1018,28 +1040,21 @@ class Engine:
       if zero_targets is None:
         zero_targets = torch.zeros([self.n_out, self.num_grid], dtype=torch.float32,
                                    device=self.device)
-      seeds = [(self.grid_out, affine.get("offset"), affine.get("add_planes"), targets_planes)]
-      seeds += [(dy[k * stride:], None, None if add_index is None else p, zero_targets)
+      seeds = [(self.grid_out, affine, targets_planes)]
+      seeds += [(dy[k * stride:], dict(scale=affine.get("scale"), add_plane_index=add_index,
+                                       add_planes=None if add_index is None else p), zero_targets)
                 for k, p in enumerate(planes)]
-      for k, (y, offset, add, targets) in enumerate(seeds):
-        _native.check(self._lib.gcb_output_loss_grad_feedback(
-            y.data_ptr(), y.shape[1], self.n_out, n_lat, self.num_grid // n_lat,
-            self._ptr(affine.get("scale")), self._ptr(offset), self._ptr(add), self._ptr(add_index),
-            targets.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), self._ptr(a_next[k]),
-            fb.dpred_row.data_ptr(), fb.n_rows, fb.resid_channel.data_ptr(), fb.carry_row.data_ptr(),
-            a_out[k].data_ptr(), g_out[k * stride:].data_ptr(), 256, self._stream()),
-            "gcb_output_loss_grad_feedback")
+      for k, (y, seed_affine, targets) in enumerate(seeds):
+        self._loss_seed(y, targets, lat_weight, coef, g_out[k * stride:], seed_affine, fb=fb,
+                        a_next=a_next[k], a_out=a_out[k], n_rows=fb.n_rows)
       # the following step's rows, the planes, targets and tangents are consumed: release them
       fb.a = a_out
-      del seeds, y, offset, add, targets, a_next, zero_targets, dy, planes, p
+      del seeds, y, seed_affine, targets, a_next, zero_targets, dy, planes
       affine = targets_planes = tangent = None
       dx = self._backward.element(grid_in, g_out, snaps, dgrid_in=True, param_grads=False,
                                   dirs=1 + nt, hvp=tsnaps)
       del g_out, snaps, tsnaps
-      for k in range(1 + nt):
-        _native.check(self._lib.gcb_input_grad(
-            dx[k * stride:].data_ptr(), dx.shape[1], self.num_grid, fb.n_rows, fb.rows.data_ptr(),
-            self._ptr(fb.in_scale), a_out[k].data_ptr(), 1, self._stream()), "gcb_input_grad")
+      self._input_grad_tail(dx, fb, a_out.unbind(0), stride)
 
   # -- tangent-linear model (input_jvp, batched_input_jvp) --------------------------------------------
   def input_jvp_element(self, tangent_planes: torch.Tensor, tangent_out: torch.Tensor, *,
@@ -1079,16 +1094,9 @@ class Engine:
     outs = [tangent_out] if single else list(tangent_out.unbind(0))
     grid_in = self.grid_in_img if grid_in is None else grid_in
     stride = self._backward.dir_stride(self.num_grid)
-    dgrid_in = self._image((dirs - 1) * stride + self.num_grid, self.c_in_pad)
-    img_stride = self._lib.gcb_a_image_bytes(stride, self.c_in_pad)
-    no_static = torch.zeros([self.num_grid, 3], dtype=torch.float32, device=self.device)
     add_index = affine.get("add_plane_index")
     with self._on_device():
-      for k, p in enumerate(planes):
-        _native.check(self._lib.gcb_pack_grid_image(
-            p.data_ptr(), self.c_in, self.num_grid, None, self._ptr(in_scale), no_static.data_ptr(), 3,
-            self.c_in_pad, dgrid_in.data_ptr() + k * img_stride, self._stream()),
-            "gcb_pack_grid_image")
+      dgrid_in = self._pack_tangents(planes, in_scale, stride)
       dy = self._backward.tangent(grid_in, dgrid_in, dirs, wts=weight_tangents)
       del dgrid_in
       if planes_out is not None:
@@ -1131,15 +1139,12 @@ class Engine:
     if self._backward is None:
       raise RuntimeError("call grads_begin() first")
     grid_in = self.grid_in_img
-    n_lat = lat_weight.shape[0]
     with self._on_device():
       dgrid_in = self._image(self.num_grid, self.c_in_pad)
       dy = self._backward.tangent(grid_in, dgrid_in, wts=weight_tangents)
       del dgrid_in
       g_out = torch.zeros([self.num_grid, 256], dtype=torch.float32, device=self.device)
-      _native.check(self._lib.gcb_output_loss_gn_seed(
-          dy.data_ptr(), dy.shape[1], self.n_out, n_lat, self.num_grid // n_lat, lat_weight.data_ptr(),
-          coef.data_ptr(), g_out.data_ptr(), 256, self._stream()), "gcb_output_loss_gn_seed")
+      self._gn_seed(dy, lat_weight, coef, g_out)
       del dy
     # The tangent pass leaves its blocks cached in shapes the backward pass cannot reuse: at 0.25
     # degree the backward pass peaks within a few GiB of an 80 GB card and would not find its 1 GiB
@@ -1176,7 +1181,6 @@ class Engine:
       raise RuntimeError("call param_hvp_begin() first")
     bw = self._backward
     grid_in = self.grid_in_img
-    n_lat = lat_weight.shape[0]
     stride = bw.dir_stride(self.num_grid)
     with self._on_device():
       dgrid_in = self._image(self.num_grid, self.c_in_pad)
@@ -1185,15 +1189,8 @@ class Engine:
       del dgrid_in
       self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
       g_out = torch.zeros([stride + self.num_grid, 256], dtype=torch.float32, device=self.device)
-      _native.check(self._lib.gcb_output_loss_grad(
-          self.grid_out.data_ptr(), 256, self.n_out, n_lat, self.num_grid // n_lat,
-          self._ptr(affine.get("scale")), self._ptr(affine.get("offset")),
-          self._ptr(affine.get("add_planes")), self._ptr(affine.get("add_plane_index")),
-          targets_planes.data_ptr(), lat_weight.data_ptr(), coef.data_ptr(), g_out.data_ptr(), 256,
-          self._stream()), "gcb_output_loss_grad")
-      _native.check(self._lib.gcb_output_loss_gn_seed(
-          dy.data_ptr(), dy.shape[1], self.n_out, n_lat, self.num_grid // n_lat, lat_weight.data_ptr(),
-          coef.data_ptr(), g_out[stride:].data_ptr(), 256, self._stream()), "gcb_output_loss_gn_seed")
+      self._loss_seed(self.grid_out, targets_planes, lat_weight, coef, g_out, affine)
+      self._gn_seed(dy, lat_weight, coef, g_out[stride:])
       del dy
       bw.element(grid_in, g_out, snaps, dirs=2, hvp=tsnaps, wts=weight_tangents)
 

@@ -26,6 +26,7 @@ from __future__ import annotations
 
 import abc
 import dataclasses
+import functools
 from typing import Any, Dict, List, Mapping, Optional, Tuple
 
 import numpy as np
@@ -347,19 +348,43 @@ class GraphCast(Predictor):
     return self._loss_and_grads(inputs, targets, forcings, norm=None)
 
   def _loss_and_grads(self, inputs, targets, forcings, norm: Optional[FusedNormalization]):
+    def begin(eng, tangents):
+      eng.grads_begin()
+      return eng.loss_and_grads_element
+    loss, diagnostics = self._param_call(
+        inputs, targets, forcings, norm, "parameter gradients cover one target time (no backprop "
+        "through time)", None, begin)
+    return loss, diagnostics, self._export_grads()
+
+  def _param_call(self, inputs, targets, forcings, norm: Optional[FusedNormalization], refusal: str,
+                  param_tangents, begin):
+    """The calls of one target time that accumulate in the engine's gradient accumulators
+    (loss_and_grads, loss_and_param_gnvp, loss_and_param_hvp), up to what they export.  Several target
+    times raise NotImplementedError(refusal), and param_tangents (None: the call takes none) are
+    checked, before anything runs.  Then `_call` runs begin(engine, checked tangents) once, which
+    prepares the engine and returns its per-element call f(targets_planes, lat_weight, coef,
+    channel_sums=..., **affine), and f for every batch element.  Returns (loss, diagnostics)."""
     inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
     if targets.sizes.get("time", 1) != 1:
-      raise NotImplementedError("parameter gradients cover one target time (no backprop through time)")
-    sizes = dict(inputs.sizes)
-    batch = sizes.get("batch", 1)
-    num_grid = sizes["lat"] * sizes["lon"]
-    slabs = model_utils.channel_layout(targets)
-    coef = 2.0 * losses.channel_kappa(slabs, num_grid, LOSS_PER_VARIABLE_WEIGHTS) / batch
-    self._call(inputs, targets, forcings, norm=norm, targets=targets, predictions=False,
-               grad_coef=coef)
-    loss, diagnostics = losses.losses_from_channel_sums(
-        self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
-    return loss, diagnostics, self._export_grads()
+      raise NotImplementedError(refusal)
+    tangents = None if param_tangents is None else self._checked_param_tangents(param_tangents)
+    slabs, coef = loss_coefficients(targets, inputs.sizes["lat"] * inputs.sizes["lon"],
+                                    dict(inputs.sizes).get("batch", 1))
+    run = lat_weight = coef_dev = None
+
+    def start():
+      nonlocal run, lat_weight, coef_dev
+      eng = self._engine
+      run = begin(eng, tangents)
+      lat_weight, coef_dev = self._lat_weight(targets, eng.device), _device_coef(coef, eng.device)
+
+    def element(b, planes_tgt, planes_out, channel_sums, affine):
+      run(planes_tgt, lat_weight, coef_dev, channel_sums=channel_sums, **affine)
+
+    self._call(inputs, targets, forcings, norm=norm, targets=targets, predictions=False, begin=start,
+               element=element)
+    run = coef_dev = None                  # with the weight tangents the element call holds
+    return self._losses(slabs)
 
   def loss_and_input_grads(self, inputs, targets, forcings, **unused_kwargs):
     """(loss, diagnostics, input_grads, forcing_grads) for one target time.
@@ -562,38 +587,16 @@ class GraphCast(Predictor):
 
   def _loss_and_param_hvp(self, inputs, targets, forcings, param_tangents,
                           norm: Optional[FusedNormalization]):
-    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
-    if targets.sizes.get("time", 1) != 1:
-      raise NotImplementedError("parameter Hessian-vector products cover one target time (several "
-                                "are not provided)")
-    tangents = self._checked_param_tangents(param_tangents)
-    batch = dict(inputs.sizes).get("batch", 1)
-    num_grid = inputs.sizes["lat"] * inputs.sizes["lon"]
-    slabs = model_utils.channel_layout(targets)
-    coef = 2.0 * losses.channel_kappa(slabs, num_grid, LOSS_PER_VARIABLE_WEIGHTS) / batch
-    state = {}
-
-    def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
-      eng = self._engine
-      if "wt" not in state:
-        eng.param_hvp_begin()
-        self._release_idle_staging()
-        state["wt"] = eng.weight_tangents(tangents, transposed=True)
-        state["lat_weight"] = self._lat_weight(targets, eng.device)
-        state["coef"] = torch.as_tensor(np.asarray(coef, np.float64)).to(eng.device)
-      eng.param_hvp_element(planes_tgt, state["lat_weight"], state["coef"], state["wt"],
-                            channel_sums=channel_sums, **affine)
-
-    self._call(inputs, targets, forcings, norm=norm, targets=targets, predictions=False,
-               element=element)
-    state.clear()
-    loss, diagnostics = losses.losses_from_channel_sums(
-        self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
-    grads = {name: {f: t.cpu().numpy() for f, t in fields.items()}
-             for name, fields in self._engine.grads().items()}
-    hvp = {name: {f: t.cpu().numpy() for f, t in fields.items()}
-           for name, fields in self._engine.param_hvp().items()}
-    return loss, diagnostics, grads, hvp
+    def begin(eng, tangents):
+      eng.param_hvp_begin()
+      self._release_idle_staging()
+      return functools.partial(eng.param_hvp_element,
+                               weight_tangents=eng.weight_tangents(tangents, transposed=True))
+    loss, diagnostics = self._param_call(
+        inputs, targets, forcings, norm, "parameter Hessian-vector products cover one target time "
+        "(several are not provided)", param_tangents, begin)
+    return (loss, diagnostics, _host_grads(self._engine.grads()),
+            _host_grads(self._engine.param_hvp()))
 
   def _param_tangent_run(self, inputs, targets_template, forcings, param_tangents, num_steps: int,
                          plan=None) -> "_TangentRun":
@@ -619,36 +622,14 @@ class GraphCast(Predictor):
 
   def _loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents,
                            norm: Optional[FusedNormalization]):
-    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
-    if targets.sizes.get("time", 1) != 1:
-      raise NotImplementedError("Gauss-Newton products cover one target time (several are not "
-                                "provided)")
-    tangents = self._checked_param_tangents(param_tangents)
-    batch = dict(inputs.sizes).get("batch", 1)
-    num_grid = inputs.sizes["lat"] * inputs.sizes["lon"]
-    slabs = model_utils.channel_layout(targets)
-    coef = 2.0 * losses.channel_kappa(slabs, num_grid, LOSS_PER_VARIABLE_WEIGHTS) / batch
-    state = {}
-
-    def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
-      eng = self._engine
-      if "wt" not in state:
-        eng.grads_begin()
-        self._release_idle_staging()
-        state["wt"] = eng.weight_tangents(tangents)
-        state["lat_weight"] = self._lat_weight(targets, eng.device)
-        state["coef"] = torch.as_tensor(np.asarray(coef, np.float64)).to(eng.device)
-      eng.param_gnvp_element(planes_tgt, state["lat_weight"], state["coef"], state["wt"],
-                             channel_sums=channel_sums, **affine)
-
-    self._call(inputs, targets, forcings, norm=norm, targets=targets, predictions=False,
-               element=element)
-    state.clear()
-    loss, diagnostics = losses.losses_from_channel_sums(
-        self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
-    gnvp = {name: {f: t.cpu().numpy() for f, t in fields.items()}
-            for name, fields in self._engine.grads().items()}
-    return loss, diagnostics, gnvp
+    def begin(eng, tangents):
+      eng.grads_begin()
+      self._release_idle_staging()
+      return functools.partial(eng.param_gnvp_element, weight_tangents=eng.weight_tangents(tangents))
+    loss, diagnostics = self._param_call(
+        inputs, targets, forcings, norm, "Gauss-Newton products cover one target time (several are "
+        "not provided)", param_tangents, begin)
+    return loss, diagnostics, _host_grads(self._engine.grads())
 
   @staticmethod
   def _one_step_tangents(inputs, targets_template, forcings, input_tangents,
@@ -668,24 +649,25 @@ class GraphCast(Predictor):
     forward and its tangent (Engine.input_jvp_element) in place of its step."""
     inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
     targets_template = xs.from_xarray(targets_template)
-    state = {}
+    out = None
 
-    def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
+    def begin():
+      nonlocal out
       eng = self._engine
-      if "out" not in state:
-        eng.input_grads_begin("input gradients" if run.param_tangents is None
-                              else "parameter tangents")
-        self._release_idle_staging()
-        state["out"] = torch.empty([run.dirs, run.batch, eng.n_out, eng.num_grid],
-                                   dtype=torch.float32, device=eng.device)
-      run.element(eng, b, state["out"][:, b], planes_out, norm, affine)
+      eng.input_grads_begin("input gradients" if run.param_tangents is None else "parameter tangents")
+      self._release_idle_staging()
+      out = torch.empty([run.dirs, run.batch, eng.n_out, eng.num_grid], dtype=torch.float32,
+                        device=eng.device)
 
-    predictions = self._call(inputs, targets_template, forcings, norm=norm, element=element)
+    def element(b, planes_tgt, planes_out, channel_sums, affine):
+      run.element(self._engine, b, out[:, b], planes_out, norm, affine)
+
+    predictions = self._call(inputs, targets_template, forcings, norm=norm, begin=begin,
+                             element=element)
     run.step += 1
     if not run.directions:
-      return predictions, self._planes_to_dataset(state["out"][0], targets_template, run.n_lat,
-                                                  run.n_lon)
-    return predictions, self._planes_to_dataset(state["out"], targets_template, run.n_lat, run.n_lon,
+      return predictions, self._planes_to_dataset(out[0], targets_template, run.n_lat, run.n_lon)
+    return predictions, self._planes_to_dataset(out, targets_template, run.n_lat, run.n_lon,
                                                 directions=run.labels)
 
   def _loss_and_input_grads(self, inputs, targets, forcings, norm: Optional[FusedNormalization],
@@ -702,15 +684,11 @@ class GraphCast(Predictor):
     if tangents is not None:
       pack = hvp_direction_tangent_planes if directions else hvp_tangent_planes
       tangent = pack(inputs, forcings, *tangents)
-    batch = dict(inputs.sizes).get("batch", 1)
-    slabs = model_utils.channel_layout(targets)
-    num_grid = inputs.sizes["lat"] * inputs.sizes["lon"]
-    coef = 2.0 * losses.channel_kappa(slabs, num_grid, LOSS_PER_VARIABLE_WEIGHTS) / batch
+    slabs, coef = loss_coefficients(targets, inputs.sizes["lat"] * inputs.sizes["lon"],
+                                    dict(inputs.sizes).get("batch", 1))
     run = self._one_step_input_grads(inputs, targets, forcings, norm, targets=targets, coef=coef,
                                      tangent_planes=tangent)
-    loss, diagnostics = losses.losses_from_channel_sums(
-        self._channel_sums.cpu().numpy(), slabs, self._engine.num_grid, LOSS_PER_VARIABLE_WEIGHTS)
-    return (loss, diagnostics) + run.finish()
+    return self._losses(slabs) + run.finish()
 
   def _input_vjp(self, inputs, targets_template, forcings, cotangents,
                  norm: Optional[FusedNormalization], directions: bool = False,
@@ -742,23 +720,26 @@ class GraphCast(Predictor):
     c_in, Ng] for K directions, with `targets`) every element runs Engine.input_hvp_element.  Returns
     the run, whose finish() gives (input_grads, forcing_grads), with tangent_planes followed by
     (input_hvp, forcing_hvp), these with a leading "direction" dim for K directions."""
-    state = {}
+    batch = dict(inputs.sizes).get("batch", 1)
+    run = cot = lat_weight = coef_dev = None
 
-    def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
+    def begin():
+      nonlocal run, cot, lat_weight, coef_dev
       eng = self._engine
-      if "run" not in state:
-        plan = feedback.FeedbackPlan.all_channels(inputs, template, forcings)
-        dirs = None
-        if directions:
-          state["cot"] = self._direction_cotangent_planes(cotangents, template, state["batch"])
-          dirs = state["cot"].shape[0]
-        state["run"] = _InputGradRun(self, plan, norm, inputs, forcings, 1, state["batch"],
-                                     release_staging=False, dirs=dirs,
-                                     hvp=_hvp_directions(tangent_planes, 0))
-        if cotangents is not None and not directions:
-          state["cot"] = self._cotangent_planes(cotangents, template, state["run"].batch)
-        if coef is not None:
-          state["coef"] = torch.as_tensor(np.asarray(coef, np.float64)).to(eng.device)
+      plan = feedback.FeedbackPlan.all_channels(inputs, template, forcings)
+      dirs = None
+      if directions:
+        cot = self._direction_cotangent_planes(cotangents, template, batch)
+        dirs = cot.shape[0]
+      run = _InputGradRun(self, plan, norm, inputs, forcings, 1, batch, release_staging=False,
+                          dirs=dirs, hvp=_hvp_directions(tangent_planes, 0))
+      if cotangents is not None and not directions:
+        cot = self._cotangent_planes(cotangents, template, batch)
+      if targets is not None:
+        lat_weight, coef_dev = self._lat_weight(targets, eng.device), _device_coef(coef, eng.device)
+
+    def element(b, planes_tgt, planes_out, channel_sums, affine):
+      eng = self._engine
       operands = dict(affine)
       if tangent_planes is not None and tangent_planes.dim() == 4:    # [K, batch, c_in, Ng]
         operands["tangent_planes"] = torch.empty(
@@ -768,22 +749,20 @@ class GraphCast(Predictor):
         operands["tangent_planes"] = tangent_planes[b].to(eng.device)
       if targets is not None:
         operands["targets_planes"] = planes_tgt
-        kw = dict(lat_weight=self._lat_weight(targets, eng.device), coef=state["coef"],
-                  channel_sums=channel_sums)
+        kw = dict(lat_weight=lat_weight, coef=coef_dev, channel_sums=channel_sums)
       else:
-        cot = state["cot"][:, b] if directions else state["cot"][b]
-        seed = torch.empty(list(cot.shape), dtype=torch.float32, device=eng.device)
-        seed.copy_(cot)
+        host = cot[:, b] if directions else cot[b]
+        seed = torch.empty(list(host.shape), dtype=torch.float32, device=eng.device)
+        seed.copy_(host)
         operands["cotangent"] = seed
         kw = {}
-      state["run"].element(b, 0, operands, planes_out=planes_out, **kw)
+      run.element(b, 0, operands, planes_out=planes_out, **kw)
 
-    state["batch"] = dict(inputs.sizes).get("batch", 1)
     out = self._call(inputs, template, forcings, norm=norm, targets=targets,
-                     predictions=predictions is not None, element=element)
+                     predictions=predictions is not None, begin=begin, element=element)
     if predictions is not None:
       predictions["predictions"] = out
-    return state["run"]
+    return run
 
   def _cotangent_planes(self, cotangents, template: xs.Dataset, batch: int,
                         out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -839,7 +818,7 @@ class GraphCast(Predictor):
                         hvp=None if tangents is None else _hvp_directions(tangents.steps[0][0][0], 1))
     eng = self._engine
     dev = eng.device
-    coef_dev = None if coef is None else torch.as_tensor(np.asarray(coef, np.float64)).to(dev)
+    coef_dev = None if coef is None else _device_coef(coef, dev)
     compute = torch.cuda.current_stream(dev)
     for b in range(run.batch):
       for t in range(run.num_steps - 1, -1, -1):
@@ -849,12 +828,7 @@ class GraphCast(Predictor):
         # so the backward pass reuses their 2.9 GB (0.25 degree).
         operands = {"planes": torch.empty([eng.c_in, eng.num_grid], dtype=torch.float32, device=dev)}
         operands["planes"].copy_(saved[0][b], non_blocking=True)
-        if norm is None:
-          eng.pack_inputs(operands.pop("planes"))
-        else:
-          eng.pack_inputs(operands["planes"], mean=norm.in_mean, scale=norm.in_scale)
-          operands.update(scale=norm.out_scale, offset=norm.out_offset,
-                          add_planes=operands.pop("planes"), add_plane_index=norm.add_plane_index)
+        operands.update(self._pack(eng, operands.pop("planes"), norm))
         if tangents is not None:
           (host_tangent,), tangent_done = tangents.steps[t]
           compute.wait_event(tangent_done)
@@ -880,8 +854,7 @@ class GraphCast(Predictor):
     sink returns after taking them on the device."""
     if self._grad_sink is not None:
       return self._grad_sink(self._engine)
-    return {name: {f: t.cpu().numpy() for f, t in fields.items()}
-            for name, fields in self._engine.grads().items()}
+    return _host_grads(self._engine.grads())
 
   def _stash_step(self, stash: "StepStash") -> None:
     """Keeps the input and target planes of the last `_call` (with targets) in pinned host memory."""
@@ -926,7 +899,7 @@ class GraphCast(Predictor):
     planes = torch.empty([eng.c_in, eng.num_grid], dtype=torch.float32, device=dev)
     tgt = torch.empty([eng.n_out, eng.num_grid], dtype=torch.float32, device=dev)
     scratch = torch.empty([eng.n_out], dtype=torch.float64, device=dev)
-    coef_dev = torch.as_tensor(np.asarray(coef, np.float64)).to(dev)
+    coef_dev = _device_coef(coef, dev)
     compute = torch.cuda.current_stream(dev)
     for b in range(stash.batch):
       fb.a = None
@@ -940,13 +913,7 @@ class GraphCast(Predictor):
           (host_tangent,), tangent_done = pred_tangents.steps[t]
           compute.wait_event(tangent_done)
           tgt.copy_(host_tangent[b], non_blocking=True)
-        affine = {}
-        if norm is None:
-          eng.pack_inputs(planes)
-        else:
-          eng.pack_inputs(planes, mean=norm.in_mean, scale=norm.in_scale)
-          affine = dict(scale=norm.out_scale, offset=norm.out_offset, add_planes=planes,
-                        add_plane_index=norm.add_plane_index)
+        affine = self._pack(eng, planes, norm)
         if pred_tangents is None:
           eng.loss_and_grads_element(tgt, lat_weight, coef_dev, channel_sums=scratch, feedback=fb,
                                      input_grad=t > 0, **affine)
@@ -970,10 +937,15 @@ class GraphCast(Predictor):
     preds = self._call(inputs, targets, forcings, norm=norm, targets=targets,
                        predictions=predictions)
     slabs = model_utils.channel_layout(targets)
-    num_grid = self._engine.num_grid
-    finish = lambda sums: losses.losses_from_channel_sums(sums, slabs, num_grid,
-                                                          LOSS_PER_VARIABLE_WEIGHTS)
-    return finish, preds, self._channel_sums
+    return (lambda sums: self._losses(slabs, sums)), preds, self._channel_sums
+
+  def _losses(self, slabs, sums: Optional[np.ndarray] = None):
+    """(loss, diagnostics), as `loss` returns them, of the host channel sums [batch, n_out] of targets
+    laid out as `slabs`; by default those of the last call, read back from self._channel_sums."""
+    if sums is None:
+      sums = self._channel_sums.cpu().numpy()
+    return losses.losses_from_channel_sums(sums, slabs, self._engine.num_grid,
+                                           LOSS_PER_VARIABLE_WEIGHTS)
 
   def _device_loss_tangent(self, inputs, targets, forcings, norm: Optional[FusedNormalization],
                            run: "_TangentRun", keep_predictions: bool = False):
@@ -985,35 +957,35 @@ class GraphCast(Predictor):
     direction, [batch, K, c_in, Ng] for a run of K (`run.directions`)).  keep_predictions (a run of one
     direction; loss_and_param_gnvp): this step's prediction tangents [batch, n_out, Ng] in their place."""
     targets = xs.from_xarray(targets)
-    state = {}
+    planes = lat_weight = None
 
-    def element(b, planes_in, planes_tgt, planes_out, channel_sums, affine):
+    def begin():
+      nonlocal planes, lat_weight
       eng = self._engine
-      if "planes" not in state:
-        eng.input_grads_begin()
-        lead = [run.dirs] if run.directions else []
-        rows = eng.n_out if keep_predictions else eng.c_in
-        state["planes"] = torch.empty([run.batch] + lead + [rows, eng.num_grid],
-                                      dtype=torch.float32, device=eng.device)
-        state["lat_weight"] = self._lat_weight(targets, eng.device)
+      eng.input_grads_begin()
+      lead = [run.dirs] if run.directions else []
+      rows = eng.n_out if keep_predictions else eng.c_in
+      planes = torch.empty([run.batch] + lead + [rows, eng.num_grid], dtype=torch.float32,
+                           device=eng.device)
+      lat_weight = self._lat_weight(targets, eng.device)
+
+    def element(b, planes_tgt, planes_out, channel_sums, affine):
+      eng = self._engine
       tangent_out = torch.empty([run.dirs, eng.n_out, eng.num_grid], dtype=torch.float32,
                                 device=eng.device)
       keep = None if keep_predictions else (
-          lambda p: state["planes"][b].copy_(p if run.directions else p[0]))
+          lambda p: planes[b].copy_(p if run.directions else p[0]))
       run.element(eng, b, tangent_out, None, norm, affine, keep=keep)
       if keep_predictions:
-        state["planes"][b].copy_(tangent_out[0])
-      eng.output_loss(planes_tgt, state["lat_weight"], channel_sums=channel_sums,
-                      planes_out=planes_out, **affine)
+        planes[b].copy_(tangent_out[0])
+      eng.output_loss(planes_tgt, lat_weight, channel_sums=channel_sums, planes_out=planes_out,
+                      **affine)
 
     preds = self._call(inputs, targets, forcings, norm=norm, targets=targets, predictions=True,
-                       element=element)
+                       begin=begin, element=element)
     run.step += 1
     slabs = model_utils.channel_layout(targets)
-    num_grid = self._engine.num_grid
-    finish = lambda sums: losses.losses_from_channel_sums(sums, slabs, num_grid,
-                                                          LOSS_PER_VARIABLE_WEIGHTS)
-    return finish, preds, self._channel_sums, state["planes"]
+    return (lambda sums: self._losses(slabs, sums)), preds, self._channel_sums, planes
 
   def _lat_weight(self, targets: xs.Dataset, device) -> torch.Tensor:
     """Normalised latitude weights of the targets' grid (float32, on the device), cached."""
@@ -1038,17 +1010,16 @@ class GraphCast(Predictor):
     return bufs[buf], fresh
 
   def _call(self, inputs, targets_template, forcings, norm: Optional[FusedNormalization],
-            targets: Optional[xs.Dataset] = None, predictions: bool = True,
-            grad_coef: Optional[np.ndarray] = None, element=None):
+            targets: Optional[xs.Dataset] = None, predictions: bool = True, begin=None,
+            element=None):
     """The step for every batch element.  With `targets` (shaped like the template, usually the
     same Dataset) the outputs go through gcb_output_loss instead of the plain unpack: the loss sums
     land in a new [batch, n_out] fp64 device tensor, self._channel_sums, and the predictions are
-    returned only when `predictions` is set (else None).  With `grad_coef` ([n_out] coefficients
-    2 kappa / batch of the loss derivative) every element also runs the backward pass, which
-    accumulates the parameter gradients in the engine (Engine.loss_and_grads_element).  With
-    `element`, element(b, planes_in[b], target planes or None, prediction planes or None, channel sums
-    or None, affine keywords) replaces the step of every batch element after its inputs are packed
-    (the input gradients of one target time)."""
+    returned only when `predictions` is set (else None).  With `element`, element(b, target planes or
+    None, prediction planes or None, channel sums or None, affine keywords of _pack) replaces the
+    step of every batch element after its inputs are packed (the derivative calls of one target
+    time); begin() runs once before the first element, after the planes are staged and the engine
+    exists."""
     inputs = xs.from_xarray(inputs)
     forcings = xs.from_xarray(forcings)
     targets_template = xs.from_xarray(targets_template)
@@ -1120,50 +1091,25 @@ class GraphCast(Predictor):
       compute.wait_event(ready)
 
     # Predictions are produced into fresh planes each call (they are handed out).
-    if grad_coef is not None:
-      coef_dev = torch.as_tensor(np.asarray(grad_coef, np.float64)).to(eng.device)
-      eng.grads_begin()
     planes_out = None
     if predictions:
       planes_out = torch.empty([batch, eng.n_out, eng.num_grid], dtype=torch.float32,
                                device=eng.device)
+    if begin is not None:
+      begin()
     for b in range(batch):
+      affine = self._pack(eng, planes_in[b], norm)
+      tgt = None if targets is None else planes_tgt[b]
+      out = None if planes_out is None else planes_out[b]
+      sums = None if targets is None else channel_sums[b]
       if element is not None:
-        if norm is None:
-          eng.pack_inputs(planes_in[b])
-        else:
-          eng.pack_inputs(planes_in[b], mean=norm.in_mean, scale=norm.in_scale)
-        affine = {} if norm is None else dict(
-            scale=norm.out_scale, offset=norm.out_offset, add_planes=planes_in[b],
-            add_plane_index=norm.add_plane_index)
-        element(b, planes_in[b], None if targets is None else planes_tgt[b],
-                None if planes_out is None else planes_out[b],
-                None if targets is None else channel_sums[b], affine)
+        element(b, tgt, out, sums, affine)
         continue
+      eng.step()
       if targets is not None:
-        affine = {} if norm is None else dict(
-            scale=norm.out_scale, offset=norm.out_offset, add_planes=planes_in[b],
-            add_plane_index=norm.add_plane_index)
-        if norm is None:
-          eng.pack_inputs(planes_in[b])
-        else:
-          eng.pack_inputs(planes_in[b], mean=norm.in_mean, scale=norm.in_scale)
-        if grad_coef is not None:
-          eng.loss_and_grads_element(planes_tgt[b], lat_weight, coef_dev,
-                                     channel_sums=channel_sums[b], **affine)
-          continue
-        eng.step()
-        eng.output_loss(planes_tgt[b], lat_weight, channel_sums=channel_sums[b],
-                        planes_out=None if planes_out is None else planes_out[b], **affine)
-      elif norm is None:
-        eng.pack_inputs(planes_in[b])
-        eng.step()
-        eng.unpack_outputs(planes_out[b])
+        eng.output_loss(tgt, lat_weight, channel_sums=sums, planes_out=out, **affine)
       else:
-        eng.pack_inputs(planes_in[b], mean=norm.in_mean, scale=norm.in_scale)
-        eng.step()
-        eng.unpack_outputs(planes_out[b], scale=norm.out_scale, offset=norm.out_offset,
-                           add_planes=planes_in[b], add_plane_index=norm.add_plane_index)
+        eng.unpack_outputs(out, **affine)
     free = torch.cuda.Event()
     free.record(compute)
     self._buf_free[buf] = free
@@ -1173,6 +1119,18 @@ class GraphCast(Predictor):
     # planes -> Dataset shaped like the template
     # (reference _grid_node_outputs_to_prediction :701-723, stacked_to_dataset).
     return self._planes_to_dataset(planes_out, targets_template, n_lat, n_lon)
+
+  @staticmethod
+  def _pack(eng: engine_lib.Engine, planes: torch.Tensor, norm: Optional[FusedNormalization]) -> dict:
+    """Packs one batch element's input planes [c_in, Ng] into eng.grid_in_img, normalised by `norm`,
+    and returns the affine keywords that unpack its step's outputs (unpack_outputs, output_loss): none
+    without `norm`."""
+    if norm is None:
+      eng.pack_inputs(planes)
+      return {}
+    eng.pack_inputs(planes, mean=norm.in_mean, scale=norm.in_scale)
+    return dict(scale=norm.out_scale, offset=norm.out_offset, add_planes=planes,
+                add_plane_index=norm.add_plane_index)
 
   @staticmethod
   def _check_template(template: xs.Dataset, n_channels: int):
@@ -1236,6 +1194,24 @@ def check_param_tangents(param_tangents, params) -> Dict[str, Dict[str, np.ndarr
         raise ValueError(f"param_tangents {name}:{f} has shape {arr.shape}, the parameter {want}")
       out.setdefault(name, {})[f] = arr
   return out
+
+
+def loss_coefficients(targets: xs.Dataset, num_grid: int, batch: int, steps: int = 1):
+  """(channel slabs of `targets`, [n_out] float64 coefficients 2 kappa / (batch * steps)): the loss
+  derivative with respect to the channel sums of gcb_output_loss (losses.channel_kappa) of the mean
+  loss over `batch` elements and `steps` target times."""
+  slabs = model_utils.channel_layout(targets)
+  return slabs, 2.0 * losses.channel_kappa(slabs, num_grid, LOSS_PER_VARIABLE_WEIGHTS) / (batch * steps)
+
+
+def _device_coef(coef: np.ndarray, device) -> torch.Tensor:
+  """Loss coefficients (loss_coefficients) as a float64 tensor on `device`."""
+  return torch.as_tensor(np.asarray(coef, np.float64)).to(device)
+
+
+def _host_grads(grads) -> Dict[str, Dict[str, np.ndarray]]:
+  """Device gradients {module: {field: tensor}} as host numpy arrays."""
+  return {name: {f: t.cpu().numpy() for f, t in fields.items()} for name, fields in grads.items()}
 
 
 def hvp_tangent_planes(inputs: xs.Dataset, forcings: xs.Dataset, input_tangents,

@@ -196,8 +196,7 @@ class InputsAndResiduals(graphcast.Predictor):
     inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
     targets_template = xs.from_xarray(targets_template)
     if isinstance(self._predictor, graphcast.GraphCast):
-      device = self._predictor._device or f"cuda:{torch.cuda.current_device()}"
-      consts = self._fused_constants(inputs, targets_template, forcings, torch.device(device))
+      consts = self._norm_of()(inputs, targets_template, forcings)
       return self._predictor._call(inputs, targets_template, forcings, norm=consts)
     norm_inputs = normalize(inputs, self._scales, self._locations)
     norm_forcings = normalize(forcings, self._scales, self._locations)
@@ -225,50 +224,43 @@ class InputsAndResiduals(graphcast.Predictor):
   def _fuses(self) -> bool:
     return isinstance(self._predictor, graphcast.GraphCast)
 
+  def _norm_of(self, what: str = "fused calls"):
+    """norm_of(inputs, targets, forcings) -> their FusedNormalization, its constants on the device the
+    wrapped GraphCast runs on (GraphCast.compute_device).  A wrapped predictor that is not a GraphCast
+    raises NotImplementedError here, `what` naming the call, so a call that refuses it before its
+    other checks asks for norm_of first."""
+    if not self._fuses():
+      raise NotImplementedError(f"{what} need a GraphCast predictor directly inside "
+                                "InputsAndResiduals (the fused normalisation)")
+    return lambda inputs, targets, forcings: self._fused_constants(
+        xs.from_xarray(inputs), xs.from_xarray(targets), xs.from_xarray(forcings),
+        self._predictor.compute_device())
+
   def _device_loss(self, inputs, targets, forcings, predictions: bool):
     """GraphCast only: the step with the fused loss (graphcast.GraphCast._device_loss), the
     target normalisation applied inside the kernel from the fused constants."""
-    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
-    targets = xs.from_xarray(targets)
-    device = self._predictor._device or f"cuda:{torch.cuda.current_device()}"
-    consts = self._fused_constants(inputs, targets, forcings, torch.device(device))
-    return self._predictor._device_loss(inputs, targets, forcings, consts, predictions)
+    norm = self._norm_of()(inputs, targets, forcings)
+    return self._predictor._device_loss(inputs, targets, forcings, norm, predictions)
 
   def loss_and_grads(self, inputs, targets, forcings, **kwargs):
     """(loss, diagnostics, grads) of `loss` and its parameter gradients (GraphCast.loss_and_grads),
     with the normalisation fused into the kernels as in `loss`.  GraphCast only."""
-    if not self._fuses():
-      raise NotImplementedError("parameter gradients need a GraphCast predictor directly inside "
-                                "InputsAndResiduals (the fused normalisation)")
-    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
-    targets = xs.from_xarray(targets)
-    device = self._predictor._device or f"cuda:{torch.cuda.current_device()}"
-    consts = self._fused_constants(inputs, targets, forcings, torch.device(device))
-    return self._predictor._loss_and_grads(inputs, targets, forcings, norm=consts)
-
-  def _fused_for(self, inputs, targets, forcings, what: str):
-    if not self._fuses():
-      raise NotImplementedError(f"{what} need a GraphCast predictor directly inside "
-                                "InputsAndResiduals (the fused normalisation)")
-    inputs, forcings = xs.from_xarray(inputs), xs.from_xarray(forcings)
-    targets = xs.from_xarray(targets)
-    device = self._predictor._device or f"cuda:{torch.cuda.current_device()}"
-    return inputs, targets, forcings, self._fused_constants(inputs, targets, forcings,
-                                                            torch.device(device))
+    norm = self._norm_of("parameter gradients")(inputs, targets, forcings)
+    return self._predictor._loss_and_grads(inputs, targets, forcings, norm=norm)
 
   def loss_and_input_grads(self, inputs, targets, forcings, **kwargs):
     """(loss, diagnostics, input_grads, forcing_grads) of `loss` (GraphCast.loss_and_input_grads):
     the gradients are in the physical units of the inputs and forcings, through the normalisation of
     the inputs, the residual add and the target normalisation.  GraphCast only."""
-    inputs, targets, forcings, consts = self._fused_for(inputs, targets, forcings, "input gradients")
-    return self._predictor._loss_and_input_grads(inputs, targets, forcings, norm=consts)
+    norm = self._norm_of("input gradients")(inputs, targets, forcings)
+    return self._predictor._loss_and_input_grads(inputs, targets, forcings, norm=norm)
 
   def loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
                          **kwargs):
     """loss_and_input_grads and the Hessian-vector product of its loss (GraphCast.loss_and_input_hvp),
     with respect to the inputs and forcings in their physical units.  GraphCast only."""
-    inputs, targets, forcings, consts = self._fused_for(inputs, targets, forcings, "input gradients")
-    return self._predictor._loss_and_input_grads(inputs, targets, forcings, norm=consts,
+    norm = self._norm_of("input gradients")(inputs, targets, forcings)
+    return self._predictor._loss_and_input_grads(inputs, targets, forcings, norm=norm,
                                                  tangents=(input_tangents, forcing_tangents))
 
   def batched_loss_and_input_hvp(self, inputs, targets, forcings, input_tangents, forcing_tangents=None,
@@ -276,27 +268,26 @@ class InputsAndResiduals(graphcast.Predictor):
     """loss_and_input_hvp along K tangent directions at once (GraphCast.batched_loss_and_input_hvp),
     with respect to the inputs and forcings in their physical units.  GraphCast only."""
     def one_pass(it, ft):
-      ins, tgt, fs, consts = self._fused_for(inputs, targets, forcings, "input gradients")
-      return self._predictor._loss_and_input_grads(ins, tgt, fs, norm=consts, tangents=(it, ft),
-                                                   directions=True)
+      norm = self._norm_of("input gradients")(inputs, targets, forcings)
+      return self._predictor._loss_and_input_grads(inputs, targets, forcings, norm=norm,
+                                                   tangents=(it, ft), directions=True)
     return graphcast.batched_hvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
                                  directions_per_pass)
 
   def input_vjp(self, inputs, targets_template, forcings, cotangents, **kwargs):
     """(predictions, input_grads, forcing_grads) of the un-normalised predictions of __call__
     (GraphCast.input_vjp).  GraphCast only."""
-    inputs, targets_template, forcings, consts = self._fused_for(inputs, targets_template, forcings,
-                                                                 "input gradients")
-    return self._predictor._input_vjp(inputs, targets_template, forcings, cotangents, norm=consts)
+    norm = self._norm_of("input gradients")(inputs, targets_template, forcings)
+    return self._predictor._input_vjp(inputs, targets_template, forcings, cotangents, norm=norm)
 
   def batched_input_vjp(self, inputs, targets_template, forcings, cotangents, *,
                         directions_per_pass=None, **kwargs):
     """input_vjp of K cotangents at once (GraphCast.batched_input_vjp), of the un-normalised
     predictions.  GraphCast only."""
     def one_pass(cot, first):
-      ins, tt, fs, consts = self._fused_for(inputs, targets_template, forcings, "input gradients")
-      return self._predictor._input_vjp(ins, tt, fs, cot, norm=consts, directions=True,
-                                        predictions=first)
+      norm = self._norm_of("input gradients")(inputs, targets_template, forcings)
+      return self._predictor._input_vjp(inputs, targets_template, forcings, cot, norm=norm,
+                                        directions=True, predictions=first)
     return graphcast.batched_vjp(one_pass, targets_template, cotangents, directions_per_pass)
 
   def input_jvp(self, inputs, targets_template, forcings, input_tangents, forcing_tangents=None,
@@ -306,9 +297,8 @@ class InputsAndResiduals(graphcast.Predictor):
     and the residual add.  GraphCast only."""
     run = graphcast.GraphCast._one_step_tangents(inputs, targets_template, forcings, input_tangents,
                                                  forcing_tangents)
-    inputs, targets_template, forcings, consts = self._fused_for(inputs, targets_template, forcings,
-                                                                 "input gradients")
-    return self._predictor._input_jvp(inputs, targets_template, forcings, run, norm=consts)
+    norm = self._norm_of("input gradients")(inputs, targets_template, forcings)
+    return self._predictor._input_jvp(inputs, targets_template, forcings, run, norm=norm)
 
   def batched_input_jvp(self, inputs, targets_template, forcings, input_tangents,
                         forcing_tangents=None, *, directions_per_pass=None, **kwargs):
@@ -317,8 +307,8 @@ class InputsAndResiduals(graphcast.Predictor):
     def one_pass(it, ft):
       run = graphcast.GraphCast._one_step_tangents(inputs, targets_template, forcings, it, ft,
                                                    directions=True)
-      ins, tt, fs, consts = self._fused_for(inputs, targets_template, forcings, "input gradients")
-      return self._predictor._input_jvp(ins, tt, fs, run, norm=consts)
+      norm = self._norm_of("input gradients")(inputs, targets_template, forcings)
+      return self._predictor._input_jvp(inputs, targets_template, forcings, run, norm=norm)
     return graphcast.batched_jvp(one_pass, inputs, forcings, input_tangents, forcing_tangents,
                                  directions_per_pass)
 
@@ -326,43 +316,33 @@ class InputsAndResiduals(graphcast.Predictor):
     """(predictions, prediction_tangents) of the un-normalised predictions of __call__ along
     param_tangents (GraphCast.param_jvp): the tangents are in physical units, through the
     un-normalisation of the outputs.  GraphCast only."""
-    self._refuse_unfused()
+    norm_of = self._norm_of("parameter gradients")
     run = self._predictor._param_tangent_run(inputs, targets_template, forcings, param_tangents,
                                              num_steps=1)
-    inputs, targets_template, forcings, consts = self._fused_for(inputs, targets_template, forcings,
-                                                                 "parameter gradients")
-    return self._predictor._input_jvp(inputs, targets_template, forcings, run, norm=consts)
+    return self._predictor._input_jvp(inputs, targets_template, forcings, run,
+                                      norm=norm_of(inputs, targets_template, forcings))
 
   def loss_and_param_gnvp(self, inputs, targets, forcings, param_tangents, **kwargs):
     """(loss, diagnostics, gnvp) of `loss` (GraphCast.loss_and_param_gnvp), with the normalisation
     fused into the kernels as in `loss`.  GraphCast only."""
-    self._refuse_unfused()
+    norm_of = self._norm_of("parameter gradients")
     if xs.from_xarray(targets).sizes.get("time", 1) != 1:
       raise NotImplementedError("Gauss-Newton products cover one target time (several are not "
                                 "provided)")
     self._predictor._checked_param_tangents(param_tangents)
-    inputs, targets, forcings, consts = self._fused_for(inputs, targets, forcings,
-                                                        "parameter gradients")
     return self._predictor._loss_and_param_gnvp(inputs, targets, forcings, param_tangents,
-                                                norm=consts)
+                                                norm=norm_of(inputs, targets, forcings))
 
   def loss_and_param_hvp(self, inputs, targets, forcings, param_tangents, **kwargs):
     """(loss, diagnostics, grads, hvp) of `loss` (GraphCast.loss_and_param_hvp), with the
     normalisation fused into the kernels as in `loss`.  GraphCast only."""
-    self._refuse_unfused()
+    norm_of = self._norm_of("parameter gradients")
     if xs.from_xarray(targets).sizes.get("time", 1) != 1:
       raise NotImplementedError("parameter Hessian-vector products cover one target time (several "
                                 "are not provided)")
     self._predictor._checked_param_tangents(param_tangents)
-    inputs, targets, forcings, consts = self._fused_for(inputs, targets, forcings,
-                                                        "parameter gradients")
     return self._predictor._loss_and_param_hvp(inputs, targets, forcings, param_tangents,
-                                               norm=consts)
-
-  def _refuse_unfused(self) -> None:
-    if not self._fuses():
-      raise NotImplementedError("parameter gradients need a GraphCast predictor directly inside "
-                                "InputsAndResiduals (the fused normalisation)")
+                                               norm=norm_of(inputs, targets, forcings))
 
   def loss(self, inputs, targets, forcings, **kwargs):
     """The loss computed on normalised inputs and targets (targets that are also inputs as
