@@ -50,6 +50,22 @@ constexpr int kChainParamVecs = 8;          // [512]-float parameter vectors (bi
 template <bool kSplit>
 using ChainConfig = StageRing<kSplit, kLnxBytes + kChainTailBytes + kChainParamVecs * kMaxN * 4>;
 
+// The accumulator table of an acc_table layer streams through the operand ring like any other
+// operand: the TMA warp copies this CTA's 256 columns of each row (1 KB, one bulk copy) into a stage,
+// TabSlab::kRows rows per stage, in TabSlab::kSteps pseudo-K-steps per unit.  16 rows per stage (bf16x3) are
+// exactly the rows of one consumer warp, 8 (bf16) the rows of one of its two row halves.  The row
+// pitch in shared memory is 1 KB + 16 B, so that the 8 rows a warp's LDS.64 touches at once fall on
+// distinct banks.
+constexpr int kTabRowBytes = kUnitN * 4;
+constexpr int kTabRowPitch = kTabRowBytes + 16;
+constexpr int kUnitRowsPerWarp = kTileM / kConsumerWarps;   // 16: rows lr0 and lr0 + 8 of its 32 lanes
+template <bool kSplit>
+struct TabSlab {
+  static constexpr int kRows = ChainConfig<kSplit>::kStageBytes / kTabRowPitch >= 16 ? 16 : 8;
+  static constexpr int kSteps = kTileM / kRows;
+  static_assert(kRows * kTabRowPitch <= ChainConfig<kSplit>::kStageBytes, "a table slab must fit a stage");
+};
+
 // kKindLN*: LayerNorm without residual / with an fp32 residual / with an operand-image residual;
 // kKindAcc: the raw accumulator to `out` (gcb_chain_layer.acc_out)
 enum { kKindPlain = 0, kKindSwish = 1, kKindLN = 2, kKindLNRes = 3, kKindLNImg = 4, kKindAcc = 5 };
@@ -150,19 +166,59 @@ __device__ __forceinline__ void epi_load_res_img(const ChainEpi& e, uint2 (&buf)
     }
 }
 
-// Accumulator of a table layer (gcb_chain_layer.acc_table): this thread's fragment, rows lr0 + 8h
-// and columns 8j + 2q (+1) of the unit, straight from the fp32 table (rows past the end: 0).
-// Fully unrolled, so every load targets a fixed accumulator register and all 64 are in flight at once.
-__device__ __forceinline__ void load_acc_table(float (&acc)[128], const float* const (&row)[2],
-                                               const bool (&ok)[2]) {
-#pragma unroll
-  for (int j = 0; j < 32; ++j)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const uint2 v = ptx::ld_global_nc_v2_pred(row[h] + 8 * j, ok[h], 0u);
-      acc[4 * j + 2 * h] = __uint_as_float(v.x);
-      acc[4 * j + 2 * h + 1] = __uint_as_float(v.y);
+// Accumulator of a table layer (gcb_chain_layer.acc_table), from the table rows the TMA warp put into
+// the next kSteps stages of the ring (TabSlab): this thread's fragment, rows lr0 + 8h and columns
+// 8j + 2q (+1) of the unit, read by the warp whose rows a stage holds (rows past the end: 0).  Every
+// consumer warp waits for every stage and releases it in both CTAs, as mma_unit does, so that the
+// stage barriers count as for a unit of MMAs.  Called for EVERY unit, `tab` false for units with MMAs:
+// then no barrier is touched, the loads read whatever the current stage holds (possibly bytes a bulk
+// copy is still writing), and a select discards them and leaves 0 in the accumulator, which the unit's
+// first wgmma overwrites.  Accumulator registers written on one path only (a branch around the loads or
+// around the MMAs, or a predicated load) make ptxas serialize every wgmma of the kernel, each waiting
+// for the previous one to retire.
+template <bool kSplit, int kStages, int kStageBytes>
+__device__ __forceinline__ void read_acc_table(float (&acc)[128], bool tab, uint8_t* stage_base, uint64_t* full_bar,
+                                               uint64_t* empty_bar, uint32_t& stage, uint32_t& phase, int lr0,
+                                               const bool (&ok)[2], uint32_t unit) {
+  using Slab = TabSlab<kSplit>;
+  constexpr int kOwn = kUnitRowsPerWarp / Slab::kRows;      // stages holding this warp's rows: 1 or 2
+  static_assert(kOwn * Slab::kRows == kUnitRowsPerWarp, "a warp's rows fill whole stages");
+  const bool lead = (threadIdx.x & 31) == 0;
+  const int first = lr0 / Slab::kRows;                     // warp-uniform: lr0 - lane / 4 is a multiple of 16
+  auto wait = [&](int p) {
+    ptx::mbar_wait(&full_bar[stage], phase);
+    if (p == 0 && threadIdx.x == 4 * 32) trace(unit, 1);
+  };
+  auto release = [&]() {
+    __syncwarp();
+    if (lead) {
+      const uint32_t a = ptx::smem_addr(&empty_bar[stage]);
+      ptx::mbar_arrive_remote_cta(ptx::mapa(a, 0));
+      ptx::mbar_arrive_remote_cta(ptx::mapa(a, 1));
     }
+    if (++stage == kStages) { stage = 0; phase ^= 1; }
+  };
+  if (tab) {
+    for (int p = 0; p < first; ++p) { wait(p); release(); }
+    wait(first);
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (h == 1 && kOwn == 2 && tab) { release(); wait(first + 1); }
+    const uint32_t ra = ptx::smem_addr(stage_base + stage * kStageBytes) + 8 * (threadIdx.x & 3) +
+                        ((lr0 + 8 * h) % Slab::kRows) * kTabRowPitch;
+    const bool use = tab && ok[h];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const uint2 v = ptx::ld_shared_v2_u32(ra + 32 * j);
+      acc[4 * j + 2 * h] = __uint_as_float(use ? v.x : 0u);
+      acc[4 * j + 2 * h + 1] = __uint_as_float(use ? v.y : 0u);
+    }
+  }
+  if (tab) {
+    release();
+    for (int p = first + kOwn; p < Slab::kSteps; ++p) { wait(p); release(); }
+  }
 }
 // kKindAcc: the accumulator itself to `out`, without the + 0 of an absent bias or residual, so that
 // a table built from it (acc_table) holds the accumulator's bits, the sign of a zero included.
@@ -431,6 +487,33 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
           const uint8_t* b_ptr = s_layer[l].w + static_cast<size_t>(crank) * b_block;
           const bool tr = tracing(tu);
           long long blocked = 0, hwait = 0;
+          if constexpr (kTab) {
+            if (s_acc[l].acc != nullptr) {
+              // A table layer (nseg = 0): its rows of this tile into the next kSteps stages, one bulk
+              // copy per row, spread over the lanes.  Rows past the end are not copied; a stage
+              // without a valid row completes with the arrive alone.
+              using Slab = TabSlab<kSplit>;
+              const AccTableInfo at = s_acc[l];
+              const long long row0 = static_cast<long long>(tile) * kTileM;
+              for (int p = 0; p < Slab::kSteps; ++p) {
+                const long long r0 = row0 + p * Slab::kRows;
+                const int nrows = static_cast<int>(max(0ll, min(static_cast<long long>(Slab::kRows), rows_total - r0)));
+                const long long w0 = tr ? clock64() : 0;
+                ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+                if (tr) blocked += clock64() - w0;
+                if (lane == 0) {
+                  if (nrows > 0) ptx::mbar_arrive_expect_tx(&full_bar[stage], nrows * kTabRowBytes);
+                  else ptx::mbar_arrive(&full_bar[stage]);
+                }
+                __syncwarp();
+                if (lane < nrows)
+                  ptx::bulk_g2s(stage_base + stage * Cfg::kStageBytes + lane * kTabRowPitch,
+                                at.acc + (r0 + lane) * at.ld + crank * kUnitN, kTabRowBytes, &full_bar[stage]);
+                __syncwarp();
+                if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+              }
+            }
+          }
           for (int s = 0; s < nseg; ++s) {
             const SegInfo sg = s_seg[l * 3 + s];
             const uint8_t* a_ptr = nullptr;
@@ -493,6 +576,17 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
           if (ti < 0 || ti >= T) continue;
           const uint32_t tile = cid + static_cast<uint32_t>(ti) * ncl;
           const int nseg = s_layer[l].nseg;
+          if constexpr (kTab) {
+            // A table layer's stages (read_acc_table): arrivals only.
+            if (any_table && s_acc[l].acc != nullptr) {
+              for (int p = 0; p < TabSlab<kSplit>::kSteps; ++p) {
+                ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+                __syncwarp();
+                if (lane == 0) ptx::mbar_arrive(&full_bar[stage]);
+                if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+              }
+            }
+          }
           for (int s = 0; any_table && s < nseg; ++s) {
             const SegInfo sg = s_seg[l * 3 + s];
             const bool is_tab = sg.src_q < 0 && sg.img == nullptr;
@@ -535,16 +629,11 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         const ChainLayer& cl = s_layer[l];
         const int kind = cl.kind;
         const float* const s_bias = cl.bias_off >= 0 ? s_param + cl.bias_off : nullptr;
-        if (eg == 0 && ti + 1 < T && (cl.residual != nullptr || cl.res_img != nullptr || (kTab && s_acc[l].acc != nullptr))) {
-          // Pull the residual (or the accumulator table) of this layer's NEXT tile into L2 now (a
-          // whole step ahead).
+        if (eg == 0 && ti + 1 < T && (cl.residual != nullptr || cl.res_img != nullptr)) {
+          // Pull the residual of this layer's NEXT tile into L2 now (a whole step ahead).
           const uint32_t ntile = tile + ncl;
           const int pr = (warp & 3) * 32 + lane;      // 128 threads: one row each
-          if (kTab && s_acc[l].acc != nullptr) {
-            const AccTableInfo at = s_acc[l];
-            const long long nrow = static_cast<long long>(ntile) * kTileM + pr;
-            if (nrow < rows_total) ptx::bulk_prefetch_l2(at.acc + nrow * at.ld + col_base, kUnitN * 4);
-          } else if (cl.residual != nullptr) {
+          if (cl.residual != nullptr) {
             const long long nrow = static_cast<long long>(ntile) * kTileM + pr;
             if (nrow < rows_total) ptx::bulk_prefetch_l2(cl.residual + nrow * cl.ld_res + col_base, kUnitN * 4);
           } else if (pr < kUnitN / kKStep) {
@@ -613,27 +702,24 @@ mlp_chain_tc_kernel(const __grid_constant__ gcb_chain_desc d, const int nq, cons
         if (want_pre) epi_load_pre(e, buf, 0, true);
         else if (kind == kKindLNRes) epi_load_res(e, buf, 0, 0, true);
         else if (kind == kKindLNImg) epi_load_res_img(e, buf, 0, 0, true);
-        const bool acc_tab = kTab && s_acc[l].acc != nullptr;
-        if (acc_tab) {
-          // No MMAs to hide the loads behind: the table rows go out together with chunk 0's inputs,
-          // before the h_free wait.
-          const long long grow0 = static_cast<long long>(tile) * kTileM + lr0;
-          const AccTableInfo at = s_acc[l];
-          const float* row[2] = {at.acc + grow0 * at.ld + col_base + 2 * q,
-                                 at.acc + (grow0 + 8) * at.ld + col_base + 2 * q};
-          load_acc_table(acc, row, e.row_ok);
-        }
         if (lead && eg == 0) trace(u, 0);
+        // A table layer's accumulator comes through the ring: read with chunk 0's inputs in flight and
+        // before the h_free wait.
+        if constexpr (kTab)
+          read_acc_table<kSplit, Cfg::kStages, Cfg::kStageBytes>(acc, s_acc[l].acc != nullptr, stage_base, full_bar,
+                                                                 empty_bar, stage, phase, lr0, e.row_ok, u);
         if (keep_q >= 0) {
           // previous readers of this slot (tile ti - nslots) are done in both CTAs
           ptx::mbar_wait(&h_free_bar[keep_q * kChainSlotsMax + (ti % nslots)],
                          (static_cast<uint32_t>(ti / nslots) & 1u) ^ 1u);
         }
         if (lead && eg == 0) { trace(u, 2); trace_val(u, 9, cl.ksteps); }
-        // A table layer has no segments: no stage was filled for it, and no scratch slot is read.
-        if (!acc_tab)
-          mma_unit<kSplit, Cfg::kStages, Cfg::kStageBytes, Cfg::kAStageBytes>(
-              acc, stage_base, full_bar, empty_bar, stage, phase, cl.ksteps, eg * 64 * 16, cmask, u);
+        // A table layer has no segments (cl.ksteps = 0): its stages hold table rows, and no scratch slot
+        // is read.  The call is not skipped for it: a branch around the MMAs makes ptxas serialize every
+        // wgmma of the kernel (each waits for the previous one to retire), which cost the MMA units of
+        // the kTab variants a third of their speed.
+        mma_unit<kSplit, Cfg::kStages, Cfg::kStageBytes, Cfg::kAStageBytes, kTab>(
+            acc, stage_base, full_bar, empty_bar, stage, phase, cl.ksteps, eg * 64 * 16, cmask, u);
         if (lane == 0) {
           // Every scratch slot this unit read is reusable (in both CTAs) once these MMAs retired.
           // The slot's readers are bulk copies that have completed (their bytes were counted on

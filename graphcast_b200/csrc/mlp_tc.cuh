@@ -164,8 +164,9 @@ struct PreAddInfo {
 // The MMAs of one unit for this warpgroup's 64 rows (A rows start a_row_off bytes into the
 // stage).  After each K-step the previous one is retired and its stage released: one arrival
 // per warp, on the local barrier (rel_mask == 0) or on the barrier of every CTA in rel_mask.
-// `unit` only indexes the timeline trace (event 1: first full barrier passed).
-template <bool kSplit, int kStages, int kStageBytes, int kAStageBytes>
+// `unit` only indexes the timeline trace (event 1: first full barrier passed).  kMayBeEmpty: ksteps may
+// be 0 (a chain unit whose accumulator came from a table), and then no stage is released.
+template <bool kSplit, int kStages, int kStageBytes, int kAStageBytes, bool kMayBeEmpty = false>
 __device__ __forceinline__ void mma_unit(float (&acc)[128], uint8_t* stage_base, uint64_t* full_bar,
                                          uint64_t* empty_bar, uint32_t& stage, uint32_t& phase,
                                          int ksteps, uint32_t a_row_off, uint32_t rel_mask, uint32_t unit) {
@@ -212,7 +213,7 @@ __device__ __forceinline__ void mma_unit(float (&acc)[128], uint8_t* stage_base,
   }
   ptx::wgmma_wait<0>();
   ptx::fence_regs(acc);
-  release(prev);
+  if (!kMayBeEmpty || ksteps > 0) release(prev);
 }
 
 // Shifted sums of this thread's two rows over the unit columns c < ncols, bias included:

@@ -150,6 +150,12 @@ __device__ __forceinline__ float2 ld_shared_v2_pred(uint32_t saddr, bool pred) {
       : "=f"(v.x), "=f"(v.y) : "r"(saddr), "r"(static_cast<uint32_t>(pred)));
   return v;
 }
+// 8 bytes from shared memory into integer registers, unpredicated (ld_shared_v2_pred is predicated).
+__device__ __forceinline__ uint2 ld_shared_v2_u32(uint32_t saddr) {
+  uint2 v;
+  asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(saddr));
+  return v;
+}
 __device__ __forceinline__ void st_global_v2_pred(void* ptr, float2 v, bool pred) {
   asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %3, 0;\n @p st.global.v2.f32 [%0], {%1, %2};\n}"
                ::"l"(ptr), "f"(v.x), "f"(v.y), "r"(static_cast<uint32_t>(pred)) : "memory");

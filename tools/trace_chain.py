@@ -8,8 +8,8 @@ the two paths, CUDA-event times, and the in-kernel timeline of cluster 0 / CTA 0
 launch (cycles; per executed unit: barrier waits, MMA phase per K-step against the 768-cycle
 tensor-pipe ideal, LayerNorm statistics, epilogue stores, scratch hand-over).  The "edge-table" case
 is the edge problem with the first layer's accumulator read from a table (gcb_chain_layer.acc_table,
-filled by an acc_out chain) instead of computed: its layer-0 units have no MMAs, and their "columns"
-cycles include the wait for the table rows."""
+filled by an acc_out chain) instead of computed: its layer-0 units have no MMAs; their operand wait
+is the wait for the first stage of table rows, and their "mma" column the walk over the rest."""
 import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
@@ -116,32 +116,43 @@ IDEAL_KSTEP = 768   # tensor cycles per K-step and CTA: 6 x m64n256k16 (bf16x3, 
 
 def print_timeline(t):
   """Events: see the trace comment in graphcast_b200/csrc/mlp_tc.cuh.  Cycles after the previous
-  event of the same unit; per K-step = MMA phase (first full barrier -> MMAs retired) / K-steps."""
+  event of the same unit; per K-step = MMA phase (first full barrier -> MMAs retired) / K-steps.  A
+  table unit (0 K-steps) reads its stages of table rows before the h_free wait: its "ops_ready" is the
+  wait for the first stage after the unit start, and its "mma" the walk over the stages plus the
+  h_free wait."""
   base = t[2, 0]
   print("   u L | start  h_free  ops_ready  mma (per K-step / ideal) | ln_stats  columns  handed"
         " | next unit | tma: blocked h_full_wait")
   tot = np.zeros(8)
   per_layer = {}
   for u in range(2, 14):
-    r = t[u].copy()
-    if r[9] == 0:
-      r[1] = r[3]                        # a table unit: no MMAs, no operand barrier
-    mma = r[3] - r[1]
+    r = t[u]
+    if r[9] > 0:
+      hfree, ops, mma = r[2] - r[0], r[1] - r[2], r[3] - r[1]
+    elif r[1] > 0:
+      hfree, ops, mma = 0, r[1] - r[0], r[3] - r[1]
+    else:                                # table read by the consumers' own global loads: no stages
+      hfree, ops, mma = r[2] - r[0], 0, 0
     ln = r[4] - r[3] if r[4] > 0 else 0
     stored = r[5] - max(r[4], r[3])      # column loop
     handed = r[6] - r[5]                 # last store issued -> h_full arrives done
     nxt = t[u + 1, 0] - r[0]
-    tot += [r[2] - r[0], r[1] - r[2], mma, ln + stored + handed, nxt, r[9], stored, handed]
-    per_layer.setdefault(int(r[11]), []).append((nxt, stored))
-    print(f"  {u:2d} {r[11]} | {r[0]-base:8d} +{r[2]-r[0]:6d} +{r[1]-r[2]:6d} +{mma:7d} ({mma / max(r[9], 1):6.0f} / {IDEAL_KSTEP}) | "
+    tot += [hfree, ops, mma if r[9] > 0 else 0, ln + stored + handed, nxt, r[9], stored, handed]
+    per_layer.setdefault(int(r[11]), []).append((nxt, stored, ops, mma, r[9]))
+    per_k = f"{mma / r[9]:6.0f}" if r[9] > 0 else " table"
+    print(f"  {u:2d} {r[11]} | {r[0]-base:8d} +{hfree:6d} +{ops:6d} +{mma:7d} ({per_k} / {IDEAL_KSTEP}) | "
           f"+{ln:6d} +{stored:7d} +{handed:6d} | +{nxt:7d} | {r[7]:7d} {r[8]:7d}")
   print(f"  units 2-13: h_free wait {tot[0]:.0f}, operand wait {tot[1]:.0f}, MMA {tot[2]:.0f} "
-        f"({tot[2] / tot[5]:.0f} cycles per K-step vs {IDEAL_KSTEP}), epilogue + hand-over {tot[3]:.0f}, "
+        f"({tot[2] / max(tot[5], 1):.0f} cycles per K-step vs {IDEAL_KSTEP}), epilogue + hand-over {tot[3]:.0f}, "
         f"unit to unit {tot[4]:.0f} cycles")
   print(f"  epilogue of units 2-13: column loop {tot[6]:.0f}, last store -> h_full arrive {tot[7]:.0f} cycles")
   for l, v in sorted(per_layer.items()):
-    print(f"  layer {l}: {len(v)} units, mean unit to unit {np.mean([a for a, _ in v]):.0f} cycles, "
-          f"mean column loop {np.mean([b for _, b in v]):.0f} cycles")
+    ks = sum(x[4] for x in v)
+    phase = (f"MMA {sum(x[3] for x in v) / ks:.0f} cycles per K-step" if ks > 0 else
+             f"table walk {np.mean([x[3] for x in v]):.0f} cycles")
+    print(f"  layer {l}: {len(v)} units, mean unit to unit {np.mean([x[0] for x in v]):.0f} cycles, "
+          f"mean column loop {np.mean([x[1] for x in v]):.0f} cycles, mean operand wait "
+          f"{np.mean([x[2] for x in v]):.0f} cycles, {phase}")
 
 
 case("edge")
