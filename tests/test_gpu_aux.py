@@ -1,4 +1,5 @@
-"""Segment sum and channel pack/unpack kernels against PyTorch references."""
+"""Segment sum and halo row packing kernels against PyTorch references (the channel pack / unpack
+kernels are checked in test_gpu_grid_io_kernels.py)."""
 import numpy as np
 import pytest
 import torch
@@ -43,54 +44,6 @@ def test_segment_sum_skewed_degrees_and_empty_rows():
   lib.gcb_segment_sum_heavy(msg.data_ptr(), 512, rp.data_ptr(), 3000, heavy.data_ptr(), heavy.numel(),
                             out4.data_ptr(), 512, 512, torch.cuda.current_stream().cuda_stream)
   assert torch.equal(out3, out4)
-
-
-def test_pack_and_unpack_are_exact_transposes_with_affine():
-  lib = _native.lib()
-  dev = torch.device("cuda:0")
-  n_ch, n_nodes, ld, n_out = 37, 1000 + 13, 48, 23
-  planes = torch.randn(n_ch, n_nodes, device=dev)
-  static = torch.randn(n_nodes, 3, device=dev)
-  mean, scale = torch.randn(n_ch, device=dev), torch.rand(n_ch, device=dev) + 0.5
-  feats = torch.full((n_nodes, ld), float("nan"), device=dev)
-  st = torch.cuda.current_stream().cuda_stream
-  _native.check(lib.gcb_pack_grid_features(planes.data_ptr(), n_ch, n_nodes, mean.data_ptr(),
-                                           scale.data_ptr(), static.data_ptr(), 3,
-                                           feats.data_ptr(), ld, st), "pack")
-  want = torch.zeros(n_nodes, ld, device=dev)
-  want[:, :n_ch] = ((planes - mean[:, None]) / scale[:, None]).t()
-  want[:, n_ch:n_ch + 3] = static
-  torch.testing.assert_close(feats, want, rtol=1e-6, atol=1e-6)
-  _native.check(lib.gcb_pack_grid_features(planes.data_ptr(), n_ch, n_nodes, None, None,
-                                           static.data_ptr(), 3, feats.data_ptr(), ld, st), "pack")
-  assert torch.equal(feats[:, :n_ch], planes.t())
-
-  # direct operand-image packing == image of the fp32 packing
-  _native.check(lib.gcb_pack_grid_features(planes.data_ptr(), n_ch, n_nodes, mean.data_ptr(),
-                                           scale.data_ptr(), static.data_ptr(), 3,
-                                           feats.data_ptr(), ld, st), "pack")
-  img_a = torch.zeros(lib.gcb_a_image_bytes(n_nodes, ld), dtype=torch.uint8, device=dev)
-  img_b = torch.zeros_like(img_a)
-  _native.check(lib.gcb_pack_grid_image(planes.data_ptr(), n_ch, n_nodes, mean.data_ptr(),
-                                        scale.data_ptr(), static.data_ptr(), 3, ld,
-                                        img_a.data_ptr(), st), "pack_image")
-  _native.check(lib.gcb_rows_to_image(feats.data_ptr(), ld, 1, n_nodes, ld, img_b.data_ptr(), st), "to_image")
-  assert torch.equal(img_a, img_b)
-
-  y = torch.randn(n_nodes, 256, device=dev)
-  oscale, ooff = torch.rand(n_out, device=dev) + 0.5, torch.randn(n_out, device=dev)
-  add_idx = torch.arange(n_out, dtype=torch.int32, device=dev) + 3
-  add_idx[4] = -1
-  out = torch.full((n_out, n_nodes), float("nan"), device=dev)
-  _native.check(lib.gcb_unpack_grid_outputs(y.data_ptr(), 256, n_out, n_nodes, oscale.data_ptr(),
-                                            ooff.data_ptr(), planes.data_ptr(), add_idx.data_ptr(),
-                                            out.data_ptr(), st), "unpack")
-  want = y[:, :n_out].t() * oscale[:, None] + ooff[:, None]
-  add = planes[(add_idx.clamp(min=0)).long()] * (add_idx >= 0)[:, None]
-  torch.testing.assert_close(out, want + add, rtol=1e-6, atol=1e-6)
-  _native.check(lib.gcb_unpack_grid_outputs(y.data_ptr(), 256, n_out, n_nodes, None, None, None,
-                                            None, out.data_ptr(), st), "unpack")
-  assert torch.equal(out, y[:, :n_out].t().contiguous())
 
 
 def test_halo_row_packing_fp32_rows_and_image_rows():

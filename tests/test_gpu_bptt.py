@@ -1,6 +1,7 @@
-"""Backprop through time on the device: the feedback-seed and input-gradient kernels against PyTorch,
-the engine's input gradient against torch autograd of the fp64 oracle, and the multi-step gradient of
-autoregressive.Predictor.loss_and_grads against an independent autograd unroll of the oracle."""
+"""Backprop through time on the device: the engine's input gradient against torch autograd of the fp64
+oracle, and the multi-step gradient of autoregressive.Predictor.loss_and_grads against an independent
+autograd unroll of the oracle.  The feedback-seed and input-gradient kernels are checked against fp64
+in test_gpu_grid_io_kernels.py."""
 import gc
 
 import numpy as np
@@ -26,105 +27,6 @@ def _st():
 
 def _i32(a):
   return torch.as_tensor(np.asarray(a, np.int32)).to(DEV)
-
-
-# ---- kernels ---------------------------------------------------------------------------------------
-def test_feedback_seed_kernel_against_fp64_formula():
-  lib = _native.lib()
-  gen = torch.Generator(device=DEV).manual_seed(11)
-  rng = np.random.default_rng(11)
-  lat = np.linspace(-90, 90, 19)
-  n_lat, n_lon, n_out, n_planes, n_next, n_rows = len(lat), 37, 45, 60, 50, 70
-  n_nodes = n_lat * n_lon
-  w = torch.as_tensor(_lat_weight(lat)).to(DEV)
-  y = torch.randn(n_nodes, 256, generator=gen, device=DEV)
-  targets = torch.randn(n_out, n_nodes, generator=gen, device=DEV)
-  add = torch.randn(n_planes, n_nodes, generator=gen, device=DEV)
-  scale = torch.rand(n_out, generator=gen, device=DEV) + 0.5
-  offset = torch.randn(n_out, generator=gen, device=DEV)
-  idx = torch.arange(n_out, dtype=torch.int32, device=DEV) + 7
-  idx[::3] = -1
-  coef = torch.rand(n_out, generator=gen, device=DEV, dtype=torch.float64)
-  a_next = torch.randn(n_next, n_nodes, generator=gen, device=DEV)
-  dpred = rng.integers(0, n_next, n_out)
-  dpred[::4] = -1
-  resid = rng.integers(0, n_out, n_rows)
-  resid[::3] = -1
-  carry = rng.integers(0, n_next, n_rows)
-  carry[::5] = -1
-  dpred_d, resid_d, carry_d = _i32(dpred), _i32(resid), _i32(carry)
-
-  def run(with_next):
-    g = torch.zeros(n_nodes, 256, device=DEV)
-    a_out = torch.full((n_rows, n_nodes), float("nan"), device=DEV)
-    _native.check(lib.gcb_output_loss_grad_feedback(
-        y.data_ptr(), 256, n_out, n_lat, n_lon, scale.data_ptr(), offset.data_ptr(), add.data_ptr(),
-        idx.data_ptr(), targets.data_ptr(), w.data_ptr(), coef.data_ptr(),
-        a_next.data_ptr() if with_next else None, dpred_d.data_ptr(), n_rows, resid_d.data_ptr(),
-        carry_d.data_ptr(), a_out.data_ptr(), g.data_ptr(), 256, _st()), "feedback")
-    return g, a_out
-
-  g, a_out = run(True)
-  a = add[idx.clamp(min=0).long()] * (idx >= 0)[:, None]
-  t_norm = ((targets - a) - offset[:, None]) / scale[:, None]
-  wn = w.double().repeat_interleave(n_lon)
-  g_loss = coef[None] * wn[:, None] * (y[:, :n_out] - t_norm.t()).double()        # [nodes, n_out]
-  dp = torch.where(torch.as_tensor(dpred >= 0, device=DEV)[None],
-                   a_next.double()[torch.as_tensor(np.maximum(dpred, 0), device=DEV)].t(), 0.0)
-  want_g = g_loss + scale.double()[None] * dp
-  assert _frob(g[:, :n_out], want_g) <= 1e-6
-  assert torch.all(g[:, n_out:] == 0)
-  want_a = torch.zeros(n_rows, n_nodes, dtype=torch.float64, device=DEV)
-  for r in range(n_rows):
-    c = resid[r]
-    if c >= 0:
-      want_a[r] = g_loss[:, c] / scale[c].double() + dp[:, c]
-    if carry[r] >= 0:
-      want_a[r] += a_next[carry[r]].double()
-  assert _frob(a_out, want_a) <= 1e-6
-  assert torch.equal(a_out[torch.as_tensor((resid < 0) & (carry < 0), device=DEV)],
-                     torch.zeros_like(a_out[torch.as_tensor((resid < 0) & (carry < 0), device=DEV)]))
-  g2, a2 = run(True)
-  assert torch.equal(g, g2) and torch.equal(a_out, a2)
-  # without the following step: g is gcb_output_loss_grad bit for bit
-  g_plain = torch.zeros(n_nodes, 256, device=DEV)
-  _native.check(lib.gcb_output_loss_grad(
-      y.data_ptr(), 256, n_out, n_lat, n_lon, scale.data_ptr(), offset.data_ptr(), add.data_ptr(),
-      idx.data_ptr(), targets.data_ptr(), w.data_ptr(), coef.data_ptr(), g_plain.data_ptr(), 256,
-      _st()), "g")
-  g_null, a_null = run(False)
-  assert torch.equal(g_null, g_plain)
-  want_null = torch.zeros_like(want_a)
-  for r in range(n_rows):
-    if resid[r] >= 0:
-      want_null[r] = g_loss[:, resid[r]] / scale[resid[r]].double()
-  assert _frob(a_null, want_null) <= 1e-6
-
-
-@pytest.mark.parametrize("with_scale", [True, False])
-def test_input_grad_kernel_is_the_same_order_expression(with_scale):
-  lib = _native.lib()
-  gen = torch.Generator(device=DEV).manual_seed(12)
-  n_nodes, ld, n_ch = 19 * 37 + 5, 64, 50
-  dx = torch.randn(n_nodes, ld, generator=gen, device=DEV)
-  ch = np.random.default_rng(12).integers(0, n_ch, 77)
-  ch_d = _i32(ch)
-  scale = torch.rand(n_ch, generator=gen, device=DEV) + 0.3
-  base = torch.randn(len(ch), n_nodes, generator=gen, device=DEV)
-  sel = dx[:, torch.as_tensor(ch, device=DEV)].t()
-  term = sel / scale[torch.as_tensor(ch, device=DEV)][:, None] if with_scale else sel
-
-  def run(acc):
-    a = base.clone() if acc else torch.full_like(base, float("nan"))
-    _native.check(lib.gcb_input_grad(dx.data_ptr(), ld, n_nodes, len(ch), ch_d.data_ptr(),
-                                      scale.data_ptr() if with_scale else None, a.data_ptr(), acc,
-                                      _st()), "gcb_input_grad")
-    return a
-
-  assert torch.equal(run(0), term)
-  got = run(1)
-  assert torch.equal(got, base + term)
-  assert torch.equal(got, run(1))
 
 
 # ---- the engine's input gradient ---------------------------------------------------------------------

@@ -160,32 +160,6 @@ def test_sender_segment_sum_and_gather_add():
   assert torch.equal(dst, add + src[idx.long()])
 
 
-def test_output_loss_grad_against_formula():
-  lib = _native.lib()
-  gen = torch.Generator(device=DEV).manual_seed(4)
-  lat = np.linspace(-90, 90, 19)
-  n_lat, n_lon, n_out, n_planes = len(lat), 37, 45, 60
-  n_nodes = n_lat * n_lon
-  w = torch.as_tensor(_lat_weight(lat)).to(DEV)
-  y = torch.randn(n_nodes, 256, generator=gen, device=DEV)
-  targets = torch.randn(n_out, n_nodes, generator=gen, device=DEV)
-  add = torch.randn(n_planes, n_nodes, generator=gen, device=DEV)
-  scale = torch.rand(n_out, generator=gen, device=DEV) + 0.5
-  offset = torch.randn(n_out, generator=gen, device=DEV)
-  idx = torch.arange(n_out, dtype=torch.int32, device=DEV) + 7
-  idx[::3] = -1
-  coef = torch.rand(n_out, generator=gen, device=DEV, dtype=torch.float64)
-  g = torch.zeros(n_nodes, 256, device=DEV)
-  _native.check(lib.gcb_output_loss_grad(
-      y.data_ptr(), 256, n_out, n_lat, n_lon, scale.data_ptr(), offset.data_ptr(), add.data_ptr(),
-      idx.data_ptr(), targets.data_ptr(), w.data_ptr(), coef.data_ptr(), g.data_ptr(), 256, _st()), "g")
-  a = add[idx.clamp(min=0).long()] * (idx >= 0)[:, None]
-  t_norm = ((targets - a) - offset[:, None]) / scale[:, None]
-  want = coef[None] * w.double().repeat_interleave(n_lon)[:, None] * (y[:, :n_out] - t_norm.t()).double()
-  assert _frob(g[:, :n_out], want) <= 1e-6
-  assert torch.all(g[:, n_out:] == 0)
-
-
 # ---- the whole step -------------------------------------------------------------------------------
 class _GradOracle(oracle_gnn.Oracle):
   """The oracle with its stage outputs kept as tensors, so that autograd sees the whole step."""

@@ -1,7 +1,8 @@
 """Gradients with respect to the inputs and forcings on the device (loss_and_input_grads, input_vjp):
-the two new kernels against fp64 torch, every variable's gradient against torch autograd of an fp64
-oracle unroll that differentiates the inputs and forcings, the bit-identity of the parameter-free
-backward pass, and, at full size, variable by variable central differences of the device loss."""
+every variable's gradient against torch autograd of an fp64 oracle unroll that differentiates the
+inputs and forcings, the bit-identity of the parameter-free backward pass, and, at full size, variable
+by variable central differences of the device loss.  The seed and broadcast-sum kernels are checked
+against fp64 in test_gpu_grid_io_kernels.py."""
 import gc
 
 import numpy as np
@@ -26,80 +27,6 @@ def _st():
 
 def _i32(a):
   return torch.as_tensor(np.asarray(a, np.int32)).to(DEV)
-
-
-# ---- kernels -----------------------------------------------------------------------------------------
-@pytest.mark.parametrize("with_scale", [True, False])
-def test_cotangent_seed_kernel_against_fp64(with_scale):
-  lib = _native.lib()
-  gen = torch.Generator(device=DEV).manual_seed(21)
-  rng = np.random.default_rng(21)
-  n_out, n_nodes, n_next, n_rows = 45, 19 * 37 + 3, 50, 70
-  cot = torch.randn(n_out, n_nodes, generator=gen, device=DEV)
-  scale = torch.rand(n_out, generator=gen, device=DEV) + 0.5
-  a_next = torch.randn(n_next, n_nodes, generator=gen, device=DEV)
-  dpred = rng.integers(0, n_next, n_out)
-  dpred[::4] = -1
-  resid = rng.integers(0, n_out, n_rows)
-  resid[::3] = -1
-  carry = rng.integers(0, n_next, n_rows)
-  carry[::5] = -1
-  dpred_d, resid_d, carry_d = _i32(dpred), _i32(resid), _i32(carry)
-
-  def run(with_next):
-    g = torch.zeros(n_nodes, 256, device=DEV)
-    a_out = torch.full((n_rows, n_nodes), float("nan"), device=DEV)
-    _native.check(lib.gcb_output_cotangent_grad_feedback(
-        n_out, n_nodes, scale.data_ptr() if with_scale else None, cot.data_ptr(),
-        a_next.data_ptr() if with_next else None, dpred_d.data_ptr(), n_rows, resid_d.data_ptr(),
-        carry_d.data_ptr(), a_out.data_ptr(), g.data_ptr(), 256, _st()), "cotangent seed")
-    return g, a_out
-
-  for with_next in (True, False):
-    g, a_out = run(with_next)
-    dp = torch.zeros(n_out, n_nodes, dtype=torch.float64, device=DEV)
-    if with_next:
-      fed = torch.as_tensor(dpred >= 0, device=DEV)
-      dp[fed] = a_next.double()[torch.as_tensor(dpred[dpred >= 0], device=DEV)]
-    d = cot.double() + dp
-    sc = scale.double() if with_scale else torch.ones(n_out, dtype=torch.float64, device=DEV)
-    assert _frob(g[:, :n_out], (sc[:, None] * d).t()) <= 1e-7
-    assert torch.all(g[:, n_out:] == 0)
-    want = torch.zeros(n_rows, n_nodes, dtype=torch.float64, device=DEV)
-    for r in range(n_rows):
-      if resid[r] >= 0:
-        want[r] = d[resid[r]]
-      if with_next and carry[r] >= 0:
-        want[r] += a_next[carry[r]].double()
-    assert _frob(a_out, want) <= 1e-7
-    g2, a2 = run(with_next)
-    assert torch.equal(g, g2) and torch.equal(a_out, a2)
-
-
-@pytest.mark.parametrize("mode", [_native.BCAST_NONE, _native.BCAST_LAT, _native.BCAST_LAT_LON])
-def test_broadcast_grad_sum_kernel_against_fp64(mode):
-  lib = _native.lib()
-  gen = torch.Generator(device=DEV).manual_seed(22)
-  n_lat, n_lon, n_planes = 181, 360, 9
-  a = torch.randn(n_planes, n_lat * n_lon, generator=gen, device=DEV)
-  rows = [7, 0, 3, 3]
-  rows_d = _i32(rows)
-  width = (n_lat * n_lon, n_lon, 1)[mode]
-  base = torch.randn(len(rows), width, generator=gen, device=DEV)
-  x = a.double()[torch.as_tensor(rows, device=DEV)].reshape(len(rows), n_lat, n_lon)
-  want = x.reshape(len(rows), -1) if mode == 0 else (x.sum(1) if mode == 1 else x.sum((1, 2))[:, None])
-
-  def run(acc):
-    out = base.clone() if acc else torch.full_like(base, float("nan"))
-    _native.check(lib.gcb_broadcast_grad_sum(a.data_ptr(), n_lat, n_lon, len(rows), rows_d.data_ptr(),
-                                             mode, out.data_ptr(), acc, _st()), "broadcast sum")
-    return out
-
-  got = run(0)
-  assert torch.equal(got, want.float())                 # fp64 sum, one rounding
-  acc = run(1)
-  assert torch.equal(acc, (base.double() + want).float())
-  assert torch.equal(run(1), acc) and torch.equal(run(0), got)
 
 
 # ---- against torch autograd of the fp64 oracle unroll --------------------------------------------------

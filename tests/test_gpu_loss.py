@@ -1,5 +1,5 @@
-"""The forecast loss on the device: gcb_output_loss against fp64 PyTorch, and GraphCast.loss /
-loss_and_predictions, InputsAndResiduals and the autoregressive loss against the host mirror of the
+"""The forecast loss on the device: the argument checks of gcb_output_loss (its arithmetic is checked
+against fp64 in test_gpu_grid_io_kernels.py), and GraphCast.loss / loss_and_predictions, InputsAndResiduals and the autoregressive loss against the host mirror of the
 reference's losses (graphcast_b200.losses, itself pinned to the executed reference in
 tests/test_reference_losses_golden.py)."""
 import numpy as np
@@ -19,71 +19,6 @@ DEV = torch.device("cuda:0")
 def _lat_weight(lat):
   da = xs.DataArray(np.zeros(len(lat), np.float32), ("lat",), coords={"lat": lat})
   return losses.normalized_latitude_weights(da).astype(np.float32)
-
-
-def _loss(lib, y, n_out, n_lat, n_lon, targets, w, *, scale=None, offset=None, add=None, idx=None,
-          planes_out=None):
-  ptr = lambda t: None if t is None else t.data_ptr()
-  nbytes = lib.gcb_output_loss_workspace_bytes(n_out)
-  ws = torch.empty(nbytes, dtype=torch.uint8, device=DEV)
-  sums = torch.full((n_out,), float("nan"), dtype=torch.float64, device=DEV)
-  _native.check(lib.gcb_output_loss(
-      y.data_ptr(), y.shape[1], n_out, n_lat, n_lon, ptr(scale), ptr(offset), ptr(add), ptr(idx),
-      targets.data_ptr(), w.data_ptr(), ptr(planes_out), ws.data_ptr(), nbytes, sums.data_ptr(),
-      torch.cuda.current_stream().cuda_stream), "gcb_output_loss")
-  return sums
-
-
-@pytest.mark.parametrize("lat", [np.linspace(-90, 90, 19), np.arange(-85.0, 90.0, 10.0)],
-                         ids=["poles", "no_poles"])
-def test_output_loss_kernel_against_fp64(lat):
-  lib = _native.lib()
-  g = torch.Generator(device=DEV).manual_seed(3)
-  n_lat, n_lon, n_out, n_planes = len(lat), 37, 45, 60     # nodes and channels off the 32-tiles
-  n_nodes = n_lat * n_lon
-  assert n_nodes % 32 and n_out % 32
-  w = torch.as_tensor(_lat_weight(lat)).to(DEV)
-  y = torch.randn(n_nodes, 256, generator=g, device=DEV)
-  targets = torch.randn(n_out, n_nodes, generator=g, device=DEV) * 3 + 1
-  add = torch.randn(n_planes, n_nodes, generator=g, device=DEV)
-  scale = torch.rand(n_out, generator=g, device=DEV) + 0.5
-  offset = torch.randn(n_out, generator=g, device=DEV)
-  idx = torch.arange(n_out, dtype=torch.int32, device=DEV) + 7
-  idx[::3] = -1                                              # targets that are not inputs
-  offset[idx >= 0] = 0                                       # residual targets: (t - last) / dstd
-  affine = dict(scale=scale, offset=offset, add=add, idx=idx)
-
-  def want(affine_on):
-    t = targets
-    if affine_on:
-      a = add[idx.clamp(min=0).long()] * (idx >= 0)[:, None]
-      t = ((targets - a) - offset[:, None]) / scale[:, None]
-    d = (y[:, :n_out].t() - t).double()
-    return (w.double().repeat_interleave(n_lon)[None] * d * d).sum(1)
-
-  for on in (True, False):
-    got = _loss(lib, y, n_out, n_lat, n_lon, targets, w, **(affine if on else {}))
-    ref = want(on)
-    assert float(((got - ref).abs() / ref.abs()).max()) <= 1e-12
-    again = _loss(lib, y, n_out, n_lat, n_lon, targets, w, **(affine if on else {}))
-    assert torch.equal(got, again)                           # deterministic, bit for bit
-
-  # the predictions written on the way equal gcb_unpack_grid_outputs bit for bit
-  po = torch.full((n_out, n_nodes), float("nan"), device=DEV)
-  with_po = _loss(lib, y, n_out, n_lat, n_lon, targets, w, planes_out=po, **affine)
-  unpacked = torch.full_like(po, float("nan"))
-  _native.check(lib.gcb_unpack_grid_outputs(y.data_ptr(), 256, n_out, n_nodes, scale.data_ptr(),
-                                            offset.data_ptr(), add.data_ptr(), idx.data_ptr(),
-                                            unpacked.data_ptr(),
-                                            torch.cuda.current_stream().cuda_stream), "unpack")
-  assert torch.equal(po, unpacked)
-  assert torch.equal(with_po, _loss(lib, y, n_out, n_lat, n_lon, targets, w, **affine))
-
-  # a NaN target makes exactly its channel NaN (skipna=False)
-  bad = targets.clone()
-  bad[7, 100] = float("nan")
-  s = _loss(lib, y, n_out, n_lat, n_lon, bad, w, **affine)
-  assert torch.isnan(s[7]) and torch.isfinite(torch.cat([s[:7], s[8:]])).all()
 
 
 def test_output_loss_argument_checks():

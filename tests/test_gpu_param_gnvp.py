@@ -1,5 +1,5 @@
 """Gauss-Newton products of the forecast loss with respect to the parameters on the device
-(loss_and_param_gnvp): the seed kernel against gcb_output_loss_grad, G v against the fp64 oracle
+(loss_and_param_gnvp): G v against the fp64 oracle
 (forward-mode J v, then reverse mode through the loss Hessian), the exact identities (symmetry, the
 quadratic form, linearity, zero tangents, the loss of loss()), and the full-Hessian limit where the
 predictions equal the targets."""
@@ -22,28 +22,6 @@ DEV = torch.device("cuda:0")
 
 def _st():
   return torch.cuda.current_stream().cuda_stream
-
-
-# ---- seed kernel -----------------------------------------------------------------------------------------
-@pytest.mark.parametrize("n_lat,n_lon,n_out,ld", [(1, 1, 1, 1), (19, 36, 83, 256), (181, 360, 227, 256)])
-def test_gn_seed_is_the_loss_seed_with_zero_targets(n_lat, n_lon, n_out, ld):
-  lib = _native.lib()
-  gen = torch.Generator(device=DEV).manual_seed(n_out)
-  ng = n_lat * n_lon
-  dy = torch.randn(ng, ld, generator=gen, device=DEV)
-  dy[0, 0] = -0.0
-  lat = torch.rand(n_lat, generator=gen, device=DEV) + 0.1
-  coef = torch.rand(n_out, generator=gen, device=DEV, dtype=torch.float64)
-  zeros = torch.zeros(n_out, ng, device=DEV)
-  want = torch.full((ng, ld), float("nan"), device=DEV)
-  got = torch.full((ng, ld), float("nan"), device=DEV)
-  _native.check(lib.gcb_output_loss_grad(dy.data_ptr(), ld, n_out, n_lat, n_lon, None, None, None,
-                                         None, zeros.data_ptr(), lat.data_ptr(), coef.data_ptr(),
-                                         want.data_ptr(), ld, _st()), "gcb_output_loss_grad")
-  _native.check(lib.gcb_output_loss_gn_seed(dy.data_ptr(), ld, n_out, n_lat, n_lon, lat.data_ptr(),
-                                            coef.data_ptr(), got.data_ptr(), ld, _st()),
-                "gcb_output_loss_gn_seed")
-  assert torch.equal(got.view(torch.int32), want.view(torch.int32))   # bits, NaN columns included
 
 
 # ---- against the fp64 oracle -----------------------------------------------------------------------------
