@@ -554,6 +554,18 @@ class Predictor(graphcast.Predictor):
                                 "are not provided)")
     return self._predictor.loss_and_param_hvp(inputs, targets, forcings, param_tangents, **kwargs)
 
+  def loss_and_joint_hvp(self, inputs, targets, forcings, param_tangents=None, input_tangents=None,
+                         forcing_tangents=None, **kwargs):
+    """(loss, diagnostics, grads, input_grads, forcing_grads, param_hvp, input_hvp, forcing_hvp) of one
+    target time (GraphCast.loss_and_joint_hvp), delegated to the inner predictor; joint Hessian-vector
+    products over several target times are not provided, with or without gradient_checkpointing."""
+    targets = xs.from_xarray(targets)
+    if targets.sizes["time"] != 1:
+      raise NotImplementedError("joint Hessian-vector products cover one target time (several are "
+                                "not provided)")
+    return self._predictor.loss_and_joint_hvp(inputs, targets, forcings, param_tangents,
+                                              input_tangents, forcing_tangents, **kwargs)
+
   def _tangent_rollout(self, inputs, targets_template, forcings, input_tangents, forcing_tangents,
                        directions: bool, param_tangents=None):
     """input_jvp (batched_input_jvp with `directions`, param_jvp with `param_tangents`) over several

@@ -32,7 +32,9 @@ gradient state like the tangent's, runs every dX product once over all direction
 the two nonlinearities with gcb_layernorm_backward_dirs and gcb_swish_jvp.
 A parameter Hessian-vector product (loss_and_param_hvp) joins the two: the tangent along weight tangents keeps
 its snapshots, and the two-direction walk element(hvp=..., param_grads=True) accumulates the gradient and its
-tangent, with every layer's weight-tangent terms (mlp_backward, dx, wgrad_dot).
+tangent, with every layer's weight-tangent terms (mlp_backward, dx, wgrad_dot).  A joint one in the
+parameters and the inputs (loss_and_joint_hvp) runs that walk along an input tangent as well, and also
+forms the input gradient and its tangent, with the grid embedder's two coupling terms.
 
 All arithmetic is in libgraphcast_b200.so; this module only sequences the launches and owns the
 buffers.  Allocation is lazy: nothing here exists until the first loss_and_grads call.
@@ -265,11 +267,13 @@ class Backward:
       out[info.stem] = wt
     return out
 
-  def pack_transposed_tangents(self, wts: Dict[str, _WeightTangent]) -> None:
+  def pack_transposed_tangents(self, wts: Dict[str, _WeightTangent], input_grad: bool = False) -> None:
     """The transposed images of packed parameter tangents (weight_tangents), packed on the device as
     _pack_transposed packs the primal ones: W1-dot^T and W0-dot^T per 512-row block (for a pre-gathered
     edge layer: we, ws, wr), so that a parameter Hessian-vector product's dX products can add their
-    dY W-dot^T terms.  Layers without a tangent get none."""
+    dY W-dot^T terms.  Layers without a tangent get none.  input_grad (a joint Hessian-vector product,
+    whose walk also forms the input gradient): the grid embedder's W0-dot^T in input_transposed's
+    [512, n] layout too (w0_in), when that layer has a tangent."""
     for info in self._all:
       wt = wts.get(info.stem)
       if wt is None:
@@ -283,6 +287,9 @@ class Backward:
             self._pack_t(wt, f"w0_{s}", wt.w0_f32.data_ptr() + 4 * s * D * D, D, D, D, D)
         elif k0 == D:
           self._pack_t(wt, "w0_0", wt.w0_f32.data_ptr(), D, D, D, D)
+        if input_grad and info is self.mlps["enc_grid"]:
+          _, n = self.input_transposed()
+          self._pack_t(wt, "w0_in", wt.w0_f32.data_ptr(), D, D, n, self.eng.c_in_pad)
 
   def repack(self, stems=None) -> None:
     """The engine's weights were rewritten (Engine.load_params / load_params_device): repacks the
@@ -559,13 +566,15 @@ class Backward:
         t.data_ptr(), t.shape[1], None, 0, None, rows, n, None, 0, ws.data_ptr(), ws.numel(),
         out.data_ptr(), None, None, 1, self._st()), "gcb_layernorm_backward")
 
-  def add_dot_product(self, rows: int, src: torch.Tensor, img, out: torch.Tensor, k: int = D) -> None:
-    """A parameter HVP's dX product: direction 1 of the stacked out (= src W^T over both directions)
-    += direction 0 of src times the transposed tangent image img (dY W-dot^T), through one GEMM with
-    that direction as an identity addend."""
+  def add_dot_product(self, rows: int, src: torch.Tensor, img, out: torch.Tensor, k: int = D,
+                      n: int = D) -> None:
+    """A parameter HVP's dX product: direction 1 of the stacked out (= src W^T over both directions,
+    n columns) += direction 0 of src times the transposed tangent image img (dY W-dot^T), through one
+    GEMM with that direction as an identity addend."""
     s = self.dir_stride(rows)
-    t = self.empty(rows)
-    self.layer(rows, [self.tab(src, k)], img, self.zero_bias, out_y=t, pre=[(out[s:s + rows], None)])
+    t = self.empty(rows, n)
+    self.layer(rows, [self.tab(src, k)], img, self.zero_bias, out_y=t, pre=[(out[s:s + rows], None)],
+               n=n)
     out[s:s + rows].copy_(t)
 
   def dx(self, info: _MlpInfo, key: str, rows: int, src: torch.Tensor,
@@ -762,7 +771,14 @@ class Backward:
     walk) and their tangents into info.gt (see mlp_backward), runs the parts that only the parameters
     need on both directions (the edge embedders, the mesh-node encoder, the first step's de product), and
     adds every weight tangent's terms: h-dot and z-dot get X W-dot + b-dot, every dX product of a layer
-    with a tangent dY_0 W-dot^T, and the node projections of the edge layers v W-dot."""
+    with a tangent dY_0 W-dot^T, and the node projections of the edge layers v W-dot.  The input
+    tangent is taken to be zero, and the grid embedder's dW0-dot has no X-dot^T dh term.
+
+    That walk with dgrid_in (a joint Hessian-vector product in the parameters and the inputs,
+    loss_and_joint_hvp): the tangent ran along the parameter tangents and a non-zero input tangent, so
+    the grid embedder's dW0-dot also gets X-dot^T dh (X-dot the packed input tangent of the snapshots),
+    and direction 1 of dx also gets dh_0 W0-dot^T (pack_transposed_tangents(input_grad=True)).  Direction
+    0 of dx is bit for bit what param_grads=False gives."""
     phvp = hvp is not None and param_grads
     if phvp:
       if dirs != 2:
@@ -891,14 +907,22 @@ class Backward:
     dvg0 = self.dx(info, "w0_1", ng, S, residual=dvg0)
     dvm0 = self.dx(info, "w0_2", nm, R, residual=dvm0)
     del S, R, vg0, vm0
-    dh = self.mlp_backward(mp["enc_grid"], ng, [grid_in], dvg0,   # (a parameter HVP: zero input tangent)
-                           tan=None if T is None else ([img(T.pop("grid_in"), eng.c_in_pad)], (), None),
-                           xdot=[None])
+    # A parameter HVP has a zero input tangent; a joint one (phvp with dgrid_in) has one, whose
+    # X-dot^T dh the grid embedder's weight-gradient tangent takes.
+    joint = self.phvp and dgrid_in
+    gin_t = None if T is None else img(T.pop("grid_in"), eng.c_in_pad)
+    dh = self.mlp_backward(mp["enc_grid"], ng, [grid_in], dvg0,
+                           tan=None if T is None else ([gin_t], (), None),
+                           xdot=[gin_t if joint else None])
+    del gin_t
     dx = None
     if dgrid_in:
       w0t, n = self.input_transposed()
       dx = self.empty(rk(ng), n)
       self.layer(rk(ng), [tab(dh)], w0t, self.zero_bias, out_y=dx, n=n)
+      wt = self.wts.get(mp["enc_grid"].stem)
+      if joint and wt is not None and "w0_in" in wt.t:    # direction 1 += dh_0 W0-dot^T
+        self.add_dot_product(ng, dh, wt.t["w0_in"], dx, n=n)
     del dh, dvg0
     if self.param_grads:
       self.mlp_backward(mp["enc_mesh"], nm, [mesh_in], dvm0)

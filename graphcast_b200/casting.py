@@ -107,3 +107,8 @@ class Bfloat16Cast(graphcast.Predictor):
 
   def loss_and_param_hvp(self, inputs, targets, forcings, param_tangents, **kwargs):
     return self._predictor.loss_and_param_hvp(inputs, targets, forcings, param_tangents, **kwargs)
+
+  def loss_and_joint_hvp(self, inputs, targets, forcings, param_tangents=None, input_tangents=None,
+                         forcing_tangents=None, **kwargs):
+    return self._predictor.loss_and_joint_hvp(inputs, targets, forcings, param_tangents,
+                                              input_tangents, forcing_tangents, **kwargs)

@@ -1109,12 +1109,14 @@ class Engine:
 
   # -- parameter tangents (param_jvp, loss_and_param_gnvp) ---------------------------------------------
   def weight_tangents(self, param_tangents: Mapping[str, Mapping[str, np.ndarray]],
-                      transposed: bool = False):
+                      transposed: bool = False, input_grad: bool = False):
     """Packs parameter tangents (host float32 arrays keyed and shaped like the params, modules and
     fields optional) into tangent weight images on the device (Backward.weight_tangents), for
     input_jvp_element, param_gnvp_element and (with `transposed`: also their transposed images,
-    Backward.pack_transposed_tangents) param_hvp_element; call input_grads_begin() or grads_begin()
-    first.  The engine's weights and weights_version are not touched."""
+    Backward.pack_transposed_tangents) param_hvp_element; with `input_grad` as well, the grid
+    embedder's transposed image of the input gradient, for joint_hvp_element.  Call
+    input_grads_begin() or grads_begin() first.  The engine's weights and weights_version are not
+    touched."""
     if self._backward is None:
       raise RuntimeError("call input_grads_begin() or grads_begin() first")
     with self._on_device():
@@ -1122,7 +1124,7 @@ class Engine:
                     for f, a in fields.items()} for name, fields in param_tangents.items()}
       wts = self._backward.weight_tangents(dev)
       if transposed:
-        self._backward.pack_transposed_tangents(wts)
+        self._backward.pack_transposed_tangents(wts, input_grad=input_grad)
       return wts
 
   def param_gnvp_element(self, targets_planes: torch.Tensor, lat_weight: torch.Tensor,
@@ -1195,9 +1197,70 @@ class Engine:
       bw.element(grid_in, g_out, snaps, dirs=2, hvp=tsnaps, wts=weight_tangents)
 
   def param_hvp(self):
-    """The accumulated Hessian-vector products of param_hvp_element: device fp32 tensors keyed and
-    shaped like the params, zeros for the parameters the step never reads."""
+    """The accumulated Hessian-vector products of param_hvp_element (or the parameter side of
+    joint_hvp_element's): device fp32 tensors keyed and shaped like the params, zeros for the
+    parameters the step never reads."""
     return self._backward.grads(tangent=True)
+
+  # -- joint Hessian-vector products (loss_and_joint_hvp) ----------------------------------------------
+  def joint_hvp_element(self, fb: "Feedback", operands: dict, *, lat_weight: torch.Tensor,
+                        coef: torch.Tensor, weight_tangents, channel_sums: torch.Tensor,
+                        zero_targets: Optional[torch.Tensor] = None) -> None:
+    """One batch element of a Hessian-vector product of the loss jointly in the parameters and the
+    inputs (call param_hvp_begin() first, then build fb; weight_tangents from weight_tangents(...,
+    transposed=True, input_grad=True)).  operands: "targets_planes", "tangent_planes" [c_in, Ng] (the
+    input tangent v_x, physical units) and the affine keywords of output_loss.  Afterwards fb.a is
+    [2, fb.n_rows, Ng]: direction 0 the gradient with respect to the input planes, direction 1 its
+    derivative along (v_theta, v_x); the parameter gradients and their derivatives are ADDED to the
+    accumulators of grads() and param_hvp().  zero_targets as in input_hvp_element.
+
+    The step runs from the packed grid_in_img with its tangent along the parameter tangents and v_x,
+    packed as input_hvp_element packs it (Backward.tangent(wts=..., snaps=..., tsnaps=...)); the loss
+    sums of that forward go to channel_sums.  Direction 0 of the seed is input_grads_element's loss
+    seed with no following step.  The seed is affine in (y, the add planes, fb.a) and the parameters
+    reach it only through y, so direction 1 is the same kernel on y-dot, add_planes = v_x, zero targets
+    and no offset, as input_hvp_element seeds its tangent.  One coupled walk
+    (Backward.element(dirs=2, hvp=..., param_grads=True, dgrid_in=True)) then forms both sides, and
+    gcb_input_grad runs per direction.  The loss sums, the parameter gradients and direction 0 are bit
+    for bit those of loss_and_grads_element and input_grads_element."""
+    if self._backward is None:
+      raise RuntimeError("call param_hvp_begin() first")
+    bw = self._backward
+    affine = {k: operands[k] for k in ("scale", "offset", "add_planes", "add_plane_index")
+              if k in operands}
+    targets_planes, tangent = operands["targets_planes"], operands["tangent_planes"]
+    operands.clear()
+    if (tuple(tangent.shape) != (self.c_in, self.num_grid) or tangent.dtype != torch.float32
+        or not tangent.is_contiguous()):
+      raise ValueError(f"tangent_planes must be a contiguous float32 [{self.c_in}, {self.num_grid}] "
+                       "tensor")
+    grid_in = self.grid_in_img
+    stride = bw.dir_stride(self.num_grid)
+    add_index = affine.get("add_plane_index")
+    with self._on_device():
+      dgrid_in = self._pack_tangents([tangent], fb.in_scale, stride)
+      snaps, tsnaps = {}, {}
+      dy = bw.tangent(grid_in, dgrid_in, snaps=snaps, tsnaps=tsnaps, wts=weight_tangents)
+      del dgrid_in
+      self.output_loss(targets_planes, lat_weight, channel_sums=channel_sums, **affine)
+      g_out = torch.zeros([stride + self.num_grid, 256], dtype=torch.float32, device=self.device)
+      a_out = torch.empty([2, fb.n_rows, self.num_grid], dtype=torch.float32, device=self.device)
+      if zero_targets is None:
+        zero_targets = torch.zeros([self.n_out, self.num_grid], dtype=torch.float32,
+                                   device=self.device)
+      self._loss_seed(self.grid_out, targets_planes, lat_weight, coef, g_out, affine, fb=fb,
+                      a_out=a_out[0], n_rows=fb.n_rows)
+      self._loss_seed(dy, zero_targets, lat_weight, coef, g_out[stride:],
+                      dict(scale=affine.get("scale"), add_plane_index=add_index,
+                           add_planes=None if add_index is None else tangent),
+                      fb=fb, a_out=a_out[1], n_rows=fb.n_rows)
+      # the planes, targets and tangents are consumed: release them
+      fb.a = a_out
+      del dy, zero_targets
+      affine = targets_planes = tangent = None
+      dx = bw.element(grid_in, g_out, snaps, dgrid_in=True, dirs=2, hvp=tsnaps, wts=weight_tangents)
+      del g_out, snaps, tsnaps
+      self._input_grad_tail(dx, fb, a_out.unbind(0), stride)
 
   def broadcast_grad_sum(self, a: torch.Tensor, n_lat: int, rows: torch.Tensor, mode: int,
                          out: torch.Tensor, accumulate: bool) -> None:

@@ -174,6 +174,16 @@ class Predictor(abc.ABC):
     `param_tangents`, a dict shaped like the params."""
     raise NotImplementedError(f"{type(self).__name__} does not implement parameter tangents")
 
+  def loss_and_joint_hvp(self, inputs, targets, forcings, param_tangents=None, input_tangents=None,
+                         forcing_tangents=None, **optional_kwargs):
+    """Returns (loss, diagnostics, grads, input_grads, forcing_grads, param_hvp, input_hvp,
+    forcing_hvp): those of loss_and_grads and loss_and_input_grads, and the Hessian of loss.mean()
+    jointly in the params, inputs and forcings times the tangents (param_tangents as
+    loss_and_param_hvp takes them, input and forcing tangents as loss_and_input_hvp does, None: zero),
+    its parameter side shaped like the params and its input side like `inputs` and `forcings`."""
+    raise NotImplementedError(f"{type(self).__name__} does not implement joint Hessian-vector "
+                              "products")
+
 
 # Per-variable weights of GraphCast's loss (reference graphcast.py:341-356); others weigh 1.
 LOSS_PER_VARIABLE_WEIGHTS = {
@@ -598,6 +608,59 @@ class GraphCast(Predictor):
     return (loss, diagnostics, _host_grads(self._engine.grads()),
             _host_grads(self._engine.param_hvp()))
 
+  def loss_and_joint_hvp(self, inputs, targets, forcings, param_tangents=None, input_tangents=None,
+                         forcing_tangents=None, **unused_kwargs):
+    """(loss, diagnostics, grads, input_grads, forcing_grads, param_hvp, input_hvp, forcing_hvp) for
+    one target time: what jax.jvp(jax.grad(loss, argnums=(params, inputs)), ...) gives along
+    (param_tangents, input and forcing tangents), with the Hessian's mixed blocks.
+
+    `loss` and `diagnostics` are bit for bit what `loss()` returns, `grads` what loss_and_grads returns
+    and `input_grads` / `forcing_grads` what loss_and_input_grads returns.  With H the Hessian of
+    loss.mean() in (params, inputs and forcings) and v = (v_theta, v_x) the tangents, `param_hvp` is
+    H_theta,theta v_theta + H_theta,x v_x, a dict shaped like the params (float32 numpy, exact zeros for
+    the mesh2grid mesh-node MLP), and `input_hvp` / `forcing_hvp` are H_x,theta v_theta + H_x,x v_x,
+    float32 Datasets shaped like `inputs` and `forcings` in physical units (variables the packing
+    broadcast summed as in loss_and_input_grads).  param_tangents is checked as loss_and_param_hvp
+    checks it, the input and forcing tangents as loss_and_input_hvp checks them; what a tangent leaves
+    out (all of it for None) is zero.  Every refusal of loss_and_param_hvp applies, before anything
+    runs.
+
+    Per batch element (Engine.joint_hvp_element): one forward with its tangent along both v_theta and
+    v_x that keeps its tangent tables, then one backward walk of two directions, the gradient and its
+    tangent, which accumulates the parameter side and forms the input side."""
+    tangents = self._joint_hvp_tangents(inputs, targets, forcings, param_tangents, input_tangents,
+                                        forcing_tangents)
+    return self._loss_and_joint_hvp(inputs, targets, forcings, tangents, norm=None)
+
+  def _joint_hvp_tangents(self, inputs, targets, forcings, param_tangents, input_tangents,
+                          forcing_tangents):
+    """The checks of loss_and_joint_hvp, before anything runs: one target time, the parameter tangents
+    (_checked_param_tangents; None: none) and the input and forcing tangents (hvp_tangent_planes).
+    Returns (checked parameter tangents, [batch, c_in, Ng] host tangent planes)."""
+    if xs.from_xarray(targets).sizes.get("time", 1) != 1:
+      raise NotImplementedError("joint Hessian-vector products cover one target time (several are "
+                                "not provided)")
+    return (self._checked_param_tangents({} if param_tangents is None else param_tangents),
+            hvp_tangent_planes(xs.from_xarray(inputs), xs.from_xarray(forcings), input_tangents,
+                               forcing_tangents))
+
+  def _loss_and_joint_hvp(self, inputs, targets, forcings, tangents,
+                          norm: Optional[FusedNormalization]):
+    """loss_and_joint_hvp of the checked tangents of _joint_hvp_tangents."""
+    inputs, targets = xs.from_xarray(inputs), xs.from_xarray(targets)
+    forcings = xs.from_xarray(forcings)
+    param_tangents, planes = tangents
+    slabs, coef = loss_coefficients(targets, inputs.sizes["lat"] * inputs.sizes["lon"],
+                                    dict(inputs.sizes).get("batch", 1))
+    run = self._one_step_input_grads(inputs, targets, forcings, norm, targets=targets, coef=coef,
+                                     tangent_planes=planes, param_tangents=param_tangents)
+    input_grads, forcing_grads, input_hvp, forcing_hvp = run.finish()
+    del run                                # with the weight tangents it holds
+    loss, diagnostics = self._losses(slabs)
+    eng = self._engine
+    return (loss, diagnostics, _host_grads(eng.grads()), input_grads, forcing_grads,
+            _host_grads(eng.param_hvp()), input_hvp, forcing_hvp)
+
   def _param_tangent_run(self, inputs, targets_template, forcings, param_tangents, num_steps: int,
                          plan=None) -> "_TangentRun":
     """The checked parameter tangents of a param_jvp of `num_steps` target times, as a _TangentRun of
@@ -709,7 +772,8 @@ class GraphCast(Predictor):
 
   def _one_step_input_grads(self, inputs, template, forcings, norm, *, targets=None, coef=None,
                             cotangents=None, predictions=None, directions: bool = False,
-                            tangent_planes: Optional[torch.Tensor] = None) -> "_InputGradRun":
+                            tangent_planes: Optional[torch.Tensor] = None,
+                            param_tangents=None) -> "_InputGradRun":
     """One target time: `_call` stages the planes once and, for every batch element, runs the
     stage-wise forward, the seed and the backward pass of Engine.input_grads_element in place of its
     step (no second forward, no host round trip).  With `targets` the loss sums land in
@@ -717,9 +781,11 @@ class GraphCast(Predictor):
     predictions, unpacked from that forward as __call__ unpacks its step's; with `directions`, the
     cotangents have a leading "direction" dim and every direction shares that forward and backward
     pass; with `tangent_planes` ([batch, c_in, Ng] host planes of the input tangents, or [K, batch,
-    c_in, Ng] for K directions, with `targets`) every element runs Engine.input_hvp_element.  Returns
-    the run, whose finish() gives (input_grads, forcing_grads), with tangent_planes followed by
-    (input_hvp, forcing_hvp), these with a leading "direction" dim for K directions."""
+    c_in, Ng] for K directions, with `targets`) every element runs Engine.input_hvp_element, and with
+    param_tangents as well (checked parameter tangents, one direction) Engine.joint_hvp_element, the
+    parameter side accumulating in the engine (param_hvp_begin).  Returns the run, whose finish() gives
+    (input_grads, forcing_grads), with tangent_planes followed by (input_hvp, forcing_hvp), these with
+    a leading "direction" dim for K directions."""
     batch = dict(inputs.sizes).get("batch", 1)
     run = cot = lat_weight = coef_dev = None
 
@@ -731,8 +797,12 @@ class GraphCast(Predictor):
       if directions:
         cot = self._direction_cotangent_planes(cotangents, template, batch)
         dirs = cot.shape[0]
+      if param_tangents is not None:         # zeroes both accumulator sets before the run is built
+        eng.param_hvp_begin()
       run = _InputGradRun(self, plan, norm, inputs, forcings, 1, batch, release_staging=False,
                           dirs=dirs, hvp=_hvp_directions(tangent_planes, 0))
+      if param_tangents is not None:
+        run.weight_tangents = eng.weight_tangents(param_tangents, transposed=True, input_grad=True)
       if cotangents is not None and not directions:
         cot = self._cotangent_planes(cotangents, template, batch)
       if targets is not None:
@@ -1410,13 +1480,16 @@ class _InputGradRun:
   hvp = (K, directions) (loss_and_input_hvp: (1, False); batched_loss_and_input_hvp: (K, True)): every
   step runs Engine.input_hvp_element, the 1 + K directions are the gradient and its derivatives along
   the K tangents, and finish() gives (input_grads, forcing_grads) from direction 0 and (input_hvp,
-  forcing_hvp) from directions 1..K, these with a leading "direction" dim when `directions`."""
+  forcing_hvp) from directions 1..K, these with a leading "direction" dim when `directions`.  With
+  weight_tangents set as well (loss_and_joint_hvp, K = 1, one target time): Engine.joint_hvp_element
+  in its place, the tangent also along those packed parameter tangents."""
 
   def __init__(self, model: GraphCast, plan, norm: Optional[FusedNormalization], inputs: xs.Dataset,
                forcings: xs.Dataset, num_steps: int, batch: int, release_staging: bool,
                dirs: Optional[int] = None, hvp: Optional[Tuple[int, bool]] = None):
     eng = self.eng = model.engine
     self.hvp, self.zero_targets = hvp, None
+    self.weight_tangents = None
     dirs = 1 + hvp[0] if hvp else dirs
     self.dirs = dirs
     lead = [] if dirs is None else [dirs]
@@ -1454,7 +1527,12 @@ class _InputGradRun:
       if self.zero_targets is None:
         self.zero_targets = torch.zeros([self.eng.n_out, self.eng.num_grid], dtype=torch.float32,
                                         device=self.eng.device)
-      self.eng.input_hvp_element(self.fb, operands, zero_targets=self.zero_targets, **kw)
+      if self.weight_tangents is not None:   # a loss: no predictions to unpack
+        kw.pop("planes_out", None)
+        self.eng.joint_hvp_element(self.fb, operands, weight_tangents=self.weight_tangents,
+                                   zero_targets=self.zero_targets, **kw)
+      else:
+        self.eng.input_hvp_element(self.fb, operands, zero_targets=self.zero_targets, **kw)
     else:
       self.eng.input_grads_element(self.fb, operands, **kw)
     for v in self.var_rows:

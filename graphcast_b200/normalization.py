@@ -344,6 +344,18 @@ class InputsAndResiduals(graphcast.Predictor):
     return self._predictor._loss_and_param_hvp(inputs, targets, forcings, param_tangents,
                                                norm=norm_of(inputs, targets, forcings))
 
+  def loss_and_joint_hvp(self, inputs, targets, forcings, param_tangents=None, input_tangents=None,
+                         forcing_tangents=None, **kwargs):
+    """(loss, diagnostics, grads, input_grads, forcing_grads, param_hvp, input_hvp, forcing_hvp) of
+    `loss` (GraphCast.loss_and_joint_hvp), with the normalisation fused into the kernels as in `loss`:
+    the input side is in the physical units of the inputs and forcings, through the normalisation of
+    the inputs, the residual add and the target normalisation.  GraphCast only."""
+    norm_of = self._norm_of("parameter gradients")
+    tangents = self._predictor._joint_hvp_tangents(inputs, targets, forcings, param_tangents,
+                                                   input_tangents, forcing_tangents)
+    return self._predictor._loss_and_joint_hvp(inputs, targets, forcings, tangents,
+                                               norm=norm_of(inputs, targets, forcings))
+
   def loss(self, inputs, targets, forcings, **kwargs):
     """The loss computed on normalised inputs and targets (targets that are also inputs as
     normalised residuals against the last input frame)."""
